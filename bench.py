@@ -1,10 +1,10 @@
 #!/usr/bin/env python3
-"""bench.py -- Mkeypoints/s of the ORB front-end hot path (extract + match) on B200.
+"""bench.py -- Mkeypoints/s of the ORB front-end hot path (extract + match) on H100.
 
 Workload (BASELINE.json configs[1]): a stream of synthetic 1920x1080 u8 frames, ORBextractor(2000, 1.2, 8,
 FAST_SCORE, 20), frame-to-frame ORBmatcher(0.9, true).SearchByProjection(Current, Last, 15).
-One "step" = `--frames` DISTINCT consecutive frames of the stream per GPU (default 256 = 531 MB of pixels, 4.2x the
-126 MB L2), processed as `--frames / --batch` batches of `--batch` frames and `--repeat` passes over them (default 4:
+One "step" = `--frames` DISTINCT consecutive frames of the stream per GPU (default 256 = 531 MB of pixels, 10x the
+50 MB L2), processed as `--frames / --batch` batches of `--batch` frames and `--repeat` passes over them (default 4:
 a step is then 1024 frame extractions + matches, ~51 ms of GPU work, 20 steps time >= 1 s): extract every frame, match every frame against
 its predecessor.  Mkeypoints/s = keypoints extracted-and-matched / time.
 
@@ -14,6 +14,8 @@ its predecessor.  Mkeypoints/s = keypoints extracted-and-matched / time.
           step's frames from pinned memory and D2H of keypoints/descriptors inside the timed region.
 
 `--impl reference` times the CPU oracle port of the reference path (oracle/) on the host cores.
+`--dump-outputs DIR` writes what the value path returned in its last timed step as DIR/<name>.npy (float32): the inputs
+are a fixed seeded stream, so two builds can be compared output for output.
 PyTorch is used only for plumbing: device buffers, pinned host memory, torch.distributed.
 """
 import argparse
@@ -148,7 +150,7 @@ def config_dict(args):
     ab = algorithmic_bytes()
     return {"workload": WORKLOAD, "frames_per_step_per_gpu": args.frames, "batch": args.batch, "passes_per_step": args.repeat,
             "parallelism": "frames sharded one stream per GPU, no data-path collective",
-            "l2": "a step's %d distinct input frames are %.0f MB (+ %.0f MB of pyramids per batch): larger than L2 (126 MB)"
+            "l2": "a step's %d distinct input frames are %.0f MB (+ %.0f MB of pyramids per batch): larger than L2 (50 MB)"
                   % (args.frames, args.frames * W * H / 1e6, args.batch * 2 * ab["P"] / 1e6),
             "semantics": SEMANTICS}
 
@@ -170,8 +172,33 @@ def backproject(kps):
     return w
 
 
+DUMP_BYTES = 64 << 20
+KP_FIELDS = ("x", "y", "size", "angle", "response", "octave", "class_id")
+
+
+def dump_outputs(out_dir, S):
+    """What the value path returned for the batch of its last timed step (a buffer set of enqueue_device_step): keypoints,
+    descriptors (one float per byte), per-frame counts, matches into the previous frame and per-frame match counts.  Slots past
+    a frame's keypoint count are zeroed (-1 for matches).  A batch larger than DUMP_BYTES is cut to its first frames."""
+    import orb_slam_b200 as fe
+    cnt = S["h_cnt"].numpy()
+    B = len(cnt)
+    n = min(B, DUMP_BYTES // (NFEAT * (len(KP_FIELDS) + 32 + 1) * 4 + 3 * 4 + 8))
+    valid = np.arange(NFEAT)[None, :] < cnt[:n, None]
+    kps = S["h_kps"].numpy().view(fe.KP_DTYPE).reshape(B, NFEAT)[:n]
+    k = np.stack([kps[f] for f in KP_FIELDS], axis=-1).astype(np.float32)
+    desc = S["h_desc"].numpy()[:n].astype(np.float32)
+    mp = S["h_mp"].numpy()[:n].astype(np.float32)
+    k[~valid], desc[~valid], mp[~valid] = 0, 0, -1
+    out = {"keypoints": k, "descriptors": desc, "keypoint_counts": cnt[:n].astype(np.float32), "matches": mp,
+           "match_counts": S["h_nm"].numpy()[:n].astype(np.float32), "frame_index": S["sb"] * B + np.arange(n, dtype=np.float64)}
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
     # the sampler runs from before the warm-up (nvidia-smi needs ~1 s to start); only samples whose arrival time
@@ -377,7 +404,8 @@ def main():
     ap.add_argument("--batch", type=int, default=64, help="frames per library call")
     ap.add_argument("--repeat", type=int, default=4, help="passes over the step's frames inside one step")
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--no-parity", action="store_true", help="skip the oracle cross-check of the step's results (ncu runs)")
+    ap.add_argument("--no-parity", action="store_true", help="skip the oracle cross-check of the step's results (profiler runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the value path's results of the last timed step as DIR/<name>.npy")
     ap.add_argument("--workload", default="stream", choices=["stream", "rig8", "dbsweep"],
                     help="stream = BASELINE configs[1] (the headline line); rig8 = configs[3] (one camera per GPU, exchange + cross-camera "
                          "SearchForInitialization); dbsweep = configs[4] (sharded keyframe-database sweep): the last two print their own line")
@@ -701,6 +729,8 @@ def main():
 
     sampler.t_begin = time.perf_counter()
     r_dev = timed(run_device, args.steps)
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, checks["device"])
     stages = {k: v / max(stage_cnt.get(k, 1), 1) * SUB for k, v in stage_acc.items()}   # ms per step (= SUB library calls)
     if rank == 0 and stage_cnt and min(stage_cnt.values()) != args.steps * SUB:
         sys.stderr.write("bench: stage intervals read back for %s of %d batches\n" % (sorted(set(stage_cnt.values())), args.steps * SUB))
@@ -780,8 +810,8 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s"
+        peak = float(peaks.get("hbm_gbs", 3350.0))
+        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s"
         # dominant kernel of the extract pipeline by measured stage time; per launch = per batch of B frames
         kernel_stages = {k: v / SUB for k, v in stages.items() if k not in ("ingest", "h2d", "d2h")}
         dom = max(kernel_stages, key=kernel_stages.get) if kernel_stages else None
@@ -789,35 +819,10 @@ def main():
         dom_ms = kernel_stages.get(dom, 0.0) if dom else 0.0
         achieved = dom_bytes / (dom_ms * 1e-3) / 1e9 if dom_ms > 0 else 0.0
         ext_ms = sum(kernel_stages.values())
-        traffic, alu = None, None
-        try:  # DRAM bytes + ALU-pipe instructions of the dominant kernel from the committed ncu capture, scaled to B frames
-            tj = json.load(open(os.path.join(ROOT, "profiles", "fast_nms_ncu.json")))
-            if dom == "fast_nms":
-                traffic = (tj["dram_bytes_read"] + tj["dram_bytes_write"]) / tj["frames_in_launch"] * B
-                # the kernel executes the same ALU-pipe instructions per frame here as under ncu, so its pipe utilisation
-                # scales with the ratio of the per-frame durations: frac_live = frac_ncu * t_ncu / t_live
-                t_ncu = tj["duration_us"] * 1e-3 / tj["frames_in_launch"]          # ms per frame under ncu
-                util_hw = tj["alu_pipe_pct_of_peak"] / 100.0 * t_ncu / (dom_ms / B)   # of the hardware peak (64 /clk/SM)
-                a = util_hw * tj["alu_peak_hw_thread_inst_per_clk_sm"]
-                scale_t = t_ncu / (dom_ms / B)
-                alu = {"achieved": a, "peak": tj["alu_peak_measured_thread_inst_per_clk_sm"],
-                       "unit": "ALU-pipe thread-instructions/clk/SM", "frac": a / tj["alu_peak_measured_thread_inst_per_clk_sm"],
-                       "peak_source": "tools/ubench_alu.cu on B200 (profiles/r2_ubench_alu.txt): 58.7 (VIMNMX3 / VIMNMX / PRMT / LOP3 share one "
-                                      "16-lane pipe per SM sub-partition; hardware peak 64)",
-                       "issue_slots_used": tj.get("issue_active_pct", 0.0) / 100.0 * scale_t,
-                       "fma_pipe_frac_of_hw_peak": tj.get("fma_pipe_pct_of_peak", 0.0) / 100.0 * scale_t,
-                       "issue_note": "warp-instructions issued per cycle per scheduler; the same microbenchmark measures 0.63-0.68 as the most a "
-                                     "mix of ALU-pipe and FMA-pipe instructions issues on this SM, 0.46 for ALU-pipe instructions alone: the "
-                                     "kernel moved its 2-input min/max pairs to the FMA pipe (exact fp16-subnormal HFMA2) until issue, not a pipe, binds",
-                       "how": "ncu sm__inst_executed_pipe_alu %.1f%% of peak, issue active %.1f%%, at %.1f us per frame, scaled by the live per-frame time"
-                              % (tj["alu_pipe_pct_of_peak"], tj.get("issue_active_pct", 0.0), t_ncu * 1e3), "source": tj.get("source")}
-        except Exception:
-            pass
-        roof = {"bound": "alu" if alu else "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak if peak else None, "traffic": traffic, "peak_source": peak_src,
-                "note": "achieved/peak/frac are the HBM roofline the metric is quoted against; fast_nms is bound by instruction issue "
-                        "(integer ALU pipe + FMA pipe, the `alu` entry), not by memory: see profiles/README.md",
-                "alu": alu,
+        roof = {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
+                "frac": achieved / peak if peak else None, "peak_source": peak_src,
+                "note": "achieved/peak/frac are the HBM roofline the metric is quoted against, from algorithmic bytes (SURVEY.md 8(d)) "
+                        "over CUDA-event stage times; fast_nms runs far below it: it is bound by integer instruction issue, not by memory",
                 "algorithmic_bytes_per_launch": dom_bytes, "launch_ms": dom_ms, "frames_per_launch": B,
                 "extract_all_kernels": {"algorithmic_bytes": ab["total"] * B, "ms": ext_ms,
                                         "achieved": ab["total"] * B / (ext_ms * 1e-3) / 1e9 if ext_ms > 0 else 0.0,

@@ -4,7 +4,7 @@
  * Frame.cc:60,92-93 and Tracking.cc:111,126 compile against it unchanged.
  *
  * Implementation: orb_slam_b200/host/ORBextractor.cc forwards to the C-ABI of liborbfe.so (include/orbfe.h);
- * pyramid, FAST, retention, orientation, blur and rBRIEF run as hand-written sm_100a CUDA kernels.
+ * pyramid, FAST, retention, orientation, blur and rBRIEF run as hand-written sm_90a CUDA kernels.
  * No CPU fallback: constructing an extractor without a usable CUDA device terminates with a message.
  */
 #ifndef ORBEXTRACTOR_H

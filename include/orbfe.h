@@ -1,5 +1,5 @@
 /*
- * orbfe.h -- C-ABI of liborbfe.so, the B200-native ORB feature front-end (extract + match).
+ * orbfe.h -- C-ABI of liborbfe.so, the H100-native ORB feature front-end (extract + match).
  *
  * This is the drop-in boundary: plain pointers and sizes, no C++/torch types.  The reference has no
  * FFI layer (its boundary is two C++ classes, include/ORBextractor.h:32-77 and include/ORBmatcher.h:37-107
@@ -95,8 +95,7 @@ int orbfe_extractor_last_launches(const OrbfeExtractor *ex);
  *   0 "chunked": the upload of chunk k+1 overlaps ALL kernels of chunk k;
  *   1 "phased":  only the pyramids follow the upload chunk by chunk, detection and description then run once over the
  *                whole batch in full-size launches (for callers whose uploads are hidden behind other GPU work).
- * Results are identical in both modes.  Measured with bench.py's two alternating handles on one B200: chunked 28.7,
- * phased 26.8 Mkeypoints/s end to end -- the default stays chunked. */
+ * Results are identical in both modes; the default is chunked. */
 int orbfe_extractor_set_batch_mode(OrbfeExtractor *ex, int mode);
 /* With profiling on, every extract call records CUDA events around its stages on the launching stream.
  * orbfe_extractor_stage_times returns (name, ms) of every stage interval recorded since the previous read --

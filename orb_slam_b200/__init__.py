@@ -1,7 +1,7 @@
-"""orb_slam_b200 -- B200-native ORB feature front-end (extract + match) behind ORB-SLAM's
-ORBextractor / ORBmatcher API.
+"""orb_slam_b200 -- H100-native ORB feature front-end (extract + match) behind ORB-SLAM's
+ORBextractor / ORBmatcher API.  (The package name is historical.)
 
-The product is `liborbfe.so` (hand-written sm_100a CUDA + a C-ABI, see include/orbfe.h) and the C++
+The product is `liborbfe.so` (hand-written sm_90a CUDA + a C-ABI, see include/orbfe.h) and the C++
 facades in orb_slam_b200/host/.  This module is only a thin ctypes binding of the C-ABI used by the
 tests and bench.py; it mirrors the reference's class names and argument meaning
 (include/ORBextractor.h:32-77, include/ORBmatcher.h:37-107 of raulmur/ORB_SLAM).
@@ -76,7 +76,7 @@ def lib():
     if _lib is not None:
         return _lib
     if not os.path.exists(_SO):
-        raise ImportError("liborbfe.so not built: run `python -m orb_slam_b200.build` (nvcc, sm_100a). "
+        raise ImportError("liborbfe.so not built: run `python -m orb_slam_b200.build` (nvcc, sm_90a). "
                           "There is no CPU fallback.")
     L = C.CDLL(_SO)
     vp, ip = C.c_void_p, C.POINTER(C.c_int)

@@ -1,4 +1,4 @@
-"""Builds liborbfe.so (hand-written sm_100a CUDA + the C-ABI) in-tree with nvcc.
+"""Builds liborbfe.so (hand-written sm_90a CUDA for H100 + the C-ABI) in-tree with nvcc.
 
 No torch, no JIT cache: the .so lands next to this file so that it travels to the GPU box with the
 repo snapshot.  nvcc cross-compiles without a GPU.
@@ -14,10 +14,10 @@ SOURCES = ["orbfe_api.cu", "extract_kernels.cu", "match_kernels.cu", "bow_kernel
            os.path.join("..", "host", "match_host.cpp"), os.path.join("..", "host", "bow_host.cpp")]
 DEPS = SOURCES + ["orbfe_internal.h", os.path.join("..", "..", "include", "orbfe.h"),
                   os.path.join("..", "..", "include", "orbfe_match.h"), os.path.join("..", "..", "include", "orbfe_bow.h"), os.path.join("..", "..", "include", "orbfe_comm.h"),
-                  os.path.join("..", "..", "include", "orbfe_brief_pattern.inc")]
+                  os.path.join("..", "..", "include", "orbfe_brief_pattern.inc"), os.path.join("..", "build.py")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-fmad=false",                       # float ops on the device are individually rounded (parity)
     "-Xcompiler", "-fPIC,-ffp-contract=off,-O2",

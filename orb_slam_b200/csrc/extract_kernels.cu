@@ -1,4 +1,4 @@
-// extract_kernels.cu -- hand-written sm_100a kernels of the ORB extractor hot path.
+// extract_kernels.cu -- hand-written sm_90a kernels of the ORB extractor hot path.
 //
 // Stage map (reference src/ORBextractor.cc; canonical algorithm = SURVEY.md Appendix A):
 //   resize_level_kernel   ComputePyramid: cv::resize INTER_LINEAR u8 (:800), integer fixed point

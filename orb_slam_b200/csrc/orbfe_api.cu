@@ -406,7 +406,7 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
         ex->d_maps = d_maps;
         cudaError_t e = (cudaError_t)fast_tma_setup();
         if (e != cudaSuccess) return fail(ORBFE_ERR_CUDA, "cudaFuncSetAttribute(fast_nms_tma_kernel): %s", cudaGetErrorString(e));
-        int nsm = 148;
+        int nsm = 132;
         cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, ex->device);
         Wk.fast_grid = Wk.fast_ctas * nsm;  // resident persistent CTAs (39 KB smem each)
     }
@@ -711,7 +711,7 @@ extern "C" int orbfe_extract_batch(OrbfeExtractor *ex, const uint8_t *imgs, int 
     rc = zero_counters(ex, s);
     if (rc) return rc;
     // H2D of chunk k+1 (copy stream) overlaps the kernels of chunk k (compute stream)
-    int nchunks = batch >= 8 ? 4 : 1;   // measured on B200 (64 x 1080p, two handles): 4 chunks 32-33, 8 chunks 31.4, 2 chunks 30.7, 1 chunk 28.1 Mkp/s end to end
+    int nchunks = batch >= 8 ? 4 : 1;   // H100, 400 W (64 x 1080p, bench.py's three handles): 1, 2 and 4 chunks within 2 % (37.4-38.1 Mkp/s end to end)
     if (const char *e = getenv("ORBFE_CHUNKS")) nchunks = std::max(1, std::min(batch, atoi(e)));  // tuning knob
     if (!ex->copy_stream) CU_TRY(cudaStreamCreateWithFlags(&ex->copy_stream, cudaStreamNonBlocking));
     while ((int)ex->chunk_ev.size() < nchunks + 1) {
@@ -846,7 +846,7 @@ extern "C" int orbfe_debug_read_level(OrbfeExtractor *ex, int frame, int level, 
 // ------------------------------------------------------------------------------------------------
 struct OrbfeMatcher {
     int device = 0;
-    int nsm = 148;
+    int nsm = 132;
     cudaStream_t stream = nullptr;
     // grow-only device scratch for the host-pointer entry points
     void *buf[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};

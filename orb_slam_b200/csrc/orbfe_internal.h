@@ -1,4 +1,4 @@
-// orbfe_internal.h -- structures shared by the host plan code and the sm_100a kernels of liborbfe.so.
+// orbfe_internal.h -- structures shared by the host plan code and the sm_90a kernels of liborbfe.so.
 // Not part of the public ABI (that is include/orbfe.h).
 #pragma once
 

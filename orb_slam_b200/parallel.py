@@ -1,4 +1,4 @@
-"""Multi-GPU plumbing (torch.distributed; NCCL on the B200 box, gloo in CPU tests).
+"""Multi-GPU plumbing (torch.distributed; NCCL on the GPUs, gloo in CPU tests).
 
 The extract path shards by frame/camera with no data-path collective (SURVEY.md 8e).  The only exchange step
 is cross-frame matching between ranks (BASELINE config 4: one camera per GPU, cross-camera

@@ -1,7 +1,7 @@
 """GPU tests of the multi-GPU entry points (include/orbfe_comm.h) that make sense on ONE device: device-resident
 SearchForInitialization (the matcher of config 4) against the oracle, and the rig exchange / sharded sweep with world = 1
 (the peer table then holds only this rank: same kernels, same flags protocol).  The N > 1 runs are tools/multi_gpu.py under
-torchrun (profiles/r2_multi_gpu_*.json); the host-side sharding logic is covered on CPU by tests/test_parallel_gloo.py."""
+torchrun; the host-side sharding logic is covered on CPU by tests/test_parallel_gloo.py."""
 import numpy as np
 import pytest
 

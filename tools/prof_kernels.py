@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Measurement harness for the configurations that are not the bench line (run on ONE B200 through gpurun):
+"""Measurement harness for the configurations that are not the bench line (run on one H100):
 
   --what config3   BASELINE configs[2]: 3840x2160, 4000 kp, 12 levels -- per-stage CUDA-event times of the extractor on a
                    device-resident batch, achieved GB/s against the 130.86 MB/frame of SURVEY.md 8(d)
@@ -71,7 +71,7 @@ def config3(args):
     reads = sum(w * h for w, h in ls[:-1]) + 2 * P
     writes = (P - W * H) + P
     alg = reads + writes + NF * (749 + 512) + NF * 60
-    peak = 6582.5
+    peak = 3350.0   # H100 SXM data sheet; MEASURED_PEAKS.json replaces it where the machine provides one
     try:
         peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
     except Exception:
