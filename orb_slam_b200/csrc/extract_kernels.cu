@@ -212,6 +212,7 @@ void launch_resize_level(const PlanDev *d_plan, const PlanDev &hp, int level, in
 #define ORBFE_FAST_ARC_DEFAULT 12   // arc-network variant of the non-TMA kernel (fast_m_arc): second form, 12 (min, max) pairs on the FMA pipe
 #endif
 #define F2_MH (F2_H + 2)           // 64 m rows
+static_assert(F2_MH == 64, "the m tile is 8 warps x 8 rows; row 64 does not exist (ti.hmask has 64 bits)");
 
 __device__ __forceinline__ uint32_t max16_u16x2(const uint32_t *w) {
     const uint32_t a0 = __vimax3_u16x2(w[0], w[1], w[2]), a1 = __vimax3_u16x2(w[3], w[4], w[5]);
@@ -266,6 +267,17 @@ __device__ __forceinline__ uint32_t hfma2(uint32_t a, uint32_t b, uint32_t c) {
     uint32_t d;
     asm("fma.rn.f16x2 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
     return d;
+}
+__device__ __forceinline__ uint32_t hmul2(uint32_t a, uint32_t b) {
+    uint32_t d;
+    asm("mul.rn.f16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
+    return d;
+}
+// max(a, b * k) per half for a, b in 0..255 (fp16 subnormals) and keep factor k = 1.0 or 0.0 (nk = k with the sign set):
+// b*k + relu(a - b*k), two exact HFMA2.  No result is -0, so the sign bit of a difference of two such values is a
+// strict comparison.
+__device__ __forceinline__ uint32_t hmax2_keep(uint32_t a, uint32_t b, uint32_t k, uint32_t nk) {
+    return hfma2(b, k, hfma2_relu(b, nk, a));
 }
 // fma_pipe is a compile-time constant at every call site once the callers' loops are unrolled
 __device__ __forceinline__ void minmax_u16x2(bool fma_pipe, uint32_t a, uint32_t b, uint32_t &mn, uint32_t &mx) {
@@ -329,8 +341,8 @@ __device__ __forceinline__ void fast_load_row(const uint8_t *row /* smem, word a
     P[7] = E2;                             // P_8 = (b8, b10)
 }
 
-// m tile in shared memory, u16x2 pairs exactly as produced: row r, group g -> [mA, mB] (8 bytes) with
-// mA = (m[x], m[x+2]), mB = (m[x+1], m[x+3]), x = x0-4+4g.
+// s tile (s = relu(m - t_lo)) in shared memory, u16x2 pairs: row r, group g -> [sA, sB] (8 bytes) with
+// sA = (s[x], s[x+2]), sB = (s[x+1], s[x+3]), x = x0-4+4g.
 __device__ __forceinline__ int m_at(const uint32_t *mt, int r, int c /* tile column, 0 <-> x0-4 */) {
     const int g = c >> 2, k = c & 3;
     const uint32_t wv = mt[(r * 32 + g) * 2 + (k & 1)];
@@ -392,23 +404,34 @@ __device__ __forceinline__ void cell_window(const LevelDev &L, int xmax, int yma
 
 // Everything after the pixel tile is staged: m map, NMS passes, candidate conversion and flush.
 // pix: staged pixel rows (stride F2_PW); mt: 16 KB m tile; s_cand: candidate list (F2_MAXC entries).
+// tile indexes wk.ftile_info; the tile's FTileInfo and level are re-read after the score loop, so that none of the geometry
+// the NMS and the flush need occupies registers while the 7-row window is live.
 template <int PSTRIDE, int ARC>
-__device__ __forceinline__ void fast_tile_compute(const PlanDev *__restrict__ plan, const WorkDev &wk, const LevelDev &L,
-                                                  const FTileInfo &ti, int f, int x0, int y0, const uint8_t *pix, uint32_t *mt,
-                                                  uint32_t *s_cand, int &s_n, int *s_cnt_lo, int *s_cnt_hi, int *s_base) {
-    const int w = L.w, h = L.h;
+__device__ __forceinline__ void fast_tile_compute(const PlanDev *__restrict__ plan, const WorkDev &wk, int tile, int level, int f, int x0, int y0, const uint8_t *pix, uint32_t *mt,
+                                                  uint32_t *s_cand, int &s_n, int *s_cnt_lo, int *s_cnt_hi,
+                                                  long long *s_kbase, int *s_klim) {
     const int tlo = plan->t_lo;
-    const int xmax = w - ORBFE_EDGE, ymax = h - ORBFE_EDGE;  // detect area is [16, xmax) x [16, ymax)
     const int g = threadIdx.x & 31, seg = threadIdx.x >> 5;
     const int gx = x0 - 4 + 4 * g;  // image x of the group's first pixel
-    // ---- m for 32 groups x 64 rows; lane = group, warp = 8-row segment ----
+    // ---- s = relu(m - t_lo) for 32 groups x 64 rows; lane = group, warp = 8-row segment ----
+    //      A pixel with m <= t_lo is never a candidate and never suppresses one (a candidate has m > t_lo), so the NMS
+    //      on s equals the NMS on m floored at t_lo; the candidates' m is s + t_lo.
     {
-        // halves of (mA, mB) that lie inside the detect area: A = (gx, gx+2), B = (gx+1, gx+3)
-        uint32_t maskA = 0, maskB = 0;
-        if (gx >= ORBFE_EDGE && gx < xmax) maskA |= 0x0000FFFFu;
-        if (gx + 2 >= ORBFE_EDGE && gx + 2 < xmax) maskA |= 0xFFFF0000u;
-        if (gx + 1 >= ORBFE_EDGE && gx + 1 < xmax) maskB |= 0x0000FFFFu;
-        if (gx + 3 >= ORBFE_EDGE && gx + 3 < xmax) maskB |= 0xFFFF0000u;
+        const int xmax = plan->lv[level].w - ORBFE_EDGE, ymax = plan->lv[level].h - ORBFE_EDGE;
+        // halves of (mA, mB) that lie inside the detect area, A = (gx, gx+2), B = (gx+1, gx+3), as fp16 factors 1.0 / 0.0
+        uint32_t keepA = 0, keepB = 0;
+        if (gx >= ORBFE_EDGE && gx < xmax) keepA |= 0x00003C00u;
+        if (gx + 2 >= ORBFE_EDGE && gx + 2 < xmax) keepA |= 0x3C000000u;
+        if (gx + 1 >= ORBFE_EDGE && gx + 1 < xmax) keepB |= 0x00003C00u;
+        if (gx + 3 >= ORBFE_EDGE && gx + 3 < xmax) keepB |= 0x3C000000u;
+        const uint32_t ntlo2 = (uint32_t)tlo * 0x00010001u | 0x80008000u;  // -t_lo per half
+        // bit i: the warp's m row i (image y0-1+8*seg+i) lies inside the detect area (one register for the 8 row tests)
+        uint32_t yin_bits = 0;
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+            const int y = y0 - 1 + seg * 8 + i;
+            if (y >= ORBFE_EDGE && y < ymax) yin_bits |= 1u << i;
+        }
         const uint8_t *base = &pix[(seg * 8) * PSTRIDE + 4 * g];  // b0 of the group = tile col 4g  (image x gx-4)
         uint32_t P[7][8];
 #pragma unroll
@@ -432,72 +455,74 @@ __device__ __forceinline__ void fast_tile_compute(const PlanDev *__restrict__ pl
             }
 #undef FROW
             const int mr = seg * 8 + i;
-            const int y = y0 - 1 + mr;
-            const bool yin = (y >= ORBFE_EDGE && y < ymax);
+            const bool yin = (yin_bits >> i) & 1u;
             uint2 o;
-            o.x = yin ? (mA & maskA) : 0u;
-            o.y = yin ? (mB & maskB) : 0u;
+            o.x = hfma2_relu(mA, yin ? keepA : 0u, ntlo2);
+            o.y = hfma2_relu(mB, yin ? keepB : 0u, ntlo2);
             *reinterpret_cast<uint2 *>(&mt[(mr * 32 + g) * 2]) = o;
         }
     }
     __syncthreads();
-
+    // the tile's cell geometry is read only from here on (after the barrier: nothing of it is live in the score loop)
+    const FTileInfo &ti = wk.ftile_info[tile];
+    const LevelDev &L = plan->lv[ti.level];
+    const int xmax = L.w - ORBFE_EDGE, ymax = L.h - ORBFE_EDGE;  // detect area is [16, xmax) x [16, ymax)
     const int thi = plan->t_hi;
-    const uint32_t tlo2 = (uint32_t)tlo * 0x00010001u;
-    // ---- windowed 3x3 NMS, two pixels per instruction.  A pixel only competes with the neighbours inside
-    //      its own cell's detect window (cv::FAST ran per cell image): neighbour relations that cross an
-    //      interior cell boundary are masked to 0 -- per-lane u16x2 masks for vertical boundaries (they kill
-    //      the left/right/diagonal terms), per-row flags for horizontal ones (they kill the row above/below).
+    // ---- windowed 3x3 NMS on s, two pixels per instruction, on the FMA pipe (hmax2_keep).  A pixel only competes
+    //      with the neighbours inside its own cell's detect window (cv::FAST ran per cell image): a neighbour across
+    //      an interior cell boundary is multiplied by 0 -- per-lane factors for vertical boundaries (they kill the
+    //      left/right/diagonal terms), per-row factors for horizontal ones (they kill the row above/below).
     //      Rows 1..62 and groups 1..30 are the detect tile.
     uint32_t fbits = 0;  // candidate flags of the lane's 4 pixels x 8 rows: bit 8k + r
     const int r0 = seg * 8;
+    // bit d = 0..4: relation (gx+d-1 <-> gx+d) crosses a vertical boundary (tile column 4g+d starts a cell)
+    uint32_t vb;
+    {
+        const uint32_t nib = (ti.vmask[g >> 3] >> (4 * (g & 7))) & 15u;
+        vb = nib | (__shfl_down_sync(0xffffffffu, nib, 1) & 1u) << 4;
+    }
     if (g >= 1 && g <= 30) {
-        // relation (gx+d-1 <-> gx+d), d = 0..4, crosses a boundary at X = 16 + cj*cw  <=>  X == gx + d
-        uint32_t mLA = 0xFFFFFFFFu, mRA = 0xFFFFFFFFu, mLB = 0xFFFFFFFFu, mRB = 0xFFFFFFFFu;
-        for (int bnd = 0; bnd < ti.nv; bnd++) {
-            const int d = ORBFE_EDGE + (ti.cj_lo + bnd) * L.cw - gx;
-            if (d == 0) mLA &= 0xFFFF0000u;
-            else if (d == 1) { mRA &= 0xFFFF0000u; mLB &= 0xFFFF0000u; }
-            else if (d == 2) { mLA &= 0x0000FFFFu; mRB &= 0xFFFF0000u; }
-            else if (d == 3) { mRA &= 0x0000FFFFu; mLB &= 0x0000FFFFu; }
-            else if (d == 4) mRB &= 0x0000FFFFu;
-        }
-        // ti.hmask bit r: tile row r (image y0-1+r) is the top row of a cell (interior horizontal boundary above it)
-        const unsigned long long hmask = ti.hmask;
+        const uint32_t ONE2 = 0x3C003C00u, NEG2 = 0xBC00BC00u;
+        // keep factors (1.0 / 0.0 per half) of leftA = (m[x-1], m[x+1]) for A, of B for A and of A for B (the same two
+        // relations), of rightB = (m[x+2], m[x+4]) for B; the negated factor is what hmax2_keep also takes
+        const uint32_t kLA = ((vb & 1u) ? 0u : 0x00003C00u) | ((vb & 4u) ? 0u : 0x3C000000u);
+        const uint32_t kM = ((vb & 2u) ? 0u : 0x00003C00u) | ((vb & 8u) ? 0u : 0x3C000000u);
+        const uint32_t kRB = ((vb & 4u) ? 0u : 0x00003C00u) | ((vb & 16u) ? 0u : 0x3C000000u);
+        const uint32_t nkM = kM | 0x80008000u;
+        // bit i: tile row r0+i is the top row of a cell (interior horizontal boundary above it); rows past 63 are 0
+        const uint32_t hm = (uint32_t)(ti.hmask >> r0);
         uint32_t A[3], B[3], lrA[3], lrB[3], fullA[3], fullB[3];
 #pragma unroll
         for (int j = 0; j < 10; j++) {
-            // load tile row r0 - 1 + j into slot j % 3
-            const int rr = min(max(r0 - 1 + j, 0), F2_MH - 1);
+            // load tile row r0 - 1 + j into slot j % 3 (rows -1 and 64 are clamped: they only neighbour rows 0 and 63)
+            const int rr = j == 0 ? max(r0 - 1, 0) : j == 9 ? min(r0 + 8, F2_MH - 1) : r0 - 1 + j;
             const uint32_t *rowp = &mt[(rr * 32 + g) * 2];
             const uint2 own = *reinterpret_cast<const uint2 *>(rowp);
             const uint32_t pB = rowp[-1], nA = rowp[2];
             const int sl = j % 3;
             A[sl] = own.x;
             B[sl] = own.y;
-            const uint32_t leftA = __byte_perm(pB, own.y, 0x5432) & mLA;   // (m[x-1], m[x+1])
-            const uint32_t rightB = __byte_perm(own.x, nA, 0x5432) & mRB;  // (m[x+2], m[x+4])
-            lrA[sl] = __vmaxu2(leftA, own.y & mRA);
-            fullA[sl] = __vmaxu2(lrA[sl], own.x);
-            lrB[sl] = __vmaxu2(own.x & mLB, rightB);
-            fullB[sl] = __vmaxu2(lrB[sl], own.y);
+            const uint32_t leftA = hmul2(__byte_perm(pB, own.y, 0x5432), kLA);   // (s[x-1], s[x+1])
+            const uint32_t rightB = hmul2(__byte_perm(own.x, nA, 0x5432), kRB);  // (s[x+2], s[x+4])
+            lrA[sl] = hmax2_keep(leftA, own.y, kM, nkM);
+            fullA[sl] = hmax2_keep(lrA[sl], own.x, ONE2, NEG2);
+            lrB[sl] = hmax2_keep(rightB, own.x, kM, nkM);
+            fullB[sl] = hmax2_keep(lrB[sl], own.y, ONE2, NEG2);
             if (j >= 2) {
-                const int cr = r0 + j - 2;  // centre row (slot (j-1)%3), above = (j-2)%3, below = j%3
+                // centre row r0 + j - 2 (slot (j-1)%3), above = (j-2)%3, below = j%3
                 const int c = (j - 1) % 3, u = (j - 2) % 3, d = j % 3;
-                const bool no_up = (hmask >> cr) & 1ull, no_dn = (hmask >> (cr + 1)) & 1ull;
-                const uint32_t upA = no_up ? 0u : fullA[u], dnA = no_dn ? 0u : fullA[d];
-                const uint32_t upB = no_up ? 0u : fullB[u], dnB = no_dn ? 0u : fullB[d];
-                // neighbour maximum, floored at t_lo: m must exceed both to be a candidate
-                const uint32_t nbA = __vmaxu2(__vimax3_u16x2(upA, dnA, lrA[c]), tlo2);
-                const uint32_t nbB = __vmaxu2(__vimax3_u16x2(upB, dnB, lrB[c]), tlo2);
-                // m - nb + 0x7FFF per half (both < 0x8000: no borrow between halves): bit 15 set  <=>  m > nb
-                const uint32_t tA = A[c] + 0x7FFF7FFFu - nbA;
-                const uint32_t tB = B[c] + 0x7FFF7FFFu - nbB;
+                const uint32_t kUp = ((hm >> (j - 2)) & 1u) ? 0u : ONE2, kDn = ((hm >> (j - 1)) & 1u) ? 0u : ONE2;
+                // e = (neighbour maximum) - s: sign bit set  <=>  s > every neighbour (s > 0 <=> m > t_lo follows)
+                const uint32_t eA = hfma2(A[c], NEG2, hmax2_keep(hmax2_keep(lrA[c], fullA[d], kDn, kDn | 0x80008000u), fullA[u], kUp, kUp | 0x80008000u));
+                const uint32_t eB = hfma2(B[c], NEG2, hmax2_keep(hmax2_keep(lrB[c], fullB[d], kDn, kDn | 0x80008000u), fullB[u], kUp, kUp | 0x80008000u));
                 // flag bytes of pixels k = 0..3 -> byte k, bit (row inside the segment); the (rare) candidates are
                 // pushed after the loop, outside the unrolled code
-                if (cr >= 1 && cr <= F2_H) fbits |= (__byte_perm(tA, tB, 0x7351) & 0x80808080u) >> (7 - (j - 2));
+                fbits |= (__byte_perm(eA, eB, 0x7351) & 0x80808080u) >> (7 - (j - 2));
             }
         }
+        // only rows 1..62 are the detect tile: drop row 0 (first row of segment 0) and row 63 (last row of segment 7)
+        if (seg == 0) fbits &= 0xFEFEFEFEu;
+        if (seg == 7) fbits &= 0x7F7F7F7Fu;
     }
     // warp-aggregated queue reservation (all 32 lanes; the halo lanes have no flags): one shared-memory atomic per
     // warp, then every lane writes its own candidates
@@ -519,7 +544,7 @@ __device__ __forceinline__ void fast_tile_compute(const PlanDev *__restrict__ pl
                 const int b = __ffs(fbits) - 1;
                 fbits &= fbits - 1;
                 const int cr = r0 + (b & 7), k = b >> 3;
-                s_cand[n++] = (uint32_t)(gx + k - x0) | ((uint32_t)(cr - 1) << 7) | ((uint32_t)m_at(mt, cr, 4 * g + k) << 13);
+                s_cand[n++] = (uint32_t)(gx + k - x0) | ((uint32_t)(cr - 1) << 7) | ((uint32_t)(m_at(mt, cr, 4 * g + k) + tlo) << 13);
             }
         }
     }
@@ -538,19 +563,23 @@ __device__ __forceinline__ void fast_tile_compute(const PlanDev *__restrict__ pl
         if (slot >= 2048) atomicExch(wk.err_flag, 3);  // 11-bit slot field (unreachable: <= 1860 maxima per tile)
         s_cand[i] = q | ((uint32_t)slot << 21);
     }
-    // ---- flush: one global atomic per (tile, cell) reserves the range, then the keys are written ----
+    // ---- flush: one global atomic per (tile, cell) reserves the range, then the keys are written.  The flushing thread
+    //      leaves the range's first key index and its room (capacity - base) in shared memory, so the key stores below
+    //      need no global load ----
     __syncthreads();
     if ((int)threadIdx.x < ncell_loc) {
         const int lc = threadIdx.x;
         const int gcell = L.cell_base + (ti.ci0 + lc / ti.ncj) * L.cols + (ti.cj0 + lc % ti.ncj);
         const size_t fc = (size_t)f * plan->ncells_total + gcell;
+        const int cap = wk.cell_cand_cap[gcell];
         int base = 0;
         if (s_cnt_lo[lc] > 0) {
             base = atomicAdd(&wk.cell_cnt_lo[fc], s_cnt_lo[lc]);
             if (s_cnt_hi[lc] > 0) atomicAdd(&wk.cell_cnt_hi[fc], s_cnt_hi[lc]);
-            if (base + s_cnt_lo[lc] > wk.cell_cand_cap[gcell]) atomicExch(wk.err_flag, 1);
+            if (base + s_cnt_lo[lc] > cap) atomicExch(wk.err_flag, 1);
         }
-        s_base[lc] = base;
+        s_kbase[lc] = (long long)f * plan->cand_total + wk.cell_cand_base[gcell] + base;
+        s_klim[lc] = cap - base;
     }
     __syncthreads();
     for (int i = threadIdx.x; i < ncand; i += blockDim.x) {
@@ -559,11 +588,9 @@ __device__ __forceinline__ void fast_tile_compute(const PlanDev *__restrict__ pl
         int ci, cj, xa, xb, ya, yb;
         cell_window(L, xmax, ymax, x, y, ci, cj, xa, xb, ya, yb);
         const int lc = (ci - ti.ci0) * ti.ncj + (cj - ti.cj0);
-        const int gcell = L.cell_base + ci * L.cols + cj;
-        const int pos = s_base[lc] + slot;
         const uint32_t raster = (uint32_t)((y - ya) * L.cw + (x - xa));
-        if (pos < wk.cell_cand_cap[gcell]) {
-            const size_t kidx = (size_t)f * plan->cand_total + wk.cell_cand_base[gcell] + pos;
+        if (slot < s_klim[lc]) {
+            const size_t kidx = (size_t)(s_kbase[lc] + slot);
             if (wk.cand_keys64) {
                 // HARRIS_SCORE (:616-620): rank by the Harris response; the FAST score rides along for eligibility
                 const float resp = harris_response(L.pyr + (size_t)f * L.plane, L.pitch, x, y, plan->harris_scale4);
@@ -580,7 +607,8 @@ __global__ void __launch_bounds__(256, 2) fast_nms_kernel(const PlanDev *__restr
     // one buffer, two lives: the staged pixel tile (until m is computed), then the candidate list
     __shared__ __align__(16) uint8_t sbuf[(F2_MAXC * 4 > F2_PH * F2_PW) ? F2_MAXC * 4 : F2_PH * F2_PW];
     __shared__ __align__(16) uint32_t mt[F2_MH * 32 * 2];  // 16 KB
-    __shared__ int s_n, s_cnt_lo[F2_MAXCELLS], s_cnt_hi[F2_MAXCELLS], s_base[F2_MAXCELLS];
+    __shared__ int s_n, s_cnt_lo[F2_MAXCELLS], s_cnt_hi[F2_MAXCELLS], s_klim[F2_MAXCELLS];
+    __shared__ long long s_kbase[F2_MAXCELLS];
     uint8_t *pix = sbuf;
     uint32_t *s_cand = reinterpret_cast<uint32_t *>(sbuf);
 
@@ -606,7 +634,7 @@ __global__ void __launch_bounds__(256, 2) fast_nms_kernel(const PlanDev *__restr
         }
     }
     __syncthreads();
-    fast_tile_compute<F2_PW, ORBFE_FAST_ARC_DEFAULT>(plan, wk, L, ti, f, x0, y0, pix, mt, s_cand, s_n, s_cnt_lo, s_cnt_hi, s_base);
+    fast_tile_compute<F2_PW, ORBFE_FAST_ARC_DEFAULT>(plan, wk, blockIdx.x, ti.level, f, x0, y0, pix, mt, s_cand, s_n, s_cnt_lo, s_cnt_hi, s_kbase, s_klim);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -654,7 +682,8 @@ __global__ void __launch_bounds__(256, MINB) fast_nms_tma_kernel(const PlanDev *
     uint8_t *pixbuf0 = dsm, *pixbuf1 = dsm + F2_PIXSLOT;
     uint32_t *mt = reinterpret_cast<uint32_t *>(dsm + 2 * F2_PIXSLOT);
     __shared__ __align__(8) uint64_t bar[2];
-    __shared__ int s_n, s_cnt_lo[F2_MAXCELLS], s_cnt_hi[F2_MAXCELLS], s_base[F2_MAXCELLS];
+    __shared__ int s_n, s_cnt_lo[F2_MAXCELLS], s_cnt_hi[F2_MAXCELLS], s_klim[F2_MAXCELLS];
+    __shared__ long long s_kbase[F2_MAXCELLS];
 
     const int ntiles = plan->nftiles_total;
     if (threadIdx.x == 0) {
@@ -673,26 +702,30 @@ __global__ void __launch_bounds__(256, MINB) fast_nms_tma_kernel(const PlanDev *
     for (int it = 0; wi < nwork; it++, wi += gridDim.x) {
         const int cur = it & 1;
         const int nxt = wi + gridDim.x;
-        if (nxt < nwork && threadIdx.x == 0) {  // prefetch the next tile into the other buffer
+        const FTileInfo ti = wk.ftile_info[wi % ntiles];
+        const int f = f0 + wi / ntiles;
+        const int x0 = ORBFE_EDGE + ti.tx * F2_W, y0 = ORBFE_EDGE + ti.ty * F2_H;
+        // No barrier ends an item: a thread gets here once every thread has passed the previous item's flush barrier,
+        // so the counters are no longer read; the previous item's key stores may still read its candidate queue (the
+        // other pixel slot) and s_kbase / s_klim, which this item writes only after the barrier below and its own
+        // first two barriers.
+        if (threadIdx.x < F2_MAXCELLS) { s_cnt_lo[threadIdx.x] = 0; s_cnt_hi[threadIdx.x] = 0; }
+        if (threadIdx.x == 0) s_n = 0;
+        mbar_wait(&bar[cur], (it >> 1) & 1);
+        __syncthreads();
+        // prefetch the next tile into the other buffer: every thread has finished the previous item, whose candidate
+        // queue lived there, and has waited on that buffer's mbarrier phase
+        if (nxt < nwork && threadIdx.x == 0) {
             const FTileInfo tn = wk.ftile_info[nxt % ntiles];
             mbar_expect_tx(&bar[cur ^ 1], F2_PIXBYTES);
             tma_load_3d(cur ? pixbuf0 : pixbuf1, &wk.tmaps[tn.level], &bar[cur ^ 1], (ORBFE_EDGE + tn.tx * F2_W - 8) & ~15,
                         ORBFE_EDGE + tn.ty * F2_H - 4, f0 + nxt / ntiles);
         }
-        const FTileInfo ti = wk.ftile_info[wi % ntiles];
-        const int f = f0 + wi / ntiles;
-        const LevelDev &L = plan->lv[ti.level];
-        const int x0 = ORBFE_EDGE + ti.tx * F2_W, y0 = ORBFE_EDGE + ti.ty * F2_H;
-        if (threadIdx.x < F2_MAXCELLS) { s_cnt_lo[threadIdx.x] = 0; s_cnt_hi[threadIdx.x] = 0; }
-        if (threadIdx.x == 0) s_n = 0;
-        mbar_wait(&bar[cur], (it >> 1) & 1);
-        __syncthreads();
         // the candidate queue reuses the current pixel slot (dead once m is computed; the next TMA into it is
-        // only issued after the __syncthreads that ends this iteration)
+        // only issued after the first barrier of the next item)
         uint8_t *slot_cur = cur ? pixbuf1 : pixbuf0;
-        fast_tile_compute<F2_TW, ARC>(plan, wk, L, ti, f, x0, y0, slot_cur + ((x0 - 8) & 15), mt, reinterpret_cast<uint32_t *>(slot_cur),
-                                 s_n, s_cnt_lo, s_cnt_hi, s_base);
-        __syncthreads();  // mt / s_cand / counters and the pixel buffer are reused by the next item
+        fast_tile_compute<F2_TW, ARC>(plan, wk, wi % ntiles, ti.level, f, x0, y0, slot_cur + ((x0 - 8) & 15), mt, reinterpret_cast<uint32_t *>(slot_cur),
+                                 s_n, s_cnt_lo, s_cnt_hi, s_kbase, s_klim);
     }
 }
 

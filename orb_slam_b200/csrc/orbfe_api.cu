@@ -327,19 +327,18 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
                     const int cj0 = std::min((x0 - ORBFE_EDGE) / L.cw, L.cols - 1), cj1 = std::min((x1 - ORBFE_EDGE) / L.cw, L.cols - 1);
                     const int ci0 = std::min((y0 - ORBFE_EDGE) / L.ch, L.rows - 1), ci1 = std::min((y1 - ORBFE_EDGE) / L.ch, L.rows - 1);
                     T.cj0 = (short)cj0; T.ci0 = (short)ci0; T.ncj = (short)(cj1 - cj0 + 1); T.nci = (short)(ci1 - ci0 + 1);
-                    // interior boundaries X = 16 + cj*cw (cj >= 1) with x0 <= X <= x0 + FT_W (columns X-1 and X)
-                    const int cj_lo = std::max(1, (x0 - ORBFE_EDGE + L.cw - 1) / L.cw);
-                    const int cj_hi = std::min(L.cols - 1, (x0 + ORBFE_FT_W - ORBFE_EDGE) / L.cw);
-                    const int ci_lo = std::max(1, (y0 - ORBFE_EDGE + L.ch - 1) / L.ch);
-                    const int ci_hi = std::min(L.rows - 1, (y0 + ORBFE_FT_H - ORBFE_EDGE) / L.ch);
                     T.level = (short)l; T.tx = (short)tx; T.ty = (short)ty; T.pad = 0;
-                    T.cj_lo = (short)cj_lo; T.nv = (short)std::max(0, cj_hi - cj_lo + 1);
-                    T.ci_lo = (short)ci_lo; T.nh = (short)std::max(0, ci_hi - ci_lo + 1);
+                    // interior cell boundaries: y = 16 + ci*ch (ci >= 1) and x = 16 + cj*cw (cj >= 1)
                     T.hmask = 0;
                     for (int r = 0; r < ORBFE_FT_H + 2; r++) {
                         const int y = y0 - 1 + r;
                         const int d = y - ORBFE_EDGE;
                         if (d >= L.ch && d % L.ch == 0 && d / L.ch <= L.rows - 1) T.hmask |= 1ull << r;
+                    }
+                    for (int w = 0; w < 4; w++) T.vmask[w] = 0;
+                    for (int c = 0; c < 128; c++) {
+                        const int d = x0 - 4 + c - ORBFE_EDGE;
+                        if (d >= L.cw && d % L.cw == 0 && d / L.cw <= L.cols - 1) T.vmask[c >> 5] |= 1u << (c & 31);
                     }
                     if (T.ncj * T.nci > 64) return fail(ORBFE_ERR_UNSUPPORTED, "level %d: a FAST tile overlaps %d cells", l, T.ncj * T.nci);
                 }

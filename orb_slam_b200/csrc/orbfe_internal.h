@@ -60,9 +60,9 @@ struct PlanDev {
 // Cell geometry of one FAST tile (host-precomputed): cells overlapped and interior cell boundaries inside it
 struct FTileInfo {
     short cj0, ci0, ncj, nci;    // first cell col/row overlapped, number of cell cols/rows overlapped
-    short cj_lo, nv, ci_lo, nh;  // interior vertical boundaries cj_lo .. cj_lo+nv-1 (x = 16 + cj*cw), horizontal likewise
     short level, tx, ty, pad;    // which level / tile this is (saves a dependent scan of the plan at CTA start)
     unsigned long long hmask;    // bit r: m-tile row r (image y0-1+r) is the first row of a cell other than the top one
+    unsigned int vmask[4];       // bit c of the 128: m-tile column c (image x0-4+c) is the first column of a cell other than the leftmost
 };
 struct BTileInfo { short level, tx, ty, pad; };  // blur tiles
 
