@@ -53,6 +53,19 @@ int orbfe_bow_descend(OrbfeVocabulary *v, const uint8_t *desc, int n, int levels
 int orbfe_bow_transform(OrbfeVocabulary *v, const uint8_t *desc, int n, int levelsup, int *nwords_out, int32_t *bow_ids,
                         double *bow_vals, int *nnodes_out, int32_t *fv_ids, int32_t *fv_ptr, int32_t *fv_feats);
 
+/* The FeatureVector half of transform() on the device, for `nframes` frames at once: d_leaf / d_node hold what
+ * orbfe_bow_descend_device wrote (frame f at f*cap, d_counts[f] valid entries -- the frame layout of
+ * orbfe_extract_batch_device).  Frame f receives the FeatureVector orbfe_bow_transform returns: d_fv_n[f] nodes, node ids
+ * d_fv_ids[f*cap + k] ascending, row starts d_fv_ptr[f*(cap+1) + k] (k = 0..d_fv_n[f]), feature indices d_fv_items[f*cap + ...]
+ * ascending inside a node.  As in DBoW2, a feature whose word has weight 0 (a stopped word; the leaf d_leaf names it) is
+ * in no node; a leaf id outside the vocabulary counts as stopped.  A frame without features gets 0 nodes and
+ * d_fv_ptr[f*(cap+1)] = 0.  One thread block per frame sorts the frame's (node id, feature index) pairs in shared memory:
+ * cap <= ORBFE_FV_MAX_CAP, else ORBFE_ERR_UNSUPPORTED.  The output is the input of orbfe_search_by_bow_device
+ * (include/orbfe_match.h).  Enqueued on `stream` (NULL = the vocabulary's stream), not synchronised. */
+#define ORBFE_FV_MAX_CAP 16384
+int orbfe_feature_vector_device(OrbfeVocabulary *v, int nframes, const int32_t *d_leaf, const int32_t *d_node, const int *d_counts,
+                                int cap, int32_t *d_fv_ids, int32_t *d_fv_ptr, int32_t *d_fv_items, int *d_fv_n, void *stream);
+
 /* MapPoint::ComputeDistinctiveDescriptors for ngroups map points at once: group g owns the descriptors
  * desc[group_ptr[g] .. group_ptr[g+1]) (its observations, in the order of the reference's vDescriptors);
  * best_out[g] = index inside the group of the descriptor with the least median distance to the group

@@ -147,6 +147,28 @@ int orbfe_search_by_bow(OrbfeMatcher *m, int variant, int n1, const uint8_t *des
                         const uint8_t *valid2, const float *angle2, int nn2, const int32_t *ids2, const int32_t *ptr2,
                         const int32_t *items2, float nnratio, int check_orientation, int32_t *out, int *nmatches_out);
 
+/* SearchByBoW (both overloads, as orbfe_search_by_bow) with EVERYTHING device-resident, for `njobs` frame pairs per call:
+ * job j matches side-1 frame d_idx1[j] against side-2 frame d_idx2[j] of the frame store d_kps / d_desc / d_counts (frame f
+ * at f*cap, as orbfe_extract_batch_device lays it out).  Many jobs may share a frame: relocalisation matches one frame
+ * against every candidate keyframe (Tracking.cc:841-901), loop closing one keyframe against every loop candidate.
+ * FeatureVectors in the layout orbfe_feature_vector_device writes (include/orbfe_bow.h): node ids d_fv_ids[f*cap + k]
+ * (strictly ascending), row starts d_fv_ptr[f*(cap+1) + k], feature indices d_fv_items[f*cap + ...], d_fv_n[f] nodes; every
+ * feature index appears in at most one node (true of any DBoW2 FeatureVector).  FeatureVectors built on the host (keyframes
+ * whose BoW was computed earlier) may be uploaded into the same layout.
+ * d_valid[f*cap + i] != 0: feature i of frame f has a map point that is not bad (side 2 of variant 0 ignores it).
+ * Angles are d_kps[].angle.  variant 0: row j of d_out (njobs x cap) is indexed by side-2 feature and holds the matched
+ * side-1 index; variant 1: indexed by side-1 feature, holding the side-2 index; -1 = no match; the first count entries of
+ * each row are written.  d_nmatches[j] = the method's return value.  Results equal orbfe_search_by_bow's.
+ * One thread block per job, no global scratch.  A FeatureVector entry outside the frame's slots (node count > cap, a row
+ * outside [0, cap], a feature index >= the frame's count) is never followed: that job's d_nmatches is -1 and
+ * orbfe_matcher_sync reports ORBFE_ERR_ARG; the other jobs of the launch are unaffected.  Frame indices are not checked.
+ * 1 <= cap <= 65535.  Enqueued on `stream` (NULL = the matcher's stream), not synchronised. */
+int orbfe_search_by_bow_device(OrbfeMatcher *m, int variant, int njobs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
+                               const int *d_counts, int cap, const int32_t *d_fv_ids, const int32_t *d_fv_ptr,
+                               const int32_t *d_fv_items, const int *d_fv_n, const uint8_t *d_valid, const int *d_idx1,
+                               const int *d_idx2, float nnratio, int check_orientation, int32_t *d_out, int *d_nmatches,
+                               void *stream);
+
 /* int ORBmatcher::SearchForTriangulation(pKF1, pKF2, F12, ...) (ORBmatcher.cc:852-1014) with CheckDistEpipolarLine
  * (:136-153).  keys1/keys2 = GetKeyPointsUn(); has_mp1/2[i] != 0 <=> the feature already has a map point (skipped);
  * FeatureVectors as in orbfe_search_by_bow; F12 = 3x3 row-major floats; sigma2_kf2[level] = pKF2->GetSigma2(level).

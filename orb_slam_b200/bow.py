@@ -29,6 +29,7 @@ def _bind():
     L.orbfe_bow_transform.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp]
     L.orbfe_distinctive_descriptors.argtypes = [vp, vp, vp, C.c_int, vp]
     L.orbfe_bow_db_detect.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, C.c_float, vp, vp, vp, vp]
+    L.orbfe_feature_vector_device.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]
     _bound = True
     return L
 
@@ -96,6 +97,15 @@ class Vocabulary:
         _check(_bind().orbfe_bow_transform(self._h, _p(desc), n, levelsup, C.byref(nw), _p(bow_ids), _p(bow_vals), C.byref(nn),
                                            _p(fv_ids), _p(fv_ptr), _p(fv_feats)))
         return (bow_ids[:nw.value], bow_vals[:nw.value]), (fv_ids[:nn.value], fv_ptr[:nn.value + 1], fv_feats[:fv_ptr[nn.value]])
+
+
+def feature_vector_device(voc: "Vocabulary", nframes, d_leaf, d_node, d_counts, cap, d_fv_ids, d_fv_ptr, d_fv_items, d_fv_n, stream=0):
+    """FeatureVectors of `nframes` frames from the leaf / node ids Vocabulary.descend_device wrote (ints = raw device addresses;
+    frame f at f*cap, d_counts[f] features).  Outputs: node ids (nframes x cap), row starts (nframes x (cap+1)), feature
+    indices (nframes x cap), node counts (nframes).  Enqueued, not synchronised; see include/orbfe_bow.h."""
+    vp = C.c_void_p
+    _check(_bind().orbfe_feature_vector_device(voc.handle, nframes, vp(d_leaf), vp(d_node), vp(d_counts), cap, vp(d_fv_ids),
+                                               vp(d_fv_ptr), vp(d_fv_items), vp(d_fv_n), vp(stream)))
 
 
 def distinctive_descriptors(matcher: ORBmatcher, desc, group_ptr):

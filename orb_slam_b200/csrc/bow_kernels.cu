@@ -145,6 +145,101 @@ void launch_bow_db_score(int nq, const int *q_ids, const double *q_vals, int nkf
     bow_db_score_kernel<<<(nkf + 127) / 128, 128, 0, s>>>(nq, q_ids, q_vals, nkf, kf_ptr, db_ids, db_vals, common, first, score);
 }
 
+// DBoW2::FeatureVector of every frame from the per-feature node ids (TemplatedVocabulary.h:1180-1190 adds feature i to
+// node nid[i] in index order).  One CTA per frame: the (node id << 32 | feature index) keys are unique, so an ascending
+// bitonic sort in shared memory is the stable sort by node id; a block scan over the run heads numbers the nodes.
+#define FV_THREADS 1024
+__global__ void __launch_bounds__(FV_THREADS) feature_vector_kernel(const int *__restrict__ leaf, const int *__restrict__ node,
+                                                                    const uint8_t *__restrict__ live, int nnodes,
+                                                                    const int *__restrict__ counts, int cap, int *__restrict__ fv_ids,
+                                                                    int *__restrict__ fv_ptr, int *__restrict__ fv_items,
+                                                                    int *__restrict__ fv_n) {
+    extern __shared__ unsigned long long fkeys[];   // [n2]
+    __shared__ int s_warp[FV_THREADS / 32];
+    const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const int n = min(max(counts[f], 0), cap);
+    int n2 = 1;
+    while (n2 < n) n2 <<= 1;
+    const int *__restrict__ nd = node + (size_t)f * cap;
+    const int *__restrict__ lf = leaf + (size_t)f * cap;
+    // a feature whose word has weight 0 (a stopped word) is in no node (TemplatedVocabulary.h:1175, `if (w > 0)`); a leaf id
+    // outside the vocabulary counts as stopped
+    int nk = 0;   // features kept: the sorted keys of [0, nk)
+    for (int c0 = 0; c0 < n2; c0 += FV_THREADS) {
+        const int i = c0 + tid;
+        bool keep = false;
+        if (i < n2) {
+            if (i < n) {
+                const int l = lf[i];
+                keep = (unsigned)l < (unsigned)nnodes && live[l];
+            }
+            fkeys[i] = keep ? ((unsigned long long)(uint32_t)nd[i] << 32) | (uint32_t)i : ~0ull;
+        }
+        nk += __syncthreads_count(keep);
+    }
+    for (int k = 2; k <= n2; k <<= 1) {
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            for (int i = tid; i < n2; i += FV_THREADS) {
+                const int ixj = i ^ j;
+                if (ixj > i) {
+                    const unsigned long long x = fkeys[i], y = fkeys[ixj];
+                    if (((i & k) == 0) ? (x > y) : (x < y)) { fkeys[i] = y; fkeys[ixj] = x; }
+                }
+            }
+            __syncthreads();
+        }
+    }
+    int *__restrict__ ids = fv_ids + (size_t)f * cap;
+    int *__restrict__ ptr = fv_ptr + (size_t)f * (cap + 1);
+    int *__restrict__ items = fv_items + (size_t)f * cap;
+    int base = 0;   // nodes started before this chunk
+    for (int c0 = 0; c0 < nk; c0 += FV_THREADS) {
+        const int i = c0 + tid;
+        unsigned long long key = 0;
+        bool head = false;
+        if (i < nk) {
+            key = fkeys[i];
+            head = i == 0 || (uint32_t)(fkeys[i - 1] >> 32) != (uint32_t)(key >> 32);
+            items[i] = (int)(uint32_t)key;
+        }
+        // exclusive scan of the head flags over the block
+        const unsigned bal = __ballot_sync(0xffffffffu, head);
+        if (lane == 0) s_warp[wid] = __popc(bal);
+        __syncthreads();
+        int before = 0, total = 0;
+        for (int w = 0; w < FV_THREADS / 32; w++) {
+            const int c = s_warp[w];
+            if (w < wid) before += c;
+            total += c;
+        }
+        if (head) {
+            const int k = base + before + __popc(bal & ((1u << lane) - 1u));
+            ids[k] = (int)(uint32_t)(key >> 32);
+            ptr[k] = i;
+        }
+        base += total;
+        __syncthreads();   // s_warp is rewritten by the next chunk
+    }
+    if (tid == 0) {
+        ptr[base] = nk;
+        fv_n[f] = base;
+    }
+}
+
+static int launch_feature_vector(int nframes, const int *d_leaf, const int *d_node, const uint8_t *d_live, int nnodes,
+                                 const int *d_counts, int cap, int *d_ids, int *d_ptr, int *d_items, int *d_n, cudaStream_t s) {
+    if (nframes <= 0) return 0;
+    int n2 = 1;   // cap <= ORBFE_FV_MAX_CAP: at most 16384 keys = 128 KB
+    while (n2 < cap) n2 <<= 1;
+    const size_t smem = sizeof(unsigned long long) * (size_t)n2;
+    if (smem > 48 * 1024) {
+        cudaError_t e = cudaFuncSetAttribute(feature_vector_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return (int)e;
+    }
+    feature_vector_kernel<<<nframes, FV_THREADS, smem, s>>>(d_leaf, d_node, d_live, nnodes, d_counts, cap, d_ids, d_ptr, d_items, d_n);
+    return 0;
+}
+
 }  // namespace orbfe
 
 using namespace orbfe;
@@ -160,6 +255,7 @@ struct OrbfeVocabulary {
     int device = 0, nnodes = 0, depth = 0, weighting = 0, norm = 0;
     cudaStream_t stream = nullptr;
     uint8_t *d_desc = nullptr;
+    uint8_t *d_live = nullptr;      // per node: weight > 0 (the FeatureVector skips stopped words)
     int *d_child_ptr = nullptr, *d_children = nullptr;
     std::vector<int32_t> word_id;   // per node, host side (leaf -> word)
     std::vector<double> weight;
@@ -173,7 +269,7 @@ extern "C" void orbfe_vocabulary_destroy(OrbfeVocabulary *v) {
     if (!v) return;
     cudaSetDevice(v->device);
     if (v->stream) cudaStreamDestroy(v->stream);
-    cudaFree(v->d_desc); cudaFree(v->d_child_ptr); cudaFree(v->d_children); cudaFree(v->d_in); cudaFree(v->d_out);
+    cudaFree(v->d_desc); cudaFree(v->d_live); cudaFree(v->d_child_ptr); cudaFree(v->d_children); cudaFree(v->d_in); cudaFree(v->d_out);
     delete v;
 }
 
@@ -202,8 +298,12 @@ extern "C" OrbfeVocabulary *orbfe_vocabulary_create(int device, int nnodes, int 
     v->device = device; v->nnodes = nnodes; v->depth = depth_L; v->weighting = weighting; v->norm = norm;
     v->word_id.assign(word_id, word_id + nnodes);
     v->weight.assign(weight, weight + nnodes);
+    std::vector<uint8_t> live(nnodes);
+    for (int i = 0; i < nnodes; i++) live[i] = weight[i] > 0 ? 1 : 0;
     bool ok = cudaSetDevice(device) == cudaSuccess && cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking) == cudaSuccess &&
               cudaMalloc((void **)&v->d_desc, (size_t)nnodes * 32) == cudaSuccess &&
+              cudaMalloc((void **)&v->d_live, (size_t)nnodes) == cudaSuccess &&
+              cudaMemcpy(v->d_live, live.data(), (size_t)nnodes, cudaMemcpyHostToDevice) == cudaSuccess &&
               cudaMalloc((void **)&v->d_child_ptr, sizeof(int) * ((size_t)nnodes + 1)) == cudaSuccess &&
               cudaMalloc((void **)&v->d_children, sizeof(int) * (size_t)std::max(nchild, 1)) == cudaSuccess &&
               cudaMemcpy(v->d_desc, node_desc, (size_t)nnodes * 32, cudaMemcpyHostToDevice) == cudaSuccess &&
@@ -227,6 +327,24 @@ extern "C" int orbfe_bow_descend_device(OrbfeVocabulary *v, const uint8_t *d_des
     bow_descend_kernel<<<(n + 7) / 8, 256, 0, s>>>(reinterpret_cast<const uint4 *>(v->d_desc), v->d_child_ptr, v->d_children,
                                                    reinterpret_cast<const uint4 *>(d_desc), n, v->depth - levelsup, d_leaf_out,
                                                    d_node_out);
+    BOW_TRY(cudaGetLastError());
+    return ORBFE_OK;
+}
+
+extern "C" int orbfe_feature_vector_device(OrbfeVocabulary *v, int nframes, const int32_t *d_leaf, const int32_t *d_node,
+                                           const int *d_counts, int cap, int32_t *d_fv_ids, int32_t *d_fv_ptr, int32_t *d_fv_items,
+                                           int *d_fv_n, void *stream) {
+    if (!v || nframes < 0 || cap < 1) return set_error(ORBFE_ERR_ARG, "bad arguments");
+    if (nframes > 0 && (!d_leaf || !d_node || !d_counts || !d_fv_ids || !d_fv_ptr || !d_fv_items || !d_fv_n))
+        return set_error(ORBFE_ERR_ARG, "NULL argument");
+    if (cap > ORBFE_FV_MAX_CAP)
+        return set_error(ORBFE_ERR_UNSUPPORTED, "cap %d exceeds the %d features per frame the FeatureVector kernel sorts in shared memory",
+                         cap, ORBFE_FV_MAX_CAP);
+    if (nframes == 0) return ORBFE_OK;
+    BOW_TRY(cudaSetDevice(v->device));
+    cudaStream_t s = stream ? (cudaStream_t)stream : v->stream;
+    BOW_TRY((cudaError_t)launch_feature_vector(nframes, d_leaf, d_node, v->d_live, v->nnodes, d_counts, cap, d_fv_ids, d_fv_ptr,
+                                               d_fv_items, d_fv_n, s));
     BOW_TRY(cudaGetLastError());
     return ORBFE_OK;
 }

@@ -236,6 +236,32 @@ __device__ __forceinline__ bool octave_ok(int o, int lo, int hi) {
     return (lo == -1 && hi == -1) || (o >= lo && o <= hi);
 }
 
+// Rotation histogram of the matchers (e.g. ORBmatcher.cc:263-281, :1583-1590): bin = round((a1 - a2 [+360]) * (1/30)), 30 -> 0.
+__device__ __forceinline__ int rot_hist_bin(float a1, float a2) {
+    float rot = __fsub_rn(a1, a2);
+    if (rot < 0.0f) rot = __fadd_rn(rot, 360.0f);
+    int bin = (int)roundf(__fmul_rn(rot, 1.0f / 30));
+    if (bin == 30) bin = 0;
+    return bin;
+}
+
+// ComputeThreeMaxima (ORBmatcher.cc:1748-1789) over the 30 bin counts `hist`: keep[0..2] = the bins whose matches stay (-1 =
+// none).  The first maximum wins ties; the second and third are dropped when below 0.1 * max1.  For one thread.  A macro rather
+// than an inline function: expanded in place it leaves the fused projection kernel's SASS exactly as it was.
+#define THREE_MAXIMA_KEEP(hist, keep)                                                                    \
+    {                                                                                                    \
+        int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;                               \
+        for (int i = 0; i < 30; i++) {                                                                   \
+            const int s = (hist)[i];                                                                     \
+            if (s > max1) { max3 = max2; max2 = max1; max1 = s; ind3 = ind2; ind2 = ind1; ind1 = i; }    \
+            else if (s > max2) { max3 = max2; max2 = s; ind3 = ind2; ind2 = i; }                         \
+            else if (s > max3) { max3 = s; ind3 = i; }                                                   \
+        }                                                                                                \
+        if ((float)max2 < __fmul_rn(0.1f, (float)max1)) { ind2 = -1; ind3 = -1; }                        \
+        else if ((float)max3 < __fmul_rn(0.1f, (float)max1)) { ind3 = -1; }                             \
+        (keep)[0] = ind1; (keep)[1] = ind2; (keep)[2] = ind3;                                            \
+    }
+
 // MODE 0: SearchByProjection(Frame, Frame) -- queries = projections of the Last frame's map points;
 // MODE 1: guided search -- explicit query windows (M3, M4, M6, M7 and the KeyFrame-level routines);
 // MODE 2: SearchForInitialization(F1, F2, vbPrevMatched, vnMatches12, windowSize) (ORBmatcher.cc:598-713) -- queries = the
@@ -754,26 +780,12 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
             for (int q = tid; q < nl; q += SBP_THREADS) {   // :666-676, one entry per ACCEPTED feature, unmatched later or not
                 const int i2 = choice[q];
                 if (i2 == 0xFFFF) continue;
-                float rot = __fsub_rn(kl[q].angle, kc[i2].angle);
-                if (rot < 0.0f) rot = __fadd_rn(rot, 360.0f);
-                int bin = (int)roundf(__fmul_rn(rot, 1.0f / 30));
-                if (bin == 30) bin = 0;
+                const int bin = rot_hist_bin(kl[q].angle, kc[i2].angle);
                 newbin[q] = (uint8_t)bin;
                 atomicAdd(&s_hist[bin], 1);
             }
             __syncthreads();
-            if (tid == 0) {
-                int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
-                for (int i = 0; i < 30; i++) {
-                    const int s = s_hist[i];
-                    if (s > max1) { max3 = max2; max2 = max1; max1 = s; ind3 = ind2; ind2 = ind1; ind1 = i; }
-                    else if (s > max2) { max3 = max2; max2 = s; ind3 = ind2; ind2 = i; }
-                    else if (s > max3) { max3 = s; ind3 = i; }
-                }
-                if ((float)max2 < __fmul_rn(0.1f, (float)max1)) { ind2 = -1; ind3 = -1; }
-                else if ((float)max3 < __fmul_rn(0.1f, (float)max1)) { ind3 = -1; }
-                s_keep[0] = ind1; s_keep[1] = ind2; s_keep[2] = ind3;
-            }
+            if (tid == 0) THREE_MAXIMA_KEEP(s_hist, s_keep)
             __syncthreads();
             int removed = 0;
             for (int q = tid; q < nl; q += SBP_THREADS) {   // :691-702: only features that are still matched lose their match
@@ -796,26 +808,12 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
         // rotation histogram of the new matches (:1583-1590), in parallel: bin = round((aLast - aCur [+360]) / 30)
         for (int i = tid; i < nc; i += SBP_THREADS) {
             if (newbin[i] != 0xFE) continue;
-            float rot = __fsub_rn(query_angle(mp[i]), kc[i].angle);
-            if (rot < 0.0f) rot = __fadd_rn(rot, 360.0f);
-            int bin = (int)roundf(__fmul_rn(rot, 1.0f / 30));
-            if (bin == 30) bin = 0;
+            const int bin = rot_hist_bin(query_angle(mp[i]), kc[i].angle);
             newbin[i] = (uint8_t)bin;
             atomicAdd(&s_hist[bin], 1);
         }
         __syncthreads();
-        if (tid == 0) {
-            int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
-            for (int i = 0; i < 30; i++) {
-                const int s = s_hist[i];
-                if (s > max1) { max3 = max2; max2 = max1; max1 = s; ind3 = ind2; ind2 = ind1; ind1 = i; }
-                else if (s > max2) { max3 = max2; max2 = s; ind3 = ind2; ind2 = i; }
-                else if (s > max3) { max3 = s; ind3 = i; }
-            }
-            if ((float)max2 < __fmul_rn(0.1f, (float)max1)) { ind2 = -1; ind3 = -1; }
-            else if ((float)max3 < __fmul_rn(0.1f, (float)max1)) { ind3 = -1; }
-            s_keep[0] = ind1; s_keep[1] = ind2; s_keep[2] = ind3;
-        }
+        if (tid == 0) THREE_MAXIMA_KEEP(s_hist, s_keep)
         __syncthreads();
         int removed = 0;
         for (int i = tid; i < nc; i += SBP_THREADS) {
@@ -879,6 +877,150 @@ int launch_guided_device(const SbpParams &P, size_t smem_bytes, int njobs, const
     G.qu = qu; G.qv = qv; G.qr = qr; G.qangle = qangle; G.qlo = qlo; G.qhi = qhi; G.qdesc = qdesc; G.q_base = q_base; G.q_cnt = q_cnt;
     sbp_device_kernel<1><<<njobs, SBP_THREADS, smem_bytes, s>>>(P, kps, desc, counts, frame_idx, nullptr, nullptr, nullptr, nullptr, G,
                                                             scratch, slot_owner, nmatches, err);
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// SearchByBoW, both overloads (ORBmatcher.cc:155-284 KeyFrame vs Frame, :715-850 KeyFrame vs KeyFrame), one CTA per job.
+// A FeatureVector holds every feature in exactly one node, so the "already matched" skip (:204 / :773) only ever sees
+// candidates of the node being processed: the common nodes are independent and each one is replayed sequentially, in list
+// order, by one warp -- the reference's result whatever order the warps take the nodes in.  The rotation histogram only
+// needs the bin counts (shared-memory atomics) and each match's bin, recomputed in the final pass.
+// Per side-1 feature the lanes take the free candidates in list order and keep their own two smallest
+// (distance << 16 | list position) keys; the warp minimum is the first minimum of the strict-< scan, and the minimum with
+// the winner's key replaced by its lane's runner-up is the reference's second best.
+// ------------------------------------------------------------------------------------------------
+#define BOW_THREADS 512
+__global__ void __launch_bounds__(BOW_THREADS) search_by_bow_kernel(int variant, const OrbfeKeyPoint *__restrict__ kps,
+                                                                    const uint8_t *__restrict__ desc, const int *__restrict__ counts,
+                                                                    int cap, const int *__restrict__ fv_ids,
+                                                                    const int *__restrict__ fv_ptr, const int *__restrict__ fv_items,
+                                                                    const int *__restrict__ fv_n, const uint8_t *__restrict__ valid,
+                                                                    const int *__restrict__ idx1, const int *__restrict__ idx2,
+                                                                    float nnratio, int check_ori, int *__restrict__ out,
+                                                                    int *__restrict__ nmatches, int *__restrict__ err) {
+    extern __shared__ uint32_t matched2[];   // [(cap + 31) / 32] side-2 feature already matched in this job
+    __shared__ int s_hist[32], s_keep[3], s_nm, s_removed, s_bad;
+    const int job = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int f1 = idx1[job], f2 = idx2[job];
+    const int n1 = min(max(counts[f1], 0), cap), n2 = min(max(counts[f2], 0), cap);
+    const int nn1 = fv_n[f1], nn2 = fv_n[f2];
+    const int nout = variant == 0 ? n2 : n1;
+    int *__restrict__ row = out + (size_t)job * cap;
+    const OrbfeKeyPoint *__restrict__ k1 = kps + (size_t)f1 * cap;
+    const OrbfeKeyPoint *__restrict__ k2 = kps + (size_t)f2 * cap;
+    const uint4 *__restrict__ d1 = reinterpret_cast<const uint4 *>(desc + (size_t)f1 * cap * 32);
+    const uint4 *__restrict__ d2 = reinterpret_cast<const uint4 *>(desc + (size_t)f2 * cap * 32);
+    const uint8_t *__restrict__ v1 = valid + (size_t)f1 * cap;
+    const uint8_t *__restrict__ v2 = valid + (size_t)f2 * cap;
+    const int *__restrict__ ids1 = fv_ids + (size_t)f1 * cap, *__restrict__ ids2 = fv_ids + (size_t)f2 * cap;
+    const int *__restrict__ ptr1 = fv_ptr + (size_t)f1 * (cap + 1), *__restrict__ ptr2 = fv_ptr + (size_t)f2 * (cap + 1);
+    const int *__restrict__ it1 = fv_items + (size_t)f1 * cap, *__restrict__ it2 = fv_items + (size_t)f2 * cap;
+
+    for (int i = tid; i < (cap + 31) / 32; i += BOW_THREADS) matched2[i] = 0;
+    for (int i = tid; i < nout; i += BOW_THREADS) row[i] = -1;
+    if (tid < 32) s_hist[tid] = 0;
+    if (tid == 0) { s_nm = 0; s_removed = 0; s_bad = (nn1 < 0 || nn1 > cap || nn2 < 0 || nn2 > cap) ? 1 : 0; }
+    __syncthreads();
+    const bool bad_n = s_bad != 0;
+    bool bad = false;   // warp-uniform: this warp met an out-of-range node row or item index
+    int nm = 0;
+    for (int a = warp; a < nn1 && !bad_n && !bad; a += BOW_THREADS / 32) {
+        // the side-2 node with the same id (ids ascending): lower_bound
+        const int id = ids1[a];
+        int lo = 0, hi = nn2;
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (ids2[mid] < id) lo = mid + 1; else hi = mid;
+        }
+        if (lo == nn2 || ids2[lo] != id) continue;
+        const int b1 = ptr1[a], e1 = ptr1[a + 1], b2 = ptr2[lo], e2 = ptr2[lo + 1];
+        if (b1 < 0 || b1 > e1 || e1 > cap || b2 < 0 || b2 > e2 || e2 > cap) { bad = true; break; }
+        // the first 32 candidates stay in registers for all side-1 features of the node
+        int c_i2 = -1;
+        uint4 c0 = make_uint4(0, 0, 0, 0), c1 = c0;
+        bool c_bad = false;
+        if (b2 + lane < e2) {
+            c_i2 = it2[b2 + lane];
+            if ((unsigned)c_i2 >= (unsigned)n2) c_bad = true;
+            else if (variant == 1 && !v2[c_i2]) c_i2 = -1;   // :777 (variant 0 does not look at the Frame's map points)
+            else { c0 = __ldg(&d2[2 * c_i2]); c1 = __ldg(&d2[2 * c_i2 + 1]); }
+        }
+        if (__any_sync(0xffffffffu, c_bad)) { bad = true; break; }
+        for (int p1 = b1; p1 < e1; p1++) {
+            const int i1 = it1[p1];
+            if ((unsigned)i1 >= (unsigned)n1) { bad = true; break; }
+            if (!v1[i1]) continue;
+            const uint4 a0 = __ldg(&d1[2 * i1]), a1 = __ldg(&d1[2 * i1 + 1]);
+            uint32_t m1 = 0xFFFFFFFFu, m2 = 0xFFFFFFFFu;   // this lane's two smallest keys
+            if (c_i2 >= 0 && !((matched2[c_i2 >> 5] >> (c_i2 & 31)) & 1u))
+                m1 = ((uint32_t)ham256(a0, a1, c0, c1) << 16) | (uint32_t)lane;
+            for (int p = b2 + 32 + lane; p - lane < e2; p += 32) {
+                bool lbad = false;
+                if (p < e2) {
+                    const int i2 = it2[p];
+                    if ((unsigned)i2 >= (unsigned)n2) lbad = true;
+                    else if ((variant == 0 || v2[i2]) && !((matched2[i2 >> 5] >> (i2 & 31)) & 1u)) {
+                        const uint32_t key = ((uint32_t)ham256(a0, a1, __ldg(&d2[2 * i2]), __ldg(&d2[2 * i2 + 1])) << 16) | (uint32_t)(p - b2);
+                        if (key < m1) { m2 = m1; m1 = key; }
+                        else if (key < m2) m2 = key;
+                    }
+                }
+                if (__any_sync(0xffffffffu, lbad)) { bad = true; break; }
+            }
+            if (bad) break;
+            const uint32_t best = __reduce_min_sync(0xffffffffu, m1);
+            if (best == 0xFFFFFFFFu) continue;
+            const uint32_t second = __reduce_min_sync(0xffffffffu, m1 == best ? m2 : m1);
+            const int bd = (int)(best >> 16);
+            // INT_MAX stands for "no second candidate": (float)INT_MAX in the reference's comparison
+            const float sd = second == 0xFFFFFFFFu ? 2147483648.0f : (float)(int)(second >> 16);
+            const bool pass = variant == 0 ? bd <= 50 : bd < 50;   // TH_LOW, :224 vs :797
+            if (pass && (float)bd < __fmul_rn(nnratio, sd)) {
+                const int i2 = it2[b2 + (int)(best & 0xFFFF)];
+                if (lane == 0) {
+                    atomicOr(&matched2[i2 >> 5], 1u << (i2 & 31));
+                    if (variant == 0) row[i2] = i1; else row[i1] = i2;
+                    if (check_ori) atomicAdd(&s_hist[rot_hist_bin(k1[i1].angle, k2[i2].angle)], 1);
+                }
+                nm++;
+                __syncwarp();
+            }
+        }
+    }
+    if (lane == 0) {
+        if (bad) s_bad = 1;
+        if (nm) atomicAdd(&s_nm, nm);
+    }
+    __syncthreads();
+    if (s_bad) {   // malformed FeatureVector: nothing outside the frames' slots was read; the row is not meaningful
+        if (tid == 0) { nmatches[job] = -1; atomicOr(err, 2); }
+        return;
+    }
+    if (check_ori) {
+        if (tid == 0) THREE_MAXIMA_KEEP(s_hist, s_keep)
+        __syncthreads();
+        int removed = 0;
+        for (int r = tid; r < nout; r += BOW_THREADS) {
+            const int o = row[r];
+            if (o < 0) continue;
+            const int bin = variant == 0 ? rot_hist_bin(k1[o].angle, k2[r].angle) : rot_hist_bin(k1[r].angle, k2[o].angle);
+            if (bin != s_keep[0] && bin != s_keep[1] && bin != s_keep[2]) { row[r] = -1; removed++; }
+        }
+        if (removed) atomicAdd(&s_removed, removed);
+        __syncthreads();
+    }
+    if (tid == 0) nmatches[job] = s_nm - s_removed;
+}
+
+int launch_search_by_bow(int variant, int njobs, const OrbfeKeyPoint *kps, const uint8_t *desc, const int *counts, int cap,
+                         const int *fv_ids, const int *fv_ptr, const int *fv_items, const int *fv_n, const uint8_t *valid,
+                         const int *idx1, const int *idx2, float nnratio, int check_ori, int *out, int *nmatches, int *err,
+                         cudaStream_t s) {
+    if (njobs <= 0) return 0;
+    const size_t smem = sizeof(uint32_t) * (((size_t)cap + 31) / 32);
+    search_by_bow_kernel<<<njobs, BOW_THREADS, smem, s>>>(variant, kps, desc, counts, cap, fv_ids, fv_ptr, fv_items, fv_n, valid,
+                                                          idx1, idx2, nnratio, check_ori, out, nmatches, err);
     return 0;
 }
 

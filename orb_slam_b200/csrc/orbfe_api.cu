@@ -941,7 +941,11 @@ extern "C" int orbfe_matcher_sync(OrbfeMatcher *m) {
     CU_TRY(cudaMemcpyAsync(m->h_err, m->d_err, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
     CU_TRY(cudaStreamSynchronize(m->stream));
     if (*m->h_err) {
+        const int flags = *m->h_err;
         CU_TRY(cudaMemsetAsync(m->d_err, 0, sizeof(int), m->stream));
+        if (flags & 2)
+            return fail(ORBFE_ERR_ARG, "orbfe_search_by_bow_device: a job's FeatureVector has an out-of-range node row or feature "
+                                       "index (its nmatches is -1)");
         return fail(ORBFE_ERR_CAPACITY, "device matcher: a pair exceeded the candidate scratch budget (its nmatches is -1); "
                                         "use orbfe_search_by_projection_frames for that pair");
     }
@@ -1101,6 +1105,27 @@ extern "C" int orbfe_guided_search_device(OrbfeMatcher *m, int njobs, const Orbf
     int rc = launch_guided_device(P, total, njobs, d_kps, d_desc, d_counts, d_frame_idx, d_qu, d_qv, d_qr, d_qlo, d_qhi, d_qdesc,
                                   d_qangle, d_q_base, d_q_cnt, m->scratch, d_slot_owner, d_nmatches, m->d_err, s);
     if (rc) return fail(ORBFE_ERR_CUDA, "cudaFuncSetAttribute failed: %s", cudaGetErrorString((cudaError_t)rc));
+    CU_TRY(cudaGetLastError());
+    m->launches += 1;
+    return ORBFE_OK;
+}
+
+// SearchByBoW (both overloads) for `njobs` frame pairs, device-resident (include/orbfe_match.h).  Arguments are checked before
+// the handle is used.
+extern "C" int orbfe_search_by_bow_device(OrbfeMatcher *m, int variant, int njobs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
+                                          const int *d_counts, int cap, const int32_t *d_fv_ids, const int32_t *d_fv_ptr,
+                                          const int32_t *d_fv_items, const int *d_fv_n, const uint8_t *d_valid, const int *d_idx1,
+                                          const int *d_idx2, float nnratio, int check_orientation, int32_t *d_out, int *d_nmatches,
+                                          void *stream) {
+    if (!m || (variant != 0 && variant != 1) || njobs < 0 || cap < 1 || cap > 65535) return fail(ORBFE_ERR_ARG, "bad arguments");
+    if (njobs == 0) return ORBFE_OK;
+    if (!d_kps || !d_desc || !d_counts || !d_fv_ids || !d_fv_ptr || !d_fv_items || !d_fv_n || !d_valid || !d_idx1 || !d_idx2 ||
+        !d_out || !d_nmatches)
+        return fail(ORBFE_ERR_ARG, "NULL argument");
+    CU_TRY(cudaSetDevice(m->device));
+    cudaStream_t s = stream ? (cudaStream_t)stream : m->stream;
+    launch_search_by_bow(variant, njobs, d_kps, d_desc, d_counts, cap, d_fv_ids, d_fv_ptr, d_fv_items, d_fv_n, d_valid, d_idx1, d_idx2,
+                         nnratio, check_orientation ? 1 : 0, d_out, d_nmatches, m->d_err, s);
     CU_TRY(cudaGetLastError());
     m->launches += 1;
     return ORBFE_OK;

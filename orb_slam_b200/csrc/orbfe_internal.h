@@ -158,6 +158,12 @@ int launch_sbp_device(const SbpParams &P, size_t smem_bytes, int npairs, const O
                       const int *counts, const int *cur_idx, const int *last_idx, const float *world, const uint8_t *flags,
                       const float *Tcw, uint32_t *scratch, int *cur_mp, int *nmatches, int *err, cudaStream_t s);
 
+// SearchByBoW for `njobs` (side 1, side 2) frame pairs (match_kernels.cu); out-of-range FeatureVector entries set bit 2 of *err
+int launch_search_by_bow(int variant, int njobs, const OrbfeKeyPoint *kps, const uint8_t *desc, const int *counts, int cap,
+                         const int *fv_ids, const int *fv_ptr, const int *fv_items, const int *fv_n, const uint8_t *valid,
+                         const int *idx1, const int *idx2, float nnratio, int check_ori, int *out, int *nmatches, int *err,
+                         cudaStream_t s);
+
 void launch_undistort(float fx, float fy, float cx, float cy, const float *dist5, const OrbfeKeyPoint *d_in, OrbfeKeyPoint *d_out,
                       int n, cudaStream_t s);
 

@@ -58,6 +58,8 @@ def _bind():
     L.orbfe_guided_best.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, C.c_int, vp]
     L.orbfe_window_search.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, vp, vp]
     L.orbfe_search_for_initialization.argtypes = [vp, vp, vp, vp, C.c_int, C.c_float, C.c_int, vp, vp]
+    L.orbfe_search_by_bow_device.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, C.c_float, C.c_int,
+                                             vp, vp, vp]
     _bound = True
     return L
 
@@ -290,6 +292,18 @@ def search_by_bow(matcher: ORBmatcher, variant, desc1, valid1, angle1, fv1, desc
                                  n2, _p(desc2), _p(valid2), _p(angle2), len(i2), _p(i2), _p(p2), _p(t2),
                                  float(matcher.mfNNratio), int(matcher.mbCheckOrientation), _p(out), C.byref(nm)))
     return nm.value, out[:(n2 if variant == 0 else n1)]
+
+
+def search_by_bow_device(matcher: ORBmatcher, variant, njobs, d_kps, d_desc, d_counts, cap, d_fv_ids, d_fv_ptr, d_fv_items, d_fv_n,
+                         d_valid, d_idx1, d_idx2, d_out, d_nmatches, stream=0):
+    """Device-pointer form (ints = raw device addresses) of SearchByBoW for `njobs` (side 1, side 2) frame pairs, with the
+    FeatureVectors in the layout of bow.feature_vector_device; see include/orbfe_match.h.  Enqueued, not synchronised."""
+    L = _bind()
+    vp = C.c_void_p
+    _check(L.orbfe_search_by_bow_device(matcher.handle, variant, njobs, vp(d_kps), vp(d_desc), vp(d_counts), cap, vp(d_fv_ids),
+                                        vp(d_fv_ptr), vp(d_fv_items), vp(d_fv_n), vp(d_valid), vp(d_idx1), vp(d_idx2),
+                                        float(matcher.mfNNratio), int(matcher.mbCheckOrientation), vp(d_out), vp(d_nmatches),
+                                        vp(stream)))
 
 
 def guided_search(matcher: ORBmatcher, f, qu, qv, qr, qlo, qhi, qdesc, qangle, rule, th_dist, hist_mode, slot_owner=None):

@@ -5,8 +5,12 @@
                    device-resident batch, achieved GB/s against the 130.86 MB/frame of SURVEY.md 8(d)
   --what config5   BASELINE configs[4]: 2000 query descriptors x (ngroups keyframes x 2000 descriptors): the brute-force
                    best/second sweep (knn2 kernel), Gpairs/s, HBM GB/s, POPC-pipe estimate
-  --what small     the latency-bound kernels once each (bow_descend, distinctive, undistort, hamming_csr, sbp single pair)
-                   so that an `ncu -k regex:` capture finds them
+  --what small     the latency-bound kernels once each (bow_descend, distinctive, undistort, hamming_csr, sbp single pair,
+                   feature_vector, search_by_bow) so that an `ncu -k regex:` capture finds them
+  --what reloc     SearchByBoW at its two call sites, device-resident: relocalisation (one 1080p / 2000-keypoint frame against
+                   32 candidate keyframes, KeyFrame-vs-Frame overload) and loop closing (one keyframe against 16 candidates,
+                   KeyFrame-vs-KeyFrame); CUDA-event ms of the FeatureVector build and of the batched search, next to the wall
+                   time of the same jobs through the per-pair host entry point orbfe_search_by_bow
 
 Prints one JSON object per --what; never a bench value when run under ncu."""
 import argparse
@@ -172,10 +176,112 @@ def small(args):
         out["bow_words"] = int(len(V.transform(d0, 2)[0][0]))
         gp = np.arange(0, len(d0) + 1, 20, dtype=np.int32)
         out["distinctive_groups"] = int(len(BW.distinctive_descriptors(m, d0[:gp[-1]], gp)))
+        # feature_vector_kernel and search_by_bow_kernel: frame 1 against frame 0, device-resident
+        dev = torch.device("cuda", 0)
+        cap = 2000
+        kk, dd = np.zeros((2, cap), fe.KP_DTYPE), np.zeros((2, cap, 32), np.uint8)
+        kk[0, :len(k0)], kk[1, :len(k1)], dd[0, :len(d0)], dd[1, :len(d1)] = k0, k1, d0, d1
+        t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+        d_k, d_d, d_c = t(kk.view(np.uint8).reshape(2, cap, 28)), t(dd), t(np.array([len(k0), len(k1)], np.int32))
+        d_leaf, d_node = (torch.zeros(2 * cap, dtype=torch.int32, device=dev) for _ in range(2))
+        d_ids, d_items, d_out = (torch.zeros((2, cap), dtype=torch.int32, device=dev) for _ in range(3))
+        d_ptr, d_n = torch.zeros((2, cap + 1), dtype=torch.int32, device=dev), torch.zeros(2, dtype=torch.int32, device=dev)
+        d_valid, d_i1, d_i2 = torch.ones((2, cap), dtype=torch.uint8, device=dev), t(np.array([1], np.int32)), t(np.array([0], np.int32))
+        d_nm = torch.zeros(1, dtype=torch.int32, device=dev)
+        s = torch.cuda.Stream(device=dev)
+        torch.cuda.synchronize()
+        V.descend_device(d_d.data_ptr(), 2 * cap, 2, d_leaf.data_ptr(), d_node.data_ptr(), s.cuda_stream)
+        BW.feature_vector_device(V, 2, d_leaf.data_ptr(), d_node.data_ptr(), d_c.data_ptr(), cap, d_ids.data_ptr(), d_ptr.data_ptr(),
+                                 d_items.data_ptr(), d_n.data_ptr(), s.cuda_stream)
+        M.search_by_bow_device(m, 0, 1, d_k.data_ptr(), d_d.data_ptr(), d_c.data_ptr(), cap, d_ids.data_ptr(), d_ptr.data_ptr(),
+                               d_items.data_ptr(), d_n.data_ptr(), d_valid.data_ptr(), d_i1.data_ptr(), d_i2.data_ptr(), d_out.data_ptr(),
+                               d_nm.data_ptr(), s.cuda_stream)
+        s.synchronize()
+        m.sync()
+        out["bow_device_matches"] = int(d_nm.item())
         V.close()
     except Exception as e:
         out["bow"] = "skipped: %r" % e
     ex.close(); m.close()
+    return out
+
+
+def reloc(args):
+    import torch
+    import orb_slam_b200 as fe
+    from orb_slam_b200 import matching as M, bow as BW
+    from orb_slam_b200.synth import textured_frame, shifted_frame, random_vocabulary
+    W, H, NF, levelsup, NKF, NLOOP = 1920, 1080, 2000, 4, 32, 16
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    s = stream.cuda_stream
+    base = textured_frame(W, H, seed=21)
+    # frame 0: the current frame; frames 1..32: the candidate keyframes (views of the same place)
+    frames = np.stack([base] + [shifted_frame(base, 4 * (i % 5) - 8, 3 * (i % 3) - 3, seed=i) for i in range(1, NKF + 1)])
+    F = len(frames)
+    ex = fe.ORBextractor(NF, 1.2, 8)
+    kps, desc, cnt = ex.extract_batch(frames)
+    ex.close()
+    voc = random_vocabulary(10, 6, seed=3)   # the shape of ORBvoc: k = 10, L = 6; levelsup 4 = nodes of level 2
+    V = BW.Vocabulary(voc)
+    valid = (np.random.default_rng(1).random((F, NF)) < 0.9).astype(np.uint8)
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    d_k, d_d, d_c, d_valid = t(kps.view(np.uint8).reshape(F, NF, 28)), t(desc), t(cnt), t(valid)
+    d_leaf, d_node = (torch.zeros(F * NF, dtype=torch.int32, device=dev) for _ in range(2))
+    d_ids, d_items = (torch.zeros((F, NF), dtype=torch.int32, device=dev) for _ in range(2))
+    d_ptr, d_n = torch.zeros((F, NF + 1), dtype=torch.int32, device=dev), torch.zeros(F, dtype=torch.int32, device=dev)
+    m = fe.ORBmatcher(0.75, True)
+    V.descend_device(d_d.data_ptr(), F * NF, levelsup, d_leaf.data_ptr(), d_node.data_ptr(), s)
+
+    def timed(fn, iters=args.iters * 4, warm=args.warmup):
+        for _ in range(warm):
+            fn()
+        stream.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        for _ in range(iters):
+            fn()
+        e1.record(stream)
+        stream.synchronize()
+        return e0.elapsed_time(e1) / iters
+
+    out = {"what": "SearchByBoW device-resident, 1920x1080 frames, %d keypoints, vocabulary k=10 L=6, levelsup %d" % (NF, levelsup),
+           "counts_min": int(cnt.min())}
+    fv = lambda nf: BW.feature_vector_device(V, nf, d_leaf.data_ptr(), d_node.data_ptr(), d_c.data_ptr(), NF, d_ids.data_ptr(),
+                                             d_ptr.data_ptr(), d_items.data_ptr(), d_n.data_ptr(), s)
+    out["feature_vector_1_frame_ms"] = timed(lambda: fv(1))
+    out["feature_vector_%d_frames_ms" % F] = timed(lambda: fv(F))
+    stream.synchronize()
+    ids, ptr, items, nn = (x.cpu().numpy() for x in (d_ids, d_ptr, d_items, d_n))
+    fvs = [(ids[f, :nn[f]], ptr[f, :nn[f] + 1], items[f, :ptr[f, nn[f]]]) for f in range(F)]
+    out["nodes_per_frame_mean"] = float(nn.mean())
+    for tag, variant, jobs in (("reloc_%dkf" % NKF, 0, [(f, 0) for f in range(1, NKF + 1)]),
+                               ("loop_%dcand" % NLOOP, 1, [(0, f) for f in range(1, NLOOP + 1)])):
+        j = np.array(jobs, np.int32)
+        d_i1, d_i2 = t(j[:, 0]), t(j[:, 1])
+        d_out = torch.zeros((len(j), NF), dtype=torch.int32, device=dev)
+        d_nm = torch.zeros(len(j), dtype=torch.int32, device=dev)
+        call = lambda: M.search_by_bow_device(m, variant, len(j), d_k.data_ptr(), d_d.data_ptr(), d_c.data_ptr(), NF, d_ids.data_ptr(),
+                                              d_ptr.data_ptr(), d_items.data_ptr(), d_n.data_ptr(), d_valid.data_ptr(), d_i1.data_ptr(),
+                                              d_i2.data_ptr(), d_out.data_ptr(), d_nm.data_ptr(), s)
+        out[tag + "_device_ms"] = timed(call)
+        m.sync()
+        dev_out, dev_nm = d_out.cpu().numpy(), d_nm.cpu().numpy()
+        same = True
+        lat = []
+        for rep in range(3):
+            t0 = time.perf_counter()
+            for q, (f1, f2) in enumerate(jobs):
+                n1, n2 = cnt[f1], cnt[f2]
+                nm, o = M.search_by_bow(m, variant, desc[f1, :n1], valid[f1, :n1], kps[f1, :n1]["angle"], fvs[f1], desc[f2, :n2],
+                                        valid[f2, :n2], kps[f2, :n2]["angle"], fvs[f2])
+                if rep == 0:
+                    same = same and nm == dev_nm[q] and np.array_equal(o, dev_out[q, :len(o)])
+            lat.append((time.perf_counter() - t0) * 1e3)
+        out[tag + "_host_per_pair_wall_ms"] = float(np.median(lat))
+        out[tag + "_matches"] = int(dev_nm.sum())
+        out[tag + "_same_as_host"] = bool(same)
+    V.close(); m.close()
     return out
 
 
@@ -465,4 +571,5 @@ if __name__ == "__main__":
     ap.add_argument("--warmup", type=int, default=2)
     args = ap.parse_args()
     for w in args.what.split(","):
-        print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fastarc": fastarc, "latency": latency}[w](args)))
+        print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fastarc": fastarc, "latency": latency,
+                          "reloc": reloc}[w](args)))
