@@ -179,6 +179,29 @@ int orbfe_search_for_triangulation(OrbfeMatcher *m, int n1, const OrbfeKeyPoint 
                                    const int32_t *ids2, const int32_t *ptr2, const int32_t *items2, const float *F12,
                                    const float *sigma2_kf2, int check_orientation, int32_t *match12_out, int *nmatches_out);
 
+/* SearchForTriangulation (as orbfe_search_for_triangulation) with the keyframes device-resident, for `njobs` keyframe pairs
+ * per call: job j matches pKF1 = frame d_idx1[j] against pKF2 = frame d_idx2[j] of the frame store d_kps / d_desc / d_counts
+ * (frame f at f*cap, as orbfe_extract_batch_device lays it out; the keypoints are the undistorted ones, e.g. after
+ * orbfe_undistort_keypoints_device in place).  Many jobs may share a frame: LocalMapping::CreateNewMapPoints
+ * (LocalMapping.cc:205-252) matches the new keyframe against each of its covisible neighbours.
+ * FeatureVectors in the layout orbfe_feature_vector_device writes, as in orbfe_search_by_bow_device.
+ * d_has_mp[f*cap + i] != 0: feature i of frame f has a map point (GetMapPointMatches()[i] != NULL, bad points included).
+ * d_F12 = njobs x 9 row-major floats (ComputeF12 of the pair); sigma2 = `nlevels` floats on the HOST (KeyFrame::GetSigma2,
+ * shared by all keyframes of one extractor).  Row j of d_match12 (njobs x cap) is indexed by side-1 feature and holds the
+ * matched side-2 index or -1 for the first counts[d_idx1[j]] entries; d_nmatches[j] = the method's return value.
+ * Results equal orbfe_search_for_triangulation's.
+ * One thread block per job, no global scratch.  A job whose FeatureVectors point outside the frames' slots (node count
+ * outside [0, cap], a row outside [0, cap], a feature index >= the frame's count) or whose side-2 features without a map
+ * point in a common node have an octave outside [0, nlevels) is never followed out of bounds: its d_nmatches is -1 and
+ * orbfe_matcher_sync reports ORBFE_ERR_ARG; the other jobs of the launch are unaffected.  Frame indices are not checked.
+ * 1 <= cap <= 65535, 1 <= nlevels <= ORBFE_MAX_LEVELS.  Enqueued on `stream` (NULL = the matcher's stream), not
+ * synchronised. */
+int orbfe_search_for_triangulation_device(OrbfeMatcher *m, int njobs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
+                                          const int *d_counts, int cap, const int32_t *d_fv_ids, const int32_t *d_fv_ptr,
+                                          const int32_t *d_fv_items, const int *d_fv_n, const uint8_t *d_has_mp, const int *d_idx1,
+                                          const int *d_idx2, const float *d_F12, const float *sigma2, int nlevels,
+                                          int check_orientation, int32_t *d_match12, int *d_nmatches, void *stream);
+
 /* int ORBmatcher::WindowSearch(F1, F2, windowSize, vpMapPointMatches2, minOctave, maxOctave)
  * (ORBmatcher.cc:409-516).  f1_has_mp[i1] != 0 <=> F1.mvpMapPoints[i1] && !isBad().
  * match21_out[i2] = i1 whose map point was matched to F2 feature i2, or -1. */

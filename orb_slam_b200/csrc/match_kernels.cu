@@ -1025,6 +1025,173 @@ int launch_search_by_bow(int variant, int njobs, const OrbfeKeyPoint *kps, const
 }
 
 // ------------------------------------------------------------------------------------------------
+// SearchForTriangulation (ORBmatcher.cc:852-1014) with CheckDistEpipolarLine (:136-153), one CTA per (pKF1, pKF2) job.
+// The node-disjointness argument of search_by_bow_kernel holds unchanged: vbMatched2 (:911, :940) only ever meets candidates
+// of the node being processed, so warps take the common nodes in any order and each one is replayed sequentially, in list
+// order, by one warp.
+// Per side-1 feature the reference sorts the free candidates with distance <= TH_LOW by (distance, side-2 index) and takes
+// the first one, up to 2 * best distance, that passes the epipolar test: the minimum (distance << 16 | idx2) key among the
+// candidates that pass, kept iff its distance <= 2 * the minimum distance of all of them (cap <= 65535 keeps idx2 in 16
+// bits).  Each lane keeps its own two minima and the warp reduces both.  Ties break by feature index, whatever order the
+// node lists its items in.
+// Every item of a common node is checked (index < count; octave in [0, nlevels) for side-2 features without a map point)
+// before the node is matched, so whether a job is rejected does not depend on the distances.
+// ------------------------------------------------------------------------------------------------
+#define TRI_THREADS 512
+struct TriParams { double thr[ORBFE_MAX_LEVELS]; };   // 3.84 * (double)GetSigma2(level), as in :152
+
+// CheckDistEpipolarLine after the line l = x1' F12 = (la, lb, lc) and den = la^2 + lb^2: individually rounded, in the
+// reference's order
+__device__ __forceinline__ bool epipolar_ok(float la, float lb, float lc, float den, float x2, float y2, double thr) {
+    const float num = __fadd_rn(__fadd_rn(__fmul_rn(la, x2), __fmul_rn(lb, y2)), lc);
+    if (den == 0.0f) return false;
+    const float dsqr = __fdiv_rn(__fmul_rn(num, num), den);
+    return (double)dsqr < thr;
+}
+
+__global__ void __launch_bounds__(TRI_THREADS) search_for_triangulation_kernel(
+    const OrbfeKeyPoint *__restrict__ kps, const uint8_t *__restrict__ desc, const int *__restrict__ counts, int cap,
+    const int *__restrict__ fv_ids, const int *__restrict__ fv_ptr, const int *__restrict__ fv_items, const int *__restrict__ fv_n,
+    const uint8_t *__restrict__ has_mp, const int *__restrict__ idx1, const int *__restrict__ idx2, const float *__restrict__ F12,
+    const TriParams T, int nlevels, int check_ori, int *__restrict__ match12, int *__restrict__ nmatches, int *__restrict__ err) {
+    extern __shared__ uint32_t matched2[];   // [(cap + 31) / 32] side-2 feature already matched in this job
+    __shared__ int s_hist[32], s_keep[3], s_nm, s_removed, s_bad;
+    const int job = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int f1 = idx1[job], f2 = idx2[job];
+    const int n1 = min(max(counts[f1], 0), cap), n2 = min(max(counts[f2], 0), cap);
+    const int nn1 = fv_n[f1], nn2 = fv_n[f2];
+    int *__restrict__ row = match12 + (size_t)job * cap;
+    const OrbfeKeyPoint *__restrict__ k1 = kps + (size_t)f1 * cap;
+    const OrbfeKeyPoint *__restrict__ k2 = kps + (size_t)f2 * cap;
+    const uint4 *__restrict__ d1 = reinterpret_cast<const uint4 *>(desc + (size_t)f1 * cap * 32);
+    const uint4 *__restrict__ d2 = reinterpret_cast<const uint4 *>(desc + (size_t)f2 * cap * 32);
+    const uint8_t *__restrict__ mp1 = has_mp + (size_t)f1 * cap;
+    const uint8_t *__restrict__ mp2 = has_mp + (size_t)f2 * cap;
+    const int *__restrict__ ids1 = fv_ids + (size_t)f1 * cap, *__restrict__ ids2 = fv_ids + (size_t)f2 * cap;
+    const int *__restrict__ ptr1 = fv_ptr + (size_t)f1 * (cap + 1), *__restrict__ ptr2 = fv_ptr + (size_t)f2 * (cap + 1);
+    const int *__restrict__ it1 = fv_items + (size_t)f1 * cap, *__restrict__ it2 = fv_items + (size_t)f2 * cap;
+    const float *__restrict__ F = F12 + (size_t)job * 9;
+    const float F0 = F[0], F1 = F[1], F2 = F[2], F3 = F[3], F4 = F[4], F5 = F[5], F6 = F[6], F7 = F[7], F8 = F[8];
+
+    for (int i = tid; i < (cap + 31) / 32; i += TRI_THREADS) matched2[i] = 0;
+    for (int i = tid; i < n1; i += TRI_THREADS) row[i] = -1;
+    if (tid < 32) s_hist[tid] = 0;
+    if (tid == 0) { s_nm = 0; s_removed = 0; s_bad = (nn1 < 0 || nn1 > cap || nn2 < 0 || nn2 > cap) ? 1 : 0; }
+    __syncthreads();
+    const bool bad_n = s_bad != 0;
+    bool bad = false;   // warp-uniform: this warp met an out-of-range node row, item index or octave
+    int nm = 0;
+    for (int a = warp; a < nn1 && !bad_n && !bad; a += TRI_THREADS / 32) {
+        // the side-2 node with the same id (ids ascending): lower_bound
+        const int id = ids1[a];
+        int lo = 0, hi = nn2;
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (ids2[mid] < id) lo = mid + 1; else hi = mid;
+        }
+        if (lo == nn2 || ids2[lo] != id) continue;
+        const int b1 = ptr1[a], e1 = ptr1[a + 1], b2 = ptr2[lo], e2 = ptr2[lo + 1];
+        if (b1 < 0 || b1 > e1 || e1 > cap || b2 < 0 || b2 > e2 || e2 > cap) { bad = true; break; }
+        bool lbad = false;
+        for (int p = b1 + lane; p < e1; p += 32) lbad |= (unsigned)it1[p] >= (unsigned)n1;
+        for (int p = b2 + lane; p < e2; p += 32) {
+            const int i2 = it2[p];
+            if ((unsigned)i2 >= (unsigned)n2) lbad = true;
+            else if (!mp2[i2] && (unsigned)k2[i2].octave >= (unsigned)nlevels) lbad = true;
+        }
+        if (__any_sync(0xffffffffu, lbad)) { bad = true; break; }
+        // the first 32 candidates stay in registers for all side-1 features of the node
+        int c_i2 = -1;
+        uint4 c0 = make_uint4(0, 0, 0, 0), c1 = c0;
+        float c_x = 0.0f, c_y = 0.0f;
+        double c_thr = 0.0;
+        if (b2 + lane < e2) {
+            c_i2 = it2[b2 + lane];
+            if (mp2[c_i2]) c_i2 = -1;   // :911
+            else {
+                c0 = __ldg(&d2[2 * c_i2]); c1 = __ldg(&d2[2 * c_i2 + 1]);
+                c_x = k2[c_i2].x; c_y = k2[c_i2].y; c_thr = T.thr[k2[c_i2].octave];
+            }
+        }
+        for (int p1 = b1; p1 < e1; p1++) {
+            const int i1 = it1[p1];
+            if (mp1[i1]) continue;   // :895
+            const uint4 a0 = __ldg(&d1[2 * i1]), a1 = __ldg(&d1[2 * i1 + 1]);
+            const float x1 = k1[i1].x, y1 = k1[i1].y;
+            const float la = __fadd_rn(__fadd_rn(__fmul_rn(x1, F0), __fmul_rn(y1, F3)), F6);
+            const float lb = __fadd_rn(__fadd_rn(__fmul_rn(x1, F1), __fmul_rn(y1, F4)), F7);
+            const float lc = __fadd_rn(__fadd_rn(__fmul_rn(x1, F2), __fmul_rn(y1, F5)), F8);
+            const float den = __fadd_rn(__fmul_rn(la, la), __fmul_rn(lb, lb));
+            uint32_t dmin = 0xFFFFFFFFu, kmin = 0xFFFFFFFFu;   // this lane's minimum distance / minimum passing key
+            if (c_i2 >= 0 && !((matched2[c_i2 >> 5] >> (c_i2 & 31)) & 1u)) {
+                const uint32_t d = (uint32_t)ham256(a0, a1, c0, c1);
+                if (d <= 50) {   // TH_LOW, :918
+                    dmin = d;
+                    if (epipolar_ok(la, lb, lc, den, c_x, c_y, c_thr)) kmin = (d << 16) | (uint32_t)c_i2;
+                }
+            }
+            for (int p = b2 + 32 + lane; p < e2; p += 32) {
+                const int i2 = it2[p];
+                if (mp2[i2] || ((matched2[i2 >> 5] >> (i2 & 31)) & 1u)) continue;
+                const uint32_t d = (uint32_t)ham256(a0, a1, __ldg(&d2[2 * i2]), __ldg(&d2[2 * i2 + 1]));
+                if (d > 50) continue;
+                dmin = min(dmin, d);
+                const uint32_t key = (d << 16) | (uint32_t)i2;
+                if (key < kmin && epipolar_ok(la, lb, lc, den, k2[i2].x, k2[i2].y, T.thr[k2[i2].octave])) kmin = key;
+            }
+            const uint32_t best = __reduce_min_sync(0xffffffffu, dmin);
+            if (best == 0xFFFFFFFFu) continue;
+            const uint32_t win = __reduce_min_sync(0xffffffffu, kmin);
+            if (win == 0xFFFFFFFFu || (win >> 16) > 2 * best) continue;   // DistTh = round(2 * BestDist), :929-934
+            if (lane == 0) {
+                const int i2 = (int)(win & 0xFFFF);
+                atomicOr(&matched2[i2 >> 5], 1u << (i2 & 31));
+                row[i1] = i2;
+                if (check_ori) atomicAdd(&s_hist[rot_hist_bin(k1[i1].angle, k2[i2].angle)], 1);
+            }
+            nm++;
+            __syncwarp();
+        }
+    }
+    if (lane == 0) {
+        if (bad) s_bad = 1;
+        if (nm) atomicAdd(&s_nm, nm);
+    }
+    __syncthreads();
+    if (s_bad) {   // malformed input: nothing outside the frames' slots was read; the row is not meaningful
+        if (tid == 0) { nmatches[job] = -1; atomicOr(err, 4); }
+        return;
+    }
+    if (check_ori) {   // :975-994
+        if (tid == 0) THREE_MAXIMA_KEEP(s_hist, s_keep)
+        __syncthreads();
+        int removed = 0;
+        for (int r = tid; r < n1; r += TRI_THREADS) {
+            const int o = row[r];
+            if (o < 0) continue;
+            const int bin = rot_hist_bin(k1[r].angle, k2[o].angle);
+            if (bin != s_keep[0] && bin != s_keep[1] && bin != s_keep[2]) { row[r] = -1; removed++; }
+        }
+        if (removed) atomicAdd(&s_removed, removed);
+        __syncthreads();
+    }
+    if (tid == 0) nmatches[job] = s_nm - s_removed;
+}
+
+int launch_search_for_triangulation(int njobs, const OrbfeKeyPoint *kps, const uint8_t *desc, const int *counts, int cap,
+                                    const int *fv_ids, const int *fv_ptr, const int *fv_items, const int *fv_n, const uint8_t *has_mp,
+                                    const int *idx1, const int *idx2, const float *F12, const float *sigma2, int nlevels,
+                                    int check_ori, int *match12, int *nmatches, int *err, cudaStream_t s) {
+    if (njobs <= 0) return 0;
+    TriParams T;
+    for (int l = 0; l < ORBFE_MAX_LEVELS; l++) T.thr[l] = l < nlevels ? 3.84 * (double)sigma2[l] : 0.0;
+    const size_t smem = sizeof(uint32_t) * (((size_t)cap + 31) / 32);
+    search_for_triangulation_kernel<<<njobs, TRI_THREADS, smem, s>>>(kps, desc, counts, cap, fv_ids, fv_ptr, fv_items, fv_n, has_mp,
+                                                                     idx1, idx2, F12, T, nlevels, check_ori, match12, nmatches, err);
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Frame::UndistortKeyPoints (reference src/Frame.cc:289-319) = cv::undistortPoints(pts, K, D, R = I, P = K): five
 // fixed-point iterations of the inverse distortion model in double, then the re-projection; every operation
 // individually rounded (no FMA), in the order OpenCV evaluates them -- bit-exact against python-cv2

@@ -946,6 +946,10 @@ extern "C" int orbfe_matcher_sync(OrbfeMatcher *m) {
         if (flags & 2)
             return fail(ORBFE_ERR_ARG, "orbfe_search_by_bow_device: a job's FeatureVector has an out-of-range node row or feature "
                                        "index (its nmatches is -1)");
+        if (flags & 4)
+            return fail(ORBFE_ERR_ARG, "orbfe_search_for_triangulation_device: a job's FeatureVector has an out-of-range node row or "
+                                       "feature index, or a side-2 feature without a map point has an octave outside [0, nlevels) "
+                                       "(its nmatches is -1)");
         return fail(ORBFE_ERR_CAPACITY, "device matcher: a pair exceeded the candidate scratch budget (its nmatches is -1); "
                                         "use orbfe_search_by_projection_frames for that pair");
     }
@@ -1126,6 +1130,28 @@ extern "C" int orbfe_search_by_bow_device(OrbfeMatcher *m, int variant, int njob
     cudaStream_t s = stream ? (cudaStream_t)stream : m->stream;
     launch_search_by_bow(variant, njobs, d_kps, d_desc, d_counts, cap, d_fv_ids, d_fv_ptr, d_fv_items, d_fv_n, d_valid, d_idx1, d_idx2,
                          nnratio, check_orientation ? 1 : 0, d_out, d_nmatches, m->d_err, s);
+    CU_TRY(cudaGetLastError());
+    m->launches += 1;
+    return ORBFE_OK;
+}
+
+// SearchForTriangulation for `njobs` keyframe pairs, device-resident (include/orbfe_match.h).  Arguments are checked before
+// the handle is used.
+extern "C" int orbfe_search_for_triangulation_device(OrbfeMatcher *m, int njobs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
+                                                     const int *d_counts, int cap, const int32_t *d_fv_ids, const int32_t *d_fv_ptr,
+                                                     const int32_t *d_fv_items, const int *d_fv_n, const uint8_t *d_has_mp,
+                                                     const int *d_idx1, const int *d_idx2, const float *d_F12, const float *sigma2,
+                                                     int nlevels, int check_orientation, int32_t *d_match12, int *d_nmatches,
+                                                     void *stream) {
+    if (!m || njobs < 0 || cap < 1 || cap > 65535 || nlevels < 1 || nlevels > ORBFE_MAX_LEVELS) return fail(ORBFE_ERR_ARG, "bad arguments");
+    if (njobs == 0) return ORBFE_OK;
+    if (!d_kps || !d_desc || !d_counts || !d_fv_ids || !d_fv_ptr || !d_fv_items || !d_fv_n || !d_has_mp || !d_idx1 || !d_idx2 ||
+        !d_F12 || !sigma2 || !d_match12 || !d_nmatches)
+        return fail(ORBFE_ERR_ARG, "NULL argument");
+    CU_TRY(cudaSetDevice(m->device));
+    cudaStream_t s = stream ? (cudaStream_t)stream : m->stream;
+    launch_search_for_triangulation(njobs, d_kps, d_desc, d_counts, cap, d_fv_ids, d_fv_ptr, d_fv_items, d_fv_n, d_has_mp, d_idx1, d_idx2,
+                                    d_F12, sigma2, nlevels, check_orientation ? 1 : 0, d_match12, d_nmatches, m->d_err, s);
     CU_TRY(cudaGetLastError());
     m->launches += 1;
     return ORBFE_OK;

@@ -164,6 +164,13 @@ int launch_search_by_bow(int variant, int njobs, const OrbfeKeyPoint *kps, const
                          const int *idx1, const int *idx2, float nnratio, int check_ori, int *out, int *nmatches, int *err,
                          cudaStream_t s);
 
+// SearchForTriangulation for `njobs` (pKF1, pKF2) frame pairs (match_kernels.cu); sigma2 = nlevels floats on the host;
+// out-of-range FeatureVector entries or side-2 octaves set bit 4 of *err
+int launch_search_for_triangulation(int njobs, const OrbfeKeyPoint *kps, const uint8_t *desc, const int *counts, int cap,
+                                    const int *fv_ids, const int *fv_ptr, const int *fv_items, const int *fv_n, const uint8_t *has_mp,
+                                    const int *idx1, const int *idx2, const float *F12, const float *sigma2, int nlevels,
+                                    int check_ori, int *match12, int *nmatches, int *err, cudaStream_t s);
+
 void launch_undistort(float fx, float fy, float cx, float cy, const float *dist5, const OrbfeKeyPoint *d_in, OrbfeKeyPoint *d_out,
                       int n, cudaStream_t s);
 

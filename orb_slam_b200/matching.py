@@ -60,6 +60,8 @@ def _bind():
     L.orbfe_search_for_initialization.argtypes = [vp, vp, vp, vp, C.c_int, C.c_float, C.c_int, vp, vp]
     L.orbfe_search_by_bow_device.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, C.c_float, C.c_int,
                                              vp, vp, vp]
+    L.orbfe_search_for_triangulation_device.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int,
+                                                        C.c_int, vp, vp, vp]
     _bound = True
     return L
 
@@ -332,6 +334,20 @@ def search_for_triangulation(matcher: ORBmatcher, keys1, desc1, has_mp1, fv1, ke
                                             len(keys2), _p(keys2), _p(desc2), _p(has_mp2), len(i2), _p(i2), _p(p2), _p(t2),
                                             _p(F12), _p(sigma2), int(matcher.mbCheckOrientation), _p(out), C.byref(nm)))
     return nm.value, out[:len(keys1)]
+
+
+def search_for_triangulation_device(matcher: ORBmatcher, njobs, d_kps, d_desc, d_counts, cap, d_fv_ids, d_fv_ptr, d_fv_items, d_fv_n,
+                                    d_has_mp, d_idx1, d_idx2, d_F12, sigma2, d_match12, d_nmatches, stream=0):
+    """Device-pointer form (ints = raw device addresses) of SearchForTriangulation for `njobs` (pKF1, pKF2) frame pairs, with
+    the FeatureVectors in the layout of bow.feature_vector_device, d_F12 = njobs x 9 float32 and `sigma2` the per-level
+    KeyFrame::GetSigma2 values on the host; see include/orbfe_match.h.  Enqueued, not synchronised."""
+    L = _bind()
+    vp = C.c_void_p
+    sig = np.ascontiguousarray(sigma2, np.float32)
+    _check(L.orbfe_search_for_triangulation_device(matcher.handle, njobs, vp(d_kps), vp(d_desc), vp(d_counts), cap, vp(d_fv_ids),
+                                                   vp(d_fv_ptr), vp(d_fv_items), vp(d_fv_n), vp(d_has_mp), vp(d_idx1), vp(d_idx2),
+                                                   vp(d_F12), _p(sig), len(sig), int(matcher.mbCheckOrientation), vp(d_match12),
+                                                   vp(d_nmatches), vp(stream)))
 
 
 def guided_best(matcher: ORBmatcher, f, qu, qv, qr, qlo, qhi, qdesc, th_dist):

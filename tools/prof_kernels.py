@@ -6,11 +6,14 @@
   --what config5   BASELINE configs[4]: 2000 query descriptors x (ngroups keyframes x 2000 descriptors): the brute-force
                    best/second sweep (knn2 kernel), Gpairs/s, HBM GB/s, POPC-pipe estimate
   --what small     the latency-bound kernels once each (bow_descend, distinctive, undistort, hamming_csr, sbp single pair,
-                   feature_vector, search_by_bow) so that an `ncu -k regex:` capture finds them
+                   feature_vector, search_by_bow, search_for_triangulation) so that an `ncu -k regex:` capture finds them
   --what reloc     SearchByBoW at its two call sites, device-resident: relocalisation (one 1080p / 2000-keypoint frame against
                    32 candidate keyframes, KeyFrame-vs-Frame overload) and loop closing (one keyframe against 16 candidates,
                    KeyFrame-vs-KeyFrame); CUDA-event ms of the FeatureVector build and of the batched search, next to the wall
                    time of the same jobs through the per-pair host entry point orbfe_search_by_bow
+  --what mapping   SearchForTriangulation at LocalMapping::CreateNewMapPoints: one 1080p / 2000-keypoint keyframe against 20
+                   neighbours, F12 from the poses as ComputeF12; CUDA-event ms of the batched call next to the wall time of the
+                   same jobs through the per-pair host entry point orbfe_search_for_triangulation, and same_as_host
 
 Prints one JSON object per --what; never a bench value when run under ncu."""
 import argparse
@@ -199,6 +202,16 @@ def small(args):
         s.synchronize()
         m.sync()
         out["bow_device_matches"] = int(d_nm.item())
+        # search_for_triangulation_kernel: frame 0 against frame 1 (shifted by (5, -3): epipolar line y2 = y1 - 3)
+        d_F = t(np.array([[0, 0, 0, 0, 0, -1, 0, 1, 3]], np.float32))
+        d_mp = torch.zeros((2, cap), dtype=torch.uint8, device=dev)
+        sigma2 = (np.float32(1.2) ** np.arange(8, dtype=np.float32)) ** 2
+        M.search_for_triangulation_device(m, 1, d_k.data_ptr(), d_d.data_ptr(), d_c.data_ptr(), cap, d_ids.data_ptr(), d_ptr.data_ptr(),
+                                          d_items.data_ptr(), d_n.data_ptr(), d_mp.data_ptr(), d_i2.data_ptr(), d_i1.data_ptr(),
+                                          d_F.data_ptr(), sigma2, d_out.data_ptr(), d_nm.data_ptr(), s.cuda_stream)
+        s.synchronize()
+        m.sync()
+        out["triangulation_device_matches"] = int(d_nm.item())
         V.close()
     except Exception as e:
         out["bow"] = "skipped: %r" % e
@@ -281,6 +294,101 @@ def reloc(args):
         out[tag + "_host_per_pair_wall_ms"] = float(np.median(lat))
         out[tag + "_matches"] = int(dev_nm.sum())
         out[tag + "_same_as_host"] = bool(same)
+    V.close(); m.close()
+    return out
+
+
+def mapping(args):
+    """SearchForTriangulation at its call site, LocalMapping::CreateNewMapPoints (LocalMapping.cc:205-252): the new keyframe
+    against its 20 covisible neighbours, ORBmatcher(0.6, false).  The neighbours are sideways camera moves (R = I, t = (tx, 0,
+    0)) seen as horizontal image shifts, and F12 is computed from the poses as ComputeF12 does (LocalMapping.cc:452-469)."""
+    import torch
+    import orb_slam_b200 as fe
+    from orb_slam_b200 import matching as M, bow as BW
+    from orb_slam_b200.synth import textured_frame, shifted_frame, random_vocabulary
+    W, H, NF, levelsup, NKF = 1920, 1080, 2000, 4, 20
+    fx = fy = 1000.0
+    cx, cy = 960.0, 540.0
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    s = stream.cuda_stream
+    base = textured_frame(W, H, seed=23)
+    dxs = [0] + [(-1) ** i * (2 + i % 7) for i in range(1, NKF + 1)]   # never 0: every neighbour passes the baseline test
+    frames = np.stack([base] + [shifted_frame(base, dxs[i], 0, seed=i) for i in range(1, NKF + 1)])
+    F = len(frames)
+    ex = fe.ORBextractor(NF, 1.2, 8)
+    kps, desc, cnt = ex.extract_batch(frames)
+    ex.close()
+    voc = random_vocabulary(10, 6, seed=3)
+    V = BW.Vocabulary(voc)
+    has_mp = (np.random.default_rng(2).random((F, NF)) < 0.3).astype(np.uint8)
+    sigma2 = (np.float32(1.2) ** np.arange(8, dtype=np.float32)) ** 2
+    K = np.array([[fx, 0, cx], [0, fy, cy], [0, 0, 1]], np.float32)
+    Kinv = np.linalg.inv(K).astype(np.float32)
+    F12 = np.zeros((NKF, 9), np.float32)
+    for j in range(NKF):   # pKF1 = frame 0 at the origin, pKF2 = frame j + 1 with R2w = I, t2w = (dx / fx * depth, 0, 0), depth 5
+        t12 = -np.array([dxs[j + 1] / fx * 5.0, 0, 0], np.float32)   # -R1w R2w^T t2w + t1w
+        t12x = np.array([[0, -t12[2], t12[1]], [t12[2], 0, -t12[0]], [-t12[1], t12[0], 0]], np.float32)
+        F12[j] = (Kinv.T @ t12x @ np.eye(3, dtype=np.float32) @ Kinv).reshape(-1)
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    d_k, d_d, d_c, d_mp, d_F = t(kps.view(np.uint8).reshape(F, NF, 28)), t(desc), t(cnt), t(has_mp), t(F12)
+    d_leaf, d_node = (torch.zeros(F * NF, dtype=torch.int32, device=dev) for _ in range(2))
+    d_ids, d_items = (torch.zeros((F, NF), dtype=torch.int32, device=dev) for _ in range(2))
+    d_ptr, d_n = torch.zeros((F, NF + 1), dtype=torch.int32, device=dev), torch.zeros(F, dtype=torch.int32, device=dev)
+    V.descend_device(d_d.data_ptr(), F * NF, levelsup, d_leaf.data_ptr(), d_node.data_ptr(), s)
+    BW.feature_vector_device(V, F, d_leaf.data_ptr(), d_node.data_ptr(), d_c.data_ptr(), NF, d_ids.data_ptr(), d_ptr.data_ptr(),
+                             d_items.data_ptr(), d_n.data_ptr(), s)
+    stream.synchronize()
+    ids, ptr, items, nn = (x.cpu().numpy() for x in (d_ids, d_ptr, d_items, d_n))
+    fvs = [(ids[f, :nn[f]], ptr[f, :nn[f] + 1], items[f, :ptr[f, nn[f]]]) for f in range(F)]
+    jobs = [(0, f) for f in range(1, NKF + 1)]
+    j = np.array(jobs, np.int32)
+    d_i1, d_i2 = t(j[:, 0]), t(j[:, 1])
+    d_out = torch.zeros((NKF, NF), dtype=torch.int32, device=dev)
+    d_nm = torch.zeros(NKF, dtype=torch.int32, device=dev)
+    m = fe.ORBmatcher(0.6, False)   # LocalMapping.cc:210
+    call = lambda: M.search_for_triangulation_device(m, NKF, d_k.data_ptr(), d_d.data_ptr(), d_c.data_ptr(), NF, d_ids.data_ptr(),
+                                                     d_ptr.data_ptr(), d_items.data_ptr(), d_n.data_ptr(), d_mp.data_ptr(),
+                                                     d_i1.data_ptr(), d_i2.data_ptr(), d_F.data_ptr(), sigma2, d_out.data_ptr(),
+                                                     d_nm.data_ptr(), s)
+    for _ in range(args.warmup):
+        call()
+    stream.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    iters = args.iters * 4
+    e0.record(stream)
+    for _ in range(iters):
+        call()
+    e1.record(stream)
+    stream.synchronize()
+    m.sync()
+    out = {"what": "SearchForTriangulation device-resident, 1920x1080 keyframe, %d keypoints, against %d neighbours, vocabulary "
+                   "k=10 L=6, levelsup %d" % (NF, NKF, levelsup),
+           "counts_min": int(cnt.min()), "nodes_per_frame_mean": float(nn.mean()),
+           "mapping_%dkf_device_ms" % NKF: e0.elapsed_time(e1) / iters}
+    dev_out, dev_nm = d_out.cpu().numpy(), d_nm.cpu().numpy()
+    same = True
+    lat = []
+    for rep in range(3):
+        t0 = time.perf_counter()
+        for q, (f1, f2) in enumerate(jobs):
+            n1, n2 = cnt[f1], cnt[f2]
+            nm, o = M.search_for_triangulation(m, kps[f1, :n1], desc[f1, :n1], has_mp[f1, :n1], fvs[f1], kps[f2, :n2], desc[f2, :n2],
+                                               has_mp[f2, :n2], fvs[f2], F12[q], sigma2)
+            if rep == 0:
+                same = same and nm == dev_nm[q] and np.array_equal(o, dev_out[q, :len(o)])
+        lat.append((time.perf_counter() - t0) * 1e3)
+    out["mapping_%dkf_host_per_pair_wall_ms" % NKF] = float(np.median(lat))
+    out["mapping_%dkf_matches" % NKF] = int(dev_nm.sum())
+    out["same_as_host"] = bool(same)
+    try:
+        pr = torch.cuda.get_device_properties(0)
+        out["gpu"] = pr.name
+        import subprocess
+        out["power_limit"] = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                                            capture_output=True, text=True).stdout.strip()
+    except Exception as e:
+        out["gpu"] = "unknown: %r" % e
     V.close(); m.close()
     return out
 
@@ -572,4 +680,4 @@ if __name__ == "__main__":
     args = ap.parse_args()
     for w in args.what.split(","):
         print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fastarc": fastarc, "latency": latency,
-                          "reloc": reloc}[w](args)))
+                          "reloc": reloc, "mapping": mapping}[w](args)))
