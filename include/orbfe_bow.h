@@ -73,6 +73,28 @@ int orbfe_feature_vector_device(OrbfeVocabulary *v, int nframes, const int32_t *
  * All N x N distances and the medians are computed on the device (one warp per map point). */
 int orbfe_distinctive_descriptors(OrbfeMatcher *m, const uint8_t *desc, const int32_t *group_ptr, int ngroups, int32_t *best_out);
 
+/* orbfe_distinctive_descriptors with the descriptors read where they already live: the frame store d_desc / d_counts
+ * in the layout orbfe_extract_batch_device writes (frame f at f*cap, `nframes` frames).  Nothing passes through the host.
+ *   Group g (one map point) owns the observations d_obs[d_group_ptr[g] .. d_group_ptr[g+1]) (ngroups + 1 pointers,
+ *   `nobs` observations).  An observation is the flat slot f*cap + i (feature i of frame f, the index d_valid / d_has_mp
+ *   use), and a group lists them in the order of the reference's vDescriptors: mObservations iteration order, with the
+ *   observations in bad keyframes left out (MapPoint.cc:204-210).
+ *   d_best[g] = position inside the group of the descriptor with the least median distance to the group (median =
+ *   sorted[(int)(0.5*(N-1))], first minimum wins, MapPoint.cc:230-244); row g of d_mp_desc (ngroups x 32 bytes)
+ *   receives that descriptor -- MapPoint::mDescriptor, and the d_qdesc row orbfe_guided_search_device reads.
+ *   An empty group gets d_best[g] = -1 and its row is left untouched (the reference returns early and keeps mDescriptor);
+ *   pass a bad map point as an empty group or leave it out.
+ * Bad input is never followed: a group with d_group_ptr[g] < 0, d_group_ptr[g] > d_group_ptr[g+1],
+ * d_group_ptr[g+1] > nobs, or an observation whose frame is >= nframes or whose feature index is >= d_counts[f], gets
+ * d_best[g] = -1 with its row untouched, and orbfe_matcher_sync then reports ORBFE_ERR_ARG; the other groups of the launch
+ * are unaffected.  One warp per map point, N x N distances: a group of hundreds of observations takes longest.
+ * ngroups >= 0, nobs >= 0, 1 <= cap <= 65535, nframes >= 1, nframes*cap < 2^31; d_desc and d_mp_desc 16-byte aligned.
+ * Arguments are checked before the handle is used; ngroups == 0 does nothing.  Enqueued on `stream` (NULL = the
+ * matcher's stream), not synchronised. */
+int orbfe_distinctive_descriptors_device(OrbfeMatcher *m, int ngroups, const uint8_t *d_desc, const int *d_counts,
+                                         int nframes, int cap, const int32_t *d_group_ptr, const int32_t *d_obs, int nobs,
+                                         int32_t *d_best, uint8_t *d_mp_desc, void *stream);
+
 /* KeyFrameDatabase::DetectLoopCandidates (mode 0, KeyFrameDatabase.cc:73-195) / DetectRelocalisationCandidates (mode 1,
  * :197-308) with the database as arrays.  Keyframe k (k = 0..nkf-1, in the order the keyframes were add()ed: that is
  * the order inside every inverted-file list) owns the BowVector db_ids/db_vals[kf_ptr[k] .. kf_ptr[k+1]) (word ids

@@ -53,7 +53,7 @@ ABI_SYMBOLS = [
     "orbfe_rig_exchange_bytes",
     # include/orbfe_bow.h
     "orbfe_vocabulary_create", "orbfe_vocabulary_destroy", "orbfe_bow_descend_device", "orbfe_bow_descend", "orbfe_bow_transform",
-    "orbfe_distinctive_descriptors", "orbfe_bow_db_detect", "orbfe_feature_vector_device",
+    "orbfe_distinctive_descriptors", "orbfe_bow_db_detect", "orbfe_feature_vector_device", "orbfe_distinctive_descriptors_device",
 ]
 
 

@@ -30,6 +30,7 @@ def _bind():
     L.orbfe_distinctive_descriptors.argtypes = [vp, vp, vp, C.c_int, vp]
     L.orbfe_bow_db_detect.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, C.c_float, vp, vp, vp, vp]
     L.orbfe_feature_vector_device.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]
+    L.orbfe_distinctive_descriptors_device.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp]
     _bound = True
     return L
 
@@ -116,6 +117,16 @@ def distinctive_descriptors(matcher: ORBmatcher, desc, group_ptr):
     best = np.zeros(max(ng, 1), np.int32)
     _check(_bind().orbfe_distinctive_descriptors(matcher.handle, _p(desc), _p(group_ptr), ng, _p(best)))
     return best[:ng]
+
+
+def distinctive_descriptors_device(matcher: ORBmatcher, ngroups, d_desc, d_counts, nframes, cap, d_group_ptr, d_obs, nobs, d_best,
+                                   d_mp_desc, stream=0):
+    """Device-pointer form (ints = raw device addresses) on the frame store: group g owns the observation slots
+    d_obs[d_group_ptr[g] .. d_group_ptr[g+1]) (f*cap + i each); d_best[g] receives the chosen position inside the group and
+    row g of d_mp_desc (ngroups x 32 bytes) the chosen descriptor.  Enqueued, not synchronised; see include/orbfe_bow.h."""
+    vp = C.c_void_p
+    _check(_bind().orbfe_distinctive_descriptors_device(matcher.handle, ngroups, vp(d_desc), vp(d_counts), nframes, cap, vp(d_group_ptr),
+                                                        vp(d_obs), nobs, vp(d_best), vp(d_mp_desc), vp(stream)))
 
 
 def db_detect(matcher: ORBmatcher, mode, q_ids, q_vals, kf_ptr, db_ids, db_vals, connected, covis_ptr, covis, min_score=0.0):

@@ -57,26 +57,52 @@ __global__ void __launch_bounds__(256) bow_descend_kernel(const uint4 *__restric
 
 // One warp per map point.  Row i of the N x N distance matrix is histogrammed (257 bins) in shared memory and the
 // (int)(0.5*(N-1))-th smallest entry read off the cumulative counts; the first row with the least median wins.
+// kObs = false (orbfe_distinctive_descriptors): descriptor j of group g is row group_ptr[g] + j of `desc`, and the host
+// has checked group_ptr.  kObs = true (orbfe_distinctive_descriptors_device): it is row obs[group_ptr[g] + j] of the frame
+// store (slot f*cap + i); a group whose pointers or observations are out of range is never followed (best -1, its
+// mp_desc row untouched, bit 8 of *err), and the chosen 32 bytes are copied to row g of mp_desc.
+template <bool kObs>
 __global__ void __launch_bounds__(128) distinctive_kernel(const uint4 *__restrict__ desc, const int *__restrict__ group_ptr,
-                                                          int ngroups, int *__restrict__ best_out) {
+                                                          const int *__restrict__ obs, int nobs, const int *__restrict__ counts,
+                                                          int nframes, int cap, int ngroups, int *__restrict__ best_out,
+                                                          uint4 *__restrict__ mp_desc, int *__restrict__ err) {
     __shared__ int hist[4][288];
     const int wq = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int g = blockIdx.x * 4 + wq;
     if (g >= ngroups) return;
-    const int b = __ldg(&group_ptr[g]), N = __ldg(&group_ptr[g + 1]) - b;
+    const int b = __ldg(&group_ptr[g]), e = __ldg(&group_ptr[g + 1]);
+    if (kObs) {
+        bool bad = b < 0 || b > e || e > nobs;
+        if (!bad) {
+            bool mine = false;
+            for (int j = b + lane; j < e; j += 32) {
+                const int o = __ldg(&obs[j]);
+                mine |= o < 0 || o / cap >= nframes || o % cap >= __ldg(&counts[o / cap]);
+            }
+            bad = __any_sync(0xffffffffu, mine);
+        }
+        if (bad) {
+            if (lane == 0) { best_out[g] = -1; atomicOr(err, 8); }
+            return;
+        }
+    }
+    const int N = e - b;
     if (N <= 0) {
         if (lane == 0) best_out[g] = -1;
         return;
     }
+    auto row = [&](int j) -> size_t { return kObs ? (size_t)__ldg(&obs[b + j]) : (size_t)(b + j); };
     const int k = (N - 1) >> 1;  // vDists[0.5*(N-1)]
     int *h = hist[wq];
     int bestMedian = 0x7FFFFFFF, bestIdx = 0;
     for (int i = 0; i < N; i++) {
         for (int t = lane; t < 288; t += 32) h[t] = 0;
         __syncwarp();
-        const uint4 a0 = __ldg(&desc[2 * (size_t)(b + i)]), a1 = __ldg(&desc[2 * (size_t)(b + i) + 1]);
+        const size_t ri = row(i);
+        const uint4 a0 = __ldg(&desc[2 * ri]), a1 = __ldg(&desc[2 * ri + 1]);
         for (int j = lane; j < N; j += 32) {
-            const int d = bow_ham256(a0, a1, __ldg(&desc[2 * (size_t)(b + j)]), __ldg(&desc[2 * (size_t)(b + j) + 1]));
+            const size_t rj = row(j);
+            const int d = bow_ham256(a0, a1, __ldg(&desc[2 * rj]), __ldg(&desc[2 * rj + 1]));
             atomicAdd(&h[d], 1);
         }
         __syncwarp();
@@ -105,6 +131,7 @@ __global__ void __launch_bounds__(128) distinctive_kernel(const uint4 *__restric
         __syncwarp();
     }
     if (lane == 0) best_out[g] = bestIdx;
+    if (kObs && lane < 2) mp_desc[2 * (size_t)g + lane] = __ldg(&desc[2 * row(bestIdx) + lane]);
 }
 
 // KeyFrameDatabase scoring: one thread per keyframe, two-pointer walk over the (ascending) word lists of the query and
@@ -381,6 +408,15 @@ void vocab_modes(const OrbfeVocabulary *v, int *weighting, int *norm) { *weighti
 
 void launch_distinctive(const uint8_t *d_desc, const int *d_group_ptr, int ngroups, int *d_best, cudaStream_t s) {
     if (ngroups <= 0) return;
-    distinctive_kernel<<<(ngroups + 3) / 4, 128, 0, s>>>(reinterpret_cast<const uint4 *>(d_desc), d_group_ptr, ngroups, d_best);
+    distinctive_kernel<false><<<(ngroups + 3) / 4, 128, 0, s>>>(reinterpret_cast<const uint4 *>(d_desc), d_group_ptr, nullptr, 0,
+                                                                nullptr, 0, 1, ngroups, d_best, nullptr, nullptr);
+}
+
+void launch_distinctive_obs(const uint8_t *d_desc, const int *d_counts, int nframes, int cap, const int *d_group_ptr,
+                            const int *d_obs, int nobs, int ngroups, int *d_best, uint8_t *d_mp_desc, int *d_err, cudaStream_t s) {
+    if (ngroups <= 0) return;
+    distinctive_kernel<true><<<(ngroups + 3) / 4, 128, 0, s>>>(reinterpret_cast<const uint4 *>(d_desc), d_group_ptr, d_obs, nobs,
+                                                               d_counts, nframes, cap, ngroups, d_best,
+                                                               reinterpret_cast<uint4 *>(d_mp_desc), d_err);
 }
 }  // namespace orbfe

@@ -950,6 +950,9 @@ extern "C" int orbfe_matcher_sync(OrbfeMatcher *m) {
             return fail(ORBFE_ERR_ARG, "orbfe_search_for_triangulation_device: a job's FeatureVector has an out-of-range node row or "
                                        "feature index, or a side-2 feature without a map point has an octave outside [0, nlevels) "
                                        "(its nmatches is -1)");
+        if (flags & 8)
+            return fail(ORBFE_ERR_ARG, "orbfe_distinctive_descriptors_device: a group's pointers or an observation's frame or "
+                                       "feature index are out of range (its best index is -1)");
         return fail(ORBFE_ERR_CAPACITY, "device matcher: a pair exceeded the candidate scratch budget (its nmatches is -1); "
                                         "use orbfe_search_by_projection_frames for that pair");
     }
@@ -1277,7 +1280,12 @@ extern "C" int orbfe_image_bounds(OrbfeMatcher *m, int cols, int rows, float fx,
 
 // MapPoint::ComputeDistinctiveDescriptors for many map points in one launch (include/orbfe_bow.h)
 #include "../../include/orbfe_bow.h"
-namespace orbfe { void launch_distinctive(const uint8_t *d_desc, const int *d_group_ptr, int ngroups, int *d_best, cudaStream_t s); }
+namespace orbfe {
+void launch_distinctive(const uint8_t *d_desc, const int *d_group_ptr, int ngroups, int *d_best, cudaStream_t s);
+// bow_kernels.cu; an out-of-range group pointer or observation sets bit 8 of *d_err
+void launch_distinctive_obs(const uint8_t *d_desc, const int *d_counts, int nframes, int cap, const int *d_group_ptr,
+                            const int *d_obs, int nobs, int ngroups, int *d_best, uint8_t *d_mp_desc, int *d_err, cudaStream_t s);
+}
 extern "C" int orbfe_distinctive_descriptors(OrbfeMatcher *m, const uint8_t *desc, const int32_t *group_ptr, int ngroups,
                                              int32_t *best_out) {
     if (!m || ngroups < 0) return fail(ORBFE_ERR_ARG, "bad arguments");
@@ -1298,6 +1306,26 @@ extern "C" int orbfe_distinctive_descriptors(OrbfeMatcher *m, const uint8_t *des
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(best_out, m->buf[3], sizeof(int) * (size_t)ngroups, cudaMemcpyDeviceToHost, s));
     CU_TRY(cudaStreamSynchronize(s));
+    m->launches += 1;
+    return ORBFE_OK;
+}
+
+// The same on the frame store, every map point's descriptors addressed through its observation list
+// (include/orbfe_bow.h).  Arguments are checked before the handle is used.
+extern "C" int orbfe_distinctive_descriptors_device(OrbfeMatcher *m, int ngroups, const uint8_t *d_desc, const int *d_counts,
+                                                    int nframes, int cap, const int32_t *d_group_ptr, const int32_t *d_obs, int nobs,
+                                                    int32_t *d_best, uint8_t *d_mp_desc, void *stream) {
+    if (!m || ngroups < 0 || nobs < 0 || cap < 1 || cap > 65535 || nframes < 1 || (long long)nframes * cap > INT32_MAX)
+        return fail(ORBFE_ERR_ARG, "orbfe_distinctive_descriptors_device: bad arguments");
+    if (ngroups == 0) return ORBFE_OK;
+    if (!d_desc || !d_counts || !d_group_ptr || !d_obs || !d_best || !d_mp_desc)
+        return fail(ORBFE_ERR_ARG, "orbfe_distinctive_descriptors_device: NULL argument");
+    if (((uintptr_t)d_desc | (uintptr_t)d_mp_desc) % 16)
+        return fail(ORBFE_ERR_ARG, "orbfe_distinctive_descriptors_device: d_desc and d_mp_desc must be 16-byte aligned");
+    CU_TRY(cudaSetDevice(m->device));
+    cudaStream_t s = stream ? (cudaStream_t)stream : m->stream;
+    launch_distinctive_obs(d_desc, d_counts, nframes, cap, d_group_ptr, d_obs, nobs, ngroups, d_best, d_mp_desc, m->d_err, s);
+    CU_TRY(cudaGetLastError());
     m->launches += 1;
     return ORBFE_OK;
 }

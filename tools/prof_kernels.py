@@ -14,6 +14,11 @@
   --what mapping   SearchForTriangulation at LocalMapping::CreateNewMapPoints: one 1080p / 2000-keypoint keyframe against 20
                    neighbours, F12 from the poses as ComputeF12; CUDA-event ms of the batched call next to the wall time of the
                    same jobs through the per-pair host entry point orbfe_search_for_triangulation, and same_as_host
+  --what mapdesc   ComputeDistinctiveDescriptors at LocalMapping::ProcessNewKeyFrame: the 2000 map points of one 2000-feature
+                   keyframe over a 60-keyframe store (synthetic descriptors), with and without one 1000-observation point;
+                   CUDA-event ms of
+                   orbfe_distinctive_descriptors_device next to the wall time of orbfe_distinctive_descriptors including the
+                   host gather of the descriptors, and same_as_host
 
 Prints one JSON object per --what; never a bench value when run under ncu."""
 import argparse
@@ -212,6 +217,14 @@ def small(args):
         s.synchronize()
         m.sync()
         out["triangulation_device_matches"] = int(d_nm.item())
+        # distinctive_kernel<true>: the same groups as above, addressed through observation slots of frame 0
+        d_gp, d_obs = t(gp), t(np.arange(gp[-1], dtype=np.int32))
+        d_best, d_mpd = torch.zeros(len(gp) - 1, dtype=torch.int32, device=dev), torch.zeros((len(gp) - 1, 32), dtype=torch.uint8, device=dev)
+        BW.distinctive_descriptors_device(m, len(gp) - 1, d_d.data_ptr(), d_c.data_ptr(), 2, cap, d_gp.data_ptr(), d_obs.data_ptr(),
+                                          int(gp[-1]), d_best.data_ptr(), d_mpd.data_ptr(), s.cuda_stream)
+        s.synchronize()
+        m.sync()
+        out["distinctive_device_groups"] = int((d_best >= 0).sum().item())
         V.close()
     except Exception as e:
         out["bow"] = "skipped: %r" % e
@@ -381,15 +394,90 @@ def mapping(args):
     out["mapping_%dkf_host_per_pair_wall_ms" % NKF] = float(np.median(lat))
     out["mapping_%dkf_matches" % NKF] = int(dev_nm.sum())
     out["same_as_host"] = bool(same)
+    _gpu_and_power_limit(out)
+    V.close(); m.close()
+    return out
+
+
+def _gpu_and_power_limit(out):
     try:
-        pr = torch.cuda.get_device_properties(0)
-        out["gpu"] = pr.name
         import subprocess
+        import torch
+        out["gpu"] = torch.cuda.get_device_properties(0).name
         out["power_limit"] = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
                                             capture_output=True, text=True).stdout.strip()
     except Exception as e:
         out["gpu"] = "unknown: %r" % e
-    V.close(); m.close()
+
+
+def mapdesc(args):
+    """MapPoint::ComputeDistinctiveDescriptors at LocalMapping::ProcessNewKeyFrame (LocalMapping.cc:150): every feature of one
+    keyframe of 2000 features (the 1080p configuration's keypoint count) is a map point, observed in a store of 60 keyframes
+    of 2000 features.  Observation counts come from a fixed seeded distribution (95 % in 2-10, 5 % in 11-150); the "tail"
+    run adds one map point with 1000 observations.  The descriptors are synthetic: the observations of one point are noisy
+    copies of one random descriptor, every other row is random.  CUDA-event ms of
+    orbfe_distinctive_descriptors_device, next to the wall time of the same groups through orbfe_distinctive_descriptors
+    including the host gather of their descriptors from a host copy of the store, and same_as_host."""
+    import torch
+    import orb_slam_b200 as fe
+    from orb_slam_b200 import bow as BW
+    from orb_slam_b200.synth import noisy_copies, random_descriptors
+    NKF, NF = 60, 2000
+    rng = np.random.default_rng(13)
+    store = random_descriptors(NKF * NF, 13).reshape(NKF, NF, 32)
+    counts = np.full(NKF, NF, np.int32)
+    free = [list(rng.permutation(NF)) for _ in range(NKF)]   # frame 0: the new keyframe, its feature p is map point p
+    free[0] = []
+    n_obs = np.where(rng.random(NF) < 0.95, rng.integers(2, 11, NF), rng.integers(11, 151, NF))
+    groups = []
+    for p in range(NF + 1):
+        tail = p == NF
+        k = 1000 if tail else int(n_obs[p]) - 1   # observations outside the new keyframe
+        frames = np.sort(rng.choice(np.arange(1, NKF), k, replace=k > NKF - 1))
+        g = ([] if tail else [p]) + [int(f) * NF + int(free[f].pop()) for f in frames]   # mObservations order: by keyframe
+        base = random_descriptors(1, 50000 + p)
+        store.reshape(-1, 32)[g] = noisy_copies(np.repeat(base, len(g), axis=0), 0.12, 60000 + p)
+        groups.append(np.array(g, np.int32))
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    s = stream.cuda_stream
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    d_desc, d_cnt = t(store), t(counts)
+    m = fe.ORBmatcher(0.6, True)
+    out = {"what": "ComputeDistinctiveDescriptors device-resident: the %d map points of one keyframe over a %d-keyframe store of %d "
+                   "features" % (NF, NKF, NF)}
+    for tag, gs in (("kf", groups[:NF]), ("kf_tail1000", groups)):
+        ptr = np.concatenate([[0], np.cumsum([len(g) for g in gs])]).astype(np.int32)
+        obs = np.concatenate(gs).astype(np.int32)
+        ng = len(gs)
+        d_ptr, d_obs = t(ptr), t(obs)
+        d_best, d_mp = torch.zeros(ng, dtype=torch.int32, device=dev), torch.zeros((ng, 32), dtype=torch.uint8, device=dev)
+        call = lambda: BW.distinctive_descriptors_device(m, ng, d_desc.data_ptr(), d_cnt.data_ptr(), NKF, NF, d_ptr.data_ptr(),
+                                                         d_obs.data_ptr(), len(obs), d_best.data_ptr(), d_mp.data_ptr(), s)
+        for _ in range(args.warmup):
+            call()
+        stream.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        iters = args.iters * 4
+        e0.record(stream)
+        for _ in range(iters):
+            call()
+        e1.record(stream)
+        stream.synchronize()
+        m.sync()
+        out[tag + "_device_ms"] = e0.elapsed_time(e1) / iters
+        out[tag + "_groups"], out[tag + "_observations"], out[tag + "_max_group"] = ng, int(len(obs)), int(np.diff(ptr).max())
+        lat, best_h = [], None
+        flat = store.reshape(-1, 32)
+        for _ in range(5):
+            t0 = time.perf_counter()
+            best_h = BW.distinctive_descriptors(m, flat[obs], ptr)
+            lat.append((time.perf_counter() - t0) * 1e3)
+        out[tag + "_host_entry_with_gather_wall_ms"] = float(np.median(lat))
+        best = d_best.cpu().numpy()
+        out[tag + "_same_as_host"] = bool(np.array_equal(best, best_h) and np.array_equal(d_mp.cpu().numpy(), flat[obs[ptr[:-1] + best]]))
+    _gpu_and_power_limit(out)
+    m.close()
     return out
 
 
@@ -680,4 +768,4 @@ if __name__ == "__main__":
     args = ap.parse_args()
     for w in args.what.split(","):
         print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fastarc": fastarc, "latency": latency,
-                          "reloc": reloc, "mapping": mapping}[w](args)))
+                          "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc}[w](args)))
