@@ -64,7 +64,7 @@ def build_native(force=False, verbose=False):
     build_e2e_driver(force)
     if not force and not is_stale():
         return SO
-    extra = os.environ.get("ORBFE_NVCC_EXTRA", "").split()   # experiments, e.g. -DORBFE_FAST_MINBLOCKS=3
+    extra = os.environ.get("ORBFE_NVCC_EXTRA", "").split()   # experiments, e.g. -Xptxas -warn-spills
     cmd = [nvcc_path()] + NVCC_FLAGS + extra + (["-Xptxas", "-v"] if verbose else []) + \
           ["-o", SO] + [os.path.join(CSRC, s) for s in SOURCES]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)

@@ -2,12 +2,13 @@
 //
 // Stage map (reference src/ORBextractor.cc; canonical algorithm = SURVEY.md Appendix A):
 //   resize_level_kernel   ComputePyramid: cv::resize INTER_LINEAR u8 (:800), integer fixed point
-//   fast_nms_kernel       cv::FAST per cell (:599-614) as ONE threshold-free score map + windowed NMS
+//   fast_nms_tma_kernel   cv::FAST per cell (:599-614) as ONE threshold-free score map + windowed NMS
 //   cell_quota_kernel     per-cell quota redistribution (:622-670)
 //   cell_select_kernel    per-cell retainBest (:683-685) as an exact radix select on unique keys
 //   level_select_kernel   level-wide retainBest (:697-701) + canonical ordering
-//   blur7_kernel          cv::GaussianBlur 7x7 sigma 2 (:760), OpenCV-2.4 integer engine
-//   describe_kernel       IC_Angle (:124-151) + computeOrbDescriptor (:155-194) + output packing (:768-777)
+//   describe_fused_kernel cv::GaussianBlur 7x7 sigma 2 (:760) at the sampled positions only + IC_Angle (:124-151) +
+//                         computeOrbDescriptor (:155-194) + output packing (:768-777)
+//   blur7_kernel          the same Gaussian over a whole level (orbfe_debug_read_level only)
 //
 // All pixel arithmetic is integer; floats appear only in IC_Angle's atan2 polynomial, the BRIEF
 // rotation and the coordinate rescale, each written with explicit round-to-nearest intrinsics
@@ -198,62 +199,27 @@ void launch_resize_level(const PlanDev *d_plan, const PlanDev &hp, int level, in
 // 32 column groups of 4 px (x0-4 .. x0+123) x 64 rows (y0-1 .. y0+62): lane = column group, warp = 8-row
 // segment.  Each thread slides a 7-row register window down its 4-px column: per new row 3 LDS.32 + 10 PRMT
 // build the eight packed pixel pairs P_j = (b_j, b_{j+2}) as u16x2; every ring pixel of the two pixel pairs
-// A = (x, x+2) and B = (x+1, x+3) is then one of those registers, and the 16 arc minima / maxima are
-// VIMNMX3.U16x2 (two pixels per instruction, no divergence):
-//     t_k = min3(r_k, r_k+1, r_k+2) ; w_k = min3(t_k, t_k+3, t_k+6) = min of the 9-arc starting at k
-//     m   = max( max_k w_k - v , v - min_k W_k , 0 )          (W_k likewise with max3)
+// A = (x, x+2) and B = (x+1, x+3) is then one of those registers, and the arc network (fast_m_arc) evaluates
+//     m = max( max_k w_k - v , v - min_k W_k , 0 )    w_k / W_k = min / max of the 9-arc starting at k
+// for both pixels of a pair at once (two pixels per instruction, no divergence).
 #define F2_W ORBFE_FT_W            // 120
 #define F2_H ORBFE_FT_H            // 62
-#define F2_PW 144                  // staged pixel row stride (bytes): cols x0-8 .. x0+135
-#define F2_PWORDS 35               // words actually loaded per row (x0-8 .. x0+131)
 #define F2_PH (F2_H + 8)           // 70 staged rows: y0-4 .. y0+65
 #define F2_MS 128                  // m tile row stride (32 groups x 4)
-#ifndef ORBFE_FAST_ARC_DEFAULT
-#define ORBFE_FAST_ARC_DEFAULT 12   // arc-network variant of the non-TMA kernel (fast_m_arc): second form, 12 (min, max) pairs on the FMA pipe
-#endif
 #define F2_MH (F2_H + 2)           // 64 m rows
 static_assert(F2_MH == 64, "the m tile is 8 warps x 8 rows; row 64 does not exist (ti.hmask has 64 bits)");
+// TMA needs the innermost box coordinate 16-byte aligned (measured: a misaligned start traps as an illegal
+// instruction): the box starts at (x0-8) & ~15 and is 160 wide; the tile's own columns begin dx = (x0-8) & 15 in.
+#define F2_TW 160                  // staged pixel row stride (bytes)
 
-__device__ __forceinline__ uint32_t max16_u16x2(const uint32_t *w) {
-    const uint32_t a0 = __vimax3_u16x2(w[0], w[1], w[2]), a1 = __vimax3_u16x2(w[3], w[4], w[5]);
-    const uint32_t a2 = __vimax3_u16x2(w[6], w[7], w[8]), a3 = __vimax3_u16x2(w[9], w[10], w[11]);
-    const uint32_t a4 = __vimax3_u16x2(w[12], w[13], w[14]);
-    return __vmaxu2(__vimax3_u16x2(a0, a1, a2), __vimax3_u16x2(a3, a4, w[15]));
-}
-__device__ __forceinline__ uint32_t min16_u16x2(const uint32_t *w) {
-    const uint32_t a0 = __vimin3_u16x2(w[0], w[1], w[2]), a1 = __vimin3_u16x2(w[3], w[4], w[5]);
-    const uint32_t a2 = __vimin3_u16x2(w[6], w[7], w[8]), a3 = __vimin3_u16x2(w[9], w[10], w[11]);
-    const uint32_t a4 = __vimin3_u16x2(w[12], w[13], w[14]);
-    return __vminu2(__vimin3_u16x2(a0, a1, a2), __vimin3_u16x2(a3, a4, w[15]));
-}
-
-// r[16]: ring pixels (two pixels per register, values 0..255 in each 16-bit half), c: the two centres
-__device__ __forceinline__ uint32_t fast_m_u16x2(const uint32_t (&r)[16], uint32_t c) {
-    uint32_t tmin[16], tmax[16], w[16];
-#pragma unroll
-    for (int k = 0; k < 16; k++) {
-        tmin[k] = __vimin3_u16x2(r[k], r[(k + 1) & 15], r[(k + 2) & 15]);
-        tmax[k] = __vimax3_u16x2(r[k], r[(k + 1) & 15], r[(k + 2) & 15]);
-    }
-#pragma unroll
-    for (int k = 0; k < 16; k++) w[k] = __vimin3_u16x2(tmin[k], tmin[(k + 3) & 15], tmin[(k + 6) & 15]);
-    const uint32_t mb = max16_u16x2(w);  // brightest guaranteed level of some 9-arc
-#pragma unroll
-    for (int k = 0; k < 16; k++) w[k] = __vimax3_u16x2(tmax[k], tmax[(k + 3) & 15], tmax[(k + 6) & 15]);
-    const uint32_t md = min16_u16x2(w);  // darkest guaranteed level of some 9-arc
-    const uint32_t bright = __vmaxu2(mb, c) - c;  // per half >= 0: no borrow across halves
-    const uint32_t dark = c - __vminu2(md, c);
-    return __vmaxu2(bright, dark);
-}
-
-// ---- arc network, second form (default).  For even k the two 9-arcs starting at k and k+1 share the 8 ring pixels
+// ---- arc network.  For even k the two 9-arcs starting at k and k+1 share the 8 ring pixels
 // k+1 .. k+8; with c_k their minimum,  max(min(c_k, r_k), min(c_k, r_k+9)) = min(c_k, max(r_k, r_k+9)), so
 //     p_j  = min(r_2j+1, r_2j+2)              8 pair minima
 //     pp_j = min(p_j, p_j+1)                  8 quad minima  (r_2j+1 .. r_2j+4)
 //     e_i  = max(r_2i, r_2i+9)                8 arc-end maxima
 //     v_i  = min3(pp_i, pp_i+2, e_i)          the better of arcs 2i and 2i+1
 //     mb   = max(v_0 .. v_7, centre)          4 three-input maxima (the centre clamp rides in the tree)
-// and the dual for the dark arcs: 36 operations per polarity instead of 40.  NPAIR of the 16 (min, max) pairs
+// and the dual for the dark arcs: 36 operations per polarity instead of 40.  The 16 (min, max) pairs
 // (p_j / P_j and e_i / E_i take the minimum AND the maximum of the same two registers) are computed on the FMA pipe
 // instead of the integer ALU pipe the rest of the kernel saturates: pixel values 0..255 in a 16-bit half are fp16
 // subnormals, on which HFMA2 is exact, so  t = relu(a - b), min = a - t, max = b + t  is three FMA-pipe
@@ -279,26 +245,19 @@ __device__ __forceinline__ uint32_t hmul2(uint32_t a, uint32_t b) {
 __device__ __forceinline__ uint32_t hmax2_keep(uint32_t a, uint32_t b, uint32_t k, uint32_t nk) {
     return hfma2(b, k, hfma2_relu(b, nk, a));
 }
-// fma_pipe is a compile-time constant at every call site once the callers' loops are unrolled
-__device__ __forceinline__ void minmax_u16x2(bool fma_pipe, uint32_t a, uint32_t b, uint32_t &mn, uint32_t &mx) {
-    if (fma_pipe) {
-        const uint32_t NEG1 = 0xBC00BC00u, ONE = 0x3C003C00u;
-        const uint32_t t = hfma2_relu(b, NEG1, a);   // relu(a - b)
-        mn = hfma2(t, NEG1, a);                      // a - relu(a - b)
-        mx = hfma2(t, ONE, b);                       // b + relu(a - b)
-    } else {
-        mn = __vminu2(a, b);
-        mx = __vmaxu2(a, b);
-    }
+__device__ __forceinline__ void minmax_u16x2(uint32_t a, uint32_t b, uint32_t &mn, uint32_t &mx) {
+    const uint32_t NEG1 = 0xBC00BC00u, ONE = 0x3C003C00u;
+    const uint32_t t = hfma2_relu(b, NEG1, a);   // relu(a - b)
+    mn = hfma2(t, NEG1, a);                      // a - relu(a - b)
+    mx = hfma2(t, ONE, b);                       // b + relu(a - b)
 }
-template <int NPAIR>
-__device__ __forceinline__ uint32_t fast_m2_u16x2(const uint32_t (&r)[16], uint32_t c) {
+// r[16]: ring pixels (two pixels per register, values 0..255 in each 16-bit half), c: the two centres
+__device__ __forceinline__ uint32_t fast_m_arc(const uint32_t (&r)[16], uint32_t c) {
     uint32_t p[8], P[8], e[8], E[8];
 #pragma unroll
     for (int j = 0; j < 8; j++) {
-        // pairs are handed to the FMA pipe interleaved (p_0, e_0, p_1, e_1, ...) so that any NPAIR spreads over the network
-        minmax_u16x2(2 * j < NPAIR, r[2 * j + 1], r[(2 * j + 2) & 15], p[j], P[j]);
-        minmax_u16x2(2 * j + 1 < NPAIR, r[2 * j], r[(2 * j + 9) & 15], E[j], e[j]);
+        minmax_u16x2(r[2 * j + 1], r[(2 * j + 2) & 15], p[j], P[j]);
+        minmax_u16x2(r[2 * j], r[(2 * j + 9) & 15], E[j], e[j]);
     }
     uint32_t pp[8], PP[8];
 #pragma unroll
@@ -316,12 +275,6 @@ __device__ __forceinline__ uint32_t fast_m2_u16x2(const uint32_t (&r)[16], uint3
     const uint32_t mb = __vimax3_u16x2(__vimax3_u16x2(v[0], v[1], v[2]), __vimax3_u16x2(v[3], v[4], v[5]), __vimax3_u16x2(v[6], v[7], c));
     const uint32_t md = __vimin3_u16x2(__vimin3_u16x2(V[0], V[1], V[2]), __vimin3_u16x2(V[3], V[4], V[5]), __vimin3_u16x2(V[6], V[7], c));
     return __vmaxu2(mb - c, c - md);
-}
-// ARC < 0: the first form (16 triple minima + 16 nine-arc minima per polarity); ARC >= 0: the second form with ARC pairs on the FMA pipe
-template <int ARC>
-__device__ __forceinline__ uint32_t fast_m_arc(const uint32_t (&r)[16], uint32_t c) {
-    if (ARC < 0) return fast_m_u16x2(r, c);
-    return fast_m2_u16x2<(ARC < 0 ? 0 : ARC)>(r, c);
 }
 
 __device__ __forceinline__ void fast_load_row(const uint8_t *row /* smem, word aligned at the group's b0 */, uint32_t (&P)[8]) {
@@ -403,10 +356,9 @@ __device__ __forceinline__ void cell_window(const LevelDev &L, int xmax, int yma
 }
 
 // Everything after the pixel tile is staged: m map, NMS passes, candidate conversion and flush.
-// pix: staged pixel rows (stride F2_PW); mt: 16 KB m tile; s_cand: candidate list (F2_MAXC entries).
+// pix: staged pixel rows (stride F2_TW); mt: 16 KB m tile; s_cand: candidate list (F2_MAXC entries).
 // tile indexes wk.ftile_info; the tile's FTileInfo and level are re-read after the score loop, so that none of the geometry
 // the NMS and the flush need occupies registers while the 7-row window is live.
-template <int PSTRIDE, int ARC>
 __device__ __forceinline__ void fast_tile_compute(const PlanDev *__restrict__ plan, const WorkDev &wk, int tile, int level, int f, int x0, int y0, const uint8_t *pix, uint32_t *mt,
                                                   uint32_t *s_cand, int &s_n, int *s_cnt_lo, int *s_cnt_hi,
                                                   long long *s_kbase, int *s_klim) {
@@ -432,13 +384,13 @@ __device__ __forceinline__ void fast_tile_compute(const PlanDev *__restrict__ pl
             const int y = y0 - 1 + seg * 8 + i;
             if (y >= ORBFE_EDGE && y < ymax) yin_bits |= 1u << i;
         }
-        const uint8_t *base = &pix[(seg * 8) * PSTRIDE + 4 * g];  // b0 of the group = tile col 4g  (image x gx-4)
+        const uint8_t *base = &pix[(seg * 8) * F2_TW + 4 * g];  // b0 of the group = tile col 4g  (image x gx-4)
         uint32_t P[7][8];
 #pragma unroll
-        for (int r = 0; r < 6; r++) fast_load_row(base + r * PSTRIDE, P[r]);
+        for (int r = 0; r < 6; r++) fast_load_row(base + r * F2_TW, P[r]);
 #pragma unroll
         for (int i = 0; i < 8; i++) {
-            fast_load_row(base + (6 + i) * PSTRIDE, P[(6 + i) % 7]);
+            fast_load_row(base + (6 + i) * F2_TW, P[(6 + i) % 7]);
 #define FROW(dy) P[(i + (dy) + 3) % 7]
             // ring in circular order, (dx,dy): (0,3)(1,3)(2,2)(3,1)(3,0)(3,-1)(2,-2)(1,-3)(0,-3)(-1,-3)(-2,-2)(-3,-1)(-3,0)(-3,1)(-2,2)(-1,3)
             // pair A uses P_{4+dx} = index 3+dx ; pair B uses P_{5+dx} = index 4+dx
@@ -446,12 +398,12 @@ __device__ __forceinline__ void fast_tile_compute(const PlanDev *__restrict__ pl
             {
                 const uint32_t r[16] = {FROW(3)[3], FROW(3)[4], FROW(2)[5], FROW(1)[6], FROW(0)[6], FROW(-1)[6], FROW(-2)[5], FROW(-3)[4],
                                         FROW(-3)[3], FROW(-3)[2], FROW(-2)[1], FROW(-1)[0], FROW(0)[0], FROW(1)[0], FROW(2)[1], FROW(3)[2]};
-                mA = fast_m_arc<ARC>(r, FROW(0)[3]);
+                mA = fast_m_arc(r, FROW(0)[3]);
             }
             {
                 const uint32_t r[16] = {FROW(3)[4], FROW(3)[5], FROW(2)[6], FROW(1)[7], FROW(0)[7], FROW(-1)[7], FROW(-2)[6], FROW(-3)[5],
                                         FROW(-3)[4], FROW(-3)[3], FROW(-2)[2], FROW(-1)[1], FROW(0)[1], FROW(1)[1], FROW(2)[2], FROW(3)[3]};
-                mB = fast_m_arc<ARC>(r, FROW(0)[4]);
+                mB = fast_m_arc(r, FROW(0)[4]);
             }
 #undef FROW
             const int mr = seg * 8 + i;
@@ -603,43 +555,9 @@ __device__ __forceinline__ void fast_tile_compute(const PlanDev *__restrict__ pl
     }
 }
 
-__global__ void __launch_bounds__(256, 2) fast_nms_kernel(const PlanDev *__restrict__ plan, WorkDev wk, int f0) {
-    // one buffer, two lives: the staged pixel tile (until m is computed), then the candidate list
-    __shared__ __align__(16) uint8_t sbuf[(F2_MAXC * 4 > F2_PH * F2_PW) ? F2_MAXC * 4 : F2_PH * F2_PW];
-    __shared__ __align__(16) uint32_t mt[F2_MH * 32 * 2];  // 16 KB
-    __shared__ int s_n, s_cnt_lo[F2_MAXCELLS], s_cnt_hi[F2_MAXCELLS], s_klim[F2_MAXCELLS];
-    __shared__ long long s_kbase[F2_MAXCELLS];
-    uint8_t *pix = sbuf;
-    uint32_t *s_cand = reinterpret_cast<uint32_t *>(sbuf);
-
-    const int f = blockIdx.y + f0;
-    const FTileInfo ti = wk.ftile_info[blockIdx.x];
-    const LevelDev &L = plan->lv[ti.level];
-    const int x0 = ORBFE_EDGE + ti.tx * F2_W, y0 = ORBFE_EDGE + ti.ty * F2_H;
-    const int h = L.h, pitch = L.pitch;
-    const uint8_t *__restrict__ img = L.pyr + (size_t)f * L.plane;
-
-    if (threadIdx.x < F2_MAXCELLS) { s_cnt_lo[threadIdx.x] = 0; s_cnt_hi[threadIdx.x] = 0; }
-    if (threadIdx.x == 0) s_n = 0;
-    // ---- stage pixel rows y0-4 .. y0+65, cols x0-8 .. x0+131 (x0 is a multiple of 4) ----
-    {
-        const int max_word = pitch / 4 - 1;
-        const int wx0 = (x0 - 8) >> 2;
-        for (int i = threadIdx.x; i < F2_PH * F2_PWORDS; i += blockDim.x) {
-            const int r = i / F2_PWORDS, c = i - r * F2_PWORDS;
-            const int gy = min(y0 - 4 + r, h - 1);
-            const int gw = min(wx0 + c, max_word);
-            *reinterpret_cast<uint32_t *>(&pix[r * F2_PW + c * 4]) =
-                __ldg(reinterpret_cast<const uint32_t *>(img + (size_t)gy * pitch) + gw);
-        }
-    }
-    __syncthreads();
-    fast_tile_compute<F2_PW, ORBFE_FAST_ARC_DEFAULT>(plan, wk, blockIdx.x, ti.level, f, x0, y0, pix, mt, s_cand, s_n, s_cnt_lo, s_cnt_hi, s_kbase, s_klim);
-}
-
 // ------------------------------------------------------------------------------------------------
-// TMA variant (default): persistent CTAs, the pixel tile of work item i+1 is fetched by the Tensor
-// Memory Accelerator (cp.async.bulk.tensor.3d -> UTMALDG) into the second buffer while item i is
+// The FAST kernel: ORBFE_FAST_BLOCKS_PER_SM persistent CTAs per SM; the pixel tile of work item i+1 is fetched by the
+// Tensor Memory Accelerator (cp.async.bulk.tensor.3d -> UTMALDG) into the second buffer while item i is
 // being computed; completion is signalled on an mbarrier.  One 3-D tensor map (x, y, frame) per level;
 // out-of-image parts of the box are zero-filled by the hardware (they only feed masked m positions).
 // ------------------------------------------------------------------------------------------------
@@ -668,16 +586,12 @@ __device__ __forceinline__ void tma_load_3d(void *smem_dst, const void *tmap, ui
         ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
 
-// TMA needs the innermost box coordinate 16-byte aligned (measured: a misaligned start traps as an illegal
-// instruction): the box starts at (x0-8) & ~15 and is 160 wide; the tile's own columns begin dx = (x0-8) & 15 in.
-#define F2_TW 160
 #define F2_PIXBYTES (F2_PH * F2_TW)                       // 11200 = TMA box 160 x 70 x 1
 #define F2_PIXSLOT ((F2_PIXBYTES + 127) / 128 * 128)      // 11264
 #define F2_TMA_SMEM (2 * F2_PIXSLOT + F2_MH * 32 * 2 * 4 + 128)
 static_assert(F2_MAXC * 4 <= F2_PIXSLOT, "the candidate queue lives in the pixel slot that was just consumed");
 
-template <int ARC, int MINB>
-__global__ void __launch_bounds__(256, MINB) fast_nms_tma_kernel(const PlanDev *__restrict__ plan, WorkDev wk, int f0, int nwork) {
+__global__ void __launch_bounds__(256, ORBFE_FAST_BLOCKS_PER_SM) fast_nms_tma_kernel(const PlanDev *__restrict__ plan, WorkDev wk, int f0, int nwork) {
     extern __shared__ __align__(128) uint8_t dsm[];
     uint8_t *pixbuf0 = dsm, *pixbuf1 = dsm + F2_PIXSLOT;
     uint32_t *mt = reinterpret_cast<uint32_t *>(dsm + 2 * F2_PIXSLOT);
@@ -724,40 +638,20 @@ __global__ void __launch_bounds__(256, MINB) fast_nms_tma_kernel(const PlanDev *
         // the candidate queue reuses the current pixel slot (dead once m is computed; the next TMA into it is
         // only issued after the first barrier of the next item)
         uint8_t *slot_cur = cur ? pixbuf1 : pixbuf0;
-        fast_tile_compute<F2_TW, ARC>(plan, wk, wi % ntiles, ti.level, f, x0, y0, slot_cur + ((x0 - 8) & 15), mt, reinterpret_cast<uint32_t *>(slot_cur),
-                                 s_n, s_cnt_lo, s_cnt_hi, s_kbase, s_klim);
+        fast_tile_compute(plan, wk, wi % ntiles, ti.level, f, x0, y0, slot_cur + ((x0 - 8) & 15), mt, reinterpret_cast<uint32_t *>(slot_cur),
+                          s_n, s_cnt_lo, s_cnt_hi, s_kbase, s_klim);
     }
 }
 
-// arc-network variants compiled in (WorkDev::fast_arc; ORBFE_FAST_ARC=n picks one, see orbfe_api.cu)
-// (arc variant, resident CTAs per SM the register budget is sized for: 4 -> 64 registers, 3 -> 80)
-#define FAST_ARC_VARIANTS(X) X(-1, 4) X(0, 4) X(4, 4) X(8, 4) X(12, 4) X(16, 4) X(12, 3) X(16, 3)
-typedef void (*FastTmaKernel)(const PlanDev *, WorkDev, int, int);
-static FastTmaKernel fast_tma_variant(int arc, int minb) {
-#define X(a, b) if (arc == (a) && minb == (b)) return fast_nms_tma_kernel<(a), (b)>;
-    FAST_ARC_VARIANTS(X)
-#undef X
-    return nullptr;
-}
-int fast_arc_supported(int arc, int ctas_per_sm) { return fast_tma_variant(arc, ctas_per_sm <= 3 ? 3 : 4) != nullptr; }
-
 int fast_tma_setup() {
-#define X(a, b) { cudaError_t e = cudaFuncSetAttribute(fast_nms_tma_kernel<(a), (b)>, cudaFuncAttributeMaxDynamicSharedMemorySize, F2_TMA_SMEM); if (e != cudaSuccess) return (int)e; }
-    FAST_ARC_VARIANTS(X)
-#undef X
-    return 0;
+    return (int)cudaFuncSetAttribute(fast_nms_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, F2_TMA_SMEM);
 }
 
 void launch_fast_nms(const PlanDev *d_plan, const PlanDev &hp, WorkDev w, int f0, int nf, cudaStream_t s) {
     if (hp.nftiles_total == 0) return;  // every level has an empty cell grid: nothing to detect
-    if (w.tmaps) {
-        const int nwork = hp.nftiles_total * nf;
-        const int grid = min(nwork, w.fast_grid);
-        launch_k(fast_tma_variant(w.fast_arc, w.fast_ctas <= 3 ? 3 : 4), dim3(grid), dim3(256), F2_TMA_SMEM, s, hp.pdl != 0, d_plan, w, f0, nwork);
-        return;
-    }
-    dim3 grid(hp.nftiles_total, nf);
-    fast_nms_kernel<<<grid, 256, 0, s>>>(d_plan, w, f0);
+    const int nwork = hp.nftiles_total * nf;
+    const int grid = min(nwork, w.fast_grid);
+    launch_k(fast_nms_tma_kernel, dim3(grid), dim3(256), F2_TMA_SMEM, s, hp.pdl != 0, d_plan, w, f0, nwork);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1178,8 +1072,7 @@ __device__ __forceinline__ uint32_t blur_round_u8(int s) {
     return (uint32_t)min(q, 255);
 }
 
-__global__ void __launch_bounds__(256) blur7_kernel(const PlanDev *__restrict__ plan, const BTileInfo *__restrict__ btiles, int f0,
-                                                    int dst_f0) {
+__global__ void __launch_bounds__(256) blur7_kernel(const PlanDev *__restrict__ plan, const BTileInfo *__restrict__ btiles, int f0) {
     __shared__ __align__(16) uint8_t pix[B2_PH * B2_PS];
 
     const int f = blockIdx.y + f0;
@@ -1215,7 +1108,7 @@ __global__ void __launch_bounds__(256) blur7_kernel(const PlanDev *__restrict__ 
         A[r] = __byte_perm(wv, 0, 0x4240);
         B[r] = __byte_perm(wv, 0, 0x4341);
     }
-    uint8_t *__restrict__ dst = L.blur + (size_t)(blockIdx.y + dst_f0) * L.plane;
+    uint8_t *__restrict__ dst = L.blur + (size_t)blockIdx.y * L.plane;
     const int gx = x0 - 4 + 4 * g;
 #pragma unroll
     for (int i = 0; i < 8; i++) {
@@ -1245,10 +1138,10 @@ __global__ void __launch_bounds__(256) blur7_kernel(const PlanDev *__restrict__ 
     }
 }
 
-// smoothed planes of frames [f0, f0+nf) are written to plane slots [dst_f0, dst_f0+nf) of lv[].blur
-void launch_blur(const PlanDev *d_plan, const PlanDev &hp, WorkDev w, int f0, int nf, int dst_f0, cudaStream_t s) {
+// smoothed planes of frames [f0, f0+nf) are written to plane slots [0, nf) of lv[].blur (the plan allocates one slot)
+void launch_blur(const PlanDev *d_plan, const PlanDev &hp, WorkDev w, int f0, int nf, cudaStream_t s) {
     dim3 grid(hp.nbtiles_total, nf);
-    blur7_kernel<<<grid, 256, 0, s>>>(d_plan, w.btile_info, f0, dst_f0);
+    blur7_kernel<<<grid, 256, 0, s>>>(d_plan, w.btile_info, f0);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1278,109 +1171,15 @@ __device__ __forceinline__ float fast_atan2_deg(float y, float x) {
     return a;
 }
 
-__global__ void __launch_bounds__(256) describe_kernel(const PlanDev *__restrict__ plan, WorkDev wk,
-                                                       const int8_t *__restrict__ g_pattern,
-                                                       OrbfeKeyPoint *__restrict__ out_kps,
-                                                       uint8_t *__restrict__ out_desc, int *__restrict__ out_counts, int f0) {
-    __shared__ __align__(16) int8_t pat[1024];
-    for (int i = threadIdx.x; i < 256; i += blockDim.x)
-        reinterpret_cast<uint32_t *>(pat)[i] = __ldg(reinterpret_cast<const uint32_t *>(g_pattern) + i);
-    __syncthreads();
-
-    const int f = blockIdx.y + f0;
-    const int lane = threadIdx.x & 31;
-    const int slot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    const int nlev = plan->nlevels;
-    const int *__restrict__ lcnt = wk.level_cnt + (size_t)f * nlev;
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
-        int tot = 0;
-        for (int k = 0; k < nlev; k++) tot += lcnt[k];
-        out_counts[f] = tot;
-    }
-    if (slot >= plan->nfeatures) return;
-    const int l = find_level_by(plan, slot, 3);
-    const LevelDev &L = plan->lv[l];
-    const int idx = slot - L.kp_base;
-    if (idx >= lcnt[l]) return;
-    int out_idx = idx;
-    for (int k = 0; k < l; k++) out_idx += lcnt[k];
-
-    const int2 kp = wk.kp_xy_score[(size_t)f * plan->nfeatures + slot];
-    const int x = kp.x & 0xFFFF, y = kp.x >> 16;
-    const int w = L.w, h = L.h, pitch = L.pitch;
-    const uint8_t *__restrict__ img = L.pyr + (size_t)f * L.plane;
-    const uint8_t *__restrict__ blr = L.blur + (size_t)f * L.plane;
-
-    // ---- IC_Angle: lane <-> column u = lane-15, loop over rows v ----
-    int m10 = 0, m01 = 0;
-    {
-        const int u = lane - 15;
-        const int au = abs(u);
-        if (lane < 31) {
-            const uint8_t *c = img + (size_t)y * pitch + x + u;
-            // all 31 row loads are independent: issue them back to back (fully unrolled), then reduce
-            int colsum = 0;
-#pragma unroll
-            for (int v = -15; v <= 15; v++) {
-                const int val = (au <= c_umax[v < 0 ? -v : v]) ? (int)__ldg(c + (ptrdiff_t)v * pitch) : 0;
-                colsum += val;
-                m01 += v * val;
-            }
-            m10 = u * colsum;
-        }
-        m10 = warp_sum(m10);
-        m01 = warp_sum(m01);
-    }
-    const float angle = fast_atan2_deg((float)m01, (float)m10);
-
-    // ---- rotated BRIEF: lane <-> descriptor byte ----
-    const float factorPI = (float)(3.14159265358979323846 / 180.f);  // (float)(CV_PI/180.f)
-    const float th = __fmul_rn(angle, factorPI);
-    const float a = (float)cos((double)th), b = (float)sin((double)th);
-    int val = 0;
-    const int8_t *pp = pat + lane * 32;
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-        int t[2];
-#pragma unroll
-        for (int e = 0; e < 2; e++) {
-            const float px = (float)pp[4 * k + 2 * e], py = (float)pp[4 * k + 2 * e + 1];
-            const int ry = __float2int_rn(__fadd_rn(__fmul_rn(px, b), __fmul_rn(py, a)));
-            const int rx = __float2int_rn(__fsub_rn(__fmul_rn(px, a), __fmul_rn(py, b)));
-            const int sx = x + rx, sy = y + ry;
-            if (sx >= 0 && sx < w && sy >= 0 && sy < h) t[e] = __ldg(blr + (size_t)sy * pitch + sx);
-            else t[e] = __ldg(img + (size_t)reflect101(sy, h) * pitch + reflect101(sx, w));  // unblurred frame
-        }
-        val |= (t[0] < t[1]) << k;
-    }
-    // pack 4 lanes' bytes into a word; lanes 0,4,8,.. store
-    uint32_t word = (uint32_t)val;
-    word |= __shfl_down_sync(0xffffffffu, (uint32_t)val, 1) << 8;
-    word |= __shfl_down_sync(0xffffffffu, (uint32_t)val, 2) << 16;
-    word |= __shfl_down_sync(0xffffffffu, (uint32_t)val, 3) << 24;
-    const size_t o = (size_t)f * plan->nfeatures + out_idx;
-    if ((lane & 3) == 0) reinterpret_cast<uint32_t *>(out_desc + o * 32)[lane >> 2] = word;
-    if (lane == 0) {
-        OrbfeKeyPoint r;
-        r.x = l ? __fmul_rn((float)x, L.scale) : (float)x;  // :768-775
-        r.y = l ? __fmul_rn((float)y, L.scale) : (float)y;
-        r.size = L.patch_size;
-        r.angle = angle;
-        r.response = wk.cand_keys64 ? __int_as_float(kp.y) : (float)kp.y;  // Harris response or FAST score
-        r.octave = l;
-        r.class_id = -1;
-        out_kps[o] = r;
-    }
-}
-
 // ------------------------------------------------------------------------------------------------
-// Fused variant (the one the pipeline runs): the 7x7 Gaussian is evaluated only where a descriptor reads it.
+// The 7x7 Gaussian is evaluated only where a descriptor reads it.
 // A rotated BRIEF offset has |dx|,|dy| <= 18 (pattern radius 18.38), so every smoothed value a keypoint needs
 // comes from the raw 43x43 patch around it.  Per warp: stage the patch in shared memory (reflect-101 at the image
 // border, exactly the frame blur7_kernel stages), IC_Angle from the staged patch, vertical 7-tap of the 37 rows a
 // sample can fall on (4x4 byte transposes, then two IDP.4A per output; u16 results: 255*257 = 65535), then the
-// horizontal 7-tap (four IDP.2A on contiguous u16) + round-half-even only at the 512 sampled positions.  Integer arithmetic throughout: bit-identical to blur7_kernel + describe_kernel, without
-// writing and re-reading a blurred copy of the pyramid (2 x P bytes per frame) and ~6x fewer filter taps.
+// horizontal 7-tap (four IDP.2A on contiguous u16) + round-half-even only at the 512 sampled positions.  Integer
+// arithmetic throughout: each sample is bit-identical to the same pixel of a level smoothed by blur7_kernel, and no
+// blurred copy of the pyramid (2 x P bytes per frame) is written or re-read; ~6x fewer filter taps than a whole level.
 // ------------------------------------------------------------------------------------------------
 #define DF_R 21                 // patch radius: 18 (largest rotated offset) + 3 (filter taps)
 #define DF_ROWS (2 * DF_R + 1)  // 43
@@ -1670,13 +1469,6 @@ void launch_describe_fused(const PlanDev *d_plan, const PlanDev &hp, WorkDev w, 
     if (grid.x == 0) grid.x = 1;
     if (peers && peers->n > 0) { describe_fused_exchange_kernel<<<grid, 256, 0, s>>>(d_plan, w, d_pattern, f0, *peers); return; }
     launch_k(describe_fused_kernel, grid, dim3(256), 0, s, hp.pdl != 0, d_plan, w, d_pattern, d_kps, d_desc, d_counts, f0);
-}
-
-void launch_describe(const PlanDev *d_plan, const PlanDev &hp, WorkDev w, const int8_t *d_pattern,
-                     OrbfeKeyPoint *d_kps, uint8_t *d_desc, int *d_counts, int f0, int nf, cudaStream_t s) {
-    dim3 grid((hp.nfeatures + 7) / 8, nf);
-    if (grid.x == 0) grid.x = 1;
-    describe_kernel<<<grid, 256, 0, s>>>(d_plan, w, d_pattern, d_kps, d_desc, d_counts, f0);
 }
 
 }  // namespace orbfe

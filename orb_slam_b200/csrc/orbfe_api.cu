@@ -81,7 +81,6 @@ struct StageTimer {
 struct OrbfeExtractor {
     int nfeatures = 0, nlevels = 0, score_type = 1, fast_th = 20, device = 0;
     int batch_mode = 0;         // orbfe_extractor_set_batch_mode
-    bool blur_planes = false;   // ORBFE_BLUR_PLANES=1: unfused blur7 + describe (smoothed copies of every level kept in HBM)
     double scale_factor = 1.2;  // double member initialised from a float (ORBextractor.h:62, .cc:459)
     float scale[ORBFE_MAX_LEVELS], inv_scale[ORBFE_MAX_LEVELS];
     int quota[ORBFE_MAX_LEVELS];
@@ -277,7 +276,7 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
     for (int l = 0; l < ex->nlevels; l++) {
         LevelDev &L = P.lv[l];
         CU_TRY(dmalloc(ex, &L.pyr, L.plane * B + 256));
-        CU_TRY(dmalloc(ex, &L.blur, L.plane * (ex->blur_planes ? B : 1) + 256));  // fused describe: one debug plane only
+        CU_TRY(dmalloc(ex, &L.blur, L.plane + 256));  // one plane, for orbfe_debug_read_level
         CU_TRY(cudaMemsetAsync(L.pyr, 0, L.plane * B + 256, ex->stream));
         if (l > 0) {
             const LevelDev &S = P.lv[l - 1];
@@ -369,14 +368,7 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
     Wk.cell_cand_base = d_cb;
     Wk.cell_cand_cap = d_cc;
     // ---- TMA tensor maps (one per level: x, y, frame) for the FAST kernel's pixel tiles ----
-    Wk.tmaps = nullptr;
-    Wk.fast_grid = 0;
-    Wk.fast_arc = ORBFE_FAST_ARC_RUNTIME_DEFAULT;
-    Wk.fast_ctas = getenv("ORBFE_FAST_CTAS") ? std::max(1, atoi(getenv("ORBFE_FAST_CTAS"))) : 3;  // 3 CTAs x 80 registers (no spills; default), or 4 x 64
-    if (const char *a = getenv("ORBFE_FAST_ARC")) Wk.fast_arc = atoi(a);
-    if (!fast_arc_supported(Wk.fast_arc, Wk.fast_ctas))
-        return fail(ORBFE_ERR_ARG, "ORBFE_FAST_ARC=%d with ORBFE_FAST_CTAS=%d is not a compiled variant of the FAST kernel", Wk.fast_arc, Wk.fast_ctas);
-    if (!getenv("ORBFE_FAST_NO_TMA")) {
+    {
         typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                                      const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
                                      CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -407,7 +399,7 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
         if (e != cudaSuccess) return fail(ORBFE_ERR_CUDA, "cudaFuncSetAttribute(fast_nms_tma_kernel): %s", cudaGetErrorString(e));
         int nsm = 132;
         cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, ex->device);
-        Wk.fast_grid = Wk.fast_ctas * nsm;  // resident persistent CTAs (39 KB smem each)
+        Wk.fast_grid = ORBFE_FAST_BLOCKS_PER_SM * nsm;  // resident persistent CTAs (39 KB smem each)
     }
     CU_TRY(dmalloc(ex, &Wk.cand_keys, (size_t)cand_total * B));
     if (ex->score_type == 0) {
@@ -509,7 +501,6 @@ extern "C" int orbfe_extractor_create(int nfeatures, float scale_factor, int nle
     ex->score_type = score_type;
     ex->fast_th = fast_th;
     ex->device = device;
-    ex->blur_planes = getenv("ORBFE_BLUR_PLANES") != nullptr;
     ex->scale_factor = (double)scale_factor;
     const double sf = ex->scale_factor;
     // mvScaleFactor / mvInvScaleFactor, :461-471
@@ -611,14 +602,7 @@ static int enqueue_pipeline(OrbfeExtractor *ex, int f0, int nf, OrbfeKeyPoint *d
     stage_mark(ex, s, "cell_select");
     launch_level_select(ex->dplan, hp, ex->work, ex->ls_smem, f0, nf, s); launches++;
     stage_mark(ex, s, "level_select");
-    if (ex->blur_planes) {
-        // unfused variant (ORBFE_BLUR_PLANES=1): smooth whole levels, then describe from the smoothed planes
-        launch_blur(ex->dplan, hp, ex->work, f0, nf, f0, s); launches++;
-        stage_mark(ex, s, "blur7");
-        launch_describe(ex->dplan, hp, ex->work, ex->d_pattern, d_kps, d_desc, d_counts, f0, nf, s); launches++;
-    } else {
-        launch_describe_fused(ex->dplan, hp, ex->work, ex->d_pattern, d_kps, d_desc, d_counts, f0, nf, s, peers); launches++;
-    }
+    launch_describe_fused(ex->dplan, hp, ex->work, ex->d_pattern, d_kps, d_desc, d_counts, f0, nf, s, peers); launches++;
     stage_mark(ex, s, "describe");
     CU_TRY(cudaGetLastError());
     ex->last_launches += launches;
@@ -674,7 +658,6 @@ int orbfe_extract_batch_device_peers(OrbfeExtractor *ex, const uint8_t *d_imgs, 
                                      int batch, const PeerOut &po, int cap, void *stream) {
     if (!ex || !d_imgs) return fail(ORBFE_ERR_ARG, "NULL argument");
     if (width <= 0 || height <= 0 || batch <= 0 || stride < (size_t)width) return fail(ORBFE_ERR_ARG, "bad geometry");
-    if (ex->blur_planes) return fail(ORBFE_ERR_UNSUPPORTED, "the fused exchange needs the fused descriptor kernel (ORBFE_BLUR_PLANES is set)");
     CU_TRY(cudaSetDevice(ex->device));
     int rc = build_plan(ex, width, height, batch);
     if (rc) return rc;
@@ -829,10 +812,10 @@ extern "C" int orbfe_debug_read_level(OrbfeExtractor *ex, int frame, int level, 
         return fail(ORBFE_ERR_ARG, "bad arguments");
     CU_TRY(cudaSetDevice(ex->device));
     const LevelDev &L = ex->hplan.lv[level];
-    const uint8_t *src = which ? L.blur + (ex->blur_planes ? (size_t)frame * L.plane : 0) : L.pyr + (size_t)frame * L.plane;
-    if (which && !ex->blur_planes) {
+    const uint8_t *src = which ? L.blur : L.pyr + (size_t)frame * L.plane;
+    if (which) {
         // the pipeline smooths only descriptor patches; materialise the smoothed level of this frame on demand
-        launch_blur(ex->dplan, ex->hplan, ex->work, frame, 1, 0, ex->stream);
+        launch_blur(ex->dplan, ex->hplan, ex->work, frame, 1, ex->stream);
         CU_TRY(cudaGetLastError());
     }
     CU_TRY(cudaStreamSynchronize(ex->stream));

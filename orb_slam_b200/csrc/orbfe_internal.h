@@ -13,7 +13,9 @@
 // FAST/NMS tile (detect-area pixels per CTA) and blur tile
 #define ORBFE_FT_W 120
 #define ORBFE_FT_H 62
-#define ORBFE_FAST_ARC_RUNTIME_DEFAULT 16  // WorkDev::fast_arc unless ORBFE_FAST_ARC overrides it (measured best with 3 CTAs x 80 registers per SM)
+// resident persistent CTAs per SM of the FAST kernel: its register budget (80) and its grid (this x SMs).  3 x 80
+// measured faster on H100 than 4 x 64, which spills (DESIGN.md §4.2).
+#define ORBFE_FAST_BLOCKS_PER_SM 3
 #define ORBFE_BT_W 120
 #define ORBFE_BT_H 64
 
@@ -24,7 +26,7 @@ namespace orbfe {
 // TMA-/vector-aligned).
 struct LevelDev {
     uint8_t *pyr;   // unblurred level (level 0 = the input image)
-    uint8_t *blur;  // 7x7 Gaussian of the level (interior only; descriptor sampling outside reads pyr by reflection)
+    uint8_t *blur;  // one plane: 7x7 Gaussian of one frame's level, for orbfe_debug_read_level (the descriptor kernel smooths its own patches)
     size_t plane;   // pitch * h
     int w, h, pitch;
     // cell grid (reference ORBextractor.cc:527-547); detect windows tile [16, w-16) x [16, h-16)
@@ -72,10 +74,8 @@ struct WorkDev {
     const int *cell_cand_cap;         // [ncells_total]
     const FTileInfo *ftile_info;      // [nftiles_total]
     const BTileInfo *btile_info;      // [nbtiles_total]
-    const CUtensorMap *tmaps;         // [nlevels] 3-D (x, y, frame) tensor maps of the unblurred levels; NULL = no TMA
-    int fast_grid;                    // persistent CTAs of the TMA FAST kernel
-    int fast_ctas;                    // resident persistent CTAs per SM (fast_grid = fast_ctas x SMs)
-    int fast_arc;                     // arc-network variant of the TMA FAST kernel (extract_kernels.cu, fast_m_arc)
+    const CUtensorMap *tmaps;         // [nlevels] 3-D (x, y, frame) tensor maps of the unblurred levels; never NULL (build_plan fails without TMA)
+    int fast_grid;                    // persistent CTAs of the FAST kernel (ORBFE_FAST_BLOCKS_PER_SM x SMs)
     uint32_t *cand_keys;              // [batch][cand_total]   (score<<24 | 0xFFFFFF - raster)
     unsigned long long *cand_keys64;  // HARRIS_SCORE only: order(resp)<<32 | (0xFFFFFF - raster)<<8 | score; NULL otherwise
     uint32_t *kept_aux;               // HARRIS_SCORE only: low raster bits + score of each kept entry
@@ -113,13 +113,10 @@ void launch_fast_nms(const PlanDev *d_plan, const PlanDev &h_plan, WorkDev w, in
 void launch_cell_quota(const PlanDev *d_plan, const PlanDev &h_plan, WorkDev w, int f0, int nf, cudaStream_t s);
 void launch_cell_select(const PlanDev *d_plan, const PlanDev &h_plan, WorkDev w, int f0, int nf, cudaStream_t s);
 void launch_level_select(const PlanDev *d_plan, const PlanDev &h_plan, WorkDev w, size_t smem_bytes, int f0, int nf, cudaStream_t s);
-void launch_blur(const PlanDev *d_plan, const PlanDev &h_plan, WorkDev w, int f0, int nf, int dst_f0, cudaStream_t s);
-void launch_describe(const PlanDev *d_plan, const PlanDev &h_plan, WorkDev w, const int8_t *d_pattern,
-                     OrbfeKeyPoint *d_kps, uint8_t *d_desc, int *d_counts, int f0, int nf, cudaStream_t s);
+void launch_blur(const PlanDev *d_plan, const PlanDev &h_plan, WorkDev w, int f0, int nf, cudaStream_t s);
 void launch_describe_fused(const PlanDev *d_plan, const PlanDev &h_plan, WorkDev w, const int8_t *d_pattern,
                      OrbfeKeyPoint *d_kps, uint8_t *d_desc, int *d_counts, int f0, int nf, cudaStream_t s, const PeerOut *peers = nullptr);
 int fast_tma_setup();
-int fast_arc_supported(int arc, int ctas_per_sm);
 int level_select_smem_bytes(int max_kept);
 int level_select_harris_smem_bytes(int max_kept);
 int set_level_select_harris_smem(int bytes);

@@ -660,9 +660,9 @@ def h2d(args):
     return out
 
 
-def fastarc(args):
+def fast(args):
     """BASELINE configs[1] geometry (1920x1080, 2000 kp, 8 levels), 64-frame device-resident batches: per-stage CUDA-event
-    times for every compiled FAST arc-network variant (ORBFE_FAST_ARC is read when the extractor plans a geometry)."""
+    times of the extractor, the FAST kernel's stage included."""
     import torch
     import orb_slam_b200 as fe
     from orb_slam_b200.synth import textured_frame, shifted_frame
@@ -675,39 +675,24 @@ def fastarc(args):
     d_desc = torch.empty((B, NF, 32), dtype=torch.uint8, device=dev)
     d_cnt = torch.empty((B,), dtype=torch.int32, device=dev)
     stream = torch.cuda.Stream(device=dev)
-    out = {"what": "FAST arc-network variants, 1080p x 64 frames, ms per batch"}
-    ref = None
-    # "arc" or "arc:ctas" (ctas = resident CTAs per SM, 4 x 64 registers or 3 x 80)
-    variants = [v for v in os.environ.get("FASTARC_VARIANTS", "-1,0,4,8,12,16,12:3,16:3").split(",")]
+    out = {"what": "FAST kernel, 1080p x 64 frames, ms per batch"}
+    ex = fe.ORBextractor(NF, 1.2, NL, fe.FAST_SCORE, 20)
+    ex.set_profiling(True)
+    for _ in range(3):
+        ex.extract_batch_device(d_frames.data_ptr(), W, H, W, W * H, B, d_kps.data_ptr(), d_desc.data_ptr(), d_cnt.data_ptr(), stream.cuda_stream)
+    stream.synchronize()
+    ex.stage_times()
+    n = 10
     for rep in range(2):
-        for var in variants:
-            arc, _, ctas = var.partition(":")
-            arc = int(arc)
-            os.environ["ORBFE_FAST_ARC"] = str(arc)
-            if ctas:
-                os.environ["ORBFE_FAST_CTAS"] = ctas
-            else:
-                os.environ.pop("ORBFE_FAST_CTAS", None)
-            ex = fe.ORBextractor(NF, 1.2, NL, fe.FAST_SCORE, 20)
-            ex.set_profiling(True)
-            for _ in range(3):
-                ex.extract_batch_device(d_frames.data_ptr(), W, H, W, W * H, B, d_kps.data_ptr(), d_desc.data_ptr(), d_cnt.data_ptr(), stream.cuda_stream)
-            stream.synchronize()
-            ex.stage_times()
-            n = 10
-            for _ in range(n):
-                ex.extract_batch_device(d_frames.data_ptr(), W, H, W, W * H, B, d_kps.data_ptr(), d_desc.data_ptr(), d_cnt.data_ptr(), stream.cuda_stream)
-            stream.synchronize()
-            acc = {}
-            for name, ms in ex.stage_times():
-                acc[name] = acc.get(name, 0.0) + ms / n
-            sig = (d_kps.cpu().numpy().tobytes(), d_desc.cpu().numpy().tobytes())
-            if ref is None:
-                ref = sig
-            out["arc%s_rep%d" % (var, rep)] = {"fast_nms": round(acc.get("fast_nms", -1), 4), "all": round(sum(acc.values()), 4), "same_bits": sig == ref}
-            ex.close()
-    os.environ.pop("ORBFE_FAST_ARC", None)
-    os.environ.pop("ORBFE_FAST_CTAS", None)
+        for _ in range(n):
+            ex.extract_batch_device(d_frames.data_ptr(), W, H, W, W * H, B, d_kps.data_ptr(), d_desc.data_ptr(), d_cnt.data_ptr(), stream.cuda_stream)
+        stream.synchronize()
+        acc = {}
+        for name, ms in ex.stage_times():
+            acc[name] = acc.get(name, 0.0) + ms / n
+        out["rep%d" % rep] = {"fast_nms": round(acc.get("fast_nms", -1), 4), "all": round(sum(acc.values()), 4),
+                              "stages": {k: round(v, 4) for k, v in acc.items()}}
+    ex.close()
     return out
 
 
@@ -767,5 +752,5 @@ if __name__ == "__main__":
     ap.add_argument("--warmup", type=int, default=2)
     args = ap.parse_args()
     for w in args.what.split(","):
-        print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fastarc": fastarc, "latency": latency,
+        print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fast": fast, "latency": latency,
                           "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc}[w](args)))
