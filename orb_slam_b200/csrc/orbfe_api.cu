@@ -166,9 +166,13 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
     P.nlevels = ex->nlevels;
     P.batch = B;
     P.nfeatures = ex->nfeatures;
-    P.t_lo = std::min(ex->fast_th, 7);
-    P.t_hi = std::max(ex->fast_th, 7);
-    P.t1_is_lo = ex->fast_th <= 7;
+    // cv::FAST keeps a pixel only if its score is strictly above all 8 neighbours', and a non-corner scores 0: a corner of
+    // score 0 (a pixel that is a corner at threshold 0 only) is never kept and suppresses nothing.  Threshold 0 therefore
+    // detects exactly what threshold 1 detects; the kernel, whose NMS input is m - t_lo, runs it as 1.
+    const int th = std::max(ex->fast_th, 1);
+    P.t_lo = std::min(th, 7);
+    P.t_hi = std::max(th, 7);
+    P.t1_is_lo = th <= 7;
     P.score_type = ex->score_type;
     {   // programmatic dependent launch of the pipeline's kernels (extract_kernels.cu, pdl_prologue); ORBFE_PDL=0 turns it off
         const char *e = getenv("ORBFE_PDL");

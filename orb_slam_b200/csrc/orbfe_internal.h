@@ -50,7 +50,7 @@ struct LevelDev {
 struct PlanDev {
     int nlevels, batch, nfeatures;
     int ncells_total, nftiles_total, nbtiles_total, kept_total;
-    int t_lo, t_hi;      // min / max of (fastTh, 7)
+    int t_lo, t_hi;      // min / max of (max(fastTh, 1), 7): threshold 0 detects what 1 does (build_plan)
     int t1_is_lo;        // fastTh <= 7
     int score_type;
     int pdl;             // host side only: launch the pipeline's kernels with programmatic stream serialization (ORBFE_PDL, default 1)
