@@ -61,21 +61,22 @@ void launch_hamming_csr(const uint8_t *q, const uint8_t *t, const int32_t *row_p
                                                     row_ptr, cols, nq, out);
 }
 
-// Dense nq x nt matrix: blockIdx.y = query, threads stride over train descriptors.
+// Dense nq x nt matrix: blockIdx.y strides over queries (grid.y is capped at 65535), threads stride over train descriptors.
 __global__ void __launch_bounds__(256) hamming_dense_kernel(const uint4 *__restrict__ q, int nq,
                                                             const uint4 *__restrict__ t, int nt,
                                                             uint16_t *__restrict__ out) {
-    const int i = blockIdx.y;
-    const uint4 a0 = __ldg(&q[2 * i]), a1 = __ldg(&q[2 * i + 1]);
-    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < nt; j += gridDim.x * blockDim.x) {
-        const uint4 b0 = __ldg(&t[2 * j]), b1 = __ldg(&t[2 * j + 1]);
-        out[(size_t)i * nt + j] = (uint16_t)ham256(a0, a1, b0, b1);
+    for (int i = blockIdx.y; i < nq; i += gridDim.y) {
+        const uint4 a0 = __ldg(&q[2 * i]), a1 = __ldg(&q[2 * i + 1]);
+        for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < nt; j += gridDim.x * blockDim.x) {
+            const uint4 b0 = __ldg(&t[2 * j]), b1 = __ldg(&t[2 * j + 1]);
+            out[(size_t)i * nt + j] = (uint16_t)ham256(a0, a1, b0, b1);
+        }
     }
 }
 
 void launch_hamming_dense(const uint8_t *q, int nq, const uint8_t *t, int nt, uint16_t *out, cudaStream_t s) {
     if (nq <= 0 || nt <= 0) return;
-    dim3 grid(min((nt + 255) / 256, 64), nq);
+    dim3 grid(min((nt + 255) / 256, 64), min(nq, 65535));
     hamming_dense_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<const uint4 *>(q), nq, reinterpret_cast<const uint4 *>(t), nt, out);
 }
 
