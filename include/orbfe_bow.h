@@ -112,6 +112,58 @@ int orbfe_bow_db_detect(OrbfeMatcher *m, int mode, int nq, const int32_t *q_ids,
                         const int32_t *covis_ptr, const int32_t *covis, float min_score, int *ncand_out, int32_t *cand_out,
                         int32_t *common_out, float *score_out);
 
+/* KeyFrameDatabase (reference src/KeyFrameDatabase.cc) as a long-lived object resident in device memory: the inverted file,
+ * the keyframes' BowVectors, their best-covisibility lists and their query fields (mnLoopQuery, mnLoopWords, mLoopScore,
+ * mnRelocQuery, mnRelocWords, mRelocScore; KeyFrame.h:160-165) live on the device, so a query costs the postings of its
+ * words and its results equal the reference's over any sequence of calls (mRelocScore of a keyframe that shares too few
+ * words with this frame is the one an earlier query left, :272-281).  A keyframe is a caller-chosen slot
+ * 0 <= slot < max_keyframes (e.g. its frame-store index, so candidates go straight to orbfe_search_by_bow_device as d_idx).
+ * Arguments are checked before the handle is used.  One call at a time per handle (the reference serialises these calls
+ * with mMutex); every call is ordered after the handle's previous work whatever stream that was enqueued on. */
+typedef struct OrbfeKeyFrameDB OrbfeKeyFrameDB;
+
+/* KeyFrameDatabase(voc) (:32-36).  Word ids are checked against the vocabulary's word count (largest word id + 1); the
+ * device is the vocabulary's.  Every buffer is allocated here (about 44 bytes per posting, 8 per vocabulary word and
+ * 150 per slot); no later call allocates device memory. */
+int orbfe_kfdb_create(OrbfeVocabulary *v, int max_keyframes, long long max_postings, OrbfeKeyFrameDB **out);
+void orbfe_kfdb_destroy(OrbfeKeyFrameDB *db);
+
+/* add(pKF) (:39-45): the BowVector ids/vals[0, nw) (word ids strictly ascending, < the vocabulary's word count) of a NEW
+ * keyframe in an empty slot; it goes to the end of every word's list.  Its query fields start as a fresh KeyFrame's:
+ * stamps 0, scores 0.  An occupied slot gives ORBFE_ERR_ARG; more than max_postings words in the database gives
+ * ORBFE_ERR_CAPACITY; in both cases the database is unchanged.  The covisibility list of the slot is left as it is.
+ * Synchronous. */
+int orbfe_kfdb_add(OrbfeKeyFrameDB *db, int slot, int nw, const int32_t *ids, const double *vals);
+/* erase(pKF) (:47-66): the keyframe leaves every word's list, its postings become free for later adds, and its covisibility
+ * list is emptied.  Erasing an empty slot does nothing, as in the reference.  Synchronous. */
+int orbfe_kfdb_erase(OrbfeKeyFrameDB *db, int slot);
+/* clear() (:68-72): every slot becomes empty. Synchronous. */
+int orbfe_kfdb_clear(OrbfeKeyFrameDB *db);
+/* Replaces the best-covisibility lists (GetBestCovisibilityKeyFrames(10), read at :150 and :264) of n distinct slots: slot
+ * slots[i] gets lists[ptr[i] .. ptr[i+1]) (ptr[0] = 0, at most 10 slot ids each, in the order that call returns).  Refresh
+ * the new keyframe and its neighbours after KeyFrame::UpdateConnections.  An entry that names an empty slot contributes
+ * nothing (an empty slot is never touched by a query).  Synchronous. */
+int orbfe_kfdb_set_covisibles(OrbfeKeyFrameDB *db, int n, const int32_t *slots, const int32_t *ptr, const int32_t *lists);
+/* Number of occupied slots and of postings held (either pointer may be NULL). */
+int orbfe_kfdb_size(OrbfeKeyFrameDB *db, int *nkeyframes, long long *npostings);
+
+/* DetectLoopCandidates (mode 0, :75-196; `connected` = the query keyframe's GetConnectedKeyFrames() as slots, min_score =
+ * minScore) / DetectRelocalisationCandidates (mode 1, :198-308; connected and min_score unused).  Every call is a new query
+ * id.  The query BowVector q_ids/q_vals[0, nq) has word ids strictly ascending, nq <= 65535.  cand_out receives the
+ * candidate slots in the order of the returned vector.  words_out / score_out (max_keyframes entries each, may be NULL)
+ * receive mnLoopWords / mnRelocWords and mLoopScore / mRelocScore of every slot this query touched (shares a word with it),
+ * -1 elsewhere.  More than `cap` candidates: ORBFE_ERR_CAPACITY with the number needed in *ncand_out.
+ * Host pointers, synchronous; a thin wrapper over orbfe_kfdb_detect_device. */
+int orbfe_kfdb_detect(OrbfeKeyFrameDB *db, int mode, int nq, const int32_t *q_ids, const double *q_vals, int nconn, const int32_t *connected,
+                      float min_score, int cap, int32_t *cand_out, int *ncand_out, int32_t *words_out, float *score_out);
+/* The same query with device arrays: d_q_ids / d_q_vals / d_connected in, d_cand (cap entries), *d_ncand (the number of
+ * candidates; when it exceeds cap only the first cap were written), d_words / d_score (max_keyframes entries each, may
+ * be NULL) out.  Word ids out of the vocabulary's range are skipped.  Enqueued on `stream` (NULL = the handle's stream),
+ * not synchronised: five kernels, no host round trip. */
+int orbfe_kfdb_detect_device(OrbfeKeyFrameDB *db, int mode, int nq, const int32_t *d_q_ids, const double *d_q_vals, int nconn,
+                             const int32_t *d_connected, float min_score, int cap, int32_t *d_cand, int *d_ncand, int32_t *d_words,
+                             float *d_score, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -142,3 +142,100 @@ def db_detect(matcher: ORBmatcher, mode, q_ids, q_vals, kf_ptr, db_ids, db_vals,
     _check(_bind().orbfe_bow_db_detect(matcher.handle, mode, len(q_ids), _p(q_ids), _p(q_vals), nkf, _p(kf_ptr), _p(db_ids), _p(db_vals),
                                        _p(connected), _p(covis_ptr), _p(covis), min_score, C.byref(nc), _p(cand), _p(common), _p(score)))
     return cand[:nc.value], common[:nkf], score[:nkf]
+
+
+_kfdb_bound = False
+
+
+def _bind_kfdb():
+    global _kfdb_bound
+    L = _bind()
+    if _kfdb_bound:
+        return L
+    vp, i = C.c_void_p, C.c_int
+    L.orbfe_kfdb_create.argtypes = [vp, i, C.c_longlong, C.POINTER(vp)]
+    L.orbfe_kfdb_destroy.argtypes = [vp]
+    L.orbfe_kfdb_destroy.restype = None
+    L.orbfe_kfdb_add.argtypes = [vp, i, i, vp, vp]
+    L.orbfe_kfdb_erase.argtypes = [vp, i]
+    L.orbfe_kfdb_clear.argtypes = [vp]
+    L.orbfe_kfdb_set_covisibles.argtypes = [vp, i, vp, vp, vp]
+    L.orbfe_kfdb_size.argtypes = [vp, vp, vp]
+    L.orbfe_kfdb_detect.argtypes = [vp, i, i, vp, vp, i, vp, C.c_float, i, vp, vp, vp, vp]
+    L.orbfe_kfdb_detect_device.argtypes = [vp, i, i, vp, vp, i, vp, C.c_float, i, vp, vp, vp, vp, vp]
+    _kfdb_bound = True
+    return L
+
+
+class KeyFrameDatabase:
+    """KeyFrameDatabase (reference src/KeyFrameDatabase.cc) resident on the vocabulary's device: keyframes are slots
+    0 <= slot < max_keyframes, the inverted file, BowVectors, covisibility lists and the per-keyframe query fields live in
+    device memory (include/orbfe_bow.h, orbfe_kfdb_*)."""
+
+    LOOP, RELOC = 0, 1
+
+    def __init__(self, voc: "Vocabulary", max_keyframes, max_postings):
+        L = _bind_kfdb()
+        h = C.c_void_p()
+        _check(L.orbfe_kfdb_create(voc.handle, int(max_keyframes), int(max_postings), C.byref(h)))
+        self._h, self.max_keyframes, self._voc = h.value, int(max_keyframes), voc
+
+    @property
+    def handle(self):
+        return self._h
+
+    def close(self):
+        if self._h:
+            lib().orbfe_kfdb_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def add(self, slot, ids, vals):
+        ids, vals = np.ascontiguousarray(ids, np.int32), np.ascontiguousarray(vals, np.float64)
+        _check(_bind_kfdb().orbfe_kfdb_add(self._h, int(slot), len(ids), _p(ids), _p(vals)))
+
+    def erase(self, slot):
+        _check(_bind_kfdb().orbfe_kfdb_erase(self._h, int(slot)))
+
+    def clear(self):
+        _check(_bind_kfdb().orbfe_kfdb_clear(self._h))
+
+    def set_covisibles(self, lists):
+        """lists: {slot: [covisible slots, best first]} (at most 10 each)."""
+        slots = np.array(sorted(lists), np.int32)
+        ptr = np.zeros(len(slots) + 1, np.int32)
+        flat = []
+        for k, s in enumerate(slots):
+            flat += list(lists[int(s)])
+            ptr[k + 1] = len(flat)
+        flat = np.array(flat if flat else [0], np.int32)
+        _check(_bind_kfdb().orbfe_kfdb_set_covisibles(self._h, len(slots), _p(slots), _p(ptr), _p(flat)))
+
+    def size(self):
+        n, p = C.c_int(0), C.c_longlong(0)
+        _check(_bind_kfdb().orbfe_kfdb_size(self._h, C.byref(n), C.byref(p)))
+        return n.value, p.value
+
+    def detect(self, mode, q_ids, q_vals, connected=(), min_score=0.0, cap=None):
+        """(candidate slots, words per slot, score per slot); words / scores are -1 where the query touched nothing."""
+        q_ids, q_vals = np.ascontiguousarray(q_ids, np.int32), np.ascontiguousarray(q_vals, np.float64)
+        conn = np.ascontiguousarray(connected if len(connected) else [0], np.int32)
+        cap = self.max_keyframes if cap is None else int(cap)
+        cand = np.zeros(max(cap, 1), np.int32)
+        words, score = np.zeros(self.max_keyframes, np.int32), np.zeros(self.max_keyframes, np.float32)
+        nc = C.c_int(0)
+        _check(_bind_kfdb().orbfe_kfdb_detect(self._h, mode, len(q_ids), _p(q_ids), _p(q_vals), len(connected), _p(conn), min_score, cap,
+                                              _p(cand), C.byref(nc), _p(words), _p(score)))
+        return cand[:nc.value], words, score
+
+    def detect_device(self, mode, nq, d_q_ids, d_q_vals, nconn, d_connected, min_score, cap, d_cand, d_ncand, d_words=0, d_score=0,
+                      stream=0):
+        """Device-pointer form (ints = raw device addresses); enqueued, not synchronised."""
+        vp = C.c_void_p
+        _check(_bind_kfdb().orbfe_kfdb_detect_device(self._h, mode, nq, vp(d_q_ids), vp(d_q_vals), nconn, vp(d_connected), min_score, cap,
+                                                     vp(d_cand), vp(d_ncand), vp(d_words or None), vp(d_score or None), vp(stream)))

@@ -10,9 +10,9 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "liborbfe.so")
-SOURCES = ["orbfe_api.cu", "extract_kernels.cu", "match_kernels.cu", "bow_kernels.cu", "comm.cu",
+SOURCES = ["orbfe_api.cu", "extract_kernels.cu", "match_kernels.cu", "bow_kernels.cu", "kfdb.cu", "comm.cu",
            os.path.join("..", "host", "match_host.cpp"), os.path.join("..", "host", "bow_host.cpp")]
-DEPS = SOURCES + ["orbfe_internal.h", os.path.join("..", "..", "include", "orbfe.h"),
+DEPS = SOURCES + ["orbfe_internal.h", "bow_l1.cuh", os.path.join("..", "..", "include", "orbfe.h"),
                   os.path.join("..", "..", "include", "orbfe_match.h"), os.path.join("..", "..", "include", "orbfe_bow.h"), os.path.join("..", "..", "include", "orbfe_comm.h"),
                   os.path.join("..", "..", "include", "orbfe_brief_pattern.inc"), os.path.join("..", "build.py")]
 

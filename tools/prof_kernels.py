@@ -19,6 +19,9 @@
                    CUDA-event ms of
                    orbfe_distinctive_descriptors_device next to the wall time of orbfe_distinctive_descriptors including the
                    host gather of the descriptors, and same_as_host
+  --what kfdb      the resident KeyFrameDatabase at 1k and 10k keyframes of ~1000 words (ids over 10^6): CUDA-event ms per loop
+                   and per relocalisation query, host ms per add / erase, and the wall time of the stateless
+                   orbfe_bow_db_detect on the same data
 
 Prints one JSON object per --what; never a bench value when run under ncu."""
 import argparse
@@ -743,6 +746,98 @@ def latency(args):
     return out
 
 
+def kfdb(args):
+    """The resident keyframe database (orbfe_kfdb_*) at 1k and 10k keyframes of about 1000 words each, word ids spread over
+    10^6 (the size of ORBvoc): device time per loop and per relocalisation query (CUDA events around orbfe_kfdb_detect_device,
+    queries taken from the keyframes' own neighbourhood so that candidates exist), host time per add and per erase (both
+    synchronous), and on the same data the wall time of the stateless orbfe_bow_db_detect (CSR arrays of the whole
+    database uploaded per query)."""
+    import time
+    import torch
+    import orb_slam_b200 as fe
+    from orb_slam_b200 import bow as BW
+    NW, WPK = 1_000_000, 1000
+    n = NW + 1
+    cp = np.zeros(n + 1, np.int32)
+    cp[1:] = NW
+    V = BW.Vocabulary({"node_desc": np.zeros((n, 32), np.uint8), "child_ptr": cp, "children": np.arange(1, n, dtype=np.int32),
+                       "word_id": np.arange(-1, NW, dtype=np.int32), "weight": np.ones(n), "L": 1})
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    m = fe.ORBmatcher(0.75, True)
+    out = {"what": "KeyFrameDatabase resident on the device: %d words per keyframe, word ids over 10^6" % WPK}
+    _gpu_and_power_limit(out)
+    for nkf in (1000, 10000):
+        rng = np.random.default_rng(nkf)
+        shift = 100
+        track = rng.integers(0, NW, nkf * shift + 4 * WPK)
+
+        def bow_at(pos):
+            w = track[pos:pos + WPK].copy()
+            flip = rng.random(WPK) < 0.25
+            w[flip] = rng.integers(0, NW, int(flip.sum()))
+            ids = np.unique(w).astype(np.int32)
+            v = rng.uniform(0.2, 3.0, len(ids))
+            return ids, v / v.sum()
+
+        bows = [bow_at(shift * k) for k in range(nkf)]
+        db = BW.KeyFrameDatabase(V, nkf, nkf * WPK + 10 * WPK)
+        t0 = time.perf_counter()
+        for k in range(nkf):
+            db.add(k, *bows[k])
+        t_add = (time.perf_counter() - t0) / nkf
+        lists = {k: [j for j in (k - 1, k + 1, k - 2, k + 2, k - 3, k + 3, k - 4, k + 4, k - 5, k + 5) if 0 <= j < nkf] for k in range(nkf)}
+        db.set_covisibles(lists)
+        queries = [bow_at(shift * int(rng.integers(0, nkf)) + 7) for _ in range(32)]
+        t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dt)).to(dev)
+        dq = [(t(q[0], np.int32), t(q[1], np.float64), len(q[0])) for q in queries]
+        d_conn = t(np.arange(10), np.int32)
+        d_cand, d_n = torch.zeros(nkf, dtype=torch.int32, device=dev), torch.zeros(1, dtype=torch.int32, device=dev)
+        torch.cuda.synchronize()
+        res = {"keyframes": nkf, "postings": db.size()[1], "add_ms": round(t_add * 1e3, 4)}
+        for mode, tag in ((0, "loop_query_ms"), (1, "reloc_query_ms")):
+            def run():
+                for qi, qv, nq in dq:
+                    db.detect_device(mode, nq, qi.data_ptr(), qv.data_ptr(), 10, d_conn.data_ptr(), 0.0, nkf, d_cand.data_ptr(), d_n.data_ptr(),
+                                     0, 0, stream.cuda_stream)
+            for _ in range(args.warmup):
+                run()
+            stream.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(stream)
+            for _ in range(args.iters):
+                run()
+            e1.record(stream)
+            stream.synchronize()
+            res[tag] = round(e0.elapsed_time(e1) / (args.iters * len(dq)), 4)
+        res["candidates_last_query"] = int(d_n.item())
+        # erase + re-add of 100 keyframes
+        t0 = time.perf_counter()
+        for k in range(100):
+            db.erase(k)
+        res["erase_ms"] = round((time.perf_counter() - t0) / 100 * 1e3, 4)
+        for k in range(100):
+            db.add(k, *bows[k])
+        # the stateless call on the same data: every keyframe's BowVector and covisibility list passed per query
+        kf_ptr = np.cumsum([0] + [len(b[0]) for b in bows]).astype(np.int32)
+        db_ids, db_vals = np.concatenate([b[0] for b in bows]), np.concatenate([b[1] for b in bows])
+        cv_ptr = np.cumsum([0] + [len(lists[k]) for k in range(nkf)]).astype(np.int32)
+        cv = np.concatenate([np.array(lists[k], np.int32) for k in range(nkf)])
+        connected = np.zeros(nkf, np.uint8)
+        connected[:10] = 1
+        for mode, tag in ((0, "stateless_loop_wall_ms"), (1, "stateless_reloc_wall_ms")):
+            BW.db_detect(m, mode, *queries[0], kf_ptr, db_ids, db_vals, connected, cv_ptr, cv)
+            t0 = time.perf_counter()
+            for q in queries[:8]:
+                BW.db_detect(m, mode, *q, kf_ptr, db_ids, db_vals, connected, cv_ptr, cv)
+            res[tag] = round((time.perf_counter() - t0) / 8 * 1e3, 4)
+        out["%dk" % (nkf // 1000)] = res
+        db.close()
+    m.close()
+    V.close()
+    return out
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--what", default="config3,config5")
@@ -753,4 +848,4 @@ if __name__ == "__main__":
     args = ap.parse_args()
     for w in args.what.split(","):
         print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fast": fast, "latency": latency,
-                          "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc}[w](args)))
+                          "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb}[w](args)))
