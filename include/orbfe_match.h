@@ -3,8 +3,10 @@
  *
  * Each function is the array-level equivalent of one ORB_SLAM::ORBmatcher method (reference
  * src/ORBmatcher.cc); the C++ facade orb_slam_b200/host/ORBmatcher.cc converts Frame / MapPoint objects
- * into these views.  Candidate enumeration and the sequential accept loop run on the host exactly in the
- * reference's order; every 256-bit Hamming distance is computed on the GPU (one launch per call).
+ * into these views.  SearchByBoW and SearchForTriangulation run entirely on the GPU.  The windowed matchers run on
+ * the fused device kernel where their inputs fit it; otherwise candidate enumeration and the sequential accept loop
+ * run on the host exactly in the reference's order and every 256-bit Hamming distance is computed on the GPU (one
+ * launch per call).
  */
 #ifndef ORBFE_MATCH_H
 #define ORBFE_MATCH_H
@@ -141,7 +143,11 @@ int orbfe_guided_best(OrbfeMatcher *m, const OrbfeFrameView *f, int nq, const fl
  * A DBoW2::FeatureVector is passed as ascending node ids + CSR (ptr, items = feature indices in insertion order).
  * valid1[i] / valid2[i]: the feature has a map point that is not bad (valid2 is ignored by variant 0).
  * angle1 / angle2: mvKeysUn[i].angle of each side.  variant 0: out has n2 entries, out[i2] = matched side-1 index;
- * variant 1: out has n1 entries, out[i1] = matched side-2 index; -1 = no match. */
+ * variant 1: out has n1 entries, out[i1] = matched side-2 index; -1 = no match.
+ * items holds ptr[nn] entries, and every feature index appears in at most one node (true of any DBoW2 FeatureVector).
+ * Runs as one job of orbfe_search_by_bow_device (staging, one launch, synchronised), so it rejects the same FeatureVectors:
+ * a common node whose row reaches outside [0, ptr[nn]] or holds a feature index outside [0, n) gives ORBFE_ERR_ARG, and out
+ * is then not meaningful.  At most 65535 features and 65535 FeatureVector nodes per side (ORBFE_ERR_UNSUPPORTED). */
 int orbfe_search_by_bow(OrbfeMatcher *m, int variant, int n1, const uint8_t *desc1, const uint8_t *valid1, const float *angle1,
                         int nn1, const int32_t *ids1, const int32_t *ptr1, const int32_t *items1, int n2, const uint8_t *desc2,
                         const uint8_t *valid2, const float *angle2, int nn2, const int32_t *ids2, const int32_t *ptr2,
@@ -158,7 +164,7 @@ int orbfe_search_by_bow(OrbfeMatcher *m, int variant, int n1, const uint8_t *des
  * d_valid[f*cap + i] != 0: feature i of frame f has a map point that is not bad (side 2 of variant 0 ignores it).
  * Angles are d_kps[].angle.  variant 0: row j of d_out (njobs x cap) is indexed by side-2 feature and holds the matched
  * side-1 index; variant 1: indexed by side-1 feature, holding the side-2 index; -1 = no match; the first count entries of
- * each row are written.  d_nmatches[j] = the method's return value.  Results equal orbfe_search_by_bow's.
+ * each row are written.  d_nmatches[j] = the method's return value.
  * One thread block per job, no global scratch.  A FeatureVector entry outside the frame's slots (node count > cap, a row
  * outside [0, cap], a feature index >= the frame's count) is never followed: that job's d_nmatches is -1 and
  * orbfe_matcher_sync reports ORBFE_ERR_ARG; the other jobs of the launch are unaffected.  Frame indices are not checked.
@@ -171,8 +177,13 @@ int orbfe_search_by_bow_device(OrbfeMatcher *m, int variant, int njobs, const Or
 
 /* int ORBmatcher::SearchForTriangulation(pKF1, pKF2, F12, ...) (ORBmatcher.cc:852-1014) with CheckDistEpipolarLine
  * (:136-153).  keys1/keys2 = GetKeyPointsUn(); has_mp1/2[i] != 0 <=> the feature already has a map point (skipped);
- * FeatureVectors as in orbfe_search_by_bow; F12 = 3x3 row-major floats; sigma2_kf2[level] = pKF2->GetSigma2(level).
- * match12_out[i1] = matched index in keyframe 2 or -1 (the caller builds vMatchedKeys1/2 and vMatchedPairs from it). */
+ * FeatureVectors as in orbfe_search_by_bow; F12 = 3x3 row-major floats; sigma2_kf2[level] = pKF2->GetSigma2(level), with an
+ * entry for every octave that occurs in keys2 (GetScaleLevels() entries do).
+ * match12_out[i1] = matched index in keyframe 2 or -1 (the caller builds vMatchedKeys1/2 and vMatchedPairs from it).
+ * Runs as one job of orbfe_search_for_triangulation_device, with nlevels = 1 + the largest octave of keys2 (at most
+ * ORBFE_MAX_LEVELS).  ORBFE_ERR_ARG for the FeatureVectors orbfe_search_by_bow rejects and for a side-2 feature without a map
+ * point, in a common node, whose octave is negative or >= ORBFE_MAX_LEVELS; match12_out is then not meaningful.  At most
+ * 65535 features and 65535 FeatureVector nodes per side (ORBFE_ERR_UNSUPPORTED). */
 int orbfe_search_for_triangulation(OrbfeMatcher *m, int n1, const OrbfeKeyPoint *keys1, const uint8_t *desc1,
                                    const uint8_t *has_mp1, int nn1, const int32_t *ids1, const int32_t *ptr1, const int32_t *items1,
                                    int n2, const OrbfeKeyPoint *keys2, const uint8_t *desc2, const uint8_t *has_mp2, int nn2,
@@ -189,7 +200,6 @@ int orbfe_search_for_triangulation(OrbfeMatcher *m, int n1, const OrbfeKeyPoint 
  * d_F12 = njobs x 9 row-major floats (ComputeF12 of the pair); sigma2 = `nlevels` floats on the HOST (KeyFrame::GetSigma2,
  * shared by all keyframes of one extractor).  Row j of d_match12 (njobs x cap) is indexed by side-1 feature and holds the
  * matched side-2 index or -1 for the first counts[d_idx1[j]] entries; d_nmatches[j] = the method's return value.
- * Results equal orbfe_search_for_triangulation's.
  * One thread block per job, no global scratch.  A job whose FeatureVectors point outside the frames' slots (node count
  * outside [0, cap], a row outside [0, cap], a feature index >= the frame's count) or whose side-2 features without a map
  * point in a common node have an octave outside [0, nlevels) is never followed out of bounds: its d_nmatches is -1 and

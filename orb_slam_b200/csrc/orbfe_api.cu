@@ -14,12 +14,15 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <string>
+#include <utility>
 #include <vector>
 #include <atomic>
 #include <thread>
 #include <unordered_map>
 
+#include "../../include/orbfe_match.h"
 #include "orbfe_internal.h"
 
 using namespace orbfe;
@@ -1104,6 +1107,28 @@ extern "C" int orbfe_guided_search_device(OrbfeMatcher *m, int njobs, const Orbf
     return ORBFE_OK;
 }
 
+// Staging block of the host-array entries that run on a device kernel: places arrays of `second` bytes at 256-byte aligned
+// offsets (*first), sets *total to the block's size and grows the pinned host block h_stage and its device twin d_stage to
+// hold it.  The caller packs h_stage, copies it to d_stage in one H2D and synchronises before it returns.
+static int stage_layout(OrbfeMatcher *m, std::initializer_list<std::pair<size_t *, size_t>> arrays, size_t *total) {
+    size_t off = 0;
+    for (const auto &a : arrays) {
+        *a.first = off;
+        off += (a.second + 255) / 256 * 256;
+    }
+    *total = off;
+    if (m->stage_cap < off) {
+        if (m->h_stage) cudaFreeHost(m->h_stage);
+        if (m->d_stage) cudaFree(m->d_stage);
+        m->h_stage = nullptr; m->d_stage = nullptr; m->stage_cap = 0;
+        const size_t want = off + off / 4;
+        CU_TRY(cudaHostAlloc((void **)&m->h_stage, want, cudaHostAllocDefault));
+        CU_TRY(cudaMalloc((void **)&m->d_stage, want));
+        m->stage_cap = want;
+    }
+    return ORBFE_OK;
+}
+
 // SearchByBoW (both overloads) for `njobs` frame pairs, device-resident (include/orbfe_match.h).  Arguments are checked before
 // the handle is used.
 extern "C" int orbfe_search_by_bow_device(OrbfeMatcher *m, int variant, int njobs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
@@ -1122,6 +1147,73 @@ extern "C" int orbfe_search_by_bow_device(OrbfeMatcher *m, int variant, int njob
                          nnratio, check_orientation ? 1 : 0, d_out, d_nmatches, m->d_err, s);
     CU_TRY(cudaGetLastError());
     m->launches += 1;
+    return ORBFE_OK;
+}
+
+// SearchByBoW on host arrays: both sides staged as a two-frame store (frame 0 = side 1, frame 1 = side 2), one H2D, one job of
+// orbfe_search_by_bow_device, one D2H.
+extern "C" int orbfe_search_by_bow(OrbfeMatcher *m, int variant, int n1, const uint8_t *desc1, const uint8_t *valid1,
+                                   const float *angle1, int nn1, const int32_t *ids1, const int32_t *ptr1, const int32_t *items1,
+                                   int n2, const uint8_t *desc2, const uint8_t *valid2, const float *angle2, int nn2,
+                                   const int32_t *ids2, const int32_t *ptr2, const int32_t *items2, float nnratio,
+                                   int check_orientation, int32_t *out, int *nmatches_out) {
+    if (!m || (variant != 0 && variant != 1) || n1 < 0 || n2 < 0 || nn1 < 0 || nn2 < 0 || !out || !nmatches_out)
+        return fail(ORBFE_ERR_ARG, "bad arguments");
+    if ((n1 > 0 && (!desc1 || !valid1 || !angle1)) || (n2 > 0 && (!desc2 || !angle2 || (variant == 1 && !valid2))) ||
+        (nn1 > 0 && (!ids1 || !ptr1 || !items1)) || (nn2 > 0 && (!ids2 || !ptr2 || !items2)))
+        return fail(ORBFE_ERR_ARG, "NULL argument");
+    const int cap = std::max({n1, n2, nn1, nn2, 1});
+    if (cap > 65535) return fail(ORBFE_ERR_UNSUPPORTED, "%d features or FeatureVector nodes on one side: at most 65535", cap);
+    CU_TRY(cudaSetDevice(m->device));
+    const size_t C = (size_t)cap;
+    size_t o_kps, o_desc, o_cnt, o_ids, o_ptr, o_items, o_nn, o_valid, o_idx, o_out, o_nm, total;
+    if (int rc = stage_layout(m, {{&o_kps, 2 * C * sizeof(OrbfeKeyPoint)}, {&o_desc, 2 * C * 32}, {&o_cnt, 2 * sizeof(int)},
+                                  {&o_ids, 2 * C * 4}, {&o_ptr, 2 * (C + 1) * 4}, {&o_items, 2 * C * 4}, {&o_nn, 2 * sizeof(int)},
+                                  {&o_valid, 2 * C}, {&o_idx, 2 * sizeof(int)}, {&o_out, C * 4}, {&o_nm, sizeof(int)}},
+                              &total))
+        return rc;
+    unsigned char *H = m->h_stage, *D = m->d_stage;
+    const int n[2] = {n1, n2}, nn[2] = {nn1, nn2};
+    const uint8_t *desc[2] = {desc1, desc2}, *valid[2] = {valid1, variant == 1 ? valid2 : nullptr};
+    const float *angle[2] = {angle1, angle2};
+    const int32_t *ids[2] = {ids1, ids2}, *ptr[2] = {ptr1, ptr2}, *items[2] = {items1, items2};
+    for (int f = 0; f < 2; f++) {
+        ((int *)(H + o_cnt))[f] = n[f];
+        ((int *)(H + o_nn))[f] = nn[f];
+        ((int *)(H + o_idx))[f] = f;
+        // search_by_bow_kernel reads no keypoint field but .angle
+        OrbfeKeyPoint *kp = (OrbfeKeyPoint *)(H + o_kps) + f * C;
+        for (int i = 0; i < n[f]; i++) kp[i].angle = angle[f][i];
+        if (n[f]) memcpy(H + o_desc + f * C * 32, desc[f], (size_t)n[f] * 32);
+        if (valid[f]) memcpy(H + o_valid + f * C, valid[f], (size_t)n[f]);
+        else memset(H + o_valid + f * C, 0, (size_t)n[f]);   // variant 0 ignores side 2's flags
+        // FeatureVector: item slots past ptr[nn] hold -1, so a row that reaches beyond the caller's items is rejected by
+        // the kernel instead of being read
+        int *fptr = (int *)(H + o_ptr) + f * (C + 1), *fitems = (int *)(H + o_items) + f * C;
+        fptr[0] = 0;
+        if (nn[f]) {
+            memcpy((int *)(H + o_ids) + f * C, ids[f], (size_t)nn[f] * 4);
+            memcpy(fptr, ptr[f], ((size_t)nn[f] + 1) * 4);
+        }
+        const int ni = nn[f] ? std::min(std::max(ptr[f][nn[f]], 0), cap) : 0;
+        if (ni) memcpy(fitems, items[f], (size_t)ni * 4);
+        std::fill(fitems + ni, fitems + C, -1);
+    }
+    cudaStream_t s = m->stream;
+    CU_TRY(cudaMemcpyAsync(D, H, o_out, cudaMemcpyHostToDevice, s));
+    const int *d_idx = (const int *)(D + o_idx);
+    int rc = orbfe_search_by_bow_device(m, variant, 1, (const OrbfeKeyPoint *)(D + o_kps), D + o_desc, (const int *)(D + o_cnt), cap,
+                                        (const int32_t *)(D + o_ids), (const int32_t *)(D + o_ptr), (const int32_t *)(D + o_items),
+                                        (const int *)(D + o_nn), D + o_valid, d_idx, d_idx + 1, nnratio, check_orientation,
+                                        (int32_t *)(D + o_out), (int *)(D + o_nm), s);
+    if (rc) return rc;
+    CU_TRY(cudaMemcpyAsync(H + o_out, D + o_out, total - o_out, cudaMemcpyDeviceToHost, s));
+    if ((rc = orbfe_matcher_sync(m))) return rc;
+    m->h2d_bytes += o_out;
+    m->d2h_bytes += total - o_out;
+    const int nout = variant == 0 ? n2 : n1;
+    if (nout) memcpy(out, H + o_out, (size_t)nout * 4);
+    *nmatches_out = *(const int *)(H + o_nm);
     return ORBFE_OK;
 }
 
@@ -1144,6 +1236,78 @@ extern "C" int orbfe_search_for_triangulation_device(OrbfeMatcher *m, int njobs,
                                     d_F12, sigma2, nlevels, check_orientation ? 1 : 0, d_match12, d_nmatches, m->d_err, s);
     CU_TRY(cudaGetLastError());
     m->launches += 1;
+    return ORBFE_OK;
+}
+
+// SearchForTriangulation on host arrays: staged and run as orbfe_search_by_bow stages and runs SearchByBoW, with F12 as the
+// job's 9 floats and as many levels as the octaves of keys2 need.
+extern "C" int orbfe_search_for_triangulation(OrbfeMatcher *m, int n1, const OrbfeKeyPoint *keys1, const uint8_t *desc1,
+                                              const uint8_t *has_mp1, int nn1, const int32_t *ids1, const int32_t *ptr1,
+                                              const int32_t *items1, int n2, const OrbfeKeyPoint *keys2, const uint8_t *desc2,
+                                              const uint8_t *has_mp2, int nn2, const int32_t *ids2, const int32_t *ptr2,
+                                              const int32_t *items2, const float *F12, const float *sigma2_kf2,
+                                              int check_orientation, int32_t *match12_out, int *nmatches_out) {
+    if (!m || n1 < 0 || n2 < 0 || nn1 < 0 || nn2 < 0 || !F12 || !sigma2_kf2 || !match12_out || !nmatches_out)
+        return fail(ORBFE_ERR_ARG, "bad arguments");
+    if ((n1 > 0 && (!keys1 || !desc1 || !has_mp1)) || (n2 > 0 && (!keys2 || !desc2 || !has_mp2)) ||
+        (nn1 > 0 && (!ids1 || !ptr1 || !items1)) || (nn2 > 0 && (!ids2 || !ptr2 || !items2)))
+        return fail(ORBFE_ERR_ARG, "NULL argument");
+    const int cap = std::max({n1, n2, nn1, nn2, 1});
+    if (cap > 65535) return fail(ORBFE_ERR_UNSUPPORTED, "%d features or FeatureVector nodes on one side: at most 65535", cap);
+    // sigma2_kf2 holds an entry for every octave of keys2; an octave outside [0, nlevels) of a feature the kernel would test
+    // rejects the job
+    int nlevels = 1;
+    for (int i = 0; i < n2; i++) nlevels = std::max(nlevels, std::min(keys2[i].octave, ORBFE_MAX_LEVELS - 1) + 1);
+    CU_TRY(cudaSetDevice(m->device));
+    const size_t C = (size_t)cap;
+    size_t o_kps, o_desc, o_cnt, o_ids, o_ptr, o_items, o_nn, o_has, o_idx, o_F, o_out, o_nm, total;
+    if (int rc = stage_layout(m, {{&o_kps, 2 * C * sizeof(OrbfeKeyPoint)}, {&o_desc, 2 * C * 32}, {&o_cnt, 2 * sizeof(int)},
+                                  {&o_ids, 2 * C * 4}, {&o_ptr, 2 * (C + 1) * 4}, {&o_items, 2 * C * 4}, {&o_nn, 2 * sizeof(int)},
+                                  {&o_has, 2 * C}, {&o_idx, 2 * sizeof(int)}, {&o_F, 9 * sizeof(float)}, {&o_out, C * 4},
+                                  {&o_nm, sizeof(int)}},
+                              &total))
+        return rc;
+    unsigned char *H = m->h_stage, *D = m->d_stage;
+    const int n[2] = {n1, n2}, nn[2] = {nn1, nn2};
+    const OrbfeKeyPoint *keys[2] = {keys1, keys2};
+    const uint8_t *desc[2] = {desc1, desc2}, *has_mp[2] = {has_mp1, has_mp2};
+    const int32_t *ids[2] = {ids1, ids2}, *ptr[2] = {ptr1, ptr2}, *items[2] = {items1, items2};
+    for (int f = 0; f < 2; f++) {
+        ((int *)(H + o_cnt))[f] = n[f];
+        ((int *)(H + o_nn))[f] = nn[f];
+        ((int *)(H + o_idx))[f] = f;
+        if (n[f]) {
+            memcpy(H + o_kps + f * C * sizeof(OrbfeKeyPoint), keys[f], (size_t)n[f] * sizeof(OrbfeKeyPoint));
+            memcpy(H + o_desc + f * C * 32, desc[f], (size_t)n[f] * 32);
+            memcpy(H + o_has + f * C, has_mp[f], (size_t)n[f]);
+        }
+        // FeatureVector, as in orbfe_search_by_bow
+        int *fptr = (int *)(H + o_ptr) + f * (C + 1), *fitems = (int *)(H + o_items) + f * C;
+        fptr[0] = 0;
+        if (nn[f]) {
+            memcpy((int *)(H + o_ids) + f * C, ids[f], (size_t)nn[f] * 4);
+            memcpy(fptr, ptr[f], ((size_t)nn[f] + 1) * 4);
+        }
+        const int ni = nn[f] ? std::min(std::max(ptr[f][nn[f]], 0), cap) : 0;
+        if (ni) memcpy(fitems, items[f], (size_t)ni * 4);
+        std::fill(fitems + ni, fitems + C, -1);
+    }
+    memcpy(H + o_F, F12, 9 * sizeof(float));
+    cudaStream_t s = m->stream;
+    CU_TRY(cudaMemcpyAsync(D, H, o_out, cudaMemcpyHostToDevice, s));
+    const int *d_idx = (const int *)(D + o_idx);
+    int rc = orbfe_search_for_triangulation_device(m, 1, (const OrbfeKeyPoint *)(D + o_kps), D + o_desc, (const int *)(D + o_cnt), cap,
+                                                   (const int32_t *)(D + o_ids), (const int32_t *)(D + o_ptr),
+                                                   (const int32_t *)(D + o_items), (const int *)(D + o_nn), D + o_has, d_idx, d_idx + 1,
+                                                   (const float *)(D + o_F), sigma2_kf2, nlevels, check_orientation,
+                                                   (int32_t *)(D + o_out), (int *)(D + o_nm), s);
+    if (rc) return rc;
+    CU_TRY(cudaMemcpyAsync(H + o_out, D + o_out, total - o_out, cudaMemcpyDeviceToHost, s));
+    if ((rc = orbfe_matcher_sync(m))) return rc;
+    m->h2d_bytes += o_out;
+    m->d2h_bytes += total - o_out;
+    if (n1) memcpy(match12_out, H + o_out, (size_t)n1 * 4);
+    *nmatches_out = *(const int *)(H + o_nm);
     return ORBFE_OK;
 }
 
@@ -1398,7 +1562,6 @@ extern "C" int orbfe_knn2_groups(OrbfeMatcher *m, const uint8_t *q, int nq, cons
 // staging block, one H2D, one launch, one D2H.  Returns 1 when the call has to take the host-replay path
 // (mixed geometries, > 65535 features, or a pair overflowed the candidate scratch).
 // ------------------------------------------------------------------------------------------------
-#include "../../include/orbfe_match.h"
 extern "C" int orbfe_sbp_frames_via_device(OrbfeMatcher *m, int npairs, const OrbfeFrameView *cur, const OrbfeFrameView *last,
                                            const uint8_t *const *last_has_mp, const uint8_t *const *last_outlier,
                                            const float *const *last_world, const float *const *Tcw, float fx, float fy,
@@ -1458,24 +1621,15 @@ extern "C" int orbfe_sbp_frames_via_device(OrbfeMatcher *m, int npairs, const Or
         }
     }
     const size_t nf = slots.size();
-    // layout of the staging block
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-    const size_t o_kps = take(nf * cap * sizeof(OrbfeKeyPoint)), o_desc = take(nf * cap * 32), o_cnt = take(nf * sizeof(int));
-    const size_t o_world = take(nf * cap * 3 * sizeof(float)), o_flags = take(nf * cap), o_T = take((size_t)npairs * 12 * sizeof(float));
-    const size_t o_ci = take((size_t)npairs * sizeof(int)), o_li = take((size_t)npairs * sizeof(int));
-    const size_t in_bytes = off;
-    const size_t o_mp = take((size_t)npairs * cap * sizeof(int)), o_nm = take((size_t)npairs * sizeof(int));
-    const size_t total = off;
-    if (m->stage_cap < total) {
-        if (m->h_stage) cudaFreeHost(m->h_stage);
-        if (m->d_stage) cudaFree(m->d_stage);
-        m->h_stage = nullptr; m->d_stage = nullptr; m->stage_cap = 0;
-        const size_t want = total + total / 4;
-        CU_TRY(cudaHostAlloc((void **)&m->h_stage, want, cudaHostAllocDefault));
-        CU_TRY(cudaMalloc((void **)&m->d_stage, want));
-        m->stage_cap = want;
-    }
+    size_t o_kps, o_desc, o_cnt, o_world, o_flags, o_T, o_ci, o_li, o_mp, o_nm, total;
+    if (int rc = stage_layout(m, {{&o_kps, nf * cap * sizeof(OrbfeKeyPoint)}, {&o_desc, nf * cap * 32}, {&o_cnt, nf * sizeof(int)},
+                                  {&o_world, nf * cap * 3 * sizeof(float)}, {&o_flags, nf * cap},
+                                  {&o_T, (size_t)npairs * 12 * sizeof(float)}, {&o_ci, (size_t)npairs * sizeof(int)},
+                                  {&o_li, (size_t)npairs * sizeof(int)}, {&o_mp, (size_t)npairs * cap * sizeof(int)},
+                                  {&o_nm, (size_t)npairs * sizeof(int)}},
+                              &total))
+        return rc;
+    const size_t in_bytes = o_mp;
     unsigned char *H = m->h_stage, *D = m->d_stage;
     int *h_cnt = (int *)(H + o_cnt), *h_ci = (int *)(H + o_ci), *h_li = (int *)(H + o_li);
     auto pack_slot = [&](int sidx) {
@@ -1543,25 +1697,15 @@ extern "C" int orbfe_guided_via_device(OrbfeMatcher *m, const OrbfeFrameView *f,
     const int cap = f->n, qcap = nq;
     if (sbp_smem_fixed_bytes(cap, qcap) + 16 * 1024 > 220 * 1024) return 1;
     CU_TRY(cudaSetDevice(m->device));
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-    const size_t o_kps = take((size_t)cap * sizeof(OrbfeKeyPoint)), o_desc = take((size_t)cap * 32), o_cnt = take(sizeof(int));
-    const size_t o_fi = take(sizeof(int)), o_qb = take(sizeof(int)), o_qc = take(sizeof(int));
-    const size_t o_qu = take((size_t)nq * 4), o_qv = take((size_t)nq * 4), o_qr = take((size_t)nq * 4), o_qa = take((size_t)nq * 4);
-    const size_t o_lo = take((size_t)nq * 4), o_hi = take((size_t)nq * 4), o_qd = take((size_t)nq * 32);
-    const size_t o_mp = take((size_t)cap * sizeof(int));
-    const size_t in_bytes = off;
-    const size_t o_nm = take(sizeof(int));
-    const size_t total = off;
-    if (m->stage_cap < total) {
-        if (m->h_stage) cudaFreeHost(m->h_stage);
-        if (m->d_stage) cudaFree(m->d_stage);
-        m->h_stage = nullptr; m->d_stage = nullptr; m->stage_cap = 0;
-        const size_t want = total + total / 4;
-        CU_TRY(cudaHostAlloc((void **)&m->h_stage, want, cudaHostAllocDefault));
-        CU_TRY(cudaMalloc((void **)&m->d_stage, want));
-        m->stage_cap = want;
-    }
+    size_t o_kps, o_desc, o_cnt, o_fi, o_qb, o_qc, o_qu, o_qv, o_qr, o_qa, o_lo, o_hi, o_qd, o_mp, o_nm, total;
+    if (int rc = stage_layout(m, {{&o_kps, (size_t)cap * sizeof(OrbfeKeyPoint)}, {&o_desc, (size_t)cap * 32}, {&o_cnt, sizeof(int)},
+                                  {&o_fi, sizeof(int)}, {&o_qb, sizeof(int)}, {&o_qc, sizeof(int)}, {&o_qu, (size_t)nq * 4},
+                                  {&o_qv, (size_t)nq * 4}, {&o_qr, (size_t)nq * 4}, {&o_qa, (size_t)nq * 4}, {&o_lo, (size_t)nq * 4},
+                                  {&o_hi, (size_t)nq * 4}, {&o_qd, (size_t)nq * 32}, {&o_mp, (size_t)cap * sizeof(int)},
+                                  {&o_nm, sizeof(int)}},
+                              &total))
+        return rc;
+    const size_t in_bytes = o_nm;
     unsigned char *H = m->h_stage, *D = m->d_stage;
     memcpy(H + o_kps, f->keys_un, (size_t)cap * sizeof(OrbfeKeyPoint));
     memcpy(H + o_desc, f->desc, (size_t)cap * 32);

@@ -10,10 +10,12 @@
   --what reloc     SearchByBoW at its two call sites, device-resident: relocalisation (one 1080p / 2000-keypoint frame against
                    32 candidate keyframes, KeyFrame-vs-Frame overload) and loop closing (one keyframe against 16 candidates,
                    KeyFrame-vs-KeyFrame); CUDA-event ms of the FeatureVector build and of the batched search, next to the wall
-                   time of the same jobs through the per-pair host entry point orbfe_search_by_bow
+                   time of the same jobs one pair per call through the host-array entry orbfe_search_by_bow (staging, one
+                   launch and a synchronise per pair)
   --what mapping   SearchForTriangulation at LocalMapping::CreateNewMapPoints: one 1080p / 2000-keypoint keyframe against 20
                    neighbours, F12 from the poses as ComputeF12; CUDA-event ms of the batched call next to the wall time of the
-                   same jobs through the per-pair host entry point orbfe_search_for_triangulation, and same_as_host
+                   same jobs one pair per call through the host-array entry orbfe_search_for_triangulation (staging, one
+                   launch and a synchronise per pair), and same_as_host
   --what mapdesc   ComputeDistinctiveDescriptors at LocalMapping::ProcessNewKeyFrame: the 2000 map points of one 2000-feature
                    keyframe over a 60-keyframe store (synthetic descriptors), with and without one 1000-observation point;
                    CUDA-event ms of
