@@ -3,10 +3,19 @@
  *
  * Each function is the array-level equivalent of one ORB_SLAM::ORBmatcher method (reference
  * src/ORBmatcher.cc); the C++ facade orb_slam_b200/host/ORBmatcher.cc converts Frame / MapPoint objects
- * into these views.  SearchByBoW and SearchForTriangulation run entirely on the GPU.  The windowed matchers run on
- * the fused device kernel where their inputs fit it; otherwise candidate enumeration and the sequential accept loop
- * run on the host exactly in the reference's order and every 256-bit Hamming distance is computed on the GPU (one
- * launch per call).
+ * into these views.  Every matcher runs on the GPU.  The windowed matchers (SearchByProjection, WindowSearch,
+ * SearchForInitialization and the guided search) run on one fused kernel: Frame's grid, GetFeaturesInArea order, the
+ * distances, the accept loop and the rotation histogram, one thread block per frame pair.  Their host-array forms stage the
+ * arrays, launch once per call and synchronise.
+ *
+ * Accepted domain of the host-array windowed matchers: a call is accepted when the kernel's per-block shared memory,
+ * sbp_smem_fixed_bytes(cap, qcap) + 16 KB, is at most 220 KB, where sbp_smem_fixed_bytes(cap, qcap) is about 24,584 +
+ * 16.125 * cap + 6.125 * qcap bytes.  For orbfe_search_by_projection_frames (cap = qcap = the most features of any view of the call) and
+ * orbfe_search_for_initialization (cap = qcap = max(F1 features, F2 features)) that is at most 8283 features.  For
+ * orbfe_window_search, orbfe_search_local_points, orbfe_search_by_projection_kf, orbfe_search_by_projection_f1f2 and
+ * orbfe_guided_search, cap = the searched frame's feature count and qcap = the number of queries (the features or map points
+ * that pass the routine's own filters): 2000 features allow about 24,800 queries.  Larger calls return ORBFE_ERR_UNSUPPORTED
+ * with a message (orbfe_last_error).  Every rejection sets orbfe_last_error.
  */
 #ifndef ORBFE_MATCH_H
 #define ORBFE_MATCH_H
@@ -40,16 +49,13 @@ void orbfe_frame_scale_factors(float scale_factor, int nlevels, float *out);
  * Tcw[j] = CurrentFrame.mTcw as 3x4 row-major floats; fx..cy = Frame::fx.. (static camera intrinsics).
  * cur_mp_inout[j][i2] = index of the Last feature whose map point got assigned to Current feature i2, or -1
  * (entries >= 0 on input are treated as already-occupied slots, CurrentFrame.mvpMapPoints[i2] != NULL).
- * nmatches_out[j] = the method's return value. */
+ * nmatches_out[j] = the method's return value.  Pairs whose Current views share bounds, grid_inv_w/h, nlevels and
+ * scale_factors run in one launch.  ORBFE_ERR_ARG when a Last map point's octave is >= its Current view's nlevels. */
 int orbfe_search_by_projection_frames(OrbfeMatcher *m, int npairs, const OrbfeFrameView *cur,
                                       const OrbfeFrameView *last, const uint8_t *const *last_has_mp,
                                       const uint8_t *const *last_outlier, const float *const *last_world,
                                       const float *const *Tcw, float fx, float fy, float cx, float cy, float th,
                                       int check_orientation, int *const *cur_mp_inout, int *nmatches_out);
-
-/* Test / debugging hook: 1 = orbfe_search_by_projection_frames always takes the host-replay path (host candidate
- * lists + device distances + host greedy loop) instead of the fused device kernel.  Results are identical. */
-void orbfe_matcher_force_host_replay(int on);
 
 /* The same routine with EVERYTHING device-resident (no host round trip between extract and match):
  * d_kps / d_desc / d_counts are the outputs of orbfe_extract_batch_device (frame f at f*cap); pair j matches

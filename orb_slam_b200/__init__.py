@@ -40,7 +40,7 @@ ABI_SYMBOLS = [
     # include/orbfe_match.h
     "orbfe_frame_scale_factors", "orbfe_search_by_projection_frames", "orbfe_search_by_projection_device", "orbfe_guided_search_device",
     "orbfe_search_for_initialization_device", "orbfe_search_by_bow_device", "orbfe_search_for_triangulation_device",
-    "orbfe_matcher_force_host_replay", "orbfe_search_local_points", "orbfe_search_by_projection_kf",
+    "orbfe_search_local_points", "orbfe_search_by_projection_kf",
     "orbfe_search_by_projection_f1f2", "orbfe_search_by_bow", "orbfe_guided_search", "orbfe_guided_best", "orbfe_search_for_triangulation",
     "orbfe_window_search",
     "orbfe_search_for_initialization",

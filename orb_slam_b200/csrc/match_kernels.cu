@@ -141,7 +141,7 @@ void launch_knn2_groups(const uint8_t *q, int nq, const uint8_t *db, int ngroups
 //   C  the sequential accept loop, replayed by one warp over the precomputed (candidate, distance) lists:
 //      strict-< argmin over the candidates whose Current slot is still free, accept if <= TH_HIGH;
 //   D  rotation histogram + ComputeThreeMaxima (:1748-1789) and removal of the inconsistent matches.
-// Bit-exact with the host replay (orbfe_search_by_projection_frames) and with the oracle.
+// Bit-exact with the oracle; the only implementation of these rules (the host-array entries stage their inputs for it).
 // ================================================================================================
 namespace orbfe {
 
@@ -453,8 +453,8 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
     if (tid == 0) q_off[nl] = run_total;
     __syncthreads();
     const int T_total = run_total;
-    if (T_total > P.scratch_per_pair) {
-        if (tid == 0) { atomicExch(err, 1); nmatches[pair] = -1; }
+    if (T_total > P.scratch_per_pair) {   // err[1]: the most entries any overflowing job needed, for a relaunch that fits
+        if (tid == 0) { atomicExch(err, 1); atomicMax(err + 1, T_total); nmatches[pair] = -1; }
         publish_ack();
         return;
     }

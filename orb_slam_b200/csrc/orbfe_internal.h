@@ -7,6 +7,7 @@
 #include <stdint.h>
 
 #include "../../include/orbfe.h"
+#include "../../include/orbfe_match.h"
 
 #define ORBFE_EDGE 16  // EDGE_THRESHOLD, reference src/ORBextractor.cc:77
 
@@ -154,6 +155,22 @@ int launch_init_device(const SbpParams &P, size_t smem_bytes, int npairs, const 
 int launch_sbp_device(const SbpParams &P, size_t smem_bytes, int npairs, const OrbfeKeyPoint *kps, const uint8_t *desc,
                       const int *counts, const int *cur_idx, const int *last_idx, const float *world, const uint8_t *flags,
                       const float *Tcw, uint32_t *scratch, int *cur_mp, int *nmatches, int *err, cudaStream_t s);
+
+// One query window of the guided search: candidates = GetFeaturesInArea(u, v, r, lo, hi) of the searched frame; a match
+// writes `owner` into the frame's slot
+struct GuidedQuery { float u, v, r; int lo, hi; const uint8_t *desc; float angle; int owner; };
+
+// Host-array forms of the windowed matchers (orbfe_api.cu).  host/match_host.cpp checks the arguments and builds the
+// queries; these stage everything in the matcher's pinned block, run sbp_device_kernel, copy the results back and
+// synchronise.  The views' own bounds, grid_inv_w/h and scale_factors are what the kernel reads.
+int sbp_frames_host(OrbfeMatcher *m, int npairs, const OrbfeFrameView *cur, const OrbfeFrameView *last,
+                    const uint8_t *const *last_has_mp, const uint8_t *const *last_outlier, const float *const *last_world,
+                    const float *const *Tcw, float fx, float fy, float cx, float cy, float th, int check_orientation,
+                    int *const *cur_mp_inout, int *nmatches_out);
+int guided_host(OrbfeMatcher *m, const OrbfeFrameView &f, int nq, const GuidedQuery *Q, int rule, float nnratio, int th_dist,
+                int check_orientation, int *slot_owner, int *nmatches_out);
+int init_host(OrbfeMatcher *m, const OrbfeFrameView &f1, const OrbfeFrameView &f2, float *prev_matched, int window,
+              float nnratio, int check_orientation, int *match12_out, int *nmatches_out);
 
 // SearchByBoW for `njobs` (side 1, side 2) frame pairs (match_kernels.cu); out-of-range FeatureVector entries set bit 2 of *err
 int launch_search_by_bow(int variant, int njobs, const OrbfeKeyPoint *kps, const uint8_t *desc, const int *counts, int cap,

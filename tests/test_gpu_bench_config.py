@@ -119,19 +119,14 @@ def test_sbp_device_at_bench_config(stream, entry_placement, th, ori):
     m.close()
 
 
-@pytest.mark.parametrize("replay", [0, 1], ids=["fused-kernel", "host-replay"])
-def test_sbp_frames_at_bench_config(stream, entry_placement, replay):
+def test_sbp_frames_at_bench_config(stream, entry_placement):
     """orbfe_search_by_projection_frames (the call behind ORBmatcher::SearchByProjection(Frame&, const Frame&, float))
-    with host views, eight pairs per call, through the fused kernel and through the host-replay path."""
+    with host views, eight pairs per call."""
     kps, desc, shifts, has, outl, pre = stream
     views = [M.FrameView(kps[f], desc[f], W, H) for f in range(NFRAMES)]
     m = fe.ORBmatcher(0.9, True)
-    fe.lib().orbfe_matcher_force_host_replay(replay)
-    try:
-        nm, mp = M.search_by_projection_frames(m, views[1:], views[:-1], has[:-1], outl[:-1], [_world(kps[f]) for f in range(NFRAMES - 1)],
-                                               [_tcw(*shifts[j]) for j in range(1, NFRAMES)], FX, FY, CX, CY, 15.0, cur_mp=pre[1:])
-    finally:
-        fe.lib().orbfe_matcher_force_host_replay(0)
+    nm, mp = M.search_by_projection_frames(m, views[1:], views[:-1], has[:-1], outl[:-1], [_world(kps[f]) for f in range(NFRAMES - 1)],
+                                           [_tcw(*shifts[j]) for j in range(1, NFRAMES)], FX, FY, CX, CY, 15.0, cur_mp=pre[1:])
     ref = _oracle(stream, 15.0, True)
     for j in range(NFRAMES - 1):
         assert nm[j] == ref[j][0] and np.array_equal(mp[j], ref[j][1]), j

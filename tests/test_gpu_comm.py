@@ -79,15 +79,18 @@ def test_rig_exchange_and_sharded_sweep_world1(gpu_required):
     import sys, os
     sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools"))
     from multi_gpu import _as_tensor
+    # the gathered buffers are read on a torch stream: wait for the epoch and release it on that same stream
+    ts = torch.cuda.Stream(device=dev)
     for epoch in range(5):
         x.extract(ex, d_frames.data_ptr(), W, H, W, W * H)
-        x.wait()
+        x.wait(ts.cuda_stream)
         a, b, c = x.buffers()
-        gk = _as_tensor(torch, a, (T, nf, 28), dev).clone()
-        gd = _as_tensor(torch, b, (T, nf, 32), dev).clone()
-        gc = _as_tensor(torch, c, (T,), dev, torch.int32).clone()
-        x.release()
-        x.check()
+        with torch.cuda.stream(ts):
+            gk = _as_tensor(torch, a, (T, nf, 28), dev).clone()
+            gd = _as_tensor(torch, b, (T, nf, 32), dev).clone()
+            gc = _as_tensor(torch, c, (T,), dev, torch.int32).clone()
+        x.release(ts.cuda_stream)
+        x.check(ts.cuda_stream)
         assert torch.equal(gc, d_cnt) and torch.equal(gk, d_kps) and torch.equal(gd, d_desc), epoch
     assert x.bytes_pushed() == 0
     # the exchange-aware matcher call (waits for the epoch inside the kernel, releases it at its end) == the plain device call

@@ -1,5 +1,5 @@
-"""GPU parity of the windowed matchers (host candidate lists + device Hamming + host greedy replay, all through
-the C-ABI of liborbfe.so) against the oracle's restatement of ORBmatcher.cc / Frame.cc."""
+"""GPU parity of the matchers (the fused windowed kernel, the BoW kernels and the Hamming kernels, all through the C-ABI of
+liborbfe.so) against the oracle's restatement of ORBmatcher.cc / Frame.cc."""
 import numpy as np
 import pytest
 
@@ -44,15 +44,6 @@ def _world(k):
     return w
 
 
-@pytest.fixture(params=[0, 1], ids=["fused-kernel", "host-replay"])
-def guided_path(request):
-    """Both implementations behind the guided matchers: the fused device kernel (default) and the CSR-distance +
-    host-replay path it falls back to when a problem does not fit the kernel."""
-    fe.lib().orbfe_matcher_force_host_replay(request.param)
-    yield request.param
-    fe.lib().orbfe_matcher_force_host_replay(0)
-
-
 def test_search_by_projection_pairs(gpu_required):
     feats, shifts = _features(4)
     m = fe.ORBmatcher(0.9, True)
@@ -71,11 +62,6 @@ def test_search_by_projection_pairs(gpu_required):
         occ[rng.random(len(kc)) < 0.03] = 5  # a few already-occupied slots
         pre.append(occ)
     nm, mp = M.search_by_projection_frames(m, curs, lasts, has, outl, world, T, FX, FY, CX, CY, 15.0, cur_mp=pre)
-    # the same call through the host-replay path (host candidate lists + device distances + host greedy loop)
-    fe.lib().orbfe_matcher_force_host_replay(1)
-    nm_h, mp_h = M.search_by_projection_frames(m, curs, lasts, has, outl, world, T, FX, FY, CX, CY, 15.0, cur_mp=pre)
-    fe.lib().orbfe_matcher_force_host_replay(0)
-    assert np.array_equal(nm, nm_h) and all(np.array_equal(a, b) for a, b in zip(mp, mp_h))
     total = 0
     for j in range(3):
         fc = O.OracleFrame(curs[j].kps, curs[j].desc, W, H)
@@ -88,7 +74,7 @@ def test_search_by_projection_pairs(gpu_required):
     m.close()
 
 
-def test_window_search_and_initialization(gpu_required, guided_path):
+def test_window_search_and_initialization(gpu_required):
     feats, shifts = _features(2)
     (k1, d1), (k2, d2) = feats
     f1, f2 = M.FrameView(k1, d1, W, H), M.FrameView(k2, d2, W, H)
@@ -180,9 +166,9 @@ def test_device_resident_search_by_projection(gpu_required):
     m2.close()
 
 
-def test_local_points_reloc_and_f1f2_projection(gpu_required, guided_path):
+def test_local_points_reloc_and_f1f2_projection(gpu_required):
     """M3 (local-map points), M4 (Frame vs KeyFrame, relocalisation) and M6 (F1->F2 projection window): array-level
-    C-ABI against the oracle's restatement, through the fused kernel and through the host-replay path."""
+    C-ABI against the oracle's restatement."""
     feats, shifts = _features(2)
     (k1, d1), (k2, d2) = feats
     n1 = len(k1)
@@ -259,7 +245,7 @@ def test_search_by_bow_both_overloads(gpu_required):
             m.close()
 
 
-def test_guided_search_all_rules(gpu_required, guided_path):
+def test_guided_search_all_rules(gpu_required):
     """The exported guided-search skeleton (used by the KeyFrame-level facade methods) against the oracle, for every
     accept rule / histogram mode, with and without octave filters (KeyFrame::GetFeaturesInArea has none)."""
     feats, shifts = _features(2)

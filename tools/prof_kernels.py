@@ -24,6 +24,9 @@
   --what kfdb      the resident KeyFrameDatabase at 1k and 10k keyframes of ~1000 words (ids over 10^6): CUDA-event ms per loop
                    and per relocalisation query, host ms per add / erase, and the wall time of the stateless
                    orbfe_bow_db_detect on the same data
+  --what windowed  wall time per call of the host-array windowed matchers (staging, launch, copy back, synchronise):
+                   orbfe_search_by_projection_frames for 1 and 8 pairs, orbfe_search_local_points and orbfe_window_search at
+                   1080p / 2000 keypoints, orbfe_search_for_initialization at 720p / 2000 keypoints
 
 Prints one JSON object per --what; never a bench value when run under ncu."""
 import argparse
@@ -563,6 +566,61 @@ def matchers(args):
     return out
 
 
+def windowed(args):
+    """The host-array windowed matchers one call at a time, as ORB-SLAM's tracking thread calls them: median wall ms per call
+    over `--iters` x 10 calls after `--warmup` calls."""
+    import orb_slam_b200 as fe
+    from orb_slam_b200 import matching as M
+    from orb_slam_b200.synth import textured_frame, shifted_frame
+    NF = 2000
+    out = {}
+
+    def wall(fn):
+        for _ in range(args.warmup):
+            fn()
+        lat = []
+        for _ in range(args.iters * 10):
+            t0 = time.perf_counter()
+            fn()
+            lat.append((time.perf_counter() - t0) * 1e3)
+        return float(np.median(lat))
+    W, H, fx, cx, cy, depth = 1920, 1080, 1000.0, 960.0, 540.0, 5.0
+    f0 = textured_frame(W, H, seed=9)
+    frames = np.stack([f0] + [shifted_frame(f0, 3 * (i % 3) - 3, 2 * (i % 2) - 1, seed=i) for i in range(1, 9)])
+    ex = fe.ORBextractor(NF, 1.2, 8)
+    kps, desc, cnt = ex.extract_batch(frames)
+    ex.close()
+    views = [M.FrameView(kps[f, :cnt[f]], desc[f, :cnt[f]], W, H) for f in range(9)]
+    world = [np.stack([(kps[f]["x"] - cx) / fx * depth, (kps[f]["y"] - cy) / fx * depth, np.full(NF, depth)], 1).astype(np.float32)
+             for f in range(9)]
+    ones, zeros, T = np.ones(NF, np.uint8), np.zeros(NF, np.uint8), np.eye(3, 4, dtype=np.float32)
+    m = fe.ORBmatcher(0.9, True)
+    for npairs in (1, 8):
+        call = lambda: M.search_by_projection_frames(m, views[1:npairs + 1], views[:npairs], [ones] * npairs, [zeros] * npairs,
+                                                     world[:npairs], [T] * npairs, fx, fx, cx, cy, 15.0)
+        out["sbp_frames_%d_pairs_wall_ms" % npairs] = wall(call)
+        out["sbp_frames_%d_pairs_matches" % npairs] = int(call()[0].sum())
+    k0, k1 = kps[0, :cnt[0]], kps[1, :cnt[1]]
+    proj = np.stack([k0["x"], k0["y"]], 1).astype(np.float32)
+    call = lambda: M.search_local_points(m, views[1], ones[:len(k0)], proj, k0["octave"], np.full(len(k0), 0.999, np.float32),
+                                         desc[0, :cnt[0]], 1.0)
+    out["local_points_wall_ms"], out["local_points_matches"] = wall(call), call()[0]
+    call = lambda: M.window_search(m, views[0], views[1], ones[:len(k0)], 50)
+    out["window_search_wall_ms"], out["window_search_matches"] = wall(call), call()[0]
+    W2, H2 = 1280, 720
+    g0 = textured_frame(W2, H2, seed=40)
+    ex2 = fe.ORBextractor(NF, 1.2, 8)
+    k2, d2, c2 = ex2.extract_batch(np.stack([g0, shifted_frame(g0, 12, 4, seed=1)]))
+    ex2.close()
+    v1, v2 = M.FrameView(k2[0, :c2[0]], d2[0, :c2[0]], W2, H2), M.FrameView(k2[1, :c2[1]], d2[1, :c2[1]], W2, H2)
+    prev = np.stack([k2[0]["x"][:c2[0]], k2[0]["y"][:c2[0]]], 1).astype(np.float32)
+    call = lambda: M.search_for_initialization(m, v1, v2, prev, 100)
+    out["init_720p_wall_ms"], out["init_720p_matches"] = wall(call), call()[0]
+    m.close()
+    _gpu_and_power_limit(out)
+    return out
+
+
 def exchange1(args):
     """The exchange variant of the descriptor kernel with a world of ONE rank (its peer table holds only this GPU): what the
     remote-store code path, the acknowledgement poll and the publish cost by themselves, without NVLink or a second rank."""
@@ -850,4 +908,5 @@ if __name__ == "__main__":
     args = ap.parse_args()
     for w in args.what.split(","):
         print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fast": fast, "latency": latency,
-                          "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb}[w](args)))
+                          "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb,
+                          "windowed": windowed}[w](args)))
