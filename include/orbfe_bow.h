@@ -66,6 +66,19 @@ int orbfe_bow_transform(OrbfeVocabulary *v, const uint8_t *desc, int n, int leve
 int orbfe_feature_vector_device(OrbfeVocabulary *v, int nframes, const int32_t *d_leaf, const int32_t *d_node, const int *d_counts,
                                 int cap, int32_t *d_fv_ids, int32_t *d_fv_ptr, int32_t *d_fv_items, int *d_fv_n, void *stream);
 
+/* The BowVector half of transform() on the device, in the frame layout of orbfe_feature_vector_device: d_leaf holds what
+ * orbfe_bow_descend_device wrote (frame f at f*cap), frame f has min(max(d_counts[f], 0), cap) features.  Frame f receives
+ * the BowVector orbfe_bow_transform returns, bit for bit: d_bow_n[f] words, word ids d_bow_ids[f*cap + k] ascending and
+ * their values d_bow_vals[f*cap + k]; entries d_bow_n[f] .. cap-1 of the row hold id INT32_MAX and value 0.0, so a whole
+ * row can be passed to orbfe_kfdb_detect_device with nq = cap.  The same features are stopped as in the FeatureVector
+ * (weight not > 0, or a leaf id outside the vocabulary).  Values follow the vocabulary's weighting and norm: per word in
+ * feature order, TF / TF_IDF add every value, IDF / BINARY keep the first; without a norm TF / TF_IDF values are divided by
+ * the number of words; with one, the norm is a single sum in ascending word order.  One thread block per frame:
+ * cap <= ORBFE_FV_MAX_CAP, else ORBFE_ERR_UNSUPPORTED.  Arguments are checked before the handle is used.  Enqueued on
+ * `stream` (NULL = the vocabulary's stream), not synchronised. */
+int orbfe_bow_vector_device(OrbfeVocabulary *v, int nframes, const int32_t *d_leaf, const int *d_counts, int cap, int32_t *d_bow_ids,
+                            double *d_bow_vals, int *d_bow_n, void *stream);
+
 /* MapPoint::ComputeDistinctiveDescriptors for ngroups map points at once: group g owns the descriptors
  * desc[group_ptr[g] .. group_ptr[g+1]) (its observations, in the order of the reference's vDescriptors);
  * best_out[g] = index inside the group of the descriptor with the least median distance to the group
@@ -134,6 +147,16 @@ void orbfe_kfdb_destroy(OrbfeKeyFrameDB *db);
  * ORBFE_ERR_CAPACITY; in both cases the database is unchanged.  The covisibility list of the slot is left as it is.
  * Synchronous. */
 int orbfe_kfdb_add(OrbfeKeyFrameDB *db, int slot, int nw, const int32_t *ids, const double *vals);
+/* n calls of orbfe_kfdb_add, in order i, with the BowVectors read where orbfe_bow_vector_device left them: keyframe slots[i]
+ * gets the d_bow_n[f] words of row f = frames[i] of d_bow_ids / d_bow_vals (row f at f*cap).  slots and frames are host
+ * arrays; the rows are on the database's device and frame indices are not bounds-checked.  All or nothing: slots out of
+ * range, repeated or occupied, a negative frame, cap outside 1 .. ORBFE_FV_MAX_CAP, or a named row whose count is outside
+ * 0 .. cap or whose ids are not strictly ascending below the vocabulary's word count give ORBFE_ERR_ARG; more than
+ * max_postings words in the database gives ORBFE_ERR_CAPACITY; in every case the database is unchanged.  The rows are
+ * checked on the device and only their counts come back to the host.  Ordered after the work already on `stream`
+ * (NULL = the handle's stream); synchronous. */
+int orbfe_kfdb_add_device(OrbfeKeyFrameDB *db, int n, const int32_t *slots, const int32_t *frames, int cap, const int32_t *d_bow_ids,
+                          const double *d_bow_vals, const int *d_bow_n, void *stream);
 /* erase(pKF) (:47-66): the keyframe leaves every word's list, its postings become free for later adds, and its covisibility
  * list is emptied.  Erasing an empty slot does nothing, as in the reference.  Synchronous. */
 int orbfe_kfdb_erase(OrbfeKeyFrameDB *db, int slot);
@@ -158,8 +181,11 @@ int orbfe_kfdb_detect(OrbfeKeyFrameDB *db, int mode, int nq, const int32_t *q_id
                       float min_score, int cap, int32_t *cand_out, int *ncand_out, int32_t *words_out, float *score_out);
 /* The same query with device arrays: d_q_ids / d_q_vals / d_connected in, d_cand (cap entries), *d_ncand (the number of
  * candidates; when it exceeds cap only the first cap were written), d_words / d_score (max_keyframes entries each, may
- * be NULL) out.  Word ids out of the vocabulary's range are skipped.  Enqueued on `stream` (NULL = the handle's stream),
- * not synchronised: five kernels, no host round trip. */
+ * be NULL) out.  Word ids out of the vocabulary's range are skipped.  In particular, entries after the last real word whose
+ * id is >= the vocabulary's word count are ignored: a padded row of orbfe_bow_vector_device passed whole (nq = cap) gives
+ * the same candidates, words and scores, and leaves the same mLoopScore / mRelocScore, as its d_bow_n[f] real words, so
+ * the host never needs the word count.  Enqueued on `stream` (NULL = the handle's stream), not synchronised: five
+ * kernels, no host round trip. */
 int orbfe_kfdb_detect_device(OrbfeKeyFrameDB *db, int mode, int nq, const int32_t *d_q_ids, const double *d_q_vals, int nconn,
                              const int32_t *d_connected, float min_score, int cap, int32_t *d_cand, int *d_ncand, int32_t *d_words,
                              float *d_score, void *stream);

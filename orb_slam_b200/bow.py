@@ -30,6 +30,7 @@ def _bind():
     L.orbfe_distinctive_descriptors.argtypes = [vp, vp, vp, C.c_int, vp]
     L.orbfe_bow_db_detect.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, C.c_float, vp, vp, vp, vp]
     L.orbfe_feature_vector_device.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]
+    L.orbfe_bow_vector_device.argtypes = [vp, C.c_int, vp, vp, C.c_int, vp, vp, vp, vp]
     L.orbfe_distinctive_descriptors_device.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp]
     _bound = True
     return L
@@ -109,6 +110,16 @@ def feature_vector_device(voc: "Vocabulary", nframes, d_leaf, d_node, d_counts, 
                                                vp(d_fv_ptr), vp(d_fv_items), vp(d_fv_n), vp(stream)))
 
 
+def bow_vector_device(voc: "Vocabulary", nframes, d_leaf, d_counts, cap, d_bow_ids, d_bow_vals, d_bow_n, stream=0):
+    """BowVectors of `nframes` frames from the leaf ids Vocabulary.descend_device wrote (ints = raw device addresses; frame f
+    at f*cap, d_counts[f] features).  Outputs: word ids (nframes x cap, int32), values (nframes x cap, float64), word counts
+    (nframes); entries past a frame's word count hold id INT32_MAX and value 0.  Enqueued, not synchronised; see
+    include/orbfe_bow.h."""
+    vp = C.c_void_p
+    _check(_bind().orbfe_bow_vector_device(voc.handle, nframes, vp(d_leaf), vp(d_counts), cap, vp(d_bow_ids), vp(d_bow_vals), vp(d_bow_n),
+                                           vp(stream)))
+
+
 def distinctive_descriptors(matcher: ORBmatcher, desc, group_ptr):
     """Index (inside its group) of the least-median-distance descriptor of every group (map point)."""
     desc = np.ascontiguousarray(desc, np.uint8).reshape(-1, 32)
@@ -157,6 +168,7 @@ def _bind_kfdb():
     L.orbfe_kfdb_destroy.argtypes = [vp]
     L.orbfe_kfdb_destroy.restype = None
     L.orbfe_kfdb_add.argtypes = [vp, i, i, vp, vp]
+    L.orbfe_kfdb_add_device.argtypes = [vp, i, vp, vp, i, vp, vp, vp, vp]
     L.orbfe_kfdb_erase.argtypes = [vp, i]
     L.orbfe_kfdb_clear.argtypes = [vp]
     L.orbfe_kfdb_set_covisibles.argtypes = [vp, i, vp, vp, vp]
@@ -198,6 +210,16 @@ class KeyFrameDatabase:
     def add(self, slot, ids, vals):
         ids, vals = np.ascontiguousarray(ids, np.int32), np.ascontiguousarray(vals, np.float64)
         _check(_bind_kfdb().orbfe_kfdb_add(self._h, int(slot), len(ids), _p(ids), _p(vals)))
+
+    def add_device(self, slots, frames, cap, d_bow_ids, d_bow_vals, d_bow_n, stream=0):
+        """add() of keyframe slots[i] with the BowVector of row frames[i] that bow_vector_device wrote (ints = raw device
+        addresses, row f at f*cap), in order i; all or nothing, synchronous."""
+        slots, frames = np.ascontiguousarray(slots, np.int32), np.ascontiguousarray(frames, np.int32)
+        if len(slots) != len(frames):
+            raise ValueError("slots and frames differ in length")
+        vp = C.c_void_p
+        _check(_bind_kfdb().orbfe_kfdb_add_device(self._h, len(slots), _p(slots), _p(frames), int(cap), vp(d_bow_ids), vp(d_bow_vals),
+                                                  vp(d_bow_n), vp(stream)))
 
     def erase(self, slot):
         _check(_bind_kfdb().orbfe_kfdb_erase(self._h, int(slot)))

@@ -93,6 +93,38 @@ __global__ void kfdb_compact_kernel(const int *__restrict__ moves, int nmove, co
     }
 }
 
+// orbfe_kfdb_add_device: one block per named row (frame frames[r] of the caller's BowVector rows) gathers its word count into
+// info[1 + r] and raises info[0] when the count is outside [0, cap] or the ids are not strictly ascending in [0, nwords).
+__global__ void kfdb_check_rows_kernel(const int *__restrict__ frames, int n, int cap, int nwords, const int *__restrict__ bow_n,
+                                       const int *__restrict__ bow_ids, int *__restrict__ info) {
+    for (int r = blockIdx.x; r < n; r += gridDim.x) {
+        const size_t f = (size_t)frames[r];
+        const int c = bow_n[f];
+        if (threadIdx.x == 0) info[1 + r] = c;
+        const int *row = bow_ids + f * (size_t)cap;
+        bool bad = c < 0 || c > cap;
+        if (!bad)
+            for (int k = threadIdx.x; k < c; k += blockDim.x) {
+                const int w = row[k];
+                bad |= (unsigned)w >= (unsigned)nwords || (k > 0 && row[k - 1] >= w);
+            }
+        if (__syncthreads_or(bad) && threadIdx.x == 0) info[0] = 1;
+    }
+}
+
+// copy the rows (frame, store begin, length) of `n` keyframes from the caller's BowVector rows into the store
+__global__ void kfdb_gather_kernel(const int *__restrict__ rows, int n, int cap, const int *__restrict__ bow_ids,
+                                   const double *__restrict__ bow_vals, int *__restrict__ id1, double *__restrict__ val1) {
+    for (int m = blockIdx.x; m < n; m += gridDim.x) {
+        const size_t src = (size_t)rows[3 * m] * (size_t)cap;
+        const int nb = rows[3 * m + 1], len = rows[3 * m + 2];
+        for (int i = threadIdx.x; i < len; i += blockDim.x) {
+            id1[nb + i] = bow_ids[src + i];
+            val1[nb + i] = bow_vals[src + i];
+        }
+    }
+}
+
 __global__ void kfdb_covis_kernel(const int *__restrict__ rows, int n, int *__restrict__ covn, int *__restrict__ cov) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -330,6 +362,7 @@ struct OrbfeKeyFrameDB {
     int *n_slot = nullptr, *n_next = nullptr, *n_prev = nullptr, *w_head = nullptr, *w_tail = nullptr;
     int *range = nullptr, *covn = nullptr, *cov = nullptr, *touched = nullptr, *list = nullptr, *best = nullptr, *info = nullptr;
     int *moves = nullptr, *covrows = nullptr;
+    int *a_info = nullptr;        // add_device: [0] bad-row flag, [1 + i] word count of row i
     unsigned *seqs = nullptr, *conn = nullptr;
     unsigned long long *state = nullptr, *keys = nullptr, *firstpos = nullptr;
     float *lscore = nullptr, *rscore = nullptr, *lsc = nullptr, *acc = nullptr;
@@ -348,7 +381,7 @@ extern "C" void orbfe_kfdb_destroy(OrbfeKeyFrameDB *db) {
     void *ptrs[] = {db->s_id[0], db->s_id[1], db->s_node[0], db->s_node[1], db->s_val[0], db->s_val[1], db->n_slot, db->n_next, db->n_prev,
                     db->w_head, db->w_tail, db->range, db->covn, db->cov, db->touched, db->list, db->best, db->info, db->moves, db->covrows,
                     db->seqs, db->conn, db->state, db->keys, db->firstpos, db->lscore, db->rscore, db->lsc, db->acc, db->q_ids, db->q_conn,
-                    db->o_cand, db->o_words, db->o_n, db->q_vals, db->o_score};
+                    db->o_cand, db->o_words, db->o_n, db->q_vals, db->o_score, db->a_info};
     for (void *p : ptrs) cudaFree(p);
     if (db->last) cudaEventDestroy(db->last);
     if (db->stream) cudaStreamDestroy(db->stream);
@@ -397,6 +430,7 @@ extern "C" int orbfe_kfdb_create(OrbfeVocabulary *v, int max_keyframes, long lon
     KFDB_ALLOC(db->keys, S); KFDB_ALLOC(db->firstpos, K); KFDB_ALLOC(db->lscore, K); KFDB_ALLOC(db->rscore, K); KFDB_ALLOC(db->lsc, K);
     KFDB_ALLOC(db->acc, K); KFDB_ALLOC(db->q_ids, KFDB_MAX_NQ); KFDB_ALLOC(db->q_vals, KFDB_MAX_NQ); KFDB_ALLOC(db->q_conn, K);
     KFDB_ALLOC(db->o_cand, K); KFDB_ALLOC(db->o_words, K); KFDB_ALLOC(db->o_score, K); KFDB_ALLOC(db->o_n, 1);
+    KFDB_ALLOC(db->a_info, K + 1);
 #undef KFDB_ALLOC
     ok = ok && cudaMemset(db->conn, 0, sizeof(unsigned) * K) == cudaSuccess && cudaMemset(db->state, 0, sizeof(unsigned long long) * K) == cudaSuccess &&
          cudaMemset(db->firstpos, 0xFF, sizeof(unsigned long long) * K) == cudaSuccess;
@@ -486,6 +520,74 @@ extern "C" int orbfe_kfdb_add(OrbfeKeyFrameDB *db, int slot, int nw, const int32
     db->nodes[slot].swap(nodes);
     db->top += nw;
     db->live += nw;
+    return ORBFE_OK;
+}
+
+extern "C" int orbfe_kfdb_add_device(OrbfeKeyFrameDB *db, int n, const int32_t *slots, const int32_t *frames, int cap,
+                                     const int32_t *d_bow_ids, const double *d_bow_vals, const int *d_bow_n, void *stream) {
+    if (!db || n < 0 || cap < 1 || cap > ORBFE_FV_MAX_CAP)
+        return set_error(ORBFE_ERR_ARG, "bad arguments (n >= 0, 1 <= cap <= %d)", ORBFE_FV_MAX_CAP);
+    if (n > 0 && (!slots || !frames || !d_bow_ids || !d_bow_vals || !d_bow_n)) return set_error(ORBFE_ERR_ARG, "NULL argument");
+    for (int i = 0; i < n; i++)
+        if (slots[i] < 0 || frames[i] < 0) return set_error(ORBFE_ERR_ARG, "negative slot or frame at %d", i);
+    std::vector<int> sorted(slots, slots + n);
+    std::sort(sorted.begin(), sorted.end());
+    for (int i = 1; i < n; i++)
+        if (sorted[i] == sorted[i - 1]) return set_error(ORBFE_ERR_ARG, "slot %d listed twice", sorted[i]);
+    if (n == 0) return ORBFE_OK;
+    for (int i = 0; i < n; i++) {
+        if (slots[i] >= db->K) return set_error(ORBFE_ERR_ARG, "slot %d out of range (max_keyframes %d)", slots[i], db->K);
+        if (db->len[slots[i]] >= 0) return set_error(ORBFE_ERR_ARG, "slot %d is occupied", slots[i]);
+    }
+    // the rows are checked on the device, after the work that wrote them; their word counts are the one readback
+    cudaStream_t s = stream ? (cudaStream_t)stream : db->stream;
+    int rc = kfdb_enter(db, s);
+    if (rc) return rc;
+    KFDB_TRY(cudaMemcpyAsync(db->moves, frames, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, s));
+    KFDB_TRY(cudaMemsetAsync(db->a_info, 0, sizeof(int), s));
+    kfdb_check_rows_kernel<<<std::min(n, 1024), 256, 0, s>>>(db->moves, n, cap, db->nwords, d_bow_n, d_bow_ids, db->a_info);
+    KFDB_TRY(cudaGetLastError());
+    std::vector<int> info((size_t)n + 1);
+    KFDB_TRY(cudaMemcpyAsync(info.data(), db->a_info, sizeof(int) * info.size(), cudaMemcpyDeviceToHost, s));
+    KFDB_TRY(cudaStreamSynchronize(s));
+    if (info[0])
+        return set_error(ORBFE_ERR_ARG, "a BowVector row has a word count outside 0 .. %d, or word ids that are not strictly ascending below %d",
+                         cap, db->nwords);
+    long long total = 0;
+    for (int i = 0; i < n; i++) total += info[1 + i];
+    if (db->live + total > db->P)
+        return set_error(ORBFE_ERR_CAPACITY, "%lld postings + %lld exceed max_postings %lld", db->live, total, db->P);
+    // `s` has drained: the handle's earlier work and the rows are complete, the rest runs on the handle's stream
+    cudaStream_t hs = db->stream;
+    if (db->top + total > db->P && (rc = kfdb_compact(db))) return rc;
+    const int c = db->cur, top = (int)db->top;
+    std::vector<int> rows(3 * (size_t)n), nodes((size_t)total);
+    for (int i = 0, pos = 0; i < n; i++) {
+        rows[3 * i] = frames[i];
+        rows[3 * i + 1] = top + pos;
+        rows[3 * i + 2] = info[1 + i];
+        for (int k = 0; k < info[1 + i]; k++, pos++) { nodes[pos] = db->free_nodes.back(); db->free_nodes.pop_back(); }
+    }
+    KFDB_TRY(cudaMemcpyAsync(db->moves, rows.data(), sizeof(int) * rows.size(), cudaMemcpyHostToDevice, hs));
+    if (total > 0) KFDB_TRY(cudaMemcpyAsync(db->s_node[c] + top, nodes.data(), sizeof(int) * nodes.size(), cudaMemcpyHostToDevice, hs));
+    kfdb_gather_kernel<<<std::min(n, 1024), 256, 0, hs>>>(db->moves, n, cap, d_bow_ids, d_bow_vals, db->s_id[c], db->s_val[c]);
+    // one keyframe after the other: two keyframes may share a word, and every word's list is in add order
+    for (int i = 0; i < n; i++) {
+        const int nw = rows[3 * i + 2];
+        kfdb_link_kernel<<<(std::max(nw, 1) + 255) / 256, 256, 0, hs>>>(slots[i], rows[3 * i + 1], nw, ++db->seq, db->s_id[c], db->s_node[c],
+                                                                        db->n_slot, db->n_next, db->n_prev, db->w_head, db->w_tail,
+                                                                        db->range, db->seqs, db->state, db->lscore, db->rscore);
+    }
+    if ((rc = kfdb_leave(db, hs, true))) return rc;
+    for (int i = 0, pos = 0; i < n; i++) {
+        const int sl = slots[i], nw = rows[3 * i + 2];
+        db->begin[sl] = rows[3 * i + 1];
+        db->len[sl] = nw;
+        db->nodes[sl].assign(nodes.begin() + pos, nodes.begin() + pos + nw);
+        pos += nw;
+    }
+    db->top += total;
+    db->live += total;
     return ORBFE_OK;
 }
 

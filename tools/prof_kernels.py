@@ -24,6 +24,9 @@
   --what kfdb      the resident KeyFrameDatabase at 1k and 10k keyframes of ~1000 words (ids over 10^6): CUDA-event ms per loop
                    and per relocalisation query, host ms per add / erase, and the wall time of the stateless
                    orbfe_bow_db_detect on the same data
+  --what bowchain  the BowVector kernel alone for 1 and 33 1080p / 2000-keypoint frames (CUDA events), relocalisation from an
+                   extracted frame to SearchByBoW results against a resident 1000-keyframe database with the BowVector built
+                   on the device vs on the host (wall time), and detect_device on a padded row vs its word count
   --what windowed  wall time per call of the host-array windowed matchers (staging, launch, copy back, synchronise):
                    orbfe_search_by_projection_frames for 1 and 8 pairs, orbfe_search_local_points and orbfe_window_search at
                    1080p / 2000 keypoints, orbfe_search_for_initialization at 720p / 2000 keypoints
@@ -898,6 +901,160 @@ def kfdb(args):
     return out
 
 
+def bowchain(args):
+    """The BowVector built on the device (orbfe_bow_vector_device) and the relocalisation chain it completes, on 1920x1080
+    frames of 2000 keypoints with a k = 10, L = 6 vocabulary (TF-IDF, L1), levelsup 4:
+      bow_vector_{1,33}_frames_ms   CUDA-event ms of orbfe_bow_vector_device alone;
+      chain_{device,host}_wall_ms   one extracted frame (descriptors in HBM) to SearchByBoW results against a resident database
+                                    of 1000 keyframes (32 views of the place, added by orbfe_kfdb_add_device, and 968 unrelated
+                                    ones).  Device: descent, BowVector, FeatureVector, detect_device on the padded row, one
+                                    readback of the candidate count, search_by_bow_device.  Host: the path without the
+                                    BowVector kernel -- descent and FeatureVector on the device, descriptors D2H,
+                                    orbfe_bow_transform, BowVector H2D, detect_device, the same search;
+      detect_{padded,exact}_ms      CUDA-event ms of detect_device on frame 0's row with nq = cap and with nq = its word count."""
+    import torch
+    import orb_slam_b200 as fe
+    from orb_slam_b200 import matching as M, bow as BW
+    from orb_slam_b200.synth import textured_frame, shifted_frame, random_vocabulary
+    W, H, NF, levelsup, NREAL, NKF = 1920, 1080, 2000, 4, 32, 1000
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    s = stream.cuda_stream
+    base = textured_frame(W, H, seed=21)
+    # frame 0: the current frame; frames 1..32: keyframes of the same place
+    frames = np.stack([base] + [shifted_frame(base, 4 * (i % 5) - 8, 3 * (i % 3) - 3, seed=i) for i in range(1, NREAL + 1)])
+    F = len(frames)
+    voc = random_vocabulary(10, 6, seed=3)
+    V = BW.Vocabulary(voc)
+    ex = fe.ORBextractor(NF, 1.2, 8)
+    m = fe.ORBmatcher(0.75, True)
+    i32 = lambda *shape: torch.zeros(shape, dtype=torch.int32, device=dev)
+    d_frames = torch.from_numpy(frames).to(dev)
+    # the frame store has a frame per database slot (slot = frame index); the unrelated keyframes' frames are empty
+    d_kps = torch.zeros((NKF, NF, 28), dtype=torch.uint8, device=dev)
+    d_desc = torch.zeros((NKF, NF, 32), dtype=torch.uint8, device=dev)
+    d_valid = torch.ones((NKF, NF), dtype=torch.uint8, device=dev)
+    d_cnt, d_leaf, d_node = i32(NKF), i32(F * NF), i32(F * NF)
+    d_fid, d_fptr, d_fitems, d_fn = i32(NKF, NF), i32(NKF, NF + 1), i32(NKF, NF), i32(NKF)
+    d_bid, d_bn = i32(F, NF), i32(F)
+    d_bval = torch.zeros((F, NF), dtype=torch.float64, device=dev)
+    d_cand, d_nc, d_zero = i32(NKF), i32(1), i32(NKF)
+    d_out, d_nm = i32(NKF, NF), i32(NKF)
+    torch.cuda.synchronize()
+    ex.extract_batch_device(d_frames.data_ptr(), W, H, W, W * H, F, d_kps.data_ptr(), d_desc.data_ptr(), d_cnt.data_ptr(), s)
+    V.descend_device(d_desc.data_ptr(), F * NF, levelsup, d_leaf.data_ptr(), d_node.data_ptr(), s)
+    bowv = lambda nf: BW.bow_vector_device(V, nf, d_leaf.data_ptr(), d_cnt.data_ptr(), NF, d_bid.data_ptr(), d_bval.data_ptr(),
+                                           d_bn.data_ptr(), s)
+    fvec = lambda nf: BW.feature_vector_device(V, nf, d_leaf.data_ptr(), d_node.data_ptr(), d_cnt.data_ptr(), NF, d_fid.data_ptr(),
+                                               d_fptr.data_ptr(), d_fitems.data_ptr(), d_fn.data_ptr(), s)
+    bowv(F)
+    fvec(F)
+    stream.synchronize()
+
+    def timed(fn, iters=args.iters * 4, warm=args.warmup):
+        for _ in range(warm):
+            fn()
+        stream.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        for _ in range(iters):
+            fn()
+        e1.record(stream)
+        stream.synchronize()
+        return e0.elapsed_time(e1) / iters
+
+    out = {"what": "BowVector on the device and the relocalisation chain, 1920x1080 frames, %d keypoints, vocabulary k=10 L=6 "
+                   "TF-IDF L1, levelsup %d, %d keyframes in the database" % (NF, levelsup, NKF), "counts_min": int(d_cnt[:F].min().item())}
+    _gpu_and_power_limit(out)
+    out["bow_vector_1_frame_ms"] = timed(lambda: bowv(1), iters=200)
+    out["bow_vector_%d_frames_ms" % F] = timed(lambda: bowv(F), iters=200)
+    out["words_per_frame_mean"] = float(d_bn.float().mean().item())
+    # the sequential norm: the same launch on a vocabulary without a norm (TF, values divided by the word count)
+    Vt = BW.Vocabulary(voc, BW.TF, BW.NORM_NONE)
+    out["bow_vector_%d_frames_no_norm_ms" % F] = timed(lambda: BW.bow_vector_device(Vt, F, d_leaf.data_ptr(), d_cnt.data_ptr(), NF, d_bid.data_ptr(),
+                                                                                   d_bval.data_ptr(), d_bn.data_ptr(), s), iters=200)
+    Vt.close()
+
+    # the database: 968 unrelated keyframes (host adds of random BowVectors), then the 32 views of the place from the device rows
+    db = BW.KeyFrameDatabase(V, NKF, NKF * NF)
+    rng = np.random.default_rng(7)
+    nwords = int((voc["word_id"] >= 0).sum())
+    for k in range(NREAL + 1, NKF):
+        ids = np.unique(rng.integers(0, nwords, 1500)).astype(np.int32)
+        v = rng.uniform(0.2, 3.0, len(ids))
+        db.add(k, ids, v / v.sum())
+    bowv(F)
+    db.add_device(np.arange(1, NREAL + 1), np.arange(1, NREAL + 1), NF, d_bid.data_ptr(), d_bval.data_ptr(), d_bn.data_ptr(), s)
+    db.set_covisibles({k: [j for j in (k - 1, k + 1, k - 2, k + 2) if 1 <= j <= NREAL] for k in range(1, NREAL + 1)})
+    detect = lambda nq, qi, qv: db.detect_device(1, nq, qi, qv, 0, 0, 0.0, NKF, d_cand.data_ptr(), d_nc.data_ptr(), 0, 0, s)
+
+    def search(nc):
+        M.search_by_bow_device(m, 0, nc, d_kps.data_ptr(), d_desc.data_ptr(), d_cnt.data_ptr(), NF, d_fid.data_ptr(), d_fptr.data_ptr(),
+                               d_fitems.data_ptr(), d_fn.data_ptr(), d_valid.data_ptr(), d_cand.data_ptr(), d_zero.data_ptr(),
+                               d_out.data_ptr(), d_nm.data_ptr(), s)
+        stream.synchronize()
+
+    def chain_device():
+        V.descend_device(d_desc.data_ptr(), NF, levelsup, d_leaf.data_ptr(), d_node.data_ptr(), s)
+        bowv(1)
+        fvec(1)
+        detect(NF, d_bid.data_ptr(), d_bval.data_ptr())
+        nc = int(d_nc.item())
+        search(nc)
+        return nc
+
+    def chain_host():
+        V.descend_device(d_desc.data_ptr(), NF, levelsup, d_leaf.data_ptr(), d_node.data_ptr(), s)
+        fvec(1)
+        n0 = int(d_cnt[0].item())
+        (ids, vals), _ = V.transform(d_desc[0, :n0].cpu().numpy(), levelsup)
+        d_qi, d_qv = torch.from_numpy(ids).to(dev), torch.from_numpy(vals).to(dev)
+        detect(len(ids), d_qi.data_ptr(), d_qv.data_ptr())
+        nc = int(d_nc.item())
+        search(nc)
+        return nc, ids, vals
+
+    with torch.cuda.stream(stream):
+        # the two chains alternate, so that both see the same share of the host
+        chains = (("device", chain_device), ("host", chain_host))
+        lat = {tag: [] for tag, _ in chains}
+        for it in range(args.warmup + args.iters * 20):
+            for tag, fn in chains:
+                t0 = time.perf_counter()
+                fn()
+                if it >= args.warmup:
+                    lat[tag].append((time.perf_counter() - t0) * 1e3)
+        results = {}
+        for tag, fn in chains:
+            out["chain_%s_wall_ms" % tag] = float(np.median(lat[tag]))
+            out["chain_%s_wall_ms_p10_p90" % tag] = [float(np.percentile(lat[tag], 10)), float(np.percentile(lat[tag], 90))]
+            r = fn()
+            nc = r if tag == "device" else r[0]
+            results[tag] = (d_cand[:nc].cpu().numpy(), d_nm[:nc].cpu().numpy(), d_out[:nc].cpu().numpy())
+            if tag == "host":
+                ids, vals = r[1], r[2]
+        m.sync()
+        chain_device()
+        n0 = int(d_bn[0].item())
+        out["same_bow_vector"] = bool(np.array_equal(d_bid[0, :n0].cpu().numpy(), ids) and
+                                      np.array_equal(d_bval[0, :n0].cpu().numpy().view(np.uint64), vals.view(np.uint64)))
+    (cd, nd, od), (ch, nh, oh) = results["device"], results["host"]
+    out["candidates"] = cd.tolist()
+    out["matches"] = int(nd.sum())
+    out["same_as_host_chain"] = bool(np.array_equal(cd, ch) and np.array_equal(nd, nh) and np.array_equal(od, oh))
+    # padded and exact alternate over several windows of 100 queries each: the spread of each is reported beside it
+    det = {"padded": [], "exact": []}
+    for _ in range(6):
+        det["padded"].append(timed(lambda: detect(NF, d_bid.data_ptr(), d_bval.data_ptr()), iters=100))
+        det["exact"].append(timed(lambda: detect(n0, d_bid.data_ptr(), d_bval.data_ptr()), iters=100))
+    for tag, v in det.items():
+        out["detect_%s_ms" % tag] = float(np.median(v))
+        out["detect_%s_ms_min_max" % tag] = [float(min(v)), float(max(v))]
+    out["words_frame0"] = n0
+    db.close(); ex.close(); V.close(); m.close()
+    return out
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--what", default="config3,config5")
@@ -908,5 +1065,5 @@ if __name__ == "__main__":
     args = ap.parse_args()
     for w in args.what.split(","):
         print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fast": fast, "latency": latency,
-                          "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb,
+                          "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb, "bowchain": bowchain,
                           "windowed": windowed}[w](args)))
