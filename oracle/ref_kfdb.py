@@ -52,8 +52,8 @@ def lib():
         L.ref_kfdb_clear.restype = None
         L.ref_kfdb_set_covisibles.argtypes = [vp, i, vp, i]
         L.ref_kfdb_set_covisibles.restype = None
-        L.ref_kfdb_detect_loop.argtypes = [vp, vp, vp, i, vp, i, C.c_float, vp, i]
-        L.ref_kfdb_detect_reloc.argtypes = [vp, vp, vp, i, vp, i]
+        L.ref_kfdb_detect_loop.argtypes = [vp, vp, vp, i, vp, i, C.c_float, vp, i, vp, vp, vp]
+        L.ref_kfdb_detect_reloc.argtypes = [vp, vp, vp, i, vp, i, vp, vp, vp]
         _lib = L
     return _lib
 
@@ -64,12 +64,15 @@ def _p(a):
 
 class RefKeyFrameDatabase:
     """Every add() is a new reference KeyFrame; a slot names the keyframe last added to it.  detect() returns the candidate
-    slots (the reference's query fields are not read back: (cands, None, None))."""
+    slots and, per slot, the query fields mnLoopWords / mnRelocWords and mLoopScore / mRelocScore of the keyframe the query
+    touched there, -1 where it touched none.  The two arrays have max_keyframes entries (as oracle/kfdb.py's); without
+    max_keyframes, one entry per slot up to the highest slot added so far."""
 
-    def __init__(self, vocabulary_text_path):
+    def __init__(self, vocabulary_text_path, max_keyframes=None):
         self.L = lib()
         self.h = self.L.ref_kfdb_create(vocabulary_text_path.encode())
         assert self.h, "loadFromTextFile failed"
+        self.K = max_keyframes
         self.k_of, self.slot_of = {}, {}
 
     def add(self, slot, ids, vals):
@@ -92,11 +95,19 @@ class RefKeyFrameDatabase:
 
     def detect(self, mode, q_ids, q_vals, connected=(), min_score=0.0):
         qi, qv = np.ascontiguousarray(q_ids, np.int32), np.ascontiguousarray(q_vals, np.float64)
-        out = np.zeros(max(len(self.slot_of), 1), np.int32)
+        nk = max(len(self.slot_of), 1)
+        out, touched, kw, ks = np.zeros(nk, np.int32), np.zeros(nk, np.int32), np.zeros(nk, np.int32), np.zeros(nk, np.float32)
         if mode == 0:
             cn = np.ascontiguousarray([self.k_of[c] for c in connected] or [0], np.int32)
-            n = self.L.ref_kfdb_detect_loop(self.h, _p(qi), _p(qv), len(qi), _p(cn), len(connected), float(min_score), _p(out), len(out))
+            n = self.L.ref_kfdb_detect_loop(self.h, _p(qi), _p(qv), len(qi), _p(cn), len(connected), float(min_score), _p(out), len(out),
+                                            _p(touched), _p(kw), _p(ks))
         else:
-            n = self.L.ref_kfdb_detect_reloc(self.h, _p(qi), _p(qv), len(qi), _p(out), len(out))
+            n = self.L.ref_kfdb_detect_reloc(self.h, _p(qi), _p(qv), len(qi), _p(out), len(out), _p(touched), _p(kw), _p(ks))
         assert n <= len(out)
-        return np.array([self.slot_of[int(k)] for k in out[:n]], np.int32), None, None
+        K = self.K if self.K is not None else max(self.slot_of.values(), default=-1) + 1
+        words, scores = np.full(K, -1, np.int32), np.full(K, -1, np.float32)
+        for k in np.flatnonzero(touched[:len(self.slot_of)]):
+            s = self.slot_of[int(k)]
+            assert self.k_of.get(s) == k, "an erased keyframe was touched"
+            words[s], scores[s] = kw[k], ks[k]
+        return np.array([self.slot_of[int(k)] for k in out[:n]], np.int32), words, scores

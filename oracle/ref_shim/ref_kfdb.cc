@@ -63,6 +63,19 @@ int copy_out(KfDb *D, const std::vector<KeyFrame *> &c, int *out, int cap) {
     for (size_t i = 0; i < c.size() && (int)i < cap; i++) out[i] = index_of(D, c[i]);
     return (int)c.size();
 }
+
+// the query fields of every keyframe after a query: touched[k] = 1 where the query touched keyframe k, and then its
+// mnLoopWords / mnRelocWords and mLoopScore / mRelocScore (words -1 and score -1 elsewhere).  A connected keyframe of a
+// loop query is never stamped; it was touched when the walk overwrote the -1 its mnLoopWords was given before the call.
+void read_fields(KfDb *D, bool loop, long unsigned int qid, const std::set<KeyFrame *> &conn, int *touched, int *words, float *scores) {
+    for (size_t k = 0; k < D->kfs.size(); k++) {
+        const KeyFrame *kf = D->kfs[k];
+        const bool t = loop ? (kf->mnLoopQuery == qid || (conn.count(D->kfs[k]) && kf->mnLoopWords != -1)) : kf->mnRelocQuery == qid;
+        touched[k] = t;
+        words[k] = t ? (loop ? kf->mnLoopWords : kf->mnRelocWords) : -1;
+        scores[k] = t ? (loop ? kf->mLoopScore : kf->mRelocScore) : -1.f;
+    }
+}
 }  // namespace
 
 extern "C" {
@@ -101,21 +114,32 @@ void ref_kfdb_set_covisibles(void *h, int k, const int *others, int n) {
     for (int i = 0; i < n; i++) kf->AddConnection(D->kfs[others[i]], 1000 - i);
 }
 
-// DetectLoopCandidates(pKF, minScore) (:75-196) for a fresh query keyframe connected to `connected`
+// DetectLoopCandidates(pKF, minScore) (:75-196) for a fresh query keyframe connected to `connected`; touched / words /
+// scores (one entry per keyframe index) as read_fields.  The reference resets mnLoopWords at a keyframe's first visit of
+// a query and reads it only for keyframes this query stamped, so the -1 given to the connected keyframes changes nothing.
 int ref_kfdb_detect_loop(void *h, const int *q_ids, const double *q_vals, int nq, const int *connected, int nconn, float min_score,
-                         int *out, int cap) {
+                         int *out, int cap, int *touched, int *words, float *scores) {
     KfDb *D = static_cast<KfDb *>(h);
     KeyFrame *q = new_keyframe(D, q_ids, q_vals, nq);
-    for (int i = 0; i < nconn; i++) q->AddConnection(D->kfs[connected[i]], 100);
-    return copy_out(D, D->db->DetectLoopCandidates(q, min_score), out, cap);
+    std::set<KeyFrame *> conn;
+    for (int i = 0; i < nconn; i++) {
+        q->AddConnection(D->kfs[connected[i]], 100);
+        conn.insert(D->kfs[connected[i]]);
+        D->kfs[connected[i]]->mnLoopWords = -1;
+    }
+    const int n = copy_out(D, D->db->DetectLoopCandidates(q, min_score), out, cap);
+    read_fields(D, true, q->mnId, conn, touched, words, scores);
+    return n;
 }
 
-// DetectRelocalisationCandidates(Frame *F) (:198-308)
-int ref_kfdb_detect_reloc(void *h, const int *q_ids, const double *q_vals, int nq, int *out, int cap) {
+// DetectRelocalisationCandidates(Frame *F) (:198-308); touched / words / scores as read_fields
+int ref_kfdb_detect_reloc(void *h, const int *q_ids, const double *q_vals, int nq, int *out, int cap, int *touched, int *words,
+                          float *scores) {
     KfDb *D = static_cast<KfDb *>(h);
     Frame *F = bare_frame();
     F->mBowVec = bow_from(q_ids, q_vals, nq);
     const int n = copy_out(D, D->db->DetectRelocalisationCandidates(F), out, cap);
+    read_fields(D, false, F->mnId, std::set<KeyFrame *>(), touched, words, scores);
     ref_frame_free(F);
     return n;
 }
