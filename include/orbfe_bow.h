@@ -45,11 +45,20 @@ int orbfe_bow_descend_device(OrbfeVocabulary *v, const uint8_t *d_desc, int n, i
                              int32_t *d_node_out, void *stream);
 int orbfe_bow_descend(OrbfeVocabulary *v, const uint8_t *desc, int n, int levelsup, int32_t *leaf_out, int32_t *node_out);
 
-/* transform(features, BowVector&, FeatureVector&, levelsup) (TemplatedVocabulary.h:1126-1196): the descent on the
- * device, the two std::map builds restated on sorted arrays on the host.
+/* The host-array entries (orbfe_bow_descend, orbfe_bow_transform) are synchronous and may be called from several threads on
+ * one vocabulary, as DBoW2's const transform() is (Tracking and LocalMapping both compute BoW): they stage through one
+ * block of the vocabulary, one call at a time, on its stream.  The device-pointer entries take no lock. */
+
+/* transform(features, BowVector&, FeatureVector&, levelsup) (TemplatedVocabulary.h:1126-1196): the descent and both
+ * std::map builds on the device, as one frame of orbfe_bow_descend_device, orbfe_bow_vector_device and
+ * orbfe_feature_vector_device with cap = n.
  *   BowVector:     *nwords_out entries (word id ascending) in bow_ids / bow_vals            (capacity n each)
  *   FeatureVector: *nnodes_out entries (node id ascending) in fv_ids, rows fv_ptr[k]..fv_ptr[k+1] of fv_feats
- *                  (feature indices ascending; capacities n, n+1, n) -- the CSR form orbfe_search_by_bow takes. */
+ *                  (feature indices ascending; capacities n, n+1, n) -- the CSR form orbfe_search_by_bow takes.
+ * Nothing is written past bow_ids / bow_vals[*nwords_out - 1], fv_ids[*nnodes_out - 1], fv_ptr[*nnodes_out] and
+ * fv_feats[fv_ptr[*nnodes_out] - 1].  The two counts and fv_ptr[0] are set to 0 before any other work, so they stay 0 on a
+ * later error; n = 0 returns there without touching the handle.  n <= ORBFE_FV_MAX_CAP, else ORBFE_ERR_UNSUPPORTED (the
+ * kernels sort a frame's keys in shared memory). */
 int orbfe_bow_transform(OrbfeVocabulary *v, const uint8_t *desc, int n, int levelsup, int *nwords_out, int32_t *bow_ids,
                         double *bow_vals, int *nnodes_out, int32_t *fv_ids, int32_t *fv_ptr, int32_t *fv_feats);
 

@@ -1,12 +1,13 @@
 // bow_kernels.cu -- the two Hamming-primitive rows of SURVEY.md section 8(f):
 //   N2  DBoW2 vocabulary-tree descent (reference Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1216-1260, FORB.cpp:79-99)
 //   N4  MapPoint::ComputeDistinctiveDescriptors, batched (reference src/MapPoint.cc:185-250)
-// plus the device-side half of the C-ABI in include/orbfe_bow.h.  The std::map builds of transform() are restated twice:
-// on the host for the host-array orbfe_bow_transform (host/bow_host.cpp), and here for batches of frames in HBM
-// (feature_vector_kernel, bow_vector_kernel).  The descent is integer work only (XOR + POPC), bound by launch latency at
-// SLAM sizes (2000 descriptors x 6 levels x 10 children = 120 k distances per frame).
+// plus the vocabulary half of the C-ABI in include/orbfe_bow.h.  The std::map builds of transform() are stated once, for
+// batches of frames in HBM (feature_vector_kernel, bow_vector_kernel); the host-array orbfe_bow_transform runs them as a
+// batch of one frame.  The descent is integer work only (XOR + POPC), bound by launch latency at SLAM sizes
+// (2000 descriptors x 6 levels x 10 children = 120 k distances per frame).
 #include <algorithm>
 #include <cstring>
+#include <mutex>
 #include <vector>
 
 #include "../../include/orbfe_bow.h"
@@ -367,26 +368,25 @@ using namespace orbfe;
 
 struct OrbfeVocabulary {
     int device = 0, nnodes = 0, depth = 0, weighting = 0, norm = 0;
+    int nwords = 0;                 // largest word id + 1
     cudaStream_t stream = nullptr;
     uint8_t *d_desc = nullptr;
     uint8_t *d_live = nullptr;      // per node: weight > 0 (the FeatureVector skips stopped words)
     int *d_child_ptr = nullptr, *d_children = nullptr;
     int *d_word_id = nullptr;       // per node, for the BowVector kernel
     double *d_weight = nullptr;
-    std::vector<int32_t> word_id;   // per node, host side (leaf -> word)
-    std::vector<double> weight;
-    // grow-only staging of the host-pointer entry point
-    uint8_t *d_in = nullptr;
-    int *d_out = nullptr;
-    size_t in_cap = 0, out_cap = 0;
+    // the host-array entries stage through `stage` on `stream`, one call at a time
+    std::mutex mu;
+    Stage stage;
 };
 
 extern "C" void orbfe_vocabulary_destroy(OrbfeVocabulary *v) {
     if (!v) return;
     cudaSetDevice(v->device);
     if (v->stream) cudaStreamDestroy(v->stream);
-    cudaFree(v->d_desc); cudaFree(v->d_live); cudaFree(v->d_child_ptr); cudaFree(v->d_children); cudaFree(v->d_in); cudaFree(v->d_out);
+    cudaFree(v->d_desc); cudaFree(v->d_live); cudaFree(v->d_child_ptr); cudaFree(v->d_children);
     cudaFree(v->d_word_id); cudaFree(v->d_weight);
+    v->stage.release();
     delete v;
 }
 
@@ -413,10 +413,11 @@ extern "C" OrbfeVocabulary *orbfe_vocabulary_create(int device, int nnodes, int 
     if (device < 0 || device >= ndev) { set_error(ORBFE_ERR_ARG, "device %d out of range", device); return nullptr; }
     OrbfeVocabulary *v = new OrbfeVocabulary();
     v->device = device; v->nnodes = nnodes; v->depth = depth_L; v->weighting = weighting; v->norm = norm;
-    v->word_id.assign(word_id, word_id + nnodes);
-    v->weight.assign(weight, weight + nnodes);
     std::vector<uint8_t> live(nnodes);
-    for (int i = 0; i < nnodes; i++) live[i] = weight[i] > 0 ? 1 : 0;
+    for (int i = 0; i < nnodes; i++) {
+        live[i] = weight[i] > 0 ? 1 : 0;
+        v->nwords = std::max(v->nwords, word_id[i] + 1);
+    }
     bool ok = cudaSetDevice(device) == cudaSuccess && cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking) == cudaSuccess &&
               cudaMalloc((void **)&v->d_desc, (size_t)nnodes * 32) == cudaSuccess &&
               cudaMalloc((void **)&v->d_live, (size_t)nnodes) == cudaSuccess &&
@@ -493,38 +494,77 @@ extern "C" int orbfe_bow_descend(OrbfeVocabulary *v, const uint8_t *desc, int n,
     if (!v || n < 0) return set_error(ORBFE_ERR_ARG, "bad arguments");
     if (n == 0) return ORBFE_OK;
     if (!desc || !leaf_out || !node_out) return set_error(ORBFE_ERR_ARG, "NULL argument");
+    const size_t N = (size_t)n;
+    std::lock_guard<std::mutex> lock(v->mu);
     BOW_TRY(cudaSetDevice(v->device));
-    if (v->in_cap < (size_t)n * 32) {
-        cudaFree(v->d_in); v->d_in = nullptr; v->in_cap = 0;
-        BOW_TRY(cudaMalloc((void **)&v->d_in, (size_t)n * 32 * 2));
-        v->in_cap = (size_t)n * 32 * 2;
-    }
-    if (v->out_cap < (size_t)n * 2) {
-        cudaFree(v->d_out); v->d_out = nullptr; v->out_cap = 0;
-        BOW_TRY(cudaMalloc((void **)&v->d_out, sizeof(int) * (size_t)n * 4));
-        v->out_cap = (size_t)n * 4;
-    }
-    BOW_TRY(cudaMemcpyAsync(v->d_in, desc, (size_t)n * 32, cudaMemcpyHostToDevice, v->stream));
-    int rc = orbfe_bow_descend_device(v, v->d_in, n, levelsup, v->d_out, v->d_out + n, v->stream);
-    if (rc) return rc;
-    BOW_TRY(cudaMemcpyAsync(leaf_out, v->d_out, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, v->stream));
-    BOW_TRY(cudaMemcpyAsync(node_out, v->d_out + n, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, v->stream));
+    size_t o_desc, o_leaf, o_node, total;
+    if (int rc = v->stage.layout({{&o_desc, N * 32}, {&o_leaf, N * 4}, {&o_node, N * 4}}, &total)) return rc;
+    unsigned char *H = v->stage.h, *D = v->stage.d;
+    memcpy(H + o_desc, desc, N * 32);
+    BOW_TRY(cudaMemcpyAsync(D, H, o_leaf, cudaMemcpyHostToDevice, v->stream));
+    if (int rc = orbfe_bow_descend_device(v, D + o_desc, n, levelsup, (int32_t *)(D + o_leaf), (int32_t *)(D + o_node), v->stream))
+        return rc;
+    BOW_TRY(cudaMemcpyAsync(H + o_leaf, D + o_leaf, total - o_leaf, cudaMemcpyDeviceToHost, v->stream));
     BOW_TRY(cudaStreamSynchronize(v->stream));
+    memcpy(leaf_out, H + o_leaf, N * 4);
+    memcpy(node_out, H + o_node, N * 4);
     return ORBFE_OK;
 }
 
-// accessors for host/bow_host.cpp (the struct layout stays private to this file)
-namespace orbfe {
-const int32_t *vocab_word_ids(const OrbfeVocabulary *v) { return v->word_id.data(); }
-const double *vocab_weights(const OrbfeVocabulary *v) { return v->weight.data(); }
-void vocab_modes(const OrbfeVocabulary *v, int *weighting, int *norm) { *weighting = v->weighting; *norm = v->norm; }
-// for kfdb.cu: the device of the node table, and the number of words (largest word id + 1)
-int vocab_device(const OrbfeVocabulary *v) { return v->device; }
-int vocab_nwords(const OrbfeVocabulary *v) {
-    int n = 0;
-    for (int32_t w : v->word_id) n = std::max(n, w + 1);
-    return n;
+// The host-array transform is one frame of the device entries, cap = n: the descriptors and the frame's count go up in one
+// H2D, descent, BowVector and FeatureVector run on the vocabulary's stream, their rows come back in one D2H.
+extern "C" int orbfe_bow_transform(OrbfeVocabulary *v, const uint8_t *desc, int n, int levelsup, int *nwords_out, int32_t *bow_ids,
+                                   double *bow_vals, int *nnodes_out, int32_t *fv_ids, int32_t *fv_ptr, int32_t *fv_feats) {
+    if (!v || n < 0 || !nwords_out || !nnodes_out || !fv_ptr) return set_error(ORBFE_ERR_ARG, "bad arguments");
+    *nwords_out = 0;
+    *nnodes_out = 0;
+    fv_ptr[0] = 0;
+    if (n == 0) return ORBFE_OK;
+    if (!desc || !bow_ids || !bow_vals || !fv_ids || !fv_feats) return set_error(ORBFE_ERR_ARG, "NULL argument");
+    if (n > ORBFE_FV_MAX_CAP)
+        return set_error(ORBFE_ERR_UNSUPPORTED, "%d descriptors exceed the %d features per frame the BowVector and FeatureVector "
+                                                "kernels sort in shared memory", n, ORBFE_FV_MAX_CAP);
+    const size_t N = (size_t)n;
+    std::lock_guard<std::mutex> lock(v->mu);
+    BOW_TRY(cudaSetDevice(v->device));
+    size_t o_desc, o_cnt, o_leaf, o_node, o_bid, o_bval, o_bn, o_fid, o_fptr, o_fitem, o_fn, total;
+    if (int rc = v->stage.layout({{&o_desc, N * 32}, {&o_cnt, sizeof(int)}, {&o_leaf, N * 4}, {&o_node, N * 4}, {&o_bid, N * 4},
+                                  {&o_bval, N * 8}, {&o_bn, sizeof(int)}, {&o_fid, N * 4}, {&o_fptr, (N + 1) * 4}, {&o_fitem, N * 4},
+                                  {&o_fn, sizeof(int)}},
+                                 &total))
+        return rc;
+    unsigned char *H = v->stage.h, *D = v->stage.d;
+    memcpy(H + o_desc, desc, N * 32);
+    *(int *)(H + o_cnt) = n;
+    cudaStream_t s = v->stream;
+    BOW_TRY(cudaMemcpyAsync(D, H, o_leaf, cudaMemcpyHostToDevice, s));
+    const int *d_cnt = (const int *)(D + o_cnt);
+    int32_t *d_leaf = (int32_t *)(D + o_leaf), *d_node = (int32_t *)(D + o_node);
+    int rc = orbfe_bow_descend_device(v, D + o_desc, n, levelsup, d_leaf, d_node, s);
+    if (!rc) rc = orbfe_bow_vector_device(v, 1, d_leaf, d_cnt, n, (int32_t *)(D + o_bid), (double *)(D + o_bval), (int *)(D + o_bn), s);
+    if (!rc)
+        rc = orbfe_feature_vector_device(v, 1, d_leaf, d_node, d_cnt, n, (int32_t *)(D + o_fid), (int32_t *)(D + o_fptr),
+                                         (int32_t *)(D + o_fitem), (int *)(D + o_fn), s);
+    if (rc) return rc;
+    BOW_TRY(cudaMemcpyAsync(H + o_bid, D + o_bid, total - o_bid, cudaMemcpyDeviceToHost, s));
+    BOW_TRY(cudaStreamSynchronize(s));
+    // exactly the entries DBoW2's maps hold: the rows' padding stays in the block
+    const int nw = *(const int *)(H + o_bn), nn = *(const int *)(H + o_fn);
+    const int32_t *ptr = (const int32_t *)(H + o_fptr);
+    memcpy(bow_ids, H + o_bid, (size_t)nw * 4);
+    memcpy(bow_vals, H + o_bval, (size_t)nw * 8);
+    memcpy(fv_ids, H + o_fid, (size_t)nn * 4);
+    memcpy(fv_ptr, ptr, ((size_t)nn + 1) * 4);
+    memcpy(fv_feats, H + o_fitem, (size_t)ptr[nn] * 4);
+    *nwords_out = nw;
+    *nnodes_out = nn;
+    return ORBFE_OK;
 }
+
+// for kfdb.cu: the device of the node table, and the number of words
+namespace orbfe {
+int vocab_device(const OrbfeVocabulary *v) { return v->device; }
+int vocab_nwords(const OrbfeVocabulary *v) { return v->nwords; }
 
 void launch_distinctive(const uint8_t *d_desc, const int *d_group_ptr, int ngroups, int *d_best, cudaStream_t s) {
     if (ngroups <= 0) return;

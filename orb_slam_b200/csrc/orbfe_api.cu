@@ -845,10 +845,7 @@ struct OrbfeMatcher {
     size_t scratch_entries = 0;
     int *d_err = nullptr;  // [0]: error flags of the last launches; [1]: candidate entries an overflowing fused-matcher job needed
     int *h_err = nullptr;  // pinned
-    // staging of the host-array entries that run on a device kernel
-    unsigned char *h_stage = nullptr;  // pinned
-    unsigned char *d_stage = nullptr;
-    size_t stage_cap = 0;
+    Stage stage;           // the host-array entries that run on a device kernel
 };
 
 // Dynamic shared memory of the fused matcher (one thread block per pair / job).  What is left after the fixed arrays
@@ -907,8 +904,7 @@ extern "C" int orbfe_matcher_destroy(OrbfeMatcher *m) {
     if (m->stream) cudaStreamSynchronize(m->stream);
     for (int i = 0; i < 6; i++) if (m->buf[i]) cudaFree(m->buf[i]);
     if (m->scratch) cudaFree(m->scratch);
-    if (m->h_stage) cudaFreeHost(m->h_stage);
-    if (m->d_stage) cudaFree(m->d_stage);
+    m->stage.release();
     if (m->d_err) cudaFree(m->d_err);
     if (m->h_err) cudaFreeHost(m->h_err);
     if (m->stream) cudaStreamDestroy(m->stream);
@@ -1093,26 +1089,27 @@ extern "C" int orbfe_guided_search_device(OrbfeMatcher *m, int njobs, const Orbf
                                                 stream ? (cudaStream_t)stream : m->stream));
 }
 
-// Staging block of the host-array entries that run on a device kernel: places arrays of `second` bytes at 256-byte aligned
-// offsets (*first), sets *total to the block's size and grows the pinned host block h_stage and its device twin d_stage to
-// hold it.  The caller packs h_stage, copies it to d_stage in one H2D and synchronises before it returns.
-static int stage_layout(OrbfeMatcher *m, std::initializer_list<std::pair<size_t *, size_t>> arrays, size_t *total) {
+int orbfe::Stage::layout(std::initializer_list<std::pair<size_t *, size_t>> arrays, size_t *total) {
     size_t off = 0;
     for (const auto &a : arrays) {
         *a.first = off;
         off += (a.second + 255) / 256 * 256;
     }
     *total = off;
-    if (m->stage_cap < off) {
-        if (m->h_stage) cudaFreeHost(m->h_stage);
-        if (m->d_stage) cudaFree(m->d_stage);
-        m->h_stage = nullptr; m->d_stage = nullptr; m->stage_cap = 0;
+    if (cap < off) {
+        release();
         const size_t want = off + off / 4;
-        CU_TRY(cudaHostAlloc((void **)&m->h_stage, want, cudaHostAllocDefault));
-        CU_TRY(cudaMalloc((void **)&m->d_stage, want));
-        m->stage_cap = want;
+        CU_TRY(cudaHostAlloc((void **)&h, want, cudaHostAllocDefault));
+        CU_TRY(cudaMalloc((void **)&d, want));
+        cap = want;
     }
     return ORBFE_OK;
+}
+
+void orbfe::Stage::release() {
+    if (h) cudaFreeHost(h);
+    if (d) cudaFree(d);
+    h = nullptr; d = nullptr; cap = 0;
 }
 
 // SearchByBoW (both overloads) for `njobs` frame pairs, device-resident (include/orbfe_match.h).  Arguments are checked before
@@ -1153,12 +1150,12 @@ extern "C" int orbfe_search_by_bow(OrbfeMatcher *m, int variant, int n1, const u
     CU_TRY(cudaSetDevice(m->device));
     const size_t C = (size_t)cap;
     size_t o_kps, o_desc, o_cnt, o_ids, o_ptr, o_items, o_nn, o_valid, o_idx, o_out, o_nm, total;
-    if (int rc = stage_layout(m, {{&o_kps, 2 * C * sizeof(OrbfeKeyPoint)}, {&o_desc, 2 * C * 32}, {&o_cnt, 2 * sizeof(int)},
+    if (int rc = m->stage.layout({{&o_kps, 2 * C * sizeof(OrbfeKeyPoint)}, {&o_desc, 2 * C * 32}, {&o_cnt, 2 * sizeof(int)},
                                   {&o_ids, 2 * C * 4}, {&o_ptr, 2 * (C + 1) * 4}, {&o_items, 2 * C * 4}, {&o_nn, 2 * sizeof(int)},
                                   {&o_valid, 2 * C}, {&o_idx, 2 * sizeof(int)}, {&o_out, C * 4}, {&o_nm, sizeof(int)}},
                               &total))
         return rc;
-    unsigned char *H = m->h_stage, *D = m->d_stage;
+    unsigned char *H = m->stage.h, *D = m->stage.d;
     const int n[2] = {n1, n2}, nn[2] = {nn1, nn2};
     const uint8_t *desc[2] = {desc1, desc2}, *valid[2] = {valid1, variant == 1 ? valid2 : nullptr};
     const float *angle[2] = {angle1, angle2};
@@ -1247,13 +1244,13 @@ extern "C" int orbfe_search_for_triangulation(OrbfeMatcher *m, int n1, const Orb
     CU_TRY(cudaSetDevice(m->device));
     const size_t C = (size_t)cap;
     size_t o_kps, o_desc, o_cnt, o_ids, o_ptr, o_items, o_nn, o_has, o_idx, o_F, o_out, o_nm, total;
-    if (int rc = stage_layout(m, {{&o_kps, 2 * C * sizeof(OrbfeKeyPoint)}, {&o_desc, 2 * C * 32}, {&o_cnt, 2 * sizeof(int)},
+    if (int rc = m->stage.layout({{&o_kps, 2 * C * sizeof(OrbfeKeyPoint)}, {&o_desc, 2 * C * 32}, {&o_cnt, 2 * sizeof(int)},
                                   {&o_ids, 2 * C * 4}, {&o_ptr, 2 * (C + 1) * 4}, {&o_items, 2 * C * 4}, {&o_nn, 2 * sizeof(int)},
                                   {&o_has, 2 * C}, {&o_idx, 2 * sizeof(int)}, {&o_F, 9 * sizeof(float)}, {&o_out, C * 4},
                                   {&o_nm, sizeof(int)}},
                               &total))
         return rc;
-    unsigned char *H = m->h_stage, *D = m->d_stage;
+    unsigned char *H = m->stage.h, *D = m->stage.d;
     const int n[2] = {n1, n2}, nn[2] = {nn1, nn2};
     const OrbfeKeyPoint *keys[2] = {keys1, keys2};
     const uint8_t *desc[2] = {desc1, desc2}, *has_mp[2] = {has_mp1, has_mp2};
@@ -1557,9 +1554,9 @@ static int run_staged(OrbfeMatcher *m, size_t inout, size_t out, size_t total, s
     cudaStream_t s = m->stream;
     for (bool grown = false;; grown = true) {
         pack_inout();
-        CU_TRY(cudaMemcpyAsync(m->d_stage, m->h_stage, out, cudaMemcpyHostToDevice, s));
+        CU_TRY(cudaMemcpyAsync(m->stage.d, m->stage.h, out, cudaMemcpyHostToDevice, s));
         if (int rc = launch(per_job)) return rc;
-        CU_TRY(cudaMemcpyAsync(m->h_stage + inout, m->d_stage + inout, total - inout, cudaMemcpyDeviceToHost, s));
+        CU_TRY(cudaMemcpyAsync(m->stage.h + inout, m->stage.d + inout, total - inout, cudaMemcpyDeviceToHost, s));
         const int rc = orbfe_matcher_sync(m);
         m->h2d_bytes += out;
         m->d2h_bytes += total - inout;
@@ -1633,14 +1630,14 @@ int orbfe::sbp_frames_host(OrbfeMatcher *m, int npairs, const OrbfeFrameView *cu
     }
     const size_t nf = slots.size();
     size_t o_kps, o_desc, o_cnt, o_world, o_flags, o_T, o_ci, o_li, o_mp, o_nm, total;
-    if (int rc = stage_layout(m, {{&o_kps, nf * cap * sizeof(OrbfeKeyPoint)}, {&o_desc, nf * cap * 32}, {&o_cnt, nf * sizeof(int)},
+    if (int rc = m->stage.layout({{&o_kps, nf * cap * sizeof(OrbfeKeyPoint)}, {&o_desc, nf * cap * 32}, {&o_cnt, nf * sizeof(int)},
                                   {&o_world, nf * cap * 3 * sizeof(float)}, {&o_flags, nf * cap},
                                   {&o_T, (size_t)npairs * 12 * sizeof(float)}, {&o_ci, (size_t)npairs * sizeof(int)},
                                   {&o_li, (size_t)npairs * sizeof(int)}, {&o_mp, (size_t)npairs * cap * sizeof(int)},
                                   {&o_nm, (size_t)npairs * sizeof(int)}},
                               &total))
         return rc;
-    unsigned char *H = m->h_stage, *D = m->d_stage;
+    unsigned char *H = m->stage.h, *D = m->stage.d;
     int *h_cnt = (int *)(H + o_cnt), *h_ci = (int *)(H + o_ci), *h_li = (int *)(H + o_li);
     auto pack_slot = [&](int sidx) {
         const Slot &S = slots[sidx];
@@ -1715,14 +1712,14 @@ int orbfe::guided_host(OrbfeMatcher *m, const OrbfeFrameView &f, int nq, const G
     const int cap = f.n;
     CU_TRY(cudaSetDevice(m->device));
     size_t o_kps, o_desc, o_cnt, o_fi, o_qb, o_qc, o_qu, o_qv, o_qr, o_qa, o_lo, o_hi, o_qd, o_mp, o_nm, total;
-    if (int rc = stage_layout(m, {{&o_kps, (size_t)cap * sizeof(OrbfeKeyPoint)}, {&o_desc, (size_t)cap * 32}, {&o_cnt, sizeof(int)},
+    if (int rc = m->stage.layout({{&o_kps, (size_t)cap * sizeof(OrbfeKeyPoint)}, {&o_desc, (size_t)cap * 32}, {&o_cnt, sizeof(int)},
                                   {&o_fi, sizeof(int)}, {&o_qb, sizeof(int)}, {&o_qc, sizeof(int)}, {&o_qu, (size_t)nq * 4},
                                   {&o_qv, (size_t)nq * 4}, {&o_qr, (size_t)nq * 4}, {&o_qa, (size_t)nq * 4}, {&o_lo, (size_t)nq * 4},
                                   {&o_hi, (size_t)nq * 4}, {&o_qd, (size_t)nq * 32}, {&o_mp, (size_t)cap * sizeof(int)},
                                   {&o_nm, sizeof(int)}},
                               &total))
         return rc;
-    unsigned char *H = m->h_stage, *D = m->d_stage;
+    unsigned char *H = m->stage.h, *D = m->stage.d;
     memcpy(H + o_kps, f.keys_un, (size_t)cap * sizeof(OrbfeKeyPoint));
     memcpy(H + o_desc, f.desc, (size_t)cap * 32);
     *(int *)(H + o_cnt) = cap; *(int *)(H + o_fi) = 0; *(int *)(H + o_qb) = 0; *(int *)(H + o_qc) = nq;
@@ -1763,12 +1760,12 @@ int orbfe::init_host(OrbfeMatcher *m, const OrbfeFrameView &f1, const OrbfeFrame
     const size_t C = (size_t)cap;
     CU_TRY(cudaSetDevice(m->device));
     size_t o_kps, o_desc, o_cnt, o_idx, o_prev, o_m12, o_nm, total;
-    if (int rc = stage_layout(m, {{&o_kps, 2 * C * sizeof(OrbfeKeyPoint)}, {&o_desc, 2 * C * 32}, {&o_cnt, 2 * sizeof(int)},
+    if (int rc = m->stage.layout({{&o_kps, 2 * C * sizeof(OrbfeKeyPoint)}, {&o_desc, 2 * C * 32}, {&o_cnt, 2 * sizeof(int)},
                                   {&o_idx, 2 * sizeof(int)}, {&o_prev, C * 2 * sizeof(float)}, {&o_m12, C * sizeof(int)},
                                   {&o_nm, sizeof(int)}},
                               &total))
         return rc;
-    unsigned char *H = m->h_stage, *D = m->d_stage;
+    unsigned char *H = m->stage.h, *D = m->stage.d;
     const OrbfeFrameView *v[2] = {&f1, &f2};
     for (int f = 0; f < 2; f++) {
         ((int *)(H + o_cnt))[f] = v[f]->n;

@@ -6,6 +6,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <initializer_list>
+#include <utility>
+
 #include "../../include/orbfe.h"
 #include "../../include/orbfe_match.h"
 
@@ -190,6 +193,19 @@ void launch_undistort(float fx, float fy, float cx, float cy, const float *dist5
 
 // records the thread's last-error string (orbfe_last_error) and returns `code`
 int set_error(int code, const char *fmt, ...);
+
+// Staging block of the host-array entries that run on a device kernel (orbfe_api.cu): a grow-only pinned host block h and
+// its device twin d.  The entry packs h, copies it to d in one H2D, runs its kernels, copies the results back in one D2H and
+// synchronises before it returns.  The block serves one call at a time: the vocabulary holds its mutex across each call.
+struct Stage {
+    unsigned char *h = nullptr;
+    unsigned char *d = nullptr;
+    size_t cap = 0;
+    // places arrays of `second` bytes at 256-byte aligned offsets (*first), sets *total to the block's size and grows the
+    // block to hold it (ORBFE_ERR_CUDA on a failed allocation)
+    int layout(std::initializer_list<std::pair<size_t *, size_t>> arrays, size_t *total);
+    void release();
+};
 
 // ---- launchers (match_kernels.cu) ----
 void launch_hamming_csr(const uint8_t *q, const uint8_t *t, const int32_t *row_ptr, const int32_t *cols, int nq,

@@ -1,107 +1,18 @@
-// bow_host.cpp -- host half of orbfe_bow_transform: TemplatedVocabulary::transform(features, BowVector&, FeatureVector&,
-// levelsup) (reference Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1126-1196).  The tree descent of every descriptor
-// runs on the device (bow_kernels.cu); what is left are the two std::map builds, restated on sorted arrays:
-//   BowVector::addWeight / addIfNotExist / normalize   (BowVector.cpp:34-84)
-//   FeatureVector::addFeature                         (FeatureVector.cpp:32-48)
-// Floating-point order is the reference's: a word's weights are added in feature order, norms are summed in word order.
-#include <algorithm>
-#include <cmath>
-#include <cstdint>
-#include <numeric>
-#include <vector>
-
-#include "../../include/orbfe_bow.h"
-
-struct OrbfeVocabulary;
-namespace orbfe {
-const int32_t *vocab_word_ids(const OrbfeVocabulary *v);
-const double *vocab_weights(const OrbfeVocabulary *v);
-void vocab_modes(const OrbfeVocabulary *v, int *weighting, int *norm);
-int set_error(int code, const char *fmt, ...);
-}  // namespace orbfe
-
-extern "C" int orbfe_bow_transform(OrbfeVocabulary *v, const uint8_t *desc, int n, int levelsup, int *nwords_out, int32_t *bow_ids,
-                                   double *bow_vals, int *nnodes_out, int32_t *fv_ids, int32_t *fv_ptr, int32_t *fv_feats) {
-    if (!v || n < 0 || !nwords_out || !nnodes_out || !fv_ptr) return orbfe::set_error(ORBFE_ERR_ARG, "bad arguments");
-    *nwords_out = 0;
-    *nnodes_out = 0;
-    fv_ptr[0] = 0;
-    if (n == 0) return ORBFE_OK;
-    if (!desc || !bow_ids || !bow_vals || !fv_ids || !fv_feats) return orbfe::set_error(ORBFE_ERR_ARG, "NULL argument");
-    std::vector<int32_t> leaf(n), node(n);
-    const int rc = orbfe_bow_descend(v, desc, n, levelsup, leaf.data(), node.data());
-    if (rc) return rc;
-    const int32_t *wid = orbfe::vocab_word_ids(v);
-    const double *wgt = orbfe::vocab_weights(v);
-    int weighting = 0, norm = 0;
-    orbfe::vocab_modes(v, &weighting, &norm);
-
-    // features that are not stopped (w > 0), in feature order
-    std::vector<int> kept;
-    kept.reserve(n);
-    for (int i = 0; i < n; i++)
-        if (wgt[leaf[i]] > 0) kept.push_back(i);
-
-    // ---- BowVector: stable order by word id, then per word the map's accumulation in feature order ----
-    std::vector<int> by_word(kept);
-    std::stable_sort(by_word.begin(), by_word.end(), [&](int a, int b) { return wid[leaf[a]] < wid[leaf[b]]; });
-    int nw = 0;
-    const bool accumulate = weighting == ORBFE_BOW_TF || weighting == ORBFE_BOW_TF_IDF;
-    for (size_t k = 0; k < by_word.size();) {
-        const int32_t id = wid[leaf[by_word[k]]];
-        double val = wgt[leaf[by_word[k]]];  // insert(id, w)
-        size_t e = k + 1;
-        for (; e < by_word.size() && wid[leaf[by_word[e]]] == id; e++)
-            if (accumulate) val += wgt[leaf[by_word[e]]];  // addWeight; addIfNotExist keeps the first
-        bow_ids[nw] = id;
-        bow_vals[nw] = val;
-        nw++;
-        k = e;
-    }
-    const bool must = norm != ORBFE_BOW_NORM_NONE;
-    if (accumulate && nw > 0 && !must) {
-        const double nd = (double)nw;
-        for (int k = 0; k < nw; k++) bow_vals[k] /= nd;
-    }
-    if (must) {
-        double s = 0.0;
-        if (norm == ORBFE_BOW_NORM_L1) {
-            for (int k = 0; k < nw; k++) s += std::fabs(bow_vals[k]);
-        } else {
-            for (int k = 0; k < nw; k++) s += bow_vals[k] * bow_vals[k];
-            s = std::sqrt(s);
-        }
-        if (s > 0.0)
-            for (int k = 0; k < nw; k++) bow_vals[k] /= s;
-    }
-    *nwords_out = nw;
-
-    // ---- FeatureVector: node id ascending, feature indices in feature order ----
-    std::vector<int> by_node(kept);
-    std::stable_sort(by_node.begin(), by_node.end(), [&](int a, int b) { return node[a] < node[b]; });
-    int nn = 0;
-    for (size_t k = 0; k < by_node.size();) {
-        const int32_t id = node[by_node[k]];
-        fv_ids[nn] = id;
-        size_t e = k;
-        for (; e < by_node.size() && node[by_node[e]] == id; e++) fv_feats[e] = by_node[e];
-        nn++;
-        fv_ptr[nn] = (int32_t)e;
-        k = e;
-    }
-    *nnodes_out = nn;
-    return ORBFE_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
+// bow_host.cpp -- host half of orbfe_bow_db_detect:
 // KeyFrameDatabase::DetectLoopCandidates / DetectRelocalisationCandidates on arrays (include/orbfe_bow.h).
 // Device: per keyframe, shared-word count + first shared word + L1 score (bow_db_score_kernel).  Host: the reference's
 // list logic.  lKFsSharingWords is filled while walking the query's words in ascending order and, inside a word, the
 // inverted-file list in insertion order: a keyframe enters at its FIRST shared word, so the list order is
 // (first shared word, keyframe index) -- keyframe indices are insertion order by contract.
-// ------------------------------------------------------------------------------------------------
+#include <algorithm>
+#include <cstdint>
+#include <vector>
+
+#include "../../include/orbfe_bow.h"
+
 struct OrbfeMatcher;
 namespace orbfe {
+int set_error(int code, const char *fmt, ...);
 int bow_db_score(OrbfeMatcher *m, int nq, const int32_t *q_ids, const double *q_vals, int nkf, const int32_t *kf_ptr,
                  const int32_t *db_ids, const double *db_vals, int32_t *common, int32_t *first, double *score);
 }

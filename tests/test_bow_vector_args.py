@@ -1,5 +1,5 @@
-"""CPU tests of the device BowVector entry points (include/orbfe_bow.h orbfe_bow_vector_device, orbfe_kfdb_add_device): bad
-arguments are rejected before the handle is used (the handles below are zeroed host buffers, never real handles); and the
+"""CPU tests of the BowVector entry points (include/orbfe_bow.h orbfe_bow_vector_device, orbfe_bow_transform,
+orbfe_kfdb_add_device): bad arguments are rejected before the handle is used (the handles below are zeroed host buffers, never real handles); and the
 oracle's BowVector, which the device kernel is tested against, equals DBoW2's own transform() for all four
 (weighting, norm) pairs on a vocabulary where the order of every sum shows in the result."""
 import ctypes as C
@@ -46,6 +46,38 @@ def test_bow_vector_device_rejects_bad_arguments():
     assert call(cap=MAX_CAP + 1) == fe.ORBFE_ERR_UNSUPPORTED
     assert b"" != fe.lib().orbfe_last_error()
     assert call(nframes=0) == fe.ORBFE_OK                 # nothing to do: the handle is not touched
+
+
+def test_bow_transform_rejects_bad_arguments():
+    """orbfe_bow_transform: NULL handle, n < 0 and NULL outputs are ORBFE_ERR_ARG; more descriptors than the kernels sort in
+    shared memory is ORBFE_ERR_UNSUPPORTED with the counts and fv_ptr[0] left 0; n = 0 is OK.  None of these touches the
+    handle."""
+    L = B._bind()
+    keep, v = _fake_handle()
+    n = MAX_CAP + 1
+    desc = np.zeros((n, 32), np.uint8)
+    bow_ids, bow_vals = np.zeros(n, np.int32), np.zeros(n, np.float64)
+    fv_ids, fv_ptr, fv_feats = np.zeros(n, np.int32), np.full(n + 1, 7, np.int32), np.zeros(n, np.int32)
+    nw, nn = C.c_int(7), C.c_int(7)
+    outs = [C.byref(nw), _p(bow_ids), _p(bow_vals), C.byref(nn), _p(fv_ids), _p(fv_ptr), _p(fv_feats)]
+
+    def call(voc=v, n=4, desc=_p(desc), outs=outs):
+        return L.orbfe_bow_transform(voc, desc, n, 4, *outs)
+
+    assert call(voc=None) == fe.ORBFE_ERR_ARG
+    assert call(n=-1) == fe.ORBFE_ERR_ARG
+    assert call(desc=None) == fe.ORBFE_ERR_ARG
+    for k in range(len(outs)):
+        o = list(outs)
+        o[k] = None
+        assert call(outs=o) == fe.ORBFE_ERR_ARG, k
+    nw.value = nn.value = fv_ptr[0] = 7
+    assert call(n=MAX_CAP + 1) == fe.ORBFE_ERR_UNSUPPORTED
+    assert b"" != fe.lib().orbfe_last_error()
+    assert nw.value == 0 and nn.value == 0 and fv_ptr[0] == 0
+    nw.value = nn.value = fv_ptr[0] = 7
+    assert call(n=0, desc=None) == fe.ORBFE_OK            # nothing to do: the handle is not touched
+    assert nw.value == 0 and nn.value == 0 and fv_ptr[0] == 0
 
 
 def test_kfdb_add_device_rejects_bad_arguments():

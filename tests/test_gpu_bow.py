@@ -11,25 +11,123 @@ from orb_slam_b200.synth import random_descriptors, noisy_copies, random_vocabul
 
 pytestmark = pytest.mark.gpu
 
+MAX_CAP = 16384   # ORBFE_FV_MAX_CAP
+
+
+def word_descriptors(voc, n, seed):
+    """n noisy copies of the vocabulary's words, every 50th descriptor unrelated (seed >= 1)."""
+    words = voc["node_desc"][voc["word_id"] >= 0]
+    rng = np.random.default_rng(seed)
+    desc = noisy_copies(words[rng.integers(0, len(words), n)], 0.1, seed + 4)
+    desc[::50] = random_descriptors(len(desc[::50]), seed - 1)  # a few unrelated descriptors
+    return desc
+
+
+def modes(L):
+    """(levelsup, weighting, norm): every weighting and norm once, levelsup from 0 to past the tree's depth."""
+    return [(4, B.TF_IDF, B.NORM_L1), (2, B.TF, B.NORM_NONE), (0, B.IDF, B.NORM_L2), (L + 1, B.BINARY, B.NORM_L1)]
+
+
+def assert_transform_equal(got, want, tag):
+    (ids, vals), (fids, fptr, ffeat) = got
+    (ids_o, vals_o), (fids_o, fptr_o, ffeat_o) = want
+    assert np.array_equal(ids, ids_o) and np.array_equal(vals.view(np.uint64), vals_o.view(np.uint64)), tag
+    assert np.array_equal(fids, fids_o) and np.array_equal(fptr, fptr_o) and np.array_equal(ffeat, ffeat_o), tag
+
 
 @pytest.mark.parametrize("k,L,ragged,n", [(10, 4, False, 2000), (7, 3, True, 777), (40, 2, False, 500), (10, 5, True, 1500)])
 def test_bow_transform_matches_oracle(gpu_required, k, L, ragged, n):
     voc = random_vocabulary(k, L, seed=k + L, ragged=ragged)
-    words = voc["node_desc"][voc["word_id"] >= 0]
-    rng = np.random.default_rng(5)
-    desc = noisy_copies(words[rng.integers(0, len(words), n)], 0.1, 9)
-    desc[::50] = random_descriptors(len(desc[::50]), 4)  # a few unrelated descriptors
-    for levelsup, weighting, norm in [(4, B.TF_IDF, B.NORM_L1), (2, B.TF, B.NORM_NONE), (0, B.IDF, B.NORM_L2), (L + 1, B.BINARY, B.NORM_L1)]:
+    desc = word_descriptors(voc, n, 5)
+    for levelsup, weighting, norm in modes(L):
         v = B.Vocabulary(voc, weighting, norm)
         leaf, node = v.descend(desc, levelsup)
         leaf_o, node_o = O.bow_descend(voc, desc, levelsup)
         assert np.array_equal(leaf, leaf_o) and np.array_equal(node, node_o)
-        (ids, vals), (fids, fptr, ffeat) = v.transform(desc, levelsup)
-        (ids_o, vals_o), (fids_o, fptr_o, ffeat_o) = O.bow_transform(voc, desc, levelsup, weighting, norm)
-        assert np.array_equal(ids, ids_o) and np.array_equal(vals.view(np.uint64), vals_o.view(np.uint64))
-        assert np.array_equal(fids, fids_o) and np.array_equal(fptr, fptr_o) and np.array_equal(ffeat, ffeat_o)
-        assert len(ids) > 10
+        got = v.transform(desc, levelsup)
+        assert_transform_equal(got, O.bow_transform(voc, desc, levelsup, weighting, norm), (levelsup, weighting, norm))
+        assert len(got[0][0]) > 10
         v.close()
+
+
+def test_bow_transform_at_max_descriptors(gpu_required):
+    """n = ORBFE_FV_MAX_CAP descriptors (128 KB of sort keys in shared memory per kernel) equals the oracle bit for bit for
+    every weighting and norm; one more descriptor is ORBFE_ERR_UNSUPPORTED."""
+    voc = random_vocabulary(10, 5, seed=15, ragged=True)
+    desc = word_descriptors(voc, MAX_CAP + 1, 8)
+    for levelsup, weighting, norm in modes(5):
+        v = B.Vocabulary(voc, weighting, norm)
+        got = v.transform(desc[:MAX_CAP], levelsup)
+        assert_transform_equal(got, O.bow_transform(voc, desc[:MAX_CAP], levelsup, weighting, norm), (levelsup, weighting, norm))
+        assert len(got[0][0]) > 1000
+        v.close()
+    v = B.Vocabulary(voc)
+    with pytest.raises(fe.OrbfeError) as e:
+        v.transform(desc, 4)
+    assert e.value.code == fe.ORBFE_ERR_UNSUPPORTED
+    v.close()
+
+
+def test_bow_transform_writes_nothing_past_its_counts(gpu_required):
+    """Output arrays of capacity n filled with a sentinel: orbfe_bow_transform writes the oracle's entries and leaves every
+    entry past bow_ids / bow_vals[nw), fv_ids[nn), fv_ptr[nn] and fv_feats[fv_ptr[nn]) as it was."""
+    import ctypes as C
+    voc = random_vocabulary(10, 3, seed=4)
+    L = B._bind()
+    p = lambda a: a.ctypes.data_as(C.c_void_p)
+    for n, seed in ((1, 1), (300, 2), (2000, 3), (5000, 4)):
+        desc = word_descriptors(voc, n, seed)
+        v = B.Vocabulary(voc)
+        bow_ids, bow_vals = np.full(n, -5, np.int32), np.full(n, -5.0)
+        fv_ids, fv_ptr, fv_feats = np.full(n, -5, np.int32), np.full(n + 1, -5, np.int32), np.full(n, -5, np.int32)
+        nw, nn = C.c_int(-5), C.c_int(-5)
+        assert L.orbfe_bow_transform(v.handle, p(desc), n, 1, C.byref(nw), p(bow_ids), p(bow_vals), C.byref(nn), p(fv_ids), p(fv_ptr),
+                                     p(fv_feats)) == fe.ORBFE_OK
+        nw, nn = nw.value, nn.value
+        nf = fv_ptr[nn]
+        assert_transform_equal(((bow_ids[:nw], bow_vals[:nw]), (fv_ids[:nn], fv_ptr[:nn + 1], fv_feats[:nf])), O.bow_transform(voc, desc, 1), n)
+        assert (bow_ids[nw:] == -5).all() and (bow_vals[nw:] == -5.0).all() and (fv_ids[nn:] == -5).all(), n
+        assert (fv_ptr[nn + 1:] == -5).all() and (fv_feats[nf:] == -5).all(), n
+        if n > 1:
+            assert nw < n and nn < n and nf < n, n   # some features fall on stopped words, several on one word
+        v.close()
+
+
+def test_bow_transform_from_several_threads(gpu_required):
+    """Four threads call transform on one vocabulary, 50 calls each on descriptor sets of 1 to 2000 descriptors, all at
+    once (ctypes releases the GIL): every result equals the oracle.  The first call is made at the largest size, so no
+    call grows the staging block while others are in flight."""
+    import threading
+    voc = random_vocabulary(10, 4, seed=2)
+    v = B.Vocabulary(voc)
+    T, K, NMAX = 4, 50, 2000
+    rng = np.random.default_rng(21)
+    sizes = rng.integers(1, NMAX + 1, (T, K))
+    sizes[:, 0] = NMAX
+    sets = [[word_descriptors(voc, int(sizes[t, k]), 1000 * t + k + 1) for k in range(K)] for t in range(T)]
+    want = [[O.bow_transform(voc, d, 4) for d in row] for row in sets]
+    assert_transform_equal(v.transform(sets[0][0], 4), want[0][0], "warm-up")
+    bad, start = [], threading.Barrier(T)
+
+    def run(t):
+        try:
+            start.wait()
+            for k in range(K):
+                got = v.transform(sets[t][k], 4)
+                try:
+                    assert_transform_equal(got, want[t][k], (t, k))
+                except AssertionError as e:
+                    bad.append(e)
+        except Exception as e:   # noqa: BLE001 -- reported below
+            bad.append(e)
+
+    threads = [threading.Thread(target=run, args=(t,)) for t in range(T)]
+    for th in threads:
+        th.start()
+    for th in threads:
+        th.join()
+    assert not bad, bad[:3]
+    v.close()
 
 
 def test_bow_descend_device_chains_after_extraction(gpu_required):

@@ -908,8 +908,8 @@ def bowchain(args):
       chain_{device,host}_wall_ms   one extracted frame (descriptors in HBM) to SearchByBoW results against a resident database
                                     of 1000 keyframes (32 views of the place, added by orbfe_kfdb_add_device, and 968 unrelated
                                     ones).  Device: descent, BowVector, FeatureVector, detect_device on the padded row, one
-                                    readback of the candidate count, search_by_bow_device.  Host: the path without the
-                                    BowVector kernel -- descent and FeatureVector on the device, descriptors D2H,
+                                    readback of the candidate count, search_by_bow_device.  Host: the path through the
+                                    host-array transform -- descent and FeatureVector on the device, descriptors D2H,
                                     orbfe_bow_transform, BowVector H2D, detect_device, the same search;
       detect_{padded,exact}_ms      CUDA-event ms of detect_device on frame 0's row with nq = cap and with nq = its word count."""
     import torch
