@@ -14,8 +14,11 @@
  * orbfe_search_for_initialization (cap = qcap = max(F1 features, F2 features)) that is at most 8283 features.  For
  * orbfe_window_search, orbfe_search_local_points, orbfe_search_by_projection_kf, orbfe_search_by_projection_f1f2 and
  * orbfe_guided_search, cap = the searched frame's feature count and qcap = the number of queries (the features or map points
- * that pass the routine's own filters): 2000 features allow about 24,800 queries.  Larger calls return ORBFE_ERR_UNSUPPORTED
- * with a message (orbfe_last_error).  Every rejection sets orbfe_last_error.
+ * that pass the routine's own filters): 2000 features allow about 24,800 queries per launch.  A call with more queries runs
+ * them in consecutive launches on the matcher's stream, with the same result, unless it applies the rotation histogram
+ * (check_orientation, hist_mode 1): such a call, like one whose features alone exceed the limit, returns
+ * ORBFE_ERR_UNSUPPORTED with a message (orbfe_last_error).  orbfe_guided_best takes any number of queries the same way.
+ * Every rejection sets orbfe_last_error.
  */
 #ifndef ORBFE_MATCH_H
 #define ORBFE_MATCH_H
@@ -138,9 +141,10 @@ int orbfe_guided_search(OrbfeMatcher *m, const OrbfeFrameView *f, int nq, const 
                         const int32_t *qlo, const int32_t *qhi, const uint8_t *qdesc, const float *qangle, int rule,
                         float nnratio, int th_dist, int hist_mode, int32_t *slot_owner_inout, int *nmatches_out);
 
-/* Guided search without slot bookkeeping: best candidate of every query, kept iff best <= th_dist (first minimum wins).
- * The inner loops of Fuse (ORBmatcher.cc:1090-1107, :1222-1239) and SearchBySim3 (:1356-1378, :1436-1458).
- * best_idx_out[q] = feature index in `f` or -1. */
+/* Guided search without slot bookkeeping: best candidate of every query, kept iff best <= th_dist (first minimum in
+ * GetFeaturesInArea order wins).  The inner loops of Fuse (ORBmatcher.cc:1090-1107, :1222-1239) and SearchBySim3
+ * (:1356-1378, :1436-1458); runs on the same fused kernel as orbfe_guided_search.  best_idx_out[q] = feature index in `f`
+ * or -1. */
 int orbfe_guided_best(OrbfeMatcher *m, const OrbfeFrameView *f, int nq, const float *qu, const float *qv, const float *qr,
                       const int32_t *qlo, const int32_t *qhi, const uint8_t *qdesc, int th_dist, int32_t *best_idx_out);
 

@@ -231,6 +231,7 @@ struct GuidedQueries {
     const int *qlo, *qhi;
     const uint8_t *qdesc;
     const int *q_base, *q_cnt;
+    int *best;   // rule SBP_RULE_BEST: per query (concatenated index) the kept candidate, or -1
 };
 
 __device__ __forceinline__ bool octave_ok(int o, int lo, int hi) {
@@ -297,6 +298,7 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
     uint32_t *resolved = reinterpret_cast<uint32_t *>(choice + P.qcap + (P.qcap & 1));  // [(qcap + 31) / 32] query has been decided
     constexpr bool EXPLICIT = MODE == 1;
     constexpr bool INIT = MODE == 2;
+    const int qown = EXPLICIT ? P.owner_base : 0;   // a matched slot receives qown + the job-local query index
     __shared__ int s_warp[SBP_WARPS], s_hist[32], s_keep[3], s_removed, s_nm, s_unres;
     uint32_t *s_ent = reinterpret_cast<uint32_t *>(smem + P.smem_fixed);  // entry staging area
 
@@ -489,6 +491,24 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
     __threadfence_block();
     __syncthreads();
 
+    // ---- C': best-only without slots (SBP_RULE_BEST, orbfe_guided_best): each query keeps the first minimum of its whole
+    //          list iff it is <= th_dist.  No slots, no histogram, no interaction between queries. ----
+    if (EXPLICIT && P.rule == SBP_RULE_BEST) {
+        int kept = 0;
+        for (int q = tid; q < nl; q += SBP_THREADS) {
+            const int b = q_off[q], e = q_off[q + 1];
+            uint32_t best = 0xFFFFFFFFu;   // dist << 16 | position: strict-< argmin in enumeration order
+            for (int p = b; p < e; p++) best = min(best, (ent[p] & 0xFFFF0000u) | (uint32_t)(p - b));
+            int idx = -1;
+            if (best != 0xFFFFFFFFu && (int)(best >> 16) <= P.th_dist) { idx = (int)(ent[b + (int)(best & 0xFFFF)] & 0xFFFF); kept++; }
+            GQ.best[qb + q] = idx;
+        }
+        if (kept) atomicAdd(&s_nm, kept);
+        __syncthreads();
+        if (tid == 0) nmatches[pair] = s_nm;
+        return;
+    }
+
     // ---- C: the accept loop.  In the reference it is sequential: query q takes the best candidate that no EARLIER query
     //         took.  Here it is resolved in parallel rounds of deterministic reservations: every undecided query picks its
     //         best free slot and stamps its index (atomicMin) on every free slot of its list.  Best-only rule (rule 0:
@@ -552,7 +572,7 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
             const int i2 = (int)(ent[q_off[q] + pos] & 0xFFFF);
             if (firstq[i2] != q) continue;
             atomicOr(&taken[i2 >> 5], 1u << (i2 & 31));
-            mp[i2] = q;
+            mp[i2] = qown + q;
             newbin[i2] = 0xFE;  // matched in this call; the rotation bin is filled in phase D
             atomicAdd(&s_nm, 1);
         }
@@ -619,7 +639,7 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
                 atomicOr(&resolved[q >> 5], 1u << (q & 31));
                 if (accept) {
                     atomicOr(&taken[i2 >> 5], 1u << (i2 & 31));
-                    mp[i2] = q;
+                    mp[i2] = qown + q;
                     newbin[i2] = 0xFE;  // matched in this call; the rotation bin is filled in phase D
                     atomicAdd(&s_nm, 1);
                 }
@@ -754,7 +774,7 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
                     const int i2 = (int)(ent[b + (int)(best & 0xFFFF)] & 0xFFFF);
                     if (lane == 0) {
                         taken[i2 >> 5] |= 1u << (i2 & 31);
-                        mp[i2] = q;
+                        mp[i2] = qown + q;
                         newbin[i2] = 0xFE;  // matched in this call; the rotation bin is filled in phase D
                     }
                     nm++;
@@ -809,7 +829,7 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
         // rotation histogram of the new matches (:1583-1590), in parallel: bin = round((aLast - aCur [+360]) / 30)
         for (int i = tid; i < nc; i += SBP_THREADS) {
             if (newbin[i] != 0xFE) continue;
-            const int bin = rot_hist_bin(query_angle(mp[i]), kc[i].angle);
+            const int bin = rot_hist_bin(query_angle(mp[i] - qown), kc[i].angle);
             newbin[i] = (uint8_t)bin;
             atomicAdd(&s_hist[bin], 1);
         }
@@ -869,13 +889,15 @@ int launch_init_device(const SbpParams &P, size_t smem_bytes, int npairs, const 
 int launch_guided_device(const SbpParams &P, size_t smem_bytes, int njobs, const OrbfeKeyPoint *kps, const uint8_t *desc,
                          const int *counts, const int *frame_idx, const float *qu, const float *qv, const float *qr,
                          const int *qlo, const int *qhi, const uint8_t *qdesc, const float *qangle, const int *q_base,
-                         const int *q_cnt, uint32_t *scratch, int *slot_owner, int *nmatches, int *err, cudaStream_t s) {
+                         const int *q_cnt, uint32_t *scratch, int *slot_owner, int *best_out, int *nmatches, int *err,
+                         cudaStream_t s) {
     if (smem_bytes > 48 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(sbp_device_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
         if (e != cudaSuccess) return (int)e;
     }
     GuidedQueries G;
     G.qu = qu; G.qv = qv; G.qr = qr; G.qangle = qangle; G.qlo = qlo; G.qhi = qhi; G.qdesc = qdesc; G.q_base = q_base; G.q_cnt = q_cnt;
+    G.best = best_out;
     sbp_device_kernel<1><<<njobs, SBP_THREADS, smem_bytes, s>>>(P, kps, desc, counts, frame_idx, nullptr, nullptr, nullptr, nullptr, G,
                                                             scratch, slot_owner, nmatches, err);
     return 0;

@@ -945,6 +945,8 @@ extern "C" int orbfe_matcher_sync(OrbfeMatcher *m) {
     return ORBFE_OK;
 }
 
+static constexpr size_t kSbpSmemMax = 220 * 1024;   // shared memory per block sbp_prepare grants the fused kernel
+
 // Prepares one launch of sbp_device_kernel over `njobs` jobs of at most `cap` features and `qcap` queries each: the image
 // bounds and their grid cell sizes (Frame.cc:77-78) in P, the split of the dynamic shared memory (returned in *smem) and
 // `per_job` global scratch entries per job.  The one place that decides whether a job fits the kernel.
@@ -956,7 +958,7 @@ static int sbp_prepare(OrbfeMatcher *m, SbpParams &P, float min_x, float min_y, 
     P.cap = cap; P.qcap = qcap;
     const size_t fixed = sbp_smem_fixed_bytes(cap, qcap);
     const size_t total = sbp_smem_total(m, fixed, njobs);
-    if (total > 220 * 1024)
+    if (total > kSbpSmemMax)
         return fail(ORBFE_ERR_UNSUPPORTED, "fused matcher: %d features and %d queries per job need %zu bytes of shared memory, more "
                     "than 220 KB (sbp_smem_fixed_bytes(cap, qcap) + 16 KB <= 220 KB: at most 8283 features when every feature is a "
                     "query)", cap, qcap, fixed + 16 * 1024);
@@ -1085,8 +1087,8 @@ extern "C" int orbfe_guided_search_device(OrbfeMatcher *m, int njobs, const Orbf
     size_t smem;
     if (int rc = sbp_prepare(m, P, min_x, min_y, max_x, max_y, cap, qcap, njobs, (size_t)64 * std::max(cap, qcap), &smem)) return rc;
     return sbp_launched(m, launch_guided_device(P, smem, njobs, d_kps, d_desc, d_counts, d_frame_idx, d_qu, d_qv, d_qr, d_qlo, d_qhi,
-                                                d_qdesc, d_qangle, d_q_base, d_q_cnt, m->scratch, d_slot_owner, d_nmatches, m->d_err,
-                                                stream ? (cudaStream_t)stream : m->stream));
+                                                d_qdesc, d_qangle, d_q_base, d_q_cnt, m->scratch, d_slot_owner, nullptr, d_nmatches,
+                                                m->d_err, stream ? (cudaStream_t)stream : m->stream));
 }
 
 int orbfe::Stage::layout(std::initializer_list<std::pair<size_t *, size_t>> arrays, size_t *total) {
@@ -1704,52 +1706,85 @@ int orbfe::sbp_frames_host(OrbfeMatcher *m, int npairs, const OrbfeFrameView *cu
     return ORBFE_OK;
 }
 
-// Guided search of `nq` query windows in frame f: one job, cap = f.n, qcap = nq.
+// the most queries (at most nq, at least 1) that one guided job over `cap` features holds in sbp_prepare's shared memory
+static int sbp_fit_qcap(int cap, int nq) {
+    int lo = 1, hi = nq;
+    while (lo < hi) {
+        const int mid = lo + (hi - lo + 1) / 2;
+        if (sbp_smem_fixed_bytes(cap, mid) + 16 * 1024 <= kSbpSmemMax) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+// Guided search of `nq` query windows in frame f: one job, cap = f.n.  Without the rotation histogram, a call whose queries
+// do not fit one launch runs them in consecutive chunks, launched in order on the matcher's stream against the same slot
+// array: under rules 0-2 query q's outcome depends only on the slots earlier queries took, under SBP_RULE_BEST on nothing
+// else, so the chunks give the one-launch result.  The histogram spans the whole call, so with it the call must fit one launch.
 int orbfe::guided_host(OrbfeMatcher *m, const OrbfeFrameView &f, int nq, const GuidedQuery *Q, int rule, float nnratio, int th_dist,
-                       int check_orientation, int *slot_owner, int *nmatches_out) {
+                       int check_orientation, int *slot_owner, int *best_out, int *nmatches_out) {
     *nmatches_out = 0;
+    if (best_out) std::fill(best_out, best_out + nq, -1);
     if (f.n == 0 || nq == 0) return ORBFE_OK;   // no candidates: nothing is matched, the slots stay as they are
     const int cap = f.n;
+    const int qcap = check_orientation ? nq : sbp_fit_qcap(cap, nq);   // queries per launch
+    const int nchunks = (nq + qcap - 1) / qcap;
     CU_TRY(cudaSetDevice(m->device));
-    size_t o_kps, o_desc, o_cnt, o_fi, o_qb, o_qc, o_qu, o_qv, o_qr, o_qa, o_lo, o_hi, o_qd, o_mp, o_nm, total;
+    size_t o_kps, o_desc, o_cnt, o_fi, o_qb, o_qc, o_qu, o_qv, o_qr, o_qa, o_lo, o_hi, o_qd, o_mp, o_nm, o_best, total;
+    const size_t nc4 = (size_t)nchunks * sizeof(int);
     if (int rc = m->stage.layout({{&o_kps, (size_t)cap * sizeof(OrbfeKeyPoint)}, {&o_desc, (size_t)cap * 32}, {&o_cnt, sizeof(int)},
-                                  {&o_fi, sizeof(int)}, {&o_qb, sizeof(int)}, {&o_qc, sizeof(int)}, {&o_qu, (size_t)nq * 4},
+                                  {&o_fi, sizeof(int)}, {&o_qb, nc4}, {&o_qc, nc4}, {&o_qu, (size_t)nq * 4},
                                   {&o_qv, (size_t)nq * 4}, {&o_qr, (size_t)nq * 4}, {&o_qa, (size_t)nq * 4}, {&o_lo, (size_t)nq * 4},
                                   {&o_hi, (size_t)nq * 4}, {&o_qd, (size_t)nq * 32}, {&o_mp, (size_t)cap * sizeof(int)},
-                                  {&o_nm, sizeof(int)}},
+                                  {&o_nm, nc4}, {&o_best, best_out ? (size_t)nq * sizeof(int) : 0}},
                               &total))
         return rc;
     unsigned char *H = m->stage.h, *D = m->stage.d;
     memcpy(H + o_kps, f.keys_un, (size_t)cap * sizeof(OrbfeKeyPoint));
     memcpy(H + o_desc, f.desc, (size_t)cap * 32);
-    *(int *)(H + o_cnt) = cap; *(int *)(H + o_fi) = 0; *(int *)(H + o_qb) = 0; *(int *)(H + o_qc) = nq;
+    *(int *)(H + o_cnt) = cap; *(int *)(H + o_fi) = 0;
+    for (int c = 0; c < nchunks; c++) {
+        ((int *)(H + o_qb))[c] = c * qcap;
+        ((int *)(H + o_qc))[c] = std::min(qcap, nq - c * qcap);
+    }
     float *qu = (float *)(H + o_qu), *qv = (float *)(H + o_qv), *qr = (float *)(H + o_qr), *qa = (float *)(H + o_qa);
     int *lo = (int *)(H + o_lo), *hi = (int *)(H + o_hi);
     for (int q = 0; q < nq; q++) {
         qu[q] = Q[q].u; qv[q] = Q[q].v; qr[q] = Q[q].r; qa[q] = Q[q].angle; lo[q] = Q[q].lo; hi[q] = Q[q].hi;
         memcpy(H + o_qd + (size_t)q * 32, Q[q].desc, 32);
     }
-    auto pack_slots = [&]() { memcpy(H + o_mp, slot_owner, (size_t)cap * sizeof(int)); };
-    auto launch = [&](size_t per_job) {
+    auto pack_slots = [&]() {
+        if (slot_owner) memcpy(H + o_mp, slot_owner, (size_t)cap * sizeof(int));
+        else memset(H + o_mp, 0xFF, (size_t)cap * sizeof(int));   // every slot free
+    };
+    auto launch = [&](size_t per_job) -> int {
         SbpParams P;
         memset(&P, 0, sizeof(P));
         P.nlevels = 1; P.check_ori = check_orientation ? 1 : 0;
         P.rule = rule; P.th_dist = th_dist; P.nnratio = nnratio;
         size_t smem;
-        if (int rc = sbp_prepare(m, P, f.min_x, f.min_y, f.max_x, f.max_y, cap, nq, 1, per_job, &smem)) return rc;
+        if (int rc = sbp_prepare(m, P, f.min_x, f.min_y, f.max_x, f.max_y, cap, qcap, 1, per_job, &smem)) return rc;
         P.gw = f.grid_inv_w; P.gh = f.grid_inv_h;
-        return sbp_launched(m, launch_guided_device(P, smem, 1, (const OrbfeKeyPoint *)(D + o_kps), D + o_desc, (const int *)(D + o_cnt),
-                                                    (const int *)(D + o_fi), (const float *)(D + o_qu), (const float *)(D + o_qv),
-                                                    (const float *)(D + o_qr), (const int *)(D + o_lo), (const int *)(D + o_hi), D + o_qd,
-                                                    (const float *)(D + o_qa), (const int *)(D + o_qb), (const int *)(D + o_qc),
-                                                    m->scratch, (int *)(D + o_mp), (int *)(D + o_nm), m->d_err, m->stream));
+        for (int c = 0; c < nchunks; c++) {
+            P.owner_base = c * qcap;   // the slots receive call-wide query indices
+            const int rc = launch_guided_device(P, smem, 1, (const OrbfeKeyPoint *)(D + o_kps), D + o_desc, (const int *)(D + o_cnt),
+                                                (const int *)(D + o_fi), (const float *)(D + o_qu), (const float *)(D + o_qv),
+                                                (const float *)(D + o_qr), (const int *)(D + o_lo), (const int *)(D + o_hi), D + o_qd,
+                                                (const float *)(D + o_qa), (const int *)(D + o_qb) + c, (const int *)(D + o_qc) + c,
+                                                m->scratch, (int *)(D + o_mp), best_out ? (int *)(D + o_best) : nullptr,
+                                                (int *)(D + o_nm) + c, m->d_err, m->stream);
+            if (int e = sbp_launched(m, rc)) return e;
+        }
+        return ORBFE_OK;
     };
-    if (int rc = run_staged(m, o_mp, o_nm, total, (size_t)64 * std::max(cap, nq), pack_slots, launch)) return rc;
+    if (int rc = run_staged(m, o_mp, o_nm, total, (size_t)64 * std::max(cap, qcap), pack_slots, launch)) return rc;
     // the kernel leaves occupied slots as they were and writes the query index into the slots it matched
     const int *mp = (const int *)(H + o_mp);
-    for (int i = 0; i < cap; i++)
-        if (slot_owner[i] < 0 && mp[i] >= 0) slot_owner[i] = Q[mp[i]].owner;
-    *nmatches_out = *(const int *)(H + o_nm);
+    if (slot_owner)
+        for (int i = 0; i < cap; i++)
+            if (slot_owner[i] < 0 && mp[i] >= 0) slot_owner[i] = Q[mp[i]].owner;
+    if (best_out) memcpy(best_out, H + o_best, (size_t)nq * sizeof(int));
+    for (int c = 0; c < nchunks; c++) *nmatches_out += ((const int *)(H + o_nm))[c];
     return ORBFE_OK;
 }
 

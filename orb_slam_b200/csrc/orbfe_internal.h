@@ -133,7 +133,7 @@ struct SbpParams {
     float scale[ORBFE_MAX_LEVELS];             // Frame::mvScaleFactors
     int nlevels, cap, check_ori;
     int qcap;                                  // queries per job the shared-memory offset table is sized for
-    int rule, th_dist;                         // accept rule 0/1/2 and distance threshold (guided search); projection mode: 0, TH_HIGH
+    int rule, th_dist;                         // accept rule 0/1/2/SBP_RULE_BEST and distance threshold (guided search); projection mode: 0, TH_HIGH
     float nnratio;
     int scratch_per_pair;                      // global scratch entries per pair
     int smem_entries;                          // entries that fit in the dynamic shared-memory staging area
@@ -146,12 +146,18 @@ struct SbpParams {
     int *xw_err;
     int xw_n;
     unsigned xw_epoch;
+    int owner_base;                            // guided search: added to the job-local query index a matched slot receives
 };
+// Guided-search accept rule without slots (orbfe_guided_best): each query keeps the first minimum of its whole candidate
+// list iff best <= th_dist, written to best_out; slot_owner is read but never written.  Internal: the exported guided searches
+// take rules 0..2 (3 is SearchForInitialization's).
+#define SBP_RULE_BEST 4
 size_t sbp_smem_fixed_bytes(int cap, int qcap);
 int launch_guided_device(const SbpParams &P, size_t smem_bytes, int njobs, const OrbfeKeyPoint *kps, const uint8_t *desc,
                          const int *counts, const int *frame_idx, const float *qu, const float *qv, const float *qr,
                          const int *qlo, const int *qhi, const uint8_t *qdesc, const float *qangle, const int *q_base,
-                         const int *q_cnt, uint32_t *scratch, int *slot_owner, int *nmatches, int *err, cudaStream_t s);
+                         const int *q_cnt, uint32_t *scratch, int *slot_owner, int *best_out, int *nmatches, int *err,
+                         cudaStream_t s);
 int launch_init_device(const SbpParams &P, size_t smem_bytes, int npairs, const OrbfeKeyPoint *kps, const uint8_t *desc,
                        const int *counts, const int *f1_idx, const int *f2_idx, float *prev_matched, uint32_t *scratch, int *match12,
                        int *nmatches, int *err, cudaStream_t s);
@@ -166,12 +172,15 @@ struct GuidedQuery { float u, v, r; int lo, hi; const uint8_t *desc; float angle
 // Host-array forms of the windowed matchers (orbfe_api.cu).  host/match_host.cpp checks the arguments and builds the
 // queries; these stage everything in the matcher's pinned block, run sbp_device_kernel, copy the results back and
 // synchronise.  The views' own bounds, grid_inv_w/h and scale_factors are what the kernel reads.
+// guided_host: best_out (nq ints, rule SBP_RULE_BEST only, else NULL) receives each query's kept candidate or -1; slot_owner
+// may then be NULL (no occupied slots).  A call too large for one launch runs its queries in consecutive chunks unless it
+// applies the rotation histogram.
 int sbp_frames_host(OrbfeMatcher *m, int npairs, const OrbfeFrameView *cur, const OrbfeFrameView *last,
                     const uint8_t *const *last_has_mp, const uint8_t *const *last_outlier, const float *const *last_world,
                     const float *const *Tcw, float fx, float fy, float cx, float cy, float th, int check_orientation,
                     int *const *cur_mp_inout, int *nmatches_out);
 int guided_host(OrbfeMatcher *m, const OrbfeFrameView &f, int nq, const GuidedQuery *Q, int rule, float nnratio, int th_dist,
-                int check_orientation, int *slot_owner, int *nmatches_out);
+                int check_orientation, int *slot_owner, int *best_out, int *nmatches_out);
 int init_host(OrbfeMatcher *m, const OrbfeFrameView &f1, const OrbfeFrameView &f2, float *prev_matched, int window,
               float nnratio, int check_orientation, int *match12_out, int *nmatches_out);
 

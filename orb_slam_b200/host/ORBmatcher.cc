@@ -1,13 +1,12 @@
 // ORBmatcher.cc -- facade of ORB_SLAM::ORBmatcher (reference src/ORBmatcher.cc) over liborbfe.so.
 //
-// Pattern of every routine here: (1) gather -- walk the queries in the reference's order and enumerate their
-// candidates (Frame's own GetFeaturesInArea, or the plain-array matchers of include/orbfe_match.h);
-// (2) one GPU launch computes all 256-bit Hamming distances of the call; (3) replay -- the reference's
-// sequential accept/skip loop runs over those distances, so results (incl. tie-breaks) are unchanged.
+// Pattern of every routine here: (1) convert -- the Frame / KeyFrame becomes an OrbfeFrameView and the map points
+// become arrays (or, for the KeyFrame-level routines, projected query windows), in the reference's order;
+// (2) one array-level entry of include/orbfe_match.h finds the candidates and runs the accept loop on the GPU;
+// (3) replay -- the resulting matches are written back into the map, with the reference's map changes.
 //
-// All thirteen search / fuse methods of the reference class are defined here.  The Frame-level ones and the
-// BoW / triangulation ones forward to array-level entry points that have oracle parity tests
-// (tests/test_gpu_matchers.py); the Sim3 / Fuse ones gather through KeyFrame's public API and use orbfe_hamming_csr.
+// All thirteen search / fuse methods of the reference class are defined here; every array-level entry they call has
+// oracle parity tests (tests/test_gpu_matchers.py).
 #include "ORBmatcher.h"
 
 #include <algorithm>
@@ -265,10 +264,11 @@ int ORBmatcher::SearchByProjection(Frame &F1, Frame &F2, int windowSize, std::ve
 }  // namespace ORB_SLAM
 
 // =================================================================================================
-// KeyFrame-level routines.  KeyFrame keeps its image bounds and grid protected (KeyFrame.h:181-187), so the
-// candidate lists come from its own public GetFeaturesInArea; the distances of a whole call go to the GPU in
-// one orbfe_hamming_csr launch (or to the array-level matchers of include/orbfe_match.h), and the reference's
-// accept loop -- including its map mutations -- is replayed on the host in the original order.
+// KeyFrame-level routines.  Each projects its map points into one query window apiece, in the reference's order:
+// (u, v, th * scale factor of the predicted level, levels [lv - 1, lv], the point's descriptor).  One array-level entry
+// walks the KeyFrame's grid and takes the best candidate: orbfe_guided_search for SearchByProjection(KeyFrame*, Scw, ...),
+// whose points compete for free slots, and orbfe_guided_best for Fuse and SearchBySim3, which keep each point's best
+// candidate.  The map changes of the reference's accept loop are then replayed on the host in the original order.
 // The cv::Mat algebra of the projections is written out element-wise with OpenCV 2.4's float/double semantics
 // (a 3x3 * 3x1 gemm with flags 0 sums in float -- OpenCV's small-matrix path, pinned to cv2.gemm -- every other product
 // in double; Mat/scalar scales by the float reciprocal).
@@ -277,22 +277,52 @@ namespace ORB_SLAM {
 
 namespace {
 
-struct Csr {
-    std::vector<int> row_ptr, cols;
-    std::vector<unsigned char> qdesc;
-    Csr() : row_ptr(1, 0) {}
-    void add_row(const cv::Mat &d) { qdesc.insert(qdesc.end(), d.ptr(0), d.ptr(0) + 32); row_ptr.push_back((int)cols.size()); }
-    int rows() const { return (int)row_ptr.size() - 1; }
+// A KeyFrame as the matchers' view.  KeyFrame keeps its image bounds and grid protected (KeyFrame.h:182-209), but they are
+// Frame's: the constructor copies the bounds and grid cell sizes from Frame's statics (KeyFrame.cc:31-34), and mGrid is
+// Frame's grid of mvKeysUn (:45-50), which the fused kernel rebuilds from the keys with the same bounds and cell sizes.  So
+// the view takes them from Frame's statics, as make_view does, and a KeyFrame searched here must come from a Frame of the
+// current image geometry.
+struct KeyFrameView {
+    KeyFrame *const pKF;
+    const std::vector<cv::KeyPoint> keys;   // GetKeyPointsUn() and GetScaleFactors() return copies: they live here
+    const std::vector<float> sf;
+    const DescBuf desc;
+    OrbfeFrameView v;
+    explicit KeyFrameView(KeyFrame *kf) : pKF(kf), keys(kf->GetKeyPointsUn()), sf(kf->GetScaleFactors()), desc(kf->GetDescriptors()) {
+        v.n = (int)keys.size();
+        v.keys_un = v.n ? reinterpret_cast<const OrbfeKeyPoint *>(&keys[0]) : NULL;
+        v.desc = desc.ptr;
+        v.min_x = (float)Frame::mnMinX; v.min_y = (float)Frame::mnMinY;
+        v.max_x = (float)Frame::mnMaxX; v.max_y = (float)Frame::mnMaxY;
+        v.grid_inv_w = Frame::mfGridElementWidthInv;
+        v.grid_inv_h = Frame::mfGridElementHeightInv;
+        v.nlevels = pKF->GetScaleLevels();
+        v.scale_factors = sf.empty() ? NULL : &sf[0];
+    }
+    // PredictScale: the first level whose factor is >= ratio, at most the last level
+    int predict_level(float ratio) const { return std::min((int)(std::lower_bound(sf.begin(), sf.end(), ratio) - sf.begin()), v.nlevels - 1); }
 };
 
-std::vector<unsigned short> distances(const Csr &c, const cv::Mat &targetDesc)
-{
-    std::vector<unsigned short> dist(c.cols.empty() ? 1 : c.cols.size());
-    if (c.cols.empty()) return dist;
-    const DescBuf t(targetDesc);
-    if (!ok(orbfe_hamming_csr(thread_matcher(), &c.qdesc[0], c.rows(), t.ptr, targetDesc.rows, &c.row_ptr[0], &c.cols[0], &dist[0]))) std::fill(dist.begin(), dist.end(), (unsigned short)0xFFFF);  // no candidate is accepted
-    return dist;
-}
+template <typename T> const T *ptr_or_null(const std::vector<T> &v) { return v.empty() ? NULL : &v[0]; }
+
+// the query windows of one call
+struct Windows {
+    std::vector<float> u, v, r;
+    std::vector<int> lo, hi;
+    std::vector<unsigned char> desc;
+    int size() const { return (int)u.size(); }
+    void add(float wu, float wv, float wr, int level, const cv::Mat &d) {
+        u.push_back(wu); v.push_back(wv); r.push_back(wr);
+        lo.push_back(level - 1); hi.push_back(level);
+        desc.insert(desc.end(), d.ptr(0), d.ptr(0) + 32);
+    }
+    // orbfe_guided_best: best[q] = the feature query q keeps (best <= th_dist) or -1; false after a reported error
+    bool best(const KeyFrameView &kf, int th_dist, std::vector<int> &best) const {
+        best.assign(size() + 1, -1);
+        return ok(orbfe_guided_best(thread_matcher(), &kf.v, size(), ptr_or_null(u), ptr_or_null(v), ptr_or_null(r), ptr_or_null(lo),
+                                    ptr_or_null(hi), ptr_or_null(desc), th_dist, &best[0]));
+    }
+};
 
 // y = R*x + t for 3x3 / 3x1 CV_32F Mats: one cv::gemm(R, x, 1, t, 1) with flags 0 -> OpenCV's unrolled small-matrix branch:
 // the three products are summed in FLOAT, left to right, then (float)(sum + t) in double (pinned to cv2.gemm golden vectors,
@@ -332,17 +362,12 @@ struct Sim3Cam {
     }
 };
 
-int predict_level(const std::vector<float> &sf, float ratio, int nMaxLevel)
+// shared gate of SearchByProjection(KF,Scw,..) and both Fuse overloads: returns false if the point is rejected; otherwise
+// appends its query window
+bool project(const KeyFrameView &kf, MapPoint *pMP, const cv::Mat &Rcw, const cv::Mat &tcw, const float Ow[3], float th,
+             bool invz_in_double, Windows &w)
 {
-    const int it = (int)(std::lower_bound(sf.begin(), sf.end(), ratio) - sf.begin());
-    return std::min(it, nMaxLevel);
-}
-
-// shared gate + candidate gathering of SearchByProjection(KF,Scw,..) and both Fuse overloads:
-// returns false if the point is rejected; otherwise appends a CSR row with the level-filtered candidates
-bool project_and_gather(KeyFrame *pKF, MapPoint *pMP, const cv::Mat &Rcw, const cv::Mat &tcw, const float Ow[3], float th,
-                        bool invz_in_double, const std::vector<float> &vfScaleFactors, int nMaxLevel, Csr &csr)
-{
+    KeyFrame *pKF = kf.pKF;
     float X[3], Xc[3];
     mat3(pMP->GetWorldPos(), X);
     transform(Rcw, tcw, X, Xc);
@@ -359,16 +384,8 @@ bool project_and_gather(KeyFrame *pKF, MapPoint *pMP, const cv::Mat &Rcw, const 
     mat3(pMP->GetNormal(), Pn);
     const double dotPn = (double)PO[0] * Pn[0] + (double)PO[1] * Pn[1] + (double)PO[2] * Pn[2];  // Mat::dot: double
     if (dotPn < 0.5 * dist) return false;  // viewing angle < 60 deg
-    const int nPredictedLevel = predict_level(vfScaleFactors, dist / minDistance, nMaxLevel);
-    const float radius = th * vfScaleFactors[nPredictedLevel];
-    const std::vector<size_t> vIndices = pKF->GetFeaturesInArea(u, v, radius);
-    if (vIndices.empty()) return false;
-    for (size_t k = 0; k < vIndices.size(); k++) {
-        const int kpLevel = pKF->GetKeyPointScaleLevel(vIndices[k]);
-        if (kpLevel < nPredictedLevel - 1 || kpLevel > nPredictedLevel) continue;
-        csr.cols.push_back((int)vIndices[k]);
-    }
-    csr.add_row(pMP->GetDescriptor());
+    const int nPredictedLevel = kf.predict_level(dist / minDistance);
+    w.add(u, v, th * kf.sf[nPredictedLevel], nPredictedLevel, pMP->GetDescriptor());
     return true;
 }
 
@@ -381,7 +398,6 @@ void feature_vector_csr(const DBoW2::FeatureVector &fv, std::vector<int> &ids, s
         ptr.push_back((int)items.size());
     }
 }
-template <typename T> const T *ptr_or_null(const std::vector<T> &v) { return v.empty() ? NULL : &v[0]; }
 
 }  // namespace
 
@@ -420,29 +436,27 @@ int ORBmatcher::SearchByProjection(Frame &CurrentFrame, KeyFrame *pKF, const std
 // ---- LoopClosing::ComputeSim3 (LoopClosing.cc:370) ------------------------------------------------------------
 int ORBmatcher::SearchByProjection(KeyFrame *pKF, cv::Mat Scw, const std::vector<MapPoint *> &vpPoints, std::vector<MapPoint *> &vpMatched, int th)
 {
-    const int nMaxLevel = pKF->GetScaleLevels() - 1;
-    const std::vector<float> vfScaleFactors = pKF->GetScaleFactors();
+    const KeyFrameView kf(pKF);
     const Sim3Cam cam(Scw);
     std::set<MapPoint *> spAlreadyFound(vpMatched.begin(), vpMatched.end());
     spAlreadyFound.erase(static_cast<MapPoint *>(NULL));
-    Csr csr;
+    Windows w;
     std::vector<int> q2mp;
     for (int iMP = 0, iend = (int)vpPoints.size(); iMP < iend; iMP++) {
         MapPoint *pMP = vpPoints[iMP];
         if (pMP->isBad() || spAlreadyFound.count(pMP)) continue;
-        if (project_and_gather(pKF, pMP, cam.Rcw, cam.tcw, cam.Ow, (float)th, false, vfScaleFactors, nMaxLevel, csr)) q2mp.push_back(iMP);
+        if (project(kf, pMP, cam.Rcw, cam.tcw, cam.Ow, (float)th, false, w)) q2mp.push_back(iMP);
     }
-    const std::vector<unsigned short> dist = distances(csr, pKF->GetDescriptors());
+    // :373-398: the best candidate whose vpMatched entry is still empty (set on entry or by an earlier point), if <= TH_LOW
+    std::vector<int> slot(kf.v.n + 1, -1);
+    for (int i = 0; i < kf.v.n; i++)
+        if (vpMatched[i]) slot[i] = INT_MAX;
     int nmatches = 0;
-    for (int q = 0; q < csr.rows(); q++) {  // :373-398
-        int bestDist = INT_MAX, bestIdx = -1;
-        for (int c = csr.row_ptr[q]; c < csr.row_ptr[q + 1]; c++) {
-            const int idx = csr.cols[c];
-            if (vpMatched[idx]) continue;
-            if (dist[c] < bestDist) { bestDist = dist[c]; bestIdx = idx; }
-        }
-        if (bestDist <= TH_LOW) { vpMatched[bestIdx] = vpPoints[q2mp[q]]; nmatches++; }
-    }
+    if (!ok(orbfe_guided_search(thread_matcher(), &kf.v, w.size(), ptr_or_null(w.u), ptr_or_null(w.v), ptr_or_null(w.r),
+                                ptr_or_null(w.lo), ptr_or_null(w.hi), ptr_or_null(w.desc), NULL, 0, 0.f, TH_LOW, 0, &slot[0],
+                                &nmatches))) return 0;
+    for (int i = 0; i < kf.v.n; i++)
+        if (slot[i] >= 0 && slot[i] != INT_MAX) vpMatched[i] = vpPoints[q2mp[slot[i]]];
     return nmatches;
 }
 
@@ -450,33 +464,30 @@ int ORBmatcher::SearchByProjection(KeyFrame *pKF, cv::Mat Scw, const std::vector
 int ORBmatcher::Fuse(KeyFrame *pKF, std::vector<MapPoint *> &vpMapPoints, float th)
 {
     const cv::Mat Rcw = pKF->GetRotation(), tcw = pKF->GetTranslation();
-    const int nMaxLevel = pKF->GetScaleLevels() - 1;
-    const std::vector<float> vfScaleFactors = pKF->GetScaleFactors();
+    const KeyFrameView kf(pKF);
     float Ow[3];
     mat3(pKF->GetCameraCenter(), Ow);
-    Csr csr;
+    Windows w;
     std::vector<int> q2mp;
     for (size_t i = 0; i < vpMapPoints.size(); i++) {
         MapPoint *pMP = vpMapPoints[i];
         if (!pMP) continue;
         if (pMP->isBad() || pMP->IsInKeyFrame(pKF)) continue;
-        if (project_and_gather(pKF, pMP, Rcw, tcw, Ow, th, false, vfScaleFactors, nMaxLevel, csr)) q2mp.push_back((int)i);
+        if (project(kf, pMP, Rcw, tcw, Ow, th, false, w)) q2mp.push_back((int)i);
     }
-    const std::vector<unsigned short> dist = distances(csr, pKF->GetDescriptors());
+    std::vector<int> best;
+    if (!w.best(kf, TH_LOW, best)) return 0;
     int nFused = 0;
-    for (int q = 0; q < csr.rows(); q++) {  // :1090-1131
-        int bestDist = INT_MAX, bestIdx = -1;
-        for (int c = csr.row_ptr[q]; c < csr.row_ptr[q + 1]; c++)
-            if (dist[c] < bestDist) { bestDist = dist[c]; bestIdx = csr.cols[c]; }
-        if (bestDist <= TH_LOW) {
-            MapPoint *pMP = vpMapPoints[q2mp[q]];
-            // the reference evaluates this gate at the point's turn (:1040): a pointer listed twice is fused once
-            if (pMP->isBad() || pMP->IsInKeyFrame(pKF)) continue;
-            MapPoint *pMPinKF = pKF->GetMapPoint(bestIdx);
-            if (pMPinKF) { if (!pMPinKF->isBad()) pMP->Replace(pMPinKF); }
-            else { pMP->AddObservation(pKF, bestIdx); pKF->AddMapPoint(pMP, bestIdx); }
-            nFused++;
-        }
+    for (int q = 0; q < w.size(); q++) {  // :1090-1131
+        const int bestIdx = best[q];
+        if (bestIdx < 0) continue;
+        MapPoint *pMP = vpMapPoints[q2mp[q]];
+        // the reference evaluates this gate at the point's turn (:1040): a pointer listed twice is fused once
+        if (pMP->isBad() || pMP->IsInKeyFrame(pKF)) continue;
+        MapPoint *pMPinKF = pKF->GetMapPoint(bestIdx);
+        if (pMPinKF) { if (!pMPinKF->isBad()) pMP->Replace(pMPinKF); }
+        else { pMP->AddObservation(pKF, bestIdx); pKF->AddMapPoint(pMP, bestIdx); }
+        nFused++;
     }
     return nFused;
 }
@@ -484,30 +495,27 @@ int ORBmatcher::Fuse(KeyFrame *pKF, std::vector<MapPoint *> &vpMapPoints, float 
 // ---- LoopClosing::SearchAndFuse (LoopClosing.cc:568) -------------------------------------------------------------
 int ORBmatcher::Fuse(KeyFrame *pKF, cv::Mat Scw, const std::vector<MapPoint *> &vpPoints, float th)
 {
+    const KeyFrameView kf(pKF);
     const Sim3Cam cam(Scw);
     const std::set<MapPoint *> spAlreadyFound = pKF->GetMapPoints();
-    const int nMaxLevel = pKF->GetScaleLevels() - 1;
-    const std::vector<float> vfScaleFactors = pKF->GetScaleFactors();
-    Csr csr;
+    Windows w;
     std::vector<int> q2mp;
     for (size_t iMP = 0; iMP < vpPoints.size(); iMP++) {
         MapPoint *pMP = vpPoints[iMP];
         if (pMP->isBad() || spAlreadyFound.count(pMP)) continue;
-        if (project_and_gather(pKF, pMP, cam.Rcw, cam.tcw, cam.Ow, th, true, vfScaleFactors, nMaxLevel, csr)) q2mp.push_back((int)iMP);
+        if (project(kf, pMP, cam.Rcw, cam.tcw, cam.Ow, th, true, w)) q2mp.push_back((int)iMP);
     }
-    const std::vector<unsigned short> dist = distances(csr, pKF->GetDescriptors());
+    std::vector<int> best;
+    if (!w.best(kf, TH_LOW, best)) return 0;
     int nFused = 0;
-    for (int q = 0; q < csr.rows(); q++) {  // :1222-1261
-        int bestDist = INT_MAX, bestIdx = -1;
-        for (int c = csr.row_ptr[q]; c < csr.row_ptr[q + 1]; c++)
-            if (dist[c] < bestDist) { bestDist = dist[c]; bestIdx = csr.cols[c]; }
-        if (bestDist <= TH_LOW) {
-            MapPoint *pMP = vpPoints[q2mp[q]];
-            MapPoint *pMPinKF = pKF->GetMapPoint(bestIdx);
-            if (pMPinKF) { if (!pMPinKF->isBad()) pMPinKF->Replace(pMP); }
-            else { pMP->AddObservation(pKF, bestIdx); pKF->AddMapPoint(pMP, bestIdx); }
-            nFused++;
-        }
+    for (int q = 0; q < w.size(); q++) {  // :1222-1261
+        const int bestIdx = best[q];
+        if (bestIdx < 0) continue;
+        MapPoint *pMP = vpPoints[q2mp[q]];
+        MapPoint *pMPinKF = pKF->GetMapPoint(bestIdx);
+        if (pMPinKF) { if (!pMPinKF->isBad()) pMPinKF->Replace(pMP); }
+        else { pMP->AddObservation(pKF, bestIdx); pKF->AddMapPoint(pMP, bestIdx); }
+        nFused++;
     }
     return nFused;
 }
@@ -640,9 +648,8 @@ int ORBmatcher::SearchBySim3(KeyFrame *pKF1, KeyFrame *pKF2, std::vector<MapPoin
     Dir dirs[2] = {{pKF1, pKF2, &R1w, &t1w, &sR21, &t21, &vp1, &done1, &vnMatch1}, {pKF2, pKF1, &R2w, &t2w, &sR12, &t12, &vp2, &done2, &vnMatch2}};
     for (int dsel = 0; dsel < 2; dsel++) {
         Dir &D = dirs[dsel];
-        const int nMaxLevel = D.to->GetScaleLevels() - 1;
-        const std::vector<float> sf = D.to->GetScaleFactors();
-        Csr csr;
+        const KeyFrameView kf(D.to);
+        Windows w;
         std::vector<int> q2i;
         for (int i = 0; i < (int)D.vp->size(); i++) {
             MapPoint *pMP = (*D.vp)[i];
@@ -659,24 +666,14 @@ int ORBmatcher::SearchBySim3(KeyFrame *pKF1, KeyFrame *pKF2, std::vector<MapPoin
             const float maxD = pMP->GetMaxDistanceInvariance(), minD = pMP->GetMinDistanceInvariance();
             const float dist3D = norm3(Xb);
             if (dist3D < minD || dist3D > maxD) continue;
-            const int lv = predict_level(sf, dist3D / minD, nMaxLevel);
-            const std::vector<size_t> vIdx = D.to->GetFeaturesInArea(u, v, th * sf[lv]);
-            if (vIdx.empty()) continue;
-            for (size_t k = 0; k < vIdx.size(); k++) {
-                const int oct = D.to->GetKeyPointUn(vIdx[k]).octave;
-                if (oct < lv - 1 || oct > lv) continue;
-                csr.cols.push_back((int)vIdx[k]);
-            }
-            csr.add_row(pMP->GetDescriptor());
+            const int lv = kf.predict_level(dist3D / minD);
+            w.add(u, v, th * kf.sf[lv], lv, pMP->GetDescriptor());
             q2i.push_back(i);
         }
-        const std::vector<unsigned short> dist = distances(csr, D.to->GetDescriptors());
-        for (int q = 0; q < csr.rows(); q++) {
-            int bestDist = INT_MAX, bestIdx = -1;
-            for (int c = csr.row_ptr[q]; c < csr.row_ptr[q + 1]; c++)
-                if (dist[c] < bestDist) { bestDist = dist[c]; bestIdx = csr.cols[c]; }
-            if (bestDist <= TH_HIGH) (*D.match)[q2i[q]] = bestIdx;
-        }
+        std::vector<int> best;
+        if (!w.best(kf, TH_HIGH, best)) return 0;
+        for (int q = 0; q < w.size(); q++)
+            if (best[q] >= 0) (*D.match)[q2i[q]] = best[q];
     }
     int nFound = 0;  // :1486-1502: keep mutual agreements
     for (int i1 = 0; i1 < N1; i1++) {

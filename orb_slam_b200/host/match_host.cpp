@@ -3,8 +3,8 @@
 //
 // Each entry checks its arguments and turns its routine's inputs into query windows: the projections of map points, the
 // predicted levels and search radii.  Frame's 64x48 grid, GetFeaturesInArea, the distances, the accept loop and the rotation
-// histogram run once, in the fused kernel (sbp_device_kernel, match_kernels.cu), staged by orbfe_api.cu.
-// orbfe_guided_best, a slot-free argmin, enumerates its candidates here and computes the distances with orbfe_hamming_csr.
+// histogram run once, in the fused kernel (sbp_device_kernel, match_kernels.cu), staged by orbfe_api.cu; so does
+// orbfe_guided_best, the slot-free argmin, under its own accept rule (SBP_RULE_BEST).
 #include <algorithm>
 #include <climits>
 #include <cmath>
@@ -18,8 +18,6 @@ using orbfe::set_error;
 
 namespace {
 
-constexpr int kGridCols = 64;  // FRAME_GRID_COLS, Frame.h:36
-constexpr int kGridRows = 48;  // FRAME_GRID_ROWS, Frame.h:35
 constexpr int kThHigh = 100;   // TH_HIGH, ORBmatcher.cc:40
 
 // A view is well formed when its arrays are present and every keypoint octave indexes scale_factors (a malformed
@@ -42,63 +40,6 @@ inline void Rx_plus_t(const float *T, const float *X, float out[3]) {
         s = s + T[4 * k + 2] * X[2];
         out[k] = (float)((double)s + (double)T[4 * k + 3]);
     }
-}
-
-struct Grid {
-    std::vector<int> start;  // kGridCols*kGridRows + 1, cell id = ix*kGridRows + iy
-    std::vector<int> items;
-};
-
-// Frame.cc:116-123 + PosInGrid :267-277
-void build_grid(const OrbfeFrameView &f, Grid &g) {
-    const int nc = kGridCols * kGridRows;
-    g.start.assign(nc + 1, 0);
-    std::vector<int> cell(f.n);
-    for (int i = 0; i < f.n; i++) {
-        const OrbfeKeyPoint &kp = f.keys_un[i];
-        const int px = (int)std::round((kp.x - f.min_x) * f.grid_inv_w);
-        const int py = (int)std::round((kp.y - f.min_y) * f.grid_inv_h);
-        if (px < 0 || px >= kGridCols || py < 0 || py >= kGridRows) { cell[i] = -1; continue; }
-        cell[i] = px * kGridRows + py;
-        g.start[cell[i] + 1]++;
-    }
-    for (int c = 0; c < nc; c++) g.start[c + 1] += g.start[c];
-    g.items.assign(std::max(f.n, 1), 0);
-    std::vector<int> fill(g.start.begin(), g.start.end() - 1);
-    for (int i = 0; i < f.n; i++)
-        if (cell[i] >= 0) g.items[fill[cell[i]]++] = i;  // ascending index inside a cell (push_back order)
-}
-
-// Frame::GetFeaturesInArea, Frame.cc:200-265: appends to `out`
-void features_in_area(const OrbfeFrameView &f, const Grid &g, float x, float y, float r, int minLevel, int maxLevel,
-                      std::vector<int> &out) {
-    int x0 = (int)std::floor((x - f.min_x - r) * f.grid_inv_w);
-    x0 = std::max(0, x0);
-    if (x0 >= kGridCols) return;
-    int x1 = (int)std::ceil((x - f.min_x + r) * f.grid_inv_w);
-    x1 = std::min(kGridCols - 1, x1);
-    if (x1 < 0) return;
-    int y0 = (int)std::floor((y - f.min_y - r) * f.grid_inv_h);
-    y0 = std::max(0, y0);
-    if (y0 >= kGridRows) return;
-    int y1 = (int)std::ceil((y - f.min_y + r) * f.grid_inv_h);
-    y1 = std::min(kGridRows - 1, y1);
-    if (y1 < 0) return;
-    bool check = true, same = false;
-    if (minLevel == -1 && maxLevel == -1) check = false;
-    else if (minLevel == maxLevel) same = true;
-    for (int ix = x0; ix <= x1; ix++)
-        for (int iy = y0; iy <= y1; iy++) {
-            const int c = ix * kGridRows + iy;
-            for (int k = g.start[c]; k < g.start[c + 1]; k++) {
-                const int idx = g.items[k];
-                const OrbfeKeyPoint &kp = f.keys_un[idx];
-                if (check && !same) { if (kp.octave < minLevel || kp.octave > maxLevel) continue; }
-                else if (same) { if (kp.octave != minLevel) continue; }
-                if (std::fabs(kp.x - x) > r || std::fabs(kp.y - y) > r) continue;
-                out.push_back(idx);
-            }
-        }
 }
 
 }  // namespace
@@ -168,7 +109,7 @@ extern "C" int orbfe_window_search(OrbfeMatcher *m, const OrbfeFrameView *f1, co
         Q.push_back({kp1.x, kp1.y, (float)window, level1, level1, f1->desc + (size_t)i1 * 32, kp1.angle, i1});
     }
     for (int i = 0; i < f2->n; i++) match21_out[i] = -1;
-    return orbfe::guided_host(m, *f2, (int)Q.size(), Q.data(), 1, nnratio, kThHigh, check_orientation, match21_out, nmatches_out);
+    return orbfe::guided_host(m, *f2, (int)Q.size(), Q.data(), 1, nnratio, kThHigh, check_orientation, match21_out, nullptr, nmatches_out);
 }
 
 // SearchByProjection(Frame &F, const vector<MapPoint*>&, th), ORBmatcher.cc:49-125
@@ -190,7 +131,7 @@ extern "C" int orbfe_search_local_points(OrbfeMatcher *m, const OrbfeFrameView *
         const int lv = level[i];
         Q.push_back({proj_xy[2 * i], proj_xy[2 * i + 1], r * f->scale_factors[lv], lv - 1, lv, desc + (size_t)i * 32, 0.f, i});
     }
-    return orbfe::guided_host(m, *f, (int)Q.size(), Q.data(), 2, nnratio, kThHigh, 0, f_mp_inout, nmatches_out);
+    return orbfe::guided_host(m, *f, (int)Q.size(), Q.data(), 2, nnratio, kThHigh, 0, f_mp_inout, nullptr, nmatches_out);
 }
 
 // SearchByProjection(Frame &CurrentFrame, KeyFrame *pKF, sAlreadyFound, th, ORBdist), ORBmatcher.cc:1622-1746
@@ -225,7 +166,8 @@ extern "C" int orbfe_search_by_projection_kf(OrbfeMatcher *m, const OrbfeFrameVi
         const int lv = std::min(it, cur->nlevels - 1);
         Q.push_back({u, v, th * sf[lv], lv - 1, lv + 1, desc + (size_t)i * 32, kf_angle[i], i});
     }
-    return orbfe::guided_host(m, *cur, (int)Q.size(), Q.data(), 0, 0.f, orb_dist, check_orientation, cur_mp_inout, nmatches_out);
+    return orbfe::guided_host(m, *cur, (int)Q.size(), Q.data(), 0, 0.f, orb_dist, check_orientation, cur_mp_inout, nullptr,
+                              nmatches_out);
 }
 
 // SearchByProjection(Frame &F1, Frame &F2, int windowSize, vpMapPointMatches2), ORBmatcher.cc:519-594
@@ -244,7 +186,7 @@ extern "C" int orbfe_search_by_projection_f1f2(OrbfeMatcher *m, const OrbfeFrame
         const float invz = (float)(1.0 / (double)xc[2]);
         Q.push_back({fx * xc[0] * invz + cx, fy * xc[1] * invz + cy, (float)window, level1, level1, f1->desc + (size_t)i1 * 32, 0.f, i1});
     }
-    return orbfe::guided_host(m, *f2, (int)Q.size(), Q.data(), 1, nnratio, kThHigh, 0, f2_mp_inout, nmatches_out);
+    return orbfe::guided_host(m, *f2, (int)Q.size(), Q.data(), 1, nnratio, kThHigh, 0, f2_mp_inout, nullptr, nmatches_out);
 }
 
 // Exported form of the guided search for callers that do their own projection (the KeyFrame-level routines
@@ -261,35 +203,19 @@ extern "C" int orbfe_guided_search(OrbfeMatcher *m, const OrbfeFrameView *f, int
     std::vector<GuidedQuery> Q(nq);
     for (int q = 0; q < nq; q++) Q[q] = {qu[q], qv[q], qr[q], qlo[q], qhi[q], qdesc + (size_t)q * 32, qangle ? qangle[q] : 0.f, q};
     // hist_mode 2 fills the histogram without applying it: the same matches as 0
-    return orbfe::guided_host(m, *f, nq, Q.data(), rule, nnratio, th_dist, hist_mode == 1, slot_owner_inout, nmatches_out);
+    return orbfe::guided_host(m, *f, nq, Q.data(), rule, nnratio, th_dist, hist_mode == 1, slot_owner_inout, nullptr, nmatches_out);
 }
 
 // Guided search without slot bookkeeping (Fuse :1090-1107 / :1222-1239, SearchBySim3 :1356-1378 / :1436-1458):
-// best candidate per query, kept iff best <= th_dist.  One distance launch for all queries.
+// best candidate per query, kept iff best <= th_dist.
 extern "C" int orbfe_guided_best(OrbfeMatcher *m, const OrbfeFrameView *f, int nq, const float *qu, const float *qv, const float *qr,
                                  const int32_t *qlo, const int32_t *qhi, const uint8_t *qdesc, int th_dist, int32_t *best_idx_out) {
-    if (!m || !f || nq < 0 || !best_idx_out) return ORBFE_ERR_ARG;
-    if (nq > 0 && (!qu || !qv || !qr || !qlo || !qhi || !qdesc)) return ORBFE_ERR_ARG;
-    Grid grid;
-    build_grid(*f, grid);
-    std::vector<int32_t> row_ptr(1, 0), cols;
-    std::vector<int> tmp;
-    for (int q = 0; q < nq; q++) {
-        tmp.clear();
-        features_in_area(*f, grid, qu[q], qv[q], qr[q], qlo[q], qhi[q], tmp);
-        cols.insert(cols.end(), tmp.begin(), tmp.end());
-        row_ptr.push_back((int32_t)cols.size());
-        best_idx_out[q] = -1;
-    }
-    if (cols.empty()) return ORBFE_OK;
-    std::vector<uint16_t> dist(cols.size());
-    const int rc = orbfe_hamming_csr(m, qdesc, nq, f->desc, f->n, row_ptr.data(), cols.data(), dist.data());
-    if (rc) return rc;
-    for (int q = 0; q < nq; q++) {
-        int bestDist = INT_MAX, bestIdx = -1;
-        for (int c = row_ptr[q]; c < row_ptr[q + 1]; c++)
-            if (dist[c] < bestDist) { bestDist = dist[c]; bestIdx = cols[c]; }
-        if (bestDist <= th_dist) best_idx_out[q] = bestIdx;
-    }
-    return ORBFE_OK;
+    if (!m || !f || nq < 0 || !best_idx_out || f->n < 0 || (f->n > 0 && (!f->keys_un || !f->desc)))
+        return set_error(ORBFE_ERR_ARG, "orbfe_guided_best: bad arguments");
+    if (nq > 0 && (!qu || !qv || !qr || !qlo || !qhi || !qdesc))
+        return set_error(ORBFE_ERR_ARG, "orbfe_guided_best: NULL argument");
+    std::vector<GuidedQuery> Q(nq);
+    for (int q = 0; q < nq; q++) Q[q] = {qu[q], qv[q], qr[q], qlo[q], qhi[q], qdesc + (size_t)q * 32, 0.f, q};
+    int nkept;
+    return orbfe::guided_host(m, *f, nq, Q.data(), SBP_RULE_BEST, 0.f, th_dist, 0, nullptr, best_idx_out, &nkept);
 }

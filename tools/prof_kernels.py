@@ -30,6 +30,9 @@
   --what windowed  wall time per call of the host-array windowed matchers (staging, launch, copy back, synchronise):
                    orbfe_search_by_projection_frames for 1 and 8 pairs, orbfe_search_local_points and orbfe_window_search at
                    1080p / 2000 keypoints, orbfe_search_for_initialization at 720p / 2000 keypoints
+  --what guided    wall time per call of orbfe_guided_best and orbfe_guided_search (rule 0, no histogram) for 1000, 5000 and
+                   30000 Fuse / SearchBySim3 windows on one 1080p / 2000-keypoint keyframe; --baseline-lib PATH alternates
+                   every call with another build of liborbfe.so in the same process and compares the outputs
 
 Prints one JSON object per --what; never a bench value when run under ncu."""
 import argparse
@@ -624,6 +627,86 @@ def windowed(args):
     return out
 
 
+def guided(args):
+    """orbfe_guided_best and orbfe_guided_search (rule 0, no histogram) one call at a time, as the facade's Fuse,
+    SearchBySim3 and SearchByProjection(KeyFrame*, Scw, ...) call them: median wall ms per call (staging, launch, copy back,
+    synchronise) for 1000, 5000 and 30000 windows on one extracted 1920x1080 keyframe of 2000 features.  Windows are map
+    points seen from a nearby pose: centred near a feature, radius th = 3 times the scale factor of the predicted level,
+    levels [lv - 1, lv].  With --baseline-lib the same calls alternate with that build of liborbfe.so in one process, and
+    same_as_baseline compares every output (a refused call is recorded as null)."""
+    import orb_slam_b200 as fe
+    from orb_slam_b200 import matching as M
+    from orb_slam_b200.synth import noisy_copies, textured_frame
+    NF, W, H = 2000, 1920, 1080
+    ex = fe.ORBextractor(NF, 1.2, 8)
+    kps, desc, cnt = ex.extract_batch(textured_frame(W, H, seed=9)[None])
+    ex.close()
+    k, d = kps[0, :cnt[0]], desc[0, :cnt[0]]
+    view = M.FrameView(k, d, W, H)
+    vp = C.c_void_p
+    libs = {"this": fe.lib()}
+    if args.baseline_lib:
+        libs["baseline"] = C.CDLL(os.path.abspath(args.baseline_lib))
+    handles = {}
+    for name, L in libs.items():
+        L.orbfe_matcher_create.argtypes = [C.c_int, C.POINTER(vp)]
+        L.orbfe_matcher_destroy.argtypes = [vp]
+        L.orbfe_guided_best.argtypes = [vp, vp, C.c_int] + [vp] * 6 + [C.c_int, vp]
+        L.orbfe_guided_search.argtypes = [vp, vp, C.c_int] + [vp] * 7 + [C.c_int, C.c_float, C.c_int, C.c_int, vp, vp]
+        h = vp()
+        assert L.orbfe_matcher_create(0, C.byref(h)) == 0, name
+        handles[name] = h
+    p = lambda a: a.ctypes.data_as(vp)
+    rng = np.random.default_rng(5)
+    out = {"what": "guided_best / guided_search (rule 0, hist 0) wall ms per call, 1920x1080 keyframe, %d features" % len(k),
+           "baseline": args.baseline_lib or None}
+    same = True
+    for nq in (1000, 5000, 30000):
+        src = rng.integers(0, len(k), nq)
+        lv = np.clip(k["octave"][src].astype(np.int32) + rng.integers(-1, 2, nq), 0, 7).astype(np.int32)
+        qu = (k["x"][src] + rng.normal(0, 1.5, nq)).astype(np.float32)
+        qv = (k["y"][src] + rng.normal(0, 1.5, nq)).astype(np.float32)
+        qr = (np.float32(3.0) * view.sf[lv]).astype(np.float32)
+        lo, hi = (lv - 1).astype(np.int32), lv
+        qd = noisy_copies(d[src], 0.1, 6)
+        res = {}
+
+        def best(name):
+            o = np.full(nq, -1, np.int32)
+            rc = libs[name].orbfe_guided_best(handles[name], C.byref(view.c), nq, p(qu), p(qv), p(qr), p(lo), p(hi), p(qd), 50, p(o))
+            return o if rc == 0 else None
+
+        def search(name):
+            so, nm = np.full(len(k), -1, np.int32), C.c_int(0)
+            rc = libs[name].orbfe_guided_search(handles[name], C.byref(view.c), nq, p(qu), p(qv), p(qr), p(lo), p(hi), p(qd), None,
+                                                0, 0.0, 50, 0, p(so), C.byref(nm))
+            return (nm.value, so) if rc == 0 else None
+        for fn_name, fn in (("best", best), ("search", search)):
+            for name in libs:
+                for _ in range(args.warmup):
+                    res[(fn_name, name)] = fn(name)
+            lat = {name: [] for name in libs}
+            order = list(libs)
+            for it in range(args.iters * 20):
+                for name in (order if it % 2 == 0 else order[::-1]):   # alternate which build goes first
+                    t0 = time.perf_counter()
+                    fn(name)
+                    lat[name].append((time.perf_counter() - t0) * 1e3)
+            for name in libs:
+                r = res[(fn_name, name)]
+                out["%s_%d_%s_wall_ms" % (fn_name, nq, name)] = float(np.median(lat[name])) if r is not None else None
+            r0 = res[(fn_name, "this")]
+            out["%s_%d_kept" % (fn_name, nq)] = int((r0 >= 0).sum()) if fn_name == "best" else r0[0]
+            if "baseline" in libs and res[(fn_name, "baseline")] is not None:
+                rb = res[(fn_name, "baseline")]
+                same &= bool(np.array_equal(r0, rb)) if fn_name == "best" else (r0[0] == rb[0] and bool(np.array_equal(r0[1], rb[1])))
+    out["same_as_baseline"] = same if "baseline" in libs else None
+    for name, L in libs.items():
+        L.orbfe_matcher_destroy(handles[name])
+    _gpu_and_power_limit(out)
+    return out
+
+
 def exchange1(args):
     """The exchange variant of the descriptor kernel with a world of ONE rank (its peer table holds only this GPU): what the
     remote-store code path, the acknowledgement poll and the publish cost by themselves, without NVLink or a second rank."""
@@ -1062,8 +1145,9 @@ if __name__ == "__main__":
     ap.add_argument("--groups", type=int, default=10000)
     ap.add_argument("--iters", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--baseline-lib", default=None, help="--what guided: another build of liborbfe.so to time alternately")
     args = ap.parse_args()
     for w in args.what.split(","):
         print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fast": fast, "latency": latency,
                           "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb, "bowchain": bowchain,
-                          "windowed": windowed}[w](args)))
+                          "windowed": windowed, "guided": guided}[w](args)))
