@@ -148,6 +148,12 @@ typedef struct OrbfeKeyFrameDB OrbfeKeyFrameDB;
  * device is the vocabulary's.  Every buffer is allocated here (about 44 bytes per posting, 8 per vocabulary word and
  * 150 per slot); no later call allocates device memory. */
 int orbfe_kfdb_create(OrbfeVocabulary *v, int max_keyframes, long long max_postings, OrbfeKeyFrameDB **out);
+/* orbfe_kfdb_create with room for batches of up to max_queries queries (1 <= max_queries <= 1024, else ORBFE_ERR_ARG);
+ * orbfe_kfdb_create is this call with max_queries = 1.  Every buffer is still allocated here: each query slot adds
+ * 40 * max_keyframes + 12 * S + 16 bytes of device memory, S = max_keyframes rounded up to a power of two (per query: the
+ * query state, connected stamps, touched list, scores, accumulations, best covisibles and first-entry tags of every slot,
+ * and the sorted sharing list). */
+int orbfe_kfdb_create_batched(OrbfeVocabulary *v, int max_keyframes, long long max_postings, int max_queries, OrbfeKeyFrameDB **out);
 void orbfe_kfdb_destroy(OrbfeKeyFrameDB *db);
 
 /* add(pKF) (:39-45): the BowVector ids/vals[0, nw) (word ids strictly ascending, < the vocabulary's word count) of a NEW
@@ -198,6 +204,32 @@ int orbfe_kfdb_detect(OrbfeKeyFrameDB *db, int mode, int nq, const int32_t *q_id
 int orbfe_kfdb_detect_device(OrbfeKeyFrameDB *db, int mode, int nq, const int32_t *d_q_ids, const double *d_q_vals, int nconn,
                              const int32_t *d_connected, float min_score, int cap, int32_t *d_cand, int *d_ncand, int32_t *d_words,
                              float *d_score, void *stream);
+
+/* nqueries queries of one mode in one launch chain, with the results of nqueries consecutive orbfe_kfdb_detect_device
+ * calls made in order b = 0 .. nqueries-1, bit for bit: query b gets the b-th of nqueries consecutive query ids, and its
+ * candidates, counts, words and scores, and the mLoopScore / mRelocScore left for later calls, are those calls'.  In
+ * particular, a slot query b touched but did not score (too few shared words, or connected in loop mode) keeps the score
+ * the last query a < b of the batch that scored it computed, or the score from before the batch when none did; that is
+ * the value query b reports in d_score and, in relocalisation mode, adds into its covisibility accumulation
+ * (KeyFrameDatabase.cc:272-281).  No query sees a score of a later query of its batch.  After the batch, every slot
+ * scored in it holds the score of the last query that scored it.
+ *   Query b is row b of d_q_ids / d_q_vals (entries b*qcap .. b*qcap+qcap-1, ids ascending); entries after the real words
+ *   with ids >= the vocabulary's word count are ignored, so a block of orbfe_bow_vector_device rows is passed as it is with
+ *   qcap = its cap.  Loop mode (0): query b's connected slots are d_connected[d_conn_ptr[b] .. d_conn_ptr[b+1])
+ *   (nqueries + 1 non-decreasing offsets; d_connected may be NULL when every range is empty) and its minScore is
+ *   d_min_score[b]; these are device arrays, so a minimum computed on the device can feed them.  Relocalisation mode (1):
+ *   all three unused, may be NULL.
+ *   Out: row b of d_cand at b*cap (cap entries), d_ncand[b] (the number of candidates; when it exceeds cap only the first
+ *   cap were written), and rows b of d_words / d_score at b*max_keyframes (may be NULL), as orbfe_kfdb_detect_device.
+ * 1 <= nqueries <= the handle's max_queries, 0 <= qcap <= 65535, cap >= 0; anything else is ORBFE_ERR_ARG and leaves the
+ * database unchanged.  Enqueued on `stream` (NULL = the handle's stream), ordered after the handle's previous work like
+ * every orbfe_kfdb_* call, not synchronised: six kernels whatever nqueries, no host round trip.
+ * A batch of loop queries equals the reference only when no add() falls between them: LoopClosing::DetectLoop adds each
+ * keyframe to the database after its own query (LoopClosing.cc:134,209), so consecutive loop queries of the reference
+ * see one more keyframe each. */
+int orbfe_kfdb_detect_batch_device(OrbfeKeyFrameDB *db, int mode, int nqueries, int qcap, const int32_t *d_q_ids, const double *d_q_vals,
+                                   const int32_t *d_conn_ptr, const int32_t *d_connected, const float *d_min_score, int cap,
+                                   int32_t *d_cand, int *d_ncand, int32_t *d_words, float *d_score, void *stream);
 
 #ifdef __cplusplus
 }

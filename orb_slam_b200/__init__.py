@@ -56,7 +56,7 @@ ABI_SYMBOLS = [
     "orbfe_distinctive_descriptors", "orbfe_bow_db_detect", "orbfe_feature_vector_device", "orbfe_distinctive_descriptors_device",
     "orbfe_bow_vector_device",
     "orbfe_kfdb_create", "orbfe_kfdb_destroy", "orbfe_kfdb_add", "orbfe_kfdb_add_device", "orbfe_kfdb_erase", "orbfe_kfdb_clear", "orbfe_kfdb_set_covisibles",
-    "orbfe_kfdb_size", "orbfe_kfdb_detect", "orbfe_kfdb_detect_device",
+    "orbfe_kfdb_size", "orbfe_kfdb_detect", "orbfe_kfdb_detect_device", "orbfe_kfdb_create_batched", "orbfe_kfdb_detect_batch_device",
 ]
 
 

@@ -175,6 +175,8 @@ def _bind_kfdb():
     L.orbfe_kfdb_size.argtypes = [vp, vp, vp]
     L.orbfe_kfdb_detect.argtypes = [vp, i, i, vp, vp, i, vp, C.c_float, i, vp, vp, vp, vp]
     L.orbfe_kfdb_detect_device.argtypes = [vp, i, i, vp, vp, i, vp, C.c_float, i, vp, vp, vp, vp, vp]
+    L.orbfe_kfdb_create_batched.argtypes = [vp, i, C.c_longlong, i, C.POINTER(vp)]
+    L.orbfe_kfdb_detect_batch_device.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp, i, vp, vp, vp, vp, vp]
     _kfdb_bound = True
     return L
 
@@ -182,15 +184,15 @@ def _bind_kfdb():
 class KeyFrameDatabase:
     """KeyFrameDatabase (reference src/KeyFrameDatabase.cc) resident on the vocabulary's device: keyframes are slots
     0 <= slot < max_keyframes, the inverted file, BowVectors, covisibility lists and the per-keyframe query fields live in
-    device memory (include/orbfe_bow.h, orbfe_kfdb_*)."""
+    device memory (include/orbfe_bow.h, orbfe_kfdb_*).  max_queries: the largest batch detect_batch_device takes."""
 
     LOOP, RELOC = 0, 1
 
-    def __init__(self, voc: "Vocabulary", max_keyframes, max_postings):
+    def __init__(self, voc: "Vocabulary", max_keyframes, max_postings, max_queries=1):
         L = _bind_kfdb()
         h = C.c_void_p()
-        _check(L.orbfe_kfdb_create(voc.handle, int(max_keyframes), int(max_postings), C.byref(h)))
-        self._h, self.max_keyframes, self._voc = h.value, int(max_keyframes), voc
+        _check(L.orbfe_kfdb_create_batched(voc.handle, int(max_keyframes), int(max_postings), int(max_queries), C.byref(h)))
+        self._h, self.max_keyframes, self.max_queries, self._voc = h.value, int(max_keyframes), int(max_queries), voc
 
     @property
     def handle(self):
@@ -261,3 +263,15 @@ class KeyFrameDatabase:
         vp = C.c_void_p
         _check(_bind_kfdb().orbfe_kfdb_detect_device(self._h, mode, nq, vp(d_q_ids), vp(d_q_vals), nconn, vp(d_connected), min_score, cap,
                                                      vp(d_cand), vp(d_ncand), vp(d_words or None), vp(d_score or None), vp(stream)))
+
+    def detect_batch_device(self, mode, nqueries, qcap, d_q_ids, d_q_vals, d_conn_ptr, d_connected, d_min_score, cap, d_cand, d_ncand,
+                            d_words=0, d_score=0, stream=0):
+        """nqueries queries of one mode as nqueries consecutive detect_device calls (ints = raw device addresses): query b is
+        row b of d_q_ids / d_q_vals (qcap entries each); in loop mode its connected slots are
+        d_connected[d_conn_ptr[b]:d_conn_ptr[b+1]] and its minScore d_min_score[b].  Row b of d_cand at b*cap, d_ncand[b],
+        rows b of d_words / d_score at b*max_keyframes.  Enqueued, not synchronised."""
+        vp = C.c_void_p
+        _check(_bind_kfdb().orbfe_kfdb_detect_batch_device(self._h, mode, nqueries, qcap, vp(d_q_ids or None), vp(d_q_vals or None),
+                                                           vp(d_conn_ptr or None), vp(d_connected or None), vp(d_min_score or None), cap,
+                                                           vp(d_cand or None), vp(d_ncand or None), vp(d_words or None), vp(d_score or None),
+                                                           vp(stream)))

@@ -14,14 +14,25 @@
 //            mnLoopWords/mnRelocWords, updated by CAS so no per-query clearing is needed), mLoopScore / mRelocScore
 //            (persistent: the relocalisation accumulation reads scores of earlier queries, :272-281), and the best
 //            covisibility list (at most 10 slots, GetBestCovisibilityKeyFrames(10)).
-// A query is five launches on one stream and no host synchronisation:
-//   kfdb_begin_kernel   stamps the query keyframe's connected slots (loop mode) and resets the touched counter;
-//   kfdb_walk_kernel    one thread per query word walks that word's list: counts shared words, keeps the lowest shared
-//                       word rank, and the first touch appends the slot to the touched list (lKFsSharingWords, unordered);
-//   kfdb_order_kernel   one block: maxCommonWords over the touched slots, the threshold, and the qualifying slots sorted by
-//                       (first shared word rank, add order) -- the order of lKFsSharingWords;
-//   kfdb_score_kernel   one thread per qualifying slot: the L1 score (bow_l1.cuh, the walk bow_db_score_kernel uses);
-//   kfdb_select_kernel  one block: covisibility accumulation and candidate selection in list order, and the outputs.
+//   rows     one row per query of a batch (max_queries rows, row b at b * max_keyframes, or b * sortcap for the sorted list):
+//            the packed query state, the connected stamps, the touched and sorted lists, the scores the query computed
+//            (`scored`: query id << 32 | float bits), the accumulations, the best covisibles and the first-entry tags.
+//            Every row entry is keyed on the query id of its row, so no row is ever cleared.
+// A batch of B queries (B = 1 for orbfe_kfdb_detect_device) gets B consecutive query ids and is six launches on one
+// stream (five when B = 1: the score kernel then writes the scores back itself), no host synchronisation:
+//   kfdb_begin_kernel     stamps each query keyframe's connected slots (loop mode) and resets the touched counters;
+//   kfdb_walk_kernel      one thread per (query, word) walks that word's list: counts shared words, keeps the lowest shared
+//                         word rank, and the first touch appends the slot to the query's touched list (lKFsSharingWords,
+//                         unordered);
+//   kfdb_order_kernel     one block per query: maxCommonWords over the touched slots, the threshold, and the qualifying
+//                         slots sorted by (first shared word rank, add order) -- the order of lKFsSharingWords;
+//   kfdb_score_kernel     one thread per (query, qualifying slot): the L1 score (bow_l1.cuh, the walk bow_db_score_kernel
+//                         uses), recorded in the query's row (and, when B = 1, in the slot's persistent score);
+//   kfdb_select_kernel    one block per query: covisibility accumulation and candidate selection in list order, and the
+//                         outputs.  A score read of slot s by query b is the one the last query a <= b of the batch
+//                         computed, else the persistent one: what B calls in order would have read;
+//   kfdb_writeback_kernel the persistent mLoopScore / mRelocScore of every slot scored in the batch, from its last scorer,
+//                         after every select has read the values from before the batch.
 // Every order-dependent step works on the sorted list, so results do not depend on block scheduling.
 #include <algorithm>
 #include <cstring>
@@ -42,13 +53,12 @@ int vocab_nwords(const OrbfeVocabulary *v);
 __global__ void kfdb_link_kernel(int slot, int base, int nw, unsigned seq, const int *__restrict__ s_id, const int *__restrict__ s_node,
                                  int *__restrict__ n_slot, int *__restrict__ n_next, int *__restrict__ n_prev, int *__restrict__ w_head,
                                  int *__restrict__ w_tail, int *__restrict__ range, unsigned *__restrict__ seqs,
-                                 unsigned long long *__restrict__ state, float *__restrict__ lscore, float *__restrict__ rscore) {
+                                 float *__restrict__ lscore, float *__restrict__ rscore) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i == 0) {   // a fresh KeyFrame: stamps 0, scores 0
+    if (i == 0) {   // a fresh KeyFrame: scores 0; its stamps are older query ids than any later query's, as 0 would be
         range[2 * slot] = base;
         range[2 * slot + 1] = base + nw;
         seqs[slot] = seq;
-        state[slot] = 0ull;
         lscore[slot] = 0.f;
         rscore[slot] = 0.f;
     }
@@ -138,24 +148,46 @@ __device__ __forceinline__ unsigned q_stamp(unsigned long long st) { return (uns
 __device__ __forceinline__ int q_rank(unsigned long long st) { return (int)((st >> 16) & 0xFFFFu); }
 __device__ __forceinline__ int q_words(unsigned long long st) { return (int)(st & 0xFFFFu); }
 
-__global__ void kfdb_begin_kernel(int loop, unsigned qid, const int *__restrict__ connected, int nconn, int K, unsigned *__restrict__ conn,
-                                  int *__restrict__ info) {
-    if (blockIdx.x == 0 && threadIdx.x == 0) info[0] = 0;   // touched count
-    if (!loop) return;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nconn; i += gridDim.x * blockDim.x) {
+// The score of slot s as query b of the batch reads it: the one the last query a <= b of the batch computed (its
+// mLoopScore / mRelocScore after query a), else the one left before the batch (KeyFrameDatabase.cc:272-281).
+__device__ __forceinline__ float kfdb_score_read(int b, unsigned qid0, int s, int K, const unsigned long long *__restrict__ scored,
+                                                 const float *__restrict__ sc) {
+    const float before = sc[s];   // loaded with the first row's entry, not after the scan
+    for (int a = b; a >= 0; a--) {
+        const unsigned long long v = scored[(size_t)a * K + s];
+        if ((unsigned)(v >> 32) == qid0 + (unsigned)a) return __uint_as_float((unsigned)v);
+    }
+    return before;
+}
+
+// grid (x, queries): query b stamps d_connected[conn_ptr[b] .. conn_ptr[b+1]) into its row; without conn_ptr (one query)
+// the range is [0, nconn)
+__global__ void kfdb_begin_kernel(int loop, unsigned qid0, const int *__restrict__ conn_ptr, const int *__restrict__ connected, int nconn,
+                                  int K, unsigned *__restrict__ conn, int *__restrict__ info) {
+    const int b = blockIdx.y;
+    if (blockIdx.x == 0 && threadIdx.x == 0) info[4 * b] = 0;   // touched count
+    if (!loop || !connected) return;
+    const int lo = conn_ptr ? conn_ptr[b] : 0, hi = conn_ptr ? conn_ptr[b + 1] : nconn;
+    unsigned *cb = conn + (size_t)b * K;
+    for (int i = lo + blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += gridDim.x * blockDim.x) {
         const int c = connected[i];
-        if ((unsigned)c < (unsigned)K) conn[c] = qid;
+        if ((unsigned)c < (unsigned)K) cb[c] = qid0 + b;
     }
 }
 
-__global__ void __launch_bounds__(128) kfdb_walk_kernel(unsigned qid, int nq, const int *__restrict__ q_ids, int nwords,
+// grid (words, queries): query b's words are q_ids[b * qcap .. b * qcap + qcap)
+__global__ void __launch_bounds__(128) kfdb_walk_kernel(unsigned qid0, int nq, const int *__restrict__ q_ids, int nwords,
                                                         const int *__restrict__ w_head, const int *__restrict__ n_slot,
-                                                        const int *__restrict__ n_next, unsigned long long *__restrict__ state,
+                                                        const int *__restrict__ n_next, unsigned long long *__restrict__ state, int K,
                                                         int *__restrict__ touched, int *__restrict__ info) {
-    const int qi = blockIdx.x * blockDim.x + threadIdx.x;
+    const int qi = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
     if (qi >= nq) return;
-    const int w = q_ids[qi];
+    const unsigned qid = qid0 + b;
+    const int w = q_ids[(size_t)b * nq + qi];
     if ((unsigned)w >= (unsigned)nwords) return;
+    state += (size_t)b * K;
+    touched += (size_t)b * K;
+    info += 4 * b;
     for (int nd = w_head[w]; nd >= 0; nd = n_next[nd]) {
         const int s = n_slot[nd];
         unsigned long long old = state[s], assumed;
@@ -172,12 +204,20 @@ __global__ void __launch_bounds__(128) kfdb_walk_kernel(unsigned qid, int nq, co
     }
 }
 
-// info: [0] touched, [1] list length, [2] minCommonWords
-__global__ void __launch_bounds__(KFDB_BLOCK) kfdb_order_kernel(int loop, unsigned qid, const unsigned long long *__restrict__ state,
+// one block per query; info row b: [0] touched, [1] list length, [2] minCommonWords
+__global__ void __launch_bounds__(KFDB_BLOCK) kfdb_order_kernel(int loop, unsigned qid0, const unsigned long long *__restrict__ state,
                                                                 const unsigned *__restrict__ conn, const unsigned *__restrict__ seqs,
                                                                 const int *__restrict__ touched, int *__restrict__ info,
-                                                                unsigned long long *__restrict__ keys, int *__restrict__ list, int K) {
+                                                                unsigned long long *__restrict__ keys, int *__restrict__ list, int K, int S) {
     __shared__ int sh[2];   // [0] list length, [1] maxCommonWords
+    const int b = blockIdx.x;
+    const unsigned qid = qid0 + b;
+    state += (size_t)b * K;
+    conn += (size_t)b * K;
+    touched += (size_t)b * K;
+    info += 4 * b;
+    keys += (size_t)b * S;
+    list += (size_t)b * S;
     const int nt = min(info[0], K);
     if (threadIdx.x == 0) sh[0] = sh[1] = 0;
     __syncthreads();
@@ -226,21 +266,41 @@ __global__ void __launch_bounds__(KFDB_BLOCK) kfdb_order_kernel(int loop, unsign
     if (threadIdx.x == 0) { info[1] = nl; info[2] = minCommon; }
 }
 
-__global__ void __launch_bounds__(128) kfdb_score_kernel(int loop, int nq, const int *__restrict__ q_ids, const double *__restrict__ q_vals,
-                                                         const int *__restrict__ info, const int *__restrict__ list, const int *__restrict__ range,
-                                                         const int *__restrict__ s_id, const double *__restrict__ s_val, float *__restrict__ lsc,
-                                                         float *__restrict__ lscore, float *__restrict__ rscore) {
-    const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= info[1]) return;
-    const int s = list[e];
+// grid (list entries, queries): query b's entry e records pKFi->mLoopScore / mRelocScore = si in the query's row; for a
+// batch of one (`persist` = the mode's persistent scores) also in the slot itself, which is then the write-back
+__global__ void __launch_bounds__(128) kfdb_score_kernel(unsigned qid0, int nq, const int *__restrict__ q_ids, const double *__restrict__ q_vals,
+                                                         const int *__restrict__ info, const int *__restrict__ list, int S,
+                                                         const int *__restrict__ range, const int *__restrict__ s_id,
+                                                         const double *__restrict__ s_val, unsigned long long *__restrict__ scored, int K,
+                                                         float *__restrict__ persist) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+    if (e >= info[4 * b + 1]) return;
+    const int s = list[(size_t)b * S + e];
     int common, first;
-    const float si = (float)bow_l1_walk(nq, q_ids, q_vals, range[2 * s], range[2 * s + 1], s_id, s_val, common, first);
-    lsc[e] = si;
-    if (loop) lscore[s] = si; else rscore[s] = si;   // pKFi->mLoopScore / mRelocScore = si
+    const size_t q0 = (size_t)b * nq;
+    const float si = (float)bow_l1_walk(nq, q_ids + q0, q_vals + q0, range[2 * s], range[2 * s + 1], s_id, s_val, common, first);
+    scored[(size_t)b * K + s] = ((unsigned long long)(qid0 + b) << 32) | __float_as_uint(si);
+    if (persist) persist[s] = si;
 }
 
-__global__ void __launch_bounds__(KFDB_BLOCK) kfdb_select_kernel(int loop, unsigned qid, float min_score, int K, const int *__restrict__ info,
-                                                                 const int *__restrict__ list, const float *__restrict__ lsc,
+// grid (list entries, queries): the persistent score of a slot query b scored, unless a later query of the batch scored
+// it too; runs after every select of the batch
+__global__ void __launch_bounds__(128) kfdb_writeback_kernel(int loop, unsigned qid0, int nb, int K, int S, const int *__restrict__ info,
+                                                             const int *__restrict__ list, const unsigned long long *__restrict__ scored,
+                                                             float *__restrict__ lscore, float *__restrict__ rscore) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+    if (e >= info[4 * b + 1]) return;
+    const int s = list[(size_t)b * S + e];
+    for (int a = b + 1; a < nb; a++)
+        if ((unsigned)(scored[(size_t)a * K + s] >> 32) == qid0 + (unsigned)a) return;
+    const float si = __uint_as_float((unsigned)scored[(size_t)b * K + s]);
+    if (loop) lscore[s] = si; else rscore[s] = si;
+}
+
+// one block per query
+__global__ void __launch_bounds__(KFDB_BLOCK) kfdb_select_kernel(int loop, unsigned qid0, const float *__restrict__ d_min_score, float min_score0,
+                                                                 int K, int S, const int *__restrict__ info, const int *__restrict__ list,
+                                                                 const unsigned long long *__restrict__ scored,
                                                                  const unsigned long long *__restrict__ state, const unsigned *__restrict__ conn,
                                                                  const float *__restrict__ lscore, const float *__restrict__ rscore,
                                                                  const int *__restrict__ covn, const int *__restrict__ cov,
@@ -250,6 +310,22 @@ __global__ void __launch_bounds__(KFDB_BLOCK) kfdb_select_kernel(int loop, unsig
     __shared__ float s_best, s_wmax[KFDB_BLOCK / 32];
     __shared__ int s_cnt[KFDB_BLOCK / 32];
     __shared__ int s_base;
+    const int q = blockIdx.x;
+    const unsigned qid = qid0 + q;
+    const float min_score = d_min_score ? d_min_score[q] : min_score0;
+    const size_t rk = (size_t)q * K;
+    info += 4 * q;
+    list += (size_t)q * S;
+    state += rk;
+    conn += rk;
+    touched += rk;
+    acc += rk;
+    best += rk;
+    firstpos += rk;
+    cand += (size_t)q * cap;
+    ncand += q;
+    if (words_out) words_out += rk;
+    if (score_out) score_out += rk;
     const int nl = info[1], minCommon = info[2], nt = min(info[0], K);
     const float *sc = loop ? lscore : rscore;
     // words_out / score_out: this query's mnLoopWords / mnRelocWords and mLoopScore / mRelocScore of every touched slot
@@ -263,7 +339,7 @@ __global__ void __launch_bounds__(KFDB_BLOCK) kfdb_select_kernel(int loop, unsig
             const int s = touched[i];
             // a connected keyframe is reset at every visit and never stamped: its mnLoopWords ends at 1 (:92-101)
             if (words_out) words_out[s] = (loop && conn[s] == qid) ? 1 : q_words(state[s]);
-            if (score_out) score_out[s] = sc[s];
+            if (score_out) score_out[s] = kfdb_score_read(q, qid0, s, K, scored, sc);
         }
     }
     if (threadIdx.x == 0) { s_best = loop ? min_score : 0.f; s_base = 0; }
@@ -272,7 +348,7 @@ __global__ void __launch_bounds__(KFDB_BLOCK) kfdb_select_kernel(int loop, unsig
     float mybest = -INFINITY;
     for (int e = threadIdx.x; e < nl; e += blockDim.x) {
         const int s = list[e];
-        const float si = lsc[e];
+        const float si = __uint_as_float((unsigned)scored[rk + s]);
         if (loop && !(si >= min_score)) { best[e] = -1; continue; }
         float bestScore = si, accScore = si;
         int b = s;
@@ -280,9 +356,10 @@ __global__ void __launch_bounds__(KFDB_BLOCK) kfdb_select_kernel(int loop, unsig
         for (int j = 0; j < nc; j++) {
             const int s2 = cov[s * KFDB_COVIS + j];
             const unsigned long long st = state[s2];
+            // an earlier query's score when s2 was only touched; read next to the stamp, used only when s2 counts
+            const float s2c = kfdb_score_read(q, qid0, s2, K, scored, sc);
             if (q_stamp(st) != qid) continue;                                              // mnLoopQuery / mnRelocQuery
             if (loop && (conn[s2] == qid || !(q_words(st) > minCommon))) continue;         // :158
-            const float s2c = sc[s2];
             accScore += s2c;
             if (s2c > bestScore) { b = s2; bestScore = s2c; }
         }
@@ -345,7 +422,7 @@ using namespace orbfe;
     } while (0)
 
 struct OrbfeKeyFrameDB {
-    int device = 0, nwords = 0, K = 0, sortcap = 1;
+    int device = 0, nwords = 0, K = 0, sortcap = 1, Q = 1;   // Q: rows of per-query state (max_queries)
     long long P = 0;
     cudaStream_t stream = nullptr;
     cudaEvent_t last = nullptr;   // the handle's most recent work: every call orders itself after it
@@ -364,8 +441,8 @@ struct OrbfeKeyFrameDB {
     int *moves = nullptr, *covrows = nullptr;
     int *a_info = nullptr;        // add_device: [0] bad-row flag, [1 + i] word count of row i
     unsigned *seqs = nullptr, *conn = nullptr;
-    unsigned long long *state = nullptr, *keys = nullptr, *firstpos = nullptr;
-    float *lscore = nullptr, *rscore = nullptr, *lsc = nullptr, *acc = nullptr;
+    unsigned long long *state = nullptr, *keys = nullptr, *firstpos = nullptr, *scored = nullptr;
+    float *lscore = nullptr, *rscore = nullptr, *acc = nullptr;
     // staging of the host-pointer detect
     int *q_ids = nullptr, *q_conn = nullptr, *o_cand = nullptr, *o_words = nullptr, *o_n = nullptr;
     double *q_vals = nullptr;
@@ -380,7 +457,7 @@ extern "C" void orbfe_kfdb_destroy(OrbfeKeyFrameDB *db) {
     if (db->stream) cudaStreamSynchronize(db->stream);
     void *ptrs[] = {db->s_id[0], db->s_id[1], db->s_node[0], db->s_node[1], db->s_val[0], db->s_val[1], db->n_slot, db->n_next, db->n_prev,
                     db->w_head, db->w_tail, db->range, db->covn, db->cov, db->touched, db->list, db->best, db->info, db->moves, db->covrows,
-                    db->seqs, db->conn, db->state, db->keys, db->firstpos, db->lscore, db->rscore, db->lsc, db->acc, db->q_ids, db->q_conn,
+                    db->seqs, db->conn, db->state, db->keys, db->firstpos, db->lscore, db->rscore, db->scored, db->acc, db->q_ids, db->q_conn,
                     db->o_cand, db->o_words, db->o_n, db->q_vals, db->o_score, db->a_info};
     for (void *p : ptrs) cudaFree(p);
     if (db->last) cudaEventDestroy(db->last);
@@ -406,34 +483,44 @@ static int kfdb_reset(OrbfeKeyFrameDB *db) {
     return ORBFE_OK;
 }
 
-extern "C" int orbfe_kfdb_create(OrbfeVocabulary *v, int max_keyframes, long long max_postings, OrbfeKeyFrameDB **out) {
+#define KFDB_MAX_QUERIES 1024
+
+extern "C" int orbfe_kfdb_create_batched(OrbfeVocabulary *v, int max_keyframes, long long max_postings, int max_queries,
+                                         OrbfeKeyFrameDB **out) {
     if (!out) return set_error(ORBFE_ERR_ARG, "NULL out");
     *out = nullptr;
-    if (!v || max_keyframes < 1 || max_keyframes > (1 << 24) || max_postings < 1 || max_postings > 0x7FFFFFFFLL)
-        return set_error(ORBFE_ERR_ARG, "bad arguments (1 <= max_keyframes <= 2^24, 1 <= max_postings < 2^31)");
+    if (!v || max_keyframes < 1 || max_keyframes > (1 << 24) || max_postings < 1 || max_postings > 0x7FFFFFFFLL || max_queries < 1 ||
+        max_queries > KFDB_MAX_QUERIES)
+        return set_error(ORBFE_ERR_ARG, "bad arguments (1 <= max_keyframes <= 2^24, 1 <= max_postings < 2^31, 1 <= max_queries <= %d)",
+                         KFDB_MAX_QUERIES);
     OrbfeKeyFrameDB *db = new OrbfeKeyFrameDB();
     db->device = vocab_device(v);
     db->nwords = std::max(vocab_nwords(v), 1);
     db->K = max_keyframes;
     db->P = max_postings;
+    db->Q = max_queries;
     while (db->sortcap < db->K) db->sortcap <<= 1;
-    const size_t K = (size_t)db->K, P = (size_t)db->P, W = (size_t)db->nwords, S = (size_t)db->sortcap;
+    const size_t K = (size_t)db->K, P = (size_t)db->P, W = (size_t)db->nwords, S = (size_t)db->sortcap, QK = (size_t)db->Q * K,
+                 QS = (size_t)db->Q * S;
     bool ok = cudaSetDevice(db->device) == cudaSuccess && cudaStreamCreateWithFlags(&db->stream, cudaStreamNonBlocking) == cudaSuccess &&
               cudaEventCreateWithFlags(&db->last, cudaEventDisableTiming) == cudaSuccess;
 #define KFDB_ALLOC(p, n) ok = ok && cudaMalloc((void **)&(p), sizeof(*(p)) * (n)) == cudaSuccess
     for (int h = 0; h < 2; h++) { KFDB_ALLOC(db->s_id[h], P); KFDB_ALLOC(db->s_node[h], P); KFDB_ALLOC(db->s_val[h], P); }
     KFDB_ALLOC(db->n_slot, P); KFDB_ALLOC(db->n_next, P); KFDB_ALLOC(db->n_prev, P);
     KFDB_ALLOC(db->w_head, W); KFDB_ALLOC(db->w_tail, W);
-    KFDB_ALLOC(db->range, 2 * K); KFDB_ALLOC(db->covn, K); KFDB_ALLOC(db->cov, K * KFDB_COVIS); KFDB_ALLOC(db->touched, K);
-    KFDB_ALLOC(db->list, S); KFDB_ALLOC(db->best, K); KFDB_ALLOC(db->info, 4); KFDB_ALLOC(db->moves, 3 * K);
-    KFDB_ALLOC(db->covrows, K * (2 + KFDB_COVIS)); KFDB_ALLOC(db->seqs, K); KFDB_ALLOC(db->conn, K); KFDB_ALLOC(db->state, K);
-    KFDB_ALLOC(db->keys, S); KFDB_ALLOC(db->firstpos, K); KFDB_ALLOC(db->lscore, K); KFDB_ALLOC(db->rscore, K); KFDB_ALLOC(db->lsc, K);
-    KFDB_ALLOC(db->acc, K); KFDB_ALLOC(db->q_ids, KFDB_MAX_NQ); KFDB_ALLOC(db->q_vals, KFDB_MAX_NQ); KFDB_ALLOC(db->q_conn, K);
+    KFDB_ALLOC(db->range, 2 * K); KFDB_ALLOC(db->covn, K); KFDB_ALLOC(db->cov, K * KFDB_COVIS); KFDB_ALLOC(db->moves, 3 * K);
+    KFDB_ALLOC(db->covrows, K * (2 + KFDB_COVIS)); KFDB_ALLOC(db->seqs, K); KFDB_ALLOC(db->lscore, K); KFDB_ALLOC(db->rscore, K);
+    // per-query rows (include/orbfe_bow.h states their size)
+    KFDB_ALLOC(db->touched, QK); KFDB_ALLOC(db->list, QS); KFDB_ALLOC(db->best, QK); KFDB_ALLOC(db->info, 4 * (size_t)db->Q);
+    KFDB_ALLOC(db->conn, QK); KFDB_ALLOC(db->state, QK); KFDB_ALLOC(db->keys, QS); KFDB_ALLOC(db->firstpos, QK);
+    KFDB_ALLOC(db->scored, QK); KFDB_ALLOC(db->acc, QK);
+    KFDB_ALLOC(db->q_ids, KFDB_MAX_NQ); KFDB_ALLOC(db->q_vals, KFDB_MAX_NQ); KFDB_ALLOC(db->q_conn, K);
     KFDB_ALLOC(db->o_cand, K); KFDB_ALLOC(db->o_words, K); KFDB_ALLOC(db->o_score, K); KFDB_ALLOC(db->o_n, 1);
     KFDB_ALLOC(db->a_info, K + 1);
 #undef KFDB_ALLOC
-    ok = ok && cudaMemset(db->conn, 0, sizeof(unsigned) * K) == cudaSuccess && cudaMemset(db->state, 0, sizeof(unsigned long long) * K) == cudaSuccess &&
-         cudaMemset(db->firstpos, 0xFF, sizeof(unsigned long long) * K) == cudaSuccess;
+    ok = ok && cudaMemset(db->conn, 0, sizeof(unsigned) * QK) == cudaSuccess && cudaMemset(db->state, 0, sizeof(unsigned long long) * QK) == cudaSuccess &&
+         cudaMemset(db->scored, 0, sizeof(unsigned long long) * QK) == cudaSuccess &&
+         cudaMemset(db->firstpos, 0xFF, sizeof(unsigned long long) * QK) == cudaSuccess;
     if (!ok) {
         const int rc = set_error(ORBFE_ERR_CUDA, "keyframe database allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
         orbfe_kfdb_destroy(db);
@@ -443,6 +530,10 @@ extern "C" int orbfe_kfdb_create(OrbfeVocabulary *v, int max_keyframes, long lon
     if (rc) { orbfe_kfdb_destroy(db); return rc; }
     *out = db;
     return ORBFE_OK;
+}
+
+extern "C" int orbfe_kfdb_create(OrbfeVocabulary *v, int max_keyframes, long long max_postings, OrbfeKeyFrameDB **out) {
+    return orbfe_kfdb_create_batched(v, max_keyframes, max_postings, 1, out);
 }
 
 // order the handle's stream after the handle's previous work (which may have been enqueued on another stream)
@@ -512,8 +603,8 @@ extern "C" int orbfe_kfdb_add(OrbfeKeyFrameDB *db, int slot, int nw, const int32
         KFDB_TRY(cudaMemcpyAsync(db->s_node[c] + base, nodes.data(), sizeof(int) * nw, cudaMemcpyHostToDevice, s));
     }
     kfdb_link_kernel<<<(std::max(nw, 1) + 255) / 256, 256, 0, s>>>(slot, base, nw, ++db->seq, db->s_id[c], db->s_node[c], db->n_slot, db->n_next,
-                                                                   db->n_prev, db->w_head, db->w_tail, db->range, db->seqs, db->state,
-                                                                   db->lscore, db->rscore);
+                                                                   db->n_prev, db->w_head, db->w_tail, db->range, db->seqs, db->lscore,
+                                                                   db->rscore);
     if ((rc = kfdb_leave(db, s, true))) return rc;
     db->begin[slot] = base;
     db->len[slot] = nw;
@@ -576,7 +667,7 @@ extern "C" int orbfe_kfdb_add_device(OrbfeKeyFrameDB *db, int n, const int32_t *
         const int nw = rows[3 * i + 2];
         kfdb_link_kernel<<<(std::max(nw, 1) + 255) / 256, 256, 0, hs>>>(slots[i], rows[3 * i + 1], nw, ++db->seq, db->s_id[c], db->s_node[c],
                                                                         db->n_slot, db->n_next, db->n_prev, db->w_head, db->w_tail,
-                                                                        db->range, db->seqs, db->state, db->lscore, db->rscore);
+                                                                        db->range, db->seqs, db->lscore, db->rscore);
     }
     if ((rc = kfdb_leave(db, hs, true))) return rc;
     for (int i = 0, pos = 0; i < n; i++) {
@@ -660,6 +751,31 @@ static int kfdb_check_detect(int mode, int nq, int nconn, int cap) {
     return ORBFE_OK;
 }
 
+// nb queries of one mode on the per-query rows 0 .. nb-1, as nb consecutive query ids; enqueued on s.  Query b's words are
+// row b of q_ids / q_vals (qcap entries); its connected slots are conn_ptr's range of `connected` (no conn_ptr: [0, nconn));
+// its minScore is d_min_score[b] (no d_min_score: min_score).
+static void kfdb_queries(OrbfeKeyFrameDB *db, int mode, int nb, int qcap, const int *q_ids, const double *q_vals, const int *conn_ptr,
+                         const int *connected, int nconn, const float *d_min_score, float min_score, int cap, int *cand, int *ncand,
+                         int *words, float *score, cudaStream_t s) {
+    const int loop = mode == 0;
+    const unsigned qid0 = db->qid + 1;
+    db->qid += (unsigned)nb;
+    const int K = db->K, S = db->sortcap, c = db->cur;
+    const int bx = conn_ptr ? 4 : std::max(1, std::min((nconn + 255) / 256, 64));
+    kfdb_begin_kernel<<<dim3(bx, nb), 256, 0, s>>>(loop, qid0, conn_ptr, connected, nconn, K, db->conn, db->info);
+    if (qcap > 0)
+        kfdb_walk_kernel<<<dim3((qcap + 127) / 128, nb), 128, 0, s>>>(qid0, qcap, q_ids, db->nwords, db->w_head, db->n_slot, db->n_next,
+                                                                      db->state, K, db->touched, db->info);
+    kfdb_order_kernel<<<nb, KFDB_BLOCK, 0, s>>>(loop, qid0, db->state, db->conn, db->seqs, db->touched, db->info, db->keys, db->list, K, S);
+    const dim3 per_entry((K + 127) / 128, nb);
+    kfdb_score_kernel<<<per_entry, 128, 0, s>>>(qid0, qcap, q_ids, q_vals, db->info, db->list, S, db->range, db->s_id[c], db->s_val[c],
+                                                db->scored, K, nb == 1 ? (loop ? db->lscore : db->rscore) : nullptr);
+    kfdb_select_kernel<<<nb, KFDB_BLOCK, 0, s>>>(loop, qid0, d_min_score, min_score, K, S, db->info, db->list, db->scored, db->state,
+                                                 db->conn, db->lscore, db->rscore, db->covn, db->cov, db->touched, db->acc, db->best,
+                                                 db->firstpos, cap, cand, ncand, words, score);
+    if (nb > 1) kfdb_writeback_kernel<<<per_entry, 128, 0, s>>>(loop, qid0, nb, K, S, db->info, db->list, db->scored, db->lscore, db->rscore);
+}
+
 extern "C" int orbfe_kfdb_detect_device(OrbfeKeyFrameDB *db, int mode, int nq, const int32_t *d_q_ids, const double *d_q_vals, int nconn,
                                         const int32_t *d_connected, float min_score, int cap, int32_t *d_cand, int *d_ncand,
                                         int32_t *d_words, float *d_score, void *stream) {
@@ -669,19 +785,25 @@ extern "C" int orbfe_kfdb_detect_device(OrbfeKeyFrameDB *db, int mode, int nq, c
         return set_error(ORBFE_ERR_ARG, "NULL argument");
     cudaStream_t s = stream ? (cudaStream_t)stream : db->stream;
     if ((rc = kfdb_enter(db, s))) return rc;
-    const int loop = mode == 0;
-    const unsigned qid = ++db->qid;
-    const int K = db->K, c = db->cur;
-    kfdb_begin_kernel<<<std::max(1, std::min((nconn + 255) / 256, 64)), 256, 0, s>>>(loop, qid, d_connected, loop ? nconn : 0, K, db->conn, db->info);
-    if (nq > 0)
-        kfdb_walk_kernel<<<(nq + 127) / 128, 128, 0, s>>>(qid, nq, d_q_ids, db->nwords, db->w_head, db->n_slot, db->n_next, db->state,
-                                                          db->touched, db->info);
-    kfdb_order_kernel<<<1, KFDB_BLOCK, 0, s>>>(loop, qid, db->state, db->conn, db->seqs, db->touched, db->info, db->keys, db->list, K);
-    kfdb_score_kernel<<<(K + 127) / 128, 128, 0, s>>>(loop, nq, d_q_ids, d_q_vals, db->info, db->list, db->range, db->s_id[c], db->s_val[c],
-                                                      db->lsc, db->lscore, db->rscore);
-    kfdb_select_kernel<<<1, KFDB_BLOCK, 0, s>>>(loop, qid, min_score, K, db->info, db->list, db->lsc, db->state, db->conn, db->lscore,
-                                                db->rscore, db->covn, db->cov, db->touched, db->acc, db->best, db->firstpos, cap, d_cand,
-                                                d_ncand, d_words, d_score);
+    kfdb_queries(db, mode, 1, nq, d_q_ids, d_q_vals, nullptr, d_connected, mode == 0 ? nconn : 0, nullptr, min_score, cap, d_cand, d_ncand,
+                 d_words, d_score, s);
+    return kfdb_leave(db, s, false);
+}
+
+extern "C" int orbfe_kfdb_detect_batch_device(OrbfeKeyFrameDB *db, int mode, int nqueries, int qcap, const int32_t *d_q_ids,
+                                              const double *d_q_vals, const int32_t *d_conn_ptr, const int32_t *d_connected,
+                                              const float *d_min_score, int cap, int32_t *d_cand, int *d_ncand, int32_t *d_words,
+                                              float *d_score, void *stream) {
+    int rc = kfdb_check_detect(mode, qcap, 0, cap);
+    if (rc) return rc;
+    if (nqueries < 1) return set_error(ORBFE_ERR_ARG, "nqueries %d < 1", nqueries);
+    if (!db || !d_ncand || (qcap > 0 && (!d_q_ids || !d_q_vals)) || (mode == 0 && (!d_conn_ptr || !d_min_score)) || (cap > 0 && !d_cand))
+        return set_error(ORBFE_ERR_ARG, "NULL argument");
+    if (nqueries > db->Q) return set_error(ORBFE_ERR_ARG, "nqueries %d > max_queries %d", nqueries, db->Q);
+    cudaStream_t s = stream ? (cudaStream_t)stream : db->stream;
+    if ((rc = kfdb_enter(db, s))) return rc;
+    kfdb_queries(db, mode, nqueries, qcap, d_q_ids, d_q_vals, mode == 0 ? d_conn_ptr : nullptr, mode == 0 ? d_connected : nullptr, 0,
+                 mode == 0 ? d_min_score : nullptr, 0.f, cap, d_cand, d_ncand, d_words, d_score, s);
     return kfdb_leave(db, s, false);
 }
 

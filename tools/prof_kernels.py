@@ -24,6 +24,9 @@
   --what kfdb      the resident KeyFrameDatabase at 1k and 10k keyframes of ~1000 words (ids over 10^6): CUDA-event ms per loop
                    and per relocalisation query, host ms per add / erase, and the wall time of the stateless
                    orbfe_bow_db_detect on the same data
+  --what kfdbbatch the same databases: CUDA-event ms of orbfe_kfdb_detect_batch_device for B = 1, 8, 32, 64 relocalisation
+                   queries (and 64 loop queries at 1k) against B consecutive orbfe_kfdb_detect_device calls, outputs compared;
+                   --baseline-lib PATH alternates the single-query detect_device of another build with this one's
   --what bowchain  the BowVector kernel alone for 1 and 33 1080p / 2000-keypoint frames (CUDA events), relocalisation from an
                    extracted frame to SearchByBoW results against a resident 1000-keyframe database with the BowVector built
                    on the device vs on the host (wall time), and detect_device on a padded row vs its word count
@@ -984,6 +987,163 @@ def kfdb(args):
     return out
 
 
+def kfdbbatch(args):
+    """orbfe_kfdb_detect_batch_device against B consecutive orbfe_kfdb_detect_device calls on one stream (CUDA events, outputs
+    compared), on the databases of --what kfdb (1k and 10k keyframes of about 1000 words, ids over 10^6): B = 1, 8, 32, 64
+    relocalisation queries as padded rows of 2048 entries (about 2000 words each), and one loop-mode line at 1k.  With
+    --baseline-lib, the single-query orbfe_kfdb_detect_device of that build and of this one alternate in one process on
+    twin databases (median of repeated CUDA-event windows of 32 queries each)."""
+    import torch
+    NW, WPK, QW, QCAP = 1_000_000, 1000, 2000, 2048
+    n = NW + 1
+    cp = np.zeros(n + 1, np.int32)
+    cp[1:] = NW
+    voc = {"node_desc": np.zeros((n, 32), np.uint8), "child_ptr": cp, "children": np.arange(1, n, dtype=np.int32),
+           "word_id": np.arange(-1, NW, dtype=np.int32), "weight": np.ones(n)}
+    vp, i_, p = C.c_void_p, C.c_int, (lambda a: a.ctypes.data_as(C.c_void_p))
+    import orb_slam_b200 as fe
+    libs = {"this": fe.lib()}
+    if args.baseline_lib:
+        libs["baseline"] = C.CDLL(os.path.abspath(args.baseline_lib))
+    for L in libs.values():
+        L.orbfe_vocabulary_create.argtypes = [i_, i_, i_, vp, vp, vp, vp, vp, i_, i_]
+        L.orbfe_vocabulary_create.restype = vp
+        L.orbfe_vocabulary_destroy.argtypes = [vp]
+        L.orbfe_kfdb_create.argtypes = [vp, i_, C.c_longlong, C.POINTER(vp)]
+        L.orbfe_kfdb_destroy.argtypes = [vp]
+        L.orbfe_kfdb_add.argtypes = [vp, i_, i_, vp, vp]
+        L.orbfe_kfdb_set_covisibles.argtypes = [vp, i_, vp, vp, vp]
+        L.orbfe_kfdb_detect_device.argtypes = [vp, i_, i_, vp, vp, i_, vp, C.c_float, i_, vp, vp, vp, vp, vp]
+    libs["this"].orbfe_kfdb_create_batched.argtypes = [vp, i_, C.c_longlong, i_, C.POINTER(vp)]
+    libs["this"].orbfe_kfdb_detect_batch_device.argtypes = [vp, i_, i_, i_, vp, vp, vp, vp, vp, i_, vp, vp, vp, vp, vp]
+    vocs = {name: L.orbfe_vocabulary_create(0, n, 1, p(voc["node_desc"]), p(voc["child_ptr"]), p(voc["children"]), p(voc["word_id"]),
+                                            p(voc["weight"]), 0, 1) for name, L in libs.items()}
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    out = {"what": "KeyFrameDatabase batched queries: CUDA-event ms per batch of B vs B consecutive detect_device calls; %d words per "
+                   "keyframe, queries of about %d words as rows of %d, word ids over 10^6" % (WPK, QW, QCAP),
+           "baseline": args.baseline_lib or None}
+    _gpu_and_power_limit(out)
+    try:
+        import subprocess
+        out["sm_clock"] = subprocess.run(["nvidia-smi", "--query-gpu=clocks.sm,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                                         capture_output=True, text=True).stdout.strip()
+    except Exception as e:
+        out["sm_clock"] = "unknown: %r" % e
+    t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dt)).to(dev)
+
+    def events(fn, iters):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        for _ in range(iters):
+            fn()
+        e1.record(stream)
+        stream.synchronize()
+        return e0.elapsed_time(e1) / iters
+
+    for nkf in (1000, 10000):
+        rng = np.random.default_rng(nkf)
+        shift = 100
+        track = rng.integers(0, NW, nkf * shift + 4 * QW)
+
+        def bow_at(pos, nw):
+            w = track[pos:pos + nw].copy()
+            flip = rng.random(nw) < 0.25
+            w[flip] = rng.integers(0, NW, int(flip.sum()))
+            ids = np.unique(w).astype(np.int32)
+            v = rng.uniform(0.2, 3.0, len(ids))
+            return ids, v / v.sum()
+
+        bows = [bow_at(shift * k, WPK) for k in range(nkf)]
+        lists = {k: [j for j in (k - 1, k + 1, k - 2, k + 2, k - 3, k + 3, k - 4, k + 4, k - 5, k + 5) if 0 <= j < nkf] for k in range(nkf)}
+        slots = np.arange(nkf, dtype=np.int32)
+        ptr = np.cumsum([0] + [len(lists[k]) for k in range(nkf)]).astype(np.int32)
+        flat = np.concatenate([np.array(lists[k], np.int32) for k in range(nkf)])
+        P = nkf * WPK + 10 * WPK
+
+        def make(name, max_queries):
+            L, h = libs[name], vp()
+            rc = (L.orbfe_kfdb_create_batched(vocs[name], nkf, P, max_queries, C.byref(h)) if max_queries > 1 else
+                  L.orbfe_kfdb_create(vocs[name], nkf, P, C.byref(h)))
+            assert rc == 0, name
+            for k in range(nkf):
+                ids, vals = np.ascontiguousarray(bows[k][0]), np.ascontiguousarray(bows[k][1])
+                assert L.orbfe_kfdb_add(h, k, len(ids), p(ids), p(vals)) == 0
+            assert L.orbfe_kfdb_set_covisibles(h, nkf, p(slots), p(ptr), p(flat)) == 0
+            return h
+
+        queries = [bow_at(shift * int(rng.integers(0, nkf)) + 7, QW) for _ in range(64)]
+        ids = np.full((64, QCAP), np.iinfo(np.int32).max, np.int32)
+        vals = np.zeros((64, QCAP))
+        for b, (qi, qv) in enumerate(queries):
+            ids[b, :len(qi)], vals[b, :len(qi)] = qi, qv
+        d_ids, d_vals = t(ids, np.int32), t(vals, np.float64)
+        conn = np.arange(10, dtype=np.int32)
+        d_conn, d_cptr = t(np.tile(conn, 64), np.int32), t(np.arange(65) * 10, np.int32)
+        d_ms = t(np.full(64, 0.0), np.float32)
+        res = {"keyframes": nkf, "query_words_mean": float(np.mean([len(q[0]) for q in queries]))}
+        batched, seq = make("this", 64), make("this", 1)
+        L = libs["this"]
+        d_cand = [torch.zeros(64 * nkf, dtype=torch.int32, device=dev) for _ in range(2)]
+        d_n = [torch.zeros(64, dtype=torch.int32, device=dev) for _ in range(2)]
+        torch.cuda.synchronize()
+        modes = [(1, B) for B in (1, 8, 32, 64)] + ([(0, 64)] if nkf == 1000 else [])
+        for mode, Bq in modes:
+            def run_batch():
+                L.orbfe_kfdb_detect_batch_device(batched, mode, Bq, QCAP, d_ids.data_ptr(), d_vals.data_ptr(), d_cptr.data_ptr(), d_conn.data_ptr(),
+                                                 d_ms.data_ptr(), nkf, d_cand[0].data_ptr(), d_n[0].data_ptr(), None, None, stream.cuda_stream)
+
+            def run_seq():
+                for b in range(Bq):
+                    L.orbfe_kfdb_detect_device(seq, mode, QCAP, d_ids[b].data_ptr(), d_vals[b].data_ptr(), 10, d_conn.data_ptr(), 0.0, nkf,
+                                               d_cand[1][b * nkf:].data_ptr(), d_n[1][b:].data_ptr(), None, None, stream.cuda_stream)
+            # same outputs first (both databases have answered the same queries so far), then the timing
+            run_batch()
+            run_seq()
+            stream.synchronize()
+            n0, n1 = d_n[0][:Bq].cpu().numpy(), d_n[1][:Bq].cpu().numpy()
+            c0, c1 = d_cand[0].cpu().numpy(), d_cand[1].cpu().numpy()
+            same = bool(np.array_equal(n0, n1)) and all(np.array_equal(c0[b * nkf:b * nkf + n0[b]], c1[b * nkf:b * nkf + n0[b]]) for b in range(Bq))
+            for _ in range(args.warmup):
+                run_batch()
+                run_seq()
+            tb, ts = [], []
+            for _ in range(5):
+                tb.append(events(run_batch, args.iters))
+                ts.append(events(run_seq, args.iters))
+            tag = "%s_B%d" % ("loop" if mode == 0 else "reloc", Bq)
+            res[tag] = {"batch_ms": round(float(np.median(tb)), 4), "sequential_ms": round(float(np.median(ts)), 4),
+                        "batch_ms_min_max": [round(min(tb), 4), round(max(tb), 4)], "sequential_ms_min_max": [round(min(ts), 4), round(max(ts), 4)],
+                        "speedup": round(float(np.median(ts) / np.median(tb)), 2), "same_outputs": same,
+                        "candidates_mean": float(n0.mean())}
+        L.orbfe_kfdb_destroy(batched)
+        L.orbfe_kfdb_destroy(seq)
+        # single-query regression: this build's detect_device and the baseline's, alternating, on twin databases
+        if "baseline" in libs:
+            hs = {name: make(name, 1) for name in libs}
+            outs = {name: (torch.zeros(nkf, dtype=torch.int32, device=dev), torch.zeros(1, dtype=torch.int32, device=dev)) for name in libs}
+            lat = {name: [] for name in libs}
+            same = True
+            for rep in range(args.iters * 4):
+                for name in (list(libs) if rep % 2 == 0 else list(libs)[::-1]):
+                    def run(name=name):
+                        for b in range(32):
+                            libs[name].orbfe_kfdb_detect_device(hs[name], 1, QCAP, d_ids[b].data_ptr(), d_vals[b].data_ptr(), 0, None, 0.0, nkf,
+                                                                outs[name][0].data_ptr(), outs[name][1].data_ptr(), None, None, stream.cuda_stream)
+                    lat[name].append(events(run, 1) / 32)
+                c = {name: (outs[name][1].item(), outs[name][0][:outs[name][1].item()].cpu().numpy()) for name in libs}
+                same &= c["this"][0] == c["baseline"][0] and bool(np.array_equal(c["this"][1], c["baseline"][1]))
+            for name in libs:
+                res["single_reloc_%s_ms" % name] = round(float(np.median(lat[name][2:])), 4)
+                res["single_reloc_%s_ms_min_max" % name] = [round(min(lat[name][2:]), 4), round(max(lat[name][2:]), 4)]
+                libs[name].orbfe_kfdb_destroy(hs[name])
+            res["single_same_as_baseline"] = same
+        out["%dk" % (nkf // 1000)] = res
+    for name, L in libs.items():
+        L.orbfe_vocabulary_destroy(vocs[name])
+    return out
+
+
 def bowchain(args):
     """The BowVector built on the device (orbfe_bow_vector_device) and the relocalisation chain it completes, on 1920x1080
     frames of 2000 keypoints with a k = 10, L = 6 vocabulary (TF-IDF, L1), levelsup 4:
@@ -1149,5 +1309,5 @@ if __name__ == "__main__":
     args = ap.parse_args()
     for w in args.what.split(","):
         print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fast": fast, "latency": latency,
-                          "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb, "bowchain": bowchain,
+                          "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb, "kfdbbatch": kfdbbatch, "bowchain": bowchain,
                           "windowed": windowed, "guided": guided}[w](args)))
