@@ -2,7 +2,9 @@
  *
  *   N2  DBoW2 vocabulary-tree transform: descriptors -> BowVector + FeatureVector
  *       (reference Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1126-1262, FORB.cpp:79-99 (distance),
- *        BowVector.cpp:34-84, FeatureVector.cpp:32-48; callers Frame.cc:280-287, KeyFrame.cc:56-65)
+ *        BowVector.cpp:34-84, FeatureVector.cpp:32-48; callers Frame.cc:280-287, KeyFrame.cc:56-65),
+ *       and ORBVocabulary::score on the BowVectors it builds (TemplatedVocabulary.h score(), ScoringObject.cpp:23-67;
+ *        caller LoopClosing.cc:117-131)
  *   N3  KeyFrameDatabase::DetectLoopCandidates / DetectRelocalisationCandidates on arrays
  *       (reference src/KeyFrameDatabase.cc:73-308, L1Scoring::score Thirdparty/DBoW2/DBoW2/ScoringObject.cpp:23-67)
  *   N4  MapPoint::ComputeDistinctiveDescriptors, batched over map points (reference src/MapPoint.cc:185-250)
@@ -87,6 +89,35 @@ int orbfe_feature_vector_device(OrbfeVocabulary *v, int nframes, const int32_t *
  * `stream` (NULL = the vocabulary's stream), not synchronised. */
 int orbfe_bow_vector_device(OrbfeVocabulary *v, int nframes, const int32_t *d_leaf, const int *d_counts, int cap, int32_t *d_bow_ids,
                             double *d_bow_vals, int *d_bow_n, void *stream);
+
+/* LoopClosing::DetectLoop's minScore (LoopClosing.cc:117-131) for nqueries keyframes at once, and the ORBVocabulary::score
+ * values it is the minimum of (L1Scoring::score, ScoringObject.cpp:23-67).  BowVector rows in the layout
+ * orbfe_bow_vector_device writes: row f at f*cap holds min(max(d_bow_n[f], 0), cap) words, ids ascending; nothing past that
+ * count is read.
+ *   Query b is row d_query_row[b]; its connected keyframes are rows d_cov_row[d_cov_ptr[b] .. d_cov_ptr[b+1]) in the order of
+ *   GetVectorCovisibleKeyFrames() (nqueries + 1 offsets, read as given).  A connected keyframe with isBad() is passed as a
+ *   negative entry and skipped.  A row index outside [0, nframes) is never followed: as a connected keyframe it is skipped
+ *   too, as a query it is an empty BowVector.
+ *   d_scores (may be NULL; d_cov_ptr[nqueries] entries): d_scores[k] = the double score(query, row d_cov_row[k]), the sum
+ *   over the shared words taken in ascending word order, so (float)d_scores[k] is the d_score the resident database reports
+ *   for that pair in a loop query; no shared word gives -0.0; nothing is clamped, whatever the vocabulary's norm.  Entries of
+ *   skipped keyframes are left untouched.
+ *   d_min_score[b]: `float minScore = 1`, then (float)score wherever that is smaller, in list order: the argument of
+ *   DetectLoopCandidates and entry b of orbfe_kfdb_detect_batch_device's d_min_score.  1.0f when nothing was scored.
+ * One thread block per query, one warp per pair, the query's words staged in shared memory: 1 <= cap <= ORBFE_FV_MAX_CAP,
+ * else ORBFE_ERR_UNSUPPORTED.  nqueries >= 0 (0 does nothing), nframes >= 1, nframes*cap < 2^31, else ORBFE_ERR_ARG.
+ * Arguments are checked before the handle is used.  Enqueued on `stream` (NULL = the vocabulary's stream), not
+ * synchronised, one launch whatever nqueries, no host round trip. */
+int orbfe_bow_min_score_device(OrbfeVocabulary *v, int nqueries, int nframes, int cap, const int32_t *d_bow_ids, const double *d_bow_vals,
+                               const int *d_bow_n, const int32_t *d_query_row, const int32_t *d_cov_ptr, const int32_t *d_cov_row,
+                               double *d_scores, float *d_min_score, void *stream);
+
+/* ORBVocabulary::score(v1, v2) of two host BowVectors (ids ascending; n = 0 may pass NULL), on the kernel of
+ * orbfe_bow_min_score_device: one query with one connected keyframe, so *score_out is the d_scores entry of that pair.
+ * 0 <= n1, n2 <= ORBFE_FV_MAX_CAP, else ORBFE_ERR_UNSUPPORTED.  Synchronous; may be called from several threads on one
+ * vocabulary, like orbfe_bow_transform. */
+int orbfe_bow_score(OrbfeVocabulary *v, int n1, const int32_t *ids1, const double *vals1, int n2, const int32_t *ids2,
+                    const double *vals2, double *score_out);
 
 /* MapPoint::ComputeDistinctiveDescriptors for ngroups map points at once: group g owns the descriptors
  * desc[group_ptr[g] .. group_ptr[g+1]) (its observations, in the order of the reference's vDescriptors);

@@ -32,6 +32,8 @@ def _bind():
     L.orbfe_feature_vector_device.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]
     L.orbfe_bow_vector_device.argtypes = [vp, C.c_int, vp, vp, C.c_int, vp, vp, vp, vp]
     L.orbfe_distinctive_descriptors_device.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp]
+    L.orbfe_bow_min_score_device.argtypes = [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.orbfe_bow_score.argtypes = [vp, C.c_int, vp, vp, C.c_int, vp, vp, vp]
     _bound = True
     return L
 
@@ -99,6 +101,29 @@ class Vocabulary:
         _check(_bind().orbfe_bow_transform(self._h, _p(desc), n, levelsup, C.byref(nw), _p(bow_ids), _p(bow_vals), C.byref(nn),
                                            _p(fv_ids), _p(fv_ptr), _p(fv_feats)))
         return (bow_ids[:nw.value], bow_vals[:nw.value]), (fv_ids[:nn.value], fv_ptr[:nn.value + 1], fv_feats[:fv_ptr[nn.value]])
+
+    def score(self, ids1, vals1, ids2, vals2):
+        """ORBVocabulary::score of two BowVectors (word ids ascending): the double L1Scoring::score returns."""
+        ids1, vals1 = np.ascontiguousarray(ids1, np.int32), np.ascontiguousarray(vals1, np.float64)
+        ids2, vals2 = np.ascontiguousarray(ids2, np.int32), np.ascontiguousarray(vals2, np.float64)
+        if len(ids1) != len(vals1) or len(ids2) != len(vals2):
+            raise ValueError("ids and values differ in length")
+        s = C.c_double(0.0)
+        _check(_bind().orbfe_bow_score(self._h, len(ids1), _p(ids1), _p(vals1), len(ids2), _p(ids2), _p(vals2), C.byref(s)))
+        return s.value
+
+
+def min_score_device(voc: "Vocabulary", nqueries, nframes, cap, d_bow_ids, d_bow_vals, d_bow_n, d_query_row, d_cov_ptr, d_cov_row,
+                     d_scores, d_min_score, stream=0):
+    """LoopClosing::DetectLoop's minScore of `nqueries` keyframes on the BowVector rows bow_vector_device wrote (ints = raw
+    device addresses; row f at f*cap): query b is row d_query_row[b], its connected keyframes are rows
+    d_cov_row[d_cov_ptr[b]:d_cov_ptr[b+1]] (negative = bad, skipped).  d_scores (0 = not wanted) receives the float64 score of
+    every pair, d_min_score[b] the float32 minimum starting at 1, which detect_batch_device takes as it is.  Enqueued, not
+    synchronised; see include/orbfe_bow.h."""
+    vp = C.c_void_p
+    _check(_bind().orbfe_bow_min_score_device(voc.handle, nqueries, nframes, cap, vp(d_bow_ids), vp(d_bow_vals), vp(d_bow_n),
+                                              vp(d_query_row), vp(d_cov_ptr), vp(d_cov_row), vp(d_scores or None), vp(d_min_score),
+                                              vp(stream)))
 
 
 def feature_vector_device(voc: "Vocabulary", nframes, d_leaf, d_node, d_counts, cap, d_fv_ids, d_fv_ptr, d_fv_items, d_fv_n, stream=0):

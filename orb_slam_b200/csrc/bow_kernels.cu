@@ -355,6 +355,87 @@ static int launch_feature_vector(int nframes, const int *d_leaf, const int *d_no
     return 0;
 }
 
+// ORBVocabulary::score for the pairs of LoopClosing::DetectLoop (LoopClosing.cc:117-131) and the minimum it keeps, on
+// BowVector rows in the frame layout of bow_vector_kernel.  One thread block per query keyframe: the query's words are
+// staged in shared memory once (12 bytes per word; a row of ORBFE_FV_MAX_CAP words takes 192 KB), the block's warps stride
+// over the query's connected keyframes, one warp per pair.  The lanes take 32 consecutive words of the connected keyframe's
+// row (coalesced) and each looks its word up in the staged query by binary search.  The terms of a chunk are added in lane
+// order by walking the ballot of the hits, every lane accumulating the same sum: chunks and lanes both ascend in word id, so
+// the additions are L1Scoring::score's (and bow_l1_walk's) in its order, each rounded once, and the double is the same.
+// The minimum is the reference's `if (score < minScore)` taken in list order: of the entries that compare equal to the least
+// float the first one gives the result, which only matters for its sign when that float is a zero.
+#define MS_THREADS 1024
+__global__ void __launch_bounds__(MS_THREADS) bow_min_score_kernel(int nframes, int cap, const int *__restrict__ bow_ids,
+                                                                   const double *__restrict__ bow_vals, const int *__restrict__ bow_n,
+                                                                   const int *__restrict__ query_row, const int *__restrict__ cov_ptr,
+                                                                   const int *__restrict__ cov_row, double *__restrict__ scores,
+                                                                   float *__restrict__ min_score) {
+    extern __shared__ double ms_q_vals[];            // [cap], then the ids
+    int *ms_q_ids = reinterpret_cast<int *>(ms_q_vals + cap);
+    __shared__ float s_min[MS_THREADS / 32];
+    __shared__ int s_first[MS_THREADS / 32];
+    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const int qr = query_row[b];
+    int nq = 0;                                      // a query row outside the store is an empty BowVector
+    if ((unsigned)qr < (unsigned)nframes) {
+        nq = min(max(bow_n[qr], 0), cap);
+        const int *__restrict__ ids = bow_ids + (size_t)qr * cap;
+        const double *__restrict__ vals = bow_vals + (size_t)qr * cap;
+        for (int i = tid; i < nq; i += MS_THREADS) {
+            ms_q_ids[i] = ids[i];
+            ms_q_vals[i] = vals[i];
+        }
+    }
+    __syncthreads();
+    const int p1 = cov_ptr[b + 1];
+    float wmin = 1.0f;                               // float minScore = 1
+    int wfirst = -1;                                 // list position that gave wmin
+    for (int k = cov_ptr[b] + wid; k < p1; k += MS_THREADS / 32) {
+        const int r = cov_row[k];
+        if ((unsigned)r >= (unsigned)nframes) continue;   // isBad()
+        const int n = min(max(bow_n[r], 0), cap);
+        const int *__restrict__ ids = bow_ids + (size_t)r * cap;
+        const double *__restrict__ vals = bow_vals + (size_t)r * cap;
+        double sum = 0.0;
+        for (int c0 = 0; c0 < n; c0 += 32) {
+            const int i = c0 + lane;
+            double term = 0.0;
+            bool hit = false;
+            if (i < n) {
+                const int w = __ldg(&ids[i]);
+                int lo = 0, hi = nq;                 // lower_bound
+                while (lo < hi) {
+                    const int mid = (lo + hi) >> 1;
+                    if (ms_q_ids[mid] < w) lo = mid + 1; else hi = mid;
+                }
+                if (lo < nq && ms_q_ids[lo] == w) {
+                    const double vi = ms_q_vals[lo], wi = __ldg(&vals[i]);
+                    term = __dsub_rn(__dsub_rn(fabs(__dsub_rn(vi, wi)), fabs(vi)), fabs(wi));
+                    hit = true;
+                }
+            }
+            unsigned bal = __ballot_sync(0xffffffffu, hit);
+            while (bal) {
+                sum = __dadd_rn(sum, __shfl_sync(0xffffffffu, term, __ffs(bal) - 1));
+                bal &= bal - 1;
+            }
+        }
+        const double score = -sum / 2.0;
+        if (scores && lane == 0) scores[k] = score;
+        const float sf = (float)score;
+        if (sf < wmin) { wmin = sf; wfirst = k; }
+    }
+    if (lane == 0) { s_min[wid] = wmin; s_first[wid] = wfirst; }
+    __syncthreads();
+    if (tid == 0) {
+        float best = 1.0f;
+        int first = -1;
+        for (int w = 0; w < MS_THREADS / 32; w++)
+            if (s_min[w] < best || (s_min[w] == best && s_first[w] < first)) { best = s_min[w]; first = s_first[w]; }
+        min_score[b] = best;
+    }
+}
+
 }  // namespace orbfe
 
 using namespace orbfe;
@@ -558,6 +639,62 @@ extern "C" int orbfe_bow_transform(OrbfeVocabulary *v, const uint8_t *desc, int 
     memcpy(fv_feats, H + o_fitem, (size_t)ptr[nn] * 4);
     *nwords_out = nw;
     *nnodes_out = nn;
+    return ORBFE_OK;
+}
+
+extern "C" int orbfe_bow_min_score_device(OrbfeVocabulary *v, int nqueries, int nframes, int cap, const int32_t *d_bow_ids,
+                                          const double *d_bow_vals, const int *d_bow_n, const int32_t *d_query_row,
+                                          const int32_t *d_cov_ptr, const int32_t *d_cov_row, double *d_scores, float *d_min_score,
+                                          void *stream) {
+    if (!v || nqueries < 0 || nframes < 1 || cap < 1) return set_error(ORBFE_ERR_ARG, "bad arguments");
+    if (nqueries > 0 && (!d_bow_ids || !d_bow_vals || !d_bow_n || !d_query_row || !d_cov_ptr || !d_cov_row || !d_min_score))
+        return set_error(ORBFE_ERR_ARG, "NULL argument");
+    if (cap > ORBFE_FV_MAX_CAP)
+        return set_error(ORBFE_ERR_UNSUPPORTED, "cap %d exceeds the %d words of a query row the score kernel stages in shared memory", cap,
+                         ORBFE_FV_MAX_CAP);
+    if ((long long)nframes * cap >= (1ll << 31)) return set_error(ORBFE_ERR_ARG, "nframes * cap = %lld does not fit 31 bits", (long long)nframes * cap);
+    if (nqueries == 0) return ORBFE_OK;
+    BOW_TRY(cudaSetDevice(v->device));
+    cudaStream_t s = stream ? (cudaStream_t)stream : v->stream;
+    const size_t smem = (sizeof(double) + sizeof(int)) * (size_t)cap;
+    if (smem > 48 * 1024) BOW_TRY(cudaFuncSetAttribute(bow_min_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    bow_min_score_kernel<<<nqueries, MS_THREADS, smem, s>>>(nframes, cap, d_bow_ids, d_bow_vals, d_bow_n, d_query_row, d_cov_ptr, d_cov_row,
+                                                            d_scores, d_min_score);
+    BOW_TRY(cudaGetLastError());
+    return ORBFE_OK;
+}
+
+// ORBVocabulary::score of two host BowVectors: a store of two rows, query row 0 with the one connected row 1.
+extern "C" int orbfe_bow_score(OrbfeVocabulary *v, int n1, const int32_t *ids1, const double *vals1, int n2, const int32_t *ids2,
+                               const double *vals2, double *score_out) {
+    if (!v || n1 < 0 || n2 < 0 || !score_out) return set_error(ORBFE_ERR_ARG, "bad arguments");
+    if ((n1 > 0 && (!ids1 || !vals1)) || (n2 > 0 && (!ids2 || !vals2))) return set_error(ORBFE_ERR_ARG, "NULL argument");
+    if (n1 > ORBFE_FV_MAX_CAP || n2 > ORBFE_FV_MAX_CAP)
+        return set_error(ORBFE_ERR_UNSUPPORTED, "%d words exceed the %d of a row the score kernel stages in shared memory", std::max(n1, n2),
+                         ORBFE_FV_MAX_CAP);
+    const int cap = std::max(std::max(n1, n2), 1);
+    const size_t N = (size_t)cap;
+    std::lock_guard<std::mutex> lock(v->mu);
+    BOW_TRY(cudaSetDevice(v->device));
+    size_t o_ids, o_vals, o_hdr, o_score, o_min, total;
+    if (int rc = v->stage.layout({{&o_ids, 2 * N * 4}, {&o_vals, 2 * N * 8}, {&o_hdr, 6 * sizeof(int)}, {&o_score, sizeof(double)},
+                                  {&o_min, sizeof(float)}},
+                                 &total))
+        return rc;
+    unsigned char *H = v->stage.h, *D = v->stage.d;
+    if (n1) { memcpy(H + o_ids, ids1, (size_t)n1 * 4); memcpy(H + o_vals, vals1, (size_t)n1 * 8); }
+    if (n2) { memcpy(H + o_ids + N * 4, ids2, (size_t)n2 * 4); memcpy(H + o_vals + N * 8, vals2, (size_t)n2 * 8); }
+    const int hdr[6] = {n1, n2, /* query row */ 0, /* cov_ptr */ 0, 1, /* cov_row */ 1};
+    memcpy(H + o_hdr, hdr, sizeof(hdr));
+    cudaStream_t s = v->stream;
+    BOW_TRY(cudaMemcpyAsync(D, H, o_score, cudaMemcpyHostToDevice, s));
+    const int *d_hdr = (const int *)(D + o_hdr);
+    if (int rc = orbfe_bow_min_score_device(v, 1, 2, cap, (const int32_t *)(D + o_ids), (const double *)(D + o_vals), d_hdr, d_hdr + 2,
+                                            d_hdr + 3, d_hdr + 5, (double *)(D + o_score), (float *)(D + o_min), s))
+        return rc;
+    BOW_TRY(cudaMemcpyAsync(H + o_score, D + o_score, sizeof(double), cudaMemcpyDeviceToHost, s));
+    BOW_TRY(cudaStreamSynchronize(s));
+    memcpy(score_out, H + o_score, sizeof(double));
     return ORBFE_OK;
 }
 

@@ -37,6 +37,9 @@
                    30000 Fuse / SearchBySim3 windows on one 1080p / 2000-keypoint keyframe; --baseline-lib PATH alternates
                    every call with another build of liborbfe.so in the same process and compares the outputs
 
+  --what loopscore LoopClosing::DetectLoop's minScore on the device (orbfe_bow_min_score_device): CUDA-event us per call for 1 query
+                   x 30 and x 100 connected keyframes and 16 queries x 30, rows of ~1000 and ~2000 words, against the host path
+                   (rows D2H, CPU score, one float H2D) and, with --baseline-lib, the same entry of another build alternately.
 Prints one JSON object per --what; never a bench value when run under ncu."""
 import argparse
 import ctypes as C
@@ -1298,6 +1301,113 @@ def bowchain(args):
     return out
 
 
+def loopscore(args):
+    """LoopClosing::DetectLoop's minScore on the device (orbfe_bow_min_score_device) at its call site's shapes: 1 keyframe with
+    30 and with 100 connected keyframes, and 16 queued keyframes with 30 each, on BowVector rows of about 1000 and about 2000
+    words (word ids over 10^6, neighbouring rows sharing most words, as --what kfdb builds them).  CUDA-event microseconds per
+    call over many launches on one stream after warm-up.  With --baseline-lib, the same entry of that build is timed
+    alternately in the same process and its outputs compared bit for bit.  host_path_us is what a host without this entry
+    does per keyframe, as wall time: one device gather of the rows and three D2H copies, L1Scoring::score on the CPU (the
+    oracle's C restatement), H2D of the one float, one synchronise."""
+    import torch
+    from oracle import bow_score as OS
+    NW = 1_000_000
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    vp, i_ = C.c_void_p, C.c_int
+    libs = {"this": C.CDLL(os.path.join(ROOT, "orb_slam_b200", "liborbfe.so"))}
+    if args.baseline_lib:
+        libs["baseline"] = C.CDLL(args.baseline_lib)
+    p = lambda a: a.ctypes.data_as(vp)
+    vocs = {}
+    for name, L in libs.items():
+        L.orbfe_vocabulary_create.argtypes = [i_, i_, i_, vp, vp, vp, vp, vp, i_, i_]
+        L.orbfe_vocabulary_create.restype = vp
+        L.orbfe_vocabulary_destroy.argtypes = [vp]
+        L.orbfe_vocabulary_destroy.restype = None
+        L.orbfe_bow_min_score_device.argtypes = [vp, i_, i_, i_, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+        flat = (np.zeros((3, 32), np.uint8), np.array([0, 2, 2, 2], np.int32), np.array([1, 2], np.int32), np.array([-1, 0, 1], np.int32),
+                np.ones(3))
+        vocs[name] = L.orbfe_vocabulary_create(0, 3, 1, p(flat[0]), p(flat[1]), p(flat[2]), p(flat[3]), p(flat[4]), 0, 1)
+        assert vocs[name]
+    out = {"what": "minScore of LoopClosing::DetectLoop on device BowVector rows, word ids over 10^6; microseconds per call"}
+    _gpu_and_power_limit(out)
+    t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dt)).to(dev)
+    F, reps = 128, 40 * args.iters
+    for wpk in (1000, 2000):
+        rng = np.random.default_rng(wpk)
+        cap = 2 * wpk
+        track = rng.integers(0, NW, F * wpk // 10 + 4 * wpk)
+        ids = np.full((F, cap), 2 ** 31 - 1, np.int32)
+        vals = np.zeros((F, cap))
+        n = np.zeros(F, np.int32)
+        for f in range(F):
+            w = track[f * wpk // 10:f * wpk // 10 + wpk].copy()
+            flip = rng.random(wpk) < 0.25
+            w[flip] = rng.integers(0, NW, int(flip.sum()))
+            u = np.unique(w).astype(np.int32)
+            v = rng.uniform(0.2, 3.0, len(u))
+            ids[f, :len(u)], vals[f, :len(u)], n[f] = u, v / v.sum(), len(u)
+        d_ids, d_vals, d_n = t(ids, np.int32), t(vals, np.float64), t(n, np.int32)
+        res = {"words_per_row": int(n.mean()), "cap": cap}
+        for nq, ncov in ((1, 30), (1, 100), (16, 30)):
+            qrow = (np.arange(nq) * 5 + 40).astype(np.int32)
+            cov = np.concatenate([(q + np.array([(-1) ** j * (j // 2 + 1) for j in range(ncov)])) % F for q in qrow]).astype(np.int32)
+            ptr = (np.arange(nq + 1) * ncov).astype(np.int32)
+            d_q, d_ptr, d_cov = t(qrow, np.int32), t(ptr, np.int32), t(cov, np.int32)
+            outs = {name: (torch.zeros(nq * ncov, dtype=torch.float64, device=dev), torch.zeros(nq, dtype=torch.float32, device=dev))
+                    for name in libs}
+            torch.cuda.synchronize()
+
+            def run(name, k):
+                for _ in range(k):
+                    rc = libs[name].orbfe_bow_min_score_device(vocs[name], nq, F, cap, d_ids.data_ptr(), d_vals.data_ptr(), d_n.data_ptr(),
+                                                               d_q.data_ptr(), d_ptr.data_ptr(), d_cov.data_ptr(), outs[name][0].data_ptr(),
+                                                               outs[name][1].data_ptr(), stream.cuda_stream)
+                    assert rc == 0
+            times = {name: [] for name in libs}
+            for name in libs:
+                run(name, 10 * args.warmup)
+            stream.synchronize()
+            for _ in range(5):                       # alternate the builds
+                for name in libs:
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record(stream)
+                    run(name, reps)
+                    e1.record(stream)
+                    stream.synchronize()
+                    times[name].append(e0.elapsed_time(e1) / reps * 1e3)
+            key = "%dq_x_%dcov" % (nq, ncov)
+            for name in libs:
+                res["%s_%s_us" % (key, name)] = [round(min(times[name]), 2), round(max(times[name]), 2)]   # least and most of 5 rounds
+            if "baseline" in libs:
+                res[key + "_same_bits"] = bool(torch.equal(outs["this"][0].view(torch.int64), outs["baseline"][0].view(torch.int64)) and
+                                               torch.equal(outs["this"][1].view(torch.int32), outs["baseline"][1].view(torch.int32)))
+            if nq == 1:
+                d_rows = t(np.concatenate([qrow, cov]), np.int64)
+
+                def host_path():
+                    hi, hv, hn = d_ids[d_rows].cpu().numpy(), d_vals[d_rows].cpu().numpy(), d_n[d_rows].cpu().numpy()
+                    m = np.float32(1)
+                    for k in range(1, len(hn)):
+                        sc = np.float32(OS.bow_score(hi[0, :hn[0]], hv[0, :hn[0]], hi[k, :hn[k]], hv[k, :hn[k]]))
+                        if sc < m:
+                            m = sc
+                    d_m = torch.tensor([m], dtype=torch.float32).to(dev, non_blocking=True)
+                    torch.cuda.synchronize()
+                    return m, d_m
+                m, _ = host_path()
+                t0 = time.perf_counter()
+                for _ in range(5 * args.iters):
+                    host_path()
+                res[key + "_host_path_us"] = round((time.perf_counter() - t0) / (5 * args.iters) * 1e6, 1)
+                res[key + "_host_same_min"] = bool(np.float32(m).tobytes() == outs["this"][1].cpu().numpy()[0].tobytes())
+        out["%d_words" % wpk] = res
+    for name, L in libs.items():
+        L.orbfe_vocabulary_destroy(vocs[name])
+    return out
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--what", default="config3,config5")
@@ -1305,9 +1415,9 @@ if __name__ == "__main__":
     ap.add_argument("--groups", type=int, default=10000)
     ap.add_argument("--iters", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
-    ap.add_argument("--baseline-lib", default=None, help="--what guided: another build of liborbfe.so to time alternately")
+    ap.add_argument("--baseline-lib", default=None, help="--what guided, kfdbbatch, loopscore: another build of liborbfe.so to time alternately")
     args = ap.parse_args()
     for w in args.what.split(","):
         print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fast": fast, "latency": latency,
                           "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb, "kfdbbatch": kfdbbatch, "bowchain": bowchain,
-                          "windowed": windowed, "guided": guided}[w](args)))
+                          "windowed": windowed, "guided": guided, "loopscore": loopscore}[w](args)))
