@@ -38,6 +38,32 @@ OrbfeVocabulary *orbfe_vocabulary_create(int device, int nnodes, int depth_L, co
                                          int norm);
 void orbfe_vocabulary_destroy(OrbfeVocabulary *v);
 
+/* TemplatedVocabulary::loadFromTextFile (Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1338-1424) on the device: the file is
+ * read in chunks through a double-buffered pinned staging area into device memory and the node table is parsed there; it
+ * never passes through host arrays.  The result equals the reference's m_nodes field for field:
+ *   header `k L scoring weighting` (any tokens after them ignored), k in [0,20], L in [1,10], scoring in [0,5],
+ *   weighting in [0,3]; norm = what the scoring object's mustNormalize gives (L1 for L1 / chi-square / KL / Bhattacharyya,
+ *   L2 for L2, none for dot product);
+ *   line n of the body is node n (node 0 is the root), `parent isLeaf b0 .. b31 weight`, any whitespace between tokens,
+ *   tokens after the weight ignored; the children of a node are in line order; a node whose isLeaf is > 0 gets the next
+ *   word id in line order, every other node word id 0; byte bi = (unsigned char)bi; the weight is the double
+ *   `istream >> double` gives (decimal tokens of at most 15 significant digits and a decimal exponent within +-22 are
+ *   converted on the device, exactly; any other token, or a missing weight, by that very extraction on the host).
+ * A final empty line (the file ends with a newline) adds no node; the reference creates one from uninitialised values.
+ * Rejected with ORBFE_ERR_ARG, the 1-based line number in orbfe_last_error: a missing or unreadable file, a bad header, an
+ * empty or blank line before the last, fewer than 34 tokens before the weight, a parent / isLeaf / descriptor token that is
+ * not a plain decimal int, a parent < 0 or >= the line's node id, a body of 2^31 bytes or more.  No device:
+ * ORBFE_ERR_NO_DEVICE.  The header is checked before any device is used.  *out is NULL on every error. */
+int orbfe_vocabulary_load_text(int device, const char *path, OrbfeVocabulary **out);
+/* Header fields and sizes of any vocabulary (any pointer may be NULL).  k and scoring are -1 for orbfe_vocabulary_create,
+ * which never receives them; nwords = the largest word id + 1. */
+int orbfe_vocabulary_info(const OrbfeVocabulary *v, int *k, int *L, int *scoring, int *weighting, int *nnodes, int *nwords);
+/* Copies the node table back in orbfe_vocabulary_create's layout (node_desc nnodes x 32, child_ptr nnodes + 1, children
+ * child_ptr[nnodes] entries -- nnodes - 1 for a loaded text --, word_id and weight nnodes each) and the parent of every node
+ * (the root's is 0).  Any pointer may be NULL.  Synchronous. */
+int orbfe_vocabulary_export(OrbfeVocabulary *v, uint8_t *node_desc, int32_t *child_ptr, int32_t *children, int32_t *word_id,
+                            double *weight, int32_t *parent);
+
 /* transform(feature, word_id, weight, &nid, levelsup) for n descriptors (TemplatedVocabulary.h:1216-1260):
  * leaf_out[i] = node id of the leaf reached, node_out[i] = id of the ancestor at level depth_L - levelsup (0 = root when
  * that level is <= 0, and also when the leaf is shallower than that level, where the reference leaves *nid unset).

@@ -52,7 +52,8 @@ ABI_SYMBOLS = [
     "orbfe_rig_exchange_wait", "orbfe_rig_exchange_release", "orbfe_search_for_initialization_exchange", "orbfe_rig_exchange_buffers", "orbfe_rig_exchange_buffers_produced", "orbfe_rig_exchange_check",
     "orbfe_rig_exchange_bytes",
     # include/orbfe_bow.h
-    "orbfe_vocabulary_create", "orbfe_vocabulary_destroy", "orbfe_bow_descend_device", "orbfe_bow_descend", "orbfe_bow_transform",
+    "orbfe_vocabulary_create", "orbfe_vocabulary_destroy", "orbfe_vocabulary_load_text", "orbfe_vocabulary_info",
+    "orbfe_vocabulary_export", "orbfe_bow_descend_device", "orbfe_bow_descend", "orbfe_bow_transform",
     "orbfe_distinctive_descriptors", "orbfe_bow_db_detect", "orbfe_feature_vector_device", "orbfe_distinctive_descriptors_device",
     "orbfe_bow_vector_device", "orbfe_bow_min_score_device", "orbfe_bow_score",
     "orbfe_kfdb_create", "orbfe_kfdb_destroy", "orbfe_kfdb_add", "orbfe_kfdb_add_device", "orbfe_kfdb_erase", "orbfe_kfdb_clear", "orbfe_kfdb_set_covisibles",

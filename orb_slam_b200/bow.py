@@ -3,6 +3,7 @@ Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1126-1262; callers Frame.cc:280-287
 MapPoint::ComputeDistinctiveDescriptors (reference src/MapPoint.cc:185-250).  No CPU fallback: every call runs the
 CUDA kernels of liborbfe.so."""
 import ctypes as C
+import os
 
 import numpy as np
 
@@ -24,6 +25,9 @@ def _bind():
     L.orbfe_vocabulary_create.restype = vp
     L.orbfe_vocabulary_destroy.argtypes = [vp]
     L.orbfe_vocabulary_destroy.restype = None
+    L.orbfe_vocabulary_load_text.argtypes = [C.c_int, C.c_char_p, C.POINTER(vp)]
+    L.orbfe_vocabulary_info.argtypes = [vp] + [C.POINTER(C.c_int)] * 6
+    L.orbfe_vocabulary_export.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     L.orbfe_bow_descend_device.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, vp]
     L.orbfe_bow_descend.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp]
     L.orbfe_bow_transform.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp]
@@ -61,6 +65,35 @@ class Vocabulary:
                                             _p(A["children"]), _p(A["word_id"]), _p(A["weight"]), weighting, norm)
         if not self._h:
             raise OrbfeError(-1, L.orbfe_last_error().decode("utf-8", "replace"))
+
+    @classmethod
+    def load_text(cls, path, device=0):
+        """TemplatedVocabulary::loadFromTextFile (e.g. ORB-SLAM's Data/ORBvoc.txt) parsed on `device`: the node table is
+        built in device memory; header, weighting and norm come from the file.  See include/orbfe_bow.h."""
+        L = _bind()
+        h = C.c_void_p()
+        _check(L.orbfe_vocabulary_load_text(int(device), os.fsencode(path), C.byref(h)))
+        self = cls.__new__(cls)
+        self._h, self.arrays = h.value, None
+        return self
+
+    def info(self):
+        """dict(k, L, scoring, weighting, nnodes, nwords); k and scoring are -1 for a vocabulary built from arrays."""
+        f = [C.c_int(0) for _ in range(6)]
+        _check(_bind().orbfe_vocabulary_info(self._h, *[C.byref(x) for x in f]))
+        return dict(zip(("k", "L", "scoring", "weighting", "nnodes", "nwords"), (x.value for x in f)))
+
+    def export(self):
+        """The node table in the constructor's layout (node_desc, child_ptr, children, word_id, weight) plus parent."""
+        n = self.info()["nnodes"]
+        child_ptr = np.zeros(n + 1, np.int32)
+        _check(_bind().orbfe_vocabulary_export(self._h, None, _p(child_ptr), None, None, None, None))
+        out = {"node_desc": np.zeros((n, 32), np.uint8), "child_ptr": child_ptr, "children": np.zeros(max(int(child_ptr[n]), 1), np.int32),
+               "word_id": np.zeros(n, np.int32), "weight": np.zeros(n, np.float64), "parent": np.zeros(n, np.int32)}
+        _check(_bind().orbfe_vocabulary_export(self._h, _p(out["node_desc"]), None, _p(out["children"]), _p(out["word_id"]),
+                                               _p(out["weight"]), _p(out["parent"])))
+        out["children"] = out["children"][:child_ptr[n]]
+        return out
 
     @property
     def handle(self):

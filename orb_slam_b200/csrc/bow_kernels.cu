@@ -13,6 +13,7 @@
 #include "../../include/orbfe_bow.h"
 #include "bow_l1.cuh"
 #include "orbfe_internal.h"
+#include "vocab.h"
 
 namespace orbfe {
 
@@ -447,19 +448,17 @@ using namespace orbfe;
             return set_error(ORBFE_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
     } while (0)
 
-struct OrbfeVocabulary {
-    int device = 0, nnodes = 0, depth = 0, weighting = 0, norm = 0;
-    int nwords = 0;                 // largest word id + 1
-    cudaStream_t stream = nullptr;
-    uint8_t *d_desc = nullptr;
-    uint8_t *d_live = nullptr;      // per node: weight > 0 (the FeatureVector skips stopped words)
-    int *d_child_ptr = nullptr, *d_children = nullptr;
-    int *d_word_id = nullptr;       // per node, for the BowVector kernel
-    double *d_weight = nullptr;
-    // the host-array entries stage through `stage` on `stream`, one call at a time
-    std::mutex mu;
-    Stage stage;
-};
+cudaError_t orbfe::vocab_alloc(OrbfeVocabulary *v, int nnodes, int nchild) {
+    const size_t n = (size_t)nnodes;
+    cudaError_t e = cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaMalloc((void **)&v->d_desc, n * 32);
+    if (e == cudaSuccess) e = cudaMalloc((void **)&v->d_live, n);
+    if (e == cudaSuccess) e = cudaMalloc((void **)&v->d_word_id, sizeof(int) * n);
+    if (e == cudaSuccess) e = cudaMalloc((void **)&v->d_weight, sizeof(double) * n);
+    if (e == cudaSuccess) e = cudaMalloc((void **)&v->d_child_ptr, sizeof(int) * (n + 1));
+    if (e == cudaSuccess) e = cudaMalloc((void **)&v->d_children, sizeof(int) * (size_t)std::max(nchild, 1));
+    return e;
+}
 
 extern "C" void orbfe_vocabulary_destroy(OrbfeVocabulary *v) {
     if (!v) return;
@@ -499,16 +498,11 @@ extern "C" OrbfeVocabulary *orbfe_vocabulary_create(int device, int nnodes, int 
         live[i] = weight[i] > 0 ? 1 : 0;
         v->nwords = std::max(v->nwords, word_id[i] + 1);
     }
-    bool ok = cudaSetDevice(device) == cudaSuccess && cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking) == cudaSuccess &&
-              cudaMalloc((void **)&v->d_desc, (size_t)nnodes * 32) == cudaSuccess &&
-              cudaMalloc((void **)&v->d_live, (size_t)nnodes) == cudaSuccess &&
+    v->nchild = nchild;
+    bool ok = cudaSetDevice(device) == cudaSuccess && vocab_alloc(v, nnodes, nchild) == cudaSuccess &&
               cudaMemcpy(v->d_live, live.data(), (size_t)nnodes, cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaMalloc((void **)&v->d_word_id, sizeof(int) * (size_t)nnodes) == cudaSuccess &&
               cudaMemcpy(v->d_word_id, word_id, sizeof(int) * (size_t)nnodes, cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaMalloc((void **)&v->d_weight, sizeof(double) * (size_t)nnodes) == cudaSuccess &&
               cudaMemcpy(v->d_weight, weight, sizeof(double) * (size_t)nnodes, cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaMalloc((void **)&v->d_child_ptr, sizeof(int) * ((size_t)nnodes + 1)) == cudaSuccess &&
-              cudaMalloc((void **)&v->d_children, sizeof(int) * (size_t)std::max(nchild, 1)) == cudaSuccess &&
               cudaMemcpy(v->d_desc, node_desc, (size_t)nnodes * 32, cudaMemcpyHostToDevice) == cudaSuccess &&
               cudaMemcpy(v->d_child_ptr, child_ptr, sizeof(int) * ((size_t)nnodes + 1), cudaMemcpyHostToDevice) == cudaSuccess &&
               (nchild == 0 || cudaMemcpy(v->d_children, children, sizeof(int) * (size_t)nchild, cudaMemcpyHostToDevice) == cudaSuccess);
@@ -518,6 +512,41 @@ extern "C" OrbfeVocabulary *orbfe_vocabulary_create(int device, int nnodes, int 
         return nullptr;
     }
     return v;
+}
+
+extern "C" int orbfe_vocabulary_info(const OrbfeVocabulary *v, int *k, int *L, int *scoring, int *weighting, int *nnodes, int *nwords) {
+    if (!v) return set_error(ORBFE_ERR_ARG, "NULL vocabulary");
+    if (k) *k = v->k;
+    if (L) *L = v->depth;
+    if (scoring) *scoring = v->scoring;
+    if (weighting) *weighting = v->weighting;
+    if (nnodes) *nnodes = v->nnodes;
+    if (nwords) *nwords = v->nwords;
+    return ORBFE_OK;
+}
+
+// The parent of every node is read off the CSR (each non-root node is the child of exactly one row in a loaded table);
+// the root's is 0, the default of DBoW2's Node.
+extern "C" int orbfe_vocabulary_export(OrbfeVocabulary *v, uint8_t *node_desc, int32_t *child_ptr, int32_t *children, int32_t *word_id,
+                                       double *weight, int32_t *parent) {
+    if (!v) return set_error(ORBFE_ERR_ARG, "NULL vocabulary");
+    const size_t n = (size_t)v->nnodes;
+    BOW_TRY(cudaSetDevice(v->device));
+    BOW_TRY(cudaStreamSynchronize(v->stream));
+    if (node_desc) BOW_TRY(cudaMemcpy(node_desc, v->d_desc, n * 32, cudaMemcpyDeviceToHost));
+    if (word_id) BOW_TRY(cudaMemcpy(word_id, v->d_word_id, sizeof(int) * n, cudaMemcpyDeviceToHost));
+    if (weight) BOW_TRY(cudaMemcpy(weight, v->d_weight, sizeof(double) * n, cudaMemcpyDeviceToHost));
+    std::vector<int32_t> ptr_tmp, ch_tmp;
+    if (!child_ptr && parent) { ptr_tmp.resize(n + 1); child_ptr = ptr_tmp.data(); }
+    if (child_ptr) BOW_TRY(cudaMemcpy(child_ptr, v->d_child_ptr, sizeof(int) * (n + 1), cudaMemcpyDeviceToHost));
+    if (!children && parent) { ch_tmp.resize((size_t)v->nchild); children = ch_tmp.data(); }
+    if (children && v->nchild > 0) BOW_TRY(cudaMemcpy(children, v->d_children, sizeof(int) * (size_t)v->nchild, cudaMemcpyDeviceToHost));
+    if (parent) {
+        std::fill(parent, parent + n, 0);
+        for (size_t i = 0; i < n; i++)
+            for (int c = child_ptr[i]; c < child_ptr[i + 1]; c++) parent[children[c]] = (int32_t)i;
+    }
+    return ORBFE_OK;
 }
 
 extern "C" int orbfe_bow_descend_device(OrbfeVocabulary *v, const uint8_t *d_desc, int n, int levelsup, int32_t *d_leaf_out,

@@ -40,6 +40,10 @@
   --what loopscore LoopClosing::DetectLoop's minScore on the device (orbfe_bow_min_score_device): CUDA-event us per call for 1 query
                    x 30 and x 100 connected keyframes and 16 queries x 30, rows of ~1000 and ~2000 words, against the host path
                    (rows D2H, CPU score, one float H2D) and, with --baseline-lib, the same entry of another build alternately.
+  --what vocload   orbfe_vocabulary_load_text on a synthetic ORBvoc-shaped text (k = 10, L = 6: 1,111,111 lines, internal nodes
+                   weighted 0, words with 6 significant digits like Data/ORBvoc.txt) and on the same tree with %r weights (the
+                   host-conversion path): wall time per load (file read included), device time per kernel and copy
+                   (torch.profiler, a run of its own), and the reference's loadFromTextFile from oracle/_ref in the same process.
 Prints one JSON object per --what; never a bench value when run under ncu."""
 import argparse
 import ctypes as C
@@ -1408,6 +1412,60 @@ def loopscore(args):
     return out
 
 
+def vocload(args):
+    import tempfile
+    import torch
+    from torch.profiler import profile, ProfilerActivity
+    from orb_slam_b200 import bow as BW
+    from orb_slam_b200.synth import random_vocabulary
+    from oracle import voc_text as VT
+    torch.zeros(1, device="cuda")
+    voc = random_vocabulary(10, 6, seed=3)
+    nd, cp, ch = voc["node_desc"], voc["child_ptr"], voc["children"]
+    n = len(nd)
+    parent = np.zeros(n, np.int64)
+    parent[ch] = np.repeat(np.arange(n), np.diff(cp))
+    leaf = (np.diff(cp) == 0).astype(int)
+    desc = [" ".join(map(str, row)) for row in nd.tolist()]
+    w = voc["weight"].tolist()
+    out = {"what": "orbfe_vocabulary_load_text, k=10 L=6 synthetic text (%d nodes), %d iterations after %d warm-up" % (n, args.iters, args.warmup)}
+    with tempfile.TemporaryDirectory() as tmp:
+        for name, fmt in (("orbvoc_like", lambda i: "%.6g" % w[i] if leaf[i] else "0"), ("repr_weights", lambda i: repr(w[i]))):
+            path = os.path.join(tmp, name + ".txt")
+            with open(path, "w") as f:
+                f.write("10 6 0 0\n" + "".join("%d %d %s  %s\n" % (parent[i], leaf[i], desc[i], fmt(i)) for i in range(1, n)))
+            res = {"bytes": os.path.getsize(path)}
+            for _ in range(args.warmup):
+                BW.Vocabulary.load_text(path).close()
+            walls = []
+            for _ in range(args.iters):
+                t0 = time.perf_counter()
+                V = BW.Vocabulary.load_text(path)
+                walls.append(time.perf_counter() - t0)
+                V.close()
+            res["load_text_wall_ms"] = {"min": round(1e3 * min(walls), 2), "median": round(1e3 * float(np.median(walls)), 2),
+                                        "max": round(1e3 * max(walls), 2)}
+            t0 = time.perf_counter()
+            open(path, "rb").read()
+            res["file_read_only_ms"] = round(1e3 * (time.perf_counter() - t0), 2)
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                BW.Vocabulary.load_text(path).close()
+            dev = {}
+            for e in prof.key_averages():
+                t = getattr(e, "device_time_total", 0)
+                if t > 0:
+                    dev[e.key.replace("orbfe::(anonymous namespace)::", "").split("(")[0].strip()[:60]] = {"calls": e.count, "us": round(t, 1)}
+            res["device_us"] = dev
+            ref_path = VT.text_for_reference(path, os.path.join(tmp, "ref.txt"))
+            ref = VT.RefVocabularyNodes(ref_path)
+            res["reference_loadFromTextFile_ms"] = round(1e3 * ref.seconds, 1)
+            ref.close()
+            os.remove(ref_path)
+            out[name] = res
+    _gpu_and_power_limit(out)
+    return out
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--what", default="config3,config5")
@@ -1420,4 +1478,4 @@ if __name__ == "__main__":
     for w in args.what.split(","):
         print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fast": fast, "latency": latency,
                           "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb, "kfdbbatch": kfdbbatch, "bowchain": bowchain,
-                          "windowed": windowed, "guided": guided, "loopscore": loopscore}[w](args)))
+                          "windowed": windowed, "guided": guided, "loopscore": loopscore, "vocload": vocload}[w](args)))
