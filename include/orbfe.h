@@ -139,7 +139,8 @@ int orbfe_hamming_csr_device(OrbfeMatcher *m, const uint8_t *d_qdesc, const uint
                              const int32_t *d_row_ptr, const int32_t *d_cols, int nq, int npairs,
                              uint16_t *d_out_dist, void *stream);
 int orbfe_matcher_sync(OrbfeMatcher *m);
-/* cumulative host<->device traffic and kernel launches of the host-pointer entry points (bench accounting) */
+/* cumulative host<->device traffic and kernel launches of the host-pointer entry points (bench accounting); the bytes are
+ * those of the staging block's uploaded and downloaded parts, every array padded to 256 bytes */
 int orbfe_matcher_counters(const OrbfeMatcher *m, unsigned long long *h2d_bytes, unsigned long long *d2h_bytes,
                            unsigned long long *launches);
 

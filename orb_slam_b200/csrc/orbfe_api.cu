@@ -22,6 +22,7 @@
 #include <thread>
 #include <unordered_map>
 
+#include "../../include/orbfe_bow.h"
 #include "../../include/orbfe_match.h"
 #include "orbfe_internal.h"
 
@@ -32,15 +33,6 @@ using namespace orbfe;
 // ------------------------------------------------------------------------------------------------
 static thread_local char g_err[512] = "";
 
-static int fail(int code, const char *fmt, ...) {
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(g_err, sizeof(g_err), fmt, ap);
-    va_end(ap);
-    return code;
-}
-
-// the same for the other translation units of the library (bow_kernels.cu, host/*.cpp)
 int orbfe::set_error(int code, const char *fmt, ...) {
     va_list ap;
     va_start(ap, fmt);
@@ -48,6 +40,7 @@ int orbfe::set_error(int code, const char *fmt, ...) {
     va_end(ap);
     return code;
 }
+static int (*const fail)(int, const char *, ...) = orbfe::set_error;  // this file's spelling
 
 #define CU_TRY(expr)                                                                                   \
     do {                                                                                               \
@@ -159,6 +152,20 @@ static void resize_axis(int dn, int sn, bool clamp_weights, std::vector<int> &of
         ab[d].x = (short)cv_round((double)((1.f - f) * 2048.f));
         ab[d].y = (short)cv_round((double)(f * 2048.f));
     }
+}
+
+// The 3-D (x, y, frame) tensor map of one unblurred level, as fast_nms_tma_kernel loads its pixel tiles: a box of
+// F2_TW x F2_PH x 1 bytes.  `encode` is the driver's cuTensorMapEncodeTiled; pitch and plane are the byte strides of y and frame.
+static CUresult encode_level_map(void *encode, CUtensorMap *map, uint8_t *ptr, int w, int h, int frames, int pitch, size_t plane) {
+    typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
+                                 const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                 CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+    const cuuint64_t dims[3] = {(cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)frames};
+    const cuuint64_t strides[2] = {(cuuint64_t)pitch, (cuuint64_t)plane};
+    const cuuint32_t box[3] = {160, ORBFE_FT_H + 8, 1};
+    const cuuint32_t estr[3] = {1, 1, 1};
+    return ((EncodeFn)encode)(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
 static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
@@ -376,9 +383,6 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
     Wk.cell_cand_cap = d_cc;
     // ---- TMA tensor maps (one per level: x, y, frame) for the FAST kernel's pixel tiles ----
     {
-        typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
-                                     const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
         void *fn = nullptr;
         cudaDriverEntryPointQueryResult qres;
         if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn ||
@@ -387,13 +391,7 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
         std::vector<CUtensorMap> maps(ex->nlevels);
         for (int l = 0; l < ex->nlevels; l++) {
             const LevelDev &L = P.lv[l];
-            const cuuint64_t dims[3] = {(cuuint64_t)L.w, (cuuint64_t)L.h, (cuuint64_t)B};
-            const cuuint64_t strides[2] = {(cuuint64_t)L.pitch, (cuuint64_t)L.plane};  // bytes, dims 1 and 2
-            const cuuint32_t box[3] = {160, ORBFE_FT_H + 8, 1};  // F2_TW x F2_PH x 1
-            const cuuint32_t estr[3] = {1, 1, 1};
-            CUresult r = ((EncodeFn)fn)(&maps[l], CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, L.pyr, dims, strides, box, estr,
-                                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+            const CUresult r = encode_level_map(fn, &maps[l], L.pyr, L.w, L.h, B, L.pitch, L.plane);
             if (r != CUDA_SUCCESS) return fail(ORBFE_ERR_CUDA, "cuTensorMapEncodeTiled(level %d) failed: %d", l, (int)r);
         }
         CUtensorMap *d_maps;
@@ -453,16 +451,8 @@ static int set_level0(OrbfeExtractor *ex, uint8_t *ptr, int pitch, size_t plane,
     L0.pyr = ptr; L0.pitch = pitch; L0.plane = plane;
     CU_TRY(cudaMemcpyAsync(&ex->dplan->lv[0], &L0, sizeof(LevelDev), cudaMemcpyHostToDevice, s));
     if (ex->d_maps && ex->tma_encode) {
-        typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
-                                     const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
         CUtensorMap m;
-        const cuuint64_t dims[3] = {(cuuint64_t)L0.w, (cuuint64_t)L0.h, (cuuint64_t)std::max(batch, ex->Bcap)};
-        const cuuint64_t strides[2] = {(cuuint64_t)pitch, (cuuint64_t)plane};
-        const cuuint32_t box[3] = {160, ORBFE_FT_H + 8, 1};
-        const cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = ((EncodeFn)ex->tma_encode)(&m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                                CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        const CUresult r = encode_level_map(ex->tma_encode, &m, ptr, L0.w, L0.h, std::max(batch, ex->Bcap), pitch, plane);
         if (r != CUDA_SUCCESS) return fail(ORBFE_ERR_CUDA, "cuTensorMapEncodeTiled(level 0, in place) failed: %d", (int)r);
         CU_TRY(cudaMemcpyAsync(&ex->d_maps[0], &m, sizeof(m), cudaMemcpyHostToDevice, s));
     }
@@ -638,24 +628,29 @@ static void profiling_collect(OrbfeExtractor *ex) {
     T.origin_pending = true;
 }
 
-static void profiling_end(OrbfeExtractor *) {}
+// Head of both device-resident extract entries: the plan for this geometry, level 0 taken from the caller's device frames
+// and the per-call counters zeroed, on *s (the caller's stream, or the handle's)
+static int begin_device_extract(OrbfeExtractor *ex, const uint8_t *d_imgs, int width, int height, size_t stride, size_t frame_stride,
+                                int batch, void *stream, cudaStream_t *s) {
+    if (width <= 0 || height <= 0 || batch <= 0 || stride < (size_t)width) return fail(ORBFE_ERR_ARG, "bad geometry");
+    CU_TRY(cudaSetDevice(ex->device));
+    int rc = build_plan(ex, width, height, batch);
+    if (rc) return rc;
+    *s = stream ? (cudaStream_t)stream : ex->stream;
+    profiling_begin(ex, *s);
+    rc = ingest_device(ex, d_imgs, width, height, stride, frame_stride, batch, *s);
+    if (rc) return rc;
+    stage_mark(ex, *s, "ingest");
+    ex->last_launches = 0;
+    return zero_counters(ex, *s);
+}
 
 extern "C" int orbfe_extract_batch_device(OrbfeExtractor *ex, const uint8_t *d_imgs, int width, int height,
                                           size_t stride, size_t frame_stride, int batch, OrbfeKeyPoint *d_kps,
                                           uint8_t *d_desc, int *d_counts, void *stream) {
     if (!ex || !d_imgs || !d_kps || !d_desc || !d_counts) return fail(ORBFE_ERR_ARG, "NULL argument");
-    if (width <= 0 || height <= 0 || batch <= 0 || stride < (size_t)width) return fail(ORBFE_ERR_ARG, "bad geometry");
-    CU_TRY(cudaSetDevice(ex->device));
-    int rc = build_plan(ex, width, height, batch);
-    if (rc) return rc;
-    cudaStream_t s = stream ? (cudaStream_t)stream : ex->stream;
-    profiling_begin(ex, s);
-    rc = ingest_device(ex, d_imgs, width, height, stride, frame_stride, batch, s);
-    if (rc) return rc;
-    stage_mark(ex, s, "ingest");
-    ex->last_launches = 0;
-    rc = zero_counters(ex, s);
-    if (rc) return rc;
+    cudaStream_t s;
+    if (int rc = begin_device_extract(ex, d_imgs, width, height, stride, frame_stride, batch, stream, &s)) return rc;
     return enqueue_pipeline(ex, 0, batch, d_kps, d_desc, d_counts, s);
 }
 
@@ -664,19 +659,9 @@ extern "C" int orbfe_extract_batch_device(OrbfeExtractor *ex, const uint8_t *d_i
 int orbfe_extract_batch_device_peers(OrbfeExtractor *ex, const uint8_t *d_imgs, int width, int height, size_t stride, size_t frame_stride,
                                      int batch, const PeerOut &po, int cap, void *stream) {
     if (!ex || !d_imgs) return fail(ORBFE_ERR_ARG, "NULL argument");
-    if (width <= 0 || height <= 0 || batch <= 0 || stride < (size_t)width) return fail(ORBFE_ERR_ARG, "bad geometry");
-    CU_TRY(cudaSetDevice(ex->device));
-    int rc = build_plan(ex, width, height, batch);
-    if (rc) return rc;
+    cudaStream_t s;
+    if (int rc = begin_device_extract(ex, d_imgs, width, height, stride, frame_stride, batch, stream, &s)) return rc;
     if (cap != ex->hplan.nfeatures) return fail(ORBFE_ERR_ARG, "exchange capacity %d != keypoint slots per frame %d", cap, ex->hplan.nfeatures);
-    cudaStream_t s = stream ? (cudaStream_t)stream : ex->stream;
-    profiling_begin(ex, s);
-    rc = ingest_device(ex, d_imgs, width, height, stride, frame_stride, batch, s);
-    if (rc) return rc;
-    stage_mark(ex, s, "ingest");
-    ex->last_launches = 0;
-    rc = zero_counters(ex, s);
-    if (rc) return rc;
     return enqueue_pipeline(ex, 0, batch, nullptr, nullptr, nullptr, s, true, &po);
 }
 
@@ -750,7 +735,6 @@ extern "C" int orbfe_extract_batch(OrbfeExtractor *ex, const uint8_t *imgs, int 
     }
     stage_mark(ex, s, "d2h");
     CU_TRY(cudaStreamSynchronize(s));
-    profiling_end(ex);
     if (*ex->h_err) {
         int code = *ex->h_err;
         cudaMemsetAsync(ex->work.err_flag, 0, sizeof(int), s);
@@ -774,7 +758,6 @@ extern "C" int orbfe_extractor_sync(OrbfeExtractor *ex) {
     if (!ex) return fail(ORBFE_ERR_ARG, "ex is NULL");
     CU_TRY(cudaSetDevice(ex->device));
     CU_TRY(cudaStreamSynchronize(ex->stream));
-    profiling_end(ex);
     return ORBFE_OK;
 }
 
@@ -837,15 +820,12 @@ struct OrbfeMatcher {
     int device = 0;
     int nsm = 132;
     cudaStream_t stream = nullptr;
-    // grow-only device scratch for the host-pointer entry points
-    void *buf[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    size_t cap[6] = {0, 0, 0, 0, 0, 0};
     unsigned long long h2d_bytes = 0, d2h_bytes = 0, launches = 0;  // cumulative, for bench.py
     uint32_t *scratch = nullptr;  // candidate entries of the device-resident matcher
     size_t scratch_entries = 0;
     int *d_err = nullptr;  // [0]: error flags of the last launches; [1]: candidate entries an overflowing fused-matcher job needed
     int *h_err = nullptr;  // pinned
-    Stage stage;           // the host-array entries that run on a device kernel
+    Stage stage;           // every host-array entry of the handle; with `scratch`, the only device memory it grows
 };
 
 // Dynamic shared memory of the fused matcher (one thread block per pair / job).  What is left after the fixed arrays
@@ -857,17 +837,6 @@ static size_t sbp_smem_total(const OrbfeMatcher *m, size_t fixed, int nblocks) {
     if (const char *e = getenv("ORBFE_SBP_SMEM_KB")) total = (size_t)std::max(0, atoi(e)) * 1024;
     total = std::max(total, fixed + 16 * 1024);
     return total;
-}
-
-static cudaError_t mreserve(OrbfeMatcher *m, int i, size_t bytes) {
-    if (m->cap[i] >= bytes) return cudaSuccess;
-    if (m->buf[i]) cudaFree(m->buf[i]);
-    m->buf[i] = nullptr;
-    m->cap[i] = 0;
-    size_t want = std::max<size_t>(bytes + bytes / 4, 4096);
-    cudaError_t e = cudaMalloc(&m->buf[i], want);
-    if (e == cudaSuccess) m->cap[i] = want;
-    return e;
 }
 
 extern "C" int orbfe_matcher_create(int device, OrbfeMatcher **out) {
@@ -902,7 +871,6 @@ extern "C" int orbfe_matcher_destroy(OrbfeMatcher *m) {
     if (!m) return ORBFE_OK;
     cudaSetDevice(m->device);
     if (m->stream) cudaStreamSynchronize(m->stream);
-    for (int i = 0; i < 6; i++) if (m->buf[i]) cudaFree(m->buf[i]);
     if (m->scratch) cudaFree(m->scratch);
     m->stage.release();
     if (m->d_err) cudaFree(m->d_err);
@@ -1135,8 +1103,31 @@ extern "C" int orbfe_search_by_bow_device(OrbfeMatcher *m, int variant, int njob
     return ORBFE_OK;
 }
 
-// SearchByBoW on host arrays: both sides staged as a two-frame store (frame 0 = side 1, frame 1 = side 2), one H2D, one job of
-// orbfe_search_by_bow_device, one D2H.
+// Offsets, in the staging block, of the two-frame store (frame 0 = side 1, frame 1 = side 2, `cap` slots each) that the
+// host-array SearchByBoW and SearchForTriangulation run as one job
+struct PairStore { size_t kps, desc, cnt, ids, ptr, items, nn, flags, idx; };
+
+// Packs side f of the store: its counts, frame index, descriptors and FeatureVector (nn nodes: ids, ptr, items).  Item slots
+// past ptr[nn] hold -1, so a row that reaches beyond the caller's items is rejected by the kernel instead of being read.
+static void pack_pair_side(unsigned char *H, const PairStore &o, int f, int cap, int n, const uint8_t *desc, int nn, const int32_t *ids,
+                           const int32_t *ptr, const int32_t *items) {
+    const size_t C = (size_t)cap;
+    ((int *)(H + o.cnt))[f] = n;
+    ((int *)(H + o.nn))[f] = nn;
+    ((int *)(H + o.idx))[f] = f;
+    if (n) memcpy(H + o.desc + f * C * 32, desc, (size_t)n * 32);
+    int *fptr = (int *)(H + o.ptr) + f * (C + 1), *fitems = (int *)(H + o.items) + f * C;
+    fptr[0] = 0;
+    if (nn) {
+        memcpy((int *)(H + o.ids) + f * C, ids, (size_t)nn * 4);
+        memcpy(fptr, ptr, ((size_t)nn + 1) * 4);
+    }
+    const int ni = nn ? std::min(std::max(ptr[nn], 0), cap) : 0;
+    if (ni) memcpy(fitems, items, (size_t)ni * 4);
+    std::fill(fitems + ni, fitems + C, -1);
+}
+
+// SearchByBoW on host arrays: both sides staged as a two-frame store, one H2D, one job of orbfe_search_by_bow_device, one D2H.
 extern "C" int orbfe_search_by_bow(OrbfeMatcher *m, int variant, int n1, const uint8_t *desc1, const uint8_t *valid1,
                                    const float *angle1, int nn1, const int32_t *ids1, const int32_t *ptr1, const int32_t *items1,
                                    int n2, const uint8_t *desc2, const uint8_t *valid2, const float *angle2, int nn2,
@@ -1151,45 +1142,32 @@ extern "C" int orbfe_search_by_bow(OrbfeMatcher *m, int variant, int n1, const u
     if (cap > 65535) return fail(ORBFE_ERR_UNSUPPORTED, "%d features or FeatureVector nodes on one side: at most 65535", cap);
     CU_TRY(cudaSetDevice(m->device));
     const size_t C = (size_t)cap;
-    size_t o_kps, o_desc, o_cnt, o_ids, o_ptr, o_items, o_nn, o_valid, o_idx, o_out, o_nm, total;
-    if (int rc = m->stage.layout({{&o_kps, 2 * C * sizeof(OrbfeKeyPoint)}, {&o_desc, 2 * C * 32}, {&o_cnt, 2 * sizeof(int)},
-                                  {&o_ids, 2 * C * 4}, {&o_ptr, 2 * (C + 1) * 4}, {&o_items, 2 * C * 4}, {&o_nn, 2 * sizeof(int)},
-                                  {&o_valid, 2 * C}, {&o_idx, 2 * sizeof(int)}, {&o_out, C * 4}, {&o_nm, sizeof(int)}},
+    PairStore o;
+    size_t o_out, o_nm, total;
+    if (int rc = m->stage.layout({{&o.kps, 2 * C * sizeof(OrbfeKeyPoint)}, {&o.desc, 2 * C * 32}, {&o.cnt, 2 * sizeof(int)},
+                                  {&o.ids, 2 * C * 4}, {&o.ptr, 2 * (C + 1) * 4}, {&o.items, 2 * C * 4}, {&o.nn, 2 * sizeof(int)},
+                                  {&o.flags, 2 * C}, {&o.idx, 2 * sizeof(int)}, {&o_out, C * 4}, {&o_nm, sizeof(int)}},
                               &total))
         return rc;
     unsigned char *H = m->stage.h, *D = m->stage.d;
-    const int n[2] = {n1, n2}, nn[2] = {nn1, nn2};
-    const uint8_t *desc[2] = {desc1, desc2}, *valid[2] = {valid1, variant == 1 ? valid2 : nullptr};
+    pack_pair_side(H, o, 0, cap, n1, desc1, nn1, ids1, ptr1, items1);
+    pack_pair_side(H, o, 1, cap, n2, desc2, nn2, ids2, ptr2, items2);
+    const int n[2] = {n1, n2};
+    const uint8_t *valid[2] = {valid1, variant == 1 ? valid2 : nullptr};
     const float *angle[2] = {angle1, angle2};
-    const int32_t *ids[2] = {ids1, ids2}, *ptr[2] = {ptr1, ptr2}, *items[2] = {items1, items2};
     for (int f = 0; f < 2; f++) {
-        ((int *)(H + o_cnt))[f] = n[f];
-        ((int *)(H + o_nn))[f] = nn[f];
-        ((int *)(H + o_idx))[f] = f;
         // search_by_bow_kernel reads no keypoint field but .angle
-        OrbfeKeyPoint *kp = (OrbfeKeyPoint *)(H + o_kps) + f * C;
+        OrbfeKeyPoint *kp = (OrbfeKeyPoint *)(H + o.kps) + f * C;
         for (int i = 0; i < n[f]; i++) kp[i].angle = angle[f][i];
-        if (n[f]) memcpy(H + o_desc + f * C * 32, desc[f], (size_t)n[f] * 32);
-        if (valid[f]) memcpy(H + o_valid + f * C, valid[f], (size_t)n[f]);
-        else memset(H + o_valid + f * C, 0, (size_t)n[f]);   // variant 0 ignores side 2's flags
-        // FeatureVector: item slots past ptr[nn] hold -1, so a row that reaches beyond the caller's items is rejected by
-        // the kernel instead of being read
-        int *fptr = (int *)(H + o_ptr) + f * (C + 1), *fitems = (int *)(H + o_items) + f * C;
-        fptr[0] = 0;
-        if (nn[f]) {
-            memcpy((int *)(H + o_ids) + f * C, ids[f], (size_t)nn[f] * 4);
-            memcpy(fptr, ptr[f], ((size_t)nn[f] + 1) * 4);
-        }
-        const int ni = nn[f] ? std::min(std::max(ptr[f][nn[f]], 0), cap) : 0;
-        if (ni) memcpy(fitems, items[f], (size_t)ni * 4);
-        std::fill(fitems + ni, fitems + C, -1);
+        if (valid[f]) memcpy(H + o.flags + f * C, valid[f], (size_t)n[f]);
+        else memset(H + o.flags + f * C, 0, (size_t)n[f]);   // variant 0 ignores side 2's flags
     }
     cudaStream_t s = m->stream;
     CU_TRY(cudaMemcpyAsync(D, H, o_out, cudaMemcpyHostToDevice, s));
-    const int *d_idx = (const int *)(D + o_idx);
-    int rc = orbfe_search_by_bow_device(m, variant, 1, (const OrbfeKeyPoint *)(D + o_kps), D + o_desc, (const int *)(D + o_cnt), cap,
-                                        (const int32_t *)(D + o_ids), (const int32_t *)(D + o_ptr), (const int32_t *)(D + o_items),
-                                        (const int *)(D + o_nn), D + o_valid, d_idx, d_idx + 1, nnratio, check_orientation,
+    const int *d_idx = (const int *)(D + o.idx);
+    int rc = orbfe_search_by_bow_device(m, variant, 1, (const OrbfeKeyPoint *)(D + o.kps), D + o.desc, (const int *)(D + o.cnt), cap,
+                                        (const int32_t *)(D + o.ids), (const int32_t *)(D + o.ptr), (const int32_t *)(D + o.items),
+                                        (const int *)(D + o.nn), D + o.flags, d_idx, d_idx + 1, nnratio, check_orientation,
                                         (int32_t *)(D + o_out), (int *)(D + o_nm), s);
     if (rc) return rc;
     CU_TRY(cudaMemcpyAsync(H + o_out, D + o_out, total - o_out, cudaMemcpyDeviceToHost, s));
@@ -1245,45 +1223,32 @@ extern "C" int orbfe_search_for_triangulation(OrbfeMatcher *m, int n1, const Orb
     for (int i = 0; i < n2; i++) nlevels = std::max(nlevels, std::min(keys2[i].octave, ORBFE_MAX_LEVELS - 1) + 1);
     CU_TRY(cudaSetDevice(m->device));
     const size_t C = (size_t)cap;
-    size_t o_kps, o_desc, o_cnt, o_ids, o_ptr, o_items, o_nn, o_has, o_idx, o_F, o_out, o_nm, total;
-    if (int rc = m->stage.layout({{&o_kps, 2 * C * sizeof(OrbfeKeyPoint)}, {&o_desc, 2 * C * 32}, {&o_cnt, 2 * sizeof(int)},
-                                  {&o_ids, 2 * C * 4}, {&o_ptr, 2 * (C + 1) * 4}, {&o_items, 2 * C * 4}, {&o_nn, 2 * sizeof(int)},
-                                  {&o_has, 2 * C}, {&o_idx, 2 * sizeof(int)}, {&o_F, 9 * sizeof(float)}, {&o_out, C * 4},
+    PairStore o;
+    size_t o_F, o_out, o_nm, total;
+    if (int rc = m->stage.layout({{&o.kps, 2 * C * sizeof(OrbfeKeyPoint)}, {&o.desc, 2 * C * 32}, {&o.cnt, 2 * sizeof(int)},
+                                  {&o.ids, 2 * C * 4}, {&o.ptr, 2 * (C + 1) * 4}, {&o.items, 2 * C * 4}, {&o.nn, 2 * sizeof(int)},
+                                  {&o.flags, 2 * C}, {&o.idx, 2 * sizeof(int)}, {&o_F, 9 * sizeof(float)}, {&o_out, C * 4},
                                   {&o_nm, sizeof(int)}},
                               &total))
         return rc;
     unsigned char *H = m->stage.h, *D = m->stage.d;
-    const int n[2] = {n1, n2}, nn[2] = {nn1, nn2};
+    pack_pair_side(H, o, 0, cap, n1, desc1, nn1, ids1, ptr1, items1);
+    pack_pair_side(H, o, 1, cap, n2, desc2, nn2, ids2, ptr2, items2);
+    const int n[2] = {n1, n2};
     const OrbfeKeyPoint *keys[2] = {keys1, keys2};
-    const uint8_t *desc[2] = {desc1, desc2}, *has_mp[2] = {has_mp1, has_mp2};
-    const int32_t *ids[2] = {ids1, ids2}, *ptr[2] = {ptr1, ptr2}, *items[2] = {items1, items2};
+    const uint8_t *has_mp[2] = {has_mp1, has_mp2};
     for (int f = 0; f < 2; f++) {
-        ((int *)(H + o_cnt))[f] = n[f];
-        ((int *)(H + o_nn))[f] = nn[f];
-        ((int *)(H + o_idx))[f] = f;
-        if (n[f]) {
-            memcpy(H + o_kps + f * C * sizeof(OrbfeKeyPoint), keys[f], (size_t)n[f] * sizeof(OrbfeKeyPoint));
-            memcpy(H + o_desc + f * C * 32, desc[f], (size_t)n[f] * 32);
-            memcpy(H + o_has + f * C, has_mp[f], (size_t)n[f]);
-        }
-        // FeatureVector, as in orbfe_search_by_bow
-        int *fptr = (int *)(H + o_ptr) + f * (C + 1), *fitems = (int *)(H + o_items) + f * C;
-        fptr[0] = 0;
-        if (nn[f]) {
-            memcpy((int *)(H + o_ids) + f * C, ids[f], (size_t)nn[f] * 4);
-            memcpy(fptr, ptr[f], ((size_t)nn[f] + 1) * 4);
-        }
-        const int ni = nn[f] ? std::min(std::max(ptr[f][nn[f]], 0), cap) : 0;
-        if (ni) memcpy(fitems, items[f], (size_t)ni * 4);
-        std::fill(fitems + ni, fitems + C, -1);
+        if (!n[f]) continue;
+        memcpy(H + o.kps + f * C * sizeof(OrbfeKeyPoint), keys[f], (size_t)n[f] * sizeof(OrbfeKeyPoint));
+        memcpy(H + o.flags + f * C, has_mp[f], (size_t)n[f]);
     }
     memcpy(H + o_F, F12, 9 * sizeof(float));
     cudaStream_t s = m->stream;
     CU_TRY(cudaMemcpyAsync(D, H, o_out, cudaMemcpyHostToDevice, s));
-    const int *d_idx = (const int *)(D + o_idx);
-    int rc = orbfe_search_for_triangulation_device(m, 1, (const OrbfeKeyPoint *)(D + o_kps), D + o_desc, (const int *)(D + o_cnt), cap,
-                                                   (const int32_t *)(D + o_ids), (const int32_t *)(D + o_ptr),
-                                                   (const int32_t *)(D + o_items), (const int *)(D + o_nn), D + o_has, d_idx, d_idx + 1,
+    const int *d_idx = (const int *)(D + o.idx);
+    int rc = orbfe_search_for_triangulation_device(m, 1, (const OrbfeKeyPoint *)(D + o.kps), D + o.desc, (const int *)(D + o.cnt), cap,
+                                                   (const int32_t *)(D + o.ids), (const int32_t *)(D + o.ptr),
+                                                   (const int32_t *)(D + o.items), (const int *)(D + o.nn), D + o.flags, d_idx, d_idx + 1,
                                                    (const float *)(D + o_F), sigma2_kf2, nlevels, check_orientation,
                                                    (int32_t *)(D + o_out), (int *)(D + o_nm), s);
     if (rc) return rc;
@@ -1313,46 +1278,56 @@ extern "C" int orbfe_hamming_csr(OrbfeMatcher *m, const uint8_t *q, int nq, cons
     if (!q || !row_ptr) return fail(ORBFE_ERR_ARG, "NULL argument");
     const int np = row_ptr[nq];
     if (np == 0) return ORBFE_OK;
+    if (np < 0) return fail(ORBFE_ERR_ARG, "row_ptr[nq]=%d is negative", np);
     if (!t || !cols || !out || nt == 0) return fail(ORBFE_ERR_ARG, "NULL argument");
     for (int k = 0; k < np; k++)
         if (cols[k] < 0 || cols[k] >= nt) return fail(ORBFE_ERR_ARG, "cols[%d]=%d out of range", k, cols[k]);
     CU_TRY(cudaSetDevice(m->device));
-    CU_TRY(mreserve(m, 0, (size_t)nq * 32));
-    CU_TRY(mreserve(m, 1, (size_t)nt * 32));
-    CU_TRY(mreserve(m, 2, sizeof(int32_t) * ((size_t)nq + 1)));
-    CU_TRY(mreserve(m, 3, sizeof(int32_t) * (size_t)np));
-    CU_TRY(mreserve(m, 4, sizeof(uint16_t) * (size_t)np));
+    const size_t b_q = (size_t)nq * 32, b_t = (size_t)nt * 32, b_row = sizeof(int32_t) * ((size_t)nq + 1);
+    const size_t b_cols = sizeof(int32_t) * (size_t)np, b_out = sizeof(uint16_t) * (size_t)np;
+    size_t o_q, o_t, o_row, o_cols, o_out, total;
+    if (int rc = m->stage.layout({{&o_q, b_q}, {&o_t, b_t}, {&o_row, b_row}, {&o_cols, b_cols}, {&o_out, b_out}}, &total)) return rc;
+    unsigned char *H = m->stage.h, *D = m->stage.d;
+    memcpy(H + o_q, q, b_q);
+    memcpy(H + o_t, t, b_t);
+    memcpy(H + o_row, row_ptr, b_row);
+    memcpy(H + o_cols, cols, b_cols);
     cudaStream_t s = m->stream;
-    CU_TRY(cudaMemcpyAsync(m->buf[0], q, (size_t)nq * 32, cudaMemcpyHostToDevice, s));
-    CU_TRY(cudaMemcpyAsync(m->buf[1], t, (size_t)nt * 32, cudaMemcpyHostToDevice, s));
-    CU_TRY(cudaMemcpyAsync(m->buf[2], row_ptr, sizeof(int32_t) * ((size_t)nq + 1), cudaMemcpyHostToDevice, s));
-    CU_TRY(cudaMemcpyAsync(m->buf[3], cols, sizeof(int32_t) * (size_t)np, cudaMemcpyHostToDevice, s));
-    launch_hamming_csr((const uint8_t *)m->buf[0], (const uint8_t *)m->buf[1], (const int32_t *)m->buf[2],
-                       (const int32_t *)m->buf[3], nq, np, (uint16_t *)m->buf[4], s);
-    CU_TRY(cudaGetLastError());
-    m->h2d_bytes += (size_t)nq * 32 + (size_t)nt * 32 + sizeof(int32_t) * ((size_t)nq + 1 + np);
-    m->d2h_bytes += sizeof(uint16_t) * (size_t)np;
+    CU_TRY(cudaMemcpyAsync(D, H, o_out, cudaMemcpyHostToDevice, s));
+    if (int rc = orbfe_hamming_csr_device(m, D + o_q, D + o_t, (const int32_t *)(D + o_row), (const int32_t *)(D + o_cols), nq, np,
+                                          (uint16_t *)(D + o_out), s))
+        return rc;
     m->launches += 1;
-    CU_TRY(cudaMemcpyAsync(out, m->buf[4], sizeof(uint16_t) * (size_t)np, cudaMemcpyDeviceToHost, s));
+    CU_TRY(cudaMemcpyAsync(H + o_out, D + o_out, total - o_out, cudaMemcpyDeviceToHost, s));
     CU_TRY(cudaStreamSynchronize(s));
+    m->h2d_bytes += o_out;
+    m->d2h_bytes += total - o_out;
+    memcpy(out, H + o_out, b_out);
     return ORBFE_OK;
 }
 
+// The staging block is pinned and sized by the largest call the handle has seen: an nq x nt output this large stays pinned
+// for the handle's lifetime.
 extern "C" int orbfe_hamming_dense(OrbfeMatcher *m, const uint8_t *q, int nq, const uint8_t *t, int nt, uint16_t *out) {
     if (!m || nq < 0 || nt < 0) return fail(ORBFE_ERR_ARG, "bad arguments");
     if (nq == 0 || nt == 0) return ORBFE_OK;
     if (!q || !t || !out) return fail(ORBFE_ERR_ARG, "NULL argument");
     CU_TRY(cudaSetDevice(m->device));
-    CU_TRY(mreserve(m, 0, (size_t)nq * 32));
-    CU_TRY(mreserve(m, 1, (size_t)nt * 32));
-    CU_TRY(mreserve(m, 4, sizeof(uint16_t) * (size_t)nq * nt));
+    const size_t b_q = (size_t)nq * 32, b_t = (size_t)nt * 32, b_out = sizeof(uint16_t) * (size_t)nq * nt;
+    size_t o_q, o_t, o_out, total;
+    if (int rc = m->stage.layout({{&o_q, b_q}, {&o_t, b_t}, {&o_out, b_out}}, &total)) return rc;
+    unsigned char *H = m->stage.h, *D = m->stage.d;
+    memcpy(H + o_q, q, b_q);
+    memcpy(H + o_t, t, b_t);
     cudaStream_t s = m->stream;
-    CU_TRY(cudaMemcpyAsync(m->buf[0], q, (size_t)nq * 32, cudaMemcpyHostToDevice, s));
-    CU_TRY(cudaMemcpyAsync(m->buf[1], t, (size_t)nt * 32, cudaMemcpyHostToDevice, s));
-    launch_hamming_dense((const uint8_t *)m->buf[0], nq, (const uint8_t *)m->buf[1], nt, (uint16_t *)m->buf[4], s);
+    CU_TRY(cudaMemcpyAsync(D, H, o_out, cudaMemcpyHostToDevice, s));
+    launch_hamming_dense(D + o_q, nq, D + o_t, nt, (uint16_t *)(D + o_out), s);
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(out, m->buf[4], sizeof(uint16_t) * (size_t)nq * nt, cudaMemcpyDeviceToHost, s));
+    CU_TRY(cudaMemcpyAsync(H + o_out, D + o_out, total - o_out, cudaMemcpyDeviceToHost, s));
     CU_TRY(cudaStreamSynchronize(s));
+    m->h2d_bytes += o_out;
+    m->d2h_bytes += total - o_out;
+    memcpy(out, H + o_out, b_out);
     return ORBFE_OK;
 }
 
@@ -1384,14 +1359,19 @@ extern "C" int orbfe_undistort_keypoints(OrbfeMatcher *m, const OrbfeKeyPoint *i
         return ORBFE_OK;
     }
     CU_TRY(cudaSetDevice(m->device));
-    CU_TRY(mreserve(m, 0, sizeof(OrbfeKeyPoint) * (size_t)n));
+    // one array, undistorted in place on the device: input and output of the block at once
+    size_t o_kps, total;
+    if (int rc = m->stage.layout({{&o_kps, sizeof(OrbfeKeyPoint) * (size_t)n}}, &total)) return rc;
+    OrbfeKeyPoint *h_kps = (OrbfeKeyPoint *)m->stage.h, *d_kps = (OrbfeKeyPoint *)m->stage.d;
+    memcpy(h_kps, in, sizeof(OrbfeKeyPoint) * (size_t)n);
     cudaStream_t s = m->stream;
-    CU_TRY(cudaMemcpyAsync(m->buf[0], in, sizeof(OrbfeKeyPoint) * (size_t)n, cudaMemcpyHostToDevice, s));
-    const int rc = orbfe_undistort_keypoints_device(m, (const OrbfeKeyPoint *)m->buf[0], (OrbfeKeyPoint *)m->buf[0], n, fx, fy, cx, cy,
-                                                    dist5, s);
-    if (rc) return rc;
-    CU_TRY(cudaMemcpyAsync(out, m->buf[0], sizeof(OrbfeKeyPoint) * (size_t)n, cudaMemcpyDeviceToHost, s));
+    CU_TRY(cudaMemcpyAsync(d_kps, h_kps, total, cudaMemcpyHostToDevice, s));
+    if (int rc = orbfe_undistort_keypoints_device(m, d_kps, d_kps, n, fx, fy, cx, cy, dist5, s)) return rc;
+    CU_TRY(cudaMemcpyAsync(h_kps, d_kps, total, cudaMemcpyDeviceToHost, s));
     CU_TRY(cudaStreamSynchronize(s));
+    m->h2d_bytes += total;
+    m->d2h_bytes += total;
+    memcpy(out, h_kps, sizeof(OrbfeKeyPoint) * (size_t)n);
     return ORBFE_OK;
 }
 
@@ -1415,13 +1395,6 @@ extern "C" int orbfe_image_bounds(OrbfeMatcher *m, int cols, int rows, float fx,
 }
 
 // MapPoint::ComputeDistinctiveDescriptors for many map points in one launch (include/orbfe_bow.h)
-#include "../../include/orbfe_bow.h"
-namespace orbfe {
-void launch_distinctive(const uint8_t *d_desc, const int *d_group_ptr, int ngroups, int *d_best, cudaStream_t s);
-// bow_kernels.cu; an out-of-range group pointer or observation sets bit 8 of *d_err
-void launch_distinctive_obs(const uint8_t *d_desc, const int *d_counts, int nframes, int cap, const int *d_group_ptr,
-                            const int *d_obs, int nobs, int ngroups, int *d_best, uint8_t *d_mp_desc, int *d_err, cudaStream_t s);
-}
 extern "C" int orbfe_distinctive_descriptors(OrbfeMatcher *m, const uint8_t *desc, const int32_t *group_ptr, int ngroups,
                                              int32_t *best_out) {
     if (!m || ngroups < 0) return fail(ORBFE_ERR_ARG, "bad arguments");
@@ -1432,17 +1405,22 @@ extern "C" int orbfe_distinctive_descriptors(OrbfeMatcher *m, const uint8_t *des
     for (int g = 0; g < ngroups; g++)
         if (group_ptr[g + 1] < group_ptr[g]) return fail(ORBFE_ERR_ARG, "group_ptr must be non-decreasing");
     CU_TRY(cudaSetDevice(m->device));
-    CU_TRY(mreserve(m, 0, (size_t)std::max(total, 1) * 32));
-    CU_TRY(mreserve(m, 2, sizeof(int) * ((size_t)ngroups + 1)));
-    CU_TRY(mreserve(m, 3, sizeof(int) * (size_t)ngroups));
+    const size_t b_desc = (size_t)total * 32, b_ptr = sizeof(int) * ((size_t)ngroups + 1), b_best = sizeof(int) * (size_t)ngroups;
+    size_t o_desc, o_ptr, o_best, nbytes;
+    if (int rc = m->stage.layout({{&o_desc, b_desc}, {&o_ptr, b_ptr}, {&o_best, b_best}}, &nbytes)) return rc;
+    unsigned char *H = m->stage.h, *D = m->stage.d;
+    if (total > 0) memcpy(H + o_desc, desc, b_desc);   // all groups empty: nothing to upload, the launch still writes every -1
+    memcpy(H + o_ptr, group_ptr, b_ptr);
     cudaStream_t s = m->stream;
-    if (total > 0) CU_TRY(cudaMemcpyAsync(m->buf[0], desc, (size_t)total * 32, cudaMemcpyHostToDevice, s));
-    CU_TRY(cudaMemcpyAsync(m->buf[2], group_ptr, sizeof(int) * ((size_t)ngroups + 1), cudaMemcpyHostToDevice, s));
-    launch_distinctive((const uint8_t *)m->buf[0], (const int *)m->buf[2], ngroups, (int *)m->buf[3], s);
+    CU_TRY(cudaMemcpyAsync(D, H, o_best, cudaMemcpyHostToDevice, s));
+    launch_distinctive(D + o_desc, (const int *)(D + o_ptr), ngroups, (int *)(D + o_best), s);
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(best_out, m->buf[3], sizeof(int) * (size_t)ngroups, cudaMemcpyDeviceToHost, s));
+    CU_TRY(cudaMemcpyAsync(H + o_best, D + o_best, nbytes - o_best, cudaMemcpyDeviceToHost, s));
     CU_TRY(cudaStreamSynchronize(s));
+    m->h2d_bytes += o_best;
+    m->d2h_bytes += nbytes - o_best;
     m->launches += 1;
+    memcpy(best_out, H + o_best, b_best);
     return ORBFE_OK;
 }
 
@@ -1467,42 +1445,41 @@ extern "C" int orbfe_distinctive_descriptors_device(OrbfeMatcher *m, int ngroups
 }
 
 // Device half of orbfe_bow_db_detect (host/bow_host.cpp): per-keyframe shared-word count, first shared word, L1 score.
-namespace orbfe {
-void launch_bow_db_score(int nq, const int *q_ids, const double *q_vals, int nkf, const int *kf_ptr, const int *db_ids,
-                         const double *db_vals, int *common, int *first, double *score, cudaStream_t s);
-int bow_db_score(OrbfeMatcher *m, int nq, const int32_t *q_ids, const double *q_vals, int nkf, const int32_t *kf_ptr,
-                 const int32_t *db_ids, const double *db_vals, int32_t *common, int32_t *first, double *score) {
-    const size_t nw = (size_t)kf_ptr[nkf];
+int orbfe::bow_db_score(OrbfeMatcher *m, int nq, const int32_t *q_ids, const double *q_vals, int nkf, const int32_t *kf_ptr,
+                        const int32_t *db_ids, const double *db_vals, int32_t *common, int32_t *first, double *score) {
+    const size_t NQ = (size_t)nq, NK = (size_t)nkf, nw = (size_t)kf_ptr[nkf];
     CU_TRY(cudaSetDevice(m->device));
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-    const size_t o_qi = take(sizeof(int) * (size_t)std::max(nq, 1)), o_qv = take(sizeof(double) * (size_t)std::max(nq, 1));
-    const size_t o_kp = take(sizeof(int) * ((size_t)nkf + 1)), o_di = take(sizeof(int) * std::max<size_t>(nw, 1));
-    const size_t o_dv = take(sizeof(double) * std::max<size_t>(nw, 1));
-    const size_t o_c = take(sizeof(int) * (size_t)nkf), o_f = take(sizeof(int) * (size_t)nkf), o_s = take(sizeof(double) * (size_t)nkf);
-    CU_TRY(mreserve(m, 5, off));
-    unsigned char *D = (unsigned char *)m->buf[5];
-    cudaStream_t s = m->stream;
+    size_t o_qi, o_qv, o_kp, o_di, o_dv, o_c, o_f, o_s, total;
+    if (int rc = m->stage.layout({{&o_qi, NQ * sizeof(int)}, {&o_qv, NQ * sizeof(double)}, {&o_kp, (NK + 1) * sizeof(int)},
+                                  {&o_di, nw * sizeof(int)}, {&o_dv, nw * sizeof(double)}, {&o_c, NK * sizeof(int)},
+                                  {&o_f, NK * sizeof(int)}, {&o_s, NK * sizeof(double)}},
+                              &total))
+        return rc;
+    unsigned char *H = m->stage.h, *D = m->stage.d;
     if (nq > 0) {
-        CU_TRY(cudaMemcpyAsync(D + o_qi, q_ids, sizeof(int) * (size_t)nq, cudaMemcpyHostToDevice, s));
-        CU_TRY(cudaMemcpyAsync(D + o_qv, q_vals, sizeof(double) * (size_t)nq, cudaMemcpyHostToDevice, s));
+        memcpy(H + o_qi, q_ids, NQ * sizeof(int));
+        memcpy(H + o_qv, q_vals, NQ * sizeof(double));
     }
-    CU_TRY(cudaMemcpyAsync(D + o_kp, kf_ptr, sizeof(int) * ((size_t)nkf + 1), cudaMemcpyHostToDevice, s));
+    memcpy(H + o_kp, kf_ptr, (NK + 1) * sizeof(int));
     if (nw > 0) {
-        CU_TRY(cudaMemcpyAsync(D + o_di, db_ids, sizeof(int) * nw, cudaMemcpyHostToDevice, s));
-        CU_TRY(cudaMemcpyAsync(D + o_dv, db_vals, sizeof(double) * nw, cudaMemcpyHostToDevice, s));
+        memcpy(H + o_di, db_ids, nw * sizeof(int));
+        memcpy(H + o_dv, db_vals, nw * sizeof(double));
     }
+    cudaStream_t s = m->stream;
+    CU_TRY(cudaMemcpyAsync(D, H, o_c, cudaMemcpyHostToDevice, s));
     launch_bow_db_score(nq, (const int *)(D + o_qi), (const double *)(D + o_qv), nkf, (const int *)(D + o_kp), (const int *)(D + o_di),
                         (const double *)(D + o_dv), (int *)(D + o_c), (int *)(D + o_f), (double *)(D + o_s), s);
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(common, D + o_c, sizeof(int) * (size_t)nkf, cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaMemcpyAsync(first, D + o_f, sizeof(int) * (size_t)nkf, cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaMemcpyAsync(score, D + o_s, sizeof(double) * (size_t)nkf, cudaMemcpyDeviceToHost, s));
+    CU_TRY(cudaMemcpyAsync(H + o_c, D + o_c, total - o_c, cudaMemcpyDeviceToHost, s));
     CU_TRY(cudaStreamSynchronize(s));
+    m->h2d_bytes += o_c;
+    m->d2h_bytes += total - o_c;
     m->launches += 1;
+    memcpy(common, H + o_c, NK * sizeof(int));
+    memcpy(first, H + o_f, NK * sizeof(int));
+    memcpy(score, H + o_s, NK * sizeof(double));
     return ORBFE_OK;
 }
-}  // namespace orbfe
 
 extern "C" int orbfe_knn2_groups_device(OrbfeMatcher *m, const uint8_t *d_q, int nq, const uint8_t *d_db, int ngroups,
                                         int group_size, uint16_t *d_best, int32_t *d_best_idx, uint16_t *d_second,
@@ -1517,28 +1494,36 @@ extern "C" int orbfe_knn2_groups_device(OrbfeMatcher *m, const uint8_t *d_q, int
     return ORBFE_OK;
 }
 
+// The database is staged through the handle's pinned block, which keeps the size of the largest call; a bulk sweep belongs on
+// orbfe_knn2_groups_device.
 extern "C" int orbfe_knn2_groups(OrbfeMatcher *m, const uint8_t *q, int nq, const uint8_t *db, int ngroups,
                                  int group_size, uint16_t *best, int32_t *best_idx, uint16_t *second) {
     if (!m || nq < 0 || ngroups < 0 || group_size < 0) return fail(ORBFE_ERR_ARG, "bad arguments");
     if (nq == 0 || ngroups == 0) return ORBFE_OK;
     if (!q || !db || !best || !best_idx || !second) return fail(ORBFE_ERR_ARG, "NULL argument");
     CU_TRY(cudaSetDevice(m->device));
-    const size_t ndb = (size_t)ngroups * group_size, no = (size_t)ngroups * nq;
-    CU_TRY(mreserve(m, 0, (size_t)nq * 32));
-    CU_TRY(mreserve(m, 1, ndb * 32));
-    CU_TRY(mreserve(m, 2, sizeof(uint16_t) * no));
-    CU_TRY(mreserve(m, 3, sizeof(int32_t) * no));
-    CU_TRY(mreserve(m, 4, sizeof(uint16_t) * no));
+    const size_t no = (size_t)ngroups * nq;
+    const size_t b_q = (size_t)nq * 32, b_db = (size_t)ngroups * group_size * 32;
+    size_t o_q, o_db, o_best, o_idx, o_second, total;
+    if (int rc = m->stage.layout({{&o_q, b_q}, {&o_db, b_db}, {&o_best, sizeof(uint16_t) * no}, {&o_idx, sizeof(int32_t) * no},
+                                  {&o_second, sizeof(uint16_t) * no}},
+                              &total))
+        return rc;
+    unsigned char *H = m->stage.h, *D = m->stage.d;
+    memcpy(H + o_q, q, b_q);
+    memcpy(H + o_db, db, b_db);
     cudaStream_t s = m->stream;
-    CU_TRY(cudaMemcpyAsync(m->buf[0], q, (size_t)nq * 32, cudaMemcpyHostToDevice, s));
-    CU_TRY(cudaMemcpyAsync(m->buf[1], db, ndb * 32, cudaMemcpyHostToDevice, s));
-    launch_knn2_groups((const uint8_t *)m->buf[0], nq, (const uint8_t *)m->buf[1], ngroups, group_size,
-                       (uint16_t *)m->buf[2], (int32_t *)m->buf[3], (uint16_t *)m->buf[4], s);
-    CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(best, m->buf[2], sizeof(uint16_t) * no, cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaMemcpyAsync(best_idx, m->buf[3], sizeof(int32_t) * no, cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaMemcpyAsync(second, m->buf[4], sizeof(uint16_t) * no, cudaMemcpyDeviceToHost, s));
+    CU_TRY(cudaMemcpyAsync(D, H, o_best, cudaMemcpyHostToDevice, s));
+    if (int rc = orbfe_knn2_groups_device(m, D + o_q, nq, D + o_db, ngroups, group_size, (uint16_t *)(D + o_best), (int32_t *)(D + o_idx),
+                                          (uint16_t *)(D + o_second), s))
+        return rc;
+    CU_TRY(cudaMemcpyAsync(H + o_best, D + o_best, total - o_best, cudaMemcpyDeviceToHost, s));
     CU_TRY(cudaStreamSynchronize(s));
+    m->h2d_bytes += o_best;
+    m->d2h_bytes += total - o_best;
+    memcpy(best, H + o_best, sizeof(uint16_t) * no);
+    memcpy(best_idx, H + o_idx, sizeof(int32_t) * no);
+    memcpy(second, H + o_second, sizeof(uint16_t) * no);
     return ORBFE_OK;
 }
 

@@ -203,9 +203,10 @@ void launch_undistort(float fx, float fy, float cx, float cy, const float *dist5
 // records the thread's last-error string (orbfe_last_error) and returns `code`
 int set_error(int code, const char *fmt, ...);
 
-// Staging block of the host-array entries that run on a device kernel (orbfe_api.cu): a grow-only pinned host block h and
-// its device twin d.  The entry packs h, copies it to d in one H2D, runs its kernels, copies the results back in one D2H and
-// synchronises before it returns.  The block serves one call at a time: the vocabulary holds its mutex across each call.
+// Staging block of every host-array entry of a matcher or vocabulary handle: a grow-only pinned host block h and its device
+// twin d.  The entry packs h, copies it to d in one H2D, runs its kernels, copies the results back in one D2H and
+// synchronises before it returns.  Both keep the size (times 1.25) of the largest call the handle has seen.  The block serves
+// one call at a time: the vocabulary holds its mutex across each call.
 struct Stage {
     unsigned char *h = nullptr;
     unsigned char *d = nullptr;
@@ -222,5 +223,18 @@ void launch_hamming_csr(const uint8_t *q, const uint8_t *t, const int32_t *row_p
 void launch_hamming_dense(const uint8_t *q, int nq, const uint8_t *t, int nt, uint16_t *out, cudaStream_t s);
 void launch_knn2_groups(const uint8_t *q, int nq, const uint8_t *db, int ngroups, int group_size,
                         uint16_t *best, int32_t *best_idx, uint16_t *second, cudaStream_t s);
+
+// ---- launchers (bow_kernels.cu) ----
+void launch_distinctive(const uint8_t *d_desc, const int *d_group_ptr, int ngroups, int *d_best, cudaStream_t s);
+// an out-of-range group pointer or observation sets bit 8 of *d_err
+void launch_distinctive_obs(const uint8_t *d_desc, const int *d_counts, int nframes, int cap, const int *d_group_ptr,
+                            const int *d_obs, int nobs, int ngroups, int *d_best, uint8_t *d_mp_desc, int *d_err, cudaStream_t s);
+void launch_bow_db_score(int nq, const int *q_ids, const double *q_vals, int nkf, const int *kf_ptr, const int *db_ids,
+                         const double *db_vals, int *common, int *first, double *score, cudaStream_t s);
+
+// Device half of orbfe_bow_db_detect (orbfe_api.cu; the host half is host/bow_host.cpp): per keyframe, the shared-word count,
+// the first shared word and the L1 score, staged through the matcher's block and synchronised
+int bow_db_score(OrbfeMatcher *m, int nq, const int32_t *q_ids, const double *q_vals, int nkf, const int32_t *kf_ptr,
+                 const int32_t *db_ids, const double *db_vals, int32_t *common, int32_t *first, double *score);
 
 }  // namespace orbfe

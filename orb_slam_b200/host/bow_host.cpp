@@ -9,13 +9,7 @@
 #include <vector>
 
 #include "../../include/orbfe_bow.h"
-
-struct OrbfeMatcher;
-namespace orbfe {
-int set_error(int code, const char *fmt, ...);
-int bow_db_score(OrbfeMatcher *m, int nq, const int32_t *q_ids, const double *q_vals, int nkf, const int32_t *kf_ptr,
-                 const int32_t *db_ids, const double *db_vals, int32_t *common, int32_t *first, double *score);
-}
+#include "../csrc/orbfe_internal.h"
 
 extern "C" int orbfe_bow_db_detect(OrbfeMatcher *m, int mode, int nq, const int32_t *q_ids, const double *q_vals, int nkf,
                                    const int32_t *kf_ptr, const int32_t *db_ids, const double *db_vals, const uint8_t *connected,
