@@ -556,9 +556,10 @@ __device__ __forceinline__ void fast_tile_compute(const PlanDev *__restrict__ pl
 }
 
 // ------------------------------------------------------------------------------------------------
-// The FAST kernel: ORBFE_FAST_BLOCKS_PER_SM persistent CTAs per SM; the pixel tile of work item i+1 is fetched by the
-// Tensor Memory Accelerator (cp.async.bulk.tensor.3d -> UTMALDG) into the second buffer while item i is
-// being computed; completion is signalled on an mbarrier.  One 3-D tensor map (x, y, frame) per level;
+// The FAST kernel: ORBFE_FAST_BLOCKS_PER_SM resident CTAs per SM; pixel tiles are fetched by the Tensor Memory
+// Accelerator (cp.async.bulk.tensor.3d -> UTMALDG), completion is signalled on an mbarrier.  A CTA walks work items
+// blockIdx.x, + gridDim.x, ...; when it has more than one, the tile of item i+1 is fetched into the second buffer while
+// item i is being computed.  One 3-D tensor map (x, y, frame) per level;
 // out-of-image parts of the box are zero-filled by the hardware (they only feed masked m positions).
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -650,8 +651,10 @@ int fast_tma_setup() {
 void launch_fast_nms(const PlanDev *d_plan, const PlanDev &hp, WorkDev w, int f0, int nf, cudaStream_t s) {
     if (hp.nftiles_total == 0) return;  // every level has an empty cell grid: nothing to detect
     const int nwork = hp.nftiles_total * nf;
-    const int grid = min(nwork, w.fast_grid);
-    launch_k(fast_nms_tma_kernel, dim3(grid), dim3(256), F2_TMA_SMEM, s, hp.pdl != 0, d_plan, w, f0, nwork);
+    // one CTA per (tile, frame): the block scheduler hands the next tile to whichever CTA slot frees first.  The cost of a
+    // tile varies with its candidates, and a persistent grid of 3 CTAs per SM walking a fixed share of the tiles finished
+    // later (H100, 64 x 1080p: 1.51 ms against 1.68 ms, DESIGN.md §4.2).
+    launch_k(fast_nms_tma_kernel, dim3(nwork), dim3(256), F2_TMA_SMEM, s, hp.pdl != 0, d_plan, w, f0, nwork);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -402,9 +402,6 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
         ex->d_maps = d_maps;
         cudaError_t e = (cudaError_t)fast_tma_setup();
         if (e != cudaSuccess) return fail(ORBFE_ERR_CUDA, "cudaFuncSetAttribute(fast_nms_tma_kernel): %s", cudaGetErrorString(e));
-        int nsm = 132;
-        cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, ex->device);
-        Wk.fast_grid = ORBFE_FAST_BLOCKS_PER_SM * nsm;  // resident persistent CTAs (39 KB smem each)
     }
     CU_TRY(dmalloc(ex, &Wk.cand_keys, (size_t)cand_total * B));
     if (ex->score_type == 0) {

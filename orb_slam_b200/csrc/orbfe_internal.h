@@ -17,8 +17,8 @@
 // FAST/NMS tile (detect-area pixels per CTA) and blur tile
 #define ORBFE_FT_W 120
 #define ORBFE_FT_H 62
-// resident persistent CTAs per SM of the FAST kernel: its register budget (80) and its grid (this x SMs).  3 x 80
-// measured faster on H100 than 4 x 64, which spills (DESIGN.md §4.2).
+// resident CTAs per SM of the FAST kernel: its launch bounds, hence its register budget (80).  3 x 80 measured faster on
+// H100 than 4 x 64, which spills (DESIGN.md §4.2).
 #define ORBFE_FAST_BLOCKS_PER_SM 3
 #define ORBFE_BT_W 120
 #define ORBFE_BT_H 64
@@ -79,7 +79,6 @@ struct WorkDev {
     const FTileInfo *ftile_info;      // [nftiles_total]
     const BTileInfo *btile_info;      // [nbtiles_total]
     const CUtensorMap *tmaps;         // [nlevels] 3-D (x, y, frame) tensor maps of the unblurred levels; never NULL (build_plan fails without TMA)
-    int fast_grid;                    // persistent CTAs of the FAST kernel (ORBFE_FAST_BLOCKS_PER_SM x SMs)
     uint32_t *cand_keys;              // [batch][cand_total]   (score<<24 | 0xFFFFFF - raster)
     unsigned long long *cand_keys64;  // HARRIS_SCORE only: order(resp)<<32 | (0xFFFFFF - raster)<<8 | score; NULL otherwise
     uint32_t *kept_aux;               // HARRIS_SCORE only: low raster bits + score of each kept entry
