@@ -7,7 +7,8 @@
  *        caller LoopClosing.cc:117-131)
  *   N3  KeyFrameDatabase::DetectLoopCandidates / DetectRelocalisationCandidates on arrays
  *       (reference src/KeyFrameDatabase.cc:73-308, L1Scoring::score Thirdparty/DBoW2/DBoW2/ScoringObject.cpp:23-67)
- *   N4  MapPoint::ComputeDistinctiveDescriptors, batched over map points (reference src/MapPoint.cc:185-250)
+ *   N4  MapPoint::ComputeDistinctiveDescriptors, batched over map points (reference src/MapPoint.cc:185-250),
+ *       and MapPoint::UpdateNormalAndDepth on the same observation lists (reference src/MapPoint.cc:273-312)
  *
  * Plain pointers and sizes; host arrays unless a parameter is named d_*.  Return values: OrbfeStatus (orbfe.h).
  */
@@ -173,6 +174,45 @@ int orbfe_distinctive_descriptors(OrbfeMatcher *m, const uint8_t *desc, const in
 int orbfe_distinctive_descriptors_device(OrbfeMatcher *m, int ngroups, const uint8_t *d_desc, const int *d_counts,
                                          int nframes, int cap, const int32_t *d_group_ptr, const int32_t *d_obs, int nobs,
                                          int32_t *d_best, uint8_t *d_mp_desc, void *stream);
+
+/* MapPoint::UpdateNormalAndDepth (MapPoint.cc:273-312) for npoints map points at once, on the observation lists of
+ * orbfe_distinctive_descriptors_device: the frame store d_kps / d_counts (frame f at f*cap, `nframes` frames), point g owns
+ * the slots d_obs[d_group_ptr[g] .. d_group_ptr[g+1]) (npoints + 1 pointers, `nobs` observations) in mObservations
+ * iteration order.  Unlike ComputeDistinctiveDescriptors the reference counts EVERY observation, those in bad keyframes
+ * included, so the same list serves both only when it has none of those.
+ *   d_centers: 3 floats per frame row, KeyFrame::GetCameraCenter() of the keyframe in that row.
+ *   d_world:   3 floats per point, MapPoint::GetWorldPos().
+ *   d_ref_obs: per point the slot of its reference keyframe's observation, slot(mpRefKF)*cap + observations[mpRefKF].  Where
+ *              mpRefKF is not among the observations the reference's map lookup reads index 0: pass slot(mpRefKF)*cap + 0.
+ *   scale_factor = KeyFrame::GetScaleFactor(), scale_factors = the nlevels floats of GetScaleFactor(l) (host arrays, shared
+ *   by the keyframes of one extractor, as sigma2 is in orbfe_search_for_triangulation_device).
+ * Outputs, per point g: d_normal[3g..3g+2] = mNormalVector, d_min_dist[g] = mfMinDistance, d_max_dist[g] = mfMaxDistance,
+ * bit for bit the values the reference computes with OpenCV 2.4 (the rule is in DESIGN.md §2: a float scaleAdd chain in list
+ * order, (float)(1.0/n) for the mean, cv::norm in double).  A point on an observer's camera centre has a NaN normal, as in
+ * the reference (its NaN payload may differ); a point on its reference centre has both distances 0.
+ * An empty group is left untouched (the reference returns early for a bad map point and keeps its values): pass a bad map
+ * point as an empty group or leave it out.  Bad input is never followed: a point with d_group_ptr[g] < 0,
+ * d_group_ptr[g] > d_group_ptr[g+1], d_group_ptr[g+1] > nobs, an observation or reference slot whose frame is >= nframes or
+ * whose feature index is >= d_counts[f], or a reference octave outside [0, nlevels), keeps its outputs untouched, and
+ * orbfe_matcher_sync then reports ORBFE_ERR_ARG; the other points of the launch are unaffected.  One warp per map point.
+ * npoints >= 0, nobs >= 0, 1 <= cap <= 65535, nframes >= 1, nframes*cap < 2^31, 1 <= nlevels <= ORBFE_MAX_LEVELS.
+ * Arguments are checked before the handle is used; npoints == 0 does nothing.  Enqueued on `stream` (NULL = the matcher's
+ * stream), not synchronised. */
+int orbfe_normal_and_depth_device(OrbfeMatcher *m, int npoints, const OrbfeKeyPoint *d_kps, const int *d_counts, int nframes, int cap,
+                                  const float *d_centers, const int32_t *d_group_ptr, const int32_t *d_obs, int nobs,
+                                  const float *d_world, const int32_t *d_ref_obs, float scale_factor, int nlevels,
+                                  const float *scale_factors, float *d_normal, float *d_min_dist, float *d_max_dist, void *stream);
+
+/* orbfe_normal_and_depth_device for callers without a frame store (e.g. the recovery loops after a bundle adjustment), all
+ * host arrays: per point g its world position world[3g..], its reference keyframe's camera centre ref_centers[3g..] and the
+ * octave of the reference keyframe's observed keypoint ref_octave[g]; the camera centres of its observers are rows
+ * group_ptr[g] .. group_ptr[g+1] of obs_centers (3 floats each, mObservations order; group_ptr[0] = 0, non-decreasing).
+ * The outputs and the rule are those of the device form; the rows of an empty group are returned as passed.  ORBFE_ERR_ARG,
+ * before the handle is used, for a bad group_ptr or a non-empty point whose ref_octave is outside [0, nlevels).  Staged
+ * through the matcher's block, one launch of the same kernel, synchronous. */
+int orbfe_normal_and_depth(OrbfeMatcher *m, int npoints, const float *world, const float *ref_centers, const int32_t *ref_octave,
+                           const int32_t *group_ptr, const float *obs_centers, float scale_factor, int nlevels, const float *scale_factors,
+                           float *normal_out, float *min_dist_out, float *max_dist_out);
 
 /* KeyFrameDatabase::DetectLoopCandidates (mode 0, KeyFrameDatabase.cc:73-195) / DetectRelocalisationCandidates (mode 1,
  * :197-308) with the database as arrays.  Keyframe k (k = 0..nkf-1, in the order the keyframes were add()ed: that is

@@ -55,7 +55,7 @@ ABI_SYMBOLS = [
     "orbfe_vocabulary_create", "orbfe_vocabulary_destroy", "orbfe_vocabulary_load_text", "orbfe_vocabulary_info",
     "orbfe_vocabulary_export", "orbfe_bow_descend_device", "orbfe_bow_descend", "orbfe_bow_transform",
     "orbfe_distinctive_descriptors", "orbfe_bow_db_detect", "orbfe_feature_vector_device", "orbfe_distinctive_descriptors_device",
-    "orbfe_bow_vector_device", "orbfe_bow_min_score_device", "orbfe_bow_score",
+    "orbfe_bow_vector_device", "orbfe_bow_min_score_device", "orbfe_bow_score", "orbfe_normal_and_depth_device", "orbfe_normal_and_depth",
     "orbfe_kfdb_create", "orbfe_kfdb_destroy", "orbfe_kfdb_add", "orbfe_kfdb_add_device", "orbfe_kfdb_erase", "orbfe_kfdb_clear", "orbfe_kfdb_set_covisibles",
     "orbfe_kfdb_size", "orbfe_kfdb_detect", "orbfe_kfdb_detect_device", "orbfe_kfdb_create_batched", "orbfe_kfdb_detect_batch_device",
 ]

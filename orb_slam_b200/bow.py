@@ -1,6 +1,7 @@
 """ctypes wrappers of include/orbfe_bow.h: the DBoW2 vocabulary-tree transform (reference
 Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1126-1262; callers Frame.cc:280-287, KeyFrame.cc:56-65) and the batched
-MapPoint::ComputeDistinctiveDescriptors (reference src/MapPoint.cc:185-250).  No CPU fallback: every call runs the
+MapPoint::ComputeDistinctiveDescriptors and MapPoint::UpdateNormalAndDepth (reference src/MapPoint.cc:185-250, 273-312).
+No CPU fallback: every call runs the
 CUDA kernels of liborbfe.so."""
 import ctypes as C
 import os
@@ -38,6 +39,9 @@ def _bind():
     L.orbfe_distinctive_descriptors_device.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp]
     L.orbfe_bow_min_score_device.argtypes = [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.orbfe_bow_score.argtypes = [vp, C.c_int, vp, vp, C.c_int, vp, vp, vp]
+    L.orbfe_normal_and_depth_device.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.c_int, vp, vp, vp, C.c_int, vp, vp, C.c_float, C.c_int, vp,
+                                                vp, vp, vp, vp]
+    L.orbfe_normal_and_depth.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, C.c_float, C.c_int, vp, vp, vp, vp]
     _bound = True
     return L
 
@@ -196,6 +200,39 @@ def distinctive_descriptors_device(matcher: ORBmatcher, ngroups, d_desc, d_count
     vp = C.c_void_p
     _check(_bind().orbfe_distinctive_descriptors_device(matcher.handle, ngroups, vp(d_desc), vp(d_counts), nframes, cap, vp(d_group_ptr),
                                                         vp(d_obs), nobs, vp(d_best), vp(d_mp_desc), vp(stream)))
+
+
+def normal_and_depth(matcher: ORBmatcher, world, ref_centers, ref_octave, group_ptr, obs_centers, scale_factor, scale_factors,
+                     normal=None, min_dist=None, max_dist=None):
+    """MapPoint::UpdateNormalAndDepth for every point (reference src/MapPoint.cc:273-312) from host arrays: world / ref_centers
+    [npoints, 3], ref_octave [npoints], observer centres obs_centers[group_ptr[g] .. group_ptr[g+1]) [.., 3].  Returns
+    (normal [npoints, 3], min_dist, max_dist) as float32; the rows of empty groups are those of `normal` / `min_dist` /
+    `max_dist` as passed (zeros when not given)."""
+    f = lambda x, n: np.ascontiguousarray(x, np.float32).reshape(n, 3)
+    group_ptr = np.ascontiguousarray(group_ptr, np.int32)
+    n = len(group_ptr) - 1
+    world, ref_centers = f(world, n), f(ref_centers, n)
+    obs_centers = f(obs_centers, -1) if len(np.asarray(obs_centers).ravel()) else np.zeros((1, 3), np.float32)
+    ref_octave = np.ascontiguousarray(ref_octave, np.int32)
+    sf = np.ascontiguousarray(scale_factors, np.float32)
+    out_n = np.zeros((max(n, 1), 3), np.float32) if normal is None else np.array(f(normal, n), copy=True)
+    out_min = np.zeros(max(n, 1), np.float32) if min_dist is None else np.array(min_dist, np.float32, copy=True)
+    out_max = np.zeros(max(n, 1), np.float32) if max_dist is None else np.array(max_dist, np.float32, copy=True)
+    _check(_bind().orbfe_normal_and_depth(matcher.handle, n, _p(world), _p(ref_centers), _p(ref_octave), _p(group_ptr), _p(obs_centers),
+                                          float(scale_factor), len(sf), _p(sf), _p(out_n), _p(out_min), _p(out_max)))
+    return out_n[:n], out_min[:n], out_max[:n]
+
+
+def normal_and_depth_device(matcher: ORBmatcher, npoints, d_kps, d_counts, nframes, cap, d_centers, d_group_ptr, d_obs, nobs, d_world,
+                            d_ref_obs, scale_factor, scale_factors, d_normal, d_min_dist, d_max_dist, stream=0):
+    """Device-pointer form (ints = raw device addresses) on the frame store and the observation lists of
+    distinctive_descriptors_device; d_centers holds 3 floats per frame row, d_ref_obs one slot per point.  Enqueued, not
+    synchronised; see include/orbfe_bow.h."""
+    vp = C.c_void_p
+    sf = np.ascontiguousarray(scale_factors, np.float32)
+    _check(_bind().orbfe_normal_and_depth_device(matcher.handle, npoints, vp(d_kps), vp(d_counts), nframes, cap, vp(d_centers),
+                                                 vp(d_group_ptr), vp(d_obs), nobs, vp(d_world), vp(d_ref_obs), float(scale_factor), len(sf),
+                                                 _p(sf), vp(d_normal), vp(d_min_dist), vp(d_max_dist), vp(stream)))
 
 
 def db_detect(matcher: ORBmatcher, mode, q_ids, q_vals, kf_ptr, db_ids, db_vals, connected, covis_ptr, covis, min_score=0.0):

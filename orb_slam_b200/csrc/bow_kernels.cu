@@ -1,6 +1,7 @@
 // bow_kernels.cu -- the two Hamming-primitive rows of SURVEY.md section 8(f):
 //   N2  DBoW2 vocabulary-tree descent (reference Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1216-1260, FORB.cpp:79-99)
 //   N4  MapPoint::ComputeDistinctiveDescriptors, batched (reference src/MapPoint.cc:185-250)
+//   and its partner MapPoint::UpdateNormalAndDepth, batched (reference src/MapPoint.cc:273-312)
 // plus the vocabulary half of the C-ABI in include/orbfe_bow.h.  The std::map builds of transform() are stated once, for
 // batches of frames in HBM (feature_vector_kernel, bow_vector_kernel); the host-array orbfe_bow_transform runs them as a
 // batch of one frame.  The descent is integer work only (XOR + POPC), bound by launch latency at SLAM sizes
@@ -137,6 +138,95 @@ __global__ void __launch_bounds__(128) distinctive_kernel(const uint4 *__restric
     }
     if (lane == 0) best_out[g] = bestIdx;
     if (kObs && lane < 2) mp_desc[2 * (size_t)g + lane] = __ldg(&desc[2 * row(bestIdx) + lane]);
+}
+
+// MapPoint::UpdateNormalAndDepth (MapPoint.cc:273-312) as the cv::Mat algebra of OpenCV 2.4 evaluates it (DESIGN §2): one
+// warp per map point.  Each lane takes one observation of a chunk of 32 and forms its term d_k * (float)(1.0 / cv::norm(d))
+// with d = P - Ow_i; the running float sum then takes the terms in lane order, every lane adding the same broadcast terms,
+// so the additions are the reference's scaleAdd loop over mObservations, each rounded once.  No FMA, explicit _rn.
+// kObs = false (orbfe_normal_and_depth): observation j of point g has camera centre row group_ptr[g] + j of `centers`, the
+// point's reference centre is row g of ref_centers and its octave ref_octave[g]; the host has checked all of it.
+// kObs = true (orbfe_normal_and_depth_device): observation j is frame-store slot obs[group_ptr[g] + j] = f*cap + i, whose
+// centre is row f of `centers`; the reference slot is ref_obs[g], its octave kps[ref_obs[g]].octave.  A point whose pointers,
+// slots or octave are out of range is never followed (outputs untouched, bit 16 of *err).  An empty group (a bad map point)
+// is left untouched in both modes.
+struct NdLevels {
+    float sf[ORBFE_MAX_LEVELS];   // KeyFrame::GetScaleFactor(l), l < nlevels
+    float scale_factor;           // KeyFrame::GetScaleFactor()
+    int nlevels;
+};
+
+template <bool kObs>
+__global__ void __launch_bounds__(128) normal_depth_kernel(const OrbfeKeyPoint *__restrict__ kps, const int *__restrict__ counts,
+                                                           int nframes, int cap, const float *__restrict__ centers,
+                                                           const int *__restrict__ group_ptr, const int *__restrict__ obs, int nobs,
+                                                           const float *__restrict__ world, const int *__restrict__ ref_obs,
+                                                           const float *__restrict__ ref_centers, const int *__restrict__ ref_octave,
+                                                           const NdLevels lv, int npoints, float *__restrict__ normal_out,
+                                                           float *__restrict__ min_out, float *__restrict__ max_out,
+                                                           int *__restrict__ err) {
+    const int lane = threadIdx.x & 31;
+    const int g = blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (g >= npoints) return;
+    const int b = __ldg(&group_ptr[g]), e = __ldg(&group_ptr[g + 1]);
+    if (kObs && (b < 0 || b > e || e > nobs)) {
+        if (lane == 0) atomicOr(err, 16);
+        return;
+    }
+    const int N = e - b;
+    if (N <= 0) return;
+    const float *oref;
+    int level;
+    if (kObs) {
+        const int r = __ldg(&ref_obs[g]);
+        bool mine = r < 0 || r / cap >= nframes || r % cap >= __ldg(&counts[r / cap]);
+        level = mine ? 0 : __ldg(&kps[r].octave);
+        mine |= level < 0 || level >= lv.nlevels;
+        for (int j = b + lane; j < e; j += 32) {
+            const int o = __ldg(&obs[j]);
+            mine |= o < 0 || o / cap >= nframes || o % cap >= __ldg(&counts[o / cap]);
+        }
+        if (__any_sync(0xffffffffu, mine)) {
+            if (lane == 0) atomicOr(err, 16);
+            return;
+        }
+        oref = centers + 3 * (size_t)(r / cap);
+    } else {
+        level = __ldg(&ref_octave[g]);
+        oref = ref_centers + 3 * (size_t)g;
+    }
+    const float px = __ldg(&world[3 * (size_t)g]), py = __ldg(&world[3 * (size_t)g + 1]), pz = __ldg(&world[3 * (size_t)g + 2]);
+    float nx = 0.0f, ny = 0.0f, nz = 0.0f;   // cv::Mat::zeros(3,1,CV_32F)
+    for (int c0 = 0; c0 < N; c0 += 32) {
+        const int j = c0 + lane;
+        float tx = 0.0f, ty = 0.0f, tz = 0.0f;
+        if (j < N) {
+            const float *ow = centers + 3 * (size_t)(kObs ? __ldg(&obs[b + j]) / cap : b + j);
+            const float dx = __fsub_rn(px, __ldg(&ow[0])), dy = __fsub_rn(py, __ldg(&ow[1])), dz = __fsub_rn(pz, __ldg(&ow[2]));
+            const double s = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn((double)dx, (double)dx), __dmul_rn((double)dy, (double)dy)),
+                                                  __dmul_rn((double)dz, (double)dz)));
+            const float a = __double2float_rn(__ddiv_rn(1.0, s));
+            tx = __fmul_rn(dx, a);
+            ty = __fmul_rn(dy, a);
+            tz = __fmul_rn(dz, a);
+        }
+        const int m = min(N - c0, 32);
+        for (int i = 0; i < m; i++) {
+            nx = __fadd_rn(nx, __shfl_sync(0xffffffffu, tx, i));
+            ny = __fadd_rn(ny, __shfl_sync(0xffffffffu, ty, i));
+            nz = __fadd_rn(nz, __shfl_sync(0xffffffffu, tz, i));
+        }
+    }
+    if (lane != 0) return;
+    const float inv_n = __double2float_rn(__ddiv_rn(1.0, (double)N));
+    normal_out[3 * (size_t)g] = __fadd_rn(__fmul_rn(nx, inv_n), 0.0f);
+    normal_out[3 * (size_t)g + 1] = __fadd_rn(__fmul_rn(ny, inv_n), 0.0f);
+    normal_out[3 * (size_t)g + 2] = __fadd_rn(__fmul_rn(nz, inv_n), 0.0f);
+    const float cx = __fsub_rn(px, __ldg(&oref[0])), cy = __fsub_rn(py, __ldg(&oref[1])), cz = __fsub_rn(pz, __ldg(&oref[2]));
+    const float dist = __double2float_rn(__dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn((double)cx, (double)cx), __dmul_rn((double)cy, (double)cy)),
+                                                              __dmul_rn((double)cz, (double)cz))));
+    min_out[g] = __fdiv_rn(__fmul_rn(__fdiv_rn(1.0f, lv.scale_factor), dist), lv.sf[level]);
+    max_out[g] = __fmul_rn(__fmul_rn(lv.scale_factor, dist), lv.sf[lv.nlevels - 1 - level]);
 }
 
 // KeyFrameDatabase scoring: one thread per keyframe, the shared L1 walk (bow_l1.cuh) over the word lists of the query and
@@ -744,5 +834,34 @@ void launch_distinctive_obs(const uint8_t *d_desc, const int *d_counts, int nfra
     distinctive_kernel<true><<<(ngroups + 3) / 4, 128, 0, s>>>(reinterpret_cast<const uint4 *>(d_desc), d_group_ptr, d_obs, nobs,
                                                                d_counts, nframes, cap, ngroups, d_best,
                                                                reinterpret_cast<uint4 *>(d_mp_desc), d_err);
+}
+
+static NdLevels nd_levels(float scale_factor, int nlevels, const float *scale_factors) {
+    NdLevels lv;
+    memset(&lv, 0, sizeof(lv));
+    for (int l = 0; l < nlevels; l++) lv.sf[l] = scale_factors[l];
+    lv.scale_factor = scale_factor;
+    lv.nlevels = nlevels;
+    return lv;
+}
+
+void launch_normal_depth_obs(const OrbfeKeyPoint *d_kps, const int *d_counts, int nframes, int cap, const float *d_centers,
+                             const int *d_group_ptr, const int *d_obs, int nobs, const float *d_world, const int *d_ref_obs,
+                             float scale_factor, int nlevels, const float *scale_factors, int npoints, float *d_normal,
+                             float *d_min_dist, float *d_max_dist, int *d_err, cudaStream_t s) {
+    if (npoints <= 0) return;
+    normal_depth_kernel<true><<<(npoints + 3) / 4, 128, 0, s>>>(d_kps, d_counts, nframes, cap, d_centers, d_group_ptr, d_obs, nobs, d_world,
+                                                                 d_ref_obs, nullptr, nullptr, nd_levels(scale_factor, nlevels, scale_factors),
+                                                                 npoints, d_normal, d_min_dist, d_max_dist, d_err);
+}
+
+void launch_normal_depth(const float *d_obs_centers, const int *d_group_ptr, const float *d_world, const float *d_ref_centers,
+                         const int *d_ref_octave, float scale_factor, int nlevels, const float *scale_factors, int npoints,
+                         float *d_normal, float *d_min_dist, float *d_max_dist, cudaStream_t s) {
+    if (npoints <= 0) return;
+    normal_depth_kernel<false><<<(npoints + 3) / 4, 128, 0, s>>>(nullptr, nullptr, 1, 1, d_obs_centers, d_group_ptr, nullptr, 0, d_world,
+                                                                  nullptr, d_ref_centers, d_ref_octave,
+                                                                  nd_levels(scale_factor, nlevels, scale_factors), npoints, d_normal,
+                                                                  d_min_dist, d_max_dist, nullptr);
 }
 }  // namespace orbfe

@@ -904,6 +904,9 @@ extern "C" int orbfe_matcher_sync(OrbfeMatcher *m) {
         if (flags & 8)
             return fail(ORBFE_ERR_ARG, "orbfe_distinctive_descriptors_device: a group's pointers or an observation's frame or "
                                        "feature index are out of range (its best index is -1)");
+        if (flags & 16)
+            return fail(ORBFE_ERR_ARG, "orbfe_normal_and_depth_device: a point's group pointers, an observation or reference slot, "
+                                       "or its reference octave are out of range (its outputs are untouched)");
         return fail(ORBFE_ERR_CAPACITY, "device matcher: a job's candidate entries exceeded its global scratch (its nmatches is -1; "
                                         "%d entries were needed)", m->h_err[1]);
     }
@@ -1438,6 +1441,79 @@ extern "C" int orbfe_distinctive_descriptors_device(OrbfeMatcher *m, int ngroups
     launch_distinctive_obs(d_desc, d_counts, nframes, cap, d_group_ptr, d_obs, nobs, ngroups, d_best, d_mp_desc, m->d_err, s);
     CU_TRY(cudaGetLastError());
     m->launches += 1;
+    return ORBFE_OK;
+}
+
+// MapPoint::UpdateNormalAndDepth for many map points in one launch, on the frame store (include/orbfe_bow.h).  Arguments
+// are checked before the handle is used.
+extern "C" int orbfe_normal_and_depth_device(OrbfeMatcher *m, int npoints, const OrbfeKeyPoint *d_kps, const int *d_counts, int nframes,
+                                             int cap, const float *d_centers, const int32_t *d_group_ptr, const int32_t *d_obs, int nobs,
+                                             const float *d_world, const int32_t *d_ref_obs, float scale_factor, int nlevels,
+                                             const float *scale_factors, float *d_normal, float *d_min_dist, float *d_max_dist,
+                                             void *stream) {
+    if (!m || npoints < 0 || nobs < 0 || cap < 1 || cap > 65535 || nframes < 1 || (long long)nframes * cap > INT32_MAX || nlevels < 1 ||
+        nlevels > ORBFE_MAX_LEVELS)
+        return fail(ORBFE_ERR_ARG, "orbfe_normal_and_depth_device: bad arguments");
+    if (npoints == 0) return ORBFE_OK;
+    if (!d_kps || !d_counts || !d_centers || !d_group_ptr || !d_obs || !d_world || !d_ref_obs || !scale_factors || !d_normal ||
+        !d_min_dist || !d_max_dist)
+        return fail(ORBFE_ERR_ARG, "orbfe_normal_and_depth_device: NULL argument");
+    CU_TRY(cudaSetDevice(m->device));
+    cudaStream_t s = stream ? (cudaStream_t)stream : m->stream;
+    launch_normal_depth_obs(d_kps, d_counts, nframes, cap, d_centers, d_group_ptr, d_obs, nobs, d_world, d_ref_obs, scale_factor, nlevels,
+                            scale_factors, npoints, d_normal, d_min_dist, d_max_dist, m->d_err, s);
+    CU_TRY(cudaGetLastError());
+    m->launches += 1;
+    return ORBFE_OK;
+}
+
+// The same for callers without a frame store: every centre given on the host, staged through the matcher's block and run
+// as one launch of the same kernel (include/orbfe_bow.h)
+extern "C" int orbfe_normal_and_depth(OrbfeMatcher *m, int npoints, const float *world, const float *ref_centers, const int32_t *ref_octave,
+                                      const int32_t *group_ptr, const float *obs_centers, float scale_factor, int nlevels,
+                                      const float *scale_factors, float *normal_out, float *min_dist_out, float *max_dist_out) {
+    if (!m || npoints < 0 || nlevels < 1 || nlevels > ORBFE_MAX_LEVELS) return fail(ORBFE_ERR_ARG, "orbfe_normal_and_depth: bad arguments");
+    if (npoints == 0) return ORBFE_OK;
+    if (!world || !ref_centers || !ref_octave || !group_ptr || !scale_factors || !normal_out || !min_dist_out || !max_dist_out)
+        return fail(ORBFE_ERR_ARG, "orbfe_normal_and_depth: NULL argument");
+    const int total = group_ptr[npoints];
+    if (group_ptr[0] != 0 || total < 0 || (total > 0 && !obs_centers)) return fail(ORBFE_ERR_ARG, "orbfe_normal_and_depth: bad group_ptr");
+    for (int g = 0; g < npoints; g++) {
+        if (group_ptr[g + 1] < group_ptr[g]) return fail(ORBFE_ERR_ARG, "orbfe_normal_and_depth: group_ptr must be non-decreasing");
+        if (group_ptr[g + 1] > group_ptr[g] && (ref_octave[g] < 0 || ref_octave[g] >= nlevels))
+            return fail(ORBFE_ERR_ARG, "orbfe_normal_and_depth: point %d has reference octave %d outside [0, %d)", g, ref_octave[g], nlevels);
+    }
+    CU_TRY(cudaSetDevice(m->device));
+    const size_t NP = (size_t)npoints, b3 = 3 * sizeof(float) * NP, b1 = sizeof(float) * NP;
+    size_t o_world, o_ref, o_oct, o_ptr, o_obs, o_normal, o_min, o_max, nbytes;
+    if (int rc = m->stage.layout({{&o_world, b3}, {&o_ref, b3}, {&o_oct, sizeof(int) * NP}, {&o_ptr, sizeof(int) * (NP + 1)},
+                                  {&o_obs, 3 * sizeof(float) * (size_t)total}, {&o_normal, b3}, {&o_min, b1}, {&o_max, b1}},
+                                 &nbytes))
+        return rc;
+    unsigned char *H = m->stage.h, *D = m->stage.d;
+    memcpy(H + o_world, world, b3);
+    memcpy(H + o_ref, ref_centers, b3);
+    memcpy(H + o_oct, ref_octave, sizeof(int) * NP);
+    memcpy(H + o_ptr, group_ptr, sizeof(int) * (NP + 1));
+    if (total > 0) memcpy(H + o_obs, obs_centers, 3 * sizeof(float) * (size_t)total);
+    // the outputs go up too: the rows of empty groups come back as the caller passed them
+    memcpy(H + o_normal, normal_out, b3);
+    memcpy(H + o_min, min_dist_out, b1);
+    memcpy(H + o_max, max_dist_out, b1);
+    cudaStream_t s = m->stream;
+    CU_TRY(cudaMemcpyAsync(D, H, nbytes, cudaMemcpyHostToDevice, s));
+    launch_normal_depth((const float *)(D + o_obs), (const int *)(D + o_ptr), (const float *)(D + o_world), (const float *)(D + o_ref),
+                        (const int *)(D + o_oct), scale_factor, nlevels, scale_factors, npoints, (float *)(D + o_normal),
+                        (float *)(D + o_min), (float *)(D + o_max), s);
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaMemcpyAsync(H + o_normal, D + o_normal, nbytes - o_normal, cudaMemcpyDeviceToHost, s));
+    CU_TRY(cudaStreamSynchronize(s));
+    m->h2d_bytes += nbytes;
+    m->d2h_bytes += nbytes - o_normal;
+    m->launches += 1;
+    memcpy(normal_out, H + o_normal, b3);
+    memcpy(min_dist_out, H + o_min, b1);
+    memcpy(max_dist_out, H + o_max, b1);
     return ORBFE_OK;
 }
 

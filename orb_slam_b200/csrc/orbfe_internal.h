@@ -228,6 +228,16 @@ void launch_distinctive(const uint8_t *d_desc, const int *d_group_ptr, int ngrou
 // an out-of-range group pointer or observation sets bit 8 of *d_err
 void launch_distinctive_obs(const uint8_t *d_desc, const int *d_counts, int nframes, int cap, const int *d_group_ptr,
                             const int *d_obs, int nobs, int ngroups, int *d_best, uint8_t *d_mp_desc, int *d_err, cudaStream_t s);
+// MapPoint::UpdateNormalAndDepth on the frame store; an out-of-range group pointer, slot or reference octave sets bit 16 of
+// *d_err.  scale_factors: nlevels floats on the host.
+void launch_normal_depth_obs(const OrbfeKeyPoint *d_kps, const int *d_counts, int nframes, int cap, const float *d_centers,
+                             const int *d_group_ptr, const int *d_obs, int nobs, const float *d_world, const int *d_ref_obs,
+                             float scale_factor, int nlevels, const float *scale_factors, int npoints, float *d_normal,
+                             float *d_min_dist, float *d_max_dist, int *d_err, cudaStream_t s);
+// the same on host-checked contiguous rows: observation centres by group, one reference centre and octave per point
+void launch_normal_depth(const float *d_obs_centers, const int *d_group_ptr, const float *d_world, const float *d_ref_centers,
+                         const int *d_ref_octave, float scale_factor, int nlevels, const float *scale_factors, int npoints,
+                         float *d_normal, float *d_min_dist, float *d_max_dist, cudaStream_t s);
 void launch_bow_db_score(int nq, const int *q_ids, const double *q_vals, int nkf, const int *kf_ptr, const int *db_ids,
                          const double *db_vals, int *common, int *first, double *score, cudaStream_t s);
 

@@ -44,6 +44,11 @@
                    weighted 0, words with 6 significant digits like Data/ORBvoc.txt) and on the same tree with %r weights (the
                    host-conversion path): wall time per load (file read included), device time per kernel and copy
                    (torch.profiler, a run of its own), and the reference's loadFromTextFile from oracle/_ref in the same process.
+  --what normaldepth MapPoint::UpdateNormalAndDepth after LocalBundleAdjustment (Optimizer.cc:488): every local map point of
+                   20 local keyframes of 2000 features (10000 points, 2-60 observations, over a 60-keyframe store) after
+                   SetWorldPos, in one batch: CUDA-event ms of orbfe_normal_and_depth_device, the wall time of
+                   orbfe_normal_and_depth including the host gather of the centres and its staging, and the wall time of the
+                   oracle's C loop on the same arrays (plain float / double C, not OpenCV's cv::Mat), outputs compared.
 Prints one JSON object per --what; never a bench value when run under ncu."""
 import argparse
 import ctypes as C
@@ -1466,6 +1471,91 @@ def vocload(args):
     return out
 
 
+def normaldepth(args):
+    """MapPoint::UpdateNormalAndDepth at the end of LocalBundleAdjustment (Optimizer.cc:488): after the optimisation every
+    local map point gets SetWorldPos and then UpdateNormalAndDepth.  The local map: 20 keyframes of 2000 features whose every
+    feature is a map point, 10000 points, each observed by 2-60 keyframes of a 60-keyframe store (95 % in 2-12, in keyframe
+    order), world positions 2-40 units in front of their reference keyframe.  CUDA-event ms of orbfe_normal_and_depth_device
+    on the frame store, the wall time of orbfe_normal_and_depth including the host gather of every observer's centre, and
+    the wall time of the oracle's C loop (oracle/orb_oracle_normal_depth.c: plain C, not OpenCV) on the same host arrays."""
+    import torch
+    import orb_slam_b200 as fe
+    from orb_slam_b200 import bow as BW
+    from oracle import normal_depth as ND
+    NKF, NF, NP = 60, 2000, 10000
+    rng = np.random.default_rng(17)
+    counts = np.full(NKF, NF, np.int32)
+    octs = rng.integers(0, 8, NKF * NF).astype(np.int32)
+    kps = np.zeros(NKF * NF, fe.KP_DTYPE)
+    kps["octave"] = octs
+    centers = (rng.standard_normal((NKF, 3)) * 3).astype(np.float32)
+    n_obs = np.where(rng.random(NP) < 0.95, rng.integers(2, 13, NP), rng.integers(13, 61, NP))
+    groups, ref = [], np.zeros(NP, np.int32)
+    for p in range(NP):
+        frames = np.sort(rng.choice(NKF, int(n_obs[p]), replace=False))
+        g = frames * NF + rng.integers(0, NF, len(frames))
+        groups.append(g.astype(np.int32))
+        ref[p] = g[rng.integers(0, len(g))]
+    gp = np.concatenate([[0], np.cumsum([len(g) for g in groups])]).astype(np.int32)
+    obs = np.concatenate(groups).astype(np.int32)
+    d = rng.standard_normal((NP, 3))
+    world = (centers[ref // NF] + d / np.linalg.norm(d, axis=1, keepdims=True) * rng.uniform(2, 40, (NP, 1))).astype(np.float32)
+    t = [np.float32(1.0)]                      # Frame.cc:90-103: the float chain of the extractor's scale factor
+    for _ in range(7):
+        t.append(np.float32(t[-1] * np.float32(1.2)))
+    sfs = np.array(t, np.float32)
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    s = stream.cuda_stream
+    tt = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    d_kps, d_cnt, d_c, d_gp, d_obs, d_ref, d_w = tt(kps.view(np.uint8)), tt(counts), tt(centers), tt(gp), tt(obs), tt(ref), tt(world)
+    d_n = torch.zeros((NP, 3), dtype=torch.float32, device=dev)
+    d_a, d_b = torch.zeros(NP, dtype=torch.float32, device=dev), torch.zeros(NP, dtype=torch.float32, device=dev)
+    m = fe.ORBmatcher(0.6, True)
+    call = lambda: BW.normal_and_depth_device(m, NP, d_kps.data_ptr(), d_cnt.data_ptr(), NKF, NF, d_c.data_ptr(), d_gp.data_ptr(),
+                                              d_obs.data_ptr(), len(obs), d_w.data_ptr(), d_ref.data_ptr(), 1.2, sfs, d_n.data_ptr(),
+                                              d_a.data_ptr(), d_b.data_ptr(), s)
+    out = {"what": "UpdateNormalAndDepth after a local BA: %d map points, %d observations (max %d per point) over a %d-keyframe store "
+                   "of %d features" % (NP, len(obs), int(n_obs.max()), NKF, NF)}
+    for _ in range(max(args.warmup, 3)):
+        call()
+    stream.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    iters = args.iters * 20
+    times = []
+    for _ in range(5):
+        e0.record(stream)
+        for _ in range(iters):
+            call()
+        e1.record(stream)
+        stream.synchronize()
+        times.append(e0.elapsed_time(e1) / iters)
+    m.sync()
+    out["device_ms"] = float(np.median(times))
+    out["device_ms_min_max"] = [float(min(times)), float(max(times))]
+    got = (d_n.cpu().numpy(), d_a.cpu().numpy(), d_b.cpu().numpy())
+    lat, host, orc = [], None, []
+    for _ in range(7):
+        t0 = time.perf_counter()
+        host = BW.normal_and_depth(m, world, centers[ref // NF], octs[ref], gp, centers[obs // NF], 1.2, sfs)
+        lat.append((time.perf_counter() - t0) * 1e3)
+    out["host_entry_with_gather_wall_ms"] = float(np.median(lat))
+    want = None
+    rc, ro, oc = centers[ref // NF], octs[ref], centers[obs // NF]
+    for _ in range(3):
+        t0 = time.perf_counter()
+        want = ND.normal_depth(world, rc, ro, gp, oc, 1.2, sfs)
+        orc.append((time.perf_counter() - t0) * 1e3)
+    out["oracle_c_loop_wall_ms_not_opencv"] = float(np.median(orc))
+    same = lambda x, y: all(np.array_equal(np.isnan(a), np.isnan(b)) and np.array_equal(np.nan_to_num(a), np.nan_to_num(b))
+                            for a, b in zip(x, y))
+    out["same_as_host"] = bool(same(got, host))
+    out["same_as_oracle"] = bool(same(got, want))
+    _gpu_and_power_limit(out)
+    m.close()
+    return out
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--what", default="config3,config5")
@@ -1478,4 +1568,5 @@ if __name__ == "__main__":
     for w in args.what.split(","):
         print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fast": fast, "latency": latency,
                           "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb, "kfdbbatch": kfdbbatch, "bowchain": bowchain,
-                          "windowed": windowed, "guided": guided, "loopscore": loopscore, "vocload": vocload}[w](args)))
+                          "windowed": windowed, "guided": guided, "loopscore": loopscore, "vocload": vocload,
+                          "normaldepth": normaldepth}[w](args)))
