@@ -8,7 +8,8 @@
  *   N3  KeyFrameDatabase::DetectLoopCandidates / DetectRelocalisationCandidates on arrays
  *       (reference src/KeyFrameDatabase.cc:73-308, L1Scoring::score Thirdparty/DBoW2/DBoW2/ScoringObject.cpp:23-67)
  *   N4  MapPoint::ComputeDistinctiveDescriptors, batched over map points (reference src/MapPoint.cc:185-250),
- *       and MapPoint::UpdateNormalAndDepth on the same observation lists (reference src/MapPoint.cc:273-312)
+ *       and MapPoint::UpdateNormalAndDepth on the same observation lists (reference src/MapPoint.cc:273-312),
+ *       and the covisibility graph KeyFrame::UpdateConnections builds from them (reference src/KeyFrame.cc:126-185, 332-421)
  *
  * Plain pointers and sizes; host arrays unless a parameter is named d_*.  Return values: OrbfeStatus (orbfe.h).
  */
@@ -279,6 +280,14 @@ int orbfe_kfdb_clear(OrbfeKeyFrameDB *db);
  * the new keyframe and its neighbours after KeyFrame::UpdateConnections.  An entry that names an empty slot contributes
  * nothing (an empty slot is never touched by a query).  Synchronous. */
 int orbfe_kfdb_set_covisibles(OrbfeKeyFrameDB *db, int n, const int32_t *slots, const int32_t *ptr, const int32_t *lists);
+/* orbfe_kfdb_set_covisibles with the lists read where orbfe_covis_lists_device (which = 0) wrote them: slot slots[i] (a host
+ * array, checked as in the host form) gets the first 10 entries of d_lists[d_ptr[i] .. d_ptr[i+1]), so a whole export with
+ * any nbest passes as it is.  A negative entry, or one >= max_keyframes, keeps its place among the 10 and contributes
+ * nothing: it is the reference's bad keyframe, still in the list but never touched by a query.  A row whose range is
+ * negative is empty.  Enqueued on `stream` (NULL = the handle's stream), ordered after the handle's previous work, not
+ * synchronised; one launch. */
+int orbfe_kfdb_set_covisibles_device(OrbfeKeyFrameDB *db, int n, const int32_t *slots, const int32_t *d_ptr, const int32_t *d_lists,
+                                     void *stream);
 /* Number of occupied slots and of postings held (either pointer may be NULL). */
 int orbfe_kfdb_size(OrbfeKeyFrameDB *db, int *nkeyframes, long long *npostings);
 
@@ -327,6 +336,76 @@ int orbfe_kfdb_detect_device(OrbfeKeyFrameDB *db, int mode, int nq, const int32_
 int orbfe_kfdb_detect_batch_device(OrbfeKeyFrameDB *db, int mode, int nqueries, int qcap, const int32_t *d_q_ids, const double *d_q_vals,
                                    const int32_t *d_conn_ptr, const int32_t *d_connected, const float *d_min_score, int cap,
                                    int32_t *d_cand, int *d_ncand, int32_t *d_words, float *d_score, void *stream);
+
+/* The covisibility graph of one map (KeyFrame::UpdateConnections, AddConnection, UpdateBestCovisibles, EraseConnection and
+ * the connection half of SetBadFlag; reference src/KeyFrame.cc:126-185, 332-421, 497-521, 596-610) resident in device
+ * memory, so the loop and relocalisation queries read their covisibility lists without host lists.
+ *   A keyframe is a slot 0 <= slot < max_keyframes equal to its frame-store row: the slot convention of orbfe_kfdb_* and
+ *   orbfe_bow_min_score_device, so exported lists go straight into those calls.
+ *   Each slot carries a caller-given 64-bit order key, (uintptr_t)pKF in an integration: every std::map iteration and every
+ *   tie of the reference (pointer order) is taken in key order.
+ * Arguments are checked before the handle is used.  One call at a time per handle; every call is ordered after the
+ * handle's previous work whatever stream that was enqueued on. */
+typedef struct OrbfeCovisGraph OrbfeCovisGraph;
+
+/* Every buffer is allocated here; no later call allocates.  max_connections: the capacity of one keyframe's weight map,
+ * 1 .. 2048; max_batch: the most keyframes per update call, 1 .. 1024; 1 <= max_keyframes <= 2^24 and
+ * max_keyframes * max_connections < 2^31.  About 16 * max_connections + 60 bytes of device memory per slot and
+ * 24 * max_connections per batch entry. */
+int orbfe_covis_create(int device, int max_keyframes, int max_connections, int max_batch, OrbfeCovisGraph **out);
+void orbfe_covis_destroy(OrbfeCovisGraph *g);
+
+/* n new keyframes (host arrays): slot slots[i], mnId ids[i] (only ids[i] == 0 matters: such a keyframe gets no parent and
+ * is never erased) and order key keys[i].  Each starts as a fresh KeyFrame: no weights, empty lists, mbFirstConnection.
+ * All or nothing, ORBFE_ERR_ARG: a slot out of range, live or listed twice, a key equal to a live slot's key or repeated,
+ * or a retired slot that some weight map still names (re-adding it would alias the reference's stale pointer).
+ * Synchronous. */
+int orbfe_covis_add(OrbfeCovisGraph *g, int n, const int32_t *slots, const int32_t *ids, const uint64_t *keys);
+
+/* UpdateConnections() of the keyframes slots[0..n) (a host array of distinct live slots, 1 <= n <= max_batch; n = 0 does
+ * nothing): the graph afterwards equals n consecutive reference calls in that order, bit for bit.
+ *   d_kf_mp[s*cap + i] (i < d_counts[s]) is the map-point index at feature i of keyframe s: -1 (any negative) where
+ *   mvpMapPoints[i] is NULL or isBad().  A point at two features counts twice, as in the reference.
+ *   Point g's observations are d_obs[d_group_ptr[g] .. d_group_ptr[g+1]): the flat slots f*cap + i of
+ *   orbfe_normal_and_depth_device (every observation counts; the frame f is the observing keyframe's slot).
+ *   parent_out (device, n entries, may be NULL): parent_out[i] = the slot call i made mpParent (its first non-empty call,
+ *   mnId != 0: the front of its ordered list), else -1.
+ * Bad input rejects the whole batch and leaves the graph unchanged: d_counts[s] outside 0 .. cap, a point index >= npoints,
+ * a group with d_group_ptr[g] < 0, d_group_ptr[g] > d_group_ptr[g+1] or d_group_ptr[g+1] > nobs, or an observation whose
+ * frame is >= nframes or not a live slot; orbfe_covis_sync then reports ORBFE_ERR_ARG.  A weight map that would exceed
+ * max_connections also rejects the whole batch unchanged; orbfe_covis_sync then reports ORBFE_ERR_CAPACITY.  Both are
+ * decided on the device.  Host-side ORBFE_ERR_ARG: a slot not live, >= nframes or repeated, nframes < 1, cap < 1,
+ * nframes*cap >= 2^31, npoints < 0, nobs < 0, a NULL array.
+ * Enqueued on `stream` (NULL = the handle's stream), not synchronised: three launches, no host round trip.
+ * A batch is n reference calls with nothing read in between: LoopClosing.cc:484-490's loop and the initial map's pair
+ * (Tracking.cc:430-431).  Where the reference reads the graph between calls (CorrectLoop's second loop, :521-536), run
+ * batches of one. */
+int orbfe_covis_update_connections_device(OrbfeCovisGraph *g, int n, const int32_t *slots, const int32_t *d_kf_mp, const int *d_counts,
+                                          int nframes, int cap, const int32_t *d_group_ptr, const int32_t *d_obs, int npoints, int nobs,
+                                          int32_t *parent_out, void *stream);
+
+/* SetBadFlag's connection half (KeyFrame.cc:497-521): every keyframe in the slot's own weight map gets EraseConnection
+ * (:596-610: the entry erased, then all its weights re-sorted); the slot's weights and lists are cleared and the slot is
+ * retired.  mnId == 0, or a slot that is not live, does nothing.  A weight map naming the slot that the slot's own map
+ * does not name keeps its stale entry, as in the reference.  The spanning tree is not kept here.  Synchronous. */
+int orbfe_covis_erase(OrbfeCovisGraph *g, int slot);
+/* Every slot becomes empty (Tracking's reset).  Synchronous. */
+int orbfe_covis_clear(OrbfeCovisGraph *g);
+
+/* CSR lists of the n host-named slots (0 <= slots[i] < max_keyframes, repeats allowed):
+ *   which = 0: GetBestCovisibilityKeyFrames(nbest), or the whole GetVectorCovisibleKeyFrames() when nbest <= 0, with
+ *              mvOrderedWeights;
+ *   which = 1: GetConnectedKeyFrames() in key order, with the weights of mConnectedKeyFrameWeights (nbest unused).
+ * d_ptr (n + 1 entries) is an exclusive scan computed on the device; d_list and d_weights (may be NULL) hold up to
+ * n x the row limit entries, the limit being min(nbest, max_connections) for which = 0 with nbest > 0, else
+ * max_connections.  A retired slot in a list is written as -1 (the isBad -> negative convention of
+ * orbfe_bow_min_score_device; orbfe_kfdb_detect_* ignore entries outside [0, max_keyframes)).  Enqueued on `stream` (NULL
+ * = the handle's stream), not synchronised; two launches. */
+int orbfe_covis_lists_device(OrbfeCovisGraph *g, int which, int n, const int32_t *slots, int nbest, int32_t *d_ptr, int32_t *d_list,
+                             int32_t *d_weights, void *stream);
+
+/* Waits for the handle's work and returns the first device-side error since the last sync (ORBFE_OK when none). */
+int orbfe_covis_sync(OrbfeCovisGraph *g);
 
 #ifdef __cplusplus
 }

@@ -58,6 +58,8 @@ ABI_SYMBOLS = [
     "orbfe_bow_vector_device", "orbfe_bow_min_score_device", "orbfe_bow_score", "orbfe_normal_and_depth_device", "orbfe_normal_and_depth",
     "orbfe_kfdb_create", "orbfe_kfdb_destroy", "orbfe_kfdb_add", "orbfe_kfdb_add_device", "orbfe_kfdb_erase", "orbfe_kfdb_clear", "orbfe_kfdb_set_covisibles",
     "orbfe_kfdb_size", "orbfe_kfdb_detect", "orbfe_kfdb_detect_device", "orbfe_kfdb_create_batched", "orbfe_kfdb_detect_batch_device",
+    "orbfe_kfdb_set_covisibles_device", "orbfe_covis_create", "orbfe_covis_destroy", "orbfe_covis_add",
+    "orbfe_covis_update_connections_device", "orbfe_covis_erase", "orbfe_covis_clear", "orbfe_covis_lists_device", "orbfe_covis_sync",
 ]
 
 

@@ -272,6 +272,16 @@ def _bind_kfdb():
     L.orbfe_kfdb_detect_device.argtypes = [vp, i, i, vp, vp, i, vp, C.c_float, i, vp, vp, vp, vp, vp]
     L.orbfe_kfdb_create_batched.argtypes = [vp, i, C.c_longlong, i, C.POINTER(vp)]
     L.orbfe_kfdb_detect_batch_device.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp, i, vp, vp, vp, vp, vp]
+    L.orbfe_kfdb_set_covisibles_device.argtypes = [vp, i, vp, vp, vp, vp]
+    L.orbfe_covis_create.argtypes = [i, i, i, i, C.POINTER(vp)]
+    L.orbfe_covis_destroy.argtypes = [vp]
+    L.orbfe_covis_destroy.restype = None
+    L.orbfe_covis_add.argtypes = [vp, i, vp, vp, vp]
+    L.orbfe_covis_update_connections_device.argtypes = [vp, i, vp, vp, vp, i, i, vp, vp, i, i, vp, vp]
+    L.orbfe_covis_erase.argtypes = [vp, i]
+    L.orbfe_covis_clear.argtypes = [vp]
+    L.orbfe_covis_lists_device.argtypes = [vp, i, i, vp, i, vp, vp, vp, vp]
+    L.orbfe_covis_sync.argtypes = [vp]
     _kfdb_bound = True
     return L
 
@@ -335,6 +345,15 @@ class KeyFrameDatabase:
         flat = np.array(flat if flat else [0], np.int32)
         _check(_bind_kfdb().orbfe_kfdb_set_covisibles(self._h, len(slots), _p(slots), _p(ptr), _p(flat)))
 
+    def set_covisibles_device(self, slots, d_ptr, d_lists, stream=0):
+        """set_covisibles() with the lists read on the device (ints = raw device addresses): slot slots[i] gets the first 10
+        entries of d_lists[d_ptr[i]:d_ptr[i+1]], a CovisibilityGraph.lists_device(0, ...) export as it is; negative entries
+        keep their place and contribute nothing.  Enqueued, not synchronised."""
+        slots = np.ascontiguousarray(slots, np.int32)
+        vp = C.c_void_p
+        _check(_bind_kfdb().orbfe_kfdb_set_covisibles_device(self._h, len(slots), _p(slots), vp(d_ptr or None), vp(d_lists or None),
+                                                             vp(stream)))
+
     def size(self):
         n, p = C.c_int(0), C.c_longlong(0)
         _check(_bind_kfdb().orbfe_kfdb_size(self._h, C.byref(n), C.byref(p)))
@@ -370,3 +389,67 @@ class KeyFrameDatabase:
                                                            vp(d_conn_ptr or None), vp(d_connected or None), vp(d_min_score or None), cap,
                                                            vp(d_cand or None), vp(d_ncand or None), vp(d_words or None), vp(d_score or None),
                                                            vp(stream)))
+
+
+class CovisibilityGraph:
+    """The covisibility graph of one map resident on `device` (include/orbfe_bow.h, orbfe_covis_*): KeyFrame::UpdateConnections
+    for batches of keyframes, the connection half of SetBadFlag, and CSR exports of the lists the loop and relocalisation
+    queries read.  A keyframe is a slot (its frame-store row) with a 64-bit order key standing for its KeyFrame*."""
+
+    BEST, CONNECTED = 0, 1
+
+    def __init__(self, max_keyframes, max_connections, max_batch=64, device=0):
+        L = _bind_kfdb()
+        h = C.c_void_p()
+        _check(L.orbfe_covis_create(int(device), int(max_keyframes), int(max_connections), int(max_batch), C.byref(h)))
+        self._h, self.max_keyframes, self.max_connections, self.max_batch = h.value, int(max_keyframes), int(max_connections), int(max_batch)
+
+    @property
+    def handle(self):
+        return self._h
+
+    def close(self):
+        if self._h:
+            lib().orbfe_covis_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def add(self, slots, ids, keys):
+        """new keyframes: slot slots[i], mnId ids[i], order key keys[i]; all or nothing, synchronous"""
+        slots, ids = np.ascontiguousarray(slots, np.int32), np.ascontiguousarray(ids, np.int32)
+        keys = np.ascontiguousarray(keys, np.uint64)
+        if not len(slots) == len(ids) == len(keys):
+            raise ValueError("slots, ids and keys differ in length")
+        _check(_bind_kfdb().orbfe_covis_add(self._h, len(slots), _p(slots), _p(ids), _p(keys)))
+
+    def update_connections_device(self, slots, d_kf_mp, d_counts, nframes, cap, d_group_ptr, d_obs, npoints, nobs, d_parent=0, stream=0):
+        """UpdateConnections of slots[0..n) in order (ints = raw device addresses); enqueued, not synchronised.  Bad input or
+        an overflowing weight map rejects the batch unchanged and sync() raises."""
+        slots = np.ascontiguousarray(slots, np.int32)
+        vp = C.c_void_p
+        _check(_bind_kfdb().orbfe_covis_update_connections_device(self._h, len(slots), _p(slots), vp(d_kf_mp or None), vp(d_counts or None),
+                                                                  int(nframes), int(cap), vp(d_group_ptr or None), vp(d_obs or None),
+                                                                  int(npoints), int(nobs), vp(d_parent or None), vp(stream)))
+
+    def erase(self, slot):
+        _check(_bind_kfdb().orbfe_covis_erase(self._h, int(slot)))
+
+    def clear(self):
+        _check(_bind_kfdb().orbfe_covis_clear(self._h))
+
+    def lists_device(self, which, slots, nbest, d_ptr, d_list, d_weights=0, stream=0):
+        """CSR lists of `slots` (which 0: best covisibles / the ordered list when nbest <= 0; 1: connected keyframes in key
+        order) into d_ptr (n+1) / d_list / d_weights; retired keyframes are written as -1.  Enqueued, not synchronised."""
+        slots = np.ascontiguousarray(slots, np.int32)
+        vp = C.c_void_p
+        _check(_bind_kfdb().orbfe_covis_lists_device(self._h, int(which), len(slots), _p(slots), int(nbest), vp(d_ptr or None),
+                                                     vp(d_list or None), vp(d_weights or None), vp(stream)))
+
+    def sync(self):
+        """waits for the handle's work; raises on the first device-side error since the last sync"""
+        _check(_bind_kfdb().orbfe_covis_sync(self._h))

@@ -1,0 +1,751 @@
+// covis.cu -- the covisibility graph of one map (reference src/KeyFrame.cc:126-185, 332-421, 497-521, 596-610) resident in
+// device memory: KeyFrame::UpdateConnections for batches of keyframes, the connection half of SetBadFlag, and the lists
+// the loop and relocalisation queries read.  C-ABI in include/orbfe_bow.h (orbfe_covis_*).
+//
+// Layout (all allocated by orbfe_covis_create), per slot s:
+//   key[s]                 the caller's order key: it stands for the KeyFrame* every std::map of the reference is ordered by
+//   state[s]               live, mnId == 0, mbFirstConnection
+//   wn / wslot / ww        mConnectedKeyFrameWeights as rows of max_connections (slot, weight), key ascending
+//   on / oslot / ow        mvpOrderedConnectedKeyFrames / mvOrderedWeights, (weight, key) descending
+//   named[s]               how many weight maps hold s as a key (a retired slot may be re-added only when this is 0)
+// Batch scratch: the counter and filtered list of every entry (rows of max_connections), and per slot the batch position,
+// a touched mark and the AddConnection events bucketed by target.  pos / tmark / evcnt / efill are -1 / 0 between batches:
+// the apply kernel restores them for every slot the batch touched.
+//
+// A batch of n UpdateConnections calls is three launches, no host round trip:
+//   covis_count_kernel  one block per entry: KFcounter in a shared-memory open-addressed table keyed by slot (the entry's
+//                       own slot skipped), sorted by key; the first strict maximum in key order; the filtered ordered list
+//                       (weights >= 15, else the maximum alone) sorted by (weight, key) descending.  Its entries are the
+//                       entry's AddConnection(target, entry, weight) events.  Bad input or an overflowing counter flags the
+//                       batch.
+//   covis_plan_kernel   one block: marks the touched slots (entries and event targets), buckets the events by target and
+//                       computes every touched weight map's final size; a flag or an oversized map rejects the batch.
+//   covis_apply_kernel  one block per touched slot writes its final state in closed form (DESIGN.md §4.6): the start map is
+//                       the slot's own counter (when it had a non-empty call) or its old map, the events of later entries
+//                       (all events without an own call) are applied to it; the ordered list is the full sort when one of
+//                       those events changed a weight, else the own call's filtered list, else unchanged.  One call's
+//                       counter reads only the observations, which a batch does not change, and an entry sends at most one
+//                       event to each target, so the result does not depend on scheduling.
+#include <algorithm>
+#include <climits>
+#include <unordered_set>
+#include <vector>
+
+#include "../../include/orbfe_bow.h"
+#include "orbfe_internal.h"
+
+namespace orbfe {
+int set_error(int code, const char *fmt, ...);
+
+#define COVIS_TH 15              // KeyFrame.cc:372
+#define COVIS_MAX_CONN 2048      // the count and apply blocks hold a weight map in shared memory
+#define COVIS_MAX_BATCH 1024
+#define COVIS_COUNT_BLOCK 512
+#define COVIS_APPLY_BLOCK 256
+enum { ST_LIVE = 1, ST_ID0 = 2, ST_FIRST = 4 };
+// flags: [0] bad input in this batch, [1] overflow in this batch, [2] batch accepted, [3] first error since the last sync,
+//        [4] touched slots of this batch
+enum { F_BAD = 0, F_OVER = 1, F_OK = 2, F_ERR = 3, F_NT = 4, F_COUNT = 8 };
+
+struct CvEnt {
+    unsigned long long k;
+    int s, w;
+};
+
+static __host__ __device__ int pow2ge(int n) {
+    int p = 1;
+    while (p < n) p <<= 1;
+    return p;
+}
+
+// bitonic sort of n2 (a power of two) entries by the whole block: ByWeight = (weight, key) descending, else key ascending
+template <bool ByWeight>
+__device__ __forceinline__ bool cv_before(const CvEnt &a, const CvEnt &b) {
+    if (ByWeight) return a.w > b.w || (a.w == b.w && a.k > b.k);
+    return a.k < b.k;
+}
+template <bool ByWeight>
+__device__ void cv_sort(CvEnt *e, int n2) {
+    for (int k = 2; k <= n2; k <<= 1)
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            for (int i = threadIdx.x; i < n2; i += blockDim.x) {
+                const int l = i ^ j;
+                if (l > i) {
+                    const CvEnt a = e[i], b = e[l];
+                    if ((i & k) == 0 ? cv_before<ByWeight>(b, a) : cv_before<ByWeight>(a, b)) { e[i] = b; e[l] = a; }
+                }
+            }
+            __syncthreads();
+        }
+}
+// padding that sorts last in either order
+__device__ __forceinline__ CvEnt cv_pad(bool by_weight) { return by_weight ? CvEnt{0ull, -1, INT_MIN} : CvEnt{~0ull, -1, 0}; }
+
+// index of `k` in the key-ascending slot row, or -1
+__device__ __forceinline__ int cv_find(const int *row, int n, const unsigned long long *key, unsigned long long k) {
+    int lo = 0, hi = n;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (key[row[mid]] < k) lo = mid + 1; else hi = mid;
+    }
+    return lo < n && key[row[lo]] == k ? lo : -1;
+}
+
+// exclusive scan of one value per thread over a block of 1024; returns the prefix and adds the block total to *carry
+__device__ int cv_block_scan(int v, int *s_warp, int *carry) {
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    int x = v;
+    for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) s_warp[wid] = x;
+    __syncthreads();
+    if (wid == 0) {
+        int w = s_warp[lane];
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, w, o);
+            if (lane >= o) w += y;
+        }
+        s_warp[lane] = w;
+    }
+    __syncthreads();
+    const int base = *carry;
+    const int r = base + (wid > 0 ? s_warp[wid - 1] : 0) + x - v;
+    __syncthreads();
+    if (threadIdx.x == 0) *carry = base + s_warp[31];
+    __syncthreads();
+    return r;
+}
+
+// ---- UpdateConnections, launch 1: one block per batch entry
+__global__ void __launch_bounds__(COVIS_COUNT_BLOCK) covis_count_kernel(
+    const int *__restrict__ slots, int C, int Cp, int P, const int *__restrict__ kf_mp, const int *__restrict__ counts, int nframes,
+    int cap, const int *__restrict__ gp, const int *__restrict__ obs, int npoints, int nobs, int K, const int *__restrict__ state,
+    const unsigned long long *__restrict__ key, int *__restrict__ cn, int *__restrict__ cslot, int *__restrict__ cw, int *__restrict__ fn,
+    int *__restrict__ fslot, int *__restrict__ fw, int *__restrict__ flags) {
+    extern __shared__ unsigned long long cv_smem[];
+    CvEnt *buf = reinterpret_cast<CvEnt *>(cv_smem);   // Cp entries: the counter, key ascending
+    int *tkey = reinterpret_cast<int *>(buf + Cp);       // P slots, then P counts; reused as Cp entries of the filtered list
+    int *tcnt = tkey + P;
+    CvEnt *flt = reinterpret_cast<CvEnt *>(tkey);
+    __shared__ int s_bad, s_full, s_n, s_c, s_nmax, s_imax, s_nth, s_f;
+    const int p = blockIdx.x, s = slots[p];
+    for (int i = threadIdx.x; i < P; i += blockDim.x) { tkey[i] = -1; tcnt[i] = 0; }
+    if (threadIdx.x == 0) { s_bad = 0; s_full = 0; s_n = 0; s_c = 0; s_nmax = 0; s_imax = INT_MAX; s_nth = 0; s_f = 0; }
+    __syncthreads();
+    const int nf = counts[s];
+    if (nf < 0 || nf > cap) {
+        if (threadIdx.x == 0) s_bad = 1;
+    } else {
+        for (int i = threadIdx.x; i < nf; i += blockDim.x) {
+            const int mp = kf_mp[(size_t)s * cap + i];
+            if (mp < 0) continue;   // NULL or isBad()
+            if (mp >= npoints) { s_bad = 1; break; }
+            const int lo = gp[mp], hi = gp[mp + 1];
+            if (lo < 0 || lo > hi || hi > nobs) { s_bad = 1; break; }
+            for (int o = lo; o < hi; o++) {
+                const int ob = obs[o];
+                const int f = ob < 0 ? -1 : ob / cap;
+                if (f < 0 || f >= nframes || f >= K || !(state[f] & ST_LIVE)) { s_bad = 1; break; }
+                if (f == s) continue;   // mit->first->mnId == mnId
+                unsigned h = ((unsigned)f * 2654435761u) & (unsigned)(P - 1);
+                for (int probe = 0;; probe++) {
+                    if (probe == P) { s_full = 1; break; }
+                    const int old = atomicCAS(&tkey[h], -1, f);
+                    if (old == -1) atomicAdd(&s_n, 1);
+                    if (old == -1 || old == f) { atomicAdd(&tcnt[h], 1); break; }
+                    h = (h + 1) & (unsigned)(P - 1);
+                }
+            }
+        }
+    }
+    __syncthreads();
+    const int n = s_n;
+    if (s_bad || s_full || n > C || n == 0) {
+        if (threadIdx.x == 0) {
+            if (s_bad) atomicOr(&flags[F_BAD], 1);
+            else if (n != 0) atomicOr(&flags[F_OVER], 1);
+            cn[p] = 0;   // an empty counter: the call returns at once (KeyFrame.cc:365)
+            fn[p] = 0;
+        }
+        return;
+    }
+    for (int h = threadIdx.x; h < P; h += blockDim.x) {
+        const int f = tkey[h];
+        if (f >= 0) buf[atomicAdd(&s_c, 1)] = CvEnt{key[f], f, tcnt[h]};
+    }
+    const int n2 = pow2ge(n);
+    for (int j = n + threadIdx.x; j < n2; j += blockDim.x) buf[j] = cv_pad(false);
+    __syncthreads();
+    cv_sort<false>(buf, n2);
+    int *crs = cslot + (size_t)p * C, *crw = cw + (size_t)p * C;
+    for (int j = threadIdx.x; j < n; j += blockDim.x) {
+        crs[j] = buf[j].s;
+        crw[j] = buf[j].w;
+        atomicMax(&s_nmax, buf[j].w);
+        if (buf[j].w >= COVIS_TH) atomicAdd(&s_nth, 1);
+    }
+    if (threadIdx.x == 0) cn[p] = n;
+    __syncthreads();   // the table is dead from here: its storage takes the filtered list
+    for (int j = threadIdx.x; j < n; j += blockDim.x)
+        if (buf[j].w == s_nmax) atomicMin(&s_imax, j);   // `mit->second > nmax` in key order: the first maximum
+    __syncthreads();
+    const int m = s_nth > 0 ? s_nth : 1;
+    if (s_nth > 0) {
+        for (int j = threadIdx.x; j < n; j += blockDim.x)
+            if (buf[j].w >= COVIS_TH) flt[atomicAdd(&s_f, 1)] = buf[j];
+    } else if (threadIdx.x == 0) {
+        flt[0] = buf[s_imax];
+    }
+    const int m2 = pow2ge(m);
+    for (int j = m + threadIdx.x; j < m2; j += blockDim.x) flt[j] = cv_pad(true);
+    __syncthreads();
+    cv_sort<true>(flt, m2);   // sort() of (weight, KeyFrame*) pairs, then push_front: descending
+    for (int j = threadIdx.x; j < m; j += blockDim.x) {
+        fslot[(size_t)p * C + j] = flt[j].s;
+        fw[(size_t)p * C + j] = flt[j].w;
+    }
+    if (threadIdx.x == 0) fn[p] = m;
+}
+
+// ---- launch 2: one block of 1024
+__global__ void __launch_bounds__(1024) covis_plan_kernel(
+    int n, const int *__restrict__ slots, int C, const int *__restrict__ cn, const int *__restrict__ cslot, const int *__restrict__ fn,
+    const int *__restrict__ fslot, const int *__restrict__ fw, const int *__restrict__ state, const unsigned long long *__restrict__ key,
+    const int *__restrict__ wn, const int *__restrict__ wslot, int *__restrict__ pos, int *__restrict__ tmark, int *__restrict__ evcnt,
+    int *__restrict__ efill, int *__restrict__ ebase, int *__restrict__ touched, int *__restrict__ ev_p, int *__restrict__ ev_w,
+    int *__restrict__ parent_out, int *__restrict__ flags) {
+    __shared__ int s_nt, s_over, s_carry, s_warp[32];
+    const int bad = flags[F_BAD], over = flags[F_OVER];
+    if (threadIdx.x == 0) { s_nt = 0; s_over = 0; s_carry = 0; }
+    __syncthreads();
+    if (bad || over) {   // rejected before anything was marked
+        if (threadIdx.x == 0) {
+            flags[F_BAD] = 0;
+            flags[F_OVER] = 0;
+            flags[F_OK] = 0;
+            flags[F_NT] = 0;
+            atomicCAS(&flags[F_ERR], 0, bad ? ORBFE_ERR_ARG : ORBFE_ERR_CAPACITY);
+        }
+        if (parent_out)
+            for (int p = threadIdx.x; p < n; p += blockDim.x) parent_out[p] = -1;
+        return;
+    }
+    for (int p = threadIdx.x; p < n; p += blockDim.x) {
+        const int s = slots[p];
+        pos[s] = p;
+        if (atomicExch(&tmark[s], 1) == 0) touched[atomicAdd(&s_nt, 1)] = s;
+    }
+    for (int p = 0; p < n; p++) {
+        const int m = fn[p];
+        for (int j = threadIdx.x; j < m; j += blockDim.x) {
+            const int t = fslot[(size_t)p * C + j];
+            atomicAdd(&evcnt[t], 1);
+            if (atomicExch(&tmark[t], 1) == 0) touched[atomicAdd(&s_nt, 1)] = t;
+        }
+    }
+    __syncthreads();
+    const int nt = s_nt;
+    for (int b = 0; b < nt; b += blockDim.x) {
+        const int i = b + threadIdx.x;
+        const int v = i < nt ? evcnt[touched[i]] : 0;
+        const int e = cv_block_scan(v, s_warp, &s_carry);
+        if (i < nt) ebase[touched[i]] = e;
+    }
+    __syncthreads();
+    for (int p = 0; p < n; p++) {
+        const int m = fn[p];
+        for (int j = threadIdx.x; j < m; j += blockDim.x) {
+            const int t = fslot[(size_t)p * C + j];
+            const int e = ebase[t] + atomicAdd(&efill[t], 1);
+            ev_p[e] = p;
+            ev_w[e] = fw[(size_t)p * C + j];
+        }
+    }
+    __syncthreads();
+    // final size of every touched weight map: its start map plus the keys the applied events add
+    for (int i = threadIdx.x; i < nt; i += blockDim.x) {
+        const int t = touched[i], pt = pos[t];
+        const bool own = pt >= 0 && cn[pt] > 0;
+        const int *row = own ? cslot + (size_t)pt * C : wslot + (size_t)t * C;
+        const int n0 = own ? cn[pt] : wn[t];
+        int extra = 0;
+        for (int e = ebase[t], e1 = e + evcnt[t]; e < e1; e++) {
+            const int q = ev_p[e];
+            if (own && q <= pt) continue;
+            if (cv_find(row, n0, key, key[slots[q]]) < 0) extra++;
+        }
+        if (n0 + extra > C) s_over = 1;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        flags[F_OK] = !s_over;
+        flags[F_NT] = nt;
+        if (s_over) atomicCAS(&flags[F_ERR], 0, ORBFE_ERR_CAPACITY);
+    }
+    if (parent_out)
+        for (int p = threadIdx.x; p < n; p += blockDim.x) {
+            const int st = state[slots[p]];
+            parent_out[p] = !s_over && cn[p] > 0 && (st & ST_FIRST) && !(st & ST_ID0) ? fslot[(size_t)p * C] : -1;
+        }
+}
+
+// ---- launch 3: blocks stride over the touched slots
+__global__ void __launch_bounds__(COVIS_APPLY_BLOCK) covis_apply_kernel(
+    const int *__restrict__ slots, int C, int Cp, int Bp, const int *__restrict__ cn, const int *__restrict__ cslot,
+    const int *__restrict__ cw, const int *__restrict__ fn, const int *__restrict__ fslot, const int *__restrict__ fw,
+    const unsigned long long *__restrict__ key, int *__restrict__ state, int *__restrict__ wn, int *__restrict__ wslot,
+    int *__restrict__ ww, int *__restrict__ on, int *__restrict__ oslot, int *__restrict__ ow, int *__restrict__ named,
+    int *__restrict__ pos, int *__restrict__ tmark, int *__restrict__ evcnt, int *__restrict__ efill, const int *__restrict__ ebase,
+    const int *__restrict__ touched, const int *__restrict__ ev_p, const int *__restrict__ ev_w, const int *__restrict__ flags) {
+    extern __shared__ unsigned long long cv_smem[];
+    CvEnt *A = reinterpret_cast<CvEnt *>(cv_smem);   // Cp: the start map, later the full sort
+    CvEnt *E = A + Cp;                                // Bp: the applied events
+    CvEnt *F = E + Bp;                                // Cp: the final map, key ascending
+    __shared__ int s_ne, s_nf, s_changed;
+    const int nt = flags[F_NT];
+    const bool ok = flags[F_OK] != 0;
+    for (int i = blockIdx.x; i < nt; i += gridDim.x) {
+        const int t = touched[i], pt = pos[t];
+        if (ok) {
+            const bool own = pt >= 0 && cn[pt] > 0;
+            const int *rs = own ? cslot + (size_t)pt * C : wslot + (size_t)t * C;
+            const int *rw = own ? cw + (size_t)pt * C : ww + (size_t)t * C;
+            const int na = own ? cn[pt] : wn[t];
+            const int nold = wn[t];
+            if (threadIdx.x == 0) { s_ne = 0; s_changed = 0; }
+            for (int j = threadIdx.x; j < na; j += blockDim.x) A[j] = CvEnt{key[rs[j]], rs[j], rw[j]};
+            __syncthreads();
+            for (int e = ebase[t] + threadIdx.x, e1 = ebase[t] + evcnt[t]; e < e1; e += blockDim.x) {
+                const int q = ev_p[e];
+                if (own && q <= pt) continue;   // overwritten by the slot's own mConnectedKeyFrameWeights = KFcounter
+                const int src = slots[q];
+                E[atomicAdd(&s_ne, 1)] = CvEnt{key[src], src, ev_w[e]};
+            }
+            __syncthreads();
+            const int ne = s_ne, ne2 = pow2ge(max(ne, 1));
+            for (int j = ne + threadIdx.x; j < ne2; j += blockDim.x) E[j] = cv_pad(false);
+            __syncthreads();
+            cv_sort<false>(E, ne2);
+            // an event changes the map when its key is absent or holds another weight (AddConnection, KeyFrame.cc:130-135)
+            for (int j = threadIdx.x; j < ne; j += blockDim.x) {
+                int lo = 0, hi = na;
+                while (lo < hi) {
+                    const int mid = (lo + hi) >> 1;
+                    if (A[mid].k < E[j].k) lo = mid + 1; else hi = mid;
+                }
+                if (lo == na || A[lo].k != E[j].k || A[lo].w != E[j].w) s_changed = 1;
+            }
+            if (threadIdx.x == 0) {   // merge by key; an event's weight replaces the start map's
+                int a = 0, b = 0, f = 0;
+                while (a < na || b < ne) {
+                    if (b == ne || (a < na && A[a].k < E[b].k)) F[f++] = A[a++];
+                    else {
+                        if (a < na && A[a].k == E[b].k) a++;
+                        F[f++] = E[b++];
+                    }
+                }
+                s_nf = f;
+            }
+            __syncthreads();
+            const int nf = s_nf;
+            int *ws = wslot + (size_t)t * C, *wv = ww + (size_t)t * C;
+            // keys that leave or enter the map
+            for (int j = threadIdx.x; j < nold; j += blockDim.x) {
+                const unsigned long long k = key[ws[j]];
+                int lo = 0, hi = nf;
+                while (lo < hi) {
+                    const int mid = (lo + hi) >> 1;
+                    if (F[mid].k < k) lo = mid + 1; else hi = mid;
+                }
+                if (lo == nf || F[lo].k != k) atomicSub(&named[ws[j]], 1);
+            }
+            for (int j = threadIdx.x; j < nf; j += blockDim.x)
+                if (cv_find(ws, nold, key, F[j].k) < 0) atomicAdd(&named[F[j].s], 1);
+            __syncthreads();
+            for (int j = threadIdx.x; j < nf; j += blockDim.x) { ws[j] = F[j].s; wv[j] = F[j].w; }
+            const bool changed = s_changed != 0;
+            int *os = oslot + (size_t)t * C, *ov = ow + (size_t)t * C;
+            if (changed) {   // UpdateBestCovisibles over the whole map
+                const int nf2 = pow2ge(nf);
+                for (int j = threadIdx.x; j < nf2; j += blockDim.x) A[j] = j < nf ? F[j] : cv_pad(true);
+                __syncthreads();
+                cv_sort<true>(A, nf2);
+                for (int j = threadIdx.x; j < nf; j += blockDim.x) { os[j] = A[j].s; ov[j] = A[j].w; }
+            } else if (own) {
+                const int m = fn[pt];
+                for (int j = threadIdx.x; j < m; j += blockDim.x) { os[j] = fslot[(size_t)pt * C + j]; ov[j] = fw[(size_t)pt * C + j]; }
+            }
+            if (threadIdx.x == 0) {
+                wn[t] = nf;
+                if (changed) on[t] = nf;
+                else if (own) on[t] = fn[pt];
+                if (own && (state[t] & ST_FIRST) && !(state[t] & ST_ID0)) state[t] &= ~ST_FIRST;
+            }
+        }
+        if (threadIdx.x == 0) {
+            tmark[t] = 0;
+            evcnt[t] = 0;
+            efill[t] = 0;
+            pos[t] = -1;
+        }
+        __syncthreads();
+    }
+}
+
+// ---- SetBadFlag's connection half: block j handles the j-th key of the slot's own map (EraseConnection on that neighbour)
+__global__ void __launch_bounds__(COVIS_APPLY_BLOCK) covis_erase_kernel(int slot, int C, const unsigned long long *__restrict__ key,
+                                                                         int *__restrict__ wn, int *__restrict__ wslot, int *__restrict__ ww,
+                                                                         int *__restrict__ on, int *__restrict__ oslot, int *__restrict__ ow,
+                                                                         int *__restrict__ named) {
+    extern __shared__ unsigned long long cv_smem[];
+    CvEnt *A = reinterpret_cast<CvEnt *>(cv_smem);
+    __shared__ int s_at;
+    const int j = blockIdx.x;
+    if (j >= wn[slot]) return;
+    const int nb = wslot[(size_t)slot * C + j];
+    int *ws = wslot + (size_t)nb * C, *wv = ww + (size_t)nb * C;
+    const int n = wn[nb];
+    if (threadIdx.x == 0) {
+        atomicSub(&named[nb], 1);   // the slot's own map is cleared
+        s_at = cv_find(ws, n, key, key[slot]);
+    }
+    __syncthreads();
+    const int at = s_at;
+    if (at < 0) return;   // a map that does not name the slot is left as it is (KeyFrame.cc:601)
+    const int m = n - 1, m2 = pow2ge(max(m, 1));
+    for (int i = threadIdx.x; i < m2; i += blockDim.x) {
+        if (i < m) {
+            const int src = i < at ? i : i + 1;
+            A[i] = CvEnt{key[ws[src]], ws[src], wv[src]};
+        } else {
+            A[i] = cv_pad(true);
+        }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < m; i += blockDim.x) { ws[i] = A[i].s; wv[i] = A[i].w; }   // key order, the entry removed
+    __syncthreads();
+    cv_sort<true>(A, m2);
+    int *os = oslot + (size_t)nb * C, *ov = ow + (size_t)nb * C;
+    for (int i = threadIdx.x; i < m; i += blockDim.x) { os[i] = A[i].s; ov[i] = A[i].w; }
+    if (threadIdx.x == 0) {
+        wn[nb] = m;
+        on[nb] = m;
+        atomicSub(&named[slot], 1);
+    }
+}
+
+__global__ void covis_retire_kernel(int slot, int *__restrict__ state, int *__restrict__ wn, int *__restrict__ on) {
+    state[slot] = 0;
+    wn[slot] = 0;
+    on[slot] = 0;
+}
+
+// rows: slot, mnId == 0, key (two ints)
+__global__ void covis_add_kernel(int n, const int *__restrict__ rows, unsigned long long *__restrict__ key, int *__restrict__ state,
+                                 int *__restrict__ wn, int *__restrict__ on) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int *r = rows + 4 * i;
+    const int s = r[0];
+    key[s] = (unsigned long long)(unsigned)r[2] | (unsigned long long)(unsigned)r[3] << 32;
+    state[s] = ST_LIVE | ST_FIRST | (r[1] ? ST_ID0 : 0);
+    wn[s] = 0;
+    on[s] = 0;
+}
+
+// ---- the exported lists: row lengths and their exclusive scan (one block of 1024), then one block per row
+__global__ void __launch_bounds__(1024) covis_lens_kernel(int n, const int *__restrict__ slots, int which, int limit,
+                                                          const int *__restrict__ wn, const int *__restrict__ on, int *__restrict__ ptr) {
+    __shared__ int s_carry, s_warp[32];
+    if (threadIdx.x == 0) s_carry = 0;
+    __syncthreads();
+    for (int b = 0; b < n; b += blockDim.x) {
+        const int i = b + threadIdx.x;
+        const int v = i < n ? min(which ? wn[slots[i]] : on[slots[i]], limit) : 0;
+        const int e = cv_block_scan(v, s_warp, &s_carry);
+        if (i < n) ptr[i] = e;
+    }
+    if (threadIdx.x == 0) ptr[n] = s_carry;
+}
+
+__global__ void covis_lists_kernel(const int *__restrict__ slots, int which, int C, const int *__restrict__ ptr,
+                                   const int *__restrict__ wslot, const int *__restrict__ ww, const int *__restrict__ oslot,
+                                   const int *__restrict__ ow, const int *__restrict__ state, int *__restrict__ list,
+                                   int *__restrict__ weights) {
+    const int i = blockIdx.x, s = slots[i];
+    const int lo = ptr[i], len = ptr[i + 1] - lo;
+    const int *rs = (which ? wslot : oslot) + (size_t)s * C, *rw = (which ? ww : ow) + (size_t)s * C;
+    for (int j = threadIdx.x; j < len; j += blockDim.x) {
+        const int v = rs[j];
+        list[lo + j] = (state[v] & ST_LIVE) ? v : -1;   // a retired keyframe still named here: isBad() -> negative
+        if (weights) weights[lo + j] = rw[j];
+    }
+}
+
+}  // namespace orbfe
+
+using namespace orbfe;
+
+#define COVIS_TRY(expr)                                                                                      \
+    do {                                                                                                     \
+        cudaError_t e__ = (expr);                                                                            \
+        if (e__ != cudaSuccess)                                                                              \
+            return set_error(ORBFE_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
+    } while (0)
+
+struct OrbfeCovisGraph {
+    int device = 0, K = 0, C = 0, Cp = 1, P = 2, B = 0, Bp = 1, apply_grid = 1;
+    size_t count_smem = 0, apply_smem = 0, erase_smem = 0;
+    cudaStream_t stream = nullptr;
+    cudaEvent_t last = nullptr;   // the handle's most recent work: every call orders itself after it
+    // host mirror of what only the synchronous calls change
+    std::vector<uint8_t> live, id0;
+    std::vector<unsigned long long> keys;
+    std::unordered_set<unsigned long long> live_keys;
+    // device
+    unsigned long long *key = nullptr;
+    int *state = nullptr, *wn = nullptr, *wslot = nullptr, *ww = nullptr, *on = nullptr, *oslot = nullptr, *ow = nullptr, *named = nullptr;
+    int *slots = nullptr, *pos = nullptr, *tmark = nullptr, *evcnt = nullptr, *efill = nullptr, *ebase = nullptr, *touched = nullptr;
+    int *cn = nullptr, *cslot = nullptr, *cw = nullptr, *fn = nullptr, *fslot = nullptr, *fw = nullptr, *ev_p = nullptr, *ev_w = nullptr;
+    int *flags = nullptr;
+};
+
+extern "C" void orbfe_covis_destroy(OrbfeCovisGraph *g) {
+    if (!g) return;
+    cudaSetDevice(g->device);
+    if (g->stream) cudaStreamSynchronize(g->stream);
+    void *ptrs[] = {g->key, g->state, g->wn, g->wslot, g->ww, g->on, g->oslot, g->ow, g->named, g->slots, g->pos, g->tmark, g->evcnt,
+                    g->efill, g->ebase, g->touched, g->cn, g->cslot, g->cw, g->fn, g->fslot, g->fw, g->ev_p, g->ev_w, g->flags};
+    for (void *p : ptrs) cudaFree(p);
+    if (g->last) cudaEventDestroy(g->last);
+    if (g->stream) cudaStreamDestroy(g->stream);
+    delete g;
+}
+
+// every slot empty; the batch scratch in its between-batches state
+static int covis_reset(OrbfeCovisGraph *g, cudaStream_t s) {
+    const size_t K = (size_t)g->K;
+    COVIS_TRY(cudaMemsetAsync(g->state, 0, sizeof(int) * K, s));
+    COVIS_TRY(cudaMemsetAsync(g->wn, 0, sizeof(int) * K, s));
+    COVIS_TRY(cudaMemsetAsync(g->on, 0, sizeof(int) * K, s));
+    COVIS_TRY(cudaMemsetAsync(g->named, 0, sizeof(int) * K, s));
+    COVIS_TRY(cudaMemsetAsync(g->pos, 0xFF, sizeof(int) * K, s));
+    COVIS_TRY(cudaMemsetAsync(g->tmark, 0, sizeof(int) * K, s));
+    COVIS_TRY(cudaMemsetAsync(g->evcnt, 0, sizeof(int) * K, s));
+    COVIS_TRY(cudaMemsetAsync(g->efill, 0, sizeof(int) * K, s));
+    g->live.assign(K, 0);
+    g->id0.assign(K, 0);
+    g->keys.assign(K, 0);
+    g->live_keys.clear();
+    return ORBFE_OK;
+}
+
+extern "C" int orbfe_covis_create(int device, int max_keyframes, int max_connections, int max_batch, OrbfeCovisGraph **out) {
+    if (!out) return set_error(ORBFE_ERR_ARG, "orbfe_covis_create: NULL out");
+    *out = nullptr;
+    if (device < 0 || max_keyframes < 1 || max_keyframes > (1 << 24) || max_connections < 1 || max_connections > COVIS_MAX_CONN ||
+        max_batch < 1 || max_batch > COVIS_MAX_BATCH)
+        return set_error(ORBFE_ERR_ARG, "orbfe_covis_create: bad arguments (device >= 0, 1 <= max_keyframes <= 2^24, 1 <= max_connections <= %d, "
+                         "1 <= max_batch <= %d)", COVIS_MAX_CONN, COVIS_MAX_BATCH);
+    if ((long long)max_keyframes * max_connections >= (1LL << 31) || (long long)max_batch * max_connections >= (1LL << 31))
+        return set_error(ORBFE_ERR_ARG, "orbfe_covis_create: max_keyframes * max_connections must be < 2^31");
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || device >= ndev) {
+        cudaGetLastError();
+        return set_error(ORBFE_ERR_NO_DEVICE, "orbfe_covis_create: no CUDA device %d", device);
+    }
+    OrbfeCovisGraph *g = new OrbfeCovisGraph();
+    g->device = device;
+    g->K = max_keyframes;
+    g->C = max_connections;
+    g->Cp = pow2ge(max_connections);
+    g->P = 2 * g->Cp;
+    g->B = max_batch;
+    g->Bp = pow2ge(max_batch);
+    g->count_smem = sizeof(CvEnt) * (size_t)g->Cp + 2 * sizeof(int) * (size_t)g->P;
+    g->apply_smem = sizeof(CvEnt) * (2 * (size_t)g->Cp + (size_t)g->Bp);
+    g->erase_smem = sizeof(CvEnt) * (size_t)g->Cp;
+    const size_t K = (size_t)g->K, KC = K * g->C, BC = (size_t)g->B * g->C;
+    bool ok = cudaSetDevice(device) == cudaSuccess && cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking) == cudaSuccess &&
+              cudaEventCreateWithFlags(&g->last, cudaEventDisableTiming) == cudaSuccess;
+    int nsm = 1;
+    ok = ok && cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device) == cudaSuccess;
+    g->apply_grid = std::max(1, std::min(g->K, 4 * nsm));
+    ok = ok && cudaFuncSetAttribute(covis_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->count_smem) == cudaSuccess &&
+         cudaFuncSetAttribute(covis_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->apply_smem) == cudaSuccess &&
+         cudaFuncSetAttribute(covis_erase_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->erase_smem) == cudaSuccess;
+#define COVIS_ALLOC(p, n) ok = ok && cudaMalloc((void **)&(p), sizeof(*(p)) * (n)) == cudaSuccess
+    COVIS_ALLOC(g->key, K); COVIS_ALLOC(g->state, K); COVIS_ALLOC(g->wn, K); COVIS_ALLOC(g->on, K); COVIS_ALLOC(g->named, K);
+    COVIS_ALLOC(g->wslot, KC); COVIS_ALLOC(g->ww, KC); COVIS_ALLOC(g->oslot, KC); COVIS_ALLOC(g->ow, KC);
+    // add stages 4 ints per keyframe; batches and lists name at most K slots
+    COVIS_ALLOC(g->slots, 4 * K); COVIS_ALLOC(g->pos, K); COVIS_ALLOC(g->tmark, K); COVIS_ALLOC(g->evcnt, K);
+    COVIS_ALLOC(g->efill, K); COVIS_ALLOC(g->ebase, K); COVIS_ALLOC(g->touched, K);
+    COVIS_ALLOC(g->cn, (size_t)g->B); COVIS_ALLOC(g->fn, (size_t)g->B); COVIS_ALLOC(g->cslot, BC); COVIS_ALLOC(g->cw, BC);
+    COVIS_ALLOC(g->fslot, BC); COVIS_ALLOC(g->fw, BC); COVIS_ALLOC(g->ev_p, BC); COVIS_ALLOC(g->ev_w, BC);
+    COVIS_ALLOC(g->flags, (size_t)F_COUNT);
+#undef COVIS_ALLOC
+    ok = ok && cudaMemset(g->flags, 0, sizeof(int) * F_COUNT) == cudaSuccess && cudaMemset(g->key, 0, sizeof(unsigned long long) * K) == cudaSuccess;
+    if (!ok) {
+        const int rc = set_error(ORBFE_ERR_CUDA, "orbfe_covis_create: allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
+        orbfe_covis_destroy(g);
+        return rc;
+    }
+    int rc = covis_reset(g, g->stream);
+    if (!rc && cudaStreamSynchronize(g->stream) != cudaSuccess) rc = set_error(ORBFE_ERR_CUDA, "orbfe_covis_create: reset failed");
+    if (rc) { orbfe_covis_destroy(g); return rc; }
+    *out = g;
+    return ORBFE_OK;
+}
+
+static int covis_enter(OrbfeCovisGraph *g, cudaStream_t s) {
+    COVIS_TRY(cudaSetDevice(g->device));
+    COVIS_TRY(cudaStreamWaitEvent(s, g->last, 0));
+    return ORBFE_OK;
+}
+static int covis_leave(OrbfeCovisGraph *g, cudaStream_t s, bool sync) {
+    COVIS_TRY(cudaGetLastError());
+    COVIS_TRY(cudaEventRecord(g->last, s));
+    if (sync) COVIS_TRY(cudaStreamSynchronize(s));
+    return ORBFE_OK;
+}
+
+extern "C" int orbfe_covis_add(OrbfeCovisGraph *g, int n, const int32_t *slots, const int32_t *ids, const uint64_t *keys) {
+    if (!g || n < 0 || (n > 0 && (!slots || !ids || !keys))) return set_error(ORBFE_ERR_ARG, "orbfe_covis_add: bad arguments");
+    for (int i = 0; i < n; i++)
+        if (slots[i] < 0) return set_error(ORBFE_ERR_ARG, "orbfe_covis_add: negative slot");
+    if (n == 0) return ORBFE_OK;
+    if (n > g->K) return set_error(ORBFE_ERR_ARG, "orbfe_covis_add: more keyframes than slots");
+    std::unordered_set<int> seen;
+    std::unordered_set<unsigned long long> new_keys;
+    for (int i = 0; i < n; i++) {
+        const int s = slots[i];
+        if (s < 0 || s >= g->K) return set_error(ORBFE_ERR_ARG, "orbfe_covis_add: slot %d out of range (max_keyframes %d)", s, g->K);
+        if (g->live[s]) return set_error(ORBFE_ERR_ARG, "orbfe_covis_add: slot %d is live", s);
+        if (!seen.insert(s).second) return set_error(ORBFE_ERR_ARG, "orbfe_covis_add: slot %d listed twice", s);
+        if (g->live_keys.count(keys[i]) || !new_keys.insert(keys[i]).second)
+            return set_error(ORBFE_ERR_ARG, "orbfe_covis_add: key of slot %d equals a live keyframe's key", s);
+    }
+    cudaStream_t st = g->stream;
+    int rc = covis_enter(g, st);
+    if (rc) return rc;
+    // a retired slot that a weight map still names is the reference's stale pointer: it cannot become a new keyframe
+    std::vector<int> named((size_t)g->K);
+    COVIS_TRY(cudaMemcpyAsync(named.data(), g->named, sizeof(int) * named.size(), cudaMemcpyDeviceToHost, st));
+    COVIS_TRY(cudaStreamSynchronize(st));
+    for (int i = 0; i < n; i++)
+        if (named[slots[i]] != 0)
+            return set_error(ORBFE_ERR_ARG, "orbfe_covis_add: retired slot %d is still named by %d weight maps", slots[i], named[slots[i]]);
+    std::vector<int> rows(4 * (size_t)n);
+    for (int i = 0; i < n; i++) {
+        rows[4 * i] = slots[i];
+        rows[4 * i + 1] = ids[i] == 0;
+        rows[4 * i + 2] = (int)(uint32_t)keys[i];
+        rows[4 * i + 3] = (int)(uint32_t)(keys[i] >> 32);
+    }
+    COVIS_TRY(cudaMemcpyAsync(g->slots, rows.data(), sizeof(int) * rows.size(), cudaMemcpyHostToDevice, st));
+    covis_add_kernel<<<(n + 127) / 128, 128, 0, st>>>(n, g->slots, g->key, g->state, g->wn, g->on);
+    if ((rc = covis_leave(g, st, true))) return rc;
+    for (int i = 0; i < n; i++) {
+        g->live[slots[i]] = 1;
+        g->id0[slots[i]] = ids[i] == 0;
+        g->keys[slots[i]] = keys[i];
+        g->live_keys.insert(keys[i]);
+    }
+    return ORBFE_OK;
+}
+
+extern "C" int orbfe_covis_update_connections_device(OrbfeCovisGraph *g, int n, const int32_t *slots, const int32_t *d_kf_mp,
+                                                     const int *d_counts, int nframes, int cap, const int32_t *d_group_ptr,
+                                                     const int32_t *d_obs, int npoints, int nobs, int32_t *parent_out, void *stream) {
+    if (!g || n < 0 || nframes < 1 || cap < 1 || npoints < 0 || nobs < 0 || (long long)nframes * cap >= (1LL << 31))
+        return set_error(ORBFE_ERR_ARG, "orbfe_covis_update_connections_device: bad arguments (n >= 0, nframes >= 1, cap >= 1, "
+                         "nframes*cap < 2^31, npoints >= 0, nobs >= 0)");
+    if (n > 0 && (!slots || !d_kf_mp || !d_counts || !d_group_ptr || (nobs > 0 && !d_obs)))
+        return set_error(ORBFE_ERR_ARG, "orbfe_covis_update_connections_device: NULL argument");
+    std::unordered_set<int> seen;
+    for (int i = 0; i < n; i++) {
+        const int s = slots[i];
+        if (s < 0 || s >= nframes) return set_error(ORBFE_ERR_ARG, "orbfe_covis_update_connections_device: slot %d outside [0, nframes)", s);
+        if (!seen.insert(s).second) return set_error(ORBFE_ERR_ARG, "orbfe_covis_update_connections_device: slot %d listed twice", s);
+    }
+    if (n == 0) return ORBFE_OK;
+    if (n > g->B) return set_error(ORBFE_ERR_ARG, "orbfe_covis_update_connections_device: n %d > max_batch %d", n, g->B);
+    for (int i = 0; i < n; i++)
+        if (slots[i] >= g->K || !g->live[slots[i]])
+            return set_error(ORBFE_ERR_ARG, "orbfe_covis_update_connections_device: slot %d is not a live keyframe", slots[i]);
+    cudaStream_t st = stream ? (cudaStream_t)stream : g->stream;
+    int rc = covis_enter(g, st);
+    if (rc) return rc;
+    COVIS_TRY(cudaMemcpyAsync(g->slots, slots, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
+    covis_count_kernel<<<n, COVIS_COUNT_BLOCK, g->count_smem, st>>>(g->slots, g->C, g->Cp, g->P, d_kf_mp, d_counts, nframes, cap,
+                                                                  d_group_ptr, d_obs, npoints, nobs, g->K, g->state, g->key, g->cn, g->cslot,
+                                                                  g->cw, g->fn, g->fslot, g->fw, g->flags);
+    covis_plan_kernel<<<1, 1024, 0, st>>>(n, g->slots, g->C, g->cn, g->cslot, g->fn, g->fslot, g->fw, g->state, g->key, g->wn, g->wslot,
+                                          g->pos, g->tmark, g->evcnt, g->efill, g->ebase, g->touched, g->ev_p, g->ev_w, parent_out, g->flags);
+    covis_apply_kernel<<<g->apply_grid, COVIS_APPLY_BLOCK, g->apply_smem, st>>>(
+        g->slots, g->C, g->Cp, g->Bp, g->cn, g->cslot, g->cw, g->fn, g->fslot, g->fw, g->key, g->state, g->wn, g->wslot, g->ww, g->on,
+        g->oslot, g->ow, g->named, g->pos, g->tmark, g->evcnt, g->efill, g->ebase, g->touched, g->ev_p, g->ev_w, g->flags);
+    return covis_leave(g, st, false);
+}
+
+extern "C" int orbfe_covis_erase(OrbfeCovisGraph *g, int slot) {
+    if (!g || slot < 0 || slot >= g->K) return set_error(ORBFE_ERR_ARG, "orbfe_covis_erase: bad arguments");
+    if (!g->live[slot] || g->id0[slot]) return ORBFE_OK;   // SetBadFlag of mnId == 0 returns at once (KeyFrame.cc:501)
+    cudaStream_t st = g->stream;
+    int rc = covis_enter(g, st);
+    if (rc) return rc;
+    covis_erase_kernel<<<g->C, COVIS_APPLY_BLOCK, g->erase_smem, st>>>(slot, g->C, g->key, g->wn, g->wslot, g->ww, g->on, g->oslot, g->ow,
+                                                                      g->named);
+    covis_retire_kernel<<<1, 1, 0, st>>>(slot, g->state, g->wn, g->on);
+    if ((rc = covis_leave(g, st, true))) return rc;
+    g->live[slot] = 0;
+    g->live_keys.erase(g->keys[slot]);
+    return ORBFE_OK;
+}
+
+extern "C" int orbfe_covis_clear(OrbfeCovisGraph *g) {
+    if (!g) return set_error(ORBFE_ERR_ARG, "orbfe_covis_clear: bad arguments");
+    int rc = covis_enter(g, g->stream);
+    if (rc) return rc;
+    if ((rc = covis_reset(g, g->stream))) return rc;
+    return covis_leave(g, g->stream, true);
+}
+
+extern "C" int orbfe_covis_lists_device(OrbfeCovisGraph *g, int which, int n, const int32_t *slots, int nbest, int32_t *d_ptr,
+                                        int32_t *d_list, int32_t *d_weights, void *stream) {
+    if (!g || (which != 0 && which != 1) || n < 0 || (n > 0 && (!slots || !d_ptr || !d_list)))
+        return set_error(ORBFE_ERR_ARG, "orbfe_covis_lists_device: bad arguments (which 0 or 1, n >= 0, slots / d_ptr / d_list non-NULL)");
+    for (int i = 0; i < n; i++)
+        if (slots[i] < 0) return set_error(ORBFE_ERR_ARG, "orbfe_covis_lists_device: negative slot");
+    if (n == 0) return ORBFE_OK;
+    if (n > g->K) return set_error(ORBFE_ERR_ARG, "orbfe_covis_lists_device: more rows than slots");
+    for (int i = 0; i < n; i++)
+        if (slots[i] >= g->K) return set_error(ORBFE_ERR_ARG, "orbfe_covis_lists_device: slot %d out of range", slots[i]);
+    const int limit = which == 0 && nbest > 0 ? std::min(nbest, g->C) : g->C;
+    cudaStream_t st = stream ? (cudaStream_t)stream : g->stream;
+    int rc = covis_enter(g, st);
+    if (rc) return rc;
+    COVIS_TRY(cudaMemcpyAsync(g->slots, slots, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
+    covis_lens_kernel<<<1, 1024, 0, st>>>(n, g->slots, which, limit, g->wn, g->on, d_ptr);
+    covis_lists_kernel<<<n, 128, 0, st>>>(g->slots, which, g->C, d_ptr, g->wslot, g->ww, g->oslot, g->ow, g->state, d_list, d_weights);
+    return covis_leave(g, st, false);
+}
+
+extern "C" int orbfe_covis_sync(OrbfeCovisGraph *g) {
+    if (!g) return set_error(ORBFE_ERR_ARG, "orbfe_covis_sync: bad arguments");
+    cudaStream_t st = g->stream;
+    int rc = covis_enter(g, st);
+    if (rc) return rc;
+    int err = 0;
+    COVIS_TRY(cudaMemcpyAsync(&err, g->flags + F_ERR, sizeof(int), cudaMemcpyDeviceToHost, st));
+    COVIS_TRY(cudaMemsetAsync(g->flags + F_ERR, 0, sizeof(int), st));
+    if ((rc = covis_leave(g, st, true))) return rc;
+    if (err == ORBFE_ERR_ARG)
+        return set_error(ORBFE_ERR_ARG, "orbfe_covis_sync: an update batch was rejected: a point index, group pointer or observation was "
+                         "out of range or named a slot that is not live");
+    if (err == ORBFE_ERR_CAPACITY)
+        return set_error(ORBFE_ERR_CAPACITY, "orbfe_covis_sync: an update batch was rejected: a weight map would exceed max_connections");
+    return err;
+}

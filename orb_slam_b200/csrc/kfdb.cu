@@ -144,6 +144,21 @@ __global__ void kfdb_covis_kernel(const int *__restrict__ rows, int n, int *__re
     for (int j = 0; j < c; j++) cov[s * KFDB_COVIS + j] = r[2 + j];
 }
 
+// the device form: row i of the CSR lists (ptr[i] .. ptr[i+1]) for slot rows[i]; only its first 10 entries are read, and an
+// entry outside [0, K) is kept in its place as -1
+__global__ void kfdb_covis_device_kernel(const int *__restrict__ rows, int n, int K, const int *__restrict__ ptr,
+                                         const int *__restrict__ lists, int *__restrict__ covn, int *__restrict__ cov) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int s = rows[i], lo = ptr[i];
+    const int c = min(max(ptr[i + 1] - lo, 0), KFDB_COVIS);
+    for (int j = 0; j < c; j++) {
+        const int v = lists[lo + j];
+        cov[s * KFDB_COVIS + j] = (unsigned)v < (unsigned)K ? v : -1;
+    }
+    covn[s] = c;
+}
+
 __device__ __forceinline__ unsigned q_stamp(unsigned long long st) { return (unsigned)(st >> 32); }
 __device__ __forceinline__ int q_rank(unsigned long long st) { return (int)((st >> 16) & 0xFFFFu); }
 __device__ __forceinline__ int q_words(unsigned long long st) { return (int)(st & 0xFFFFu); }
@@ -355,6 +370,7 @@ __global__ void __launch_bounds__(KFDB_BLOCK) kfdb_select_kernel(int loop, unsig
         const int nc = covn[s];
         for (int j = 0; j < nc; j++) {
             const int s2 = cov[s * KFDB_COVIS + j];
+            if (s2 < 0) continue;   // a bad keyframe in a device-written list: it holds its place and contributes nothing
             const unsigned long long st = state[s2];
             // an earlier query's score when s2 was only touched; read next to the stamp, used only when s2 counts
             const float s2c = kfdb_score_read(q, qid0, s2, K, scored, sc);
@@ -741,6 +757,26 @@ extern "C" int orbfe_kfdb_set_covisibles(OrbfeKeyFrameDB *db, int n, const int32
     KFDB_TRY(cudaMemcpyAsync(db->covrows, rows.data(), sizeof(int) * rows.size(), cudaMemcpyHostToDevice, s));
     kfdb_covis_kernel<<<(n + 127) / 128, 128, 0, s>>>(db->covrows, n, db->covn, db->cov);
     return kfdb_leave(db, s, true);
+}
+
+extern "C" int orbfe_kfdb_set_covisibles_device(OrbfeKeyFrameDB *db, int n, const int32_t *slots, const int32_t *d_ptr,
+                                                const int32_t *d_lists, void *stream) {
+    if (!db || n < 0 || (n > 0 && (!slots || !d_ptr || !d_lists))) return set_error(ORBFE_ERR_ARG, "bad arguments");
+    for (int i = 0; i < n; i++)
+        if (slots[i] < 0) return set_error(ORBFE_ERR_ARG, "negative slot");
+    if (n == 0) return ORBFE_OK;
+    if (n > db->K) return set_error(ORBFE_ERR_ARG, "more lists than slots");
+    std::vector<uint8_t> seen(db->K, 0);
+    for (int i = 0; i < n; i++) {
+        if (slots[i] >= db->K) return set_error(ORBFE_ERR_ARG, "slot %d out of range", slots[i]);
+        if (seen[slots[i]]++) return set_error(ORBFE_ERR_ARG, "slot %d listed twice", slots[i]);
+    }
+    cudaStream_t s = stream ? (cudaStream_t)stream : db->stream;
+    int rc = kfdb_enter(db, s);
+    if (rc) return rc;
+    KFDB_TRY(cudaMemcpyAsync(db->covrows, slots, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, s));
+    kfdb_covis_device_kernel<<<(n + 127) / 128, 128, 0, s>>>(db->covrows, n, db->K, d_ptr, d_lists, db->covn, db->cov);
+    return kfdb_leave(db, s, false);
 }
 
 static int kfdb_check_detect(int mode, int nq, int nconn, int cap) {

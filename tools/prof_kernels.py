@@ -49,6 +49,11 @@
                    SetWorldPos, in one batch: CUDA-event ms of orbfe_normal_and_depth_device, the wall time of
                    orbfe_normal_and_depth including the host gather of the centres and its staging, and the wall time of the
                    oracle's C loop on the same arrays (plain float / double C, not OpenCV's cv::Mat), outputs compared.
+  --what covis     KeyFrame::UpdateConnections on the resident covisibility graph (orbfe_covis_update_connections_device) of a
+                   2000-keyframe map (2000 features each, ~8 observations per point, tests/covis_scenes.py scene_large), after
+                   every keyframe was updated once: CUDA-event ms of a batch of 1 (LocalMapping's call) and of a batch of 64
+                   (loop correction), and the wall time of the oracle's C restatement (oracle/orb_oracle_covis.c: dense rows, not
+                   the reference's std::map) for the same calls.
 Prints one JSON object per --what; never a bench value when run under ncu."""
 import argparse
 import ctypes as C
@@ -1556,6 +1561,69 @@ def normaldepth(args):
     return out
 
 
+def covis(args):
+    """UpdateConnections of one keyframe and of 64 keyframes of a 2000-keyframe map, each keyframe already updated once (a
+    repeated call leaves the graph as it is, so every timed call does the same work)."""
+    import torch
+    from orb_slam_b200 import bow as BW
+    from oracle.covis import CovisOracle
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests"))
+    import covis_scenes as CS
+    scene = CS.scene_large()
+    K, cap = scene.nkf, scene.cap
+    slot_of = scene.slots()
+    model = CS.Model(scene)
+    for st in scene.steps:
+        model.apply(st)
+    kf_mp, counts, gp, obs = model.inputs(slot_of, K)
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    s = stream.cuda_stream
+    tt = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    d_mp, d_cnt, d_gp, d_obs = tt(kf_mp), tt(counts), tt(gp), tt(obs)
+    g = BW.CovisibilityGraph(K, 64, 64)
+    orc = CovisOracle(K)
+    g.add(slot_of, np.arange(K), np.arange(K))
+    for k in range(K):
+        orc.add(slot_of[k], k, k)
+    upd = lambda sl: g.update_connections_device(sl, d_mp.data_ptr(), d_cnt.data_ptr(), K, cap, d_gp.data_ptr(), d_obs.data_ptr(),
+                                                 len(gp) - 1, len(obs), stream=s)
+    order = [int(slot_of[k]) for k in range(K)]
+    for b in range(0, K, 64):
+        upd(order[b:b + 64])
+    orc.replay(order, kf_mp, counts, cap, gp, obs)
+    g.sync()
+    out = {"what": "UpdateConnections on a %d-keyframe map of %d features, %d points, %d observations" % (K, cap, len(gp) - 1, len(obs))}
+    mid = K // 2
+    for name, sl in (("batch1", order[mid:mid + 1]), ("batch64", order[mid:mid + 64])):
+        for _ in range(max(args.warmup, 3)):
+            upd(sl)
+        stream.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        iters = args.iters * 20
+        times = []
+        for _ in range(5):
+            e0.record(stream)
+            for _ in range(iters):
+                upd(sl)
+            e1.record(stream)
+            stream.synchronize()
+            times.append(e0.elapsed_time(e1) / iters)
+        g.sync()
+        out[name + "_device_ms"] = float(np.median(times))
+        out[name + "_device_ms_min_max"] = [float(min(times)), float(max(times))]
+        orc_ms = []
+        for _ in range(3):
+            t0 = time.perf_counter()
+            orc.replay(sl, kf_mp, counts, cap, gp, obs)
+            orc_ms.append((time.perf_counter() - t0) * 1e3)
+        out[name + "_oracle_c_wall_ms_not_reference"] = float(np.median(orc_ms))
+    g.close()
+    orc.close()
+    _gpu_and_power_limit(out)
+    return out
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--what", default="config3,config5")
@@ -1569,4 +1637,4 @@ if __name__ == "__main__":
         print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fast": fast, "latency": latency,
                           "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb, "kfdbbatch": kfdbbatch, "bowchain": bowchain,
                           "windowed": windowed, "guided": guided, "loopscore": loopscore, "vocload": vocload,
-                          "normaldepth": normaldepth}[w](args)))
+                          "normaldepth": normaldepth, "covis": covis}[w](args)))
