@@ -531,22 +531,15 @@ __global__ void __launch_bounds__(MS_THREADS) bow_min_score_kernel(int nframes, 
 
 using namespace orbfe;
 
-#define BOW_TRY(expr)                                                                                        \
-    do {                                                                                                     \
-        cudaError_t e__ = (expr);                                                                            \
-        if (e__ != cudaSuccess)                                                                              \
-            return set_error(ORBFE_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-    } while (0)
-
 cudaError_t orbfe::vocab_alloc(OrbfeVocabulary *v, int nnodes, int nchild) {
     const size_t n = (size_t)nnodes;
     cudaError_t e = cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaMalloc((void **)&v->d_desc, n * 32);
-    if (e == cudaSuccess) e = cudaMalloc((void **)&v->d_live, n);
-    if (e == cudaSuccess) e = cudaMalloc((void **)&v->d_word_id, sizeof(int) * n);
-    if (e == cudaSuccess) e = cudaMalloc((void **)&v->d_weight, sizeof(double) * n);
-    if (e == cudaSuccess) e = cudaMalloc((void **)&v->d_child_ptr, sizeof(int) * (n + 1));
-    if (e == cudaSuccess) e = cudaMalloc((void **)&v->d_children, sizeof(int) * (size_t)std::max(nchild, 1));
+    if (e == cudaSuccess) e = v->mem.alloc(&v->d_desc, n * 32);
+    if (e == cudaSuccess) e = v->mem.alloc(&v->d_live, n);
+    if (e == cudaSuccess) e = v->mem.alloc(&v->d_word_id, n);
+    if (e == cudaSuccess) e = v->mem.alloc(&v->d_weight, n);
+    if (e == cudaSuccess) e = v->mem.alloc(&v->d_child_ptr, n + 1);
+    if (e == cudaSuccess) e = v->mem.alloc(&v->d_children, (size_t)std::max(nchild, 1));
     return e;
 }
 
@@ -554,8 +547,7 @@ extern "C" void orbfe_vocabulary_destroy(OrbfeVocabulary *v) {
     if (!v) return;
     cudaSetDevice(v->device);
     if (v->stream) cudaStreamDestroy(v->stream);
-    cudaFree(v->d_desc); cudaFree(v->d_live); cudaFree(v->d_child_ptr); cudaFree(v->d_children);
-    cudaFree(v->d_word_id); cudaFree(v->d_weight);
+    v->mem.release();
     v->stage.release();
     delete v;
 }
@@ -621,16 +613,16 @@ extern "C" int orbfe_vocabulary_export(OrbfeVocabulary *v, uint8_t *node_desc, i
                                        double *weight, int32_t *parent) {
     if (!v) return set_error(ORBFE_ERR_ARG, "NULL vocabulary");
     const size_t n = (size_t)v->nnodes;
-    BOW_TRY(cudaSetDevice(v->device));
-    BOW_TRY(cudaStreamSynchronize(v->stream));
-    if (node_desc) BOW_TRY(cudaMemcpy(node_desc, v->d_desc, n * 32, cudaMemcpyDeviceToHost));
-    if (word_id) BOW_TRY(cudaMemcpy(word_id, v->d_word_id, sizeof(int) * n, cudaMemcpyDeviceToHost));
-    if (weight) BOW_TRY(cudaMemcpy(weight, v->d_weight, sizeof(double) * n, cudaMemcpyDeviceToHost));
+    ORBFE_CUDA_TRY(cudaSetDevice(v->device));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(v->stream));
+    if (node_desc) ORBFE_CUDA_TRY(cudaMemcpy(node_desc, v->d_desc, n * 32, cudaMemcpyDeviceToHost));
+    if (word_id) ORBFE_CUDA_TRY(cudaMemcpy(word_id, v->d_word_id, sizeof(int) * n, cudaMemcpyDeviceToHost));
+    if (weight) ORBFE_CUDA_TRY(cudaMemcpy(weight, v->d_weight, sizeof(double) * n, cudaMemcpyDeviceToHost));
     std::vector<int32_t> ptr_tmp, ch_tmp;
     if (!child_ptr && parent) { ptr_tmp.resize(n + 1); child_ptr = ptr_tmp.data(); }
-    if (child_ptr) BOW_TRY(cudaMemcpy(child_ptr, v->d_child_ptr, sizeof(int) * (n + 1), cudaMemcpyDeviceToHost));
+    if (child_ptr) ORBFE_CUDA_TRY(cudaMemcpy(child_ptr, v->d_child_ptr, sizeof(int) * (n + 1), cudaMemcpyDeviceToHost));
     if (!children && parent) { ch_tmp.resize((size_t)v->nchild); children = ch_tmp.data(); }
-    if (children && v->nchild > 0) BOW_TRY(cudaMemcpy(children, v->d_children, sizeof(int) * (size_t)v->nchild, cudaMemcpyDeviceToHost));
+    if (children && v->nchild > 0) ORBFE_CUDA_TRY(cudaMemcpy(children, v->d_children, sizeof(int) * (size_t)v->nchild, cudaMemcpyDeviceToHost));
     if (parent) {
         std::fill(parent, parent + n, 0);
         for (size_t i = 0; i < n; i++)
@@ -644,12 +636,12 @@ extern "C" int orbfe_bow_descend_device(OrbfeVocabulary *v, const uint8_t *d_des
     if (!v || n < 0) return set_error(ORBFE_ERR_ARG, "bad arguments");
     if (n == 0) return ORBFE_OK;
     if (!d_desc || !d_leaf_out || !d_node_out) return set_error(ORBFE_ERR_ARG, "NULL argument");
-    BOW_TRY(cudaSetDevice(v->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(v->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : v->stream;
     bow_descend_kernel<<<(n + 7) / 8, 256, 0, s>>>(reinterpret_cast<const uint4 *>(v->d_desc), v->d_child_ptr, v->d_children,
                                                    reinterpret_cast<const uint4 *>(d_desc), n, v->depth - levelsup, d_leaf_out,
                                                    d_node_out);
-    BOW_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     return ORBFE_OK;
 }
 
@@ -663,11 +655,11 @@ extern "C" int orbfe_feature_vector_device(OrbfeVocabulary *v, int nframes, cons
         return set_error(ORBFE_ERR_UNSUPPORTED, "cap %d exceeds the %d features per frame the FeatureVector kernel sorts in shared memory",
                          cap, ORBFE_FV_MAX_CAP);
     if (nframes == 0) return ORBFE_OK;
-    BOW_TRY(cudaSetDevice(v->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(v->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : v->stream;
-    BOW_TRY((cudaError_t)launch_feature_vector(nframes, d_leaf, d_node, v->d_live, v->nnodes, d_counts, cap, d_fv_ids, d_fv_ptr,
+    ORBFE_CUDA_TRY((cudaError_t)launch_feature_vector(nframes, d_leaf, d_node, v->d_live, v->nnodes, d_counts, cap, d_fv_ids, d_fv_ptr,
                                                d_fv_items, d_fv_n, s));
-    BOW_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     return ORBFE_OK;
 }
 
@@ -679,14 +671,14 @@ extern "C" int orbfe_bow_vector_device(OrbfeVocabulary *v, int nframes, const in
         return set_error(ORBFE_ERR_UNSUPPORTED, "cap %d exceeds the %d features per frame the BowVector kernel sorts in shared memory",
                          cap, ORBFE_FV_MAX_CAP);
     if (nframes == 0) return ORBFE_OK;
-    BOW_TRY(cudaSetDevice(v->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(v->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : v->stream;
     size_t smem = 0;
-    BOW_TRY(fv_smem(bow_vector_kernel, cap, &smem));
+    ORBFE_CUDA_TRY(fv_smem(bow_vector_kernel, cap, &smem));
     const int accumulate = v->weighting == ORBFE_BOW_TF || v->weighting == ORBFE_BOW_TF_IDF;
     bow_vector_kernel<<<nframes, FV_THREADS, smem, s>>>(d_leaf, v->d_live, v->d_word_id, v->d_weight, v->nnodes, accumulate, v->norm,
                                                         d_counts, cap, d_bow_ids, d_bow_vals, d_bow_n);
-    BOW_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     return ORBFE_OK;
 }
 
@@ -696,16 +688,16 @@ extern "C" int orbfe_bow_descend(OrbfeVocabulary *v, const uint8_t *desc, int n,
     if (!desc || !leaf_out || !node_out) return set_error(ORBFE_ERR_ARG, "NULL argument");
     const size_t N = (size_t)n;
     std::lock_guard<std::mutex> lock(v->mu);
-    BOW_TRY(cudaSetDevice(v->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(v->device));
     size_t o_desc, o_leaf, o_node, total;
     if (int rc = v->stage.layout({{&o_desc, N * 32}, {&o_leaf, N * 4}, {&o_node, N * 4}}, &total)) return rc;
     unsigned char *H = v->stage.h, *D = v->stage.d;
     memcpy(H + o_desc, desc, N * 32);
-    BOW_TRY(cudaMemcpyAsync(D, H, o_leaf, cudaMemcpyHostToDevice, v->stream));
-    if (int rc = orbfe_bow_descend_device(v, D + o_desc, n, levelsup, (int32_t *)(D + o_leaf), (int32_t *)(D + o_node), v->stream))
+    if (int rc = v->stage.round_trip(v->stream, o_leaf, o_leaf, total, [&] {
+            return orbfe_bow_descend_device(v, D + o_desc, n, levelsup, (int32_t *)(D + o_leaf), (int32_t *)(D + o_node), v->stream);
+        }))
         return rc;
-    BOW_TRY(cudaMemcpyAsync(H + o_leaf, D + o_leaf, total - o_leaf, cudaMemcpyDeviceToHost, v->stream));
-    BOW_TRY(cudaStreamSynchronize(v->stream));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(v->stream));
     memcpy(leaf_out, H + o_leaf, N * 4);
     memcpy(node_out, H + o_node, N * 4);
     return ORBFE_OK;
@@ -726,7 +718,7 @@ extern "C" int orbfe_bow_transform(OrbfeVocabulary *v, const uint8_t *desc, int 
                                                 "kernels sort in shared memory", n, ORBFE_FV_MAX_CAP);
     const size_t N = (size_t)n;
     std::lock_guard<std::mutex> lock(v->mu);
-    BOW_TRY(cudaSetDevice(v->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(v->device));
     size_t o_desc, o_cnt, o_leaf, o_node, o_bid, o_bval, o_bn, o_fid, o_fptr, o_fitem, o_fn, total;
     if (int rc = v->stage.layout({{&o_desc, N * 32}, {&o_cnt, sizeof(int)}, {&o_leaf, N * 4}, {&o_node, N * 4}, {&o_bid, N * 4},
                                   {&o_bval, N * 8}, {&o_bn, sizeof(int)}, {&o_fid, N * 4}, {&o_fptr, (N + 1) * 4}, {&o_fitem, N * 4},
@@ -737,17 +729,19 @@ extern "C" int orbfe_bow_transform(OrbfeVocabulary *v, const uint8_t *desc, int 
     memcpy(H + o_desc, desc, N * 32);
     *(int *)(H + o_cnt) = n;
     cudaStream_t s = v->stream;
-    BOW_TRY(cudaMemcpyAsync(D, H, o_leaf, cudaMemcpyHostToDevice, s));
     const int *d_cnt = (const int *)(D + o_cnt);
     int32_t *d_leaf = (int32_t *)(D + o_leaf), *d_node = (int32_t *)(D + o_node);
-    int rc = orbfe_bow_descend_device(v, D + o_desc, n, levelsup, d_leaf, d_node, s);
-    if (!rc) rc = orbfe_bow_vector_device(v, 1, d_leaf, d_cnt, n, (int32_t *)(D + o_bid), (double *)(D + o_bval), (int *)(D + o_bn), s);
-    if (!rc)
-        rc = orbfe_feature_vector_device(v, 1, d_leaf, d_node, d_cnt, n, (int32_t *)(D + o_fid), (int32_t *)(D + o_fptr),
-                                         (int32_t *)(D + o_fitem), (int *)(D + o_fn), s);
-    if (rc) return rc;
-    BOW_TRY(cudaMemcpyAsync(H + o_bid, D + o_bid, total - o_bid, cudaMemcpyDeviceToHost, s));
-    BOW_TRY(cudaStreamSynchronize(s));
+    if (int rc = v->stage.round_trip(s, o_leaf, o_bid, total, [&] {
+            int rc = orbfe_bow_descend_device(v, D + o_desc, n, levelsup, d_leaf, d_node, s);
+            if (!rc)
+                rc = orbfe_bow_vector_device(v, 1, d_leaf, d_cnt, n, (int32_t *)(D + o_bid), (double *)(D + o_bval), (int *)(D + o_bn), s);
+            if (!rc)
+                rc = orbfe_feature_vector_device(v, 1, d_leaf, d_node, d_cnt, n, (int32_t *)(D + o_fid), (int32_t *)(D + o_fptr),
+                                                 (int32_t *)(D + o_fitem), (int *)(D + o_fn), s);
+            return rc;
+        }))
+        return rc;
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(s));
     // exactly the entries DBoW2's maps hold: the rows' padding stays in the block
     const int nw = *(const int *)(H + o_bn), nn = *(const int *)(H + o_fn);
     const int32_t *ptr = (const int32_t *)(H + o_fptr);
@@ -773,13 +767,13 @@ extern "C" int orbfe_bow_min_score_device(OrbfeVocabulary *v, int nqueries, int 
                          ORBFE_FV_MAX_CAP);
     if ((long long)nframes * cap >= (1ll << 31)) return set_error(ORBFE_ERR_ARG, "nframes * cap = %lld does not fit 31 bits", (long long)nframes * cap);
     if (nqueries == 0) return ORBFE_OK;
-    BOW_TRY(cudaSetDevice(v->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(v->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : v->stream;
     const size_t smem = (sizeof(double) + sizeof(int)) * (size_t)cap;
-    if (smem > 48 * 1024) BOW_TRY(cudaFuncSetAttribute(bow_min_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (smem > 48 * 1024) ORBFE_CUDA_TRY(cudaFuncSetAttribute(bow_min_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     bow_min_score_kernel<<<nqueries, MS_THREADS, smem, s>>>(nframes, cap, d_bow_ids, d_bow_vals, d_bow_n, d_query_row, d_cov_ptr, d_cov_row,
                                                             d_scores, d_min_score);
-    BOW_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     return ORBFE_OK;
 }
 
@@ -794,7 +788,7 @@ extern "C" int orbfe_bow_score(OrbfeVocabulary *v, int n1, const int32_t *ids1, 
     const int cap = std::max(std::max(n1, n2), 1);
     const size_t N = (size_t)cap;
     std::lock_guard<std::mutex> lock(v->mu);
-    BOW_TRY(cudaSetDevice(v->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(v->device));
     size_t o_ids, o_vals, o_hdr, o_score, o_min, total;
     if (int rc = v->stage.layout({{&o_ids, 2 * N * 4}, {&o_vals, 2 * N * 8}, {&o_hdr, 6 * sizeof(int)}, {&o_score, sizeof(double)},
                                   {&o_min, sizeof(float)}},
@@ -806,13 +800,13 @@ extern "C" int orbfe_bow_score(OrbfeVocabulary *v, int n1, const int32_t *ids1, 
     const int hdr[6] = {n1, n2, /* query row */ 0, /* cov_ptr */ 0, 1, /* cov_row */ 1};
     memcpy(H + o_hdr, hdr, sizeof(hdr));
     cudaStream_t s = v->stream;
-    BOW_TRY(cudaMemcpyAsync(D, H, o_score, cudaMemcpyHostToDevice, s));
     const int *d_hdr = (const int *)(D + o_hdr);
-    if (int rc = orbfe_bow_min_score_device(v, 1, 2, cap, (const int32_t *)(D + o_ids), (const double *)(D + o_vals), d_hdr, d_hdr + 2,
-                                            d_hdr + 3, d_hdr + 5, (double *)(D + o_score), (float *)(D + o_min), s))
+    if (int rc = v->stage.round_trip(s, o_score, o_score, total, [&] {
+            return orbfe_bow_min_score_device(v, 1, 2, cap, (const int32_t *)(D + o_ids), (const double *)(D + o_vals), d_hdr, d_hdr + 2,
+                                              d_hdr + 3, d_hdr + 5, (double *)(D + o_score), (float *)(D + o_min), s);
+        }))
         return rc;
-    BOW_TRY(cudaMemcpyAsync(H + o_score, D + o_score, sizeof(double), cudaMemcpyDeviceToHost, s));
-    BOW_TRY(cudaStreamSynchronize(s));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(s));
     memcpy(score_out, H + o_score, sizeof(double));
     return ORBFE_OK;
 }

@@ -59,12 +59,6 @@ NcclApi &nccl() {
     return a;
 }
 
-#define CU_TRY(expr)                                                                                                  \
-    do {                                                                                                              \
-        cudaError_t e__ = (expr);                                                                                     \
-        if (e__ != cudaSuccess)                                                                                       \
-            return set_error(ORBFE_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-    } while (0)
 #define NCCL_TRY(expr)                                                                                                \
     do {                                                                                                              \
         ncclResult_t r__ = (expr);                                                                                    \
@@ -106,7 +100,7 @@ extern "C" int orbfe_comm_create(const uint8_t id[ORBFE_COMM_ID_BYTES], int worl
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return set_error(ORBFE_ERR_NO_DEVICE, "no CUDA device"); }
     if (device < 0 || device >= ndev) return set_error(ORBFE_ERR_ARG, "device %d out of range", device);
     if (!nccl().ok) return set_error(ORBFE_ERR_UNSUPPORTED, "libnccl.so.2 could not be loaded");
-    CU_TRY(cudaSetDevice(device));
+    ORBFE_CUDA_TRY(cudaSetDevice(device));
     OrbfeComm *c = new OrbfeComm();
     c->world = world; c->rank = rank; c->device = device;
     ncclUniqueId u;
@@ -116,7 +110,7 @@ extern "C" int orbfe_comm_create(const uint8_t id[ORBFE_COMM_ID_BYTES], int worl
     cudaError_t e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
     if (e == cudaSuccess) e = cudaMalloc((void **)&c->d_token, 2 * sizeof(int));
     if (e == cudaSuccess) e = cudaMemset(c->d_token, 0, 2 * sizeof(int));
-    if (e != cudaSuccess) { nccl().CommDestroy(c->comm); delete c; return set_error(ORBFE_ERR_CUDA, "communicator setup failed: %s", cudaGetErrorString(e)); }
+    if (e != cudaSuccess) { orbfe_comm_destroy(c); return set_error(ORBFE_ERR_CUDA, "communicator setup failed: %s", cudaGetErrorString(e)); }
     *out = c;
     return ORBFE_OK;
 }
@@ -137,14 +131,14 @@ extern "C" int orbfe_comm_rank(const OrbfeComm *c) { return c ? c->rank : -1; }
 
 extern "C" int orbfe_comm_sync(OrbfeComm *c) {
     if (!c) return set_error(ORBFE_ERR_ARG, "c is NULL");
-    CU_TRY(cudaSetDevice(c->device));
-    CU_TRY(cudaStreamSynchronize(c->stream));
+    ORBFE_CUDA_TRY(cudaSetDevice(c->device));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(c->stream));
     return ORBFE_OK;
 }
 
 extern "C" int orbfe_comm_barrier(OrbfeComm *c, void *stream) {
     if (!c) return set_error(ORBFE_ERR_ARG, "c is NULL");
-    CU_TRY(cudaSetDevice(c->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(c->device));
     NCCL_TRY(nccl().AllReduce(c->d_token, c->d_token + 1, 1, ncclInt32, ncclSum, c->comm, stream ? (cudaStream_t)stream : c->stream));
     return ORBFE_OK;
 }
@@ -152,7 +146,7 @@ extern "C" int orbfe_comm_barrier(OrbfeComm *c, void *stream) {
 extern "C" int orbfe_comm_broadcast(OrbfeComm *c, void *d_buf, size_t bytes, int root, void *stream) {
     if (!c || !d_buf || root < 0 || root >= c->world) return set_error(ORBFE_ERR_ARG, "bad arguments");
     if (bytes == 0) return ORBFE_OK;
-    CU_TRY(cudaSetDevice(c->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(c->device));
     NCCL_TRY(nccl().Broadcast(d_buf, d_buf, bytes, ncclUint8, root, c->comm, stream ? (cudaStream_t)stream : c->stream));
     return ORBFE_OK;
 }
@@ -160,7 +154,7 @@ extern "C" int orbfe_comm_broadcast(OrbfeComm *c, void *d_buf, size_t bytes, int
 extern "C" int orbfe_comm_allgather(OrbfeComm *c, const void *d_send, void *d_recv, size_t bytes_per_rank, void *stream) {
     if (!c || !d_send || !d_recv) return set_error(ORBFE_ERR_ARG, "bad arguments");
     if (bytes_per_rank == 0) return ORBFE_OK;
-    CU_TRY(cudaSetDevice(c->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(c->device));
     NCCL_TRY(nccl().AllGather(d_send, d_recv, bytes_per_rank, ncclUint8, c->comm, stream ? (cudaStream_t)stream : c->stream));
     return ORBFE_OK;
 }
@@ -169,7 +163,7 @@ extern "C" int orbfe_allgather_desc(OrbfeComm *c, const OrbfeKeyPoint *d_kps, co
                                     OrbfeKeyPoint *d_all_kps, uint8_t *d_all_desc, int *d_all_counts, void *stream) {
     if (!c || !d_kps || !d_desc || !d_counts || !d_all_kps || !d_all_desc || !d_all_counts || cap < 1 || nslots < 1)
         return set_error(ORBFE_ERR_ARG, "bad arguments");
-    CU_TRY(cudaSetDevice(c->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(c->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : c->stream;
     const size_t n = (size_t)cap * nslots;
     NCCL_TRY(nccl().GroupStart());
@@ -216,7 +210,7 @@ extern "C" int orbfe_knn2_sweep_sharded(OrbfeComm *c, OrbfeMatcher *m, uint8_t *
                                         uint16_t *d_second_all, void *d_scratch, void *stream) {
     if (!c || !m || !d_query || nq < 1 || ngroups_total < 1 || group_size < 1 || !d_best_all || !d_best_idx_all || !d_second_all || !d_scratch)
         return set_error(ORBFE_ERR_ARG, "bad arguments");
-    CU_TRY(cudaSetDevice(c->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(c->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : c->stream;
     int lo, hi;
     orbfe_shard_range(ngroups_total, c->world, c->rank, &lo, &hi);
@@ -244,7 +238,7 @@ extern "C" int orbfe_knn2_sweep_sharded(OrbfeComm *c, OrbfeMatcher *m, uint8_t *
     NCCL_TRY(nccl().GroupEnd());
     NCCL_TRY(r1); NCCL_TRY(r2); NCCL_TRY(r3);
     unpad_results_kernel<<<296, 256, 0, s>>>(gb, gi, gs, c->world, gmax, ngroups_total, nq, d_best_all, d_best_idx_all, d_second_all);
-    CU_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     return ORBFE_OK;
 }
 
@@ -294,7 +288,7 @@ extern "C" int orbfe_rig_exchange_create(OrbfeComm *c, int cap, int nslots, Orbf
     if (!out) return set_error(ORBFE_ERR_ARG, "out is NULL");
     *out = nullptr;
     if (!c || cap < 1 || nslots < 1) return set_error(ORBFE_ERR_ARG, "bad arguments");
-    CU_TRY(cudaSetDevice(c->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(c->device));
     OrbfeRigExchange *x = new OrbfeRigExchange();
     x->c = c; x->cap = cap; x->nslots = nslots; x->world = c->world; x->rank = c->rank;
     const size_t n = (size_t)c->world * nslots * cap;
@@ -370,7 +364,7 @@ extern "C" int orbfe_extract_batch_device_exchange(OrbfeExtractor *ex, const uin
                                                    size_t frame_stride, int batch, OrbfeRigExchange *x, void *stream) {
     if (!ex || !x || !d_imgs) return set_error(ORBFE_ERR_ARG, "NULL argument");
     if (batch != x->nslots) return set_error(ORBFE_ERR_ARG, "batch %d != nslots %d of the exchange", batch, x->nslots);
-    CU_TRY(cudaSetDevice(x->c->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(x->c->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : x->c->stream;
     const unsigned epoch = x->epoch + 1;
     const int half = (int)(epoch & 1u);
@@ -415,7 +409,7 @@ extern "C" int orbfe_search_for_initialization_exchange(OrbfeMatcher *m, OrbfeRi
                                                         float max_y, int window, float nnratio, int check_orientation, int *d_match12,
                                                         int *d_nmatches, void *stream) {
     if (!m || !x) return set_error(ORBFE_ERR_ARG, "NULL argument");
-    CU_TRY(cudaSetDevice(x->c->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(x->c->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : x->c->stream;
     x->waited = x->epoch;
     uint8_t *hb = x->base + (size_t)(x->waited & 1u) * x->half_bytes;
@@ -434,23 +428,23 @@ extern "C" int orbfe_search_for_initialization_exchange(OrbfeMatcher *m, OrbfeRi
 
 extern "C" int orbfe_rig_exchange_wait(OrbfeRigExchange *x, void *stream) {
     if (!x) return set_error(ORBFE_ERR_ARG, "x is NULL");
-    CU_TRY(cudaSetDevice(x->c->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(x->c->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : x->c->stream;
     wait_flags_kernel<<<1, 32, 0, s>>>((unsigned *)(x->base + x->flags_off), x->world, x->epoch, x->d_err, 1);
-    CU_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     x->waited = x->epoch;
     return ORBFE_OK;
 }
 
 extern "C" int orbfe_rig_exchange_release(OrbfeRigExchange *x, void *stream) {
     if (!x) return set_error(ORBFE_ERR_ARG, "x is NULL");
-    CU_TRY(cudaSetDevice(x->c->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(x->c->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : x->c->stream;
     AckTargets t;
     t.n = x->world;
     for (int p = 0; p < x->world; p++) t.p[p] = (unsigned *)(x->peer_base[p] + x->flags_off) + ORBFE_MAX_RANKS + x->rank;
     publish_kernel<<<1, 32, 0, s>>>(t, x->waited);
-    CU_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     return ORBFE_OK;
 }
 
@@ -474,10 +468,10 @@ extern "C" int orbfe_rig_exchange_buffers_produced(OrbfeRigExchange *x, OrbfeKey
 
 extern "C" int orbfe_rig_exchange_check(OrbfeRigExchange *x, void *stream) {
     if (!x) return set_error(ORBFE_ERR_ARG, "x is NULL");
-    CU_TRY(cudaSetDevice(x->c->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(x->c->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : x->c->stream;
-    CU_TRY(cudaMemcpyAsync(x->h_err, x->d_err, sizeof(int), cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaStreamSynchronize(s));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(x->h_err, x->d_err, sizeof(int), cudaMemcpyDeviceToHost, s));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(s));
     if (*x->h_err) {
         const int code = *x->h_err;
         cudaMemsetAsync(x->d_err, 0, sizeof(int), s);

@@ -35,7 +35,6 @@
 #include "orbfe_internal.h"
 
 namespace orbfe {
-int set_error(int code, const char *fmt, ...);
 
 #define COVIS_TH 15              // KeyFrame.cc:372
 #define COVIS_MAX_CONN 2048      // the count and apply blocks hold a weight map in shared memory
@@ -488,22 +487,15 @@ __global__ void covis_lists_kernel(const int *__restrict__ slots, int which, int
 
 using namespace orbfe;
 
-#define COVIS_TRY(expr)                                                                                      \
-    do {                                                                                                     \
-        cudaError_t e__ = (expr);                                                                            \
-        if (e__ != cudaSuccess)                                                                              \
-            return set_error(ORBFE_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-    } while (0)
-
 struct OrbfeCovisGraph {
-    int device = 0, K = 0, C = 0, Cp = 1, P = 2, B = 0, Bp = 1, apply_grid = 1;
+    int K = 0, C = 0, Cp = 1, P = 2, B = 0, Bp = 1, apply_grid = 1;
     size_t count_smem = 0, apply_smem = 0, erase_smem = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t last = nullptr;   // the handle's most recent work: every call orders itself after it
     // host mirror of what only the synchronous calls change
     std::vector<uint8_t> live, id0;
     std::vector<unsigned long long> keys;
     std::unordered_set<unsigned long long> live_keys;
+    HandleStream hs;
+    DeviceBuffers mem;   // every device array below
     // device
     unsigned long long *key = nullptr;
     int *state = nullptr, *wn = nullptr, *wslot = nullptr, *ww = nullptr, *on = nullptr, *oslot = nullptr, *ow = nullptr, *named = nullptr;
@@ -514,27 +506,24 @@ struct OrbfeCovisGraph {
 
 extern "C" void orbfe_covis_destroy(OrbfeCovisGraph *g) {
     if (!g) return;
-    cudaSetDevice(g->device);
-    if (g->stream) cudaStreamSynchronize(g->stream);
-    void *ptrs[] = {g->key, g->state, g->wn, g->wslot, g->ww, g->on, g->oslot, g->ow, g->named, g->slots, g->pos, g->tmark, g->evcnt,
-                    g->efill, g->ebase, g->touched, g->cn, g->cslot, g->cw, g->fn, g->fslot, g->fw, g->ev_p, g->ev_w, g->flags};
-    for (void *p : ptrs) cudaFree(p);
-    if (g->last) cudaEventDestroy(g->last);
-    if (g->stream) cudaStreamDestroy(g->stream);
+    cudaSetDevice(g->hs.device);
+    if (g->hs.stream) cudaStreamSynchronize(g->hs.stream);
+    g->mem.release();
+    g->hs.destroy();
     delete g;
 }
 
 // every slot empty; the batch scratch in its between-batches state
 static int covis_reset(OrbfeCovisGraph *g, cudaStream_t s) {
     const size_t K = (size_t)g->K;
-    COVIS_TRY(cudaMemsetAsync(g->state, 0, sizeof(int) * K, s));
-    COVIS_TRY(cudaMemsetAsync(g->wn, 0, sizeof(int) * K, s));
-    COVIS_TRY(cudaMemsetAsync(g->on, 0, sizeof(int) * K, s));
-    COVIS_TRY(cudaMemsetAsync(g->named, 0, sizeof(int) * K, s));
-    COVIS_TRY(cudaMemsetAsync(g->pos, 0xFF, sizeof(int) * K, s));
-    COVIS_TRY(cudaMemsetAsync(g->tmark, 0, sizeof(int) * K, s));
-    COVIS_TRY(cudaMemsetAsync(g->evcnt, 0, sizeof(int) * K, s));
-    COVIS_TRY(cudaMemsetAsync(g->efill, 0, sizeof(int) * K, s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(g->state, 0, sizeof(int) * K, s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(g->wn, 0, sizeof(int) * K, s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(g->on, 0, sizeof(int) * K, s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(g->named, 0, sizeof(int) * K, s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(g->pos, 0xFF, sizeof(int) * K, s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(g->tmark, 0, sizeof(int) * K, s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(g->evcnt, 0, sizeof(int) * K, s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(g->efill, 0, sizeof(int) * K, s));
     g->live.assign(K, 0);
     g->id0.assign(K, 0);
     g->keys.assign(K, 0);
@@ -557,7 +546,6 @@ extern "C" int orbfe_covis_create(int device, int max_keyframes, int max_connect
         return set_error(ORBFE_ERR_NO_DEVICE, "orbfe_covis_create: no CUDA device %d", device);
     }
     OrbfeCovisGraph *g = new OrbfeCovisGraph();
-    g->device = device;
     g->K = max_keyframes;
     g->C = max_connections;
     g->Cp = pow2ge(max_connections);
@@ -568,46 +556,32 @@ extern "C" int orbfe_covis_create(int device, int max_keyframes, int max_connect
     g->apply_smem = sizeof(CvEnt) * (2 * (size_t)g->Cp + (size_t)g->Bp);
     g->erase_smem = sizeof(CvEnt) * (size_t)g->Cp;
     const size_t K = (size_t)g->K, KC = K * g->C, BC = (size_t)g->B * g->C;
-    bool ok = cudaSetDevice(device) == cudaSuccess && cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking) == cudaSuccess &&
-              cudaEventCreateWithFlags(&g->last, cudaEventDisableTiming) == cudaSuccess;
+    bool ok = g->hs.create(device) == cudaSuccess;
     int nsm = 1;
     ok = ok && cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device) == cudaSuccess;
     g->apply_grid = std::max(1, std::min(g->K, 4 * nsm));
     ok = ok && cudaFuncSetAttribute(covis_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->count_smem) == cudaSuccess &&
          cudaFuncSetAttribute(covis_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->apply_smem) == cudaSuccess &&
          cudaFuncSetAttribute(covis_erase_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->erase_smem) == cudaSuccess;
-#define COVIS_ALLOC(p, n) ok = ok && cudaMalloc((void **)&(p), sizeof(*(p)) * (n)) == cudaSuccess
-    COVIS_ALLOC(g->key, K); COVIS_ALLOC(g->state, K); COVIS_ALLOC(g->wn, K); COVIS_ALLOC(g->on, K); COVIS_ALLOC(g->named, K);
-    COVIS_ALLOC(g->wslot, KC); COVIS_ALLOC(g->ww, KC); COVIS_ALLOC(g->oslot, KC); COVIS_ALLOC(g->ow, KC);
+    const auto alloc = [&](auto **p, size_t n) { ok = ok && g->mem.alloc(p, n) == cudaSuccess; };
+    alloc(&g->key, K); alloc(&g->state, K); alloc(&g->wn, K); alloc(&g->on, K); alloc(&g->named, K);
+    alloc(&g->wslot, KC); alloc(&g->ww, KC); alloc(&g->oslot, KC); alloc(&g->ow, KC);
     // add stages 4 ints per keyframe; batches and lists name at most K slots
-    COVIS_ALLOC(g->slots, 4 * K); COVIS_ALLOC(g->pos, K); COVIS_ALLOC(g->tmark, K); COVIS_ALLOC(g->evcnt, K);
-    COVIS_ALLOC(g->efill, K); COVIS_ALLOC(g->ebase, K); COVIS_ALLOC(g->touched, K);
-    COVIS_ALLOC(g->cn, (size_t)g->B); COVIS_ALLOC(g->fn, (size_t)g->B); COVIS_ALLOC(g->cslot, BC); COVIS_ALLOC(g->cw, BC);
-    COVIS_ALLOC(g->fslot, BC); COVIS_ALLOC(g->fw, BC); COVIS_ALLOC(g->ev_p, BC); COVIS_ALLOC(g->ev_w, BC);
-    COVIS_ALLOC(g->flags, (size_t)F_COUNT);
-#undef COVIS_ALLOC
+    alloc(&g->slots, 4 * K); alloc(&g->pos, K); alloc(&g->tmark, K); alloc(&g->evcnt, K);
+    alloc(&g->efill, K); alloc(&g->ebase, K); alloc(&g->touched, K);
+    alloc(&g->cn, (size_t)g->B); alloc(&g->fn, (size_t)g->B); alloc(&g->cslot, BC); alloc(&g->cw, BC);
+    alloc(&g->fslot, BC); alloc(&g->fw, BC); alloc(&g->ev_p, BC); alloc(&g->ev_w, BC);
+    alloc(&g->flags, (size_t)F_COUNT);
     ok = ok && cudaMemset(g->flags, 0, sizeof(int) * F_COUNT) == cudaSuccess && cudaMemset(g->key, 0, sizeof(unsigned long long) * K) == cudaSuccess;
     if (!ok) {
         const int rc = set_error(ORBFE_ERR_CUDA, "orbfe_covis_create: allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
         orbfe_covis_destroy(g);
         return rc;
     }
-    int rc = covis_reset(g, g->stream);
-    if (!rc && cudaStreamSynchronize(g->stream) != cudaSuccess) rc = set_error(ORBFE_ERR_CUDA, "orbfe_covis_create: reset failed");
+    int rc = covis_reset(g, g->hs.stream);
+    if (!rc && cudaStreamSynchronize(g->hs.stream) != cudaSuccess) rc = set_error(ORBFE_ERR_CUDA, "orbfe_covis_create: reset failed");
     if (rc) { orbfe_covis_destroy(g); return rc; }
     *out = g;
-    return ORBFE_OK;
-}
-
-static int covis_enter(OrbfeCovisGraph *g, cudaStream_t s) {
-    COVIS_TRY(cudaSetDevice(g->device));
-    COVIS_TRY(cudaStreamWaitEvent(s, g->last, 0));
-    return ORBFE_OK;
-}
-static int covis_leave(OrbfeCovisGraph *g, cudaStream_t s, bool sync) {
-    COVIS_TRY(cudaGetLastError());
-    COVIS_TRY(cudaEventRecord(g->last, s));
-    if (sync) COVIS_TRY(cudaStreamSynchronize(s));
     return ORBFE_OK;
 }
 
@@ -627,13 +601,13 @@ extern "C" int orbfe_covis_add(OrbfeCovisGraph *g, int n, const int32_t *slots, 
         if (g->live_keys.count(keys[i]) || !new_keys.insert(keys[i]).second)
             return set_error(ORBFE_ERR_ARG, "orbfe_covis_add: key of slot %d equals a live keyframe's key", s);
     }
-    cudaStream_t st = g->stream;
-    int rc = covis_enter(g, st);
+    cudaStream_t st = g->hs.stream;
+    int rc = g->hs.enter(st);
     if (rc) return rc;
     // a retired slot that a weight map still names is the reference's stale pointer: it cannot become a new keyframe
     std::vector<int> named((size_t)g->K);
-    COVIS_TRY(cudaMemcpyAsync(named.data(), g->named, sizeof(int) * named.size(), cudaMemcpyDeviceToHost, st));
-    COVIS_TRY(cudaStreamSynchronize(st));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(named.data(), g->named, sizeof(int) * named.size(), cudaMemcpyDeviceToHost, st));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(st));
     for (int i = 0; i < n; i++)
         if (named[slots[i]] != 0)
             return set_error(ORBFE_ERR_ARG, "orbfe_covis_add: retired slot %d is still named by %d weight maps", slots[i], named[slots[i]]);
@@ -644,9 +618,9 @@ extern "C" int orbfe_covis_add(OrbfeCovisGraph *g, int n, const int32_t *slots, 
         rows[4 * i + 2] = (int)(uint32_t)keys[i];
         rows[4 * i + 3] = (int)(uint32_t)(keys[i] >> 32);
     }
-    COVIS_TRY(cudaMemcpyAsync(g->slots, rows.data(), sizeof(int) * rows.size(), cudaMemcpyHostToDevice, st));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(g->slots, rows.data(), sizeof(int) * rows.size(), cudaMemcpyHostToDevice, st));
     covis_add_kernel<<<(n + 127) / 128, 128, 0, st>>>(n, g->slots, g->key, g->state, g->wn, g->on);
-    if ((rc = covis_leave(g, st, true))) return rc;
+    if ((rc = g->hs.leave(st, true))) return rc;
     for (int i = 0; i < n; i++) {
         g->live[slots[i]] = 1;
         g->id0[slots[i]] = ids[i] == 0;
@@ -675,10 +649,10 @@ extern "C" int orbfe_covis_update_connections_device(OrbfeCovisGraph *g, int n, 
     for (int i = 0; i < n; i++)
         if (slots[i] >= g->K || !g->live[slots[i]])
             return set_error(ORBFE_ERR_ARG, "orbfe_covis_update_connections_device: slot %d is not a live keyframe", slots[i]);
-    cudaStream_t st = stream ? (cudaStream_t)stream : g->stream;
-    int rc = covis_enter(g, st);
+    cudaStream_t st = g->hs.pick(stream);
+    int rc = g->hs.enter(st);
     if (rc) return rc;
-    COVIS_TRY(cudaMemcpyAsync(g->slots, slots, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(g->slots, slots, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
     covis_count_kernel<<<n, COVIS_COUNT_BLOCK, g->count_smem, st>>>(g->slots, g->C, g->Cp, g->P, d_kf_mp, d_counts, nframes, cap,
                                                                   d_group_ptr, d_obs, npoints, nobs, g->K, g->state, g->key, g->cn, g->cslot,
                                                                   g->cw, g->fn, g->fslot, g->fw, g->flags);
@@ -687,19 +661,19 @@ extern "C" int orbfe_covis_update_connections_device(OrbfeCovisGraph *g, int n, 
     covis_apply_kernel<<<g->apply_grid, COVIS_APPLY_BLOCK, g->apply_smem, st>>>(
         g->slots, g->C, g->Cp, g->Bp, g->cn, g->cslot, g->cw, g->fn, g->fslot, g->fw, g->key, g->state, g->wn, g->wslot, g->ww, g->on,
         g->oslot, g->ow, g->named, g->pos, g->tmark, g->evcnt, g->efill, g->ebase, g->touched, g->ev_p, g->ev_w, g->flags);
-    return covis_leave(g, st, false);
+    return g->hs.leave(st, false);
 }
 
 extern "C" int orbfe_covis_erase(OrbfeCovisGraph *g, int slot) {
     if (!g || slot < 0 || slot >= g->K) return set_error(ORBFE_ERR_ARG, "orbfe_covis_erase: bad arguments");
     if (!g->live[slot] || g->id0[slot]) return ORBFE_OK;   // SetBadFlag of mnId == 0 returns at once (KeyFrame.cc:501)
-    cudaStream_t st = g->stream;
-    int rc = covis_enter(g, st);
+    cudaStream_t st = g->hs.stream;
+    int rc = g->hs.enter(st);
     if (rc) return rc;
     covis_erase_kernel<<<g->C, COVIS_APPLY_BLOCK, g->erase_smem, st>>>(slot, g->C, g->key, g->wn, g->wslot, g->ww, g->on, g->oslot, g->ow,
                                                                       g->named);
     covis_retire_kernel<<<1, 1, 0, st>>>(slot, g->state, g->wn, g->on);
-    if ((rc = covis_leave(g, st, true))) return rc;
+    if ((rc = g->hs.leave(st, true))) return rc;
     g->live[slot] = 0;
     g->live_keys.erase(g->keys[slot]);
     return ORBFE_OK;
@@ -707,10 +681,10 @@ extern "C" int orbfe_covis_erase(OrbfeCovisGraph *g, int slot) {
 
 extern "C" int orbfe_covis_clear(OrbfeCovisGraph *g) {
     if (!g) return set_error(ORBFE_ERR_ARG, "orbfe_covis_clear: bad arguments");
-    int rc = covis_enter(g, g->stream);
+    int rc = g->hs.enter(g->hs.stream);
     if (rc) return rc;
-    if ((rc = covis_reset(g, g->stream))) return rc;
-    return covis_leave(g, g->stream, true);
+    if ((rc = covis_reset(g, g->hs.stream))) return rc;
+    return g->hs.leave(g->hs.stream, true);
 }
 
 extern "C" int orbfe_covis_lists_device(OrbfeCovisGraph *g, int which, int n, const int32_t *slots, int nbest, int32_t *d_ptr,
@@ -724,24 +698,24 @@ extern "C" int orbfe_covis_lists_device(OrbfeCovisGraph *g, int which, int n, co
     for (int i = 0; i < n; i++)
         if (slots[i] >= g->K) return set_error(ORBFE_ERR_ARG, "orbfe_covis_lists_device: slot %d out of range", slots[i]);
     const int limit = which == 0 && nbest > 0 ? std::min(nbest, g->C) : g->C;
-    cudaStream_t st = stream ? (cudaStream_t)stream : g->stream;
-    int rc = covis_enter(g, st);
+    cudaStream_t st = g->hs.pick(stream);
+    int rc = g->hs.enter(st);
     if (rc) return rc;
-    COVIS_TRY(cudaMemcpyAsync(g->slots, slots, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(g->slots, slots, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
     covis_lens_kernel<<<1, 1024, 0, st>>>(n, g->slots, which, limit, g->wn, g->on, d_ptr);
     covis_lists_kernel<<<n, 128, 0, st>>>(g->slots, which, g->C, d_ptr, g->wslot, g->ww, g->oslot, g->ow, g->state, d_list, d_weights);
-    return covis_leave(g, st, false);
+    return g->hs.leave(st, false);
 }
 
 extern "C" int orbfe_covis_sync(OrbfeCovisGraph *g) {
     if (!g) return set_error(ORBFE_ERR_ARG, "orbfe_covis_sync: bad arguments");
-    cudaStream_t st = g->stream;
-    int rc = covis_enter(g, st);
+    cudaStream_t st = g->hs.stream;
+    int rc = g->hs.enter(st);
     if (rc) return rc;
     int err = 0;
-    COVIS_TRY(cudaMemcpyAsync(&err, g->flags + F_ERR, sizeof(int), cudaMemcpyDeviceToHost, st));
-    COVIS_TRY(cudaMemsetAsync(g->flags + F_ERR, 0, sizeof(int), st));
-    if ((rc = covis_leave(g, st, true))) return rc;
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(&err, g->flags + F_ERR, sizeof(int), cudaMemcpyDeviceToHost, st));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(g->flags + F_ERR, 0, sizeof(int), st));
+    if ((rc = g->hs.leave(st, true))) return rc;
     if (err == ORBFE_ERR_ARG)
         return set_error(ORBFE_ERR_ARG, "orbfe_covis_sync: an update batch was rejected: a point index, group pointer or observation was "
                          "out of range or named a slot that is not live");

@@ -43,7 +43,6 @@
 #include "orbfe_internal.h"
 
 namespace orbfe {
-int set_error(int code, const char *fmt, ...);
 int vocab_device(const OrbfeVocabulary *v);
 int vocab_nwords(const OrbfeVocabulary *v);
 
@@ -430,18 +429,11 @@ __global__ void __launch_bounds__(KFDB_BLOCK) kfdb_select_kernel(int loop, unsig
 
 using namespace orbfe;
 
-#define KFDB_TRY(expr)                                                                                       \
-    do {                                                                                                     \
-        cudaError_t e__ = (expr);                                                                            \
-        if (e__ != cudaSuccess)                                                                              \
-            return set_error(ORBFE_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-    } while (0)
-
 struct OrbfeKeyFrameDB {
-    int device = 0, nwords = 0, K = 0, sortcap = 1, Q = 1;   // Q: rows of per-query state (max_queries)
+    int nwords = 0, K = 0, sortcap = 1, Q = 1;   // Q: rows of per-query state (max_queries)
     long long P = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t last = nullptr;   // the handle's most recent work: every call orders itself after it
+    HandleStream hs;
+    DeviceBuffers mem;            // every device array below
     // host side: allocation only
     std::vector<int> begin, len;   // store rows of each slot; len -1 = empty
     std::vector<std::vector<int>> nodes;
@@ -469,15 +461,10 @@ struct OrbfeKeyFrameDB {
 
 extern "C" void orbfe_kfdb_destroy(OrbfeKeyFrameDB *db) {
     if (!db) return;
-    cudaSetDevice(db->device);
-    if (db->stream) cudaStreamSynchronize(db->stream);
-    void *ptrs[] = {db->s_id[0], db->s_id[1], db->s_node[0], db->s_node[1], db->s_val[0], db->s_val[1], db->n_slot, db->n_next, db->n_prev,
-                    db->w_head, db->w_tail, db->range, db->covn, db->cov, db->touched, db->list, db->best, db->info, db->moves, db->covrows,
-                    db->seqs, db->conn, db->state, db->keys, db->firstpos, db->lscore, db->rscore, db->scored, db->acc, db->q_ids, db->q_conn,
-                    db->o_cand, db->o_words, db->o_n, db->q_vals, db->o_score, db->a_info};
-    for (void *p : ptrs) cudaFree(p);
-    if (db->last) cudaEventDestroy(db->last);
-    if (db->stream) cudaStreamDestroy(db->stream);
+    cudaSetDevice(db->hs.device);
+    if (db->hs.stream) cudaStreamSynchronize(db->hs.stream);
+    db->mem.release();
+    db->hs.destroy();
     delete db;
 }
 
@@ -488,14 +475,14 @@ static int kfdb_reset(OrbfeKeyFrameDB *db) {
     db->free_nodes.resize((size_t)db->P);
     for (long long i = 0; i < db->P; i++) db->free_nodes[(size_t)i] = (int)(db->P - 1 - i);   // pops 0, 1, 2, ...
     db->top = db->live = 0;
-    cudaStream_t s = db->stream;
-    KFDB_TRY(cudaMemsetAsync(db->w_head, 0xFF, sizeof(int) * (size_t)db->nwords, s));
-    KFDB_TRY(cudaMemsetAsync(db->w_tail, 0xFF, sizeof(int) * (size_t)db->nwords, s));
+    cudaStream_t s = db->hs.stream;
+    ORBFE_CUDA_TRY(cudaMemsetAsync(db->w_head, 0xFF, sizeof(int) * (size_t)db->nwords, s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(db->w_tail, 0xFF, sizeof(int) * (size_t)db->nwords, s));
     std::vector<int> r(2 * (size_t)db->K);
     for (int k = 0; k < db->K; k++) { r[2 * k] = 0; r[2 * k + 1] = -1; }
-    KFDB_TRY(cudaMemcpyAsync(db->range, r.data(), sizeof(int) * r.size(), cudaMemcpyHostToDevice, s));
-    KFDB_TRY(cudaMemsetAsync(db->covn, 0, sizeof(int) * (size_t)db->K, s));
-    KFDB_TRY(cudaStreamSynchronize(s));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(db->range, r.data(), sizeof(int) * r.size(), cudaMemcpyHostToDevice, s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(db->covn, 0, sizeof(int) * (size_t)db->K, s));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(s));
     return ORBFE_OK;
 }
 
@@ -510,7 +497,6 @@ extern "C" int orbfe_kfdb_create_batched(OrbfeVocabulary *v, int max_keyframes, 
         return set_error(ORBFE_ERR_ARG, "bad arguments (1 <= max_keyframes <= 2^24, 1 <= max_postings < 2^31, 1 <= max_queries <= %d)",
                          KFDB_MAX_QUERIES);
     OrbfeKeyFrameDB *db = new OrbfeKeyFrameDB();
-    db->device = vocab_device(v);
     db->nwords = std::max(vocab_nwords(v), 1);
     db->K = max_keyframes;
     db->P = max_postings;
@@ -518,22 +504,20 @@ extern "C" int orbfe_kfdb_create_batched(OrbfeVocabulary *v, int max_keyframes, 
     while (db->sortcap < db->K) db->sortcap <<= 1;
     const size_t K = (size_t)db->K, P = (size_t)db->P, W = (size_t)db->nwords, S = (size_t)db->sortcap, QK = (size_t)db->Q * K,
                  QS = (size_t)db->Q * S;
-    bool ok = cudaSetDevice(db->device) == cudaSuccess && cudaStreamCreateWithFlags(&db->stream, cudaStreamNonBlocking) == cudaSuccess &&
-              cudaEventCreateWithFlags(&db->last, cudaEventDisableTiming) == cudaSuccess;
-#define KFDB_ALLOC(p, n) ok = ok && cudaMalloc((void **)&(p), sizeof(*(p)) * (n)) == cudaSuccess
-    for (int h = 0; h < 2; h++) { KFDB_ALLOC(db->s_id[h], P); KFDB_ALLOC(db->s_node[h], P); KFDB_ALLOC(db->s_val[h], P); }
-    KFDB_ALLOC(db->n_slot, P); KFDB_ALLOC(db->n_next, P); KFDB_ALLOC(db->n_prev, P);
-    KFDB_ALLOC(db->w_head, W); KFDB_ALLOC(db->w_tail, W);
-    KFDB_ALLOC(db->range, 2 * K); KFDB_ALLOC(db->covn, K); KFDB_ALLOC(db->cov, K * KFDB_COVIS); KFDB_ALLOC(db->moves, 3 * K);
-    KFDB_ALLOC(db->covrows, K * (2 + KFDB_COVIS)); KFDB_ALLOC(db->seqs, K); KFDB_ALLOC(db->lscore, K); KFDB_ALLOC(db->rscore, K);
+    bool ok = db->hs.create(vocab_device(v)) == cudaSuccess;
+    const auto alloc = [&](auto **p, size_t n) { ok = ok && db->mem.alloc(p, n) == cudaSuccess; };
+    for (int h = 0; h < 2; h++) { alloc(&db->s_id[h], P); alloc(&db->s_node[h], P); alloc(&db->s_val[h], P); }
+    alloc(&db->n_slot, P); alloc(&db->n_next, P); alloc(&db->n_prev, P);
+    alloc(&db->w_head, W); alloc(&db->w_tail, W);
+    alloc(&db->range, 2 * K); alloc(&db->covn, K); alloc(&db->cov, K * KFDB_COVIS); alloc(&db->moves, 3 * K);
+    alloc(&db->covrows, K * (2 + KFDB_COVIS)); alloc(&db->seqs, K); alloc(&db->lscore, K); alloc(&db->rscore, K);
     // per-query rows (include/orbfe_bow.h states their size)
-    KFDB_ALLOC(db->touched, QK); KFDB_ALLOC(db->list, QS); KFDB_ALLOC(db->best, QK); KFDB_ALLOC(db->info, 4 * (size_t)db->Q);
-    KFDB_ALLOC(db->conn, QK); KFDB_ALLOC(db->state, QK); KFDB_ALLOC(db->keys, QS); KFDB_ALLOC(db->firstpos, QK);
-    KFDB_ALLOC(db->scored, QK); KFDB_ALLOC(db->acc, QK);
-    KFDB_ALLOC(db->q_ids, KFDB_MAX_NQ); KFDB_ALLOC(db->q_vals, KFDB_MAX_NQ); KFDB_ALLOC(db->q_conn, K);
-    KFDB_ALLOC(db->o_cand, K); KFDB_ALLOC(db->o_words, K); KFDB_ALLOC(db->o_score, K); KFDB_ALLOC(db->o_n, 1);
-    KFDB_ALLOC(db->a_info, K + 1);
-#undef KFDB_ALLOC
+    alloc(&db->touched, QK); alloc(&db->list, QS); alloc(&db->best, QK); alloc(&db->info, 4 * (size_t)db->Q);
+    alloc(&db->conn, QK); alloc(&db->state, QK); alloc(&db->keys, QS); alloc(&db->firstpos, QK);
+    alloc(&db->scored, QK); alloc(&db->acc, QK);
+    alloc(&db->q_ids, KFDB_MAX_NQ); alloc(&db->q_vals, KFDB_MAX_NQ); alloc(&db->q_conn, K);
+    alloc(&db->o_cand, K); alloc(&db->o_words, K); alloc(&db->o_score, K); alloc(&db->o_n, 1);
+    alloc(&db->a_info, K + 1);
     ok = ok && cudaMemset(db->conn, 0, sizeof(unsigned) * QK) == cudaSuccess && cudaMemset(db->state, 0, sizeof(unsigned long long) * QK) == cudaSuccess &&
          cudaMemset(db->scored, 0, sizeof(unsigned long long) * QK) == cudaSuccess &&
          cudaMemset(db->firstpos, 0xFF, sizeof(unsigned long long) * QK) == cudaSuccess;
@@ -550,19 +534,6 @@ extern "C" int orbfe_kfdb_create_batched(OrbfeVocabulary *v, int max_keyframes, 
 
 extern "C" int orbfe_kfdb_create(OrbfeVocabulary *v, int max_keyframes, long long max_postings, OrbfeKeyFrameDB **out) {
     return orbfe_kfdb_create_batched(v, max_keyframes, max_postings, 1, out);
-}
-
-// order the handle's stream after the handle's previous work (which may have been enqueued on another stream)
-static int kfdb_enter(OrbfeKeyFrameDB *db, cudaStream_t s) {
-    KFDB_TRY(cudaSetDevice(db->device));
-    KFDB_TRY(cudaStreamWaitEvent(s, db->last, 0));
-    return ORBFE_OK;
-}
-static int kfdb_leave(OrbfeKeyFrameDB *db, cudaStream_t s, bool sync) {
-    KFDB_TRY(cudaGetLastError());
-    KFDB_TRY(cudaEventRecord(db->last, s));
-    if (sync) KFDB_TRY(cudaStreamSynchronize(s));
-    return ORBFE_OK;
 }
 
 // move every live slot's rows to the front of the other half of the store
@@ -582,16 +553,16 @@ static int kfdb_compact(OrbfeKeyFrameDB *db) {
         r[2 * k] = db->len[k] >= 0 ? db->begin[k] : 0;
         r[2 * k + 1] = db->len[k] >= 0 ? db->begin[k] + db->len[k] : -1;
     }
-    cudaStream_t s = db->stream;
+    cudaStream_t s = db->hs.stream;
     const int o = db->cur, n = 1 - db->cur;
     const int nmove = (int)order.size();
     if (nmove > 0) {
-        KFDB_TRY(cudaMemcpyAsync(db->moves, moves.data(), sizeof(int) * moves.size(), cudaMemcpyHostToDevice, s));
+        ORBFE_CUDA_TRY(cudaMemcpyAsync(db->moves, moves.data(), sizeof(int) * moves.size(), cudaMemcpyHostToDevice, s));
         kfdb_compact_kernel<<<std::min(nmove, 1024), 256, 0, s>>>(db->moves, nmove, db->s_id[o], db->s_val[o], db->s_node[o], db->s_id[n],
                                                                   db->s_val[n], db->s_node[n]);
     }
-    KFDB_TRY(cudaMemcpyAsync(db->range, r.data(), sizeof(int) * r.size(), cudaMemcpyHostToDevice, s));
-    KFDB_TRY(cudaStreamSynchronize(s));   // `moves` / `r` are host locals
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(db->range, r.data(), sizeof(int) * r.size(), cudaMemcpyHostToDevice, s));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(s));   // `moves` / `r` are host locals
     db->cur = n;
     db->top = pos;
     return ORBFE_OK;
@@ -606,22 +577,22 @@ extern "C" int orbfe_kfdb_add(OrbfeKeyFrameDB *db, int slot, int nw, const int32
     if (db->len[slot] >= 0) return set_error(ORBFE_ERR_ARG, "slot %d is occupied", slot);
     if (db->live + nw > db->P)
         return set_error(ORBFE_ERR_CAPACITY, "%lld postings + %d exceed max_postings %lld", db->live, nw, db->P);
-    cudaStream_t s = db->stream;
-    int rc = kfdb_enter(db, s);
+    cudaStream_t s = db->hs.stream;
+    int rc = db->hs.enter(s);
     if (rc) return rc;
     if (db->top + nw > db->P && (rc = kfdb_compact(db))) return rc;
     std::vector<int> nodes(nw);
     for (int i = 0; i < nw; i++) { nodes[i] = db->free_nodes.back(); db->free_nodes.pop_back(); }
     const int base = (int)db->top, c = db->cur;
     if (nw > 0) {
-        KFDB_TRY(cudaMemcpyAsync(db->s_id[c] + base, ids, sizeof(int) * nw, cudaMemcpyHostToDevice, s));
-        KFDB_TRY(cudaMemcpyAsync(db->s_val[c] + base, vals, sizeof(double) * nw, cudaMemcpyHostToDevice, s));
-        KFDB_TRY(cudaMemcpyAsync(db->s_node[c] + base, nodes.data(), sizeof(int) * nw, cudaMemcpyHostToDevice, s));
+        ORBFE_CUDA_TRY(cudaMemcpyAsync(db->s_id[c] + base, ids, sizeof(int) * nw, cudaMemcpyHostToDevice, s));
+        ORBFE_CUDA_TRY(cudaMemcpyAsync(db->s_val[c] + base, vals, sizeof(double) * nw, cudaMemcpyHostToDevice, s));
+        ORBFE_CUDA_TRY(cudaMemcpyAsync(db->s_node[c] + base, nodes.data(), sizeof(int) * nw, cudaMemcpyHostToDevice, s));
     }
     kfdb_link_kernel<<<(std::max(nw, 1) + 255) / 256, 256, 0, s>>>(slot, base, nw, ++db->seq, db->s_id[c], db->s_node[c], db->n_slot, db->n_next,
                                                                    db->n_prev, db->w_head, db->w_tail, db->range, db->seqs, db->lscore,
                                                                    db->rscore);
-    if ((rc = kfdb_leave(db, s, true))) return rc;
+    if ((rc = db->hs.leave(s, true))) return rc;
     db->begin[slot] = base;
     db->len[slot] = nw;
     db->nodes[slot].swap(nodes);
@@ -647,16 +618,16 @@ extern "C" int orbfe_kfdb_add_device(OrbfeKeyFrameDB *db, int n, const int32_t *
         if (db->len[slots[i]] >= 0) return set_error(ORBFE_ERR_ARG, "slot %d is occupied", slots[i]);
     }
     // the rows are checked on the device, after the work that wrote them; their word counts are the one readback
-    cudaStream_t s = stream ? (cudaStream_t)stream : db->stream;
-    int rc = kfdb_enter(db, s);
+    cudaStream_t s = db->hs.pick(stream);
+    int rc = db->hs.enter(s);
     if (rc) return rc;
-    KFDB_TRY(cudaMemcpyAsync(db->moves, frames, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, s));
-    KFDB_TRY(cudaMemsetAsync(db->a_info, 0, sizeof(int), s));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(db->moves, frames, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(db->a_info, 0, sizeof(int), s));
     kfdb_check_rows_kernel<<<std::min(n, 1024), 256, 0, s>>>(db->moves, n, cap, db->nwords, d_bow_n, d_bow_ids, db->a_info);
-    KFDB_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     std::vector<int> info((size_t)n + 1);
-    KFDB_TRY(cudaMemcpyAsync(info.data(), db->a_info, sizeof(int) * info.size(), cudaMemcpyDeviceToHost, s));
-    KFDB_TRY(cudaStreamSynchronize(s));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(info.data(), db->a_info, sizeof(int) * info.size(), cudaMemcpyDeviceToHost, s));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(s));
     if (info[0])
         return set_error(ORBFE_ERR_ARG, "a BowVector row has a word count outside 0 .. %d, or word ids that are not strictly ascending below %d",
                          cap, db->nwords);
@@ -665,7 +636,7 @@ extern "C" int orbfe_kfdb_add_device(OrbfeKeyFrameDB *db, int n, const int32_t *
     if (db->live + total > db->P)
         return set_error(ORBFE_ERR_CAPACITY, "%lld postings + %lld exceed max_postings %lld", db->live, total, db->P);
     // `s` has drained: the handle's earlier work and the rows are complete, the rest runs on the handle's stream
-    cudaStream_t hs = db->stream;
+    cudaStream_t hs = db->hs.stream;
     if (db->top + total > db->P && (rc = kfdb_compact(db))) return rc;
     const int c = db->cur, top = (int)db->top;
     std::vector<int> rows(3 * (size_t)n), nodes((size_t)total);
@@ -675,8 +646,8 @@ extern "C" int orbfe_kfdb_add_device(OrbfeKeyFrameDB *db, int n, const int32_t *
         rows[3 * i + 2] = info[1 + i];
         for (int k = 0; k < info[1 + i]; k++, pos++) { nodes[pos] = db->free_nodes.back(); db->free_nodes.pop_back(); }
     }
-    KFDB_TRY(cudaMemcpyAsync(db->moves, rows.data(), sizeof(int) * rows.size(), cudaMemcpyHostToDevice, hs));
-    if (total > 0) KFDB_TRY(cudaMemcpyAsync(db->s_node[c] + top, nodes.data(), sizeof(int) * nodes.size(), cudaMemcpyHostToDevice, hs));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(db->moves, rows.data(), sizeof(int) * rows.size(), cudaMemcpyHostToDevice, hs));
+    if (total > 0) ORBFE_CUDA_TRY(cudaMemcpyAsync(db->s_node[c] + top, nodes.data(), sizeof(int) * nodes.size(), cudaMemcpyHostToDevice, hs));
     kfdb_gather_kernel<<<std::min(n, 1024), 256, 0, hs>>>(db->moves, n, cap, d_bow_ids, d_bow_vals, db->s_id[c], db->s_val[c]);
     // one keyframe after the other: two keyframes may share a word, and every word's list is in add order
     for (int i = 0; i < n; i++) {
@@ -685,7 +656,7 @@ extern "C" int orbfe_kfdb_add_device(OrbfeKeyFrameDB *db, int n, const int32_t *
                                                                         db->n_slot, db->n_next, db->n_prev, db->w_head, db->w_tail,
                                                                         db->range, db->seqs, db->lscore, db->rscore);
     }
-    if ((rc = kfdb_leave(db, hs, true))) return rc;
+    if ((rc = db->hs.leave(hs, true))) return rc;
     for (int i = 0, pos = 0; i < n; i++) {
         const int sl = slots[i], nw = rows[3 * i + 2];
         db->begin[sl] = rows[3 * i + 1];
@@ -702,13 +673,13 @@ extern "C" int orbfe_kfdb_erase(OrbfeKeyFrameDB *db, int slot) {
     if (!db || slot < 0) return set_error(ORBFE_ERR_ARG, "bad arguments");
     if (slot >= db->K) return set_error(ORBFE_ERR_ARG, "slot %d out of range (max_keyframes %d)", slot, db->K);
     if (db->len[slot] < 0) return ORBFE_OK;   // erase of a keyframe that is not in the database: nothing to unlink
-    cudaStream_t s = db->stream;
-    int rc = kfdb_enter(db, s);
+    cudaStream_t s = db->hs.stream;
+    int rc = db->hs.enter(s);
     if (rc) return rc;
     const int nw = db->len[slot];
     kfdb_unlink_kernel<<<(std::max(nw, 1) + 255) / 256, 256, 0, s>>>(slot, db->begin[slot], nw, db->s_id[db->cur], db->s_node[db->cur], db->n_next,
                                                                      db->n_prev, db->w_head, db->w_tail, db->range, db->covn);
-    if ((rc = kfdb_leave(db, s, true))) return rc;
+    if ((rc = db->hs.leave(s, true))) return rc;
     for (int nd : db->nodes[slot]) db->free_nodes.push_back(nd);
     db->nodes[slot].clear();
     if (db->begin[slot] + nw == db->top) db->top -= nw;   // the last rows: the tail shrinks back
@@ -719,10 +690,10 @@ extern "C" int orbfe_kfdb_erase(OrbfeKeyFrameDB *db, int slot) {
 
 extern "C" int orbfe_kfdb_clear(OrbfeKeyFrameDB *db) {
     if (!db) return set_error(ORBFE_ERR_ARG, "bad arguments");
-    int rc = kfdb_enter(db, db->stream);
+    int rc = db->hs.enter(db->hs.stream);
     if (rc) return rc;
     if ((rc = kfdb_reset(db))) return rc;
-    return kfdb_leave(db, db->stream, true);
+    return db->hs.leave(db->hs.stream, true);
 }
 
 extern "C" int orbfe_kfdb_set_covisibles(OrbfeKeyFrameDB *db, int n, const int32_t *slots, const int32_t *ptr, const int32_t *lists) {
@@ -751,12 +722,12 @@ extern "C" int orbfe_kfdb_set_covisibles(OrbfeKeyFrameDB *db, int n, const int32
             r[2 + j - ptr[i]] = lists[j];
         }
     }
-    cudaStream_t s = db->stream;
-    int rc = kfdb_enter(db, s);
+    cudaStream_t s = db->hs.stream;
+    int rc = db->hs.enter(s);
     if (rc) return rc;
-    KFDB_TRY(cudaMemcpyAsync(db->covrows, rows.data(), sizeof(int) * rows.size(), cudaMemcpyHostToDevice, s));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(db->covrows, rows.data(), sizeof(int) * rows.size(), cudaMemcpyHostToDevice, s));
     kfdb_covis_kernel<<<(n + 127) / 128, 128, 0, s>>>(db->covrows, n, db->covn, db->cov);
-    return kfdb_leave(db, s, true);
+    return db->hs.leave(s, true);
 }
 
 extern "C" int orbfe_kfdb_set_covisibles_device(OrbfeKeyFrameDB *db, int n, const int32_t *slots, const int32_t *d_ptr,
@@ -771,12 +742,12 @@ extern "C" int orbfe_kfdb_set_covisibles_device(OrbfeKeyFrameDB *db, int n, cons
         if (slots[i] >= db->K) return set_error(ORBFE_ERR_ARG, "slot %d out of range", slots[i]);
         if (seen[slots[i]]++) return set_error(ORBFE_ERR_ARG, "slot %d listed twice", slots[i]);
     }
-    cudaStream_t s = stream ? (cudaStream_t)stream : db->stream;
-    int rc = kfdb_enter(db, s);
+    cudaStream_t s = db->hs.pick(stream);
+    int rc = db->hs.enter(s);
     if (rc) return rc;
-    KFDB_TRY(cudaMemcpyAsync(db->covrows, slots, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, s));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(db->covrows, slots, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, s));
     kfdb_covis_device_kernel<<<(n + 127) / 128, 128, 0, s>>>(db->covrows, n, db->K, d_ptr, d_lists, db->covn, db->cov);
-    return kfdb_leave(db, s, false);
+    return db->hs.leave(s, false);
 }
 
 static int kfdb_check_detect(int mode, int nq, int nconn, int cap) {
@@ -819,11 +790,11 @@ extern "C" int orbfe_kfdb_detect_device(OrbfeKeyFrameDB *db, int mode, int nq, c
     if (rc) return rc;
     if (!db || !d_ncand || (nq > 0 && (!d_q_ids || !d_q_vals)) || (mode == 0 && nconn > 0 && !d_connected) || (cap > 0 && !d_cand))
         return set_error(ORBFE_ERR_ARG, "NULL argument");
-    cudaStream_t s = stream ? (cudaStream_t)stream : db->stream;
-    if ((rc = kfdb_enter(db, s))) return rc;
+    cudaStream_t s = db->hs.pick(stream);
+    if ((rc = db->hs.enter(s))) return rc;
     kfdb_queries(db, mode, 1, nq, d_q_ids, d_q_vals, nullptr, d_connected, mode == 0 ? nconn : 0, nullptr, min_score, cap, d_cand, d_ncand,
                  d_words, d_score, s);
-    return kfdb_leave(db, s, false);
+    return db->hs.leave(s, false);
 }
 
 extern "C" int orbfe_kfdb_detect_batch_device(OrbfeKeyFrameDB *db, int mode, int nqueries, int qcap, const int32_t *d_q_ids,
@@ -836,11 +807,11 @@ extern "C" int orbfe_kfdb_detect_batch_device(OrbfeKeyFrameDB *db, int mode, int
     if (!db || !d_ncand || (qcap > 0 && (!d_q_ids || !d_q_vals)) || (mode == 0 && (!d_conn_ptr || !d_min_score)) || (cap > 0 && !d_cand))
         return set_error(ORBFE_ERR_ARG, "NULL argument");
     if (nqueries > db->Q) return set_error(ORBFE_ERR_ARG, "nqueries %d > max_queries %d", nqueries, db->Q);
-    cudaStream_t s = stream ? (cudaStream_t)stream : db->stream;
-    if ((rc = kfdb_enter(db, s))) return rc;
+    cudaStream_t s = db->hs.pick(stream);
+    if ((rc = db->hs.enter(s))) return rc;
     kfdb_queries(db, mode, nqueries, qcap, d_q_ids, d_q_vals, mode == 0 ? d_conn_ptr : nullptr, mode == 0 ? d_connected : nullptr, 0,
                  mode == 0 ? d_min_score : nullptr, 0.f, cap, d_cand, d_ncand, d_words, d_score, s);
-    return kfdb_leave(db, s, false);
+    return db->hs.leave(s, false);
 }
 
 extern "C" int orbfe_kfdb_detect(OrbfeKeyFrameDB *db, int mode, int nq, const int32_t *q_ids, const double *q_vals, int nconn,
@@ -858,24 +829,24 @@ extern "C" int orbfe_kfdb_detect(OrbfeKeyFrameDB *db, int mode, int nq, const in
         for (int i = 0; i < nconn; i++)
             if (connected[i] < 0 || connected[i] >= db->K) return set_error(ORBFE_ERR_ARG, "connected slot %d out of range", connected[i]);
     }
-    cudaStream_t s = db->stream;
-    if ((rc = kfdb_enter(db, s))) return rc;
+    cudaStream_t s = db->hs.stream;
+    if ((rc = db->hs.enter(s))) return rc;
     if (nq > 0) {
-        KFDB_TRY(cudaMemcpyAsync(db->q_ids, q_ids, sizeof(int) * nq, cudaMemcpyHostToDevice, s));
-        KFDB_TRY(cudaMemcpyAsync(db->q_vals, q_vals, sizeof(double) * nq, cudaMemcpyHostToDevice, s));
+        ORBFE_CUDA_TRY(cudaMemcpyAsync(db->q_ids, q_ids, sizeof(int) * nq, cudaMemcpyHostToDevice, s));
+        ORBFE_CUDA_TRY(cudaMemcpyAsync(db->q_vals, q_vals, sizeof(double) * nq, cudaMemcpyHostToDevice, s));
     }
-    if (mode == 0 && nconn > 0) KFDB_TRY(cudaMemcpyAsync(db->q_conn, connected, sizeof(int) * nconn, cudaMemcpyHostToDevice, s));
+    if (mode == 0 && nconn > 0) ORBFE_CUDA_TRY(cudaMemcpyAsync(db->q_conn, connected, sizeof(int) * nconn, cudaMemcpyHostToDevice, s));
     rc = orbfe_kfdb_detect_device(db, mode, nq, db->q_ids, db->q_vals, mode == 0 ? nconn : 0, db->q_conn, min_score, db->K, db->o_cand,
                                   db->o_n, db->o_words, db->o_score, s);
     if (rc) return rc;
     int n = 0;
-    KFDB_TRY(cudaMemcpyAsync(&n, db->o_n, sizeof(int), cudaMemcpyDeviceToHost, s));
-    if (words_out) KFDB_TRY(cudaMemcpyAsync(words_out, db->o_words, sizeof(int) * (size_t)db->K, cudaMemcpyDeviceToHost, s));
-    if (score_out) KFDB_TRY(cudaMemcpyAsync(score_out, db->o_score, sizeof(float) * (size_t)db->K, cudaMemcpyDeviceToHost, s));
-    KFDB_TRY(cudaStreamSynchronize(s));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(&n, db->o_n, sizeof(int), cudaMemcpyDeviceToHost, s));
+    if (words_out) ORBFE_CUDA_TRY(cudaMemcpyAsync(words_out, db->o_words, sizeof(int) * (size_t)db->K, cudaMemcpyDeviceToHost, s));
+    if (score_out) ORBFE_CUDA_TRY(cudaMemcpyAsync(score_out, db->o_score, sizeof(float) * (size_t)db->K, cudaMemcpyDeviceToHost, s));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(s));
     *ncand_out = n;
     if (n > cap) return set_error(ORBFE_ERR_CAPACITY, "%d candidates exceed cap %d", n, cap);
-    if (n > 0) KFDB_TRY(cudaMemcpy(cand_out, db->o_cand, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost));
+    if (n > 0) ORBFE_CUDA_TRY(cudaMemcpy(cand_out, db->o_cand, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost));
     return ORBFE_OK;
 }
 

@@ -42,13 +42,6 @@ int orbfe::set_error(int code, const char *fmt, ...) {
 }
 static int (*const fail)(int, const char *, ...) = orbfe::set_error;  // this file's spelling
 
-#define CU_TRY(expr)                                                                                   \
-    do {                                                                                               \
-        cudaError_t e__ = (expr);                                                                      \
-        if (e__ != cudaSuccess)                                                                        \
-            return fail(ORBFE_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-    } while (0)
-
 extern "C" const char *orbfe_last_error(void) { return g_err; }
 extern "C" int orbfe_version(void) { return ORBFE_VERSION; }
 extern "C" int orbfe_device_count(void) {
@@ -86,7 +79,7 @@ struct OrbfeExtractor {
     PlanDev hplan;
     PlanDev *dplan = nullptr;
     WorkDev work;
-    std::vector<void *> allocs;  // device allocations of the current plan
+    DeviceBuffers plan_mem;      // device allocations of the current plan
     void *counters = nullptr;    // cell_cnt_lo | cell_cnt_hi | kept_cnt (zeroed per call)
     size_t counters_bytes = 0;
     size_t ls_smem = 0;
@@ -116,8 +109,7 @@ struct OrbfeExtractor {
 };
 
 static void free_plan(OrbfeExtractor *ex) {
-    for (void *p : ex->allocs) cudaFree(p);
-    ex->allocs.clear();
+    ex->plan_mem.release();
     ex->dplan = nullptr;
     ex->own_pyr0 = nullptr; ex->d_maps = nullptr;
     ex->counters = nullptr;
@@ -125,14 +117,6 @@ static void free_plan(OrbfeExtractor *ex) {
     ex->d_desc = nullptr;
     ex->d_counts = nullptr;
     ex->W = ex->H = ex->Bcap = 0;
-}
-
-template <typename T>
-static cudaError_t dmalloc(OrbfeExtractor *ex, T **p, size_t count) {
-    void *q = nullptr;
-    cudaError_t e = cudaMalloc(&q, std::max<size_t>(count * sizeof(T), 256));
-    if (e == cudaSuccess) { ex->allocs.push_back(q); *p = (T *)q; }
-    return e;
 }
 
 // cv::resize INTER_LINEAR tap tables for one axis (OpenCV imgproc resize.cpp semantics, see SURVEY 8c)
@@ -281,7 +265,7 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
     if (ex->ls_smem > 200 * 1024)
         return fail(ORBFE_ERR_UNSUPPORTED, "nfeatures too large for the level-select kernel (%zu B smem)", ex->ls_smem);
 
-    CU_TRY(cudaSetDevice(ex->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
     if (ex->ls_smem > 48 * 1024) {
         cudaError_t e = (cudaError_t)(ex->score_type == 0 ? set_level_select_harris_smem((int)ex->ls_smem) : set_level_select_smem((int)ex->ls_smem));
         if (e != cudaSuccess) return fail(ORBFE_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
@@ -289,9 +273,9 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
     // ---- device memory ----
     for (int l = 0; l < ex->nlevels; l++) {
         LevelDev &L = P.lv[l];
-        CU_TRY(dmalloc(ex, &L.pyr, L.plane * B + 256));
-        CU_TRY(dmalloc(ex, &L.blur, L.plane + 256));  // one plane, for orbfe_debug_read_level
-        CU_TRY(cudaMemsetAsync(L.pyr, 0, L.plane * B + 256, ex->stream));
+        ORBFE_CUDA_TRY(ex->plan_mem.alloc(&L.pyr, L.plane * B + 256));
+        ORBFE_CUDA_TRY(ex->plan_mem.alloc(&L.blur, L.plane + 256));  // one plane, for orbfe_debug_read_level
+        ORBFE_CUDA_TRY(cudaMemsetAsync(L.pyr, 0, L.plane * B + 256, ex->stream));
         if (l > 0) {
             const LevelDev &S = P.lv[l - 1];
             std::vector<int> xo, yo;
@@ -314,14 +298,14 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
                     if (xo[x4 + 2] - (xo[x4] & ~3) > 6) L.rz_fast = 1;
             }
             int *dxo; short2 *dxab; int2 *dyr; short2 *dyab;
-            CU_TRY(dmalloc(ex, &dxo, xo.size()));
-            CU_TRY(dmalloc(ex, &dxab, xab.size()));
-            CU_TRY(dmalloc(ex, &dyr, (size_t)L.h));
-            CU_TRY(dmalloc(ex, &dyab, (size_t)L.h));
-            CU_TRY(cudaMemcpy(dxo, xo.data(), sizeof(int) * xo.size(), cudaMemcpyHostToDevice));
-            CU_TRY(cudaMemcpy(dxab, xab.data(), sizeof(short2) * xab.size(), cudaMemcpyHostToDevice));
-            CU_TRY(cudaMemcpy(dyr, yr.data(), sizeof(int2) * L.h, cudaMemcpyHostToDevice));
-            CU_TRY(cudaMemcpy(dyab, yab.data(), sizeof(short2) * L.h, cudaMemcpyHostToDevice));
+            ORBFE_CUDA_TRY(ex->plan_mem.alloc(&dxo, xo.size()));
+            ORBFE_CUDA_TRY(ex->plan_mem.alloc(&dxab, xab.size()));
+            ORBFE_CUDA_TRY(ex->plan_mem.alloc(&dyr, (size_t)L.h));
+            ORBFE_CUDA_TRY(ex->plan_mem.alloc(&dyab, (size_t)L.h));
+            ORBFE_CUDA_TRY(cudaMemcpy(dxo, xo.data(), sizeof(int) * xo.size(), cudaMemcpyHostToDevice));
+            ORBFE_CUDA_TRY(cudaMemcpy(dxab, xab.data(), sizeof(short2) * xab.size(), cudaMemcpyHostToDevice));
+            ORBFE_CUDA_TRY(cudaMemcpy(dyr, yr.data(), sizeof(int2) * L.h, cudaMemcpyHostToDevice));
+            ORBFE_CUDA_TRY(cudaMemcpy(dyab, yab.data(), sizeof(short2) * L.h, cudaMemcpyHostToDevice));
             L.xofs = dxo; L.xab = dxab; L.yrows = dyr; L.yab = dyab;
         }
     }
@@ -357,8 +341,8 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
                 }
         }
         FTileInfo *d_info;
-        CU_TRY(dmalloc(ex, &d_info, info.size()));
-        CU_TRY(cudaMemcpy(d_info, info.data(), sizeof(FTileInfo) * info.size(), cudaMemcpyHostToDevice));
+        ORBFE_CUDA_TRY(ex->plan_mem.alloc(&d_info, info.size()));
+        ORBFE_CUDA_TRY(cudaMemcpy(d_info, info.data(), sizeof(FTileInfo) * info.size(), cudaMemcpyHostToDevice));
         Wk.ftile_info = d_info;
         std::vector<BTileInfo> binfo((size_t)P.nbtiles_total);
         for (int l = 0; l < ex->nlevels; l++) {
@@ -370,15 +354,15 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
                 }
         }
         BTileInfo *d_binfo;
-        CU_TRY(dmalloc(ex, &d_binfo, binfo.size()));
-        CU_TRY(cudaMemcpy(d_binfo, binfo.data(), sizeof(BTileInfo) * binfo.size(), cudaMemcpyHostToDevice));
+        ORBFE_CUDA_TRY(ex->plan_mem.alloc(&d_binfo, binfo.size()));
+        ORBFE_CUDA_TRY(cudaMemcpy(d_binfo, binfo.data(), sizeof(BTileInfo) * binfo.size(), cudaMemcpyHostToDevice));
         Wk.btile_info = d_binfo;
     }
     long long *d_cb; int *d_cc;
-    CU_TRY(dmalloc(ex, &d_cb, cand_base.size()));
-    CU_TRY(dmalloc(ex, &d_cc, cand_cap.size()));
-    CU_TRY(cudaMemcpy(d_cb, cand_base.data(), sizeof(long long) * cand_base.size(), cudaMemcpyHostToDevice));
-    CU_TRY(cudaMemcpy(d_cc, cand_cap.data(), sizeof(int) * cand_cap.size(), cudaMemcpyHostToDevice));
+    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&d_cb, cand_base.size()));
+    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&d_cc, cand_cap.size()));
+    ORBFE_CUDA_TRY(cudaMemcpy(d_cb, cand_base.data(), sizeof(long long) * cand_base.size(), cudaMemcpyHostToDevice));
+    ORBFE_CUDA_TRY(cudaMemcpy(d_cc, cand_cap.data(), sizeof(int) * cand_cap.size(), cudaMemcpyHostToDevice));
     Wk.cell_cand_base = d_cb;
     Wk.cell_cand_cap = d_cc;
     // ---- TMA tensor maps (one per level: x, y, frame) for the FAST kernel's pixel tiles ----
@@ -395,45 +379,45 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
             if (r != CUDA_SUCCESS) return fail(ORBFE_ERR_CUDA, "cuTensorMapEncodeTiled(level %d) failed: %d", l, (int)r);
         }
         CUtensorMap *d_maps;
-        CU_TRY(dmalloc(ex, &d_maps, maps.size()));
-        CU_TRY(cudaMemcpy(d_maps, maps.data(), sizeof(CUtensorMap) * maps.size(), cudaMemcpyHostToDevice));
+        ORBFE_CUDA_TRY(ex->plan_mem.alloc(&d_maps, maps.size()));
+        ORBFE_CUDA_TRY(cudaMemcpy(d_maps, maps.data(), sizeof(CUtensorMap) * maps.size(), cudaMemcpyHostToDevice));
         Wk.tmaps = d_maps;
         ex->tma_encode = fn;
         ex->d_maps = d_maps;
         cudaError_t e = (cudaError_t)fast_tma_setup();
         if (e != cudaSuccess) return fail(ORBFE_ERR_CUDA, "cudaFuncSetAttribute(fast_nms_tma_kernel): %s", cudaGetErrorString(e));
     }
-    CU_TRY(dmalloc(ex, &Wk.cand_keys, (size_t)cand_total * B));
+    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.cand_keys, (size_t)cand_total * B));
     if (ex->score_type == 0) {
-        CU_TRY(dmalloc(ex, &Wk.cand_keys64, (size_t)cand_total * B));
-        CU_TRY(dmalloc(ex, &Wk.kept_aux, (size_t)P.kept_total * B));
+        ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.cand_keys64, (size_t)cand_total * B));
+        ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.kept_aux, (size_t)P.kept_total * B));
     }
     const size_t nc = (size_t)P.ncells_total * B, nl = (size_t)P.nlevels * B;
     int *cnt;
     ex->counters_bytes = sizeof(int) * (2 * nc + nl);
-    CU_TRY(dmalloc(ex, &cnt, 2 * nc + nl));
+    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&cnt, 2 * nc + nl));
     ex->counters = cnt;
     Wk.cell_cnt_lo = cnt;
     Wk.cell_cnt_hi = cnt + nc;
     Wk.kept_cnt = cnt + 2 * nc;
-    CU_TRY(dmalloc(ex, &Wk.cell_keep, nc));
-    CU_TRY(dmalloc(ex, &Wk.cell_min_key, nc));
-    CU_TRY(dmalloc(ex, &Wk.kept_keys, (size_t)P.kept_total * B));
-    CU_TRY(dmalloc(ex, &Wk.kp_xy_score, (size_t)std::max(P.nfeatures, 1) * B));
-    CU_TRY(dmalloc(ex, &Wk.level_cnt, nl));
-    CU_TRY(dmalloc(ex, &Wk.err_flag, 1));
-    CU_TRY(cudaMemsetAsync(Wk.err_flag, 0, sizeof(int), ex->stream));
-    CU_TRY(dmalloc(ex, &ex->d_kps, (size_t)std::max(P.nfeatures, 1) * B));
-    CU_TRY(dmalloc(ex, &ex->d_desc, (size_t)std::max(P.nfeatures, 1) * B * 32));
-    CU_TRY(dmalloc(ex, &ex->d_counts, (size_t)B));
-    CU_TRY(dmalloc(ex, &ex->dplan, 1));
-    CU_TRY(cudaMemcpyAsync(ex->dplan, &P, sizeof(P), cudaMemcpyHostToDevice, ex->stream));
+    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.cell_keep, nc));
+    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.cell_min_key, nc));
+    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.kept_keys, (size_t)P.kept_total * B));
+    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.kp_xy_score, (size_t)std::max(P.nfeatures, 1) * B));
+    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.level_cnt, nl));
+    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.err_flag, 1));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(Wk.err_flag, 0, sizeof(int), ex->stream));
+    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->d_kps, (size_t)std::max(P.nfeatures, 1) * B));
+    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->d_desc, (size_t)std::max(P.nfeatures, 1) * B * 32));
+    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->d_counts, (size_t)B));
+    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->dplan, 1));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->dplan, &P, sizeof(P), cudaMemcpyHostToDevice, ex->stream));
     if (ex->h_counts_cap < (size_t)B) {
         if (ex->h_counts) cudaFreeHost(ex->h_counts);
-        CU_TRY(cudaHostAlloc((void **)&ex->h_counts, sizeof(int) * B, cudaHostAllocDefault));
+        ORBFE_CUDA_TRY(cudaHostAlloc((void **)&ex->h_counts, sizeof(int) * B, cudaHostAllocDefault));
         ex->h_counts_cap = B;
     }
-    CU_TRY(cudaStreamSynchronize(ex->stream));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(ex->stream));
     ex->W = W; ex->H = H; ex->Bcap = B;
     ex->own_pyr0 = P.lv[0].pyr; ex->own_pitch0 = P.lv[0].pitch; ex->own_plane0 = P.lv[0].plane;
     return ORBFE_OK;
@@ -446,12 +430,12 @@ static int set_level0(OrbfeExtractor *ex, uint8_t *ptr, int pitch, size_t plane,
     LevelDev &L0 = ex->hplan.lv[0];
     if (L0.pyr == ptr && L0.pitch == pitch && L0.plane == plane) return ORBFE_OK;
     L0.pyr = ptr; L0.pitch = pitch; L0.plane = plane;
-    CU_TRY(cudaMemcpyAsync(&ex->dplan->lv[0], &L0, sizeof(LevelDev), cudaMemcpyHostToDevice, s));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(&ex->dplan->lv[0], &L0, sizeof(LevelDev), cudaMemcpyHostToDevice, s));
     if (ex->d_maps && ex->tma_encode) {
         CUtensorMap m;
         const CUresult r = encode_level_map(ex->tma_encode, &m, ptr, L0.w, L0.h, std::max(batch, ex->Bcap), pitch, plane);
         if (r != CUDA_SUCCESS) return fail(ORBFE_ERR_CUDA, "cuTensorMapEncodeTiled(level 0, in place) failed: %d", (int)r);
-        CU_TRY(cudaMemcpyAsync(&ex->d_maps[0], &m, sizeof(m), cudaMemcpyHostToDevice, s));
+        ORBFE_CUDA_TRY(cudaMemcpyAsync(&ex->d_maps[0], &m, sizeof(m), cudaMemcpyHostToDevice, s));
     }
     return ORBFE_OK;
 }
@@ -466,10 +450,10 @@ static int ingest_device(OrbfeExtractor *ex, const uint8_t *d_imgs, int width, i
     if (rc) return rc;
     const LevelDev &L0 = ex->hplan.lv[0];
     if (frame_stride == stride * (size_t)height && L0.plane == (size_t)L0.pitch * height) {
-        CU_TRY(cudaMemcpy2DAsync(L0.pyr, L0.pitch, d_imgs, stride, width, (size_t)height * batch, cudaMemcpyDeviceToDevice, s));
+        ORBFE_CUDA_TRY(cudaMemcpy2DAsync(L0.pyr, L0.pitch, d_imgs, stride, width, (size_t)height * batch, cudaMemcpyDeviceToDevice, s));
     } else {
         for (int f = 0; f < batch; f++)
-            CU_TRY(cudaMemcpy2DAsync(L0.pyr + f * L0.plane, L0.pitch, d_imgs + f * frame_stride, stride, width, height,
+            ORBFE_CUDA_TRY(cudaMemcpy2DAsync(L0.pyr + f * L0.plane, L0.pitch, d_imgs + f * frame_stride, stride, width, height,
                                      cudaMemcpyDeviceToDevice, s));
     }
     return ORBFE_OK;
@@ -520,7 +504,7 @@ extern "C" int orbfe_extractor_create(int nfeatures, float scale_factor, int nle
     if (e == cudaSuccess) e = cudaMemcpy(ex->d_pattern, kBriefPattern, 1024, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaHostAlloc((void **)&ex->h_err, sizeof(int), cudaHostAllocDefault);
     if (e != cudaSuccess) {
-        delete ex;
+        orbfe_extractor_destroy(ex);
         return fail(ORBFE_ERR_CUDA, "extractor setup failed: %s", cudaGetErrorString(e));
     }
     *out = ex;
@@ -572,7 +556,7 @@ static void stage_mark(OrbfeExtractor *ex, cudaStream_t s, const char *name) {
 // Enqueue the device pipeline for frames [f0, f0+nf) whose level-0 images are already in lv[0].pyr.
 // The per-call counters must have been zeroed (zero_counters) before the first chunk.
 static int zero_counters(OrbfeExtractor *ex, cudaStream_t s) {
-    CU_TRY(cudaMemsetAsync(ex->counters, 0, ex->counters_bytes, s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(ex->counters, 0, ex->counters_bytes, s));
     return ORBFE_OK;
 }
 
@@ -598,7 +582,7 @@ static int enqueue_pipeline(OrbfeExtractor *ex, int f0, int nf, OrbfeKeyPoint *d
     stage_mark(ex, s, "level_select");
     launch_describe_fused(ex->dplan, hp, ex->work, ex->d_pattern, d_kps, d_desc, d_counts, f0, nf, s, peers); launches++;
     stage_mark(ex, s, "describe");
-    CU_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     ex->last_launches += launches;
     return ORBFE_OK;
 }
@@ -630,7 +614,7 @@ static void profiling_collect(OrbfeExtractor *ex) {
 static int begin_device_extract(OrbfeExtractor *ex, const uint8_t *d_imgs, int width, int height, size_t stride, size_t frame_stride,
                                 int batch, void *stream, cudaStream_t *s) {
     if (width <= 0 || height <= 0 || batch <= 0 || stride < (size_t)width) return fail(ORBFE_ERR_ARG, "bad geometry");
-    CU_TRY(cudaSetDevice(ex->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
     int rc = build_plan(ex, width, height, batch);
     if (rc) return rc;
     *s = stream ? (cudaStream_t)stream : ex->stream;
@@ -669,7 +653,7 @@ extern "C" int orbfe_extract_batch(OrbfeExtractor *ex, const uint8_t *imgs, int 
     for (int f = 0; f < std::max(batch, 0); f++) n_out[f] = 0;
     if (!imgs || width <= 0 || height <= 0) return ORBFE_OK;  // empty image: silent return (ORBextractor.cc:721-722)
     if (batch <= 0 || stride < (size_t)width || cap < 0 || (cap > 0 && (!kps || !desc))) return fail(ORBFE_ERR_ARG, "bad arguments");
-    CU_TRY(cudaSetDevice(ex->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
     int rc = build_plan(ex, width, height, batch);
     if (rc) return rc;
     cudaStream_t s = ex->stream;
@@ -684,32 +668,32 @@ extern "C" int orbfe_extract_batch(OrbfeExtractor *ex, const uint8_t *imgs, int 
     // H2D of chunk k+1 (copy stream) overlaps the kernels of chunk k (compute stream)
     int nchunks = batch >= 8 ? 4 : 1;   // H100, 400 W (64 x 1080p, bench.py's three handles): 1, 2 and 4 chunks within 2 % (37.4-38.1 Mkp/s end to end)
     if (const char *e = getenv("ORBFE_CHUNKS")) nchunks = std::max(1, std::min(batch, atoi(e)));  // tuning knob
-    if (!ex->copy_stream) CU_TRY(cudaStreamCreateWithFlags(&ex->copy_stream, cudaStreamNonBlocking));
+    if (!ex->copy_stream) ORBFE_CUDA_TRY(cudaStreamCreateWithFlags(&ex->copy_stream, cudaStreamNonBlocking));
     while ((int)ex->chunk_ev.size() < nchunks + 1) {
         cudaEvent_t e;
-        CU_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        ORBFE_CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         ex->chunk_ev.push_back(e);
     }
     // the copy stream must not overwrite level 0 before earlier work of this handle has drained
-    CU_TRY(cudaEventRecord(ex->chunk_ev[nchunks], s));
-    CU_TRY(cudaStreamWaitEvent(ex->copy_stream, ex->chunk_ev[nchunks], 0));
+    ORBFE_CUDA_TRY(cudaEventRecord(ex->chunk_ev[nchunks], s));
+    ORBFE_CUDA_TRY(cudaStreamWaitEvent(ex->copy_stream, ex->chunk_ev[nchunks], 0));
     for (int k = 0; k < nchunks; k++) {
         const int f0 = (int)((long long)batch * k / nchunks), f1 = (int)((long long)batch * (k + 1) / nchunks);
         if (f1 <= f0) continue;
         if (frame_stride == stride * (size_t)height && stride == (size_t)width && L0.pitch == width) {
             // fully contiguous on both sides: one linear DMA
-            CU_TRY(cudaMemcpyAsync(L0.pyr + (size_t)f0 * L0.plane, imgs + (size_t)f0 * frame_stride, (size_t)width * height * (f1 - f0),
+            ORBFE_CUDA_TRY(cudaMemcpyAsync(L0.pyr + (size_t)f0 * L0.plane, imgs + (size_t)f0 * frame_stride, (size_t)width * height * (f1 - f0),
                                    cudaMemcpyHostToDevice, ex->copy_stream));
         } else if (frame_stride == stride * (size_t)height) {
-            CU_TRY(cudaMemcpy2DAsync(L0.pyr + (size_t)f0 * L0.plane, L0.pitch, imgs + (size_t)f0 * frame_stride, stride, width,
+            ORBFE_CUDA_TRY(cudaMemcpy2DAsync(L0.pyr + (size_t)f0 * L0.plane, L0.pitch, imgs + (size_t)f0 * frame_stride, stride, width,
                                      (size_t)height * (f1 - f0), cudaMemcpyHostToDevice, ex->copy_stream));
         } else {
             for (int f = f0; f < f1; f++)
-                CU_TRY(cudaMemcpy2DAsync(L0.pyr + f * L0.plane, L0.pitch, imgs + f * frame_stride, stride, width, height,
+                ORBFE_CUDA_TRY(cudaMemcpy2DAsync(L0.pyr + f * L0.plane, L0.pitch, imgs + f * frame_stride, stride, width, height,
                                          cudaMemcpyHostToDevice, ex->copy_stream));
         }
-        CU_TRY(cudaEventRecord(ex->chunk_ev[k], ex->copy_stream));
-        CU_TRY(cudaStreamWaitEvent(s, ex->chunk_ev[k], 0));
+        ORBFE_CUDA_TRY(cudaEventRecord(ex->chunk_ev[k], ex->copy_stream));
+        ORBFE_CUDA_TRY(cudaStreamWaitEvent(s, ex->chunk_ev[k], 0));
         if (ex->batch_mode == 1) {
             enqueue_pyramid(ex, f0, f1 - f0, s);   // phased: only the pyramids follow the upload chunk by chunk
         } else {
@@ -722,16 +706,16 @@ extern "C" int orbfe_extract_batch(OrbfeExtractor *ex, const uint8_t *imgs, int 
         if (rc) return rc;
     }
     const int ncopy = std::min(cap, P.nfeatures);
-    CU_TRY(cudaMemcpyAsync(ex->h_counts, ex->d_counts, sizeof(int) * batch, cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaMemcpyAsync(ex->h_err, ex->work.err_flag, sizeof(int), cudaMemcpyDeviceToHost, s));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->h_counts, ex->d_counts, sizeof(int) * batch, cudaMemcpyDeviceToHost, s));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->h_err, ex->work.err_flag, sizeof(int), cudaMemcpyDeviceToHost, s));
     if (ncopy > 0) {
-        CU_TRY(cudaMemcpy2DAsync(kps, sizeof(OrbfeKeyPoint) * cap, ex->d_kps, sizeof(OrbfeKeyPoint) * P.nfeatures,
+        ORBFE_CUDA_TRY(cudaMemcpy2DAsync(kps, sizeof(OrbfeKeyPoint) * cap, ex->d_kps, sizeof(OrbfeKeyPoint) * P.nfeatures,
                                  sizeof(OrbfeKeyPoint) * ncopy, batch, cudaMemcpyDeviceToHost, s));
-        CU_TRY(cudaMemcpy2DAsync(desc, (size_t)32 * cap, ex->d_desc, (size_t)32 * P.nfeatures, (size_t)32 * ncopy, batch,
+        ORBFE_CUDA_TRY(cudaMemcpy2DAsync(desc, (size_t)32 * cap, ex->d_desc, (size_t)32 * P.nfeatures, (size_t)32 * ncopy, batch,
                                  cudaMemcpyDeviceToHost, s));
     }
     stage_mark(ex, s, "d2h");
-    CU_TRY(cudaStreamSynchronize(s));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(s));
     if (*ex->h_err) {
         int code = *ex->h_err;
         cudaMemsetAsync(ex->work.err_flag, 0, sizeof(int), s);
@@ -753,8 +737,8 @@ extern "C" int orbfe_extract(OrbfeExtractor *ex, const uint8_t *img, int width, 
 
 extern "C" int orbfe_extractor_sync(OrbfeExtractor *ex) {
     if (!ex) return fail(ORBFE_ERR_ARG, "ex is NULL");
-    CU_TRY(cudaSetDevice(ex->device));
-    CU_TRY(cudaStreamSynchronize(ex->stream));
+    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(ex->stream));
     return ORBFE_OK;
 }
 
@@ -797,16 +781,16 @@ extern "C" int orbfe_debug_level_size(const OrbfeExtractor *ex, int level, int *
 extern "C" int orbfe_debug_read_level(OrbfeExtractor *ex, int frame, int level, int which, uint8_t *out, size_t out_stride) {
     if (!ex || !out || level < 0 || level >= ex->nlevels || frame < 0 || frame >= ex->Bcap)
         return fail(ORBFE_ERR_ARG, "bad arguments");
-    CU_TRY(cudaSetDevice(ex->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
     const LevelDev &L = ex->hplan.lv[level];
     const uint8_t *src = which ? L.blur : L.pyr + (size_t)frame * L.plane;
     if (which) {
         // the pipeline smooths only descriptor patches; materialise the smoothed level of this frame on demand
         launch_blur(ex->dplan, ex->hplan, ex->work, frame, 1, ex->stream);
-        CU_TRY(cudaGetLastError());
+        ORBFE_CUDA_TRY(cudaGetLastError());
     }
-    CU_TRY(cudaStreamSynchronize(ex->stream));
-    CU_TRY(cudaMemcpy2D(out, out_stride, src, L.pitch, L.w, L.h, cudaMemcpyDeviceToHost));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(ex->stream));
+    ORBFE_CUDA_TRY(cudaMemcpy2D(out, out_stride, src, L.pitch, L.w, L.h, cudaMemcpyDeviceToHost));
     return ORBFE_OK;
 }
 
@@ -859,7 +843,7 @@ extern "C" int orbfe_matcher_create(int device, OrbfeMatcher **out) {
     if (e == cudaSuccess) e = cudaMalloc((void **)&m->d_err, 2 * sizeof(int));
     if (e == cudaSuccess) e = cudaMemset(m->d_err, 0, 2 * sizeof(int));
     if (e == cudaSuccess) e = cudaHostAlloc((void **)&m->h_err, 2 * sizeof(int), cudaHostAllocDefault);
-    if (e != cudaSuccess) { delete m; return fail(ORBFE_ERR_CUDA, "matcher setup failed: %s", cudaGetErrorString(e)); }
+    if (e != cudaSuccess) { orbfe_matcher_destroy(m); return fail(ORBFE_ERR_CUDA, "matcher setup failed: %s", cudaGetErrorString(e)); }
     *out = m;
     return ORBFE_OK;
 }
@@ -888,12 +872,12 @@ extern "C" int orbfe_matcher_counters(const OrbfeMatcher *m, unsigned long long 
 
 extern "C" int orbfe_matcher_sync(OrbfeMatcher *m) {
     if (!m) return fail(ORBFE_ERR_ARG, "m is NULL");
-    CU_TRY(cudaSetDevice(m->device));
-    CU_TRY(cudaMemcpyAsync(m->h_err, m->d_err, 2 * sizeof(int), cudaMemcpyDeviceToHost, m->stream));
-    CU_TRY(cudaStreamSynchronize(m->stream));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(m->h_err, m->d_err, 2 * sizeof(int), cudaMemcpyDeviceToHost, m->stream));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(m->stream));
     if (*m->h_err) {
         const int flags = *m->h_err;
-        CU_TRY(cudaMemsetAsync(m->d_err, 0, 2 * sizeof(int), m->stream));
+        ORBFE_CUDA_TRY(cudaMemsetAsync(m->d_err, 0, 2 * sizeof(int), m->stream));
         if (flags & 2)
             return fail(ORBFE_ERR_ARG, "orbfe_search_by_bow_device: a job's FeatureVector has an out-of-range node row or feature "
                                        "index (its nmatches is -1)");
@@ -939,7 +923,7 @@ static int sbp_prepare(OrbfeMatcher *m, SbpParams &P, float min_x, float min_y, 
     if (m->scratch_entries < need) {
         if (m->scratch) cudaFree(m->scratch);
         m->scratch = nullptr; m->scratch_entries = 0;
-        CU_TRY(cudaMalloc((void **)&m->scratch, need * sizeof(uint32_t)));
+        ORBFE_CUDA_TRY(cudaMalloc((void **)&m->scratch, need * sizeof(uint32_t)));
         m->scratch_entries = need;
     }
     *smem = total;
@@ -949,7 +933,7 @@ static int sbp_prepare(OrbfeMatcher *m, SbpParams &P, float min_x, float min_y, 
 // the launchers' cudaFuncSetAttribute result, then the launch itself
 static int sbp_launched(OrbfeMatcher *m, int rc) {
     if (rc) return fail(ORBFE_ERR_CUDA, "cudaFuncSetAttribute failed: %s", cudaGetErrorString((cudaError_t)rc));
-    CU_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     m->launches += 1;
     return ORBFE_OK;
 }
@@ -966,7 +950,7 @@ extern "C" int orbfe_search_by_projection_device(OrbfeMatcher *m, int npairs, co
     if (!d_kps || !d_desc || !d_counts || !d_cur_idx || !d_last_idx || !d_world || !d_flags || !d_Tcw || !d_cur_mp || !d_nmatches)
         return fail(ORBFE_ERR_ARG, "NULL argument");
     if (!(max_x > min_x) || !(max_y > min_y)) return fail(ORBFE_ERR_ARG, "bad image bounds");
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     SbpParams P;
     memset(&P, 0, sizeof(P));
     P.fx = fx; P.fy = fy; P.cx = cx; P.cy = cy; P.th = th;
@@ -1021,7 +1005,7 @@ int orbfe_search_for_initialization_hooked(OrbfeMatcher *m, int npairs, const Or
     if (!d_kps || !d_desc || !d_counts || !d_f1_idx || !d_f2_idx || !d_prev_matched || !d_match12 || !d_nmatches)
         return fail(ORBFE_ERR_ARG, "NULL argument");
     if (!(max_x > min_x) || !(max_y > min_y)) return fail(ORBFE_ERR_ARG, "bad image bounds");
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     SbpParams P = init_params(window, nnratio, check_orientation);
     if (hooks) {
         P.xw_flags = hooks->xw_flags; P.xw_done = hooks->xw_done; P.xw_err = hooks->xw_err; P.xw_n = hooks->xw_n; P.xw_epoch = hooks->xw_epoch;
@@ -1047,7 +1031,7 @@ extern "C" int orbfe_guided_search_device(OrbfeMatcher *m, int njobs, const Orbf
         !d_q_cnt || !d_slot_owner || !d_nmatches || (check_orientation && !d_qangle))
         return fail(ORBFE_ERR_ARG, "NULL argument");
     if (!(max_x > min_x) || !(max_y > min_y)) return fail(ORBFE_ERR_ARG, "bad image bounds");
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     SbpParams P;
     memset(&P, 0, sizeof(P));
     P.nlevels = 1; P.check_ori = check_orientation ? 1 : 0;
@@ -1069,8 +1053,8 @@ int orbfe::Stage::layout(std::initializer_list<std::pair<size_t *, size_t>> arra
     if (cap < off) {
         release();
         const size_t want = off + off / 4;
-        CU_TRY(cudaHostAlloc((void **)&h, want, cudaHostAllocDefault));
-        CU_TRY(cudaMalloc((void **)&d, want));
+        ORBFE_CUDA_TRY(cudaHostAlloc((void **)&h, want, cudaHostAllocDefault));
+        ORBFE_CUDA_TRY(cudaMalloc((void **)&d, want));
         cap = want;
     }
     return ORBFE_OK;
@@ -1080,6 +1064,18 @@ void orbfe::Stage::release() {
     if (h) cudaFreeHost(h);
     if (d) cudaFree(d);
     h = nullptr; d = nullptr; cap = 0;
+}
+
+// One host-array matcher call on the staged block: the round trip on the matcher's stream, its bytes counted, then either
+// orbfe_matcher_sync (`read_flags`: the call's kernels report through d_err) or a plain synchronise.
+template <class Enqueue>
+static int matcher_round_trip(OrbfeMatcher *m, bool read_flags, size_t up, size_t down, size_t total, Enqueue enqueue) {
+    if (int rc = m->stage.round_trip(m->stream, up, down, total, enqueue)) return rc;
+    m->h2d_bytes += up;
+    m->d2h_bytes += total - down;
+    if (read_flags) return orbfe_matcher_sync(m);
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    return ORBFE_OK;
 }
 
 // SearchByBoW (both overloads) for `njobs` frame pairs, device-resident (include/orbfe_match.h).  Arguments are checked before
@@ -1094,11 +1090,11 @@ extern "C" int orbfe_search_by_bow_device(OrbfeMatcher *m, int variant, int njob
     if (!d_kps || !d_desc || !d_counts || !d_fv_ids || !d_fv_ptr || !d_fv_items || !d_fv_n || !d_valid || !d_idx1 || !d_idx2 ||
         !d_out || !d_nmatches)
         return fail(ORBFE_ERR_ARG, "NULL argument");
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : m->stream;
     launch_search_by_bow(variant, njobs, d_kps, d_desc, d_counts, cap, d_fv_ids, d_fv_ptr, d_fv_items, d_fv_n, d_valid, d_idx1, d_idx2,
                          nnratio, check_orientation ? 1 : 0, d_out, d_nmatches, m->d_err, s);
-    CU_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     m->launches += 1;
     return ORBFE_OK;
 }
@@ -1140,7 +1136,7 @@ extern "C" int orbfe_search_by_bow(OrbfeMatcher *m, int variant, int n1, const u
         return fail(ORBFE_ERR_ARG, "NULL argument");
     const int cap = std::max({n1, n2, nn1, nn2, 1});
     if (cap > 65535) return fail(ORBFE_ERR_UNSUPPORTED, "%d features or FeatureVector nodes on one side: at most 65535", cap);
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     const size_t C = (size_t)cap;
     PairStore o;
     size_t o_out, o_nm, total;
@@ -1162,18 +1158,14 @@ extern "C" int orbfe_search_by_bow(OrbfeMatcher *m, int variant, int n1, const u
         if (valid[f]) memcpy(H + o.flags + f * C, valid[f], (size_t)n[f]);
         else memset(H + o.flags + f * C, 0, (size_t)n[f]);   // variant 0 ignores side 2's flags
     }
-    cudaStream_t s = m->stream;
-    CU_TRY(cudaMemcpyAsync(D, H, o_out, cudaMemcpyHostToDevice, s));
     const int *d_idx = (const int *)(D + o.idx);
-    int rc = orbfe_search_by_bow_device(m, variant, 1, (const OrbfeKeyPoint *)(D + o.kps), D + o.desc, (const int *)(D + o.cnt), cap,
-                                        (const int32_t *)(D + o.ids), (const int32_t *)(D + o.ptr), (const int32_t *)(D + o.items),
-                                        (const int *)(D + o.nn), D + o.flags, d_idx, d_idx + 1, nnratio, check_orientation,
-                                        (int32_t *)(D + o_out), (int *)(D + o_nm), s);
-    if (rc) return rc;
-    CU_TRY(cudaMemcpyAsync(H + o_out, D + o_out, total - o_out, cudaMemcpyDeviceToHost, s));
-    if ((rc = orbfe_matcher_sync(m))) return rc;
-    m->h2d_bytes += o_out;
-    m->d2h_bytes += total - o_out;
+    if (int rc = matcher_round_trip(m, true, o_out, o_out, total, [&] {
+            return orbfe_search_by_bow_device(m, variant, 1, (const OrbfeKeyPoint *)(D + o.kps), D + o.desc, (const int *)(D + o.cnt),
+                                              cap, (const int32_t *)(D + o.ids), (const int32_t *)(D + o.ptr),
+                                              (const int32_t *)(D + o.items), (const int *)(D + o.nn), D + o.flags, d_idx, d_idx + 1,
+                                              nnratio, check_orientation, (int32_t *)(D + o_out), (int *)(D + o_nm), m->stream);
+        }))
+        return rc;
     const int nout = variant == 0 ? n2 : n1;
     if (nout) memcpy(out, H + o_out, (size_t)nout * 4);
     *nmatches_out = *(const int *)(H + o_nm);
@@ -1193,11 +1185,11 @@ extern "C" int orbfe_search_for_triangulation_device(OrbfeMatcher *m, int njobs,
     if (!d_kps || !d_desc || !d_counts || !d_fv_ids || !d_fv_ptr || !d_fv_items || !d_fv_n || !d_has_mp || !d_idx1 || !d_idx2 ||
         !d_F12 || !sigma2 || !d_match12 || !d_nmatches)
         return fail(ORBFE_ERR_ARG, "NULL argument");
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : m->stream;
     launch_search_for_triangulation(njobs, d_kps, d_desc, d_counts, cap, d_fv_ids, d_fv_ptr, d_fv_items, d_fv_n, d_has_mp, d_idx1, d_idx2,
                                     d_F12, sigma2, nlevels, check_orientation ? 1 : 0, d_match12, d_nmatches, m->d_err, s);
-    CU_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     m->launches += 1;
     return ORBFE_OK;
 }
@@ -1221,7 +1213,7 @@ extern "C" int orbfe_search_for_triangulation(OrbfeMatcher *m, int n1, const Orb
     // rejects the job
     int nlevels = 1;
     for (int i = 0; i < n2; i++) nlevels = std::max(nlevels, std::min(keys2[i].octave, ORBFE_MAX_LEVELS - 1) + 1);
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     const size_t C = (size_t)cap;
     PairStore o;
     size_t o_F, o_out, o_nm, total;
@@ -1243,19 +1235,15 @@ extern "C" int orbfe_search_for_triangulation(OrbfeMatcher *m, int n1, const Orb
         memcpy(H + o.flags + f * C, has_mp[f], (size_t)n[f]);
     }
     memcpy(H + o_F, F12, 9 * sizeof(float));
-    cudaStream_t s = m->stream;
-    CU_TRY(cudaMemcpyAsync(D, H, o_out, cudaMemcpyHostToDevice, s));
     const int *d_idx = (const int *)(D + o.idx);
-    int rc = orbfe_search_for_triangulation_device(m, 1, (const OrbfeKeyPoint *)(D + o.kps), D + o.desc, (const int *)(D + o.cnt), cap,
-                                                   (const int32_t *)(D + o.ids), (const int32_t *)(D + o.ptr),
-                                                   (const int32_t *)(D + o.items), (const int *)(D + o.nn), D + o.flags, d_idx, d_idx + 1,
-                                                   (const float *)(D + o_F), sigma2_kf2, nlevels, check_orientation,
-                                                   (int32_t *)(D + o_out), (int *)(D + o_nm), s);
-    if (rc) return rc;
-    CU_TRY(cudaMemcpyAsync(H + o_out, D + o_out, total - o_out, cudaMemcpyDeviceToHost, s));
-    if ((rc = orbfe_matcher_sync(m))) return rc;
-    m->h2d_bytes += o_out;
-    m->d2h_bytes += total - o_out;
+    if (int rc = matcher_round_trip(m, true, o_out, o_out, total, [&] {
+            return orbfe_search_for_triangulation_device(m, 1, (const OrbfeKeyPoint *)(D + o.kps), D + o.desc, (const int *)(D + o.cnt),
+                                                         cap, (const int32_t *)(D + o.ids), (const int32_t *)(D + o.ptr),
+                                                         (const int32_t *)(D + o.items), (const int *)(D + o.nn), D + o.flags, d_idx,
+                                                         d_idx + 1, (const float *)(D + o_F), sigma2_kf2, nlevels, check_orientation,
+                                                         (int32_t *)(D + o_out), (int *)(D + o_nm), m->stream);
+        }))
+        return rc;
     if (n1) memcpy(match12_out, H + o_out, (size_t)n1 * 4);
     *nmatches_out = *(const int *)(H + o_nm);
     return ORBFE_OK;
@@ -1264,10 +1252,10 @@ extern "C" int orbfe_search_for_triangulation(OrbfeMatcher *m, int n1, const Orb
 extern "C" int orbfe_hamming_csr_device(OrbfeMatcher *m, const uint8_t *d_q, const uint8_t *d_t, const int32_t *d_row_ptr,
                                         const int32_t *d_cols, int nq, int npairs, uint16_t *d_out, void *stream) {
     if (!m || (nq > 0 && (!d_q || !d_t || !d_row_ptr))) return fail(ORBFE_ERR_ARG, "NULL argument");
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     if (nq <= 0 || npairs <= 0) return ORBFE_OK;
     launch_hamming_csr(d_q, d_t, d_row_ptr, d_cols, nq, npairs, d_out, stream ? (cudaStream_t)stream : m->stream);
-    CU_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     return ORBFE_OK;
 }
 
@@ -1282,7 +1270,7 @@ extern "C" int orbfe_hamming_csr(OrbfeMatcher *m, const uint8_t *q, int nq, cons
     if (!t || !cols || !out || nt == 0) return fail(ORBFE_ERR_ARG, "NULL argument");
     for (int k = 0; k < np; k++)
         if (cols[k] < 0 || cols[k] >= nt) return fail(ORBFE_ERR_ARG, "cols[%d]=%d out of range", k, cols[k]);
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     const size_t b_q = (size_t)nq * 32, b_t = (size_t)nt * 32, b_row = sizeof(int32_t) * ((size_t)nq + 1);
     const size_t b_cols = sizeof(int32_t) * (size_t)np, b_out = sizeof(uint16_t) * (size_t)np;
     size_t o_q, o_t, o_row, o_cols, o_out, total;
@@ -1292,16 +1280,14 @@ extern "C" int orbfe_hamming_csr(OrbfeMatcher *m, const uint8_t *q, int nq, cons
     memcpy(H + o_t, t, b_t);
     memcpy(H + o_row, row_ptr, b_row);
     memcpy(H + o_cols, cols, b_cols);
-    cudaStream_t s = m->stream;
-    CU_TRY(cudaMemcpyAsync(D, H, o_out, cudaMemcpyHostToDevice, s));
-    if (int rc = orbfe_hamming_csr_device(m, D + o_q, D + o_t, (const int32_t *)(D + o_row), (const int32_t *)(D + o_cols), nq, np,
-                                          (uint16_t *)(D + o_out), s))
+    if (int rc = matcher_round_trip(m, false, o_out, o_out, total, [&]() -> int {
+            if (int rc = orbfe_hamming_csr_device(m, D + o_q, D + o_t, (const int32_t *)(D + o_row), (const int32_t *)(D + o_cols), nq,
+                                                  np, (uint16_t *)(D + o_out), m->stream))
+                return rc;
+            m->launches += 1;
+            return ORBFE_OK;
+        }))
         return rc;
-    m->launches += 1;
-    CU_TRY(cudaMemcpyAsync(H + o_out, D + o_out, total - o_out, cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaStreamSynchronize(s));
-    m->h2d_bytes += o_out;
-    m->d2h_bytes += total - o_out;
     memcpy(out, H + o_out, b_out);
     return ORBFE_OK;
 }
@@ -1312,21 +1298,19 @@ extern "C" int orbfe_hamming_dense(OrbfeMatcher *m, const uint8_t *q, int nq, co
     if (!m || nq < 0 || nt < 0) return fail(ORBFE_ERR_ARG, "bad arguments");
     if (nq == 0 || nt == 0) return ORBFE_OK;
     if (!q || !t || !out) return fail(ORBFE_ERR_ARG, "NULL argument");
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     const size_t b_q = (size_t)nq * 32, b_t = (size_t)nt * 32, b_out = sizeof(uint16_t) * (size_t)nq * nt;
     size_t o_q, o_t, o_out, total;
     if (int rc = m->stage.layout({{&o_q, b_q}, {&o_t, b_t}, {&o_out, b_out}}, &total)) return rc;
     unsigned char *H = m->stage.h, *D = m->stage.d;
     memcpy(H + o_q, q, b_q);
     memcpy(H + o_t, t, b_t);
-    cudaStream_t s = m->stream;
-    CU_TRY(cudaMemcpyAsync(D, H, o_out, cudaMemcpyHostToDevice, s));
-    launch_hamming_dense(D + o_q, nq, D + o_t, nt, (uint16_t *)(D + o_out), s);
-    CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(H + o_out, D + o_out, total - o_out, cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaStreamSynchronize(s));
-    m->h2d_bytes += o_out;
-    m->d2h_bytes += total - o_out;
+    if (int rc = matcher_round_trip(m, false, o_out, o_out, total, [&]() -> int {
+            launch_hamming_dense(D + o_q, nq, D + o_t, nt, (uint16_t *)(D + o_out), m->stream);
+            ORBFE_CUDA_TRY(cudaGetLastError());
+            return ORBFE_OK;
+        }))
+        return rc;
     memcpy(out, H + o_out, b_out);
     return ORBFE_OK;
 }
@@ -1337,14 +1321,14 @@ extern "C" int orbfe_undistort_keypoints_device(OrbfeMatcher *m, const OrbfeKeyP
     if (!m || n < 0 || !dist5 || !(fx != 0.f) || !(fy != 0.f)) return fail(ORBFE_ERR_ARG, "bad arguments");
     if (n == 0) return ORBFE_OK;
     if (!d_in || !d_out) return fail(ORBFE_ERR_ARG, "NULL argument");
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : m->stream;
     if (dist5[0] == 0.0f) {  // mvKeysUn = mvKeys (Frame.cc:291-295)
-        if (d_in != d_out) CU_TRY(cudaMemcpyAsync(d_out, d_in, sizeof(OrbfeKeyPoint) * (size_t)n, cudaMemcpyDeviceToDevice, s));
+        if (d_in != d_out) ORBFE_CUDA_TRY(cudaMemcpyAsync(d_out, d_in, sizeof(OrbfeKeyPoint) * (size_t)n, cudaMemcpyDeviceToDevice, s));
         return ORBFE_OK;
     }
     launch_undistort(fx, fy, cx, cy, dist5, d_in, d_out, n, s);
-    CU_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     m->launches += 1;
     return ORBFE_OK;
 }
@@ -1358,19 +1342,16 @@ extern "C" int orbfe_undistort_keypoints(OrbfeMatcher *m, const OrbfeKeyPoint *i
         if (in != out) memcpy(out, in, sizeof(OrbfeKeyPoint) * (size_t)n);
         return ORBFE_OK;
     }
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     // one array, undistorted in place on the device: input and output of the block at once
     size_t o_kps, total;
     if (int rc = m->stage.layout({{&o_kps, sizeof(OrbfeKeyPoint) * (size_t)n}}, &total)) return rc;
     OrbfeKeyPoint *h_kps = (OrbfeKeyPoint *)m->stage.h, *d_kps = (OrbfeKeyPoint *)m->stage.d;
     memcpy(h_kps, in, sizeof(OrbfeKeyPoint) * (size_t)n);
-    cudaStream_t s = m->stream;
-    CU_TRY(cudaMemcpyAsync(d_kps, h_kps, total, cudaMemcpyHostToDevice, s));
-    if (int rc = orbfe_undistort_keypoints_device(m, d_kps, d_kps, n, fx, fy, cx, cy, dist5, s)) return rc;
-    CU_TRY(cudaMemcpyAsync(h_kps, d_kps, total, cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaStreamSynchronize(s));
-    m->h2d_bytes += total;
-    m->d2h_bytes += total;
+    if (int rc = matcher_round_trip(m, false, total, 0, total, [&] {
+            return orbfe_undistort_keypoints_device(m, d_kps, d_kps, n, fx, fy, cx, cy, dist5, m->stream);
+        }))
+        return rc;
     memcpy(out, h_kps, sizeof(OrbfeKeyPoint) * (size_t)n);
     return ORBFE_OK;
 }
@@ -1404,21 +1385,19 @@ extern "C" int orbfe_distinctive_descriptors(OrbfeMatcher *m, const uint8_t *des
     if (group_ptr[0] != 0 || total < 0 || (total > 0 && !desc)) return fail(ORBFE_ERR_ARG, "bad group_ptr");
     for (int g = 0; g < ngroups; g++)
         if (group_ptr[g + 1] < group_ptr[g]) return fail(ORBFE_ERR_ARG, "group_ptr must be non-decreasing");
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     const size_t b_desc = (size_t)total * 32, b_ptr = sizeof(int) * ((size_t)ngroups + 1), b_best = sizeof(int) * (size_t)ngroups;
     size_t o_desc, o_ptr, o_best, nbytes;
     if (int rc = m->stage.layout({{&o_desc, b_desc}, {&o_ptr, b_ptr}, {&o_best, b_best}}, &nbytes)) return rc;
     unsigned char *H = m->stage.h, *D = m->stage.d;
     if (total > 0) memcpy(H + o_desc, desc, b_desc);   // all groups empty: nothing to upload, the launch still writes every -1
     memcpy(H + o_ptr, group_ptr, b_ptr);
-    cudaStream_t s = m->stream;
-    CU_TRY(cudaMemcpyAsync(D, H, o_best, cudaMemcpyHostToDevice, s));
-    launch_distinctive(D + o_desc, (const int *)(D + o_ptr), ngroups, (int *)(D + o_best), s);
-    CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(H + o_best, D + o_best, nbytes - o_best, cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaStreamSynchronize(s));
-    m->h2d_bytes += o_best;
-    m->d2h_bytes += nbytes - o_best;
+    if (int rc = matcher_round_trip(m, false, o_best, o_best, nbytes, [&]() -> int {
+            launch_distinctive(D + o_desc, (const int *)(D + o_ptr), ngroups, (int *)(D + o_best), m->stream);
+            ORBFE_CUDA_TRY(cudaGetLastError());
+            return ORBFE_OK;
+        }))
+        return rc;
     m->launches += 1;
     memcpy(best_out, H + o_best, b_best);
     return ORBFE_OK;
@@ -1436,10 +1415,10 @@ extern "C" int orbfe_distinctive_descriptors_device(OrbfeMatcher *m, int ngroups
         return fail(ORBFE_ERR_ARG, "orbfe_distinctive_descriptors_device: NULL argument");
     if (((uintptr_t)d_desc | (uintptr_t)d_mp_desc) % 16)
         return fail(ORBFE_ERR_ARG, "orbfe_distinctive_descriptors_device: d_desc and d_mp_desc must be 16-byte aligned");
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : m->stream;
     launch_distinctive_obs(d_desc, d_counts, nframes, cap, d_group_ptr, d_obs, nobs, ngroups, d_best, d_mp_desc, m->d_err, s);
-    CU_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     m->launches += 1;
     return ORBFE_OK;
 }
@@ -1458,11 +1437,11 @@ extern "C" int orbfe_normal_and_depth_device(OrbfeMatcher *m, int npoints, const
     if (!d_kps || !d_counts || !d_centers || !d_group_ptr || !d_obs || !d_world || !d_ref_obs || !scale_factors || !d_normal ||
         !d_min_dist || !d_max_dist)
         return fail(ORBFE_ERR_ARG, "orbfe_normal_and_depth_device: NULL argument");
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : m->stream;
     launch_normal_depth_obs(d_kps, d_counts, nframes, cap, d_centers, d_group_ptr, d_obs, nobs, d_world, d_ref_obs, scale_factor, nlevels,
                             scale_factors, npoints, d_normal, d_min_dist, d_max_dist, m->d_err, s);
-    CU_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     m->launches += 1;
     return ORBFE_OK;
 }
@@ -1483,7 +1462,7 @@ extern "C" int orbfe_normal_and_depth(OrbfeMatcher *m, int npoints, const float 
         if (group_ptr[g + 1] > group_ptr[g] && (ref_octave[g] < 0 || ref_octave[g] >= nlevels))
             return fail(ORBFE_ERR_ARG, "orbfe_normal_and_depth: point %d has reference octave %d outside [0, %d)", g, ref_octave[g], nlevels);
     }
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     const size_t NP = (size_t)npoints, b3 = 3 * sizeof(float) * NP, b1 = sizeof(float) * NP;
     size_t o_world, o_ref, o_oct, o_ptr, o_obs, o_normal, o_min, o_max, nbytes;
     if (int rc = m->stage.layout({{&o_world, b3}, {&o_ref, b3}, {&o_oct, sizeof(int) * NP}, {&o_ptr, sizeof(int) * (NP + 1)},
@@ -1500,16 +1479,14 @@ extern "C" int orbfe_normal_and_depth(OrbfeMatcher *m, int npoints, const float 
     memcpy(H + o_normal, normal_out, b3);
     memcpy(H + o_min, min_dist_out, b1);
     memcpy(H + o_max, max_dist_out, b1);
-    cudaStream_t s = m->stream;
-    CU_TRY(cudaMemcpyAsync(D, H, nbytes, cudaMemcpyHostToDevice, s));
-    launch_normal_depth((const float *)(D + o_obs), (const int *)(D + o_ptr), (const float *)(D + o_world), (const float *)(D + o_ref),
-                        (const int *)(D + o_oct), scale_factor, nlevels, scale_factors, npoints, (float *)(D + o_normal),
-                        (float *)(D + o_min), (float *)(D + o_max), s);
-    CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(H + o_normal, D + o_normal, nbytes - o_normal, cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaStreamSynchronize(s));
-    m->h2d_bytes += nbytes;
-    m->d2h_bytes += nbytes - o_normal;
+    if (int rc = matcher_round_trip(m, false, nbytes, o_normal, nbytes, [&]() -> int {
+            launch_normal_depth((const float *)(D + o_obs), (const int *)(D + o_ptr), (const float *)(D + o_world),
+                                (const float *)(D + o_ref), (const int *)(D + o_oct), scale_factor, nlevels, scale_factors, npoints,
+                                (float *)(D + o_normal), (float *)(D + o_min), (float *)(D + o_max), m->stream);
+            ORBFE_CUDA_TRY(cudaGetLastError());
+            return ORBFE_OK;
+        }))
+        return rc;
     m->launches += 1;
     memcpy(normal_out, H + o_normal, b3);
     memcpy(min_dist_out, H + o_min, b1);
@@ -1521,7 +1498,7 @@ extern "C" int orbfe_normal_and_depth(OrbfeMatcher *m, int npoints, const float 
 int orbfe::bow_db_score(OrbfeMatcher *m, int nq, const int32_t *q_ids, const double *q_vals, int nkf, const int32_t *kf_ptr,
                         const int32_t *db_ids, const double *db_vals, int32_t *common, int32_t *first, double *score) {
     const size_t NQ = (size_t)nq, NK = (size_t)nkf, nw = (size_t)kf_ptr[nkf];
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     size_t o_qi, o_qv, o_kp, o_di, o_dv, o_c, o_f, o_s, total;
     if (int rc = m->stage.layout({{&o_qi, NQ * sizeof(int)}, {&o_qv, NQ * sizeof(double)}, {&o_kp, (NK + 1) * sizeof(int)},
                                   {&o_di, nw * sizeof(int)}, {&o_dv, nw * sizeof(double)}, {&o_c, NK * sizeof(int)},
@@ -1538,15 +1515,14 @@ int orbfe::bow_db_score(OrbfeMatcher *m, int nq, const int32_t *q_ids, const dou
         memcpy(H + o_di, db_ids, nw * sizeof(int));
         memcpy(H + o_dv, db_vals, nw * sizeof(double));
     }
-    cudaStream_t s = m->stream;
-    CU_TRY(cudaMemcpyAsync(D, H, o_c, cudaMemcpyHostToDevice, s));
-    launch_bow_db_score(nq, (const int *)(D + o_qi), (const double *)(D + o_qv), nkf, (const int *)(D + o_kp), (const int *)(D + o_di),
-                        (const double *)(D + o_dv), (int *)(D + o_c), (int *)(D + o_f), (double *)(D + o_s), s);
-    CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(H + o_c, D + o_c, total - o_c, cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaStreamSynchronize(s));
-    m->h2d_bytes += o_c;
-    m->d2h_bytes += total - o_c;
+    if (int rc = matcher_round_trip(m, false, o_c, o_c, total, [&]() -> int {
+            launch_bow_db_score(nq, (const int *)(D + o_qi), (const double *)(D + o_qv), nkf, (const int *)(D + o_kp),
+                                (const int *)(D + o_di), (const double *)(D + o_dv), (int *)(D + o_c), (int *)(D + o_f),
+                                (double *)(D + o_s), m->stream);
+            ORBFE_CUDA_TRY(cudaGetLastError());
+            return ORBFE_OK;
+        }))
+        return rc;
     m->launches += 1;
     memcpy(common, H + o_c, NK * sizeof(int));
     memcpy(first, H + o_f, NK * sizeof(int));
@@ -1560,10 +1536,10 @@ extern "C" int orbfe_knn2_groups_device(OrbfeMatcher *m, const uint8_t *d_q, int
     if (!m || nq < 0 || ngroups < 0 || group_size < 0) return fail(ORBFE_ERR_ARG, "bad arguments");
     if (nq == 0 || ngroups == 0) return ORBFE_OK;
     if (!d_q || !d_db || !d_best || !d_best_idx || !d_second) return fail(ORBFE_ERR_ARG, "NULL argument");
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     launch_knn2_groups(d_q, nq, d_db, ngroups, group_size, d_best, d_best_idx, d_second,
                        stream ? (cudaStream_t)stream : m->stream);
-    CU_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaGetLastError());
     return ORBFE_OK;
 }
 
@@ -1574,7 +1550,7 @@ extern "C" int orbfe_knn2_groups(OrbfeMatcher *m, const uint8_t *q, int nq, cons
     if (!m || nq < 0 || ngroups < 0 || group_size < 0) return fail(ORBFE_ERR_ARG, "bad arguments");
     if (nq == 0 || ngroups == 0) return ORBFE_OK;
     if (!q || !db || !best || !best_idx || !second) return fail(ORBFE_ERR_ARG, "NULL argument");
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     const size_t no = (size_t)ngroups * nq;
     const size_t b_q = (size_t)nq * 32, b_db = (size_t)ngroups * group_size * 32;
     size_t o_q, o_db, o_best, o_idx, o_second, total;
@@ -1585,15 +1561,11 @@ extern "C" int orbfe_knn2_groups(OrbfeMatcher *m, const uint8_t *q, int nq, cons
     unsigned char *H = m->stage.h, *D = m->stage.d;
     memcpy(H + o_q, q, b_q);
     memcpy(H + o_db, db, b_db);
-    cudaStream_t s = m->stream;
-    CU_TRY(cudaMemcpyAsync(D, H, o_best, cudaMemcpyHostToDevice, s));
-    if (int rc = orbfe_knn2_groups_device(m, D + o_q, nq, D + o_db, ngroups, group_size, (uint16_t *)(D + o_best), (int32_t *)(D + o_idx),
-                                          (uint16_t *)(D + o_second), s))
+    if (int rc = matcher_round_trip(m, false, o_best, o_best, total, [&] {
+            return orbfe_knn2_groups_device(m, D + o_q, nq, D + o_db, ngroups, group_size, (uint16_t *)(D + o_best),
+                                            (int32_t *)(D + o_idx), (uint16_t *)(D + o_second), m->stream);
+        }))
         return rc;
-    CU_TRY(cudaMemcpyAsync(H + o_best, D + o_best, total - o_best, cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaStreamSynchronize(s));
-    m->h2d_bytes += o_best;
-    m->d2h_bytes += total - o_best;
     memcpy(best, H + o_best, sizeof(uint16_t) * no);
     memcpy(best_idx, H + o_idx, sizeof(int32_t) * no);
     memcpy(second, H + o_second, sizeof(uint16_t) * no);
@@ -1611,15 +1583,9 @@ extern "C" int orbfe_knn2_groups(OrbfeMatcher *m, const uint8_t *q, int nq, cons
 // (sbp_device_kernel, d_err[1]); the call then runs once more from the caller's arrays with exactly that scratch.
 template <class Pack, class Launch>
 static int run_staged(OrbfeMatcher *m, size_t inout, size_t out, size_t total, size_t per_job, Pack pack_inout, Launch launch) {
-    cudaStream_t s = m->stream;
     for (bool grown = false;; grown = true) {
         pack_inout();
-        CU_TRY(cudaMemcpyAsync(m->stage.d, m->stage.h, out, cudaMemcpyHostToDevice, s));
-        if (int rc = launch(per_job)) return rc;
-        CU_TRY(cudaMemcpyAsync(m->stage.h + inout, m->stage.d + inout, total - inout, cudaMemcpyDeviceToHost, s));
-        const int rc = orbfe_matcher_sync(m);
-        m->h2d_bytes += out;
-        m->d2h_bytes += total - inout;
+        const int rc = matcher_round_trip(m, true, out, inout, total, [&] { return launch(per_job); });
         if (rc != ORBFE_ERR_CAPACITY || grown) return rc;
         per_job = (size_t)m->h_err[1];
     }
@@ -1658,7 +1624,7 @@ int orbfe::sbp_frames_host(OrbfeMatcher *m, int npairs, const OrbfeFrameView *cu
             if (group[j] == g) order.push_back(j);
     }
     gbeg.push_back(npairs);
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     // frame slots: a frame that appears several times (in a video stream the Last frame of pair j is the Current
     // frame of pair j-1) is staged and uploaded once.  Identity = same keypoint and descriptor arrays.
     // A frame used as Last carries that pair's world/flags arrays; two pairs that share a Last frame but pass
@@ -1787,7 +1753,7 @@ int orbfe::guided_host(OrbfeMatcher *m, const OrbfeFrameView &f, int nq, const G
     const int cap = f.n;
     const int qcap = check_orientation ? nq : sbp_fit_qcap(cap, nq);   // queries per launch
     const int nchunks = (nq + qcap - 1) / qcap;
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     size_t o_kps, o_desc, o_cnt, o_fi, o_qb, o_qc, o_qu, o_qv, o_qr, o_qa, o_lo, o_hi, o_qd, o_mp, o_nm, o_best, total;
     const size_t nc4 = (size_t)nchunks * sizeof(int);
     if (int rc = m->stage.layout({{&o_kps, (size_t)cap * sizeof(OrbfeKeyPoint)}, {&o_desc, (size_t)cap * 32}, {&o_cnt, sizeof(int)},
@@ -1851,7 +1817,7 @@ int orbfe::init_host(OrbfeMatcher *m, const OrbfeFrameView &f1, const OrbfeFrame
                      float nnratio, int check_orientation, int *match12_out, int *nmatches_out) {
     const int cap = std::max({f1.n, f2.n, 1});
     const size_t C = (size_t)cap;
-    CU_TRY(cudaSetDevice(m->device));
+    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     size_t o_kps, o_desc, o_cnt, o_idx, o_prev, o_m12, o_nm, total;
     if (int rc = m->stage.layout({{&o_kps, 2 * C * sizeof(OrbfeKeyPoint)}, {&o_desc, 2 * C * 32}, {&o_cnt, 2 * sizeof(int)},
                                   {&o_idx, 2 * sizeof(int)}, {&o_prev, C * 2 * sizeof(float)}, {&o_m12, C * sizeof(int)},

@@ -6,8 +6,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <initializer_list>
 #include <utility>
+#include <vector>
 
 #include "../../include/orbfe.h"
 #include "../../include/orbfe_match.h"
@@ -202,10 +204,70 @@ void launch_undistort(float fx, float fy, float cx, float cy, const float *dist5
 // records the thread's last-error string (orbfe_last_error) and returns `code`
 int set_error(int code, const char *fmt, ...);
 
+// returns ORBFE_ERR_CUDA from the enclosing function, naming the failed call in orbfe_last_error, when `expr` is not cudaSuccess
+#define ORBFE_CUDA_TRY(expr)                                                                                                   \
+    do {                                                                                                                       \
+        cudaError_t e__ = (expr);                                                                                              \
+        if (e__ != cudaSuccess)                                                                                                \
+            return orbfe::set_error(ORBFE_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
+    } while (0)
+
+// The device arrays a handle owns: every alloc is recorded (at least 256 bytes each) and release() frees them all, so an
+// array is named once, where it is allocated.  Pinned host memory, streams and events are not kept here.
+struct DeviceBuffers {
+    std::vector<void *> ptrs;
+    template <class T>
+    cudaError_t alloc(T **p, size_t count) {
+        void *q = nullptr;
+        const cudaError_t e = cudaMalloc(&q, std::max<size_t>(count * sizeof(T), 256));
+        if (e == cudaSuccess) { ptrs.push_back(q); *p = (T *)q; }
+        return e;
+    }
+    void release() {
+        for (void *q : ptrs) cudaFree(q);
+        ptrs.clear();
+    }
+};
+
+// The own stream of a handle whose entries may also run on caller streams, and the rule that makes that safe: every call
+// enters (its stream waits for the handle's last work) and leaves (records its own), so the handle's calls run in call order
+// whichever streams they were enqueued on.
+struct HandleStream {
+    int device = 0;
+    cudaStream_t stream = nullptr;   // non-blocking
+    cudaEvent_t last = nullptr;      // the handle's most recent work
+    cudaError_t create(int dev) {
+        device = dev;
+        cudaError_t e = cudaSetDevice(dev);
+        if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&last, cudaEventDisableTiming);
+        return e;
+    }
+    void destroy() {
+        if (last) cudaEventDestroy(last);
+        if (stream) cudaStreamDestroy(stream);
+        last = nullptr;
+        stream = nullptr;
+    }
+    // the caller's stream if one was given, else the handle's own
+    cudaStream_t pick(void *caller) const { return caller ? (cudaStream_t)caller : stream; }
+    int enter(cudaStream_t s) {
+        ORBFE_CUDA_TRY(cudaSetDevice(device));
+        ORBFE_CUDA_TRY(cudaStreamWaitEvent(s, last, 0));
+        return ORBFE_OK;
+    }
+    int leave(cudaStream_t s, bool sync) {
+        ORBFE_CUDA_TRY(cudaGetLastError());
+        ORBFE_CUDA_TRY(cudaEventRecord(last, s));
+        if (sync) ORBFE_CUDA_TRY(cudaStreamSynchronize(s));
+        return ORBFE_OK;
+    }
+};
+
 // Staging block of every host-array entry of a matcher or vocabulary handle: a grow-only pinned host block h and its device
-// twin d.  The entry packs h, copies it to d in one H2D, runs its kernels, copies the results back in one D2H and
-// synchronises before it returns.  Both keep the size (times 1.25) of the largest call the handle has seen.  The block serves
-// one call at a time: the vocabulary holds its mutex across each call.
+// twin d.  The entry lays out and packs h, moves it with round_trip and synchronises before it reads the results.  Both keep
+// the size (times 1.25) of the largest call the handle has seen.  The block serves one call at a time: the vocabulary holds
+// its mutex across each call.
 struct Stage {
     unsigned char *h = nullptr;
     unsigned char *d = nullptr;
@@ -214,6 +276,15 @@ struct Stage {
     // block to hold it (ORBFE_ERR_CUDA on a failed allocation)
     int layout(std::initializer_list<std::pair<size_t *, size_t>> arrays, size_t *total);
     void release();
+    // on stream s: the inputs [0, up) to the device, enqueue() (the call's kernels; returns an orbfe code), the outputs
+    // [down, total) back.  Returns the first error; the caller synchronises s before it reads h.
+    template <class Enqueue>
+    int round_trip(cudaStream_t s, size_t up, size_t down, size_t total, Enqueue enqueue) {
+        ORBFE_CUDA_TRY(cudaMemcpyAsync(d, h, up, cudaMemcpyHostToDevice, s));
+        if (int rc = enqueue()) return rc;
+        ORBFE_CUDA_TRY(cudaMemcpyAsync(h + down, d + down, total - down, cudaMemcpyDeviceToHost, s));
+        return ORBFE_OK;
+    }
 };
 
 // ---- launchers (match_kernels.cu) ----

@@ -14,6 +14,7 @@ struct OrbfeVocabulary {
     int nwords = 0;                 // largest word id + 1
     int nchild = 0;                 // entries of d_children (child_ptr[nnodes])
     cudaStream_t stream = nullptr;
+    orbfe::DeviceBuffers mem;       // the node table below
     uint8_t *d_desc = nullptr;
     uint8_t *d_live = nullptr;      // per node: weight > 0 (the FeatureVector skips stopped words)
     int *d_child_ptr = nullptr, *d_children = nullptr;

@@ -378,19 +378,13 @@ __global__ void __launch_bounds__(kRsThreads) rs_scatter_kernel(const int *__res
     }
 }
 
-#define VT_TRY(expr)                                                                                                  \
-    do {                                                                                                              \
-        cudaError_t e__ = (expr);                                                                                     \
-        if (e__ != cudaSuccess)                                                                                       \
-            return set_error(ORBFE_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-    } while (0)
-
 // Everything load_text allocates besides the vocabulary itself; released on every return.
 struct Scratch {
     FILE *f = nullptr;
     unsigned char *h_stage[2] = {nullptr, nullptr};
     cudaEvent_t ev[2] = {nullptr, nullptr};
     cudaStream_t s0 = nullptr;
+    DeviceBuffers mem;                 // the device arrays below
     uint8_t *d_text = nullptr;
     int *d_tiles = nullptr, *d_sums = nullptr, *d_starts = nullptr, *d_parent = nullptr, *d_leaf = nullptr, *d_cnt = nullptr;
     int *d_keys[2] = {nullptr, nullptr}, *d_vals = nullptr, *d_hist = nullptr, *d_scal = nullptr;
@@ -405,10 +399,7 @@ struct Scratch {
             if (ev[b]) cudaEventDestroy(ev[b]);
         }
         if (s0) cudaStreamDestroy(s0);
-        for (void *p : {(void *)d_text, (void *)d_tiles, (void *)d_sums, (void *)d_starts, (void *)d_parent, (void *)d_leaf, (void *)d_cnt,
-                        (void *)d_keys[0], (void *)d_keys[1], (void *)d_vals, (void *)d_hist, (void *)d_scal, (void *)d_err, (void *)d_fb,
-                        (void *)d_fbw})
-            cudaFree(p);
+        mem.release();
         if (v) orbfe_vocabulary_destroy(v);
     }
 };
@@ -482,28 +473,28 @@ extern "C" int orbfe_vocabulary_load_text(int device, const char *path, OrbfeVoc
         return set_error(ORBFE_ERR_NO_DEVICE, "no CUDA device: this library has no CPU fallback");
     }
     if (device < 0 || device >= ndev) return set_error(ORBFE_ERR_ARG, "device %d out of range", device);
-    VT_TRY(cudaSetDevice(device));
+    ORBFE_CUDA_TRY(cudaSetDevice(device));
 
     // ---- the body into device memory, chunk by chunk through two pinned buffers ----
-    VT_TRY(cudaStreamCreateWithFlags(&S.s0, cudaStreamNonBlocking));
+    ORBFE_CUDA_TRY(cudaStreamCreateWithFlags(&S.s0, cudaStreamNonBlocking));
     cudaStream_t s = S.s0;
     const int ntl = std::max(div_up(T, kNlTile), 1);
-    VT_TRY(cudaMalloc((void **)&S.d_text, (size_t)T + 32));
-    VT_TRY(cudaMalloc((void **)&S.d_tiles, sizeof(int) * (size_t)ntl));
-    VT_TRY(cudaMalloc((void **)&S.d_sums, sizeof(int) * (size_t)(div_up(std::max<long long>(ntl, 2ll * T + 1024), kScTile) + 1)));
-    VT_TRY(cudaMalloc((void **)&S.d_scal, sizeof(int) * 8));
-    VT_TRY(cudaMalloc((void **)&S.d_err, sizeof(unsigned long long)));
+    ORBFE_CUDA_TRY(S.mem.alloc(&S.d_text, (size_t)T + 32));
+    ORBFE_CUDA_TRY(S.mem.alloc(&S.d_tiles, (size_t)ntl));
+    ORBFE_CUDA_TRY(S.mem.alloc(&S.d_sums, (size_t)(div_up(std::max<long long>(ntl, 2ll * T + 1024), kScTile) + 1)));
+    ORBFE_CUDA_TRY(S.mem.alloc(&S.d_scal, 8));
+    ORBFE_CUDA_TRY(S.mem.alloc(&S.d_err, 1));
     for (int b = 0; b < 2; b++) {
-        VT_TRY(cudaHostAlloc((void **)&S.h_stage[b], kChunk, cudaHostAllocDefault));
-        VT_TRY(cudaEventCreateWithFlags(&S.ev[b], cudaEventDisableTiming));
+        ORBFE_CUDA_TRY(cudaHostAlloc((void **)&S.h_stage[b], kChunk, cudaHostAllocDefault));
+        ORBFE_CUDA_TRY(cudaEventCreateWithFlags(&S.ev[b], cudaEventDisableTiming));
     }
     for (long long off = 0, k = 0; off < T; k++) {
         const int b = (int)(k & 1);
-        if (k >= 2) VT_TRY(cudaEventSynchronize(S.ev[b]));
+        if (k >= 2) ORBFE_CUDA_TRY(cudaEventSynchronize(S.ev[b]));
         const size_t len = (size_t)std::min<long long>(kChunk, T - off);
         if (fread(S.h_stage[b], 1, len, S.f) != len) return set_error(ORBFE_ERR_ARG, "cannot read %s: short read", path);
-        VT_TRY(cudaMemcpyAsync(S.d_text + off, S.h_stage[b], len, cudaMemcpyHostToDevice, s));
-        VT_TRY(cudaEventRecord(S.ev[b], s));
+        ORBFE_CUDA_TRY(cudaMemcpyAsync(S.d_text + off, S.h_stage[b], len, cudaMemcpyHostToDevice, s));
+        ORBFE_CUDA_TRY(cudaEventRecord(S.ev[b], s));
         off += (long long)len;
     }
     fclose(S.f);
@@ -511,78 +502,78 @@ extern "C" int orbfe_vocabulary_load_text(int device, const char *path, OrbfeVoc
 
     // ---- line starts ----
     int *d_nl = S.d_scal;           // scalars: [0] newlines, [1] fallbacks, [2] last line blank, [3] leaf flags
-    VT_TRY(cudaMemsetAsync(S.d_scal, 0, sizeof(int) * 8, s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(S.d_scal, 0, sizeof(int) * 8, s));
     if (T > 0) {
         nl_count_kernel<<<ntl, kNlThreads, 0, s>>>(S.d_text, T, S.d_tiles);
         scan_excl(S.d_tiles, S.d_tiles, ntl, S.d_sums, d_nl, s);
     }
     int nl = 0;
-    VT_TRY(cudaMemcpyAsync(&nl, d_nl, sizeof(int), cudaMemcpyDeviceToHost, s));
-    VT_TRY(cudaStreamSynchronize(s));
-    VT_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(&nl, d_nl, sizeof(int), cudaMemcpyDeviceToHost, s));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(s));
+    ORBFE_CUDA_TRY(cudaGetLastError());
     if ((long long)nl + 2 > INT_MAX) return set_error(ORBFE_ERR_ARG, "%s: more than %d nodes", path, INT_MAX);
     const int cap = nl + 2;         // nodes if the text after the last newline is a node line
-    VT_TRY(cudaMalloc((void **)&S.d_starts, sizeof(int) * ((size_t)nl + 1)));
-    VT_TRY(cudaMemsetAsync(S.d_starts, 0, sizeof(int), s));
+    ORBFE_CUDA_TRY(S.mem.alloc(&S.d_starts, (size_t)nl + 1));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(S.d_starts, 0, sizeof(int), s));
     if (nl > 0) nl_starts_kernel<<<ntl, kNlThreads, 0, s>>>(S.d_text, T, S.d_tiles, S.d_starts);
 
     // ---- parse into the vocabulary's own table ----
     OrbfeVocabulary *v = S.v = new OrbfeVocabulary();
     v->device = device;
-    VT_TRY(vocab_alloc(v, cap, cap - 1));
-    VT_TRY(cudaMalloc((void **)&S.d_parent, sizeof(int) * (size_t)cap));
-    VT_TRY(cudaMalloc((void **)&S.d_leaf, sizeof(int) * (size_t)cap));
-    VT_TRY(cudaMalloc((void **)&S.d_fb, sizeof(FbSlot) * ((size_t)nl + 1)));
-    VT_TRY(cudaMemsetAsync(S.d_parent, 0, sizeof(int), s));
-    VT_TRY(cudaMemsetAsync(S.d_leaf, 0, sizeof(int), s));
-    VT_TRY(cudaMemsetAsync(v->d_weight, 0, sizeof(double), s));
-    VT_TRY(cudaMemsetAsync(v->d_desc, 0, 32, s));
-    VT_TRY(cudaMemsetAsync(S.d_err, 0xFF, sizeof(unsigned long long), s));
+    ORBFE_CUDA_TRY(vocab_alloc(v, cap, cap - 1));
+    ORBFE_CUDA_TRY(S.mem.alloc(&S.d_parent, (size_t)cap));
+    ORBFE_CUDA_TRY(S.mem.alloc(&S.d_leaf, (size_t)cap));
+    ORBFE_CUDA_TRY(S.mem.alloc(&S.d_fb, (size_t)nl + 1));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(S.d_parent, 0, sizeof(int), s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(S.d_leaf, 0, sizeof(int), s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(v->d_weight, 0, sizeof(double), s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(v->d_desc, 0, 32, s));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(S.d_err, 0xFF, sizeof(unsigned long long), s));
     parse_kernel<<<div_up((long long)nl + 1, 256), 256, 0, s>>>(S.d_text, T, S.d_starts, nl, S.d_parent, S.d_leaf,
                                                                 reinterpret_cast<uint32_t *>(v->d_desc), v->d_weight, S.d_fb,
                                                                 S.d_scal + 1, S.d_err, S.d_scal + 2);
     int scal[3];
     unsigned long long err = 0;
-    VT_TRY(cudaMemcpyAsync(scal, S.d_scal, sizeof(scal), cudaMemcpyDeviceToHost, s));
-    VT_TRY(cudaMemcpyAsync(&err, S.d_err, sizeof(err), cudaMemcpyDeviceToHost, s));
-    VT_TRY(cudaStreamSynchronize(s));
-    VT_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(scal, S.d_scal, sizeof(scal), cudaMemcpyDeviceToHost, s));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(&err, S.d_err, sizeof(err), cudaMemcpyDeviceToHost, s));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(s));
+    ORBFE_CUDA_TRY(cudaGetLastError());
     if (err != ~0ull) return set_error(ORBFE_ERR_ARG, "%s: line %llu: %s", path, err >> 8, error_text((int)(err & 0xFF)));
     const int nfb = scal[1];
     const int nnodes = 1 + nl + (scal[2] ? 0 : 1);
 
     // ---- weights the device did not convert: `>> double` on their tokens, in batches through the staging buffers ----
     if (nfb > 0) {
-        VT_TRY(cudaMalloc((void **)&S.d_fbw, sizeof(double) * (size_t)nfb));
+        ORBFE_CUDA_TRY(S.mem.alloc(&S.d_fbw, (size_t)nfb));
         const int batch = (int)(kChunk / sizeof(FbSlot));
         const FbSlot *slots = reinterpret_cast<const FbSlot *>(S.h_stage[0]);
         double *w = reinterpret_cast<double *>(S.h_stage[1]);
         std::string tok;
         for (int b0 = 0; b0 < nfb; b0 += batch) {
             const int nb = std::min(batch, nfb - b0);
-            VT_TRY(cudaMemcpyAsync(S.h_stage[0], S.d_fb + b0, sizeof(FbSlot) * (size_t)nb, cudaMemcpyDeviceToHost, s));
-            VT_TRY(cudaStreamSynchronize(s));   // also: the previous batch's weights have left h_stage[1]
+            ORBFE_CUDA_TRY(cudaMemcpyAsync(S.h_stage[0], S.d_fb + b0, sizeof(FbSlot) * (size_t)nb, cudaMemcpyDeviceToHost, s));
+            ORBFE_CUDA_TRY(cudaStreamSynchronize(s));   // also: the previous batch's weights have left h_stage[1]
             for (int k = 0; k < nb; k++) {
                 const FbSlot &sl = slots[k];
                 if (sl.len < kFbText) {
                     tok.assign(sl.text, (size_t)sl.len);
                 } else {
                     tok.resize((size_t)sl.len);
-                    VT_TRY(cudaMemcpy(&tok[0], S.d_text + sl.start, (size_t)sl.len, cudaMemcpyDeviceToHost));
+                    ORBFE_CUDA_TRY(cudaMemcpy(&tok[0], S.d_text + sl.start, (size_t)sl.len, cudaMemcpyDeviceToHost));
                 }
                 std::istringstream is(tok);
                 double x = 0.0;                 // Node()'s weight: kept when nothing is extracted
                 is >> x;
                 w[k] = x;
             }
-            VT_TRY(cudaMemcpyAsync(S.d_fbw + b0, w, sizeof(double) * (size_t)nb, cudaMemcpyHostToDevice, s));
+            ORBFE_CUDA_TRY(cudaMemcpyAsync(S.d_fbw + b0, w, sizeof(double) * (size_t)nb, cudaMemcpyHostToDevice, s));
         }
         fallback_scatter_kernel<<<div_up(nfb, 256), 256, 0, s>>>(S.d_fb, S.d_fbw, nfb, v->d_weight);
     }
 
     // ---- CSR, word ids, live flags ----
-    VT_TRY(cudaMalloc((void **)&S.d_cnt, sizeof(int) * ((size_t)nnodes + 1)));
-    VT_TRY(cudaMemsetAsync(S.d_cnt, 0, sizeof(int) * ((size_t)nnodes + 1), s));
+    ORBFE_CUDA_TRY(S.mem.alloc(&S.d_cnt, (size_t)nnodes + 1));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(S.d_cnt, 0, sizeof(int) * ((size_t)nnodes + 1), s));
     child_count_kernel<<<div_up(nnodes, 256), 256, 0, s>>>(S.d_parent, nnodes, S.d_cnt);
     scan_excl(S.d_cnt, v->d_child_ptr, nnodes + 1, S.d_sums, nullptr, s);
     scan_excl(S.d_leaf, v->d_word_id, nnodes, S.d_sums, S.d_scal + 3, s);
@@ -592,9 +583,9 @@ extern "C" int orbfe_vocabulary_load_text(int device, const char *path, OrbfeVoc
         int bits = 1;
         while (bits < 31 && (1 << bits) <= nnodes - 1) bits++;
         const int npass = (bits + 7) / 8, ntiles = div_up(nitems, kRsTile);
-        VT_TRY(cudaMalloc((void **)&S.d_hist, sizeof(int) * 256 * (size_t)ntiles));
-        VT_TRY(cudaMalloc((void **)&S.d_vals, sizeof(int) * (size_t)nitems));
-        for (int b = 0; b < 2 && npass > 1; b++) VT_TRY(cudaMalloc((void **)&S.d_keys[b], sizeof(int) * (size_t)nitems));
+        ORBFE_CUDA_TRY(S.mem.alloc(&S.d_hist, 256 * (size_t)ntiles));
+        ORBFE_CUDA_TRY(S.mem.alloc(&S.d_vals, (size_t)nitems));
+        for (int b = 0; b < 2 && npass > 1; b++) ORBFE_CUDA_TRY(S.mem.alloc(&S.d_keys[b], (size_t)nitems));
         const int *keys = S.d_parent + 1, *vals = nullptr;
         for (int ps = 0; ps < npass; ps++) {
             const bool last = ps == npass - 1;
@@ -609,9 +600,9 @@ extern "C" int orbfe_vocabulary_load_text(int device, const char *path, OrbfeVoc
         }
     }
     int nleaf = 0;
-    VT_TRY(cudaMemcpyAsync(&nleaf, S.d_scal + 3, sizeof(int), cudaMemcpyDeviceToHost, s));
-    VT_TRY(cudaStreamSynchronize(s));
-    VT_TRY(cudaGetLastError());
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(&nleaf, S.d_scal + 3, sizeof(int), cudaMemcpyDeviceToHost, s));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(s));
+    ORBFE_CUDA_TRY(cudaGetLastError());
 
     v->nnodes = nnodes;
     v->nchild = nitems;
