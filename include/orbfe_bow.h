@@ -404,6 +404,38 @@ int orbfe_covis_clear(OrbfeCovisGraph *g);
 int orbfe_covis_lists_device(OrbfeCovisGraph *g, int which, int n, const int32_t *slots, int nbest, int32_t *d_ptr, int32_t *d_list,
                              int32_t *d_weights, void *stream);
 
+/* MapPoint::GetObservations() (reference src/MapPoint.cc:93-97) of the n named points d_points[0..n), built on the device as
+ * the inverse of the live slots' map-point rows.  The reference keeps mObservations and mvpMapPoints in step (AddMapPoint /
+ * AddObservation, EraseMapPointMatch / EraseObservation, Replace, both SetBadFlags), so at every call boundary a point's
+ * observations are the live keyframes whose row names it.
+ *   Observers: the live slots (added, not erased).  Slot s's row is d_kf_mp[s*cap + i], i < d_counts[s], as in
+ *   orbfe_covis_update_connections_device: a negative value is NULL or isBad().  A keyframe is an observer from its
+ *   orbfe_covis_add on, so add it when its observations are added (Tracking's initial pair, the start of ProcessNewKeyFrame),
+ *   not while it waits in LocalMapping's queue.
+ *   List of p = d_points[j]: one entry per live slot whose row names p, written s*cap + i.  A row naming p at several
+ *   features gives the largest i (ProcessNewKeyFrame's mObservations[pKF] = i runs in ascending i).  Entries are in key
+ *   order, ascending: the std::map order.  Point j's entries are d_obs[d_ptr[j] .. d_ptr[j+1]); d_ptr (n + 1 entries) is an
+ *   exclusive scan and *d_nobs the total, so (d_ptr, d_obs) is exactly the d_group_ptr / d_obs of
+ *   orbfe_distinctive_descriptors_device, orbfe_normal_and_depth_device and orbfe_covis_update_connections_device.
+ *   d_ref_slot / d_ref_obs (n entries each, both or neither when n > 0): d_ref_obs[j] = ref*cap + i for ref = d_ref_slot[j] (the slot of
+ *   mpRefKF) and i its entry in the list, else ref*cap + 0 (observations[pRefKF] inserts 0): the d_ref_obs of
+ *   orbfe_normal_and_depth_device.
+ * A total over obs_cap writes d_ptr and *d_nobs (the size needed) and nothing else; orbfe_covis_sync then reports
+ * ORBFE_ERR_CAPACITY.  Decided on the device, with only d_ptr written and ORBFE_ERR_ARG from orbfe_covis_sync: a named point
+ * outside [0, npoints) or named twice, a live slot's d_counts[s] outside 0 .. cap, a row value >= npoints, a reference slot
+ * outside [0, nframes).  Host-side ORBFE_ERR_ARG: n < 0, n > npoints, nframes < 1, cap < 1, nframes*cap >= 2^31, obs_cap < 0,
+ * a live slot >= nframes, a NULL array (d_points may be NULL when n = 0, d_obs when obs_cap = 0) or one of d_ref_slot /
+ * d_ref_obs without the other when n > 0, d_scratch not 4-byte aligned;
+ * cap > ORBFE_COVIS_OBS_MAX_CAP is ORBFE_ERR_UNSUPPORTED.
+ * d_scratch: ORBFE_COVIS_OBS_SCRATCH_BYTES(npoints, nframes, cap, obs_cap) bytes of device memory, contents ignored; the call
+ * allocates nothing.  The graph is only read.  Enqueued on `stream` (NULL = the handle's stream) after the handle's previous
+ * work, not synchronised: five launches, no host round trip. */
+#define ORBFE_COVIS_OBS_MAX_CAP 8192
+#define ORBFE_COVIS_OBS_SCRATCH_BYTES(npoints, nframes, cap, obs_cap) (4 * (2 * (size_t)(npoints) + (size_t)(obs_cap)))
+int orbfe_covis_observations_device(OrbfeCovisGraph *g, int n, const int32_t *d_points, int npoints, const int32_t *d_kf_mp,
+                                    const int *d_counts, int nframes, int cap, const int32_t *d_ref_slot, int obs_cap, int32_t *d_ptr,
+                                    int32_t *d_obs, int *d_nobs, int32_t *d_ref_obs, void *d_scratch, void *stream);
+
 /* Waits for the handle's work and returns the first device-side error since the last sync (ORBFE_OK when none). */
 int orbfe_covis_sync(OrbfeCovisGraph *g);
 

@@ -282,6 +282,7 @@ def _bind_kfdb():
     L.orbfe_covis_clear.argtypes = [vp]
     L.orbfe_covis_lists_device.argtypes = [vp, i, i, vp, i, vp, vp, vp, vp]
     L.orbfe_covis_sync.argtypes = [vp]
+    L.orbfe_covis_observations_device.argtypes = [vp, i, vp, i, vp, vp, i, i, vp, i, vp, vp, vp, vp, vp, vp]
     _kfdb_bound = True
     return L
 
@@ -449,6 +450,23 @@ class CovisibilityGraph:
         vp = C.c_void_p
         _check(_bind_kfdb().orbfe_covis_lists_device(self._h, int(which), len(slots), _p(slots), int(nbest), vp(d_ptr or None),
                                                      vp(d_list or None), vp(d_weights or None), vp(stream)))
+
+    @staticmethod
+    def observations_scratch_bytes(npoints, nframes, cap, obs_cap):
+        """bytes of the d_scratch observations_device takes (ORBFE_COVIS_OBS_SCRATCH_BYTES)"""
+        return 4 * (2 * int(npoints) + int(obs_cap))
+
+    def observations_device(self, n, d_points, npoints, d_kf_mp, d_counts, nframes, cap, obs_cap, d_ptr, d_obs, d_nobs, d_scratch,
+                            d_ref_slot=0, d_ref_obs=0, stream=0):
+        """MapPoint::GetObservations() of the n points d_points[0..n) as the inverse of the live slots' rows (ints = raw device
+        addresses): point j's entries s*cap + i in key order are d_obs[d_ptr[j]:d_ptr[j+1]], *d_nobs the total, and with
+        d_ref_slot, d_ref_obs[j] = ref*cap + observations[ref] (0 when absent).  Enqueued, not synchronised; an overflow or
+        bad input writes d_ptr only (and *d_nobs on overflow) and sync() raises."""
+        vp = C.c_void_p
+        _check(_bind_kfdb().orbfe_covis_observations_device(self._h, int(n), vp(d_points or None), int(npoints), vp(d_kf_mp or None),
+                                                            vp(d_counts or None), int(nframes), int(cap), vp(d_ref_slot or None),
+                                                            int(obs_cap), vp(d_ptr or None), vp(d_obs or None), vp(d_nobs or None),
+                                                            vp(d_ref_obs or None), vp(d_scratch or None), vp(stream)))
 
     def sync(self):
         """waits for the handle's work; raises on the first device-side error since the last sync"""

@@ -26,6 +26,9 @@
 //                       those events changed a weight, else the own call's filtered list, else unchanged.  One call's
 //                       counter reads only the observations, which a batch does not change, and an entry sends at most one
 //                       event to each target, so the result does not depend on scheduling.
+//
+// MapPoint::GetObservations() for named points (orbfe_covis_observations_device) is five launches, no host round trip: stamp
+// the named points, count per (live slot, point) with the row's last feature index, scan, scatter, rank each list by key.
 #include <algorithm>
 #include <climits>
 #include <unordered_set>
@@ -483,12 +486,203 @@ __global__ void covis_lists_kernel(const int *__restrict__ slots, int which, int
     }
 }
 
+// ---- MapPoint::GetObservations() of named points, built as the inverse of the live slots' map-point rows (DESIGN.md §4.7).
+// Five launches, no host round trip.  The scratch is the caller's: stamp[npoints], cnt[npoints], tmp[obs_cap]; none of it
+// has to be initialised, because a stamp is only believed when points[stamp[v]] == v.
+#define COVIS_OBS_MAX_CAP ORBFE_COVIS_OBS_MAX_CAP   // a row's table (2 * cap entries, rounded up to a power of two) is in shared memory
+#define COVIS_OBS_BLOCK 512
+#define COVIS_OBS_SCAN_ITEMS 8
+#define COVIS_OBS_SORT_BLOCK 256
+#define COVIS_OBS_TILE 1024
+// flags of this entry: [5] bad input in this call, [6] this call stops after the scan, [7] the entry that set [3]
+enum { F_OBS_BAD = 5, F_OBS_STOP = 6, F_ERR_SRC = 7 };
+
+// the position of point v among the named points, or -1
+__device__ __forceinline__ int obs_pos(int v, int n, const int *points, const int *stamp) {
+    const int j = stamp[v];
+    return j >= 0 && j < n && points[j] == v ? j : -1;
+}
+
+// launch 1: stamp[p] = j for the named point p = points[j]; the per-position counts start at 0
+__global__ void covis_obs_stamp_kernel(int n, const int *__restrict__ points, int npoints, int *__restrict__ stamp, int *__restrict__ cnt,
+                                       int *__restrict__ flags) {
+    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+        const int p = points[j];
+        if (p < 0 || p >= npoints) atomicOr(&flags[F_OBS_BAD], 1);
+        else stamp[p] = j;
+        cnt[j] = 0;
+    }
+}
+
+// launches 2 and 4: blocks stride over the live slots.  A row's named points go into a shared-memory table keyed by point
+// that keeps the largest feature index (ProcessNewKeyFrame writes mObservations[pKF] = i in ascending i: the last one stays).
+// Scatter = false counts one observation per (slot, point) and checks the input; Scatter = true writes s*cap + i at the
+// point's next free entry of tmp, counting its count back down to 0.
+template <bool Scatter>
+__global__ void __launch_bounds__(COVIS_OBS_BLOCK) covis_obs_rows_kernel(
+    int nslots, int T, const int *__restrict__ state, const int *__restrict__ kf_mp, const int *__restrict__ counts, int cap, int npoints,
+    int n, const int *__restrict__ points, const int *__restrict__ stamp, int *__restrict__ cnt, const int *__restrict__ ptr,
+    int *__restrict__ tmp, int *__restrict__ flags) {
+    extern __shared__ int2 ob_tab[];
+    if (Scatter && flags[F_OBS_STOP]) return;
+    if (!Scatter)   // a point named twice: one of its positions lost the stamp
+        for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+            const int p = points[j];
+            if (p >= 0 && p < npoints && stamp[p] != j) atomicOr(&flags[F_OBS_BAD], 1);
+        }
+    for (int s = blockIdx.x; s < nslots; s += gridDim.x) {
+        if (!(state[s] & ST_LIVE)) continue;   // not an observer: never added, or retired
+        const int c = counts[s];
+        if (c < 0 || c > cap) {
+            if (!Scatter && threadIdx.x == 0) atomicOr(&flags[F_OBS_BAD], 1);
+            continue;
+        }
+        for (int h = threadIdx.x; h < T; h += blockDim.x) ob_tab[h] = make_int2(-1, -1);
+        __syncthreads();
+        const int *row = kf_mp + (size_t)s * cap;
+        for (int i = threadIdx.x; i < c; i += blockDim.x) {
+            const int v = row[i];
+            if (v < 0) continue;   // NULL or isBad()
+            if (v >= npoints) {
+                if (!Scatter) atomicOr(&flags[F_OBS_BAD], 1);
+                continue;
+            }
+            if (obs_pos(v, n, points, stamp) < 0) continue;
+            unsigned h = ((unsigned)v * 2654435761u) & (unsigned)(T - 1);
+            for (;;) {   // T >= 2 * cap: never full
+                const int old = atomicCAS(&ob_tab[h].x, -1, v);
+                if (old == -1 || old == v) { atomicMax(&ob_tab[h].y, i); break; }
+                h = (h + 1) & (unsigned)(T - 1);
+            }
+        }
+        __syncthreads();
+        for (int h = threadIdx.x; h < T; h += blockDim.x) {
+            const int2 e = ob_tab[h];
+            if (e.x < 0) continue;
+            const int j = stamp[e.x];
+            if (Scatter) tmp[ptr[j] + atomicSub(&cnt[j], 1) - 1] = s * cap + e.y;
+            else atomicAdd(&cnt[j], 1);
+        }
+        __syncthreads();
+    }
+}
+
+// launch 3: one block of 1024.  ptr = the exclusive scan of the counts (tiles of 1024 x 8), the reference slots checked, the
+// call decided: bad input stops it with ptr written, a total over obs_cap stops it with ptr and *nobs_out written.
+__global__ void __launch_bounds__(1024) covis_obs_scan_kernel(int n, const int *__restrict__ cnt, const int *__restrict__ ref_slot,
+                                                              int nframes, int obs_cap, int *__restrict__ ptr, int *__restrict__ nobs_out,
+                                                              int *__restrict__ flags) {
+    __shared__ int s_carry, s_badref, s_warp[32];
+    __shared__ int s_v[1024 * COVIS_OBS_SCAN_ITEMS];
+    const int TN = 1024 * COVIS_OBS_SCAN_ITEMS;
+    if (threadIdx.x == 0) { s_carry = 0; s_badref = 0; }
+    __syncthreads();
+    for (int b = 0; b < n; b += TN) {
+        for (int k = threadIdx.x; k < TN; k += blockDim.x) s_v[k] = b + k < n ? cnt[b + k] : 0;
+        __syncthreads();
+        int *mine = s_v + threadIdx.x * COVIS_OBS_SCAN_ITEMS, loc = 0;
+        for (int q = 0; q < COVIS_OBS_SCAN_ITEMS; q++) loc += mine[q];
+        int run = cv_block_scan(loc, s_warp, &s_carry);
+        for (int q = 0; q < COVIS_OBS_SCAN_ITEMS; q++) {
+            const int v = mine[q];
+            mine[q] = run;
+            run += v;
+        }
+        __syncthreads();
+        for (int k = threadIdx.x; k < TN && b + k < n; k += blockDim.x) ptr[b + k] = s_v[k];
+        __syncthreads();
+    }
+    if (ref_slot)
+        for (int j = threadIdx.x; j < n; j += blockDim.x) {
+            const int r = ref_slot[j];
+            if (r < 0 || r >= nframes) s_badref = 1;
+        }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const int total = s_carry;
+        ptr[n] = total;
+        const int bad = flags[F_OBS_BAD] | s_badref;
+        flags[F_OBS_BAD] = 0;
+        int code = ORBFE_OK;
+        if (bad) {
+            code = ORBFE_ERR_ARG;
+        } else {
+            *nobs_out = total;
+            if (total > obs_cap) code = ORBFE_ERR_CAPACITY;
+        }
+        flags[F_OBS_STOP] = code != ORBFE_OK;
+        if (code != ORBFE_OK && atomicCAS(&flags[F_ERR], 0, code) == 0) flags[F_ERR_SRC] = 1;
+    }
+}
+
+// launch 5: every list in key order, and the reference observation.  Blocks stride over groups of 8 points, one warp per
+// point: a list of at most 32 entries is ranked in registers; a longer one is queued and ranked by the whole block against
+// its keys staged in shared memory.  A list's keys are distinct (one entry per live slot), so the ranks are a permutation.
+__global__ void __launch_bounds__(COVIS_OBS_SORT_BLOCK) covis_obs_sort_kernel(
+    int n, int cap, const unsigned long long *__restrict__ key, const int *__restrict__ ptr, const int *__restrict__ tmp,
+    const int *__restrict__ ref_slot, int *__restrict__ obs, int *__restrict__ ref_obs, const int *__restrict__ flags) {
+    __shared__ unsigned long long s_key[COVIS_OBS_TILE];
+    __shared__ int s_long[COVIS_OBS_SORT_BLOCK / 32], s_nlong, s_found;
+    if (flags[F_OBS_STOP]) return;
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, W = COVIS_OBS_SORT_BLOCK / 32;
+    for (int g0 = blockIdx.x * W; g0 < n; g0 += gridDim.x * W) {
+        if (threadIdx.x == 0) s_nlong = 0;
+        __syncthreads();
+        const int j = g0 + wid;
+        if (j < n) {
+            const int lo = ptr[j], L = ptr[j + 1] - lo;
+            if (L > 32) {
+                if (lane == 0) s_long[atomicAdd(&s_nlong, 1)] = j;
+            } else {
+                const int v = lane < L ? tmp[lo + lane] : 0;
+                const unsigned long long k = lane < L ? key[v / cap] : ~0ull;
+                int r = 0;
+                for (int o = 0; o < L; o++) r += __shfl_sync(0xffffffffu, k, o) < k;
+                if (lane < L) obs[lo + r] = v;
+                if (ref_obs) {   // observations[pRefKF], the map's insert-0 when absent
+                    const int ref = ref_slot[j];
+                    const unsigned m = __ballot_sync(0xffffffffu, lane < L && v / cap == ref);
+                    if (lane == (m ? __ffs(m) - 1 : 0)) ref_obs[j] = m ? v : ref * cap;
+                }
+            }
+        }
+        __syncthreads();
+        for (int q = 0; q < s_nlong; q++) {
+            const int jl = s_long[q], lo = ptr[jl], L = ptr[jl + 1] - lo;
+            const int ref = ref_obs ? ref_slot[jl] : -1;
+            if (threadIdx.x == 0) s_found = ref * cap;
+            for (int b = 0; b < L; b += blockDim.x) {
+                const int e = b + threadIdx.x;
+                const int v = e < L ? tmp[lo + e] : 0;
+                const unsigned long long k = e < L ? key[v / cap] : 0ull;
+                int r = 0;
+                for (int t0 = 0; t0 < L; t0 += COVIS_OBS_TILE) {
+                    const int tn = min(COVIS_OBS_TILE, L - t0);
+                    __syncthreads();
+                    for (int x = threadIdx.x; x < tn; x += blockDim.x) s_key[x] = key[tmp[lo + t0 + x] / cap];
+                    __syncthreads();
+                    if (e < L)
+                        for (int x = 0; x < tn; x++) r += s_key[x] < k;
+                }
+                if (e < L) {
+                    obs[lo + r] = v;
+                    if (v / cap == ref) s_found = v;   // at most one entry per slot
+                }
+            }
+            __syncthreads();
+            if (ref_obs && threadIdx.x == 0) ref_obs[jl] = s_found;
+            __syncthreads();
+        }
+        __syncthreads();
+    }
+}
+
 }  // namespace orbfe
 
 using namespace orbfe;
 
 struct OrbfeCovisGraph {
-    int K = 0, C = 0, Cp = 1, P = 2, B = 0, Bp = 1, apply_grid = 1;
+    int K = 0, C = 0, Cp = 1, P = 2, B = 0, Bp = 1, apply_grid = 1, obs_grid = 1;
     size_t count_smem = 0, apply_smem = 0, erase_smem = 0;
     // host mirror of what only the synchronous calls change
     std::vector<uint8_t> live, id0;
@@ -560,9 +754,13 @@ extern "C" int orbfe_covis_create(int device, int max_keyframes, int max_connect
     int nsm = 1;
     ok = ok && cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device) == cudaSuccess;
     g->apply_grid = std::max(1, std::min(g->K, 4 * nsm));
+    g->obs_grid = 8 * nsm;
     ok = ok && cudaFuncSetAttribute(covis_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->count_smem) == cudaSuccess &&
          cudaFuncSetAttribute(covis_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->apply_smem) == cudaSuccess &&
          cudaFuncSetAttribute(covis_erase_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->erase_smem) == cudaSuccess;
+    const int obs_smem = (int)(sizeof(int2) * (size_t)pow2ge(2 * COVIS_OBS_MAX_CAP));
+    ok = ok && cudaFuncSetAttribute(covis_obs_rows_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, obs_smem) == cudaSuccess &&
+         cudaFuncSetAttribute(covis_obs_rows_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, obs_smem) == cudaSuccess;
     const auto alloc = [&](auto **p, size_t n) { ok = ok && g->mem.alloc(p, n) == cudaSuccess; };
     alloc(&g->key, K); alloc(&g->state, K); alloc(&g->wn, K); alloc(&g->on, K); alloc(&g->named, K);
     alloc(&g->wslot, KC); alloc(&g->ww, KC); alloc(&g->oslot, KC); alloc(&g->ow, KC);
@@ -707,15 +905,56 @@ extern "C" int orbfe_covis_lists_device(OrbfeCovisGraph *g, int which, int n, co
     return g->hs.leave(st, false);
 }
 
+extern "C" int orbfe_covis_observations_device(OrbfeCovisGraph *g, int n, const int32_t *d_points, int npoints, const int32_t *d_kf_mp,
+                                               const int *d_counts, int nframes, int cap, const int32_t *d_ref_slot, int obs_cap,
+                                               int32_t *d_ptr, int32_t *d_obs, int *d_nobs, int32_t *d_ref_obs, void *d_scratch, void *stream) {
+    if (!g || n < 0 || npoints < 0 || n > npoints || nframes < 1 || cap < 1 || obs_cap < 0 || (long long)nframes * cap >= (1LL << 31))
+        return set_error(ORBFE_ERR_ARG, "orbfe_covis_observations_device: bad arguments (0 <= n <= npoints, nframes >= 1, cap >= 1, "
+                         "nframes*cap < 2^31, obs_cap >= 0)");
+    if (!d_kf_mp || !d_counts || !d_ptr || !d_nobs || !d_scratch || (n > 0 && !d_points) || (obs_cap > 0 && !d_obs) ||
+        (n > 0 && (d_ref_slot == nullptr) != (d_ref_obs == nullptr)))
+        return set_error(ORBFE_ERR_ARG, "orbfe_covis_observations_device: NULL argument (d_ref_slot and d_ref_obs go together when n > 0)");
+    if ((uintptr_t)d_scratch % alignof(int) != 0)
+        return set_error(ORBFE_ERR_ARG, "orbfe_covis_observations_device: d_scratch is not 4-byte aligned");
+    if (cap > COVIS_OBS_MAX_CAP)
+        return set_error(ORBFE_ERR_UNSUPPORTED, "orbfe_covis_observations_device: cap %d > %d", cap, COVIS_OBS_MAX_CAP);
+    for (int s = nframes; s < g->K; s++)
+        if (g->live[s]) return set_error(ORBFE_ERR_ARG, "orbfe_covis_observations_device: live slot %d >= nframes %d", s, nframes);
+    cudaStream_t st = g->hs.pick(stream);
+    int rc = g->hs.enter(st);
+    if (rc) return rc;
+    int *stamp = static_cast<int *>(d_scratch), *cnt = stamp + npoints, *tmp = cnt + npoints;
+    const int nslots = std::min(g->K, nframes), T = pow2ge(2 * cap);
+    const int rows_grid = std::min(nslots, 4 * g->obs_grid);
+    const size_t smem = sizeof(int2) * (size_t)T;
+    const int W = COVIS_OBS_SORT_BLOCK / 32;
+    covis_obs_stamp_kernel<<<std::max(1, std::min((n + 255) / 256, g->obs_grid)), 256, 0, st>>>(n, d_points, npoints, stamp, cnt, g->flags);
+    covis_obs_rows_kernel<false><<<rows_grid, COVIS_OBS_BLOCK, smem, st>>>(nslots, T, g->state, d_kf_mp, d_counts, cap, npoints, n, d_points,
+                                                                            stamp, cnt, d_ptr, tmp, g->flags);
+    covis_obs_scan_kernel<<<1, 1024, 0, st>>>(n, cnt, d_ref_slot, nframes, obs_cap, d_ptr, d_nobs, g->flags);
+    covis_obs_rows_kernel<true><<<rows_grid, COVIS_OBS_BLOCK, smem, st>>>(nslots, T, g->state, d_kf_mp, d_counts, cap, npoints, n, d_points,
+                                                                           stamp, cnt, d_ptr, tmp, g->flags);
+    covis_obs_sort_kernel<<<std::max(1, std::min((n + W - 1) / W, g->obs_grid)), COVIS_OBS_SORT_BLOCK, 0, st>>>(
+        n, cap, g->key, d_ptr, tmp, d_ref_slot, d_obs, d_ref_obs, g->flags);
+    return g->hs.leave(st, false);
+}
+
 extern "C" int orbfe_covis_sync(OrbfeCovisGraph *g) {
     if (!g) return set_error(ORBFE_ERR_ARG, "orbfe_covis_sync: bad arguments");
     cudaStream_t st = g->hs.stream;
     int rc = g->hs.enter(st);
     if (rc) return rc;
-    int err = 0;
+    int err = 0, src = 0;
     ORBFE_CUDA_TRY(cudaMemcpyAsync(&err, g->flags + F_ERR, sizeof(int), cudaMemcpyDeviceToHost, st));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(&src, g->flags + F_ERR_SRC, sizeof(int), cudaMemcpyDeviceToHost, st));
     ORBFE_CUDA_TRY(cudaMemsetAsync(g->flags + F_ERR, 0, sizeof(int), st));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(g->flags + F_ERR_SRC, 0, sizeof(int), st));
     if ((rc = g->hs.leave(st, true))) return rc;
+    if (src == 1 && err == ORBFE_ERR_ARG)
+        return set_error(ORBFE_ERR_ARG, "orbfe_covis_sync: an observations call was rejected: a named point out of range or named "
+                         "twice, a count outside 0 .. cap, a row value >= npoints or a reference slot outside [0, nframes)");
+    if (src == 1 && err == ORBFE_ERR_CAPACITY)
+        return set_error(ORBFE_ERR_CAPACITY, "orbfe_covis_sync: an observations call needed more than obs_cap entries");
     if (err == ORBFE_ERR_ARG)
         return set_error(ORBFE_ERR_ARG, "orbfe_covis_sync: an update batch was rejected: a point index, group pointer or observation was "
                          "out of range or named a slot that is not live");

@@ -54,6 +54,11 @@
                    every keyframe was updated once: CUDA-event ms of a batch of 1 (LocalMapping's call) and of a batch of 64
                    (loop correction), and the wall time of the oracle's C restatement (oracle/orb_oracle_covis.c: dense rows, not
                    the reference's std::map) for the same calls.
+  --what observations MapPoint::GetObservations() built on the device from the keyframes' rows
+                   (orbfe_covis_observations_device) on the same 2000-keyframe map: CUDA-event ms for the points of one
+                   keyframe's row (ProcessNewKeyFrame) and for every point of the map, and the wall time of the host build
+                   of the same lists from the reference's own MapPoints (GetObservations() copied, walked and flattened;
+                   the upload not included), lists compared.
 Prints one JSON object per --what; never a bench value when run under ncu."""
 import argparse
 import ctypes as C
@@ -1624,6 +1629,79 @@ def covis(args):
     return out
 
 
+def observations(args):
+    """the lists of the points of one keyframe and of every point of a 2000-keyframe map, on the device and on the host
+    from the reference's own maps"""
+    import torch
+    from orb_slam_b200 import bow as BW
+    from oracle import observations as OO
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests"))
+    import covis_scenes as CS
+    scene = CS.scene_large()
+    K, cap = scene.nkf, scene.cap
+    slot_of = scene.slots()
+    model = CS.Model(scene)
+    ref = OO.RefObservations()
+    for st in scene.steps:
+        model.apply(st)
+        if st[0] == "kf":
+            ref.add_keyframe(st[1])
+        elif st[0] == "pts":
+            ref.add_points(st[1])
+            ref.observe_many(st[2], st[3], st[4])
+    kf_mp, counts, gp, obs = model.inputs(slot_of, K)
+    npts = len(gp) - 1
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    tt = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    d_mp, d_cnt = tt(kf_mp), tt(counts)
+    g = BW.CovisibilityGraph(K, 64, 64)
+    g.add(slot_of, np.arange(K), np.arange(K))
+    row = kf_mp[int(slot_of[K // 2]) * cap:(int(slot_of[K // 2]) + 1) * cap]
+    out = {"what": "GetObservations lists on a %d-keyframe map of %d features, %d points, %d observations" % (K, cap, npts, len(obs))}
+    for name, pts in (("one_keyframe", np.unique(row[row >= 0]).astype(np.int32)), ("all_points", np.arange(npts, dtype=np.int32))):
+        n = len(pts)
+        d_pts, d_rs = tt(pts), tt(np.zeros(n, np.int32))
+        z = lambda k: torch.zeros(max(k, 1), dtype=torch.int32, device=dev)
+        d_ptr, d_obs, d_nobs, d_ro = z(n + 1), z(len(obs)), z(1), z(n)
+        d_scr = torch.zeros(BW.CovisibilityGraph.observations_scratch_bytes(npts, K, cap, len(obs)) // 4 + 1, dtype=torch.int32, device=dev)
+        torch.cuda.synchronize()
+        call = lambda: g.observations_device(n, d_pts.data_ptr(), npts, d_mp.data_ptr(), d_cnt.data_ptr(), K, cap, len(obs), d_ptr.data_ptr(),
+                                             d_obs.data_ptr(), d_nobs.data_ptr(), d_scr.data_ptr(), d_rs.data_ptr(), d_ro.data_ptr(),
+                                             stream.cuda_stream)
+        for _ in range(max(args.warmup, 3)):
+            call()
+        stream.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        iters = args.iters * 20
+        times = []
+        for _ in range(5):
+            e0.record(stream)
+            for _ in range(iters):
+                call()
+            e1.record(stream)
+            stream.synchronize()
+            times.append(e0.elapsed_time(e1) / iters)
+        g.sync()
+        out[name + "_points"] = n
+        out[name + "_device_ms"] = float(np.median(times))
+        out[name + "_device_ms_min_max"] = [float(min(times)), float(max(times))]
+        hptr, hobs = np.zeros(n + 1, np.int32), np.zeros(max(len(obs), 1), np.int32)
+        host_ms = []
+        for _ in range(3):
+            t0 = time.perf_counter()
+            tot = ref.flatten(pts, slot_of, cap, hptr, hobs)
+            host_ms.append((time.perf_counter() - t0) * 1e3)
+        out[name + "_host_from_reference_maps_wall_ms"] = float(np.median(host_ms))
+        nd = int(d_nobs.item())
+        out[name + "_lists_equal"] = bool(nd == tot and np.array_equal(d_ptr.cpu().numpy(), hptr) and
+                                          np.array_equal(d_obs.cpu().numpy()[:nd], hobs[:tot]))
+    g.close()
+    ref.close()
+    _gpu_and_power_limit(out)
+    return out
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--what", default="config3,config5")
@@ -1637,4 +1715,4 @@ if __name__ == "__main__":
         print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fast": fast, "latency": latency,
                           "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb, "kfdbbatch": kfdbbatch, "bowchain": bowchain,
                           "windowed": windowed, "guided": guided, "loopscore": loopscore, "vocload": vocload,
-                          "normaldepth": normaldepth, "covis": covis}[w](args)))
+                          "normaldepth": normaldepth, "covis": covis, "observations": observations}[w](args)))
