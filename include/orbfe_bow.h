@@ -436,6 +436,52 @@ int orbfe_covis_observations_device(OrbfeCovisGraph *g, int n, const int32_t *d_
                                     const int *d_counts, int nframes, int cap, const int32_t *d_ref_slot, int obs_cap, int32_t *d_ptr,
                                     int32_t *d_obs, int *d_nobs, int32_t *d_ref_obs, void *d_scratch, void *stream);
 
+/* LocalMapping::KeyFrameCulling() (reference src/LocalMapping.cc:524-578) for the current keyframe `current_slot`, with the
+ * map-point half of every KeyFrame::SetBadFlag it calls (EraseObservation and MapPoint::SetBadFlag, MapPoint.cc:71-122).
+ *   The list is current_slot's GetVectorCovisibleKeyFrames() as the graph holds it, taken once; entry t is decided after
+ *   the erases of entries 0 .. t-1, as in the reference.  A stale entry (a retired slot the list still names, -1 in
+ *   orbfe_covis_lists_device) is evaluated on its unchanged row.  Rows, d_counts and d_kps (frame-store rows of cap
+ *   OrbfeKeyPoint, octave = GetKeyPointUn(i).octave) are those of orbfe_covis_observations_device; a point's observers are
+ *   the live slots whose rows name it, each at its largest feature index.
+ *   d_point_bad[npoints] (in/out): MapPoint::isBad(); d_ref_slot[npoints] (in/out): the slot of mpRefKF.
+ *   not_erase_slots (host, n_not_erase entries): the keyframes with mbNotErase.
+ * Outputs, one entry per list position t < *d_ncand (at most max_connections): d_verdict_slot[t] the entry's slot (the
+ * true slot for a stale entry), d_verdict[t] one of ORBFE_CULL_*, d_nmps[t] / d_nredundant[t] (both may be NULL) nMPs and
+ * nRedundantObservations (0 for a skipped entry).  d_bad_points[0 .. *d_nbad) are the points this call made bad, ascending.
+ * Writes on success: d_point_bad and d_ref_slot of the points the erases touched (a point left without observers goes bad
+ * with its d_ref_slot unwritten: the reference's read there is undefined); in the rows of the slots live at the call, every
+ * cell that names a point made bad while the slot was its observer becomes -1, duplicate cells included (the reference
+ * NULLs only the observation's cell; DESIGN.md §2).  An erased keyframe's row and the rows of slots that are not live stay
+ * as they are.  The graph is only read: replay orbfe_covis_erase for the ERASED verdicts, in order, on the host.
+ * All or nothing, decided on the device and reported by orbfe_covis_sync, with nothing written but *d_nobs: more than
+ * obs_cap observation entries over all points (ORBFE_ERR_CAPACITY, *d_nobs = the number needed); a live slot's or a listed
+ * slot's count outside 0 .. cap, a row value >= npoints, a listed slot >= nframes, an octave outside 0 .. ORBFE_MAX_LEVELS-1
+ * of a listed keyframe's cell or of an observer of a point it names, or such a point's d_ref_slot outside [0, nframes)
+ * (ORBFE_ERR_ARG).  Host-side ORBFE_ERR_ARG before the handle is used: current_slot not live or >= nframes, npoints < 0,
+ * nframes < 1, cap < 1, nframes*cap >= 2^31, obs_cap < 0, n_not_erase < 0 or > max_keyframes, an mbNotErase slot outside
+ * [0, nframes), a live slot >= nframes, a NULL array (d_point_bad, d_ref_slot, d_bad_points may be NULL when npoints = 0),
+ * d_scratch not 4-byte aligned; cap > ORBFE_COVIS_OBS_MAX_CAP is ORBFE_ERR_UNSUPPORTED.
+ * obs_cap: the call builds the observation lists of every point 0 .. npoints-1, not only of the points the listed keyframes
+ * name (so it needs no host count of those points), and obs_cap bounds their total: the number of distinct (live slot,
+ * point) pairs in the live rows, at most the number of non-negative cells in the live rows.  Size it for the whole map.
+ * That build reads every live row twice and is most of a call with a short list (about 0.8 ms of 1.0 ms at 20 covisible
+ * keyframes on a 2000-keyframe x 2000-feature map, DESIGN.md §4.8).
+ * d_scratch: ORBFE_COVIS_CULL_SCRATCH_BYTES(npoints, nframes, cap, obs_cap) bytes of device memory, contents ignored.
+ * Enqueued on `stream` (NULL = the handle's stream) after the handle's previous work, not synchronised: nine launches and
+ * three memsets (and the upload of not_erase_slots), no host round trip. */
+#define ORBFE_CULL_KEPT 0        /* not redundant */
+#define ORBFE_CULL_SKIP_ID0 1    /* mnId == 0: skipped */
+#define ORBFE_CULL_ERASED 2      /* redundant: SetBadFlag erased it (its point half is done) */
+#define ORBFE_CULL_NOT_ERASE 3   /* redundant, mbNotErase: SetBadFlag only sets mbToBeErased */
+#define ORBFE_CULL_RETIRED 4     /* redundant, already retired: SetBadFlag again changes no point */
+#define ORBFE_COVIS_CULL_SCRATCH_BYTES(npoints, nframes, cap, obs_cap) \
+    (4 * (6 * (size_t)(npoints) + 1 + 2 * (size_t)(obs_cap) + 2 * (size_t)(nframes) + 8) + (size_t)(obs_cap))
+int orbfe_covis_keyframe_culling_device(OrbfeCovisGraph *g, int current_slot, int32_t *d_kf_mp, const int *d_counts,
+                                        const OrbfeKeyPoint *d_kps, int nframes, int cap, uint8_t *d_point_bad, int32_t *d_ref_slot,
+                                        int npoints, int n_not_erase, const int32_t *not_erase_slots, int obs_cap, int *d_nobs,
+                                        int32_t *d_verdict_slot, int32_t *d_verdict, int *d_ncand, int32_t *d_nmps,
+                                        int32_t *d_nredundant, int32_t *d_bad_points, int *d_nbad, void *d_scratch, void *stream);
+
 /* Waits for the handle's work and returns the first device-side error since the last sync (ORBFE_OK when none). */
 int orbfe_covis_sync(OrbfeCovisGraph *g);
 

@@ -283,6 +283,8 @@ def _bind_kfdb():
     L.orbfe_covis_lists_device.argtypes = [vp, i, i, vp, i, vp, vp, vp, vp]
     L.orbfe_covis_sync.argtypes = [vp]
     L.orbfe_covis_observations_device.argtypes = [vp, i, vp, i, vp, vp, i, i, vp, i, vp, vp, vp, vp, vp, vp]
+    L.orbfe_covis_keyframe_culling_device.argtypes = [vp, i, vp, vp, vp, i, i, vp, vp, i, i, vp, i, vp, vp, vp, vp, vp, vp, vp, vp,
+                                                      vp, vp]
     _kfdb_bound = True
     return L
 
@@ -467,6 +469,31 @@ class CovisibilityGraph:
                                                             vp(d_counts or None), int(nframes), int(cap), vp(d_ref_slot or None),
                                                             int(obs_cap), vp(d_ptr or None), vp(d_obs or None), vp(d_nobs or None),
                                                             vp(d_ref_obs or None), vp(d_scratch or None), vp(stream)))
+
+    # verdicts of keyframe_culling_device (ORBFE_CULL_*)
+    CULL_KEPT, CULL_SKIP_ID0, CULL_ERASED, CULL_NOT_ERASE, CULL_RETIRED = 0, 1, 2, 3, 4
+
+    @staticmethod
+    def cull_scratch_bytes(npoints, nframes, cap, obs_cap):
+        """bytes of the d_scratch keyframe_culling_device takes (ORBFE_COVIS_CULL_SCRATCH_BYTES)"""
+        return 4 * (6 * int(npoints) + 1 + 2 * int(obs_cap) + 2 * int(nframes) + 8) + int(obs_cap)
+
+    def keyframe_culling_device(self, current_slot, d_kf_mp, d_counts, d_kps, nframes, cap, d_point_bad, d_ref_slot, npoints, not_erase,
+                                obs_cap, d_nobs, d_verdict_slot, d_verdict, d_ncand, d_bad_points, d_nbad, d_scratch, d_nmps=0,
+                                d_nredundant=0, stream=0):
+        """LocalMapping::KeyFrameCulling() for the current keyframe current_slot, with SetBadFlag's map-point half (ints = raw
+        device addresses; not_erase = the host list of mbNotErase slots).  Verdict t of d_ncand[0] entries is
+        (d_verdict_slot[t], d_verdict[t]) with CULL_* codes; d_point_bad / d_ref_slot / the live rows are updated and
+        d_bad_points[0:d_nbad[0]] lists the points made bad, ascending.  obs_cap bounds the observation lists of every point
+        of the map (they are all built), not only the listed keyframes' points.  Enqueued, not synchronised; bad input or an
+        overflow writes nothing (but d_nobs on overflow) and sync() raises."""
+        ne = np.ascontiguousarray(not_erase, np.int32)
+        vp = C.c_void_p
+        _check(_bind_kfdb().orbfe_covis_keyframe_culling_device(
+            self._h, int(current_slot), vp(d_kf_mp or None), vp(d_counts or None), vp(d_kps or None), int(nframes), int(cap),
+            vp(d_point_bad or None), vp(d_ref_slot or None), int(npoints), len(ne), _p(ne) if len(ne) else None, int(obs_cap),
+            vp(d_nobs or None), vp(d_verdict_slot or None), vp(d_verdict or None), vp(d_ncand or None), vp(d_nmps or None),
+            vp(d_nredundant or None), vp(d_bad_points or None), vp(d_nbad or None), vp(d_scratch or None), vp(stream)))
 
     def sync(self):
         """waits for the handle's work; raises on the first device-side error since the last sync"""

@@ -29,6 +29,9 @@
 //
 // MapPoint::GetObservations() for named points (orbfe_covis_observations_device) is five launches, no host round trip: stamp
 // the named points, count per (live slot, point) with the row's last feature index, scan, scatter, rank each list by key.
+//
+// LocalMapping::KeyFrameCulling (orbfe_covis_keyframe_culling_device) is those five launches over every point, then the
+// candidates' checks, one block that walks the current keyframe's list in order, and the NULLing of made-bad points' cells.
 #include <algorithm>
 #include <climits>
 #include <unordered_set>
@@ -677,6 +680,204 @@ __global__ void __launch_bounds__(COVIS_OBS_SORT_BLOCK) covis_obs_sort_kernel(
     }
 }
 
+// ---- LocalMapping::KeyFrameCulling (LocalMapping.cc:524-578) for the current keyframe's GetVectorCovisibleKeyFrames(), with
+// KeyFrame::SetBadFlag's point half (MapPoint::EraseObservation / SetBadFlag, MapPoint.cc:71-122) applied in list order
+// (DESIGN.md §4.8).  After the five observation launches (every point's list, so no host count is needed), three launches:
+// the candidates' checks, one persistent block that walks the list, and the NULLing of the made-bad points' cells.
+// Scratch beyond the observation kernels' (all ints, then one byte per list entry):
+//   pts[npoints] = 0, 1, ..  (the named points of the observation build), ptr[npoints + 1], obs[obs_cap],
+//   lcnt[npoints]   live observers of each point the candidates name
+//   bad_at[npoints] the list position whose SetBadFlag made the point bad, else CULL_NEVER
+//   gone_at[nframes] the list position that erased the slot, else CULL_NEVER
+//   ne[nframes]     mbNotErase
+//   ctl[8]          [0] bad input, [1] an error was pending before this call
+//   alive[obs_cap]  the entry is still in mObservations
+#define COVIS_CULL_BLOCK 1024
+#define COVIS_CULL_CHECK_BLOCK 256
+#define CULL_NEVER 0x7F7F7F7F   // the memset byte 0x7F: after every list position
+enum { CULL_KEPT = ORBFE_CULL_KEPT, CULL_SKIP_ID0 = ORBFE_CULL_SKIP_ID0, CULL_ERASED = ORBFE_CULL_ERASED,
+       CULL_NOT_ERASE = ORBFE_CULL_NOT_ERASE, CULL_RETIRED = ORBFE_CULL_RETIRED };
+enum { CTL_BAD = 0, CTL_PENDING = 1, CTL_COUNT = 8 };
+
+struct CullScratch {
+    int *stamp, *cnt, *tmp, *pts, *ptr, *obs, *lcnt, *bad_at, *gone_at, *ne, *ctl;
+    unsigned char *alive;
+};
+
+// the named points are all points; mbNotErase marks; whether an error was already pending
+__global__ void covis_cull_prep_kernel(int npoints, int n_ne, const int *__restrict__ ne_slots, CullScratch w, const int *__restrict__ flags) {
+    const int t0 = blockIdx.x * blockDim.x + threadIdx.x, T = gridDim.x * blockDim.x;
+    for (int p = t0; p < npoints; p += T) w.pts[p] = p;
+    for (int j = t0; j < n_ne; j += T) w.ne[ne_slots[j]] = 1;
+    if (t0 == 0) w.ctl[CTL_PENDING] = flags[F_ERR] != 0;
+}
+
+__device__ __forceinline__ bool cull_octave_ok(int o) { return o >= 0 && o < ORBFE_MAX_LEVELS; }
+
+// one block per list position: the candidate's count, row values, octaves, its points' reference slots and their observers'
+// octaves are checked; the live count and entry flags of every point it names are set (several blocks may write the same
+// values)
+__global__ void __launch_bounds__(COVIS_CULL_CHECK_BLOCK) covis_cull_check_kernel(
+    int cur, int C, const int *__restrict__ on, const int *__restrict__ oslot, const int *__restrict__ kf_mp, const int *__restrict__ counts,
+    const OrbfeKeyPoint *__restrict__ kps, int nframes, int cap, const unsigned char *__restrict__ point_bad,
+    const int *__restrict__ ref_slot, int npoints, CullScratch w, const int *__restrict__ flags) {
+    const int n = on[cur];
+    if (flags[F_OBS_STOP]) return;
+    for (int t = blockIdx.x; t < n; t += gridDim.x) {
+        const int v = oslot[(size_t)cur * C + t];
+        const int c = v < nframes ? counts[v] : -1;
+        if (c < 0 || c > cap) {
+            if (threadIdx.x == 0) atomicOr(&w.ctl[CTL_BAD], 1);
+            continue;
+        }
+        for (int i = threadIdx.x; i < c; i += blockDim.x) {
+            const int p = kf_mp[(size_t)v * cap + i];
+            if (p < 0) continue;
+            if (p >= npoints) { atomicOr(&w.ctl[CTL_BAD], 1); continue; }
+            if (point_bad[p]) continue;
+            bool ok = cull_octave_ok(kps[(size_t)v * cap + i].octave);
+            const int r = ref_slot[p];
+            ok &= r >= 0 && r < nframes;
+            const int lo = w.ptr[p], hi = w.ptr[p + 1];
+            for (int e = lo; e < hi; e++) {
+                ok &= cull_octave_ok(kps[w.obs[e]].octave);
+                w.alive[e] = 1;
+            }
+            w.lcnt[p] = hi - lo;
+            if (!ok) atomicOr(&w.ctl[CTL_BAD], 1);
+        }
+    }
+}
+
+// the sum of v over the block, returned to every thread
+__device__ int cull_block_sum(int v, int *s_warp) {
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = v;
+    __syncthreads();
+    int s = 0;
+    for (int k = 0; k < COVIS_CULL_BLOCK / 32; k++) s += s_warp[k];
+    __syncthreads();
+    return s;
+}
+
+// one block of 1024 walks the list in order; each step's cells are spread over the block, and an erase's cascade runs on
+// the row's cells in parallel (one point per cell that holds the point's observation of the keyframe: its largest index)
+__global__ void __launch_bounds__(COVIS_CULL_BLOCK) covis_cull_kernel(
+    int cur, int C, const int *__restrict__ on, const int *__restrict__ oslot, const int *__restrict__ state, const unsigned long long *__restrict__ key,
+    const int *__restrict__ kf_mp, const int *__restrict__ counts, const OrbfeKeyPoint *__restrict__ kps, int cap,
+    unsigned char *__restrict__ point_bad, int *__restrict__ ref_slot, int npoints, int *__restrict__ verdict_slot, int *__restrict__ verdict,
+    int *__restrict__ ncand, int *__restrict__ nmps_out, int *__restrict__ nred_out, int *__restrict__ bad_points, int *__restrict__ nbad,
+    CullScratch w, int *__restrict__ flags) {
+    __shared__ int s_warp[COVIS_CULL_BLOCK / 32], s_carry;
+    if (flags[F_OBS_STOP] || w.ctl[CTL_BAD]) {   // nothing written
+        if (threadIdx.x == 0) {
+            if (w.ctl[CTL_BAD] && !flags[F_OBS_STOP]) atomicCAS(&flags[F_ERR], 0, ORBFE_ERR_ARG);
+            if (!w.ctl[CTL_PENDING]) flags[F_ERR_SRC] = 2;
+        }
+        return;
+    }
+    const int n = on[cur];
+    for (int t = 0; t < n; t++) {
+        const int v = oslot[(size_t)cur * C + t];
+        const int st = state[v];
+        if (st & ST_ID0) {   // pKF->mnId == 0: skipped before anything is counted
+            if (threadIdx.x == 0) {
+                verdict_slot[t] = v;
+                verdict[t] = CULL_SKIP_ID0;
+                if (nmps_out) nmps_out[t] = 0;
+                if (nred_out) nred_out[t] = 0;
+            }
+            continue;
+        }
+        const int c = counts[v];
+        const int *row = kf_mp + (size_t)v * cap;
+        const OrbfeKeyPoint *kp = kps + (size_t)v * cap;
+        int nm = 0, nr = 0;
+        for (int i = threadIdx.x; i < c; i += blockDim.x) {
+            const int p = row[i];
+            if (p < 0 || point_bad[p]) continue;
+            nm++;
+            if (w.lcnt[p] <= 3) continue;   // Observations() counts pKF itself when it observes p
+            const int lvl = kp[i].octave;
+            int m = 0;
+            for (int e = w.ptr[p], e1 = w.ptr[p + 1]; e < e1 && m < 3; e++) {
+                const int o = w.obs[e];
+                if (!w.alive[e] || o / cap == v) continue;
+                if (kps[o].octave <= lvl + 1) m++;
+            }
+            nr += m >= 3;
+        }
+        const int NM = cull_block_sum(nm, s_warp), NR = cull_block_sum(nr, s_warp);
+        const bool redundant = 10 * (long long)NR > 9 * (long long)NM;   // == (double)NR > 0.9 * NM for every int (DESIGN §2)
+        const int code = !redundant ? CULL_KEPT : w.ne[v] ? CULL_NOT_ERASE : !(st & ST_LIVE) ? CULL_RETIRED : CULL_ERASED;
+        if (threadIdx.x == 0) {
+            verdict_slot[t] = v;
+            verdict[t] = code;
+            if (nmps_out) nmps_out[t] = NM;
+            if (nred_out) nred_out[t] = NR;
+            if (code == CULL_ERASED) w.gone_at[v] = t;
+        }
+        if (code == CULL_ERASED) {
+            const unsigned long long kv = key[v];
+            for (int i = threadIdx.x; i < c; i += blockDim.x) {
+                const int p = row[i];
+                if (p < 0 || point_bad[p]) continue;
+                const int lo = w.ptr[p], hi = w.ptr[p + 1];
+                int a = lo, b = hi;   // the list is in key order: v's entry
+                while (a < b) {
+                    const int mid = (a + b) >> 1;
+                    if (key[w.obs[mid] / cap] < kv) a = mid + 1; else b = mid;
+                }
+                if (a == hi || w.obs[a] != v * cap + i || !w.alive[a]) continue;   // not an observer, or not this cell
+                w.alive[a] = 0;
+                const int left = --w.lcnt[p];
+                if (ref_slot[p] == v) {   // mpRefKF = mObservations.begin()->first; undefined when none is left
+                    for (int e = lo; e < hi; e++)
+                        if (w.alive[e]) { ref_slot[p] = w.obs[e] / cap; break; }
+                }
+                if (left <= 2) {
+                    point_bad[p] = 1;
+                    w.bad_at[p] = t;
+                }
+            }
+        }
+        __syncthreads();
+    }
+    // the points this call made bad, ascending: tiles of 1024 x 8, each thread's 8 points consecutive
+    if (threadIdx.x == 0) s_carry = 0;
+    __syncthreads();
+    for (int b = 0; b < npoints; b += COVIS_CULL_BLOCK * COVIS_OBS_SCAN_ITEMS) {
+        const int p0 = b + threadIdx.x * COVIS_OBS_SCAN_ITEMS;
+        unsigned mine = 0;
+        for (int q = 0; q < COVIS_OBS_SCAN_ITEMS; q++)
+            if (p0 + q < npoints && w.bad_at[p0 + q] != CULL_NEVER) mine |= 1u << q;
+        int at = cv_block_scan(__popc(mine), s_warp, &s_carry);
+        for (int q = 0; q < COVIS_OBS_SCAN_ITEMS; q++)
+            if (mine >> q & 1) bad_points[at++] = p0 + q;
+    }
+    if (threadIdx.x == 0) {
+        *nbad = s_carry;
+        *ncand = n;
+    }
+}
+
+// blocks stride over the slots live at the call: a cell naming a point made bad while the slot was still its observer (before
+// the slot's own erase, if any) becomes NULL, duplicates included
+__global__ void __launch_bounds__(256) covis_cull_null_kernel(int nslots, const int *__restrict__ state, int *__restrict__ kf_mp,
+                                                              const int *__restrict__ counts, int cap, CullScratch w,
+                                                              const int *__restrict__ flags) {
+    if (flags[F_OBS_STOP] || w.ctl[CTL_BAD]) return;
+    for (int s = blockIdx.x; s < nslots; s += gridDim.x) {
+        if (!(state[s] & ST_LIVE)) continue;
+        const int gone = w.gone_at[s], c = counts[s];
+        int *row = kf_mp + (size_t)s * cap;
+        for (int i = threadIdx.x; i < c; i += blockDim.x) {
+            const int p = row[i];
+            if (p >= 0 && w.bad_at[p] < gone) row[i] = -1;
+        }
+    }
+}
+
 }  // namespace orbfe
 
 using namespace orbfe;
@@ -939,6 +1140,74 @@ extern "C" int orbfe_covis_observations_device(OrbfeCovisGraph *g, int n, const 
     return g->hs.leave(st, false);
 }
 
+extern "C" int orbfe_covis_keyframe_culling_device(OrbfeCovisGraph *g, int current_slot, int32_t *d_kf_mp, const int *d_counts,
+                                                   const OrbfeKeyPoint *d_kps, int nframes, int cap, uint8_t *d_point_bad,
+                                                   int32_t *d_ref_slot, int npoints, int n_not_erase, const int32_t *not_erase_slots,
+                                                   int obs_cap, int *d_nobs, int32_t *d_verdict_slot, int32_t *d_verdict, int *d_ncand,
+                                                   int32_t *d_nmps, int32_t *d_nredundant, int32_t *d_bad_points, int *d_nbad,
+                                                   void *d_scratch, void *stream) {
+    static const char *fn = "orbfe_covis_keyframe_culling_device";
+    if (!g || npoints < 0 || nframes < 1 || cap < 1 || obs_cap < 0 || n_not_erase < 0 || (long long)nframes * cap >= (1LL << 31))
+        return set_error(ORBFE_ERR_ARG, "%s: bad arguments (npoints >= 0, nframes >= 1, cap >= 1, nframes*cap < 2^31, obs_cap >= 0, "
+                         "n_not_erase >= 0)", fn);
+    if (!d_kf_mp || !d_counts || !d_kps || !d_nobs || !d_verdict_slot || !d_verdict || !d_ncand || !d_nbad || !d_scratch ||
+        (npoints > 0 && (!d_point_bad || !d_ref_slot || !d_bad_points)) || (n_not_erase > 0 && !not_erase_slots))
+        return set_error(ORBFE_ERR_ARG, "%s: NULL argument", fn);
+    if ((uintptr_t)d_scratch % alignof(int) != 0) return set_error(ORBFE_ERR_ARG, "%s: d_scratch is not 4-byte aligned", fn);
+    if (cap > COVIS_OBS_MAX_CAP) return set_error(ORBFE_ERR_UNSUPPORTED, "%s: cap %d > %d", fn, cap, COVIS_OBS_MAX_CAP);
+    if (current_slot < 0 || current_slot >= g->K || current_slot >= nframes || !g->live[current_slot])
+        return set_error(ORBFE_ERR_ARG, "%s: current slot %d is not a live keyframe below nframes", fn, current_slot);
+    if (n_not_erase > g->K) return set_error(ORBFE_ERR_ARG, "%s: n_not_erase %d > max_keyframes %d", fn, n_not_erase, g->K);
+    for (int j = 0; j < n_not_erase; j++)
+        if (not_erase_slots[j] < 0 || not_erase_slots[j] >= nframes)
+            return set_error(ORBFE_ERR_ARG, "%s: mbNotErase slot %d outside [0, nframes)", fn, not_erase_slots[j]);
+    for (int s = nframes; s < g->K; s++)
+        if (g->live[s]) return set_error(ORBFE_ERR_ARG, "%s: live slot %d >= nframes %d", fn, s, nframes);
+    cudaStream_t st = g->hs.pick(stream);
+    int rc = g->hs.enter(st);
+    if (rc) return rc;
+    const size_t np = (size_t)npoints, nf = (size_t)nframes;
+    CullScratch w;
+    w.stamp = static_cast<int *>(d_scratch);
+    w.cnt = w.stamp + np;
+    w.tmp = w.cnt + np;
+    w.pts = w.tmp + obs_cap;
+    w.ptr = w.pts + np;
+    w.obs = w.ptr + np + 1;
+    w.lcnt = w.obs + obs_cap;
+    w.bad_at = w.lcnt + np;
+    w.gone_at = w.bad_at + np;
+    w.ne = w.gone_at + nf;
+    w.ctl = w.ne + nf;
+    w.alive = reinterpret_cast<unsigned char *>(w.ctl + CTL_COUNT);
+    ORBFE_CUDA_TRY(cudaMemsetAsync(w.bad_at, 0x7F, sizeof(int) * np, st));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(w.gone_at, 0x7F, sizeof(int) * nf, st));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(w.ne, 0, sizeof(int) * (nf + CTL_COUNT), st));
+    if (n_not_erase > 0)
+        ORBFE_CUDA_TRY(cudaMemcpyAsync(g->slots, not_erase_slots, sizeof(int) * (size_t)n_not_erase, cudaMemcpyHostToDevice, st));
+    const int T = pow2ge(2 * cap), nslots = std::min(g->K, nframes), rows_grid = std::min(nslots, 4 * g->obs_grid);
+    const size_t smem = sizeof(int2) * (size_t)T;
+    const int W = COVIS_OBS_SORT_BLOCK / 32;
+    covis_cull_prep_kernel<<<g->obs_grid, 256, 0, st>>>(npoints, n_not_erase, g->slots, w, g->flags);
+    // every point's observation list: the launches of orbfe_covis_observations_device over the points 0 .. npoints-1
+    covis_obs_stamp_kernel<<<std::max(1, std::min((npoints + 255) / 256, g->obs_grid)), 256, 0, st>>>(npoints, w.pts, npoints, w.stamp, w.cnt,
+                                                                                                       g->flags);
+    covis_obs_rows_kernel<false><<<rows_grid, COVIS_OBS_BLOCK, smem, st>>>(nslots, T, g->state, d_kf_mp, d_counts, cap, npoints, npoints,
+                                                                            w.pts, w.stamp, w.cnt, w.ptr, w.tmp, g->flags);
+    covis_obs_scan_kernel<<<1, 1024, 0, st>>>(npoints, w.cnt, nullptr, nframes, obs_cap, w.ptr, d_nobs, g->flags);
+    covis_obs_rows_kernel<true><<<rows_grid, COVIS_OBS_BLOCK, smem, st>>>(nslots, T, g->state, d_kf_mp, d_counts, cap, npoints, npoints,
+                                                                           w.pts, w.stamp, w.cnt, w.ptr, w.tmp, g->flags);
+    covis_obs_sort_kernel<<<std::max(1, std::min((npoints + W - 1) / W, g->obs_grid)), COVIS_OBS_SORT_BLOCK, 0, st>>>(
+        npoints, cap, g->key, w.ptr, w.tmp, nullptr, w.obs, nullptr, g->flags);
+    covis_cull_check_kernel<<<g->C, COVIS_CULL_CHECK_BLOCK, 0, st>>>(current_slot, g->C, g->on, g->oslot, d_kf_mp, d_counts, d_kps, nframes,
+                                                                    cap, d_point_bad, d_ref_slot, npoints, w, g->flags);
+    covis_cull_kernel<<<1, COVIS_CULL_BLOCK, 0, st>>>(current_slot, g->C, g->on, g->oslot, g->state, g->key, d_kf_mp, d_counts, d_kps, cap,
+                                                      d_point_bad, d_ref_slot, npoints, d_verdict_slot, d_verdict, d_ncand, d_nmps,
+                                                      d_nredundant, d_bad_points, d_nbad, w, g->flags);
+    covis_cull_null_kernel<<<rows_grid, 256, 0, st>>>(nslots, g->state, d_kf_mp, d_counts, cap, w, g->flags);
+    return g->hs.leave(st, false);
+}
+
 extern "C" int orbfe_covis_sync(OrbfeCovisGraph *g) {
     if (!g) return set_error(ORBFE_ERR_ARG, "orbfe_covis_sync: bad arguments");
     cudaStream_t st = g->hs.stream;
@@ -955,6 +1224,12 @@ extern "C" int orbfe_covis_sync(OrbfeCovisGraph *g) {
                          "twice, a count outside 0 .. cap, a row value >= npoints or a reference slot outside [0, nframes)");
     if (src == 1 && err == ORBFE_ERR_CAPACITY)
         return set_error(ORBFE_ERR_CAPACITY, "orbfe_covis_sync: an observations call needed more than obs_cap entries");
+    if (src == 2 && err == ORBFE_ERR_ARG)
+        return set_error(ORBFE_ERR_ARG, "orbfe_covis_sync: a keyframe culling call was rejected: a count outside 0 .. cap, a row value >= "
+                         "npoints, a listed slot >= nframes, an octave outside 0 .. %d or a reference slot outside [0, nframes)",
+                         ORBFE_MAX_LEVELS - 1);
+    if (src == 2 && err == ORBFE_ERR_CAPACITY)
+        return set_error(ORBFE_ERR_CAPACITY, "orbfe_covis_sync: a keyframe culling call needed more than obs_cap observation entries");
     if (err == ORBFE_ERR_ARG)
         return set_error(ORBFE_ERR_ARG, "orbfe_covis_sync: an update batch was rejected: a point index, group pointer or observation was "
                          "out of range or named a slot that is not live");

@@ -59,6 +59,12 @@
                    keyframe's row (ProcessNewKeyFrame) and for every point of the map, and the wall time of the host build
                    of the same lists from the reference's own MapPoints (GetObservations() copied, walked and flattened;
                    the upload not included), lists compared.
+  --what kfculling LocalMapping::KeyFrameCulling on the device (orbfe_covis_keyframe_culling_device) on 2000-keyframe maps of
+                   2000 features (tests/covis_scenes.py scene_large with points spread over +-5, +-25 and +-64 keyframes, so the
+                   current keyframe has about 20, 100 and up to 256 = max_connections covisible keyframes): CUDA-event ms of one call
+                   with culls allowed at the front of the list, in its middle and nowhere (mbNotErase on the others), each from
+                   the same state; the wall time of the C oracle for the same calls (verdicts compared); and the wall time of the
+                   reference's own KeyFrameCulling() on the same map with culls nowhere.
 Prints one JSON object per --what; never a bench value when run under ncu."""
 import argparse
 import ctypes as C
@@ -1702,6 +1708,108 @@ def observations(args):
     return out
 
 
+def kfculling(args):
+    """one KeyFrameCulling call on the device, the oracle and the reference, for three list lengths and three cull places"""
+    import torch
+    from orb_slam_b200 import bow as BW
+    from oracle import kf_culling as KC
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests"))
+    import covis_scenes as CS
+    import kf_culling_scenes as KS
+    from test_oracle_kf_culling import cull_inputs
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    tt = lambda a, dt=np.int32: torch.from_numpy(np.ascontiguousarray(a, dt)).to(dev)
+    C = 256
+    out = {"what": "KeyFrameCulling for one current keyframe of a 2000-keyframe x 2000-feature map; ms per call"}
+    for window in (5, 25, 64):
+        scene = CS.scene_large(window=window)
+        K, cap = scene.nkf, scene.cap
+        slot_of = scene.slots()
+        model = KS.CullModel(scene)
+        g = BW.CovisibilityGraph(K, C, 64)
+        g.add(slot_of, np.arange(K), np.arange(K))
+        ref = KC.RefKfCulling() if KC.ref_available() else None
+        for st in scene.steps:
+            model.apply(st)
+            if st[0] == "update":
+                kf_mp, counts, gp, obs = model.inputs(slot_of, K)
+                d = [tt(kf_mp), tt(counts), tt(gp), tt(obs)]
+                g.update_connections_device([int(slot_of[k]) for k in st[1]], d[0].data_ptr(), d[1].data_ptr(), K, cap, d[2].data_ptr(),
+                                            d[3].data_ptr(), len(gp) - 1, len(obs))
+            if ref is not None:
+                if st[0] == "kf":
+                    ref.add_keyframe(st[1])
+                elif st[0] == "pts":
+                    ref.add_points(st[1])
+                    ref.observe_many(st[2], st[3], st[4])
+                elif st[0] == "update":
+                    for k in st[1]:
+                        ref.update(k)
+        g.sync()
+        cur = K // 2
+        a = cull_inputs(model, slot_of, K)
+        npts = len(a["point_bad"])
+        d_lp, d_l = torch.zeros(2, dtype=torch.int32, device=dev), torch.zeros(C, dtype=torch.int32, device=dev)
+        g.lists_device(0, [int(slot_of[cur])], 0, d_lp.data_ptr(), d_l.data_ptr())
+        g.sync()
+        n = int(d_lp[1].item())
+        lst = d_l.cpu().numpy()[:n]
+        kf_of = np.argsort(slot_of)
+        obs_cap = int(np.count_nonzero(a["kf_mp"] >= 0))
+        pristine = dict(kf_mp=tt(a["kf_mp"]), point_bad=tt(a["point_bad"], np.uint8), ref_slot=tt(a["ref_slot"]))
+        work = {k: v.clone() for k, v in pristine.items()}
+        kp = np.zeros(K * cap, dtype=__import__("orb_slam_b200").KP_DTYPE)
+        kp["octave"] = a["octave"]
+        d_cnt, d_kps = tt(a["counts"]), tt(kp.view(np.uint8), np.uint8)
+        z = lambda k: torch.zeros(max(k, 1), dtype=torch.int32, device=dev)
+        o_nobs, o_vs, o_vd, o_nc, o_bp, o_nb = z(1), z(C), z(C), z(1), z(npts), z(1)
+        d_scr = z(BW.CovisibilityGraph.cull_scratch_bytes(npts, K, cap, obs_cap) // 4 + 1)
+        tag = "covisibles_%d" % n
+        for place, allowed in (("front", lst[:5]), ("middle", lst[n // 2:n // 2 + 5]), ("nowhere", lst[:0])):
+            ne = [int(s) for s in lst if s not in set(allowed.tolist())]
+            times = []
+            for it in range(max(args.warmup, 2) + 5):
+                for k in work:
+                    work[k].copy_(pristine[k])
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                torch.cuda.synchronize()
+                e0.record(stream)
+                g.keyframe_culling_device(int(slot_of[cur]), work["kf_mp"].data_ptr(), d_cnt.data_ptr(), d_kps.data_ptr(), K, cap,
+                                          work["point_bad"].data_ptr(), work["ref_slot"].data_ptr(), npts, ne, obs_cap, o_nobs.data_ptr(),
+                                          o_vs.data_ptr(), o_vd.data_ptr(), o_nc.data_ptr(), o_bp.data_ptr(), o_nb.data_ptr(), d_scr.data_ptr(),
+                                          stream=stream.cuda_stream)
+                e1.record(stream)
+                stream.synchronize()
+                if it >= max(args.warmup, 2):
+                    times.append(e0.elapsed_time(e1))
+            g.sync()
+            ne_flags = a["not_erase"].copy()
+            ne_flags[ne] = 1
+            t0 = time.perf_counter()
+            o = KC.cull(lst, a["live"], a["id0"], a["keys"], ne_flags, a["kf_mp"], a["counts"], a["octave"], cap, a["point_bad"],
+                        a["ref_slot"])
+            out[tag + "_" + place + "_oracle_wall_ms"] = (time.perf_counter() - t0) * 1e3
+            out[tag + "_" + place + "_device_ms"] = float(np.median(times))
+            out[tag + "_" + place + "_device_ms_min_max"] = [float(min(times)), float(max(times))]
+            vd = o_vd.cpu().numpy()[:n]
+            out[tag + "_" + place + "_erased"] = int((vd == KC.ERASED).sum())
+            out[tag + "_" + place + "_made_bad"] = int(o_nb.item())
+            out[tag + "_" + place + "_equals_oracle"] = bool(o["status"] == 0 and vd.tolist() == o["verdict"].tolist() and
+                                                             np.array_equal(work["kf_mp"].cpu().numpy(), o["kf_mp"]))
+            if place == "nowhere" and ref is not None:
+                for s in ne:
+                    ref.set_not_erase(int(kf_of[s]))
+                ids, verdicts, ns = ref.cull(cur)
+                out[tag + "_nowhere_reference_wall_ms"] = ns / 1e6
+                out[tag + "_nowhere_reference_verdicts_equal"] = verdicts == vd.tolist() and [int(slot_of[i]) for i in ids] == lst.tolist()
+        g.close()
+        if ref is not None:
+            ref.close()
+    _gpu_and_power_limit(out)
+    return out
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--what", default="config3,config5")
@@ -1715,4 +1823,4 @@ if __name__ == "__main__":
         print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fast": fast, "latency": latency,
                           "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb, "kfdbbatch": kfdbbatch, "bowchain": bowchain,
                           "windowed": windowed, "guided": guided, "loopscore": loopscore, "vocload": vocload,
-                          "normaldepth": normaldepth, "covis": covis, "observations": observations}[w](args)))
+                          "normaldepth": normaldepth, "covis": covis, "observations": observations, "kfculling": kfculling}[w](args)))
