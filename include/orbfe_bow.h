@@ -482,6 +482,35 @@ int orbfe_covis_keyframe_culling_device(OrbfeCovisGraph *g, int current_slot, in
                                         int32_t *d_verdict_slot, int32_t *d_verdict, int *d_ncand, int32_t *d_nmps,
                                         int32_t *d_nredundant, int32_t *d_bad_points, int *d_nbad, void *d_scratch, void *stream);
 
+/* Tracking::UpdateReference() (reference src/Tracking.cc:728-839) for one frame: UpdateReferenceKeyFrames and
+ * UpdateReferencePoints on the graph and the keyframes' rows.  SetReferenceMapPoints (visualisation) stays with the caller.
+ *   d_frame_mp[nf] (in/out): the frame's mvpMapPoints as point indices, -1 = NULL; a cell naming a point with d_point_bad
+ *   set becomes -1.  d_point_bad[npoints]: MapPoint::isBad().  Rows, d_counts and the observers are those of
+ *   orbfe_covis_observations_device: slot s's row is d_kf_mp[s*cap + i] for i < d_counts[s], a point's observers are the
+ *   live slots whose rows name it, and a row that names a point twice is one observation.
+ * Outputs:
+ *   d_local_kf[0 .. *d_nlocal_kf) (capacity nframes): mvpLocalKeyFrames.  Every remaining frame cell adds 1 to each
+ *     observer of its point (a point at k cells votes k times); the counted slots in key order; then, visiting only those
+ *     entries and stopping before a visit once the list holds more than 80, each visit appends the first of the entry's
+ *     first 10 ordered neighbours that is live and not yet listed.  A retired neighbour (stale) is skipped.
+ *   *d_ref_kf: mpReferenceKF, the first strict maximum of the counter in key order (the smallest key on a tie); -1 when
+ *     nothing was counted.
+ *   d_local_points[0 .. *d_nlocal_points) (capacity npoints): mvpLocalMapPoints, the rows of the list's entries in list
+ *     order, each in ascending i < d_counts[s], negative cells and bad points skipped, each point at its first occurrence.
+ * The graph is only read.  Bad input found on the device writes nothing and is reported by orbfe_covis_sync as
+ * ORBFE_ERR_ARG: a frame cell or a live row's value >= npoints, a live slot's count outside 0 .. cap.  Host-side
+ * ORBFE_ERR_ARG before the handle is used: nf < 0, npoints < 0, nframes < 1, cap < 1, nframes*cap >= 2^31, a NULL array
+ * (d_frame_mp may be NULL when nf = 0, d_point_bad and d_local_points when npoints = 0), d_scratch not 4-byte aligned, a
+ * live slot >= nframes; cap > ORBFE_COVIS_OBS_MAX_CAP is ORBFE_ERR_UNSUPPORTED.
+ * d_scratch: ORBFE_COVIS_LOCAL_MAP_SCRATCH_BYTES(npoints, nframes) bytes of device memory, contents ignored.
+ * Enqueued on `stream` (NULL = the handle's stream) after the handle's previous work, not synchronised: six launches and
+ * two memsets, no host round trip. */
+#define ORBFE_COVIS_LOCAL_MAP_SCRATCH_BYTES(npoints, nframes) (4 * (2 * (size_t)(npoints) + 4 * (size_t)(nframes) + 5))
+int orbfe_covis_local_map_device(OrbfeCovisGraph *g, int nf, int32_t *d_frame_mp, const uint8_t *d_point_bad, int npoints,
+                                 const int32_t *d_kf_mp, const int *d_counts, int nframes, int cap, int32_t *d_local_kf,
+                                 int *d_nlocal_kf, int32_t *d_ref_kf, int32_t *d_local_points, int *d_nlocal_points,
+                                 void *d_scratch, void *stream);
+
 /* Waits for the handle's work and returns the first device-side error since the last sync (ORBFE_OK when none). */
 int orbfe_covis_sync(OrbfeCovisGraph *g);
 

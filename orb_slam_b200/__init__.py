@@ -60,7 +60,7 @@ ABI_SYMBOLS = [
     "orbfe_kfdb_size", "orbfe_kfdb_detect", "orbfe_kfdb_detect_device", "orbfe_kfdb_create_batched", "orbfe_kfdb_detect_batch_device",
     "orbfe_kfdb_set_covisibles_device", "orbfe_covis_create", "orbfe_covis_destroy", "orbfe_covis_add",
     "orbfe_covis_update_connections_device", "orbfe_covis_erase", "orbfe_covis_clear", "orbfe_covis_lists_device", "orbfe_covis_sync",
-    "orbfe_covis_observations_device", "orbfe_covis_keyframe_culling_device",
+    "orbfe_covis_observations_device", "orbfe_covis_keyframe_culling_device", "orbfe_covis_local_map_device",
 ]
 
 

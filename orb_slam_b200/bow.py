@@ -285,6 +285,7 @@ def _bind_kfdb():
     L.orbfe_covis_observations_device.argtypes = [vp, i, vp, i, vp, vp, i, i, vp, i, vp, vp, vp, vp, vp, vp]
     L.orbfe_covis_keyframe_culling_device.argtypes = [vp, i, vp, vp, vp, i, i, vp, vp, i, i, vp, i, vp, vp, vp, vp, vp, vp, vp, vp,
                                                       vp, vp]
+    L.orbfe_covis_local_map_device.argtypes = [vp, i, vp, vp, i, vp, vp, i, i, vp, vp, vp, vp, vp, vp, vp]
     _kfdb_bound = True
     return L
 
@@ -494,6 +495,23 @@ class CovisibilityGraph:
             vp(d_point_bad or None), vp(d_ref_slot or None), int(npoints), len(ne), _p(ne) if len(ne) else None, int(obs_cap),
             vp(d_nobs or None), vp(d_verdict_slot or None), vp(d_verdict or None), vp(d_ncand or None), vp(d_nmps or None),
             vp(d_nredundant or None), vp(d_bad_points or None), vp(d_nbad or None), vp(d_scratch or None), vp(stream)))
+
+    @staticmethod
+    def local_map_scratch_bytes(npoints, nframes):
+        """bytes of the d_scratch local_map_device takes (ORBFE_COVIS_LOCAL_MAP_SCRATCH_BYTES)"""
+        return 4 * (2 * int(npoints) + 4 * int(nframes) + 5)
+
+    def local_map_device(self, nf, d_frame_mp, d_point_bad, npoints, d_kf_mp, d_counts, nframes, cap, d_local_kf, d_nlocal_kf, d_ref_kf,
+                         d_local_points, d_nlocal_points, d_scratch, stream=0):
+        """Tracking::UpdateReference() for one frame (ints = raw device addresses): the frame's nf cells d_frame_mp lose
+        their bad points; d_local_kf[0:d_nlocal_kf[0]] is mvpLocalKeyFrames as slots, d_ref_kf[0] mpReferenceKF (-1 for
+        NULL), d_local_points[0:d_nlocal_points[0]] mvpLocalMapPoints.  Enqueued, not synchronised; bad input writes
+        nothing and sync() raises."""
+        vp = C.c_void_p
+        _check(_bind_kfdb().orbfe_covis_local_map_device(
+            self._h, int(nf), vp(d_frame_mp or None), vp(d_point_bad or None), int(npoints), vp(d_kf_mp or None), vp(d_counts or None),
+            int(nframes), int(cap), vp(d_local_kf or None), vp(d_nlocal_kf or None), vp(d_ref_kf or None), vp(d_local_points or None),
+            vp(d_nlocal_points or None), vp(d_scratch or None), vp(stream)))
 
     def sync(self):
         """waits for the handle's work; raises on the first device-side error since the last sync"""

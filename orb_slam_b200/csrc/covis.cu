@@ -32,6 +32,9 @@
 //
 // LocalMapping::KeyFrameCulling (orbfe_covis_keyframe_culling_device) is those five launches over every point, then the
 // candidates' checks, one block that walks the current keyframe's list in order, and the NULLing of made-bad points' cells.
+//
+// Tracking::UpdateReference (orbfe_covis_local_map_device) is six launches: the frame's point multiplicities, the keyframe
+// counter from the live rows, one block that builds the local keyframe list, and three that collect the list's points.
 #include <algorithm>
 #include <climits>
 #include <unordered_set>
@@ -878,6 +881,274 @@ __global__ void __launch_bounds__(256) covis_cull_null_kernel(int nslots, const 
     }
 }
 
+// ---- Tracking::UpdateReference (Tracking.cc:728-839) for one frame: UpdateReferenceKeyFrames and UpdateReferencePoints on
+// the graph and the live slots' rows (DESIGN.md §4.9).  Six launches after two memsets, no host round trip:
+//   frame   mult[p] = the frame cells naming p (p not bad); cells >= npoints flag the call
+//   vote    one block per live row: the row's points with mult > 0, deduplicated in a shared-memory table, add their mult
+//           to the slot's counter (a point at k cells votes k times; a row naming it twice is one observation)
+//   list    one block: NULL the bad frame cells, compact the counted slots, rank them by key, the first strict maximum,
+//           the sequential extension by one warp, the row offsets of the list's entries
+//   first   atomicMin of each point's position in the concatenated rows of the list
+//   keep / scatter   the cells holding their point's first position, counted per row and written in row order
+// Scratch (ints): mult[npoints], ctl[LM_CTL] (zeroed by the entry), first[npoints] (set to all ones by the entry),
+// cnt[nframes], cand[nframes], rowoff[nframes + 1], kcnt[nframes].
+#define COVIS_LM_BLOCK 1024
+#define COVIS_LM_VOTE_BLOCK 512
+#define LM_NEIGH 10       // GetBestCovisibilityKeyFrames(10), Tracking.cc:820
+#define LM_MAX_KF 80      // `mvpLocalKeyFrames.size() > 80` stops the extension, Tracking.cc:815
+#define LM_HASH 256       // the appended slots (at most LM_MAX_KF + 1) in shared memory
+enum { LM_BAD = 0, LM_NL = 1, LM_CTL = 4 };
+
+struct LmScratch {
+    int *mult, *ctl;
+    unsigned *first;
+    int *cnt, *cand, *rowoff, *kcnt;
+};
+
+__global__ void covis_lm_frame_kernel(int nf, const int *__restrict__ frame_mp, const unsigned char *__restrict__ point_bad, int npoints,
+                                      LmScratch w) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nf; i += gridDim.x * blockDim.x) {
+        const int p = frame_mp[i];
+        if (p < 0) continue;
+        if (p >= npoints) atomicOr(&w.ctl[LM_BAD], 1);
+        else if (!point_bad[p]) atomicAdd(&w.mult[p], 1);
+    }
+}
+
+// blocks stride over the slots; a slot that is not live counts 0 (retired slots are not observers)
+__global__ void __launch_bounds__(COVIS_LM_VOTE_BLOCK) covis_lm_vote_kernel(int nslots, int T, const int *__restrict__ state,
+                                                                           const int *__restrict__ kf_mp, const int *__restrict__ counts,
+                                                                           int cap, int npoints, LmScratch w) {
+    extern __shared__ int lm_tab[];
+    __shared__ int s_warp[COVIS_LM_VOTE_BLOCK / 32];
+    for (int s = blockIdx.x; s < nslots; s += gridDim.x) {
+        if (!(state[s] & ST_LIVE)) {
+            if (threadIdx.x == 0) w.cnt[s] = 0;
+            continue;
+        }
+        const int c = counts[s];
+        if (c < 0 || c > cap) {
+            if (threadIdx.x == 0) {
+                atomicOr(&w.ctl[LM_BAD], 1);
+                w.cnt[s] = 0;
+            }
+            continue;
+        }
+        for (int h = threadIdx.x; h < T; h += blockDim.x) lm_tab[h] = -1;
+        __syncthreads();
+        const int *row = kf_mp + (size_t)s * cap;
+        for (int i = threadIdx.x; i < c; i += blockDim.x) {
+            const int p = row[i];
+            if (p < 0) continue;   // NULL or isBad()
+            if (p >= npoints) {
+                atomicOr(&w.ctl[LM_BAD], 1);
+                continue;
+            }
+            if (w.mult[p] == 0) continue;   // not in the frame
+            unsigned h = ((unsigned)p * 2654435761u) & (unsigned)(T - 1);
+            for (;;) {   // T >= 2 * cap: never full
+                const int old = atomicCAS(&lm_tab[h], -1, p);
+                if (old == -1 || old == p) break;
+                h = (h + 1) & (unsigned)(T - 1);
+            }
+        }
+        __syncthreads();
+        int v = 0;
+        for (int h = threadIdx.x; h < T; h += blockDim.x)
+            if (lm_tab[h] >= 0) v += w.mult[lm_tab[h]];
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = v;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            int t = 0;
+            for (int k = 0; k < COVIS_LM_VOTE_BLOCK / 32; k++) t += s_warp[k];
+            w.cnt[s] = t;
+        }
+        __syncthreads();
+    }
+}
+
+__device__ __forceinline__ bool lm_hash_has(const int *tab, int u) {
+    for (unsigned h = ((unsigned)u * 2654435761u) & (LM_HASH - 1);; h = (h + 1) & (LM_HASH - 1)) {
+        if (tab[h] == u) return true;
+        if (tab[h] < 0) return false;
+    }
+}
+
+__device__ __forceinline__ void lm_hash_put(int *tab, int u) {
+    unsigned h = ((unsigned)u * 2654435761u) & (LM_HASH - 1);
+    while (tab[h] >= 0) h = (h + 1) & (LM_HASH - 1);
+    tab[h] = u;
+}
+
+__global__ void __launch_bounds__(COVIS_LM_BLOCK) covis_lm_list_kernel(
+    int nslots, int C, const int *__restrict__ on, const int *__restrict__ oslot, const int *__restrict__ state,
+    const unsigned long long *__restrict__ key, const int *__restrict__ counts, int nf, int *__restrict__ frame_mp,
+    const unsigned char *__restrict__ point_bad, int *__restrict__ local_kf, int *__restrict__ nlocal_kf, int *__restrict__ ref_kf,
+    LmScratch w, int *__restrict__ flags) {
+    __shared__ unsigned long long s_key[COVIS_LM_BLOCK], s_kmin;
+    __shared__ int s_warp[32], s_carry, s_max, s_ref, s_n;
+    __shared__ int s_nb[LM_MAX_KF * LM_NEIGH], s_app[LM_HASH];
+    if (w.ctl[LM_BAD]) {   // nothing written
+        if (threadIdx.x == 0 && atomicCAS(&flags[F_ERR], 0, ORBFE_ERR_ARG) == 0) flags[F_ERR_SRC] = 3;
+        return;
+    }
+    for (int i = threadIdx.x; i < nf; i += blockDim.x) {   // Tracking.cc:779-782
+        const int p = frame_mp[i];
+        if (p >= 0 && point_bad[p]) frame_mp[i] = -1;
+    }
+    if (threadIdx.x == 0) { s_carry = 0; s_max = 0; s_kmin = ~0ull; s_ref = -1; }
+    __syncthreads();
+    // the counted slots in slot order, and the largest count
+    int mx = 0;
+    for (int b = 0; b < nslots; b += blockDim.x) {
+        const int s = b + threadIdx.x;
+        const int c = s < nslots ? w.cnt[s] : 0;
+        const int at = cv_block_scan(c > 0, s_warp, &s_carry);
+        if (c > 0) {
+            w.cand[at] = s;
+            mx = max(mx, c);
+        }
+    }
+    atomicMax(&s_max, mx);
+    __syncthreads();
+    const int n0 = s_carry, M = s_max;
+    // `it->second > max` over the map in key order: the first maximum, the smallest key among the maxima
+    for (int e = threadIdx.x; e < n0; e += blockDim.x) {
+        const int s = w.cand[e];
+        if (w.cnt[s] == M) atomicMin(&s_kmin, key[s]);
+    }
+    __syncthreads();
+    // std::map<KeyFrame*, int> order: each counted slot's rank among the counted keys (distinct: one per live slot)
+    for (int b = 0; b < n0; b += blockDim.x) {
+        const int e = b + threadIdx.x;
+        const int s = e < n0 ? w.cand[e] : -1;
+        const unsigned long long k = e < n0 ? key[s] : 0ull;
+        int r = 0;
+        for (int t0 = 0; t0 < n0; t0 += COVIS_LM_BLOCK) {
+            const int tn = min(COVIS_LM_BLOCK, n0 - t0);
+            __syncthreads();
+            if (threadIdx.x < tn) s_key[threadIdx.x] = key[w.cand[t0 + threadIdx.x]];
+            __syncthreads();
+            if (e < n0)
+                for (int x = 0; x < tn; x++) r += s_key[x] < k;
+        }
+        if (e < n0) {
+            local_kf[r] = s;
+            if (k == s_kmin) s_ref = s;
+        }
+    }
+    // the extension visits only the n0 entries above (its end iterator is fixed) and stops before a visit once the list
+    // holds more than 80: with n0 > 80 nothing is visited.  Each visit's first 10 neighbours are staged with the ones that
+    // cannot be taken (retired: a stale entry; or counted: listed above) already removed.
+    const int V = n0 <= LM_MAX_KF ? n0 : 0;
+    for (int h = threadIdx.x; h < LM_HASH; h += blockDim.x) s_app[h] = -1;
+    __syncthreads();
+    for (int j = threadIdx.x; j < V * LM_NEIGH; j += blockDim.x) {
+        const int t = j / LM_NEIGH, q = j - t * LM_NEIGH, v = local_kf[t];
+        const int u = q < on[v] ? oslot[(size_t)v * C + q] : -1;
+        s_nb[j] = u >= 0 && (state[u] & ST_LIVE) && w.cnt[u] == 0 ? u : -1;   // a live slot is < nslots
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        const int lane = threadIdx.x;
+        int n = n0;
+        for (int t = 0; t < V && n <= LM_MAX_KF; t++) {
+            const int u = lane < LM_NEIGH ? s_nb[t * LM_NEIGH + lane] : -1;
+            const unsigned m = __ballot_sync(0xffffffffu, u >= 0 && !lm_hash_has(s_app, u));
+            if (m) {   // the first neighbour not yet listed is appended, and the walk of this entry's neighbours stops
+                const int take = __shfl_sync(0xffffffffu, u, __ffs(m) - 1);
+                if (lane == 0) {
+                    lm_hash_put(s_app, take);
+                    local_kf[n] = take;
+                }
+                n++;
+            }
+            __syncwarp();
+        }
+        if (lane == 0) s_n = n;
+    }
+    __syncthreads();
+    const int nl = s_n;
+    if (threadIdx.x == 0) {
+        *nlocal_kf = nl;
+        *ref_kf = s_ref;   // NULL when nothing was counted
+        w.ctl[LM_NL] = nl;
+        s_carry = 0;
+    }
+    __syncthreads();
+    // where each entry's row starts in the list's concatenated rows
+    for (int b = 0; b < nl; b += blockDim.x) {
+        const int t = b + threadIdx.x;
+        const int c = t < nl ? counts[local_kf[t]] : 0;
+        const int o = cv_block_scan(c, s_warp, &s_carry);
+        if (t < nl) w.rowoff[t] = o;
+    }
+    if (threadIdx.x == 0) w.rowoff[nl] = s_carry;
+}
+
+// blocks stride over the list's entries: each point's first position in the concatenated rows
+__global__ void __launch_bounds__(256) covis_lm_first_kernel(const int *__restrict__ kf_mp, const int *__restrict__ counts, int cap,
+                                                             const unsigned char *__restrict__ point_bad, const int *__restrict__ local_kf,
+                                                             LmScratch w) {
+    if (w.ctl[LM_BAD]) return;
+    const int nl = w.ctl[LM_NL];
+    for (int t = blockIdx.x; t < nl; t += gridDim.x) {
+        const int v = local_kf[t], c = counts[v], base = w.rowoff[t];
+        const int *row = kf_mp + (size_t)v * cap;
+        for (int i = threadIdx.x; i < c; i += blockDim.x) {
+            const int p = row[i];
+            if (p >= 0 && !point_bad[p]) atomicMin(&w.first[p], (unsigned)(base + i));
+        }
+    }
+}
+
+// the cell at position pos keeps its point when it is the point's first position (so the point is not bad)
+__device__ __forceinline__ bool lm_keep(int p, int pos, const LmScratch &w) { return p >= 0 && w.first[p] == (unsigned)pos; }
+
+__global__ void __launch_bounds__(COVIS_LM_BLOCK) covis_lm_keep_kernel(const int *__restrict__ kf_mp, const int *__restrict__ counts, int cap,
+                                                                      const int *__restrict__ local_kf, LmScratch w) {
+    __shared__ int s_warp[COVIS_LM_BLOCK / 32];
+    if (w.ctl[LM_BAD]) return;
+    const int nl = w.ctl[LM_NL];
+    for (int t = blockIdx.x; t < nl; t += gridDim.x) {
+        const int v = local_kf[t], c = counts[v], base = w.rowoff[t];
+        const int *row = kf_mp + (size_t)v * cap;
+        int k = 0;
+        for (int i = threadIdx.x; i < c; i += blockDim.x) k += lm_keep(row[i], base + i, w);
+        k = cull_block_sum(k, s_warp);
+        if (threadIdx.x == 0) w.kcnt[t] = k;
+    }
+}
+
+__global__ void __launch_bounds__(COVIS_LM_BLOCK) covis_lm_scatter_kernel(const int *__restrict__ kf_mp, const int *__restrict__ counts,
+                                                                         int cap, const int *__restrict__ local_kf,
+                                                                         int *__restrict__ local_points, int *__restrict__ nlocal_points,
+                                                                         LmScratch w) {
+    __shared__ int s_warp[32], s_carry;
+    if (w.ctl[LM_BAD]) return;
+    const int nl = w.ctl[LM_NL];
+    if (nl == 0 && blockIdx.x == 0 && threadIdx.x == 0) *nlocal_points = 0;
+    for (int t = blockIdx.x; t < nl; t += gridDim.x) {
+        int before = 0;
+        for (int x = threadIdx.x; x < t; x += blockDim.x) before += w.kcnt[x];
+        before = cull_block_sum(before, s_warp);
+        if (threadIdx.x == 0) s_carry = before;
+        __syncthreads();
+        const int v = local_kf[t], c = counts[v], base = w.rowoff[t];
+        const int *row = kf_mp + (size_t)v * cap;
+        for (int b = 0; b < c; b += blockDim.x) {
+            const int i = b + threadIdx.x;
+            const int p = i < c ? row[i] : -1;
+            const bool keep = i < c && lm_keep(p, base + i, w);
+            const int at = cv_block_scan(keep, s_warp, &s_carry);
+            if (keep) local_points[at] = p;
+        }
+        if (t == nl - 1 && threadIdx.x == 0) *nlocal_points = s_carry;
+        __syncthreads();
+    }
+}
+
 }  // namespace orbfe
 
 using namespace orbfe;
@@ -961,7 +1232,8 @@ extern "C" int orbfe_covis_create(int device, int max_keyframes, int max_connect
          cudaFuncSetAttribute(covis_erase_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->erase_smem) == cudaSuccess;
     const int obs_smem = (int)(sizeof(int2) * (size_t)pow2ge(2 * COVIS_OBS_MAX_CAP));
     ok = ok && cudaFuncSetAttribute(covis_obs_rows_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, obs_smem) == cudaSuccess &&
-         cudaFuncSetAttribute(covis_obs_rows_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, obs_smem) == cudaSuccess;
+         cudaFuncSetAttribute(covis_obs_rows_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, obs_smem) == cudaSuccess &&
+         cudaFuncSetAttribute(covis_lm_vote_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, obs_smem / 2) == cudaSuccess;
     const auto alloc = [&](auto **p, size_t n) { ok = ok && g->mem.alloc(p, n) == cudaSuccess; };
     alloc(&g->key, K); alloc(&g->state, K); alloc(&g->wn, K); alloc(&g->on, K); alloc(&g->named, K);
     alloc(&g->wslot, KC); alloc(&g->ww, KC); alloc(&g->oslot, KC); alloc(&g->ow, KC);
@@ -1208,6 +1480,45 @@ extern "C" int orbfe_covis_keyframe_culling_device(OrbfeCovisGraph *g, int curre
     return g->hs.leave(st, false);
 }
 
+extern "C" int orbfe_covis_local_map_device(OrbfeCovisGraph *g, int nf, int32_t *d_frame_mp, const uint8_t *d_point_bad, int npoints,
+                                            const int32_t *d_kf_mp, const int *d_counts, int nframes, int cap, int32_t *d_local_kf,
+                                            int *d_nlocal_kf, int32_t *d_ref_kf, int32_t *d_local_points, int *d_nlocal_points,
+                                            void *d_scratch, void *stream) {
+    static const char *fn = "orbfe_covis_local_map_device";
+    if (!g || nf < 0 || npoints < 0 || nframes < 1 || cap < 1 || (long long)nframes * cap >= (1LL << 31))
+        return set_error(ORBFE_ERR_ARG, "%s: bad arguments (nf >= 0, npoints >= 0, nframes >= 1, cap >= 1, nframes*cap < 2^31)", fn);
+    if (!d_kf_mp || !d_counts || !d_local_kf || !d_nlocal_kf || !d_ref_kf || !d_nlocal_points || !d_scratch || (nf > 0 && !d_frame_mp) ||
+        (npoints > 0 && (!d_point_bad || !d_local_points)))
+        return set_error(ORBFE_ERR_ARG, "%s: NULL argument", fn);
+    if ((uintptr_t)d_scratch % alignof(int) != 0) return set_error(ORBFE_ERR_ARG, "%s: d_scratch is not 4-byte aligned", fn);
+    if (cap > COVIS_OBS_MAX_CAP) return set_error(ORBFE_ERR_UNSUPPORTED, "%s: cap %d > %d", fn, cap, COVIS_OBS_MAX_CAP);
+    for (int s = nframes; s < g->K; s++)
+        if (g->live[s]) return set_error(ORBFE_ERR_ARG, "%s: live slot %d >= nframes %d", fn, s, nframes);
+    cudaStream_t st = g->hs.pick(stream);
+    int rc = g->hs.enter(st);
+    if (rc) return rc;
+    const size_t np = (size_t)npoints, nfr = (size_t)nframes;
+    LmScratch w;
+    w.mult = static_cast<int *>(d_scratch);
+    w.ctl = w.mult + np;
+    w.first = reinterpret_cast<unsigned *>(w.ctl + LM_CTL);
+    w.cnt = reinterpret_cast<int *>(w.first + np);
+    w.cand = w.cnt + nfr;
+    w.rowoff = w.cand + nfr;
+    w.kcnt = w.rowoff + nfr + 1;
+    ORBFE_CUDA_TRY(cudaMemsetAsync(w.mult, 0, sizeof(int) * (np + LM_CTL), st));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(w.first, 0xFF, sizeof(unsigned) * np, st));
+    const int nslots = std::min(g->K, nframes), T = pow2ge(2 * cap), grid = std::max(1, std::min(nslots, 4 * g->obs_grid));
+    covis_lm_frame_kernel<<<std::max(1, std::min((nf + 255) / 256, g->obs_grid)), 256, 0, st>>>(nf, d_frame_mp, d_point_bad, npoints, w);
+    covis_lm_vote_kernel<<<grid, COVIS_LM_VOTE_BLOCK, sizeof(int) * (size_t)T, st>>>(nslots, T, g->state, d_kf_mp, d_counts, cap, npoints, w);
+    covis_lm_list_kernel<<<1, COVIS_LM_BLOCK, 0, st>>>(nslots, g->C, g->on, g->oslot, g->state, g->key, d_counts, nf, d_frame_mp, d_point_bad,
+                                                       d_local_kf, d_nlocal_kf, d_ref_kf, w, g->flags);
+    covis_lm_first_kernel<<<grid, 256, 0, st>>>(d_kf_mp, d_counts, cap, d_point_bad, d_local_kf, w);
+    covis_lm_keep_kernel<<<grid, COVIS_LM_BLOCK, 0, st>>>(d_kf_mp, d_counts, cap, d_local_kf, w);
+    covis_lm_scatter_kernel<<<grid, COVIS_LM_BLOCK, 0, st>>>(d_kf_mp, d_counts, cap, d_local_kf, d_local_points, d_nlocal_points, w);
+    return g->hs.leave(st, false);
+}
+
 extern "C" int orbfe_covis_sync(OrbfeCovisGraph *g) {
     if (!g) return set_error(ORBFE_ERR_ARG, "orbfe_covis_sync: bad arguments");
     cudaStream_t st = g->hs.stream;
@@ -1230,6 +1541,9 @@ extern "C" int orbfe_covis_sync(OrbfeCovisGraph *g) {
                          ORBFE_MAX_LEVELS - 1);
     if (src == 2 && err == ORBFE_ERR_CAPACITY)
         return set_error(ORBFE_ERR_CAPACITY, "orbfe_covis_sync: a keyframe culling call needed more than obs_cap observation entries");
+    if (src == 3 && err == ORBFE_ERR_ARG)
+        return set_error(ORBFE_ERR_ARG, "orbfe_covis_sync: a local map call was rejected: a frame cell or row value >= npoints, or a "
+                         "live slot's count outside 0 .. cap");
     if (err == ORBFE_ERR_ARG)
         return set_error(ORBFE_ERR_ARG, "orbfe_covis_sync: an update batch was rejected: a point index, group pointer or observation was "
                          "out of range or named a slot that is not live");

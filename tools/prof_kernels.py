@@ -65,6 +65,10 @@
                    with culls allowed at the front of the list, in its middle and nowhere (mbNotErase on the others), each from
                    the same state; the wall time of the C oracle for the same calls (verdicts compared); and the wall time of the
                    reference's own KeyFrameCulling() on the same map with culls nowhere.
+  --what localmap  Tracking::UpdateReference on the device (orbfe_covis_local_map_device) on the 2000-keyframe x 2000-feature map
+                   of tests/covis_scenes.py scene_large, for frames of about 300, 1000 and 2000 matched points
+                   (tests/local_map_scenes.py large_frames): the median of CUDA-event windows of one call each, and the wall
+                   time of the reference's own UpdateReference() on the same map with the same lists (results compared).
 Prints one JSON object per --what; never a bench value when run under ncu."""
 import argparse
 import ctypes as C
@@ -1810,6 +1814,84 @@ def kfculling(args):
     return out
 
 
+def localmap(args):
+    """one UpdateReference call on the device and in the reference, for three frame sizes"""
+    import torch
+    from orb_slam_b200 import bow as BW
+    from oracle import local_map as LM
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests"))
+    import covis_scenes as CS
+    import local_map_scenes as LS
+    from test_oracle_local_map import lm_inputs
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    tt = lambda a, dt=np.int32: torch.from_numpy(np.ascontiguousarray(a, dt)).to(dev)
+    scene = CS.scene_large()
+    K, cap = scene.nkf, scene.cap
+    slot_of = scene.slots()
+    model = LS.LmModel(scene)
+    g = BW.CovisibilityGraph(K, 64, 64)
+    g.add(slot_of, np.arange(K), np.arange(K))
+    ref = LM.RefLocalMap() if LM.ref_available() else None
+    for st in scene.steps:
+        model.apply(st)
+        if st[0] == "update":
+            kf_mp, counts, gp, obs = model.inputs(slot_of, K)
+            d = [tt(kf_mp), tt(counts), tt(gp), tt(obs)]
+            g.update_connections_device([int(slot_of[k]) for k in st[1]], d[0].data_ptr(), d[1].data_ptr(), K, cap, d[2].data_ptr(),
+                                        d[3].data_ptr(), len(gp) - 1, len(obs))
+        if ref is not None:
+            if st[0] == "kf":
+                ref.add_keyframe(st[1])
+            elif st[0] == "pts":
+                ref.add_points(st[1])
+                ref.observe_many(st[2], st[3], st[4])
+            elif st[0] == "update":
+                for k in st[1]:
+                    ref.update(k)
+    g.sync()
+    a = lm_inputs(model, slot_of, K)
+    npts = len(a["point_bad"])
+    d_kf_mp, d_cnt, d_pb = tt(a["kf_mp"]), tt(a["counts"]), tt(a["point_bad"], np.uint8)
+    z = lambda k: torch.zeros(max(k, 1), dtype=torch.int32, device=dev)
+    d_lk, d_nlk, d_ref, d_lp, d_nlp = z(K), z(1), z(1), z(npts), z(1)
+    d_scr = z(BW.CovisibilityGraph.local_map_scratch_bytes(npts, K) // 4 + 1)
+    out = {"what": "Tracking::UpdateReference for one frame on a %d-keyframe x %d-feature map (%d points); ms per call" % (K, cap, npts)}
+    for cells in LS.large_frames(model, slot_of):
+        tag = "frame_%d" % len(cells)
+        d_frame = tt(cells)
+        times = []
+        for it in range(max(args.warmup, 2) + 20):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            torch.cuda.synchronize()
+            e0.record(stream)
+            g.local_map_device(len(cells), d_frame.data_ptr(), d_pb.data_ptr(), npts, d_kf_mp.data_ptr(), d_cnt.data_ptr(), K, cap,
+                               d_lk.data_ptr(), d_nlk.data_ptr(), d_ref.data_ptr(), d_lp.data_ptr(), d_nlp.data_ptr(), d_scr.data_ptr(),
+                               stream=stream.cuda_stream)
+            e1.record(stream)
+            stream.synchronize()
+            if it >= max(args.warmup, 2):
+                times.append(e0.elapsed_time(e1))
+        g.sync()
+        nlk, nlp = int(d_nlk.item()), int(d_nlp.item())
+        out[tag + "_device_ms"] = float(np.median(times))
+        out[tag + "_device_ms_min_max"] = [float(min(times)), float(max(times))]
+        out[tag + "_local_keyframes"] = nlk
+        out[tag + "_local_points"] = nlp
+        if ref is not None:
+            fm, lk, rk, lp, ns = ref.update_reference(cells)
+            out[tag + "_reference_wall_ms"] = ns / 1e6
+            out[tag + "_equals_reference"] = bool(d_lk.cpu().numpy()[:nlk].tolist() == [int(slot_of[k]) for k in lk] and
+                                                  d_lp.cpu().numpy()[:nlp].tolist() == lp and int(d_ref.item()) == int(slot_of[rk]))
+        else:
+            out[tag + "_reference_wall_ms"] = "not measured: oracle/_ref/libref_local_map.so absent"
+    g.close()
+    if ref is not None:
+        ref.close()
+    _gpu_and_power_limit(out)
+    return out
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--what", default="config3,config5")
@@ -1823,4 +1905,5 @@ if __name__ == "__main__":
         print(json.dumps({"config3": config3, "config5": config5, "small": small, "exchange1": exchange1, "matchers": matchers, "h2d": h2d, "fast": fast, "latency": latency,
                           "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb, "kfdbbatch": kfdbbatch, "bowchain": bowchain,
                           "windowed": windowed, "guided": guided, "loopscore": loopscore, "vocload": vocload,
-                          "normaldepth": normaldepth, "covis": covis, "observations": observations, "kfculling": kfculling}[w](args)))
+                          "normaldepth": normaldepth, "covis": covis, "observations": observations, "kfculling": kfculling,
+                          "localmap": localmap}[w](args)))
