@@ -9,8 +9,7 @@ import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "liborb_oracle.so")
+from . import _cdll
 
 MAX_LEVELS = 32
 EDGE = 16
@@ -50,83 +49,51 @@ class Frame(C.Structure):
                 ("cell_start", C.c_int * (GRID_COLS * GRID_ROWS + 1)), ("cell_items", C.c_void_p)]
 
 
-def build(force=False):
-    """Compile the oracle with oracle/Makefile (gcc/g++). Building the checker is not using it."""
-    srcs = ["orb_oracle.c", "orb_oracle_match.c", "orb_oracle_bow.c", "orb_oracle_nth.cpp", "orb_oracle.h",
-            os.path.join("..", "include", "orbfe_brief_pattern.inc")]
-    stale = force or not os.path.exists(_SO) or any(
-        os.path.getmtime(os.path.join(_HERE, s)) > os.path.getmtime(_SO) for s in srcs)
-    if stale:
-        subprocess.check_call(["make", "-C", _HERE, "-s"], env={**os.environ, "CC": "gcc", "CXX": "g++"})
-    return _SO
+def build():
+    """Bring oracle/liborb_oracle.so up to date with oracle/Makefile (gcc/g++). Building the checker is not using it."""
+    subprocess.check_call(["make", "-C", _cdll.HERE, "-s"])
+    return os.path.join(_cdll.HERE, "liborb_oracle.so")
 
 
-_lib = None
+def _signatures():
+    vp, i, f, sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
+    P, PI, FR = C.POINTER(Params), C.POINTER(C.c_int), C.POINTER(Frame)
+    return {
+        "orb_oracle_params_init": (i, [P, i, f, i, i, i]),
+        "orb_oracle_level_size": (i, [P, i, i, i, PI, PI]),
+        "orb_oracle_cell_grid": (i, [P, i, i, i, i, i, C.POINTER(CellGrid)]),
+        "orb_oracle_resize_linear_u8": (None, [vp, i, i, sz, vp, i, i, sz]),
+        "orb_oracle_reflect101_frame": (None, [vp, i, i, sz, i]),
+        "orb_oracle_fast_m": (i, [vp, sz]),
+        "orb_oracle_fast_detect": (i, [vp, i, i, sz, i, vp, vp, vp, i]),
+        "orb_oracle_blur7_u8": (None, [vp, i, i, sz, vp, sz]),
+        "orb_oracle_fast_atan2": (f, [f, f]),
+        "orb_oracle_ic_angle": (f, [vp, sz, vp]),
+        "orb_oracle_ic_moments": (None, [vp, sz, vp, PI, PI]),
+        "orb_oracle_brief": (None, [vp, sz, f, i, vp]),
+        "orb_oracle_extract": (i, [P, vp, i, i, sz, vp, vp, i, PI, C.POINTER(Dump)]),
+        "orb_oracle_dump_free": (None, [C.POINTER(Dump)]),
+        "orb_oracle_hamming": (i, [vp, vp]),
+        "orb_oracle_frame_grid": (None, [FR]),
+        "orb_oracle_features_in_area": (i, [FR, f, f, f, i, i, vp, i]),
+        "orb_oracle_frame_scale_factors": (None, [f, i, vp]),
+        "orb_oracle_three_maxima": (None, [vp, i, PI, PI, PI]),
+        "orb_oracle_search_by_projection_ff": (i, [FR, FR, vp, vp, vp, vp, f, f, f, f, f, i, vp]),
+        "orb_oracle_window_search": (i, [FR, FR, vp, i, i, i, f, i, vp]),
+        "orb_oracle_search_for_initialization": (i, [FR, FR, vp, i, f, i, vp]),
+        "orb_oracle_search_local_points": (i, [FR, i, vp, vp, vp, vp, vp, f, f, vp]),
+        "orb_oracle_search_by_projection_kf": (i, [FR, i, vp, vp, vp, vp, vp, vp, f, f, f, f, f, i, i, vp]),
+        "orb_oracle_search_by_projection_f1f2": (i, [FR, FR, vp, vp, vp, f, f, f, f, i, f, vp]),
+        "orb_oracle_guided_search": (i, [FR, i, vp, vp, vp, vp, vp, vp, vp, i, f, i, i, vp]),
+        "orb_oracle_search_for_triangulation": (i, [i, vp, vp, vp, i, vp, vp, vp, i, vp, vp, vp, i, vp, vp, vp, vp, vp, i, vp]),
+        "orb_oracle_guided_best": (None, [FR, i, vp, vp, vp, vp, vp, vp, i, vp]),
+        "orb_oracle_search_by_bow": (i, [i, i, vp, vp, vp, i, vp, vp, vp, i, vp, vp, vp, i, vp, vp, vp, f, i, vp]),
+        "orb_oracle_knn2": (None, [vp, i, vp, C.c_long, vp, vp, vp]),
+    }
 
 
-def lib():
-    global _lib
-    if _lib is None:
-        build()
-        L = C.CDLL(_SO)
-        u8p, i32p, f32p = C.c_void_p, C.c_void_p, C.c_void_p
-        L.orb_oracle_params_init.argtypes = [C.POINTER(Params), C.c_int, C.c_float, C.c_int, C.c_int, C.c_int]
-        L.orb_oracle_level_size.argtypes = [C.POINTER(Params), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-        L.orb_oracle_cell_grid.argtypes = [C.POINTER(Params), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(CellGrid)]
-        L.orb_oracle_resize_linear_u8.argtypes = [u8p, C.c_int, C.c_int, C.c_size_t, u8p, C.c_int, C.c_int, C.c_size_t]
-        L.orb_oracle_resize_linear_u8.restype = None
-        L.orb_oracle_reflect101_frame.argtypes = [u8p, C.c_int, C.c_int, C.c_size_t, C.c_int]
-        L.orb_oracle_reflect101_frame.restype = None
-        L.orb_oracle_fast_m.argtypes = [u8p, C.c_size_t]
-        L.orb_oracle_fast_detect.argtypes = [u8p, C.c_int, C.c_int, C.c_size_t, C.c_int, i32p, i32p, i32p, C.c_int]
-        L.orb_oracle_blur7_u8.argtypes = [u8p, C.c_int, C.c_int, C.c_size_t, u8p, C.c_size_t]
-        L.orb_oracle_blur7_u8.restype = None
-        L.orb_oracle_fast_atan2.argtypes = [C.c_float, C.c_float]
-        L.orb_oracle_fast_atan2.restype = C.c_float
-        L.orb_oracle_ic_angle.argtypes = [u8p, C.c_size_t, i32p]
-        L.orb_oracle_ic_angle.restype = C.c_float
-        L.orb_oracle_ic_moments.argtypes = [u8p, C.c_size_t, i32p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-        L.orb_oracle_ic_moments.restype = None
-        L.orb_oracle_brief.argtypes = [u8p, C.c_size_t, C.c_float, C.c_int, u8p]
-        L.orb_oracle_brief.restype = None
-        L.orb_oracle_extract.argtypes = [C.POINTER(Params), u8p, C.c_int, C.c_int, C.c_size_t, C.c_void_p, u8p,
-                                         C.c_int, C.POINTER(C.c_int), C.POINTER(Dump)]
-        L.orb_oracle_dump_free.argtypes = [C.POINTER(Dump)]
-        L.orb_oracle_dump_free.restype = None
-        L.orb_oracle_hamming.argtypes = [u8p, u8p]
-        L.orb_oracle_frame_grid.argtypes = [C.POINTER(Frame)]
-        L.orb_oracle_frame_grid.restype = None
-        L.orb_oracle_features_in_area.argtypes = [C.POINTER(Frame), C.c_float, C.c_float, C.c_float, C.c_int, C.c_int, i32p, C.c_int]
-        L.orb_oracle_frame_scale_factors.argtypes = [C.c_float, C.c_int, f32p]
-        L.orb_oracle_frame_scale_factors.restype = None
-        L.orb_oracle_three_maxima.argtypes = [i32p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
-        L.orb_oracle_three_maxima.restype = None
-        L.orb_oracle_search_by_projection_ff.argtypes = [C.POINTER(Frame), C.POINTER(Frame), u8p, u8p, f32p, f32p,
-                                                         C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, i32p]
-        L.orb_oracle_window_search.argtypes = [C.POINTER(Frame), C.POINTER(Frame), u8p, C.c_int, C.c_int, C.c_int,
-                                               C.c_float, C.c_int, i32p]
-        L.orb_oracle_search_for_initialization.argtypes = [C.POINTER(Frame), C.POINTER(Frame), f32p, C.c_int, C.c_float, C.c_int, i32p]
-        L.orb_oracle_search_local_points.argtypes = [C.POINTER(Frame), C.c_int, u8p, f32p, i32p, f32p, u8p, C.c_float, C.c_float, i32p]
-        L.orb_oracle_search_by_projection_kf.argtypes = [C.POINTER(Frame), C.c_int, u8p, f32p, f32p, u8p, f32p, f32p, C.c_float,
-                                                         C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_int, i32p]
-        L.orb_oracle_search_by_projection_f1f2.argtypes = [C.POINTER(Frame), C.POINTER(Frame), u8p, f32p, f32p, C.c_float, C.c_float,
-                                                           C.c_float, C.c_float, C.c_int, C.c_float, i32p]
-        L.orb_oracle_guided_search.argtypes = [C.POINTER(Frame), C.c_int, f32p, f32p, f32p, i32p, i32p, u8p, f32p, C.c_int, C.c_float,
-                                               C.c_int, C.c_int, i32p]
-        L.orb_oracle_search_for_triangulation.argtypes = [C.c_int, C.c_void_p, u8p, u8p, C.c_int, i32p, i32p, i32p, C.c_int, C.c_void_p, u8p,
-                                                          u8p, C.c_int, i32p, i32p, i32p, f32p, f32p, C.c_int, i32p]
-        L.orb_oracle_guided_best.argtypes = [C.POINTER(Frame), C.c_int, f32p, f32p, f32p, i32p, i32p, u8p, C.c_int, i32p]
-        L.orb_oracle_guided_best.restype = None
-        L.orb_oracle_search_by_bow.argtypes = [C.c_int, C.c_int, u8p, u8p, f32p, C.c_int, i32p, i32p, i32p, C.c_int, u8p, u8p, f32p,
-                                               C.c_int, i32p, i32p, i32p, C.c_float, C.c_int, i32p]
-        L.orb_oracle_knn2.argtypes = [u8p, C.c_int, u8p, C.c_long, i32p, i32p, i32p]
-        L.orb_oracle_knn2.restype = None
-        _lib = L
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+_p = _cdll.p
+lib = _cdll.loader("liborb_oracle.so", _signatures())
 
 
 def make_params(nfeatures=1000, scale_factor=1.2, nlevels=8, score_type=1, fast_th=20,

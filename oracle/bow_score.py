@@ -1,64 +1,31 @@
 """ORBVocabulary::score and LoopClosing::DetectLoop's minScore loop (src/LoopClosing.cc:117-131) for the tests of
 orbfe_bow_min_score_device / orbfe_bow_score (TEST INFRASTRUCTURE ONLY).
 
-  bow_score, loop_min_score   the oracle's restatement, oracle/orb_oracle_bow_score.c, compiled here into
-                              oracle/liborb_oracle_bow_score.so with the flags of oracle/Makefile
-  RefVocabularyScore          the reference's own ORBVocabulary::score: oracle/ref_shim/ref_voc_score.cc compiled into
-                              oracle/_ref/libref_voc_score.so, linked against libref_orbslam.so (the reference's DBoW2,
-                              unmodified), where the reference sources exist; elsewhere the prebuilt library is used as it is"""
+  bow_score, loop_min_score   the oracle's restatement, oracle/orb_oracle_bow_score.c in oracle/liborb_oracle.so
+  RefVocabularyScore          the reference's own ORBVocabulary::score: oracle/ref_shim/ref_voc_score.cc in
+                              oracle/_ref/libref_drivers.so, linked against libref_orbslam.so (the reference's DBoW2,
+                              unmodified)"""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from . import ref as R
+from . import _cdll
+from ._cdll import p as _p
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "liborb_oracle_bow_score.so")
-_SRC = os.path.join(_HERE, "orb_oracle_bow_score.c")
-_REF_SO = os.path.join(R._DIR, "libref_voc_score.so")
-_REF_SRC = os.path.join(_HERE, "ref_shim", "ref_voc_score.cc")
-_lib = None
-_ref_lib = None
-
-
-def build(force=False):
-    """Compile the oracle library, and the reference driver where the reference sources exist (after `make ref`)."""
-    if force or not os.path.exists(_SO) or os.path.getmtime(_SO) < os.path.getmtime(_SRC):
-        subprocess.check_call(["/usr/bin/gcc", "-O3", "-march=x86-64-v3", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-Wall",
-                               "-std=gnu11", "-shared", _SRC, "-o", _SO, "-lm"])
-    root = R.REFERENCE_ROOT
-    if os.path.isdir(os.path.join(root, "src")):
-        base = R.build()
-        if force or not os.path.exists(_REF_SO) or os.path.getmtime(_REF_SO) < max(os.path.getmtime(_REF_SRC), os.path.getmtime(base)):
-            subprocess.check_call(["/usr/bin/g++", "-std=c++14", "-O2", "-march=x86-64-v3", "-ffp-contract=off", "-fno-fast-math", "-fPIC",
-                                   "-w", "-shared", "-I" + os.path.join(_HERE, "ref_shim"), "-I" + os.path.join(root, "include"),
-                                   "-I" + root, _REF_SRC, "-o", _REF_SO, "-L" + R._DIR, "-lref_orbslam", "-Wl,-rpath,$ORIGIN",
-                                   "-lpthread"])
-    return _SO
+vp, i = C.c_void_p, C.c_int
+lib = _cdll.loader("liborb_oracle.so", {
+    "orb_oracle_bow_score": (C.c_double, [vp, vp, i, vp, vp, i]),
+    "orb_oracle_loop_min_score": (C.c_float, [vp, vp, i, i, vp, vp, vp, vp]),
+})
+_ref = _cdll.loader("_ref/libref_drivers.so", {
+    "ref_voc_score_create": (vp, [C.c_char_p]),
+    "ref_voc_score_free": (None, [vp]),
+    "ref_voc_score": (C.c_double, [vp, vp, vp, i, vp, vp, i]),
+})
 
 
 def ref_available():
-    return os.path.exists(_REF_SO) and R.available()
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        build()
-        L = C.CDLL(_SO)
-        vp, i = C.c_void_p, C.c_int
-        L.orb_oracle_bow_score.argtypes = [vp, vp, i, vp, vp, i]
-        L.orb_oracle_bow_score.restype = C.c_double
-        L.orb_oracle_loop_min_score.argtypes = [vp, vp, i, i, vp, vp, vp, vp]
-        L.orb_oracle_loop_min_score.restype = C.c_float
-        _lib = L
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return _cdll.ref_available("libref_drivers.so")
 
 
 def _bow(ids, vals):
@@ -89,20 +56,7 @@ class RefVocabularyScore:
     """score() of a reference ORBVocabulary loaded from DBoW2's text format."""
 
     def __init__(self, vocabulary_text_path):
-        global _ref_lib
-        if _ref_lib is None:
-            if not os.path.exists(_REF_SO):
-                build()
-            L = C.CDLL(_REF_SO, mode=os.RTLD_NOW | os.RTLD_LOCAL)
-            vp, i = C.c_void_p, C.c_int
-            L.ref_voc_score_create.argtypes = [C.c_char_p]
-            L.ref_voc_score_create.restype = vp
-            L.ref_voc_score_free.argtypes = [vp]
-            L.ref_voc_score_free.restype = None
-            L.ref_voc_score.argtypes = [vp, vp, vp, i, vp, vp, i]
-            L.ref_voc_score.restype = C.c_double
-            _ref_lib = L
-        self.L = _ref_lib
+        self.L = _ref()
         self.h = self.L.ref_voc_score_create(vocabulary_text_path.encode())
         assert self.h, "loadFromTextFile failed"
 

@@ -1,75 +1,60 @@
 """The covisibility graph (KeyFrame::UpdateConnections and its helpers, src/KeyFrame.cc) for the tests of orbfe_covis_*
 (TEST INFRASTRUCTURE ONLY).
 
-  CovisOracle   the oracle's restatement, oracle/orb_oracle_covis.c, compiled here into oracle/liborb_oracle_covis.so with
-                the flags of oracle/Makefile; replay() runs a batch as consecutive calls
-  RefCovis      the reference's own KeyFrame / MapPoint on a scripted map: oracle/ref_shim/ref_covis.cc compiled into
-                oracle/_ref/libref_covis.so, linked against libref_orbslam.so (the reference's sources, unmodified), where
-                the reference sources exist; elsewhere the prebuilt library is used as it is"""
+  CovisOracle   the oracle's restatement, oracle/orb_oracle_covis.c in oracle/liborb_oracle.so; replay() runs a batch as
+                consecutive calls
+  RefCovis      the reference's own KeyFrame / MapPoint on a scripted map: oracle/ref_shim/ref_covis.cc (through
+                ref_observations.cc) in oracle/_ref/libref_drivers.so, linked against libref_orbslam.so (the reference's
+                sources, unmodified)
+
+REF_CV is the signature table of the ref_cv_* driver functions; oracle.observations, oracle.kf_culling and oracle.local_map
+extend it for the libraries that hold those functions too."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from . import ref as R
+from . import _cdll
+from ._cdll import p as _p
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "liborb_oracle_covis.so")
-_SRC = os.path.join(_HERE, "orb_oracle_covis.c")
-_REF_SO = os.path.join(R._DIR, "libref_covis.so")
-_REF_SRC = os.path.join(_HERE, "ref_shim", "ref_covis.cc")
-_lib = None
-_ref_lib = None
-
-
-def build(force=False):
-    """Compile the oracle library, and the reference driver where the reference sources exist (after `make ref`)."""
-    if force or not os.path.exists(_SO) or os.path.getmtime(_SO) < os.path.getmtime(_SRC):
-        subprocess.check_call(["/usr/bin/gcc", "-O3", "-march=x86-64-v3", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-Wall",
-                               "-std=gnu11", "-shared", _SRC, "-o", _SO])
-    root = R.REFERENCE_ROOT
-    if os.path.isdir(os.path.join(root, "src")):
-        base = R.build()
-        if force or not os.path.exists(_REF_SO) or os.path.getmtime(_REF_SO) < max(os.path.getmtime(_REF_SRC), os.path.getmtime(base)):
-            subprocess.check_call(["/usr/bin/g++", "-std=c++14", "-O2", "-march=x86-64-v3", "-ffp-contract=off", "-fno-fast-math", "-fPIC",
-                                   "-w", "-shared", "-I" + os.path.join(_HERE, "ref_shim"), "-I" + os.path.join(root, "include"),
-                                   "-I" + root, _REF_SRC, "-o", _REF_SO, "-L" + R._DIR, "-lref_orbslam", "-Wl,-rpath,$ORIGIN",
-                                   "-lpthread"])
-    return _SO
+vp, i = C.c_void_p, C.c_int
+lib = _cdll.loader("liborb_oracle.so", {
+    "covis_oracle_create": (vp, [i]),
+    "covis_oracle_free": (None, [vp]),
+    "covis_oracle_add": (None, [vp, i, i, C.c_uint64]),
+    "covis_oracle_update": (i, [vp, i, vp, vp, i, vp, vp]),
+    "covis_oracle_erase": (None, [vp, i]),
+    "covis_oracle_clear": (None, [vp]),
+    "covis_oracle_ordered": (i, [vp, i, vp, vp]),
+    "covis_oracle_weights": (i, [vp, i, vp, vp]),
+    "covis_oracle_parent": (i, [vp, i]),
+    "covis_oracle_live": (i, [vp, i]),
+})
+REF_CV = {
+    "ref_cv_create": (vp, []),
+    "ref_cv_free": (i, [vp]),
+    "ref_cv_add_keyframe": (i, [vp, i]),
+    "ref_cv_add_point": (i, [vp, i]),
+    "ref_cv_add_points": (i, [vp, i, vp]),
+    "ref_cv_observe": (i, [vp, i, i, i]),
+    "ref_cv_observe_many": (i, [vp, i, vp, vp, vp]),
+    "ref_cv_update": (i, [vp, i]),
+    "ref_cv_set_bad_keyframe": (i, [vp, i]),
+    "ref_cv_set_bad_point": (i, [vp, i]),
+    "ref_cv_erase_match": (i, [vp, i, i]),
+    "ref_cv_ordered": (i, [vp, i, vp, vp, i]),
+    "ref_cv_weights": (i, [vp, i, vp, vp, i]),
+    "ref_cv_parent": (i, [vp, i]),
+    "ref_cv_keyframe_bad": (i, [vp, i]),
+    "ref_cv_keyframe_mnid": (C.c_long, [vp, i]),
+    "ref_cv_matches": (i, [vp, i, vp, i]),
+    "ref_cv_observations": (i, [vp, i, vp, vp, i]),
+    "ref_cv_point_bad": (i, [vp, i]),
+}
+_ref = _cdll.loader("_ref/libref_drivers.so", REF_CV)
 
 
 def ref_available():
-    return os.path.exists(_REF_SO) and R.available()
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        build()
-        L = C.CDLL(_SO)
-        vp, i = C.c_void_p, C.c_int
-        L.covis_oracle_create.argtypes = [i]
-        L.covis_oracle_create.restype = vp
-        L.covis_oracle_free.argtypes = [vp]
-        L.covis_oracle_free.restype = None
-        L.covis_oracle_add.argtypes = [vp, i, i, C.c_uint64]
-        L.covis_oracle_add.restype = None
-        L.covis_oracle_update.argtypes = [vp, i, vp, vp, i, vp, vp]
-        L.covis_oracle_erase.argtypes = [vp, i]
-        L.covis_oracle_erase.restype = None
-        L.covis_oracle_clear.argtypes = [vp]
-        L.covis_oracle_clear.restype = None
-        L.covis_oracle_ordered.argtypes = [vp, i, vp, vp]
-        L.covis_oracle_weights.argtypes = [vp, i, vp, vp]
-        L.covis_oracle_parent.argtypes = [vp, i]
-        L.covis_oracle_live.argtypes = [vp, i]
-        _lib = L
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return _cdll.ref_available("libref_drivers.so")
 
 
 class CovisOracle:
@@ -127,29 +112,6 @@ class CovisOracle:
 
     def live(self, slot):
         return bool(self.L.covis_oracle_live(self.h, int(slot)))
-
-
-def _ref():
-    global _ref_lib
-    if _ref_lib is None:
-        if not os.path.exists(_REF_SO):
-            build()
-        L = C.CDLL(_REF_SO, mode=os.RTLD_NOW | os.RTLD_LOCAL)
-        vp, i = C.c_void_p, C.c_int
-        L.ref_cv_create.restype = vp
-        L.ref_cv_free.argtypes = [vp]
-        for f, a in (("ref_cv_add_keyframe", [vp, i]), ("ref_cv_add_point", [vp, i]), ("ref_cv_observe", [vp, i, i, i]),
-                     ("ref_cv_update", [vp, i]), ("ref_cv_set_bad_keyframe", [vp, i]), ("ref_cv_set_bad_point", [vp, i]),
-                     ("ref_cv_erase_match", [vp, i, i]), ("ref_cv_ordered", [vp, i, vp, vp, i]), ("ref_cv_weights", [vp, i, vp, vp, i]),
-                     ("ref_cv_parent", [vp, i]), ("ref_cv_keyframe_bad", [vp, i]), ("ref_cv_matches", [vp, i, vp, i]),
-                     ("ref_cv_observations", [vp, i, vp, vp, i]), ("ref_cv_point_bad", [vp, i])):
-            getattr(L, f).argtypes = a
-        L.ref_cv_observe_many.argtypes = [vp, i, vp, vp, vp]
-        L.ref_cv_add_points.argtypes = [vp, i, vp]
-        L.ref_cv_keyframe_mnid.argtypes = [vp, i]
-        L.ref_cv_keyframe_mnid.restype = C.c_long
-        _ref_lib = L
-    return _ref_lib
 
 
 class RefCovis:

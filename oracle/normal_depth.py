@@ -1,63 +1,37 @@
 """MapPoint::UpdateNormalAndDepth (src/MapPoint.cc:273-312) for the tests of orbfe_normal_and_depth(_device) (TEST
 INFRASTRUCTURE ONLY).
 
-  normal_depth     the oracle's restatement, oracle/orb_oracle_normal_depth.c, compiled here into
-                   oracle/liborb_oracle_normal_depth.so with the flags of oracle/Makefile
-  RefMap           the reference's own MapPoint / KeyFrame on a scripted map: oracle/ref_shim/ref_map_point.cc compiled into
-                   oracle/_ref/libref_map_point.so, linked against libref_orbslam.so (the reference's sources, unmodified),
-                   where the reference sources exist; elsewhere the prebuilt library is used as it is
+  normal_depth     the oracle's restatement, oracle/orb_oracle_normal_depth.c in oracle/liborb_oracle.so
+  RefMap           the reference's own MapPoint / KeyFrame on a scripted map: oracle/ref_shim/ref_map_point.cc in
+                   oracle/_ref/libref_drivers.so, linked against libref_orbslam.so (the reference's sources, unmodified)
   shim_scale_add   the shim's `x + y*beta` (the MatExpr of `normal + normali/cv::norm(normali)`), from the same library"""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from . import ref as R
+from . import _cdll
+from ._cdll import p as _p
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "liborb_oracle_normal_depth.so")
-_SRC = os.path.join(_HERE, "orb_oracle_normal_depth.c")
-_REF_SO = os.path.join(R._DIR, "libref_map_point.so")
-_REF_SRC = os.path.join(_HERE, "ref_shim", "ref_map_point.cc")
-_lib = None
-_ref_lib = None
-
-
-def build(force=False):
-    """Compile the oracle library, and the reference driver where the reference sources exist (after `make ref`)."""
-    if force or not os.path.exists(_SO) or os.path.getmtime(_SO) < os.path.getmtime(_SRC):
-        subprocess.check_call(["/usr/bin/gcc", "-O3", "-march=x86-64-v3", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-Wall",
-                               "-std=gnu11", "-shared", _SRC, "-o", _SO, "-lm"])
-    root = R.REFERENCE_ROOT
-    if os.path.isdir(os.path.join(root, "src")):
-        base = R.build()
-        if force or not os.path.exists(_REF_SO) or os.path.getmtime(_REF_SO) < max(os.path.getmtime(_REF_SRC), os.path.getmtime(base)):
-            subprocess.check_call(["/usr/bin/g++", "-std=c++14", "-O2", "-march=x86-64-v3", "-ffp-contract=off", "-fno-fast-math", "-fPIC",
-                                   "-w", "-shared", "-I" + os.path.join(_HERE, "ref_shim"), "-I" + os.path.join(root, "include"),
-                                   "-I" + root, _REF_SRC, "-o", _REF_SO, "-L" + R._DIR, "-lref_orbslam", "-Wl,-rpath,$ORIGIN",
-                                   "-lpthread"])
-    return _SO
+vp, i = C.c_void_p, C.c_int
+lib = _cdll.loader("liborb_oracle.so", {"orb_oracle_normal_depth": (None, [i, vp, vp, vp, vp, vp, C.c_float, i, vp, vp, vp, vp])})
+_ref = _cdll.loader("_ref/libref_drivers.so", {
+    "ref_nd_create": (vp, []),
+    "ref_nd_free": (i, [vp]),
+    "ref_nd_add_keyframe": (i, [vp, vp, vp, i, C.c_float, i, i]),
+    "ref_nd_keyframe": (i, [vp, i, vp, vp, vp]),
+    "ref_nd_add_point": (i, [vp, vp, i]),
+    "ref_nd_add_observation": (i, [vp, i, i, i]),
+    "ref_nd_set_point_bad": (i, [vp, i]),
+    "ref_nd_set_world_pos": (i, [vp, i, vp]),
+    "ref_nd_update": (i, [vp, i]),
+    "ref_nd_get": (i, [vp, i, vp, vp, vp]),
+    "ref_nd_observations": (i, [vp, i, vp, vp, i]),
+    "ref_shim_scale_add": (None, [vp, vp, C.c_double, i, vp]),
+})
 
 
 def ref_available():
-    return os.path.exists(_REF_SO) and R.available()
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        build()
-        L = C.CDLL(_SO)
-        vp, i = C.c_void_p, C.c_int
-        L.orb_oracle_normal_depth.argtypes = [i, vp, vp, vp, vp, vp, C.c_float, i, vp, vp, vp, vp]
-        L.orb_oracle_normal_depth.restype = None
-        _lib = L
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return _cdll.ref_available("libref_drivers.so")
 
 
 def normal_depth(world, ref_centers, ref_octave, group_ptr, obs_centers, scale_factor, scale_factors, normal=None, min_dist=None,
@@ -77,30 +51,6 @@ def normal_depth(world, ref_centers, ref_octave, group_ptr, obs_centers, scale_f
     lib().orb_oracle_normal_depth(n, _p(w), _p(rc), _p(oct_), _p(gp), _p(oc), float(np.float32(scale_factor)), len(sf), _p(sf), _p(on),
                                   _p(omin), _p(omax))
     return on[:n], omin[:n], omax[:n]
-
-
-def _ref():
-    global _ref_lib
-    if _ref_lib is None:
-        if not os.path.exists(_REF_SO):
-            build()
-        L = C.CDLL(_REF_SO, mode=os.RTLD_NOW | os.RTLD_LOCAL)
-        vp, i = C.c_void_p, C.c_int
-        L.ref_nd_create.restype = vp
-        L.ref_nd_free.argtypes = [vp]
-        L.ref_nd_add_keyframe.argtypes = [vp, vp, vp, i, C.c_float, i, i]
-        L.ref_nd_keyframe.argtypes = [vp, i, vp, vp, vp]
-        L.ref_nd_add_point.argtypes = [vp, vp, i]
-        L.ref_nd_add_observation.argtypes = [vp, i, i, i]
-        L.ref_nd_set_point_bad.argtypes = [vp, i]
-        L.ref_nd_set_world_pos.argtypes = [vp, i, vp]
-        L.ref_nd_update.argtypes = [vp, i]
-        L.ref_nd_get.argtypes = [vp, i, vp, vp, vp]
-        L.ref_nd_observations.argtypes = [vp, i, vp, vp, i]
-        L.ref_shim_scale_add.argtypes = [vp, vp, C.c_double, i, vp]
-        L.ref_shim_scale_add.restype = None
-        _ref_lib = L
-    return _ref_lib
 
 
 def shim_scale_add(x, y, beta):

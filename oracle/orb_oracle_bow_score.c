@@ -2,8 +2,8 @@
  * LoopClosing::DetectLoop uses it (src/LoopClosing.cc:117-131):
  *   L1Scoring::score          Thirdparty/DBoW2/DBoW2/ScoringObject.cpp:23-67
  *   the minScore loop         src/LoopClosing.cc:117-131
- * BowVectors are sorted arrays of (word id, value), as everywhere in the oracle.  Built into its own library
- * (liborb_oracle_bow_score.so) by oracle/bow_score.py with the flags of oracle/Makefile; pinned to the reference's DBoW2 by
+ * BowVectors are sorted arrays of (word id, value), as everywhere in the oracle.  Built into oracle/liborb_oracle.so as
+ * its own object by oracle/Makefile; pinned to the reference's DBoW2 by
  * tests/test_oracle_bow_score.py.  LoopClosing.cc itself needs ROS and is not compiled: its five-line loop is restated.
  */
 #include <math.h>

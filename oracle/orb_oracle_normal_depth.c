@@ -5,8 +5,8 @@
  *   cv::norm                                   sqrt of the double sum of squares, x, y, z in order
  *   normal/n                                   convertTo scaling: normal_k * (float)(1.0/n) + 0.0f
  *   mfMinDistance = (1.0f/scaleFactor)*dist / GetScaleFactor(level), mfMaxDistance = scaleFactor*dist * GetScaleFactor(nLevels-1-level)
- * Host arrays in the layout of orbfe_normal_and_depth.  Built into its own library (liborb_oracle_normal_depth.so) by
- * oracle/normal_depth.py with the flags of oracle/Makefile (-ffp-contract=off: no FMA); pinned to the reference's own
+ * Host arrays in the layout of orbfe_normal_and_depth.  Built into oracle/liborb_oracle.so as its own object by
+ * oracle/Makefile (-ffp-contract=off: no FMA); pinned to the reference's own
  * UpdateNormalAndDepth by tests/test_oracle_normal_depth.py.
  */
 #include <math.h>

@@ -11,60 +11,81 @@ import subprocess
 
 import numpy as np
 
-from . import KP_DTYPE
+from . import KP_DTYPE, _cdll
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_DIR = os.path.join(_HERE, "_ref")
 REFERENCE_ROOT = os.environ.get("ORB_REFERENCE_ROOT", "/root/reference")
-_libs = {}
 
 
-def build(force=False):
-    """Build oracle/_ref/*.so from the reference sources when they are present (this container); otherwise keep what is there."""
+def build():
+    """Build oracle/_ref/ with oracle/Makefile (`make ref`) where the reference sources are present (this container);
+    otherwise keep what is there."""
     if os.path.isdir(os.path.join(REFERENCE_ROOT, "src")):
-        from . import build as build_oracle
-        build_oracle()
-        if force:
-            subprocess.call(["rm", "-rf", _DIR])
-        subprocess.check_call(["make", "-C", _HERE, "-s", "ref", "REF=" + REFERENCE_ROOT], env={**os.environ, "CC": "gcc", "CXX": "g++"})
-    return os.path.join(_DIR, "libref_orbslam.so")
+        subprocess.check_call(["make", "-C", _cdll.HERE, "-s", "ref", "REF=" + REFERENCE_ROOT])
+    return os.path.join(_cdll.REF_DIR, "libref_orbslam.so")
 
 
 def available(which="ref"):
-    return os.path.exists(os.path.join(_DIR, "lib%s_orbslam.so" % which))
+    return os.path.exists(os.path.join(_cdll.REF_DIR, "lib%s_orbslam.so" % which))
+
+
+def _signatures():
+    vp, f, i = C.c_void_p, C.c_float, C.c_int
+    return {
+        "ref_extract": (i, [i, f, i, i, i, vp, i, i, C.c_size_t, vp, vp, i]),
+        "ref_frame_from_image": (vp, [vp, i, i, C.c_size_t, f, f, f, f, vp, i, f, i, i, i]),
+        "ref_frame_from_arrays": (vp, [vp, vp, i, i, i, f, f, f, f, f, i]),
+        "ref_frame_free": (i, [vp]),
+        "ref_frame_n": (i, [vp]),
+        "ref_frame_get": (i, [vp, vp, vp, vp, vp, vp]),
+        "ref_frame_grid": (i, [vp, vp, vp]),
+        "ref_frame_features_in_area": (i, [vp, f, f, f, i, i, vp, i]),
+        "ref_search_by_projection_ff": (i, [vp, vp, vp, vp, vp, vp, f, f, i, vp]),
+        "ref_window_search": (i, [vp, vp, vp, i, i, i, f, i, vp]),
+        "ref_search_for_initialization": (i, [vp, vp, vp, i, f, i, vp]),
+        "ref_search_local_points": (i, [vp, i, vp, vp, vp, vp, vp, f, f, vp]),
+        "ref_search_by_projection_f1f2": (i, [vp, vp, vp, vp, vp, i, f, vp]),
+        "ref_descriptor_distance": (i, [vp, vp]),
+        # KeyFrame-level scenes (M4, M5, M9-M12, N4): the id-based driver API
+        "ref_frame_set_pose": (i, [vp, vp]),
+        "ref_frame_set_feature_vector": (i, [vp, i, vp, vp, vp]),
+        "ref_frame_set_map_points": (i, [vp, vp]),
+        "ref_frame_get_map_points": (i, [vp, vp]),
+        "ref_kf_create": (i, [vp, vp]),
+        "ref_kf_set_feature_vector": (i, [i, i, vp, vp, vp]),
+        "ref_mp_create": (i, [vp, vp, vp, f, f, i]),
+        "ref_mp_set_bad": (i, [i]),
+        "ref_kf_add_map_point": (i, [i, i, i]),
+        "ref_kf_get_map_points": (i, [i, vp]),
+        "ref_kf_n": (i, [i]),
+        "ref_mp_state": (i, [i, vp, vp, vp, i]),
+        "ref_search_by_projection_frame_kf": (i, [vp, i, vp, i, f, i, f, i, vp]),
+        "ref_search_by_projection_sim3": (i, [i, vp, vp, i, vp, i, f]),
+        "ref_search_by_bow_kf_frame": (i, [i, vp, f, i, vp]),
+        "ref_search_by_bow_kf_kf": (i, [i, i, f, i, vp]),
+        "ref_search_for_triangulation": (i, [i, i, vp, f, i, vp, i]),
+        "ref_search_by_sim3": (i, [i, i, vp, f, vp, vp, f]),
+        "ref_fuse": (i, [i, vp, i, f]),
+        "ref_fuse_sim3": (i, [i, vp, vp, i, f]),
+        "ref_mp_compute_distinctive": (i, [i, vp]),
+        "ref_world_counts": (i, [vp, vp]),
+        # N2 / N3: DBoW2 vocabulary and KeyFrameDatabase
+        "ref_voc_load": (vp, [C.c_char_p]),
+        "ref_voc_words": (i, [vp]),
+        "ref_bow_transform": (i, [vp, vp, i, i, vp, vp, vp, vp, vp, vp, vp]),
+        "ref_db_add": (i, [vp, vp, vp, i]),
+        "ref_db_set_covisibles": (i, [vp, i, vp, i]),
+        "ref_db_detect_loop": (i, [vp, vp, vp, i, vp, i, f, vp, i]),
+        "ref_db_detect_reloc": (i, [vp, vp, vp, i, vp, i]),
+    }
+
+
+_libs = {which: _cdll.loader("_ref/lib%s_orbslam.so" % which, _signatures()) for which in ("ref", "facade")}
+_p = _cdll.p
 
 
 def lib(which="ref"):
     """which = "ref" (reference ORBextractor.cc / ORBmatcher.cc) or "facade" (the product's facades over liborbfe.so)."""
-    if which in _libs:
-        return _libs[which]
-    path = os.path.join(_DIR, "lib%s_orbslam.so" % which)
-    if not os.path.exists(path):
-        build()
-    L = C.CDLL(path, mode=os.RTLD_NOW | os.RTLD_LOCAL)
-    vp, f, i = C.c_void_p, C.c_float, C.c_int
-    L.ref_extract.argtypes = [i, f, i, i, i, vp, i, i, C.c_size_t, vp, vp, i]
-    L.ref_frame_from_image.argtypes = [vp, i, i, C.c_size_t, f, f, f, f, vp, i, f, i, i, i]
-    L.ref_frame_from_image.restype = vp
-    L.ref_frame_from_arrays.argtypes = [vp, vp, i, i, i, f, f, f, f, f, i]
-    L.ref_frame_from_arrays.restype = vp
-    L.ref_frame_free.argtypes = [vp]
-    L.ref_frame_n.argtypes = [vp]
-    L.ref_frame_get.argtypes = [vp, vp, vp, vp, vp, vp]
-    L.ref_frame_grid.argtypes = [vp, vp, vp]
-    L.ref_frame_features_in_area.argtypes = [vp, f, f, f, i, i, vp, i]
-    L.ref_search_by_projection_ff.argtypes = [vp, vp, vp, vp, vp, vp, f, f, i, vp]
-    L.ref_window_search.argtypes = [vp, vp, vp, i, i, i, f, i, vp]
-    L.ref_search_for_initialization.argtypes = [vp, vp, vp, i, f, i, vp]
-    L.ref_search_local_points.argtypes = [vp, i, vp, vp, vp, vp, vp, f, f, vp]
-    L.ref_search_by_projection_f1f2.argtypes = [vp, vp, vp, vp, vp, i, f, vp]
-    L.ref_descriptor_distance.argtypes = [vp, vp]
-    _libs[which] = L
-    return L
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p) if a is not None else None
+    return _libs[which]()
 
 
 def extract(img, nfeatures=1000, scale_factor=1.2, nlevels=8, score_type=1, fast_th=20, which="ref"):
@@ -169,36 +190,6 @@ def descriptor_distance(a, b, which="ref"):
 
 
 # ---- KeyFrame-level scenes (M4, M5, M9-M12, N4): thin wrappers over the id-based driver API ------------------------------
-def _bind_scene(L):
-    if getattr(L, "_scene_bound", False):
-        return L
-    vp, f, i = C.c_void_p, C.c_float, C.c_int
-    L.ref_frame_set_pose.argtypes = [vp, vp]
-    L.ref_frame_set_feature_vector.argtypes = [vp, i, vp, vp, vp]
-    L.ref_frame_set_map_points.argtypes = [vp, vp]
-    L.ref_frame_get_map_points.argtypes = [vp, vp]
-    L.ref_kf_create.argtypes = [vp, vp]
-    L.ref_kf_set_feature_vector.argtypes = [i, i, vp, vp, vp]
-    L.ref_mp_create.argtypes = [vp, vp, vp, f, f, i]
-    L.ref_mp_set_bad.argtypes = [i]
-    L.ref_kf_add_map_point.argtypes = [i, i, i]
-    L.ref_kf_get_map_points.argtypes = [i, vp]
-    L.ref_kf_n.argtypes = [i]
-    L.ref_mp_state.argtypes = [i, vp, vp, vp, i]
-    L.ref_search_by_projection_frame_kf.argtypes = [vp, i, vp, i, f, i, f, i, vp]
-    L.ref_search_by_projection_sim3.argtypes = [i, vp, vp, i, vp, i, f]
-    L.ref_search_by_bow_kf_frame.argtypes = [i, vp, f, i, vp]
-    L.ref_search_by_bow_kf_kf.argtypes = [i, i, f, i, vp]
-    L.ref_search_for_triangulation.argtypes = [i, i, vp, f, i, vp, i]
-    L.ref_search_by_sim3.argtypes = [i, i, vp, f, vp, vp, f]
-    L.ref_fuse.argtypes = [i, vp, i, f]
-    L.ref_fuse_sim3.argtypes = [i, vp, vp, i, f]
-    L.ref_mp_compute_distinctive.argtypes = [i, vp]
-    L.ref_world_counts.argtypes = [vp, vp]
-    L._scene_bound = True
-    return L
-
-
 def _i32(a):
     return np.ascontiguousarray(a, np.int32)
 
@@ -212,7 +203,7 @@ class Scene:
 
     def __init__(self, which="ref"):
         self.which = which
-        self.L = _bind_scene(lib(which))
+        self.L = lib(which)
 
     def frame(self, kps, desc, W, H, fx, fy, cx, cy, scale_factor=1.2, nlevels=8):
         return RefFrame.from_arrays(kps, desc, W, H, fx, fy, cx, cy, scale_factor, nlevels, which=self.which)
@@ -346,18 +337,8 @@ def write_vocabulary_text(voc, path, scoring=0, weighting=0):
 
 class RefVocabulary:
     def __init__(self, path, which="ref"):
-        L = lib(which)
-        vp, i = C.c_void_p, C.c_int
-        L.ref_voc_load.argtypes = [C.c_char_p]
-        L.ref_voc_load.restype = vp
-        L.ref_voc_words.argtypes = [vp]
-        L.ref_bow_transform.argtypes = [vp, vp, i, i, vp, vp, vp, vp, vp, vp, vp]
-        L.ref_db_add.argtypes = [vp, vp, vp, i]
-        L.ref_db_set_covisibles.argtypes = [vp, i, vp, i]
-        L.ref_db_detect_loop.argtypes = [vp, vp, vp, i, vp, i, C.c_float, vp, i]
-        L.ref_db_detect_reloc.argtypes = [vp, vp, vp, i, vp, i]
-        self.L = L
-        self.h = L.ref_voc_load(path.encode())
+        self.L = lib(which)
+        self.h = self.L.ref_voc_load(path.encode())
         assert self.h, "loadFromTextFile failed"
         self.nkf = 0
 

@@ -1,65 +1,28 @@
 """The reference's own KeyFrameDatabase (src/KeyFrameDatabase.cc, compiled unmodified into oracle/_ref/libref_orbslam.so)
 behind the slot interface of orbfe_kfdb_*, for replaying scripted sequences (TEST INFRASTRUCTURE ONLY).
 
-oracle/ref_shim/ref_kfdb.cc is the driver; build() compiles it into oracle/_ref/libref_kfdb.so, linked against
-libref_orbslam.so, where the reference sources exist.  Elsewhere the prebuilt library is used as it is."""
+oracle/ref_shim/ref_kfdb.cc is the driver, in oracle/_ref/libref_drivers.so, linked against libref_orbslam.so."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from . import ref as R
+from . import _cdll
+from ._cdll import p as _p
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(R._DIR, "libref_kfdb.so")
-_SRC = os.path.join(_HERE, "ref_shim", "ref_kfdb.cc")
-_lib = None
-
-
-def build(force=False):
-    """Compile the driver with the flags of oracle/Makefile's reference objects (after `make ref`)."""
-    root = R.REFERENCE_ROOT
-    if not os.path.isdir(os.path.join(root, "src")):
-        return _SO
-    base = R.build()
-    if not force and os.path.exists(_SO) and os.path.getmtime(_SO) >= max(os.path.getmtime(_SRC), os.path.getmtime(base)):
-        return _SO
-    cmd = ["/usr/bin/g++", "-std=c++14", "-O2", "-march=x86-64-v3", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-w", "-shared",
-           "-I" + os.path.join(_HERE, "ref_shim"), "-I" + os.path.join(root, "include"), "-I" + root, _SRC, "-o", _SO,
-           "-L" + R._DIR, "-lref_orbslam", "-Wl,-rpath,$ORIGIN", "-lpthread"]
-    subprocess.check_call(cmd)
-    return _SO
+vp, i = C.c_void_p, C.c_int
+lib = _cdll.loader("_ref/libref_drivers.so", {
+    "ref_kfdb_create": (vp, [C.c_char_p]),
+    "ref_kfdb_add": (i, [vp, vp, vp, i]),
+    "ref_kfdb_erase": (None, [vp, i]),
+    "ref_kfdb_clear": (None, [vp]),
+    "ref_kfdb_set_covisibles": (None, [vp, i, vp, i]),
+    "ref_kfdb_detect_loop": (i, [vp, vp, vp, i, vp, i, C.c_float, vp, i, vp, vp, vp]),
+    "ref_kfdb_detect_reloc": (i, [vp, vp, vp, i, vp, i, vp, vp, vp]),
+})
 
 
 def available():
-    return os.path.exists(_SO) and os.path.exists(os.path.join(R._DIR, "libref_orbslam.so"))
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        if not os.path.exists(_SO):
-            build()
-        L = C.CDLL(_SO, mode=os.RTLD_NOW | os.RTLD_LOCAL)
-        vp, i = C.c_void_p, C.c_int
-        L.ref_kfdb_create.argtypes = [C.c_char_p]
-        L.ref_kfdb_create.restype = vp
-        L.ref_kfdb_add.argtypes = [vp, vp, vp, i]
-        L.ref_kfdb_erase.argtypes = [vp, i]
-        L.ref_kfdb_erase.restype = None
-        L.ref_kfdb_clear.argtypes = [vp]
-        L.ref_kfdb_clear.restype = None
-        L.ref_kfdb_set_covisibles.argtypes = [vp, i, vp, i]
-        L.ref_kfdb_set_covisibles.restype = None
-        L.ref_kfdb_detect_loop.argtypes = [vp, vp, vp, i, vp, i, C.c_float, vp, i, vp, vp, vp]
-        L.ref_kfdb_detect_reloc.argtypes = [vp, vp, vp, i, vp, i, vp, vp, vp]
-        _lib = L
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return _cdll.ref_available("libref_drivers.so")
 
 
 class RefKeyFrameDatabase:

@@ -2,7 +2,7 @@
 // AddConnection, UpdateBestCovisibles, EraseConnection, SetBadFlag; src/KeyFrame.cc) on scripted maps (TEST INFRASTRUCTURE
 // ONLY).
 //
-// Built by oracle/covis.py into oracle/_ref/libref_covis.so next to, and linked against, libref_orbslam.so: the KeyFrame /
+// Included by ref_observations.cc (oracle/_ref/libref_drivers.so, linked against libref_orbslam.so): the KeyFrame /
 // MapPoint / Map code that runs is the reference's, compiled unmodified there.  A handle owns one map whose keyframes and
 // points sit in one arena in creation order, so every std::map keyed by KeyFrame* iterates in creation order and every
 // pointer tie falls the way creation order does: the creation index is the order key the oracle and the device take.

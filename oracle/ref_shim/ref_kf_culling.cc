@@ -1,8 +1,8 @@
 // oracle/ref_shim/ref_kf_culling.cc -- the driver of ref_observations.cc with the reference's own, unmodified
 // LocalMapping::KeyFrameCulling (src/LocalMapping.cc:524-578) on scripted maps (TEST INFRASTRUCTURE ONLY).
 //
-// Built by oracle/kf_culling.py into oracle/_ref/libref_kf_culling.so together with the reference's src/LocalMapping.cc,
-// both against the stand-in headers of oracle/ref_shim_lm/ (ROS, tf and g2o names that LocalMapping.h pulls in), linked
+// Built by oracle/Makefile into oracle/_ref/libref_kf_culling.so together with the reference's src/LocalMapping.cc,
+// both against the stand-in headers of oracle/ref_shim_slam/ (ROS, tf and g2o names that LocalMapping.h pulls in), linked
 // against libref_orbslam.so.  A culling call sets mpCurrentKeyFrame and calls KeyFrameCulling(); the verdict of each entry
 // of the current keyframe's GetVectorCovisibleKeyFrames() is read from what SetBadFlag left behind: every listed keyframe
 // is put into the Map just before the call, and SetBadFlag removes it (Map::EraseKeyFrame) only when it runs past its

@@ -1,7 +1,7 @@
 // oracle/ref_shim/ref_kfdb.cc -- extern "C" driver of the reference's OWN KeyFrameDatabase (src/KeyFrameDatabase.cc) for
 // scripted sequences of add / erase / clear / covisibility changes / queries (TEST INFRASTRUCTURE ONLY).
 //
-// Built by oracle/ref_kfdb.py into oracle/_ref/libref_kfdb.so next to, and linked against, libref_orbslam.so: the
+// Built by oracle/Makefile into oracle/_ref/libref_drivers.so next to, and linked against, libref_orbslam.so: the
 // KeyFrame / KeyFrameDatabase / DBoW2 code that runs is the reference's, compiled unmodified there.  Frames come from that
 // library's ref_frame_from_arrays.  Each handle owns its vocabulary, map and database; keyframe k is the k-th add().
 // Keyframes are placed in zeroed memory: KeyFrame's constructor leaves mLoopScore / mRelocScore uninitialised, and the

@@ -2,8 +2,8 @@
 // Tracking::UpdateReference (src/Tracking.cc:728-839: UpdateReferenceKeyFrames and UpdateReferencePoints) on scripted maps
 // (TEST INFRASTRUCTURE ONLY).
 //
-// Built by oracle/local_map.py into oracle/_ref/libref_local_map.so together with the reference's src/Tracking.cc, both
-// against the stand-in headers of oracle/ref_shim_tr/ and oracle/ref_shim_lm/ (ROS, tf, cv_bridge and g2o names that
+// Built by oracle/Makefile into oracle/_ref/libref_local_map.so together with the reference's src/Tracking.cc, both
+// against the stand-in headers of oracle/ref_shim_slam/ (ROS, tf, cv_bridge and g2o names that
 // Tracking.h and Tracking.cc pull in), linked against libref_orbslam.so.  One Tracking per map is made by the reference's
 // constructor (its settings file is the fixed table of ref_tr_prelude.h).  A call builds mCurrentFrame as
 // ref_cv_add_keyframe builds its Frames, with a fresh Frame::nNextId (so no stamp of an earlier call matches) and the

@@ -1,7 +1,7 @@
 // oracle/ref_shim/ref_map_point.cc -- extern "C" driver of the reference's OWN MapPoint::UpdateNormalAndDepth
 // (src/MapPoint.cc:273-312) on scripted maps (TEST INFRASTRUCTURE ONLY).
 //
-// Built by oracle/normal_depth.py into oracle/_ref/libref_map_point.so next to, and linked against, libref_orbslam.so: the
+// Built by oracle/Makefile into oracle/_ref/libref_drivers.so next to, and linked against, libref_orbslam.so: the
 // MapPoint / KeyFrame / Frame code that runs is the reference's, compiled unmodified there.  A handle owns one map: keyframes
 // built from a pose and keypoint octaves, map points with a reference keyframe and observations.  Scripts set a point's
 // position with SetWorldPos, call UpdateNormalAndDepth, and read back GetNormal / GetMin/MaxDistanceInvariance and every

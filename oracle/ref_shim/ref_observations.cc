@@ -4,8 +4,8 @@
 // an observation on their own (Tracking fills a new keyframe's mvpMapPoints before ProcessNewKeyFrame adds the
 // observations), and the readback of GetReferenceKeyFrame().
 //
-// Built by oracle/observations.py into oracle/_ref/libref_observations.so, linked against libref_orbslam.so like
-// libref_covis.so.  Keyframes made here carry zero descriptors, so Replace's ComputeDistinctiveDescriptors has rows to read.
+// Built by oracle/Makefile into oracle/_ref/libref_drivers.so, linked against libref_orbslam.so; the culling and local-map
+// drivers include it.  Keyframes made here carry zero descriptors, so Replace's ComputeDistinctiveDescriptors has rows to read.
 #include "ref_covis.cc"
 
 extern "C" {

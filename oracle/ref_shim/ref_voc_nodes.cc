@@ -1,7 +1,7 @@
 // oracle/ref_shim/ref_voc_nodes.cc -- extern "C" driver of the reference's OWN TemplatedVocabulary::loadFromTextFile
 // (Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1338-1424), the call of src/main.cc (TEST INFRASTRUCTURE ONLY).
 //
-// Built by oracle/voc_text.py into oracle/_ref/libref_voc_nodes.so, linked against libref_orbslam.so (the reference's DBoW2
+// Built by oracle/Makefile into oracle/_ref/libref_drivers.so, linked against libref_orbslam.so (the reference's DBoW2
 // compiled unmodified).  m_nodes is protected: a class derived from ORBVocabulary reads it out, field for field.
 #include <opencv2/core/core.hpp>
 

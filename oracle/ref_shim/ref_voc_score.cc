@@ -1,7 +1,7 @@
 // oracle/ref_shim/ref_voc_score.cc -- extern "C" driver of the reference's OWN ORBVocabulary::score (DBoW2
 // TemplatedVocabulary::score -> L1Scoring::score), the call of LoopClosing.cc:127 (TEST INFRASTRUCTURE ONLY).
 //
-// Built by oracle/bow_score.py into oracle/_ref/libref_voc_score.so next to, and linked against, libref_orbslam.so: the
+// Built by oracle/Makefile into oracle/_ref/libref_drivers.so next to, and linked against, libref_orbslam.so: the
 // DBoW2 code that runs is the reference's, compiled unmodified there.  A handle owns a vocabulary loaded from DBoW2's text
 // format; its header names the scoring object.
 #include <opencv2/core/core.hpp>

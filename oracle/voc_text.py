@@ -1,63 +1,28 @@
 """The reference's own TemplatedVocabulary::loadFromTextFile and its m_nodes, for the tests of orbfe_vocabulary_load_text
 (TEST INFRASTRUCTURE ONLY).
 
-  RefVocabularyNodes   oracle/ref_shim/ref_voc_nodes.cc compiled into oracle/_ref/libref_voc_nodes.so, linked against
-                       libref_orbslam.so (the reference's DBoW2, unmodified), where the reference sources exist; elsewhere the
-                       prebuilt library is used as it is
+  RefVocabularyNodes   oracle/ref_shim/ref_voc_nodes.cc in oracle/_ref/libref_drivers.so, linked against libref_orbslam.so
+                       (the reference's DBoW2, unmodified)
   text_for_reference   the text the reference is given: the same bytes without a final newline (a final newline makes the
                        reference read one more, empty line and create a node from uninitialised values)"""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 
-from . import ref as R
+from . import _cdll
+from ._cdll import p as _p
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_REF_SO = os.path.join(R._DIR, "libref_voc_nodes.so")
-_REF_SRC = os.path.join(_HERE, "ref_shim", "ref_voc_nodes.cc")
-_lib = None
-
-
-def build(force=False):
-    """Compile the driver where the reference sources exist (after `make ref`)."""
-    root = R.REFERENCE_ROOT
-    if os.path.isdir(os.path.join(root, "src")):
-        base = R.build()
-        if force or not os.path.exists(_REF_SO) or os.path.getmtime(_REF_SO) < max(os.path.getmtime(_REF_SRC), os.path.getmtime(base)):
-            subprocess.check_call(["/usr/bin/g++", "-std=c++14", "-O2", "-march=x86-64-v3", "-ffp-contract=off", "-fno-fast-math", "-fPIC",
-                                   "-w", "-shared", "-I" + os.path.join(_HERE, "ref_shim"), "-I" + os.path.join(root, "include"),
-                                   "-I" + root, _REF_SRC, "-o", _REF_SO, "-L" + R._DIR, "-lref_orbslam", "-Wl,-rpath,$ORIGIN",
-                                   "-lpthread"])
-    return _REF_SO
+_load = _cdll.loader("_ref/libref_drivers.so", {
+    "ref_voc_nodes_load": (C.c_void_p, [C.c_char_p, C.POINTER(C.c_double)]),
+    "ref_voc_nodes_free": (None, [C.c_void_p]),
+    "ref_voc_nodes_info": (None, [C.c_void_p] + [C.POINTER(C.c_int)] * 7),
+    "ref_voc_nodes_export": (None, [C.c_void_p] * 7),
+})
 
 
 def available():
-    return os.path.exists(_REF_SO) and R.available()
-
-
-def _load():
-    global _lib
-    if _lib is None:
-        if not os.path.exists(_REF_SO):
-            build()
-        L = C.CDLL(_REF_SO, mode=os.RTLD_NOW | os.RTLD_LOCAL)
-        vp, ip = C.c_void_p, C.POINTER(C.c_int)
-        L.ref_voc_nodes_load.argtypes = [C.c_char_p, C.POINTER(C.c_double)]
-        L.ref_voc_nodes_load.restype = vp
-        L.ref_voc_nodes_free.argtypes = [vp]
-        L.ref_voc_nodes_free.restype = None
-        L.ref_voc_nodes_info.argtypes = [vp] + [ip] * 7
-        L.ref_voc_nodes_info.restype = None
-        L.ref_voc_nodes_export.argtypes = [vp] * 7
-        L.ref_voc_nodes_export.restype = None
-        _lib = L
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return _cdll.ref_available("libref_drivers.so")
 
 
 def text_for_reference(src, dst):

@@ -16,7 +16,7 @@ from oracle.kfdb import l1_score
 import bow_score_scenes as S
 
 needs_ref = pytest.mark.skipif(not OS.ref_available() and not os.path.isdir(os.path.join(R.REFERENCE_ROOT, "src")),
-                               reason="oracle/_ref/libref_voc_score.so not built and the reference sources are absent")
+                               reason="oracle/_ref/libref_drivers.so not built and the reference sources are absent")
 PAIRS = S.hand_made_pairs()
 
 

@@ -8,7 +8,7 @@ import pytest
 import covis_scenes as S
 from oracle import covis as OC
 
-pytestmark = pytest.mark.skipif(not OC.ref_available(), reason="oracle/_ref/libref_covis.so not built (needs the reference sources)")
+pytestmark = pytest.mark.skipif(not OC.ref_available(), reason="oracle/_ref/libref_drivers.so not built (needs the reference sources)")
 
 
 def _compare(ref, orc, slot_of, kfs, where):

@@ -16,7 +16,7 @@ from oracle.kfdb import KeyFrameDatabase as OracleDB
 import kfdb_scenarios as S
 
 pytestmark = pytest.mark.skipif(not RK.available() and not os.path.isdir(os.path.join(R.REFERENCE_ROOT, "src")),
-                                reason="oracle/_ref/libref_kfdb.so not built and the reference sources are absent")
+                                reason="oracle/_ref/libref_drivers.so not built and the reference sources are absent")
 
 
 def same_outputs(got, want, tag):

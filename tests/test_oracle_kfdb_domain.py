@@ -16,7 +16,7 @@ from oracle.kfdb import F32, KeyFrameDatabase as OracleDB, l1_score
 from test_oracle_kfdb import same_outputs
 
 HAVE_REF = RK.available() or os.path.isdir(os.path.join(R.REFERENCE_ROOT, "src"))
-needs_ref = pytest.mark.skipif(not HAVE_REF, reason="oracle/_ref/libref_kfdb.so not built and the reference sources are absent")
+needs_ref = pytest.mark.skipif(not HAVE_REF, reason="oracle/_ref/libref_drivers.so not built and the reference sources are absent")
 
 
 def run_oracle(sc):

@@ -14,7 +14,7 @@ GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "openc
 SCENES = S.all_scenes()
 IDS = [s["name"] for s in SCENES]
 
-needs_ref = pytest.mark.skipif(not N.ref_available(), reason="oracle/_ref/libref_map_point.so not built (reference sources absent)")
+needs_ref = pytest.mark.skipif(not N.ref_available(), reason="oracle/_ref/libref_drivers.so not built (reference sources absent)")
 
 
 def _oracle(scene):

@@ -10,7 +10,7 @@ import covis_scenes as S
 import observation_scenes as OS
 from oracle import observations as OO
 
-needs_ref = pytest.mark.skipif(not OO.ref_available(), reason="oracle/_ref/libref_observations.so not built (needs the reference sources)")
+needs_ref = pytest.mark.skipif(not OO.ref_available(), reason="oracle/_ref/libref_drivers.so not built (needs the reference sources)")
 
 
 def oracle_inputs(model, slot_of, K):

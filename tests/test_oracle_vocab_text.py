@@ -11,7 +11,7 @@ from oracle import voc_text as VT
 from orb_slam_b200.synth import random_vocabulary
 
 needs_ref = pytest.mark.skipif(not VT.available() and not os.path.isdir(os.path.join(R.REFERENCE_ROOT, "src")),
-                               reason="oracle/_ref/libref_voc_nodes.so not built and the reference sources are absent")
+                               reason="oracle/_ref/libref_drivers.so not built and the reference sources are absent")
 
 
 def parents_of(voc):
