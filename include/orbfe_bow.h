@@ -356,10 +356,13 @@ int orbfe_covis_create(int device, int max_keyframes, int max_connections, int m
 void orbfe_covis_destroy(OrbfeCovisGraph *g);
 
 /* n new keyframes (host arrays): slot slots[i], mnId ids[i] (only ids[i] == 0 matters: such a keyframe gets no parent and
- * is never erased) and order key keys[i].  Each starts as a fresh KeyFrame: no weights, empty lists, mbFirstConnection.
+ * is never erased) and order key keys[i].  Every uint64_t is a valid key, 0 and 2^64 - 1 included.  Each starts as a fresh
+ * KeyFrame: no weights, empty lists, mbFirstConnection.
  * All or nothing, ORBFE_ERR_ARG: a slot out of range, live or listed twice, a key equal to a live slot's key or repeated,
- * or a retired slot that some weight map still names (re-adding it would alias the reference's stale pointer).
- * Synchronous. */
+ * a retired slot that some weight map still names (re-adding it would alias the reference's stale pointer), or a key equal
+ * to the key of such a retired slot (the reference never reuses a bad KeyFrame's pointer; the new keyframe would merge
+ * onto the stale entry).  The check reads the host's copy of the keys and the same copy of the name counts as the check
+ * before it.  Synchronous. */
 int orbfe_covis_add(OrbfeCovisGraph *g, int n, const int32_t *slots, const int32_t *ids, const uint64_t *keys);
 
 /* UpdateConnections() of the keyframes slots[0..n) (a host array of distinct live slots, 1 <= n <= max_batch; n = 0 does

@@ -31,17 +31,27 @@ def _open(name):
     return C.CDLL(path, mode=os.RTLD_NOW | os.RTLD_LOCAL)
 
 
-def loader(name, sigs):
+def loader(name, sigs, optional=()):
     """A function returning oracle/<name> ("liborb_oracle.so" or "_ref/lib*.so") with the signature table
-    {function: (restype, [argtypes])} applied.  A library is opened once per name; each table is applied on its first call."""
+    {function: (restype, [argtypes])} applied.  A library is opened once per name; each table is applied on its first call.
+    The functions named in `optional` may be absent (a prebuilt _ref/ library older than its driver source, where the
+    reference sources to rebuild it are not present): they are left unbound, so `has(lib, f)` is False; every other
+    function of the table must be there."""
     @functools.cache
     def lib():
         L = _open(name)
         for f, (restype, argtypes) in sigs.items():
+            if f in optional and not hasattr(L, f):
+                continue
             fn = getattr(L, f)
             fn.restype, fn.argtypes = restype, argtypes
         return L
     return lib
+
+
+def has(lib, f):
+    """whether the library returned by loader function `lib` exports function `f`"""
+    return hasattr(lib(), f)
 
 
 def ref_available(name):

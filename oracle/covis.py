@@ -32,6 +32,7 @@ lib = _cdll.loader("liborb_oracle.so", {
 REF_CV = {
     "ref_cv_create": (vp, []),
     "ref_cv_free": (i, [vp]),
+    "ref_cv_set_kf_order": (i, [vp, i, vp]),
     "ref_cv_add_keyframe": (i, [vp, i]),
     "ref_cv_add_point": (i, [vp, i]),
     "ref_cv_add_points": (i, [vp, i, vp]),
@@ -50,11 +51,18 @@ REF_CV = {
     "ref_cv_observations": (i, [vp, i, vp, vp, i]),
     "ref_cv_point_bad": (i, [vp, i]),
 }
-_ref = _cdll.loader("_ref/libref_drivers.so", REF_CV)
+# newer than the rest of the driver: a prebuilt library may lack it (see ref_kf_order_available)
+REF_CV_OPTIONAL = ("ref_cv_set_kf_order",)
+_ref = _cdll.loader("_ref/libref_drivers.so", REF_CV, REF_CV_OPTIONAL)
 
 
 def ref_available():
     return _cdll.ref_available("libref_drivers.so")
+
+
+def ref_kf_order_available():
+    """the driver is built and can lay keyframes out in a given order (RefCovis.set_kf_order)"""
+    return ref_available() and _cdll.has(_ref, "ref_cv_set_kf_order")
 
 
 class CovisOracle:
@@ -115,7 +123,8 @@ class CovisOracle:
 
 
 class RefCovis:
-    """A scripted map of the reference's own KeyFrames and MapPoints (ids = creation order; the first keyframe has mnId 0)."""
+    """A scripted map of the reference's own KeyFrames and MapPoints (ids = creation order; the first keyframe has mnId 0).
+    Pointer order is creation order unless set_kf_order() gives another."""
 
     def __init__(self, cap=1 << 16):
         self.L = _ref()
@@ -132,6 +141,13 @@ class RefCovis:
             self.close()
         except Exception:
             pass
+
+    def set_kf_order(self, rank):
+        """Before the first keyframe: keyframe k is placed at rank[k] among the keyframes' addresses (rank a permutation of
+        0 .. n-1), so every pointer order of the map is rank order rather than creation order; at most n keyframes follow."""
+        r = np.ascontiguousarray(rank, np.int32)
+        if self.L.ref_cv_set_kf_order(self.h, len(r), _p(r)) != 0:
+            raise ValueError("ref_cv_set_kf_order: a keyframe exists or rank is not a permutation")
 
     def add_keyframe(self, nfeatures):
         return self.L.ref_cv_add_keyframe(self.h, int(nfeatures))

@@ -10,6 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _cdll
+from . import covis as CV
 from . import observations as OB
 from ._cdll import p as _p
 
@@ -21,7 +22,7 @@ _ref = _cdll.loader("_ref/libref_kf_culling.so", {
     "ref_kc_set_octaves": (i, [vp, i, i, vp]),
     "ref_kc_set_not_erase": (i, [vp, i]),
     "ref_kc_cull": (i, [vp, i, vp, vp, i, vp]),
-})
+}, CV.REF_CV_OPTIONAL)
 
 # verdicts (ORBFE_CULL_*)
 KEPT, SKIP_ID0, ERASED, NOT_ERASE, RETIRED = 0, 1, 2, 3, 4
@@ -29,6 +30,11 @@ KEPT, SKIP_ID0, ERASED, NOT_ERASE, RETIRED = 0, 1, 2, 3, 4
 
 def ref_available():
     return _cdll.ref_available("libref_kf_culling.so")
+
+
+def ref_kf_order_available():
+    """the driver is built and can lay keyframes out in a given order (RefCovis.set_kf_order)"""
+    return ref_available() and _cdll.has(_ref, "ref_cv_set_kf_order")
 
 
 def cull(cand, live, id0, keys, not_erase, kf_mp, counts, octave, cap, point_bad, ref_slot, obs_cap=None):

@@ -10,6 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _cdll
+from . import covis as CV
 from . import observations as OB
 from ._cdll import p as _p
 
@@ -21,11 +22,16 @@ _ref = _cdll.loader("_ref/libref_local_map.so", {
     "ref_lm_free": (i, [vp]),
     "ref_lm_to_be_erased": (i, [vp, i]),
     "ref_lm_update_reference": (i, [vp, i, vp, vp, i, vp, vp, i, vp, vp]),
-})
+}, CV.REF_CV_OPTIONAL)
 
 
 def ref_available():
     return _cdll.ref_available("libref_local_map.so")
+
+
+def ref_kf_order_available():
+    """the driver is built and can lay keyframes out in a given order (RefCovis.set_kf_order)"""
+    return ref_available() and _cdll.has(_ref, "ref_cv_set_kf_order")
 
 
 def neighbours(lists, nframes):

@@ -27,7 +27,7 @@ REF_OB = {
     "ref_ob_reference": (i, [vp, i]),
     "ref_ob_flatten": (i, [vp, i, vp, vp, i, vp, vp]),
 }
-_ref = _cdll.loader("_ref/libref_drivers.so", REF_OB)
+_ref = _cdll.loader("_ref/libref_drivers.so", REF_OB, CV.REF_CV_OPTIONAL)
 ref_available = CV.ref_available
 
 

@@ -6,6 +6,7 @@ TEST INFRASTRUCTURE ONLY (like everything under oracle/): used by tests/ to vali
 reference's real control flow, and optionally by bench.py's CPU arm.  /root/reference does not exist on the GPU box: there
 the prebuilt library travels with the snapshot and `available()` only reports whether it can be loaded."""
 import ctypes as C
+import hashlib
 import os
 import subprocess
 
@@ -16,11 +17,41 @@ from . import KP_DTYPE, _cdll
 REFERENCE_ROOT = os.environ.get("ORB_REFERENCE_ROOT", "/root/reference")
 
 
+def _sources_digest():
+    """sha256 of this repository's inputs to oracle/_ref/: the Makefile, the stand-in headers and drivers, the facades"""
+    root = os.path.dirname(_cdll.HERE)
+    paths = [os.path.join(_cdll.HERE, "Makefile")]
+    for d in ("ref_shim", "ref_shim_slam"):
+        for dirpath, dirs, files in os.walk(os.path.join(_cdll.HERE, d)):
+            dirs.sort()
+            paths += [os.path.join(dirpath, f) for f in sorted(files)]
+    paths += [os.path.join(root, p) for p in ("include/ORBextractor.h", "include/ORBmatcher.h", "orb_slam_b200/host/ORBextractor.cc",
+                                              "orb_slam_b200/host/ORBmatcher.cc")]
+    h = hashlib.sha256()
+    for p in paths:
+        h.update(os.path.relpath(p, root).encode() + b"\0")
+        with open(p, "rb") as f:
+            h.update(f.read())
+    return h.hexdigest()
+
+
 def build():
     """Build oracle/_ref/ with oracle/Makefile (`make ref`) where the reference sources are present (this container);
-    otherwise keep what is there."""
+    otherwise keep what is there.  make compares times, and a prebuilt _ref/ placed after a checkout is newer than every
+    source, so the digest of the sources it was built from is kept beside it: when the sources differ, everything is
+    rebuilt."""
     if os.path.isdir(os.path.join(REFERENCE_ROOT, "src")):
-        subprocess.check_call(["make", "-C", _cdll.HERE, "-s", "ref", "REF=" + REFERENCE_ROOT])
+        stamp = os.path.join(_cdll.REF_DIR, ".sources.sha256")
+        digest = _sources_digest()
+        try:
+            with open(stamp) as f:
+                built_from = f.read().strip()
+        except OSError:
+            built_from = None
+        force = ["-B"] if built_from != digest else []
+        subprocess.check_call(["make", "-C", _cdll.HERE, "-s"] + force + ["ref", "REF=" + REFERENCE_ROOT])
+        with open(stamp, "w") as f:
+            f.write(digest + "\n")
     return os.path.join(_cdll.REF_DIR, "libref_orbslam.so")
 
 

@@ -6,6 +6,8 @@
 // MapPoint / Map code that runs is the reference's, compiled unmodified there.  A handle owns one map whose keyframes and
 // points sit in one arena in creation order, so every std::map keyed by KeyFrame* iterates in creation order and every
 // pointer tie falls the way creation order does: the creation index is the order key the oracle and the device take.
+// ref_cv_set_kf_order places the keyframes in a given order instead, so that any key map the oracle and the device take
+// has the reference's decision beside it: the key of keyframe k ranks rank[k] among the keys.
 // Observations are made with MapPoint::AddObservation + KeyFrame::AddMapPoint.  The getters read back the graph and the
 // inputs of the next call (every keyframe's mvpMapPoints, every point's observations and isBad()).
 #include <opencv2/core/core.hpp>   // every standard header first: the access hack below must not reach libstdc++
@@ -41,7 +43,10 @@ struct CvMap {
     std::map<const MapPoint *, int> mp_index;
     char *arena;
     size_t used, cap;
-    CvMap() : db(voc), arena(NULL), used(0), cap((size_t)4 << 30) { arena = static_cast<char *>(std::malloc(cap)); }
+    // ref_cv_set_kf_order: keyframe k goes to kf_region + kf_rank[k] * sizeof(KeyFrame); empty: the arena in creation order
+    char *kf_region;
+    std::vector<int> kf_rank;
+    CvMap() : db(voc), arena(NULL), used(0), cap((size_t)4 << 30), kf_region(NULL) { arena = static_cast<char *>(std::malloc(cap)); }
     void *alloc(size_t bytes) {
         used = (used + 63) / 64 * 64;
         if (!arena || used + bytes > cap) { std::fprintf(stderr, "ref_covis: arena exhausted\n"); std::abort(); }
@@ -71,6 +76,22 @@ void *ref_cv_create() {
 }
 void ref_cv_free(void *h) { delete static_cast<CvMap *>(h); }
 
+// Before the first keyframe: keyframe k (k < n) is placed at rank[k] in one region of n KeyFrames, so pointer order, and
+// with it every std::map keyed by KeyFrame* and every pointer tie, is rank order instead of creation order.  rank is a
+// permutation of 0 .. n-1.  Returns 0, or -1 (nothing changed) when a keyframe exists or rank is not a permutation.
+int ref_cv_set_kf_order(void *h, int n, const int *rank) {
+    CvMap &M = *static_cast<CvMap *>(h);
+    if (!M.kfs.empty() || n < 1) return -1;
+    std::vector<char> seen((size_t)n, 0);
+    for (int k = 0; k < n; k++) {
+        if (rank[k] < 0 || rank[k] >= n || seen[(size_t)rank[k]]) return -1;
+        seen[(size_t)rank[k]] = 1;
+    }
+    M.kf_rank.assign(rank, rank + n);
+    M.kf_region = static_cast<char *>(M.alloc(sizeof(KeyFrame) * (size_t)n));
+    return 0;
+}
+
 // KeyFrame(Frame&, Map*, KeyFrameDatabase*) from a Frame of n features without map points, identity pose
 int ref_cv_add_keyframe(void *h, int n) {
     CvMap &M = *static_cast<CvMap *>(h);
@@ -91,7 +112,13 @@ int ref_cv_add_keyframe(void *h, int n) {
     F.mvLevelSigma2.assign(1, 1.0f);
     F.mvInvLevelSigma2.assign(1, 1.0f);
     F.mTcw = cv::Mat::eye(4, 4, CV_32F);
-    KeyFrame *kf = new (M.alloc(sizeof(KeyFrame))) KeyFrame(F, &M.map, &M.db);
+    const size_t k = M.kfs.size();
+    if (M.kf_region && k >= M.kf_rank.size()) {
+        std::fprintf(stderr, "ref_covis: keyframe %zu has no place in the order of ref_cv_set_kf_order\n", k);
+        std::abort();
+    }
+    void *at = M.kf_region ? M.kf_region + (size_t)M.kf_rank[k] * sizeof(KeyFrame) : M.alloc(sizeof(KeyFrame));
+    KeyFrame *kf = new (at) KeyFrame(F, &M.map, &M.db);
     M.kf_index[kf] = (int)M.kfs.size();
     M.kfs.push_back(kf);
     return (int)M.kfs.size() - 1;

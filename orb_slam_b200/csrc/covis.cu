@@ -66,11 +66,13 @@ static __host__ __device__ int pow2ge(int n) {
     return p;
 }
 
-// bitonic sort of n2 (a power of two) entries by the whole block: ByWeight = (weight, key) descending, else key ascending
+// bitonic sort of n2 (a power of two) entries by the whole block: ByWeight = (weight, key) descending, else (key, slot)
+// ascending.  Live keys are distinct, so the slot only orders a real entry against padding: every uint64_t is a valid key,
+// ~0ull included, and the network is not stable, so a key-only comparison could let padding take a real entry's place.
 template <bool ByWeight>
 __device__ __forceinline__ bool cv_before(const CvEnt &a, const CvEnt &b) {
     if (ByWeight) return a.w > b.w || (a.w == b.w && a.k > b.k);
-    return a.k < b.k;
+    return a.k < b.k || (a.k == b.k && a.s < b.s);
 }
 template <bool ByWeight>
 __device__ void cv_sort(CvEnt *e, int n2) {
@@ -86,8 +88,8 @@ __device__ void cv_sort(CvEnt *e, int n2) {
             __syncthreads();
         }
 }
-// padding that sorts last in either order
-__device__ __forceinline__ CvEnt cv_pad(bool by_weight) { return by_weight ? CvEnt{0ull, -1, INT_MIN} : CvEnt{~0ull, -1, 0}; }
+// padding that sorts last in either order: by key it is (~0ull, INT_MAX), after a real entry of key ~0ull too
+__device__ __forceinline__ CvEnt cv_pad(bool by_weight) { return by_weight ? CvEnt{0ull, -1, INT_MIN} : CvEnt{~0ull, INT_MAX, 0}; }
 
 // index of `k` in the key-ascending slot row, or -1
 __device__ __forceinline__ int cv_find(const int *row, int n, const unsigned long long *key, unsigned long long k) {
@@ -1282,6 +1284,14 @@ extern "C" int orbfe_covis_add(OrbfeCovisGraph *g, int n, const int32_t *slots, 
     for (int i = 0; i < n; i++)
         if (named[slots[i]] != 0)
             return set_error(ORBFE_ERR_ARG, "orbfe_covis_add: retired slot %d is still named by %d weight maps", slots[i], named[slots[i]]);
+    // nor can its key, which a weight map still holds: an event of the new keyframe would merge onto the stale entry
+    std::unordered_set<unsigned long long> stale_keys;
+    for (int r = 0; r < g->K; r++)
+        if (named[r] != 0 && !g->live[r]) stale_keys.insert(g->keys[r]);
+    for (int i = 0; i < n; i++)
+        if (stale_keys.count(keys[i]))
+            return set_error(ORBFE_ERR_ARG, "orbfe_covis_add: key of slot %d equals the key of a retired slot a weight map still names",
+                             slots[i]);
     std::vector<int> rows(4 * (size_t)n);
     for (int i = 0; i < n; i++) {
         rows[4 * i] = slots[i];

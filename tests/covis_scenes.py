@@ -57,10 +57,11 @@ class Scene:
 
 class Model:
     """The scene's map as the reference holds it: mvpMapPoints per keyframe (point index, -1 = NULL), mObservations per
-    point (dict kf -> feature; the reference's map iterates in kf creation order), isBad per point."""
+    point (dict kf -> feature; the reference's map iterates in key order), isBad per point.  keys[k] is keyframe k's order
+    key (the creation index when None)."""
 
-    def __init__(self, scene: Scene):
-        self.cap = scene.cap
+    def __init__(self, scene: Scene, keys=None):
+        self.cap, self.keys = scene.cap, keys
         self.nfeat = []
         self.kf_mp = np.zeros((0, scene.cap), np.int32)
         self.obs = []
@@ -102,6 +103,10 @@ class Model:
             self.kf_bad[kf] = True
         else:
             self.version -= 1
+
+    def key(self, k):
+        """keyframe k's order key: mObservations, like every map keyed by KeyFrame*, iterates in this order"""
+        return int(k) if self.keys is None else int(self.keys[k])
 
     def _point_bad(self, m):
         self.bad[m] = True
@@ -295,9 +300,22 @@ def scene_culling():
     return s
 
 
+def scene_three_events():
+    """a hub updated first in a batch, then three keyframes that each share 15 or more points with it: the hub's counter
+    holds 3 entries and its map receives 3 events in the batch, the last from the newest keyframe (sorted with one padding
+    entry, whatever the newest keyframe's key)"""
+    s = Scene("three_events", 64, seed=14)
+    hub, a, b, c = s.kf(), s.kf(), s.kf(), s.kf()
+    f = [0] * 4
+    for other, n in ((a, 15), (b, 17), (c, 16)):
+        f[hub], f[other] = _share(s, hub, other, n, f[hub], f[other])
+    s.update([hub, a, b, c])
+    return s
+
+
 def small_scenes():
     return [scene_initial_pair(), scene_local_mapping(), scene_threshold(), scene_tied_max(), scene_weight_ties(),
-            scene_changed_unchanged(), scene_empty_and_duplicates(), scene_batch30(), scene_culling()]
+            scene_changed_unchanged(), scene_empty_and_duplicates(), scene_batch30(), scene_culling(), scene_three_events()]
 
 
 def scene_large(nkf=2000, nfeat=2000, obs_per_point=8, window=12, batch=64, seed=11):

@@ -56,8 +56,8 @@ class CullScene(OS.ObsScene):
 class CullModel(OS.ObsModel):
     """ObsModel plus every keyframe's octaves."""
 
-    def __init__(self, scene):
-        super().__init__(scene)
+    def __init__(self, scene, keys=None):
+        super().__init__(scene, keys)
         self.oct = np.zeros((0, scene.cap), np.int32)
 
     def apply(self, step, erased=()):

@@ -45,8 +45,8 @@ class ObsScene(S.Scene):
 class ObsModel(S.Model):
     """Model plus mpRefKF per point (-2 where the reference's pointer is undefined) and the observer flag per keyframe."""
 
-    def __init__(self, scene):
-        super().__init__(scene)
+    def __init__(self, scene, keys=None):
+        super().__init__(scene, keys)
         self.ref = []
         self.observer = []
         self.divergent = set()   # the old and new point of a row overwrite: mObservations and the rows disagree on them
@@ -115,7 +115,7 @@ class ObsModel(S.Model):
             return
         del self.obs[m][kf]
         if self.ref[m] == kf:
-            self.ref[m] = min(self.obs[m]) if self.obs[m] else -2
+            self.ref[m] = min(self.obs[m], key=self.key) if self.obs[m] else -2   # mObservations.begin()->first
         if len(self.obs[m]) <= 2:
             self._point_bad(m)
 

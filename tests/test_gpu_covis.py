@@ -12,6 +12,7 @@ import orb_slam_b200 as fe
 from oracle.covis import CovisOracle
 from orb_slam_b200 import bow as B
 
+import covis_key_scenes as KM
 import covis_scenes as S
 
 pytestmark = pytest.mark.gpu
@@ -64,13 +65,14 @@ def oracle_state(orc, K):
 
 
 class Run:
-    """A scene on the device graph (batches as given, or cut into batches of one) and on the oracle."""
+    """A scene on the device graph (batches as given, or cut into batches of one) and on the oracle.  keys[k] is keyframe
+    k's order key (the creation index when None)."""
 
-    def __init__(self, scene, single=False, max_batch=64, max_connections=None):
-        self.scene, self.single = scene, single
+    def __init__(self, scene, single=False, max_batch=64, max_connections=None, keys=None):
+        self.scene, self.single, self.keys = scene, single, keys
         self.K = scene.nkf
         self.slot_of = scene.slots()
-        self.model = S.Model(scene)
+        self.model = S.Model(scene, keys)
         self.g = B.CovisibilityGraph(self.K, max_connections or scene.max_connections, max_batch)
         self.orc = CovisOracle(self.K)
         self._dv = None
@@ -101,8 +103,8 @@ class Run:
         if op == "kf":
             k = len(self.model.nfeat) - 1
             s = int(self.slot_of[k])
-            self.g.add([s], [k], [k])
-            self.orc.add(s, k, k)
+            self.g.add([s], [k], [KM.key_of(self.keys, k)])
+            self.orc.add(s, k, KM.key_of(self.keys, k))
         elif op == "update":
             slots = [int(self.slot_of[k]) for k in step[1]]
             _, (kf_mp, counts, gp, obs) = self.inputs()

@@ -14,6 +14,7 @@ from oracle import kf_culling as KC
 from oracle import observations as OO
 from oracle.covis import CovisOracle
 
+import covis_key_scenes as KM
 import covis_scenes as S
 import kf_culling_scenes as KS
 from test_oracle_kf_culling import cull_inputs
@@ -46,12 +47,12 @@ def _kps(octave):
 
 class Run:
     """A scene on the device graph and the oracle graph (keyframes added when they become observers), on the model, and
-    the culls on both."""
+    the culls on both.  keys[k] is keyframe k's order key (the creation index when None)."""
 
-    def __init__(self, scene):
-        self.scene, self.K, self.cap = scene, scene.nkf, scene.cap
+    def __init__(self, scene, keys=None):
+        self.scene, self.K, self.cap, self.keys = scene, scene.nkf, scene.cap, keys
         self.slot_of = scene.slots()
-        self.model = KS.CullModel(scene)
+        self.model = KS.CullModel(scene, keys)
         self.g = B.CovisibilityGraph(self.K, scene.max_connections, 64)
         self.orc = CovisOracle(self.K)
 
@@ -61,8 +62,8 @@ class Run:
 
     def add(self, k):
         s = int(self.slot_of[k])
-        self.g.add([s], [k], [k])
-        self.orc.add(s, k, k)
+        self.g.add([s], [k], [KM.key_of(self.keys, k)])
+        self.orc.add(s, k, KM.key_of(self.keys, k))
 
     def erase(self, s):
         self.g.erase(s)
@@ -88,7 +89,7 @@ class Run:
             self.g.sync()
 
     def oracle(self, cur, not_erase=(), a=None, obs_cap=None):
-        a = cull_inputs(self.model, self.slot_of, self.K, not_erase) if a is None else a
+        a = cull_inputs(self.model, self.slot_of, self.K, not_erase, self.keys) if a is None else a
         cand = np.array(self.orc.ordered(int(self.slot_of[cur]))[0], np.int32)
         return KC.cull(cand, a["live"], a["id0"], a["keys"], a["not_erase"], a["kf_mp"], a["counts"], a["octave"], self.cap,
                        a["point_bad"], a["ref_slot"], obs_cap=obs_cap), a
@@ -98,7 +99,7 @@ class Run:
         buffers and the scratch given, nothing is allocated and the device is not synchronised before the call, so the call
         is enqueued right behind whatever the caller enqueued last"""
         torch, dev = _torch()
-        a = cull_inputs(self.model, self.slot_of, self.K, not_erase) if a is None else a
+        a = cull_inputs(self.model, self.slot_of, self.K, not_erase, self.keys) if a is None else a
         npts = len(a["point_bad"])
         if obs_cap is None:
             obs_cap = int(np.count_nonzero(a["kf_mp"] >= 0))
@@ -139,10 +140,10 @@ class Run:
         return o, got
 
 
-def _play(scene, check_all=True):
+def _play(scene, check_all=True, keys=None):
     """every step on the device and the oracle; after each step keyframe 1 (the scenes' current keyframe) is culled on both
     without applying it, and a cull step applies the oracle's erases to the model and the graphs"""
-    r = Run(scene)
+    r = Run(scene, keys)
     try:
         for t, step in enumerate(scene.steps):
             where = (scene.name, t, step[0])

@@ -37,15 +37,15 @@ def _past_counts(a, cap):
 class Run(CullRun):
     """a scene on the device graph, the oracle graph and the model, with local-map calls on both"""
 
-    def __init__(self, scene):
-        super().__init__(scene)
-        self.model = LS.LmModel(scene)
+    def __init__(self, scene, keys=None):
+        super().__init__(scene, keys)
+        self.model = LS.LmModel(scene, keys)
 
     def lists(self):
         return {s: self.orc.ordered(s)[0] for s in range(self.K)}
 
     def oracle(self, cells, a=None):
-        a = _past_counts(lm_inputs(self.model, self.slot_of, self.K), self.cap) if a is None else a
+        a = _past_counts(lm_inputs(self.model, self.slot_of, self.K, self.keys), self.cap) if a is None else a
         nb, nnb = LM.neighbours(self.lists(), self.K)
         return LM.local_map(cells, a["point_bad"], a["kf_mp"], a["counts"], self.cap, a["live"], a["keys"], nb, nnb), a
 
@@ -91,8 +91,8 @@ def compare(got, o, nf, where, tails=True):
     assert not tails or (got["lp"][nlp:] == FILL).all(), where
 
 
-def _play(scene, check_all=True):
-    r = Run(scene)
+def _play(scene, check_all=True, keys=None):
+    r = Run(scene, keys)
     try:
         for t, step in enumerate(scene.steps):
             where = (scene.name, t, step[0])

@@ -13,6 +13,7 @@ import orb_slam_b200 as fe
 from orb_slam_b200 import bow as B
 from oracle import observations as OO
 
+import covis_key_scenes as KM
 import covis_scenes as S
 import observation_scenes as OS
 from test_oracle_observations import oracle_inputs
@@ -39,12 +40,12 @@ def _full(n, v=FILL):
 
 class Run:
     """A scene on the device graph (a keyframe is added when it becomes an observer, erased with KeyFrame::SetBadFlag) and
-    on the model the oracle reads."""
+    on the model the oracle reads.  keys[k] is keyframe k's order key (the creation index when None)."""
 
-    def __init__(self, scene):
-        self.scene, self.K, self.cap = scene, scene.nkf, scene.cap
+    def __init__(self, scene, keys=None):
+        self.scene, self.K, self.cap, self.keys = scene, scene.nkf, scene.cap, keys
         self.slot_of = scene.slots()
-        self.model = OS.ObsModel(scene)
+        self.model = OS.ObsModel(scene, keys)
         self.g = B.CovisibilityGraph(self.K, scene.max_connections, 64)
         self._dv = None
 
@@ -56,12 +57,12 @@ class Run:
         op = step[0]
         if op == "kf" or op == "process":
             k = len(self.model.nfeat) - 1 if op == "kf" else step[1]
-            self.g.add([int(self.slot_of[k])], [k], [k])
+            self.g.add([int(self.slot_of[k])], [k], [KM.key_of(self.keys, k)])
         elif op == "erase_kf":
             self.g.erase(int(self.slot_of[step[1]]))
 
     def inputs(self):
-        kf_mp, counts, gp, obs, live, keys, ref_slot = oracle_inputs(self.model, self.slot_of, self.K)
+        kf_mp, counts, gp, obs, live, keys, ref_slot = oracle_inputs(self.model, self.slot_of, self.K, self.keys)
         if self._dv is None or self._dv[0] != self.model.version:
             self._dv = (self.model.version, _dev(kf_mp), _dev(counts))
         return (kf_mp, counts, gp, obs, live, keys, ref_slot), self._dv[1:]

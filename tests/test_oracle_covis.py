@@ -5,6 +5,7 @@ holds."""
 import numpy as np
 import pytest
 
+import covis_key_scenes as KM
 import covis_scenes as S
 from oracle import covis as OC
 
@@ -33,18 +34,23 @@ def _check_inputs(ref, model, scene, nkf):
     for mp in range(len(model.obs)):
         ks, ix = ref.observations(mp)
         o = model.obs[mp]
-        assert ks == sorted(o) and ix == [o[k] for k in sorted(o)], ("observations", mp)
+        order = sorted(o, key=model.key)
+        assert ks == order and ix == [o[k] for k in order], ("observations", mp)
         assert ref.point_bad(mp) == bool(model.bad[mp])
 
 
-def run(scene, full=True):
+def run(scene, full=True, keys=None, trace=None):
     """Replays the scene on the reference, the model and the oracle; compares after every step (every keyframe when
-    `full`, else the keyframes the step can change)."""
-    ref, model, slot_of = OC.RefCovis(), S.Model(scene), scene.slots()
+    `full`, else the keyframes the step can change).  keys[k] is keyframe k's order key (the creation index when None; the
+    reference's keyframes are laid out in key order).  With `trace`, the oracle's graph (ordered list, weight map and parent
+    of every slot) is appended to it after every step."""
+    ref, model, slot_of = OC.RefCovis(), S.Model(scene, keys), scene.slots()
     K = max(scene.nkf, 1)
     orc = OC.CovisOracle(K)
     nkf = 0
     try:
+        if keys is not None:
+            ref.set_kf_order(KM.rank(keys[:scene.nkf]))
         for t, step in enumerate(scene.steps):
             op = step[0]
             model.apply(step)
@@ -52,7 +58,7 @@ def run(scene, full=True):
             if op == "kf":
                 k = ref.add_keyframe(step[1])
                 assert k == nkf and ref.mnid(k) == k
-                orc.add(slot_of[k], k, k)
+                orc.add(slot_of[k], k, KM.key_of(keys, k))
                 nkf += 1
             elif op == "pts":
                 ref.add_points(step[1])
@@ -77,6 +83,8 @@ def run(scene, full=True):
             _compare(ref, orc, slot_of, range(nkf) if full else sorted(set(touched)), (scene.name, t, op))
             if full:
                 _check_inputs(ref, model, scene, nkf)
+            if trace is not None:
+                trace.append([(orc.ordered(s), orc.weights(s), orc.parent(s)) for s in range(K)])
         _compare(ref, orc, slot_of, range(nkf), (scene.name, "end"))
         return ref, orc, slot_of
     finally:

@@ -8,6 +8,7 @@ oracle's statuses."""
 import numpy as np
 import pytest
 
+import covis_key_scenes as KM
 import covis_scenes as S
 import kf_culling_scenes as KS
 from oracle import kf_culling as KC
@@ -16,26 +17,26 @@ from test_oracle_observations import ref_step as obs_ref_step
 needs_ref = pytest.mark.skipif(not KC.ref_available(), reason="oracle/_ref/libref_kf_culling.so not built (needs the reference sources)")
 
 
-def cull_inputs(model, slot_of, K, not_erase=()):
-    """the oracle's (and the device's) per-slot arrays from the model: rows (bad points -1), counts, live, mnId == 0, keys,
-    mbNotErase, octaves, point flags and reference slots"""
+def cull_inputs(model, slot_of, K, not_erase=(), keys=None):
+    """the oracle's (and the device's) per-slot arrays from the model: rows (bad points -1), counts, live, mnId == 0, keys
+    (keys[k] for keyframe k; the creation index when None), mbNotErase, octaves, point flags and reference slots"""
     cap, n = model.cap, len(model.nfeat)
     kf_mp, counts, _, _ = model.inputs(slot_of, K)
     live, id0, ne = np.zeros(K, np.uint8), np.zeros(K, np.uint8), np.zeros(K, np.uint8)
-    keys = np.zeros(K, np.uint64)
+    key_slot = np.zeros(K, np.uint64)
     live[slot_of[:n]] = model.live()
     id0[slot_of[:n]] = [m == 0 for m in model.mnid]
-    keys[slot_of[:n]] = np.arange(n, dtype=np.uint64)
+    key_slot[slot_of[:n]] = KM.key_list(keys, n)
     ne[[int(slot_of[k]) for k in not_erase]] = 1
     octave = np.zeros((K, cap), np.int32)
     octave[slot_of[:n]] = model.oct
     ref_slot = np.array([slot_of[r] if r >= 0 else 0 for r in model.ref], np.int32)
-    return dict(kf_mp=kf_mp, counts=counts, live=live, id0=id0, keys=keys, not_erase=ne, octave=octave.ravel(),
+    return dict(kf_mp=kf_mp, counts=counts, live=live, id0=id0, keys=key_slot, not_erase=ne, octave=octave.ravel(),
                 point_bad=model.bad.astype(np.uint8), ref_slot=ref_slot)
 
 
-def oracle_cull(model, slot_of, K, cand_slots, not_erase=(), obs_cap=None):
-    a = cull_inputs(model, slot_of, K, not_erase)
+def oracle_cull(model, slot_of, K, cand_slots, not_erase=(), obs_cap=None, keys=None):
+    a = cull_inputs(model, slot_of, K, not_erase, keys)
     return KC.cull(cand_slots, a["live"], a["id0"], a["keys"], a["not_erase"], a["kf_mp"], a["counts"], a["octave"], model.cap,
                    a["point_bad"], a["ref_slot"], obs_cap=obs_cap), a
 
@@ -56,15 +57,19 @@ def compare_map(ref, model, where, points=None):
     for m in (range(len(model.obs)) if points is None else points):
         assert ref.point_bad(m) == bool(model.bad[m]), (where, "isBad", m)
         ks, ix = ref.observations(m)
-        assert list(zip(ks, ix)) == sorted(model.obs[m].items()), (where, "observations", m)
+        assert list(zip(ks, ix)) == sorted(model.obs[m].items(), key=lambda e: model.key(e[0])), (where, "observations", m)
         if not model.bad[m]:
             assert ref.reference(m) == model.ref[m], (where, "mpRefKF", m)
 
 
-def run(scene, check_every=True):
-    ref, model, slot_of = KC.RefKfCulling(), KS.CullModel(scene), scene.slots()
+def run(scene, check_every=True, keys=None, trace=None):
+    """keys[k] is keyframe k's order key (the creation index when None); with `trace`, every cull's oracle result is
+    appended to it"""
+    ref, model, slot_of = KC.RefKfCulling(), KS.CullModel(scene, keys), scene.slots()
     K = scene.nkf
     try:
+        if keys is not None:
+            ref.set_kf_order(KM.rank(keys[:scene.nkf]))
         for t, step in enumerate(scene.steps):
             where = (scene.name, t, step[0])
             op = step[0]
@@ -82,8 +87,10 @@ def run(scene, check_every=True):
             for k in ne:
                 ref.set_not_erase(k)
             ids = ref.ordered(cur)[0]
-            out, _ = oracle_cull(model, slot_of, K, slot_of[ids], ne)
+            out, _ = oracle_cull(model, slot_of, K, slot_of[ids], ne, keys=keys)
             assert out["status"] == 0, where
+            if trace is not None:
+                trace.append({k: (v.tolist() if hasattr(v, "tolist") else v) for k, v in out.items()})
             rids, verdicts, _ = ref.cull(cur)
             assert rids == ids, where
             assert out["verdict_slot"].tolist() == slot_of[ids].tolist(), where

@@ -6,6 +6,7 @@ the case it is built for, and the oracle's statuses."""
 import numpy as np
 import pytest
 
+import covis_key_scenes as KM
 import covis_scenes as S
 import local_map_scenes as LS
 from oracle import local_map as LM
@@ -14,18 +15,18 @@ from test_oracle_observations import ref_step as obs_ref_step
 needs_ref = pytest.mark.skipif(not LM.ref_available(), reason="oracle/_ref/libref_local_map.so not built (needs the reference sources)")
 
 
-def lm_inputs(model, slot_of, K):
+def lm_inputs(model, slot_of, K, keys=None):
     """the oracle's (and the device's) per-slot arrays from the model: the rows as the keyframes hold them, counts, live,
-    keys (creation index) and point flags"""
+    keys (keys[k] for keyframe k; the creation index when None) and point flags"""
     cap, n = model.cap, len(model.nfeat)
     kf_mp = np.full((K, cap), -1, np.int32)
     counts = np.zeros(K, np.int32)
     kf_mp[slot_of[:n]] = model.kf_mp
     counts[slot_of[:n]] = model.nfeat
-    live, keys = np.zeros(K, np.uint8), np.zeros(K, np.uint64)
+    live, key_slot = np.zeros(K, np.uint8), np.zeros(K, np.uint64)
     live[slot_of[:n]] = model.live()
-    keys[slot_of[:n]] = np.arange(n, dtype=np.uint64)
-    return dict(kf_mp=kf_mp.ravel(), counts=counts, live=live, keys=keys, point_bad=model.bad.astype(np.uint8))
+    key_slot[slot_of[:n]] = KM.key_list(keys, n)
+    return dict(kf_mp=kf_mp.ravel(), counts=counts, live=live, keys=key_slot, point_bad=model.bad.astype(np.uint8))
 
 
 def oracle_local_map(a, cells, lists, K, cap):
@@ -36,9 +37,13 @@ def oracle_local_map(a, cells, lists, K, cap):
 class RefRun:
     """a scene on the reference's own map and on the model"""
 
-    def __init__(self, scene):
-        self.scene, self.K, self.cap = scene, scene.nkf, scene.cap
-        self.ref, self.model, self.slot_of = LM.RefLocalMap(), LS.LmModel(scene), scene.slots()
+    def __init__(self, scene, keys=None):
+        """keys[k] is keyframe k's order key (the creation index when None)"""
+        self.scene, self.K, self.cap, self.keys = scene, scene.nkf, scene.cap, keys
+        self.ref, self.model, self.slot_of = LM.RefLocalMap(), LS.LmModel(scene, keys), scene.slots()
+        self.trace = []
+        if keys is not None:
+            self.ref.set_kf_order(KM.rank(keys[:scene.nkf]))
 
     def close(self):
         self.ref.close()
@@ -59,7 +64,8 @@ class RefRun:
         """the reference and the oracle on one frame; returns the reference's (cells, local keyframes, reference keyframe,
         local points) by creation index"""
         so = self.slot_of
-        o = oracle_local_map(lm_inputs(self.model, so, self.K), cells, self.lists(), self.K, self.cap)
+        o = oracle_local_map(lm_inputs(self.model, so, self.K, self.keys), cells, self.lists(), self.K, self.cap)
+        self.trace.append({k: (v.tolist() if hasattr(v, "tolist") else v) for k, v in o.items()})
         fm, lk, rk, lp, _ = self.ref.update_reference(cells)
         assert o["status"] == 0, where
         assert o["frame_mp"].tolist() == fm.tolist(), (where, "frame cells")
@@ -69,8 +75,9 @@ class RefRun:
         return fm.tolist(), lk, rk, lp
 
 
-def run(scene, check_every=True):
-    r = RefRun(scene)
+def run(scene, check_every=True, keys=None, trace=None):
+    """with `trace`, every comparison's oracle result is appended to it"""
+    r = RefRun(scene, keys)
     got = []
     try:
         for t, step in enumerate(scene.steps):
@@ -80,6 +87,8 @@ def run(scene, check_every=True):
                 got.append(r.compare(step[1], where))
             elif check_every:
                 r.compare(LS.probe_frame(r.model), where + ("probe",))
+        if trace is not None:
+            trace += r.trace
         return got
     finally:
         r.close()

@@ -6,6 +6,7 @@ cell without a reference path differs from the reference exactly as DESIGN.md §
 import numpy as np
 import pytest
 
+import covis_key_scenes as KM
 import covis_scenes as S
 import observation_scenes as OS
 from oracle import observations as OO
@@ -13,16 +14,17 @@ from oracle import observations as OO
 needs_ref = pytest.mark.skipif(not OO.ref_available(), reason="oracle/_ref/libref_drivers.so not built (needs the reference sources)")
 
 
-def oracle_inputs(model, slot_of, K):
-    """kf_mp / counts in slot rows (Model.inputs), live and keys per slot (key = creation index), ref slot per point"""
+def oracle_inputs(model, slot_of, K, keys=None):
+    """kf_mp / counts in slot rows (Model.inputs), live and keys per slot (keys[k] for keyframe k; the creation index when
+    None), ref slot per point"""
     kf_mp, counts, gp, obs = model.inputs(slot_of, K)
     n = len(model.nfeat)
-    live, keys = np.zeros(K, np.uint8), np.zeros(K, np.uint64)
+    live, key_slot = np.zeros(K, np.uint8), np.zeros(K, np.uint64)
     live[slot_of[:n]] = model.live() if isinstance(model, OS.ObsModel) else ~np.array(model.kf_bad, bool)
-    keys[slot_of[:n]] = np.arange(n, dtype=np.uint64)
+    key_slot[slot_of[:n]] = KM.key_list(keys, n)
     ref = getattr(model, "ref", None)
     ref_slot = np.array([slot_of[r] if r >= 0 else 0 for r in ref], np.int32) if ref is not None else None
-    return kf_mp, counts, gp, obs, live, keys, ref_slot
+    return kf_mp, counts, gp, obs, live, key_slot, ref_slot
 
 
 def ref_step(ref, model, step):
@@ -56,10 +58,10 @@ def ref_step(ref, model, step):
         ref.ba_erase(step[1], step[2])
 
 
-def compare(ref, model, scene, slot_of, points, where):
+def compare(ref, model, scene, slot_of, points, where, keys=None):
     K, cap = scene.nkf, scene.cap
-    kf_mp, counts, gp, obs, live, keys, ref_slot = oracle_inputs(model, slot_of, K)
-    rc, ptr, got, nobs, ref_obs = OO.observations(points, len(model.obs), kf_mp, counts, cap, live, keys, ref_slot)
+    kf_mp, counts, gp, obs, live, key_slot, ref_slot = oracle_inputs(model, slot_of, K, keys)
+    rc, ptr, got, nobs, ref_obs = OO.observations(points, len(model.obs), kf_mp, counts, cap, live, key_slot, ref_slot)
     assert rc == 0, where
     div = getattr(model, "divergent", set())
     for j, m in enumerate(points):
@@ -74,17 +76,23 @@ def compare(ref, model, scene, slot_of, points, where):
             assert r == model.ref[m], (where, "mpRefKF", m)
             o = dict(zip(ks, ix))
             assert ref_obs[j] == int(slot_of[r]) * cap + o.get(r, 0), (where, "ref_obs", m)
-    return ptr, got
+    return ptr, got, ref_obs
 
 
-def run(scene, model_cls=OS.ObsModel, every=True):
-    ref, model, slot_of = OO.RefObservations(), model_cls(scene), scene.slots()
+def run(scene, model_cls=OS.ObsModel, every=True, keys=None, trace=None):
+    """keys[k] is keyframe k's order key (the creation index when None); with `trace`, every comparison's oracle lists and
+    ref_obs are appended to it"""
+    ref, model, slot_of = OO.RefObservations(), model_cls(scene, keys), scene.slots()
     try:
+        if keys is not None:
+            ref.set_kf_order(KM.rank(keys[:scene.nkf]))
         for t, step in enumerate(scene.steps):
             model.apply(step)
             ref_step(ref, model, step)
             if every or step[0] != "update":
-                compare(ref, model, scene, slot_of, list(range(len(model.obs))), (scene.name, t, step[0]))
+                out = compare(ref, model, scene, slot_of, list(range(len(model.obs))), (scene.name, t, step[0]), keys)
+                if trace is not None:
+                    trace.append([None if x is None else x.tolist() for x in out])
         return model
     finally:
         ref.close()
