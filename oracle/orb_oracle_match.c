@@ -713,6 +713,10 @@ void orb_oracle_guided_best(const OrbOracleFrame *f, int nq, const float *qu, co
  * mDistCoef, cv::Mat(), mK) = OpenCV's cvUndistortPoints with R = I, P = K: 5 fixed-point iterations of the inverse
  * distortion model in double, then the re-projection with P.  Pinned bit-exactly against python-cv2
  * (tests/golden/opencv_undistort.npz).  dist = (k1, k2, p1, p2, k3); k4..k6 = 0 as in the reference's settings.
+ * These are OpenCV 2.4's semantics: the five iterations always run.  OpenCV 4.x stops at the first iteration whose
+ * denominator 1 + k1 r^2 + k2 r^4 + k3 r^6 is below 0 and returns the distorted point; the two agree on every point where no
+ * iteration meets such a denominator and differ on most points where one does (strong barrel distortion near the image
+ * corners: tests/golden/opencv_undistort_models.npz, test_oracle_camera_domain.py).
  * ------------------------------------------------------------------------------------------------ */
 void orb_oracle_undistort_points(const float *pts, int n, float fx, float fy, float cx, float cy, const float *dist, float *out) {
     const double k0 = dist[0], k1 = dist[1], k2 = dist[2], k3 = dist[3], k4 = dist[4];
@@ -752,16 +756,24 @@ void orb_oracle_undistort_keypoints(const OrbOracleKeyPoint *in, int n, float fx
     }
 }
 
+/* std::min / std::max as Frame.cc:336-339 calls them: (b < a) ? b : a and (a < b) ? b : a.  Unlike fminf / fmaxf they keep a
+ * NaN first argument (a corner whose undistortion meets a zero denominator) and drop a NaN second one. */
+static float std_min(float a, float b) { return (b < a) ? b : a; }
+static float std_max(float a, float b) { return (a < b) ? b : a; }
+/* Frame's bounds are `static int` (Frame.h:121-124): the float is converted as x86-64 does, NaN and values outside
+ * [-2^31, 2^31) becoming INT_MIN */
+static float frame_int(float f) { return (f >= -2147483648.0f && f < 2147483648.0f) ? (float)(int)f : -2147483648.0f; }
+
 /* ComputeImageBounds, Frame.cc:321-350: bounds = (mnMinX, mnMinY, mnMaxX, mnMaxY) */
 void orb_oracle_image_bounds(int cols, int rows, float fx, float fy, float cx, float cy, const float *dist, float *bounds) {
     if (dist[0] != 0.0f) {
         const float c[8] = {0.f, 0.f, (float)cols, 0.f, 0.f, (float)rows, (float)cols, (float)rows};
         float u[8];
         orb_oracle_undistort_points(c, 4, fx, fy, cx, cy, dist, u);
-        bounds[0] = fminf(floorf(u[0]), floorf(u[4]));
-        bounds[2] = fmaxf(ceilf(u[2]), ceilf(u[6]));
-        bounds[1] = fminf(floorf(u[1]), floorf(u[3]));
-        bounds[3] = fmaxf(ceilf(u[5]), ceilf(u[7]));
+        bounds[0] = frame_int(std_min(floorf(u[0]), floorf(u[4])));
+        bounds[2] = frame_int(std_max(ceilf(u[2]), ceilf(u[6])));
+        bounds[1] = frame_int(std_min(floorf(u[1]), floorf(u[3])));
+        bounds[3] = frame_int(std_max(ceilf(u[5]), ceilf(u[7])));
     } else {
         bounds[0] = 0; bounds[2] = (float)cols; bounds[1] = 0; bounds[3] = (float)rows;
     }

@@ -184,18 +184,25 @@ struct SbpQuery {
     bool ok;
 };
 
+// `int nMinCellX = floor(...)` and its three siblings (Frame.cc:205-223) convert a float to int the x86-64 way (cvttss2si):
+// NaN and every value outside [-2^31, 2^31) give INT_MIN, so a window with a NaN or infinite centre or radius, or one reaching
+// 2^31 cells, is empty.  The device's conversion saturates and turns NaN into 0, which would scan cell 0 or the whole grid.
+__device__ __forceinline__ int cell_bound(float f) {
+    return (f >= -2147483648.0f && f < 2147483648.0f) ? (int)f : (int)0x80000000u;
+}
+
 // cell range of Frame::GetFeaturesInArea (Frame.cc:205-223); false if the window misses the grid
 __device__ __forceinline__ bool sbp_cell_range(const SbpParams &P, SbpQuery &q) {
-    int x0 = (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(q.u, P.min_x), q.r), P.gw));
+    int x0 = cell_bound(floorf(__fmul_rn(__fsub_rn(__fsub_rn(q.u, P.min_x), q.r), P.gw)));
     x0 = max(0, x0);
     if (x0 >= SBP_GCOLS) return false;
-    int x1 = (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(q.u, P.min_x), q.r), P.gw));
+    int x1 = cell_bound(ceilf(__fmul_rn(__fadd_rn(__fsub_rn(q.u, P.min_x), q.r), P.gw)));
     x1 = min(SBP_GCOLS - 1, x1);
     if (x1 < 0) return false;
-    int y0 = (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(q.v, P.min_y), q.r), P.gh));
+    int y0 = cell_bound(floorf(__fmul_rn(__fsub_rn(__fsub_rn(q.v, P.min_y), q.r), P.gh)));
     y0 = max(0, y0);
     if (y0 >= SBP_GROWS) return false;
-    int y1 = (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(q.v, P.min_y), q.r), P.gh));
+    int y1 = cell_bound(ceilf(__fmul_rn(__fadd_rn(__fsub_rn(q.v, P.min_y), q.r), P.gh)));
     y1 = min(SBP_GROWS - 1, y1);
     if (y1 < 0) return false;
     q.x0 = x0; q.x1 = x1; q.y0 = y0; q.y1 = y1;

@@ -1368,10 +1368,13 @@ extern "C" int orbfe_image_bounds(OrbfeMatcher *m, int cols, int rows, float fx,
     c[1].x = (float)cols; c[2].y = (float)rows; c[3].x = (float)cols; c[3].y = (float)rows;   // Frame.cc:325-329
     const int rc = orbfe_undistort_keypoints(m, c, c, 4, fx, fy, cx, cy, dist5);
     if (rc) return rc;
-    bounds4[0] = std::min(std::floor(c[0].x), std::floor(c[2].x));   // :336-339
-    bounds4[2] = std::max(std::ceil(c[1].x), std::ceil(c[3].x));
-    bounds4[1] = std::min(std::floor(c[0].y), std::floor(c[1].y));
-    bounds4[3] = std::max(std::ceil(c[2].y), std::ceil(c[3].y));
+    // Frame's bounds are `static int` (Frame.h:121-124), converted as x86-64 does: NaN (a corner whose undistortion meets a zero
+    // denominator) and values outside [-2^31, 2^31) become INT_MIN
+    auto frame_int = [](float f) { return (f >= -2147483648.0f && f < 2147483648.0f) ? (float)(int)f : -2147483648.0f; };
+    bounds4[0] = frame_int(std::min(std::floor(c[0].x), std::floor(c[2].x)));   // :336-339
+    bounds4[2] = frame_int(std::max(std::ceil(c[1].x), std::ceil(c[3].x)));
+    bounds4[1] = frame_int(std::min(std::floor(c[0].y), std::floor(c[1].y)));
+    bounds4[3] = frame_int(std::max(std::ceil(c[2].y), std::ceil(c[3].y)));
     return ORBFE_OK;
 }
 
