@@ -14,7 +14,7 @@ def _same(gk, gd, ok, od):
     assert len(gk) == len(ok)
     for name in ("x", "y", "size", "response", "octave", "class_id"):
         assert np.array_equal(gk[name], ok[name]), name
-    assert np.max(np.abs(gk["angle"] - ok["angle"]), initial=0.0) <= 1e-4
+    assert np.array_equal(gk["angle"].view(np.uint32), ok["angle"].view(np.uint32))
     assert np.array_equal(gd, od)
 
 

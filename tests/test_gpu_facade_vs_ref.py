@@ -78,12 +78,12 @@ def test_extractor_facade_against_the_reference_sources(gpu_required):
     rc, ok, od, _ = O.extract(O.make_params(1000, 1.2, 8, 1, 20), img)     # the facade == the oracle's canonical mode, bit for bit
     for f in ("x", "y", "size", "response", "octave", "class_id"):
         assert np.array_equal(fk[f], ok[f]), f
-    assert np.max(np.abs(fk["angle"] - ok["angle"])) <= 1e-4 and np.array_equal(fd, od)
+    assert np.array_equal(fk["angle"].view(np.uint32), ok["angle"].view(np.uint32)) and np.array_equal(fd, od)
     key = lambda k: list(zip(k["octave"].tolist(), k["x"].tolist(), k["y"].tolist()))
     rmap = {kk: i for i, kk in enumerate(key(rk))}
     common = [(rmap[kk], j) for j, kk in enumerate(key(fk)) if kk in rmap]
     assert len(common) >= 970
     for i, j in common:
-        assert np.array_equal(rd[i], fd[j]) and abs(rk["angle"][i] - fk["angle"][j]) <= 1e-4 and rk["response"][i] == fk["response"][j]
+        assert np.array_equal(rd[i], fd[j]) and rk["angle"][i].view(np.uint32) == fk["angle"][j].view(np.uint32) and rk["response"][i] == fk["response"][j]
     for l in range(8):
         assert np.array_equal(np.sort(rk["response"][rk["octave"] == l]), np.sort(fk["response"][fk["octave"] == l]))
