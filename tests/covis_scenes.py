@@ -63,7 +63,7 @@ class Model:
     def __init__(self, scene: Scene, keys=None):
         self.cap, self.keys = scene.cap, keys
         self.nfeat = []
-        self.kf_mp = np.zeros((0, scene.cap), np.int32)
+        self._mp = np.zeros((0, scene.cap), np.int32)   # rows grow by doubling: kf_mp is its first len(nfeat) rows
         self.obs = []
         self.bad = np.zeros(0, bool)
         self.kf_bad = []
@@ -75,8 +75,9 @@ class Model:
         op = step[0]
         self.version += 1
         if op == "kf":
+            if len(self.nfeat) == len(self._mp):
+                self._mp = np.vstack([self._mp, np.full((max(len(self._mp), 1), self.cap), -1, np.int32)])
             self.nfeat.append(step[1])
-            self.kf_mp = np.vstack([self.kf_mp, np.full((1, self.cap), -1, np.int32)])
             self.kf_bad.append(False)
             self.mnid.append(len(self.mnid))
         elif op == "pts":
@@ -103,6 +104,10 @@ class Model:
             self.kf_bad[kf] = True
         else:
             self.version -= 1
+
+    @property
+    def kf_mp(self):
+        return self._mp[:len(self.nfeat)]
 
     def key(self, k):
         """keyframe k's order key: mObservations, like every map keyed by KeyFrame*, iterates in this order"""

@@ -58,12 +58,16 @@ class CullModel(OS.ObsModel):
 
     def __init__(self, scene, keys=None):
         super().__init__(scene, keys)
-        self.oct = np.zeros((0, scene.cap), np.int32)
+        self._oct = np.zeros((0, scene.cap), np.int32)   # rows grow by doubling: oct is its first len(nfeat) rows
+
+    @property
+    def oct(self):
+        return self._oct[:len(self.nfeat)]
 
     def apply(self, step, erased=()):
         op = step[0]
-        if op in ("kf", "kfq"):
-            self.oct = np.vstack([self.oct, np.zeros((1, self.cap), np.int32)])
+        if op in ("kf", "kfq") and len(self.nfeat) == len(self._oct):
+            self._oct = np.vstack([self._oct, np.zeros((max(len(self._oct), 1), self.cap), np.int32)])
         if op == "octave":
             self.oct[step[1], step[2]] = step[3]
             return

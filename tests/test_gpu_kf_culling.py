@@ -49,11 +49,11 @@ class Run:
     """A scene on the device graph and the oracle graph (keyframes added when they become observers), on the model, and
     the culls on both.  keys[k] is keyframe k's order key (the creation index when None)."""
 
-    def __init__(self, scene, keys=None):
+    def __init__(self, scene, keys=None, max_batch=64):
         self.scene, self.K, self.cap, self.keys = scene, scene.nkf, scene.cap, keys
         self.slot_of = scene.slots()
         self.model = KS.CullModel(scene, keys)
-        self.g = B.CovisibilityGraph(self.K, scene.max_connections, 64)
+        self.g = B.CovisibilityGraph(self.K, scene.max_connections, max_batch)
         self.orc = CovisOracle(self.K)
 
     def close(self):
@@ -84,7 +84,7 @@ class Run:
             self.orc.replay(slots, kf_mp, counts, self.cap, gp, obs)
             d = [_dev(kf_mp), _dev(counts), _dev(gp), _dev(obs if len(obs) else [0])]
             for i in range(0, len(slots), self.g.max_batch):
-                self.g.update_connections_device(slots[i:i + 64], d[0].data_ptr(), d[1].data_ptr(), self.K, self.cap, d[2].data_ptr(),
+                self.g.update_connections_device(slots[i:i + self.g.max_batch], d[0].data_ptr(), d[1].data_ptr(), self.K, self.cap, d[2].data_ptr(),
                                                  d[3].data_ptr(), len(gp) - 1, len(obs))
             self.g.sync()
 

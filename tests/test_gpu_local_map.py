@@ -37,8 +37,8 @@ def _past_counts(a, cap):
 class Run(CullRun):
     """a scene on the device graph, the oracle graph and the model, with local-map calls on both"""
 
-    def __init__(self, scene, keys=None):
-        super().__init__(scene, keys)
+    def __init__(self, scene, keys=None, max_batch=64):
+        super().__init__(scene, keys, max_batch)
         self.model = LS.LmModel(scene, keys)
 
     def lists(self):

@@ -42,11 +42,11 @@ class Run:
     """A scene on the device graph (a keyframe is added when it becomes an observer, erased with KeyFrame::SetBadFlag) and
     on the model the oracle reads.  keys[k] is keyframe k's order key (the creation index when None)."""
 
-    def __init__(self, scene, keys=None):
+    def __init__(self, scene, keys=None, max_batch=64):
         self.scene, self.K, self.cap, self.keys = scene, scene.nkf, scene.cap, keys
         self.slot_of = scene.slots()
         self.model = OS.ObsModel(scene, keys)
-        self.g = B.CovisibilityGraph(self.K, scene.max_connections, 64)
+        self.g = B.CovisibilityGraph(self.K, scene.max_connections, max_batch)
         self._dv = None
 
     def close(self):
