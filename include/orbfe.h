@@ -10,7 +10,9 @@
  * the ABI; a handle owns all of its device memory and its CUDA stream; there is NO CPU fallback -- if
  * no CUDA device is usable the create functions fail with ORBFE_ERR_NO_DEVICE.
  * Threading: one in-flight call per extractor handle (the reference's extractor is not re-entrant either,
- * ORBextractor.h:74-75); matcher handles are independent (one per calling thread).
+ * ORBextractor.h:74-75); matcher handles are independent (one per calling thread).  Calls on one handle run in call order,
+ * whichever streams they are enqueued on: a call's stream waits for the handle's previous call, so two pending calls
+ * never share the handle's work buffers, and the handle's sync and read-back functions see its most recent call.
  */
 #ifndef ORBFE_H
 #define ORBFE_H
@@ -86,7 +88,7 @@ int orbfe_extract_batch(OrbfeExtractor *ex, const uint8_t *imgs, int width, int 
 int orbfe_extract_batch_device(OrbfeExtractor *ex, const uint8_t *d_imgs, int width, int height, size_t stride,
                                size_t frame_stride, int batch, OrbfeKeyPoint *d_kps, uint8_t *d_desc,
                                int *d_counts, void *stream);
-/* block until everything enqueued on the handle's own stream is done */
+/* block until the handle's calls are done, whichever streams they were enqueued on */
 int orbfe_extractor_sync(OrbfeExtractor *ex);
 /* number of kernels the last extract call launched (for bench.py's gpu_launches) */
 int orbfe_extractor_last_launches(const OrbfeExtractor *ex);
@@ -138,6 +140,8 @@ int orbfe_knn2_groups_device(OrbfeMatcher *m, const uint8_t *d_qdesc, int nq, co
 int orbfe_hamming_csr_device(OrbfeMatcher *m, const uint8_t *d_qdesc, const uint8_t *d_tdesc,
                              const int32_t *d_row_ptr, const int32_t *d_cols, int nq, int npairs,
                              uint16_t *d_out_dist, void *stream);
+/* block until the matcher's calls are done, whichever streams they were enqueued on, and report (then clear) the error
+ * flags they raised */
 int orbfe_matcher_sync(OrbfeMatcher *m);
 /* cumulative host<->device traffic and kernel launches of the host-pointer entry points (bench accounting); the bytes are
  * those of the staging block's uploaded and downloaded parts, every array padded to 256 bytes */

@@ -6,7 +6,9 @@
  * into these views.  Every matcher runs on the GPU.  The windowed matchers (SearchByProjection, WindowSearch,
  * SearchForInitialization and the guided search) run on one fused kernel: Frame's grid, GetFeaturesInArea order, the
  * distances, the accept loop and the rotation histogram, one thread block per frame pair.  Their host-array forms stage the
- * arrays, launch once per call and synchronise.
+ * arrays, launch once per call and synchronise.  Calls on one matcher run in call order, whichever streams they are
+ * enqueued on: a device entry's stream first waits for the matcher's previous call (they share its candidate scratch and
+ * error flags), and orbfe_matcher_sync reports the flags of every call made before it.
  *
  * Accepted domain of the host-array windowed matchers: a call is accepted when the kernel's per-block shared memory,
  * sbp_smem_fixed_bytes(cap, qcap) + 16 KB, is at most 220 KB, where sbp_smem_fixed_bytes(cap, qcap) is about 24,584 +

@@ -98,7 +98,7 @@ struct OrbfeExtractor {
     int *h_err = nullptr;     // pinned
     size_t h_counts_cap = 0;
 
-    cudaStream_t stream = nullptr;
+    HandleStream hs;             // every call enters and leaves it, whichever stream it is enqueued on
     cudaStream_t copy_stream = nullptr;
     std::vector<cudaEvent_t> chunk_ev;
     int last_launches = 0;
@@ -154,6 +154,8 @@ static CUresult encode_level_map(void *encode, CUtensorMap *map, uint8_t *ptr, i
 
 static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
     if (ex->W == W && ex->H == H && B <= ex->Bcap) return ORBFE_OK;
+    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
+    ORBFE_CUDA_TRY(cudaEventSynchronize(ex->hs.last));   // the handle's pending calls still use the plan
     free_plan(ex);
     PlanDev &P = ex->hplan;
     memset(&P, 0, sizeof(P));
@@ -275,7 +277,7 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
         LevelDev &L = P.lv[l];
         ORBFE_CUDA_TRY(ex->plan_mem.alloc(&L.pyr, L.plane * B + 256));
         ORBFE_CUDA_TRY(ex->plan_mem.alloc(&L.blur, L.plane + 256));  // one plane, for orbfe_debug_read_level
-        ORBFE_CUDA_TRY(cudaMemsetAsync(L.pyr, 0, L.plane * B + 256, ex->stream));
+        ORBFE_CUDA_TRY(cudaMemsetAsync(L.pyr, 0, L.plane * B + 256, ex->hs.stream));
         if (l > 0) {
             const LevelDev &S = P.lv[l - 1];
             std::vector<int> xo, yo;
@@ -406,18 +408,18 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
     ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.kp_xy_score, (size_t)std::max(P.nfeatures, 1) * B));
     ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.level_cnt, nl));
     ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.err_flag, 1));
-    ORBFE_CUDA_TRY(cudaMemsetAsync(Wk.err_flag, 0, sizeof(int), ex->stream));
+    ORBFE_CUDA_TRY(cudaMemsetAsync(Wk.err_flag, 0, sizeof(int), ex->hs.stream));
     ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->d_kps, (size_t)std::max(P.nfeatures, 1) * B));
     ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->d_desc, (size_t)std::max(P.nfeatures, 1) * B * 32));
     ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->d_counts, (size_t)B));
     ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->dplan, 1));
-    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->dplan, &P, sizeof(P), cudaMemcpyHostToDevice, ex->stream));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->dplan, &P, sizeof(P), cudaMemcpyHostToDevice, ex->hs.stream));
     if (ex->h_counts_cap < (size_t)B) {
         if (ex->h_counts) cudaFreeHost(ex->h_counts);
         ORBFE_CUDA_TRY(cudaHostAlloc((void **)&ex->h_counts, sizeof(int) * B, cudaHostAllocDefault));
         ex->h_counts_cap = B;
     }
-    ORBFE_CUDA_TRY(cudaStreamSynchronize(ex->stream));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(ex->hs.stream));
     ex->W = W; ex->H = H; ex->Bcap = B;
     ex->own_pyr0 = P.lv[0].pyr; ex->own_pitch0 = P.lv[0].pitch; ex->own_plane0 = P.lv[0].plane;
     return ORBFE_OK;
@@ -498,8 +500,7 @@ extern "C" int orbfe_extractor_create(int nfeatures, float scale_factor, int nle
     }
     ex->quota[nlevels - 1] = std::max(nfeatures - sum, 0);
 
-    cudaError_t e = cudaSetDevice(device);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ex->stream, cudaStreamNonBlocking);
+    cudaError_t e = ex->hs.create(device);
     if (e == cudaSuccess) e = cudaMalloc((void **)&ex->d_pattern, 1024);
     if (e == cudaSuccess) e = cudaMemcpy(ex->d_pattern, kBriefPattern, 1024, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaHostAlloc((void **)&ex->h_err, sizeof(int), cudaHostAllocDefault);
@@ -514,7 +515,8 @@ extern "C" int orbfe_extractor_create(int nfeatures, float scale_factor, int nle
 extern "C" int orbfe_extractor_destroy(OrbfeExtractor *ex) {
     if (!ex) return ORBFE_OK;
     cudaSetDevice(ex->device);
-    if (ex->stream) cudaStreamSynchronize(ex->stream);
+    if (ex->hs.last) cudaEventSynchronize(ex->hs.last);
+    if (ex->hs.stream) cudaStreamSynchronize(ex->hs.stream);
     free_plan(ex);
     if (ex->d_pattern) cudaFree(ex->d_pattern);
     if (ex->h_counts) cudaFreeHost(ex->h_counts);
@@ -522,7 +524,7 @@ extern "C" int orbfe_extractor_destroy(OrbfeExtractor *ex) {
     for (cudaEvent_t ev : ex->timer.ev) cudaEventDestroy(ev);
     for (cudaEvent_t ev : ex->chunk_ev) cudaEventDestroy(ev);
     if (ex->copy_stream) cudaStreamDestroy(ex->copy_stream);
-    if (ex->stream) cudaStreamDestroy(ex->stream);
+    ex->hs.destroy();
     delete ex;
     return ORBFE_OK;
 }
@@ -609,15 +611,17 @@ static void profiling_collect(OrbfeExtractor *ex) {
     T.origin_pending = true;
 }
 
-// Head of both device-resident extract entries: the plan for this geometry, level 0 taken from the caller's device frames
-// and the per-call counters zeroed, on *s (the caller's stream, or the handle's)
+// Head of both device-resident extract entries: the plan for this geometry, then on *s (the caller's stream, or the handle's),
+// behind the handle's earlier calls, level 0 taken from the caller's device frames and the per-call counters zeroed.  The
+// entry leaves the handle's stream after its last launch.
 static int begin_device_extract(OrbfeExtractor *ex, const uint8_t *d_imgs, int width, int height, size_t stride, size_t frame_stride,
                                 int batch, void *stream, cudaStream_t *s) {
     if (width <= 0 || height <= 0 || batch <= 0 || stride < (size_t)width) return fail(ORBFE_ERR_ARG, "bad geometry");
     ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
     int rc = build_plan(ex, width, height, batch);
     if (rc) return rc;
-    *s = stream ? (cudaStream_t)stream : ex->stream;
+    *s = ex->hs.pick(stream);
+    if ((rc = ex->hs.enter(*s))) return rc;
     profiling_begin(ex, *s);
     rc = ingest_device(ex, d_imgs, width, height, stride, frame_stride, batch, *s);
     if (rc) return rc;
@@ -632,7 +636,8 @@ extern "C" int orbfe_extract_batch_device(OrbfeExtractor *ex, const uint8_t *d_i
     if (!ex || !d_imgs || !d_kps || !d_desc || !d_counts) return fail(ORBFE_ERR_ARG, "NULL argument");
     cudaStream_t s;
     if (int rc = begin_device_extract(ex, d_imgs, width, height, stride, frame_stride, batch, stream, &s)) return rc;
-    return enqueue_pipeline(ex, 0, batch, d_kps, d_desc, d_counts, s);
+    if (int rc = enqueue_pipeline(ex, 0, batch, d_kps, d_desc, d_counts, s)) return rc;
+    return ex->hs.leave(s, false);
 }
 
 // The device-resident extract with the descriptor kernel's outputs redirected into the gather buffers of a rig exchange
@@ -642,8 +647,12 @@ int orbfe_extract_batch_device_peers(OrbfeExtractor *ex, const uint8_t *d_imgs, 
     if (!ex || !d_imgs) return fail(ORBFE_ERR_ARG, "NULL argument");
     cudaStream_t s;
     if (int rc = begin_device_extract(ex, d_imgs, width, height, stride, frame_stride, batch, stream, &s)) return rc;
-    if (cap != ex->hplan.nfeatures) return fail(ORBFE_ERR_ARG, "exchange capacity %d != keypoint slots per frame %d", cap, ex->hplan.nfeatures);
-    return enqueue_pipeline(ex, 0, batch, nullptr, nullptr, nullptr, s, true, &po);
+    if (cap != ex->hplan.nfeatures) {
+        ex->hs.leave(s, false);   // the ingest is enqueued
+        return fail(ORBFE_ERR_ARG, "exchange capacity %d != keypoint slots per frame %d", cap, ex->hplan.nfeatures);
+    }
+    if (int rc = enqueue_pipeline(ex, 0, batch, nullptr, nullptr, nullptr, s, true, &po)) return rc;
+    return ex->hs.leave(s, false);
 }
 
 extern "C" int orbfe_extract_batch(OrbfeExtractor *ex, const uint8_t *imgs, int width, int height, size_t stride,
@@ -656,7 +665,8 @@ extern "C" int orbfe_extract_batch(OrbfeExtractor *ex, const uint8_t *imgs, int 
     ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
     int rc = build_plan(ex, width, height, batch);
     if (rc) return rc;
-    cudaStream_t s = ex->stream;
+    cudaStream_t s = ex->hs.stream;
+    if ((rc = ex->hs.enter(s))) return rc;
     rc = set_level0(ex, ex->own_pyr0, ex->own_pitch0, ex->own_plane0, batch, s);   // the uploads land in the plan's own planes
     if (rc) return rc;
     const PlanDev &P = ex->hplan;
@@ -674,7 +684,8 @@ extern "C" int orbfe_extract_batch(OrbfeExtractor *ex, const uint8_t *imgs, int 
         ORBFE_CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         ex->chunk_ev.push_back(e);
     }
-    // the copy stream must not overwrite level 0 before earlier work of this handle has drained
+    // the copy stream must not overwrite level 0 before earlier work of this handle has drained: s has entered (it waits for
+    // the handle's last call, whichever stream that ran on), so an event recorded on it now covers that call too
     ORBFE_CUDA_TRY(cudaEventRecord(ex->chunk_ev[nchunks], s));
     ORBFE_CUDA_TRY(cudaStreamWaitEvent(ex->copy_stream, ex->chunk_ev[nchunks], 0));
     for (int k = 0; k < nchunks; k++) {
@@ -715,10 +726,11 @@ extern "C" int orbfe_extract_batch(OrbfeExtractor *ex, const uint8_t *imgs, int 
                                  cudaMemcpyDeviceToHost, s));
     }
     stage_mark(ex, s, "d2h");
-    ORBFE_CUDA_TRY(cudaStreamSynchronize(s));
+    if ((rc = ex->hs.leave(s, true))) return rc;
     if (*ex->h_err) {
         int code = *ex->h_err;
         cudaMemsetAsync(ex->work.err_flag, 0, sizeof(int), s);
+        ex->hs.leave(s, false);
         return fail(ORBFE_ERR_INTERNAL, "device overflow flag %d", code);
     }
     int status = ORBFE_OK;
@@ -737,8 +749,8 @@ extern "C" int orbfe_extract(OrbfeExtractor *ex, const uint8_t *img, int width, 
 
 extern "C" int orbfe_extractor_sync(OrbfeExtractor *ex) {
     if (!ex) return fail(ORBFE_ERR_ARG, "ex is NULL");
-    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
-    ORBFE_CUDA_TRY(cudaStreamSynchronize(ex->stream));
+    if (int rc = ex->hs.enter(ex->hs.stream)) return rc;   // the handle's last call may have run on a caller's stream
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(ex->hs.stream));
     return ORBFE_OK;
 }
 
@@ -760,8 +772,7 @@ extern "C" int orbfe_extractor_stage_times(const OrbfeExtractor *ex_c, char (*na
     if (!ex_c) return 0;
     OrbfeExtractor *ex = const_cast<OrbfeExtractor *>(ex_c);
     if (!ex->profiling) return 0;
-    cudaSetDevice(ex->device);
-    cudaStreamSynchronize(ex->stream);
+    if (ex->hs.enter(ex->hs.stream) || cudaStreamSynchronize(ex->hs.stream) != cudaSuccess) return 0;   // every timed call has ended
     profiling_collect(ex);
     int n = (int)std::min<size_t>(ex->stage_ms.size(), (size_t)std::max(cap, 0));
     for (int i = 0; i < n; i++) {
@@ -781,15 +792,14 @@ extern "C" int orbfe_debug_level_size(const OrbfeExtractor *ex, int level, int *
 extern "C" int orbfe_debug_read_level(OrbfeExtractor *ex, int frame, int level, int which, uint8_t *out, size_t out_stride) {
     if (!ex || !out || level < 0 || level >= ex->nlevels || frame < 0 || frame >= ex->Bcap)
         return fail(ORBFE_ERR_ARG, "bad arguments");
-    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
+    // the levels of the handle's last call, whichever stream it ran on
+    cudaStream_t s = ex->hs.stream;
+    if (int rc = ex->hs.enter(s)) return rc;
     const LevelDev &L = ex->hplan.lv[level];
     const uint8_t *src = which ? L.blur : L.pyr + (size_t)frame * L.plane;
-    if (which) {
-        // the pipeline smooths only descriptor patches; materialise the smoothed level of this frame on demand
-        launch_blur(ex->dplan, ex->hplan, ex->work, frame, 1, ex->stream);
-        ORBFE_CUDA_TRY(cudaGetLastError());
-    }
-    ORBFE_CUDA_TRY(cudaStreamSynchronize(ex->stream));
+    // the pipeline smooths only descriptor patches; materialise the smoothed level of this frame on demand
+    if (which) launch_blur(ex->dplan, ex->hplan, ex->work, frame, 1, s);
+    if (int rc = ex->hs.leave(s, true)) return rc;
     ORBFE_CUDA_TRY(cudaMemcpy2D(out, out_stride, src, L.pitch, L.w, L.h, cudaMemcpyDeviceToHost));
     return ORBFE_OK;
 }
@@ -800,7 +810,7 @@ extern "C" int orbfe_debug_read_level(OrbfeExtractor *ex, int frame, int level, 
 struct OrbfeMatcher {
     int device = 0;
     int nsm = 132;
-    cudaStream_t stream = nullptr;
+    HandleStream hs;       // every entry enters and leaves it, whichever stream it is enqueued on
     unsigned long long h2d_bytes = 0, d2h_bytes = 0, launches = 0;  // cumulative, for bench.py
     uint32_t *scratch = nullptr;  // candidate entries of the device-resident matcher
     size_t scratch_entries = 0;
@@ -837,7 +847,7 @@ extern "C" int orbfe_matcher_create(int device, OrbfeMatcher **out) {
         // thread blocks go first whenever an SM frees up
         int lo = 0, hi = 0;
         cudaDeviceGetStreamPriorityRange(&lo, &hi);
-        e = cudaStreamCreateWithPriority(&m->stream, cudaStreamNonBlocking, hi);
+        e = m->hs.create(device, hi);
     }
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&m->nsm, cudaDevAttrMultiProcessorCount, device);
     if (e == cudaSuccess) e = cudaMalloc((void **)&m->d_err, 2 * sizeof(int));
@@ -851,12 +861,13 @@ extern "C" int orbfe_matcher_create(int device, OrbfeMatcher **out) {
 extern "C" int orbfe_matcher_destroy(OrbfeMatcher *m) {
     if (!m) return ORBFE_OK;
     cudaSetDevice(m->device);
-    if (m->stream) cudaStreamSynchronize(m->stream);
+    if (m->hs.last) cudaEventSynchronize(m->hs.last);
+    if (m->hs.stream) cudaStreamSynchronize(m->hs.stream);
     if (m->scratch) cudaFree(m->scratch);
     m->stage.release();
     if (m->d_err) cudaFree(m->d_err);
     if (m->h_err) cudaFreeHost(m->h_err);
-    if (m->stream) cudaStreamDestroy(m->stream);
+    m->hs.destroy();
     delete m;
     return ORBFE_OK;
 }
@@ -870,14 +881,17 @@ extern "C" int orbfe_matcher_counters(const OrbfeMatcher *m, unsigned long long 
     return ORBFE_OK;
 }
 
+// Reads the flags the handle's calls so far have raised, whichever streams they ran on, and clears them
 extern "C" int orbfe_matcher_sync(OrbfeMatcher *m) {
     if (!m) return fail(ORBFE_ERR_ARG, "m is NULL");
-    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
-    ORBFE_CUDA_TRY(cudaMemcpyAsync(m->h_err, m->d_err, 2 * sizeof(int), cudaMemcpyDeviceToHost, m->stream));
-    ORBFE_CUDA_TRY(cudaStreamSynchronize(m->stream));
+    cudaStream_t s = m->hs.stream;
+    if (int rc = m->hs.enter(s)) return rc;
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(m->h_err, m->d_err, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
+    if (int rc = m->hs.leave(s, true)) return rc;
     if (*m->h_err) {
         const int flags = *m->h_err;
-        ORBFE_CUDA_TRY(cudaMemsetAsync(m->d_err, 0, 2 * sizeof(int), m->stream));
+        ORBFE_CUDA_TRY(cudaMemsetAsync(m->d_err, 0, 2 * sizeof(int), s));
+        if (int rc = m->hs.leave(s, false)) return rc;   // the next call's flags land after the clear
         if (flags & 2)
             return fail(ORBFE_ERR_ARG, "orbfe_search_by_bow_device: a job's FeatureVector has an out-of-range node row or feature "
                                        "index (its nmatches is -1)");
@@ -921,6 +935,7 @@ static int sbp_prepare(OrbfeMatcher *m, SbpParams &P, float min_x, float min_y, 
     P.scratch_per_pair = (int)per_job;
     const size_t need = (size_t)njobs * per_job;
     if (m->scratch_entries < need) {
+        ORBFE_CUDA_TRY(cudaEventSynchronize(m->hs.last));   // the handle's pending launches still use the scratch
         if (m->scratch) cudaFree(m->scratch);
         m->scratch = nullptr; m->scratch_entries = 0;
         ORBFE_CUDA_TRY(cudaMalloc((void **)&m->scratch, need * sizeof(uint32_t)));
@@ -950,7 +965,8 @@ extern "C" int orbfe_search_by_projection_device(OrbfeMatcher *m, int npairs, co
     if (!d_kps || !d_desc || !d_counts || !d_cur_idx || !d_last_idx || !d_world || !d_flags || !d_Tcw || !d_cur_mp || !d_nmatches)
         return fail(ORBFE_ERR_ARG, "NULL argument");
     if (!(max_x > min_x) || !(max_y > min_y)) return fail(ORBFE_ERR_ARG, "bad image bounds");
-    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
+    cudaStream_t s = m->hs.pick(stream);
+    if (int rc = m->hs.enter(s)) return rc;
     SbpParams P;
     memset(&P, 0, sizeof(P));
     P.fx = fx; P.fy = fy; P.cx = cx; P.cy = cy; P.th = th;
@@ -960,8 +976,10 @@ extern "C" int orbfe_search_by_projection_device(OrbfeMatcher *m, int npairs, co
     P.rule = 0; P.th_dist = 100 /* TH_HIGH, ORBmatcher.cc:1576 */; P.nnratio = 0.f;
     size_t smem;
     if (int rc = sbp_prepare(m, P, min_x, min_y, max_x, max_y, cap, cap, npairs, (size_t)64 * cap, &smem)) return rc;
-    return sbp_launched(m, launch_sbp_device(P, smem, npairs, d_kps, d_desc, d_counts, d_cur_idx, d_last_idx, d_world, d_flags, d_Tcw,
-                                             m->scratch, d_cur_mp, d_nmatches, m->d_err, stream ? (cudaStream_t)stream : m->stream));
+    if (int rc = sbp_launched(m, launch_sbp_device(P, smem, npairs, d_kps, d_desc, d_counts, d_cur_idx, d_last_idx, d_world, d_flags, d_Tcw,
+                                                   m->scratch, d_cur_mp, d_nmatches, m->d_err, s)))
+        return rc;
+    return m->hs.leave(s, false);
 }
 
 // SearchForInitialization(F1, F2, vbPrevMatched, vnMatches12, windowSize) for `npairs` (F1, F2) pairs, device-resident
@@ -1005,7 +1023,8 @@ int orbfe_search_for_initialization_hooked(OrbfeMatcher *m, int npairs, const Or
     if (!d_kps || !d_desc || !d_counts || !d_f1_idx || !d_f2_idx || !d_prev_matched || !d_match12 || !d_nmatches)
         return fail(ORBFE_ERR_ARG, "NULL argument");
     if (!(max_x > min_x) || !(max_y > min_y)) return fail(ORBFE_ERR_ARG, "bad image bounds");
-    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
+    cudaStream_t s = m->hs.pick(stream);
+    if (int rc = m->hs.enter(s)) return rc;
     SbpParams P = init_params(window, nnratio, check_orientation);
     if (hooks) {
         P.xw_flags = hooks->xw_flags; P.xw_done = hooks->xw_done; P.xw_err = hooks->xw_err; P.xw_n = hooks->xw_n; P.xw_epoch = hooks->xw_epoch;
@@ -1013,8 +1032,10 @@ int orbfe_search_for_initialization_hooked(OrbfeMatcher *m, int npairs, const Or
     }
     size_t smem;
     if (int rc = sbp_prepare(m, P, min_x, min_y, max_x, max_y, cap, cap, npairs, init_scratch_per_pair(cap), &smem)) return rc;
-    return sbp_launched(m, launch_init_device(P, smem, npairs, d_kps, d_desc, d_counts, d_f1_idx, d_f2_idx, d_prev_matched, m->scratch,
-                                              d_match12, d_nmatches, m->d_err, stream ? (cudaStream_t)stream : m->stream));
+    if (int rc = sbp_launched(m, launch_init_device(P, smem, npairs, d_kps, d_desc, d_counts, d_f1_idx, d_f2_idx, d_prev_matched, m->scratch,
+                                                    d_match12, d_nmatches, m->d_err, s)))
+        return rc;
+    return m->hs.leave(s, false);
 }
 
 // Guided search with explicit query windows, device-resident (same kernel, EXPLICIT query source).
@@ -1031,16 +1052,19 @@ extern "C" int orbfe_guided_search_device(OrbfeMatcher *m, int njobs, const Orbf
         !d_q_cnt || !d_slot_owner || !d_nmatches || (check_orientation && !d_qangle))
         return fail(ORBFE_ERR_ARG, "NULL argument");
     if (!(max_x > min_x) || !(max_y > min_y)) return fail(ORBFE_ERR_ARG, "bad image bounds");
-    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
+    cudaStream_t s = m->hs.pick(stream);
+    if (int rc = m->hs.enter(s)) return rc;
     SbpParams P;
     memset(&P, 0, sizeof(P));
     P.nlevels = 1; P.check_ori = check_orientation ? 1 : 0;
     P.rule = rule; P.th_dist = th_dist; P.nnratio = nnratio;
     size_t smem;
     if (int rc = sbp_prepare(m, P, min_x, min_y, max_x, max_y, cap, qcap, njobs, (size_t)64 * std::max(cap, qcap), &smem)) return rc;
-    return sbp_launched(m, launch_guided_device(P, smem, njobs, d_kps, d_desc, d_counts, d_frame_idx, d_qu, d_qv, d_qr, d_qlo, d_qhi,
-                                                d_qdesc, d_qangle, d_q_base, d_q_cnt, m->scratch, d_slot_owner, nullptr, d_nmatches,
-                                                m->d_err, stream ? (cudaStream_t)stream : m->stream));
+    if (int rc = sbp_launched(m, launch_guided_device(P, smem, njobs, d_kps, d_desc, d_counts, d_frame_idx, d_qu, d_qv, d_qr, d_qlo, d_qhi,
+                                                      d_qdesc, d_qangle, d_q_base, d_q_cnt, m->scratch, d_slot_owner, nullptr, d_nmatches,
+                                                      m->d_err, s)))
+        return rc;
+    return m->hs.leave(s, false);
 }
 
 int orbfe::Stage::layout(std::initializer_list<std::pair<size_t *, size_t>> arrays, size_t *total) {
@@ -1066,16 +1090,18 @@ void orbfe::Stage::release() {
     h = nullptr; d = nullptr; cap = 0;
 }
 
-// One host-array matcher call on the staged block: the round trip on the matcher's stream, its bytes counted, then either
-// orbfe_matcher_sync (`read_flags`: the call's kernels report through d_err) or a plain synchronise.
+// One host-array matcher call on the staged block: the round trip on the matcher's stream behind the handle's earlier calls,
+// its bytes counted, then either orbfe_matcher_sync (`read_flags`: the call's kernels report through d_err) or a plain
+// synchronise.  The enqueued device entries enter and leave the same stream again, which orders nothing new.
 template <class Enqueue>
 static int matcher_round_trip(OrbfeMatcher *m, bool read_flags, size_t up, size_t down, size_t total, Enqueue enqueue) {
-    if (int rc = m->stage.round_trip(m->stream, up, down, total, enqueue)) return rc;
+    cudaStream_t s = m->hs.stream;
+    if (int rc = m->hs.enter(s)) return rc;
+    if (int rc = m->stage.round_trip(s, up, down, total, enqueue)) return rc;
     m->h2d_bytes += up;
     m->d2h_bytes += total - down;
-    if (read_flags) return orbfe_matcher_sync(m);
-    ORBFE_CUDA_TRY(cudaStreamSynchronize(m->stream));
-    return ORBFE_OK;
+    if (int rc = m->hs.leave(s, !read_flags)) return rc;
+    return read_flags ? orbfe_matcher_sync(m) : ORBFE_OK;
 }
 
 // SearchByBoW (both overloads) for `njobs` frame pairs, device-resident (include/orbfe_match.h).  Arguments are checked before
@@ -1090,13 +1116,12 @@ extern "C" int orbfe_search_by_bow_device(OrbfeMatcher *m, int variant, int njob
     if (!d_kps || !d_desc || !d_counts || !d_fv_ids || !d_fv_ptr || !d_fv_items || !d_fv_n || !d_valid || !d_idx1 || !d_idx2 ||
         !d_out || !d_nmatches)
         return fail(ORBFE_ERR_ARG, "NULL argument");
-    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
-    cudaStream_t s = stream ? (cudaStream_t)stream : m->stream;
+    cudaStream_t s = m->hs.pick(stream);
+    if (int rc = m->hs.enter(s)) return rc;
     launch_search_by_bow(variant, njobs, d_kps, d_desc, d_counts, cap, d_fv_ids, d_fv_ptr, d_fv_items, d_fv_n, d_valid, d_idx1, d_idx2,
                          nnratio, check_orientation ? 1 : 0, d_out, d_nmatches, m->d_err, s);
-    ORBFE_CUDA_TRY(cudaGetLastError());
     m->launches += 1;
-    return ORBFE_OK;
+    return m->hs.leave(s, false);
 }
 
 // Offsets, in the staging block, of the two-frame store (frame 0 = side 1, frame 1 = side 2, `cap` slots each) that the
@@ -1163,7 +1188,7 @@ extern "C" int orbfe_search_by_bow(OrbfeMatcher *m, int variant, int n1, const u
             return orbfe_search_by_bow_device(m, variant, 1, (const OrbfeKeyPoint *)(D + o.kps), D + o.desc, (const int *)(D + o.cnt),
                                               cap, (const int32_t *)(D + o.ids), (const int32_t *)(D + o.ptr),
                                               (const int32_t *)(D + o.items), (const int *)(D + o.nn), D + o.flags, d_idx, d_idx + 1,
-                                              nnratio, check_orientation, (int32_t *)(D + o_out), (int *)(D + o_nm), m->stream);
+                                              nnratio, check_orientation, (int32_t *)(D + o_out), (int *)(D + o_nm), m->hs.stream);
         }))
         return rc;
     const int nout = variant == 0 ? n2 : n1;
@@ -1185,13 +1210,12 @@ extern "C" int orbfe_search_for_triangulation_device(OrbfeMatcher *m, int njobs,
     if (!d_kps || !d_desc || !d_counts || !d_fv_ids || !d_fv_ptr || !d_fv_items || !d_fv_n || !d_has_mp || !d_idx1 || !d_idx2 ||
         !d_F12 || !sigma2 || !d_match12 || !d_nmatches)
         return fail(ORBFE_ERR_ARG, "NULL argument");
-    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
-    cudaStream_t s = stream ? (cudaStream_t)stream : m->stream;
+    cudaStream_t s = m->hs.pick(stream);
+    if (int rc = m->hs.enter(s)) return rc;
     launch_search_for_triangulation(njobs, d_kps, d_desc, d_counts, cap, d_fv_ids, d_fv_ptr, d_fv_items, d_fv_n, d_has_mp, d_idx1, d_idx2,
                                     d_F12, sigma2, nlevels, check_orientation ? 1 : 0, d_match12, d_nmatches, m->d_err, s);
-    ORBFE_CUDA_TRY(cudaGetLastError());
     m->launches += 1;
-    return ORBFE_OK;
+    return m->hs.leave(s, false);
 }
 
 // SearchForTriangulation on host arrays: staged and run as orbfe_search_by_bow stages and runs SearchByBoW, with F12 as the
@@ -1241,7 +1265,7 @@ extern "C" int orbfe_search_for_triangulation(OrbfeMatcher *m, int n1, const Orb
                                                          cap, (const int32_t *)(D + o.ids), (const int32_t *)(D + o.ptr),
                                                          (const int32_t *)(D + o.items), (const int *)(D + o.nn), D + o.flags, d_idx,
                                                          d_idx + 1, (const float *)(D + o_F), sigma2_kf2, nlevels, check_orientation,
-                                                         (int32_t *)(D + o_out), (int *)(D + o_nm), m->stream);
+                                                         (int32_t *)(D + o_out), (int *)(D + o_nm), m->hs.stream);
         }))
         return rc;
     if (n1) memcpy(match12_out, H + o_out, (size_t)n1 * 4);
@@ -1254,9 +1278,10 @@ extern "C" int orbfe_hamming_csr_device(OrbfeMatcher *m, const uint8_t *d_q, con
     if (!m || (nq > 0 && (!d_q || !d_t || !d_row_ptr))) return fail(ORBFE_ERR_ARG, "NULL argument");
     ORBFE_CUDA_TRY(cudaSetDevice(m->device));
     if (nq <= 0 || npairs <= 0) return ORBFE_OK;
-    launch_hamming_csr(d_q, d_t, d_row_ptr, d_cols, nq, npairs, d_out, stream ? (cudaStream_t)stream : m->stream);
-    ORBFE_CUDA_TRY(cudaGetLastError());
-    return ORBFE_OK;
+    cudaStream_t s = m->hs.pick(stream);
+    if (int rc = m->hs.enter(s)) return rc;
+    launch_hamming_csr(d_q, d_t, d_row_ptr, d_cols, nq, npairs, d_out, s);
+    return m->hs.leave(s, false);
 }
 
 extern "C" int orbfe_hamming_csr(OrbfeMatcher *m, const uint8_t *q, int nq, const uint8_t *t, int nt,
@@ -1282,7 +1307,7 @@ extern "C" int orbfe_hamming_csr(OrbfeMatcher *m, const uint8_t *q, int nq, cons
     memcpy(H + o_cols, cols, b_cols);
     if (int rc = matcher_round_trip(m, false, o_out, o_out, total, [&]() -> int {
             if (int rc = orbfe_hamming_csr_device(m, D + o_q, D + o_t, (const int32_t *)(D + o_row), (const int32_t *)(D + o_cols), nq,
-                                                  np, (uint16_t *)(D + o_out), m->stream))
+                                                  np, (uint16_t *)(D + o_out), m->hs.stream))
                 return rc;
             m->launches += 1;
             return ORBFE_OK;
@@ -1306,7 +1331,7 @@ extern "C" int orbfe_hamming_dense(OrbfeMatcher *m, const uint8_t *q, int nq, co
     memcpy(H + o_q, q, b_q);
     memcpy(H + o_t, t, b_t);
     if (int rc = matcher_round_trip(m, false, o_out, o_out, total, [&]() -> int {
-            launch_hamming_dense(D + o_q, nq, D + o_t, nt, (uint16_t *)(D + o_out), m->stream);
+            launch_hamming_dense(D + o_q, nq, D + o_t, nt, (uint16_t *)(D + o_out), m->hs.stream);
             ORBFE_CUDA_TRY(cudaGetLastError());
             return ORBFE_OK;
         }))
@@ -1321,16 +1346,15 @@ extern "C" int orbfe_undistort_keypoints_device(OrbfeMatcher *m, const OrbfeKeyP
     if (!m || n < 0 || !dist5 || !(fx != 0.f) || !(fy != 0.f)) return fail(ORBFE_ERR_ARG, "bad arguments");
     if (n == 0) return ORBFE_OK;
     if (!d_in || !d_out) return fail(ORBFE_ERR_ARG, "NULL argument");
-    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
-    cudaStream_t s = stream ? (cudaStream_t)stream : m->stream;
+    cudaStream_t s = m->hs.pick(stream);
+    if (int rc = m->hs.enter(s)) return rc;
     if (dist5[0] == 0.0f) {  // mvKeysUn = mvKeys (Frame.cc:291-295)
         if (d_in != d_out) ORBFE_CUDA_TRY(cudaMemcpyAsync(d_out, d_in, sizeof(OrbfeKeyPoint) * (size_t)n, cudaMemcpyDeviceToDevice, s));
-        return ORBFE_OK;
+        return m->hs.leave(s, false);
     }
     launch_undistort(fx, fy, cx, cy, dist5, d_in, d_out, n, s);
-    ORBFE_CUDA_TRY(cudaGetLastError());
     m->launches += 1;
-    return ORBFE_OK;
+    return m->hs.leave(s, false);
 }
 
 extern "C" int orbfe_undistort_keypoints(OrbfeMatcher *m, const OrbfeKeyPoint *in, OrbfeKeyPoint *out, int n, float fx, float fy,
@@ -1349,7 +1373,7 @@ extern "C" int orbfe_undistort_keypoints(OrbfeMatcher *m, const OrbfeKeyPoint *i
     OrbfeKeyPoint *h_kps = (OrbfeKeyPoint *)m->stage.h, *d_kps = (OrbfeKeyPoint *)m->stage.d;
     memcpy(h_kps, in, sizeof(OrbfeKeyPoint) * (size_t)n);
     if (int rc = matcher_round_trip(m, false, total, 0, total, [&] {
-            return orbfe_undistort_keypoints_device(m, d_kps, d_kps, n, fx, fy, cx, cy, dist5, m->stream);
+            return orbfe_undistort_keypoints_device(m, d_kps, d_kps, n, fx, fy, cx, cy, dist5, m->hs.stream);
         }))
         return rc;
     memcpy(out, h_kps, sizeof(OrbfeKeyPoint) * (size_t)n);
@@ -1396,7 +1420,7 @@ extern "C" int orbfe_distinctive_descriptors(OrbfeMatcher *m, const uint8_t *des
     if (total > 0) memcpy(H + o_desc, desc, b_desc);   // all groups empty: nothing to upload, the launch still writes every -1
     memcpy(H + o_ptr, group_ptr, b_ptr);
     if (int rc = matcher_round_trip(m, false, o_best, o_best, nbytes, [&]() -> int {
-            launch_distinctive(D + o_desc, (const int *)(D + o_ptr), ngroups, (int *)(D + o_best), m->stream);
+            launch_distinctive(D + o_desc, (const int *)(D + o_ptr), ngroups, (int *)(D + o_best), m->hs.stream);
             ORBFE_CUDA_TRY(cudaGetLastError());
             return ORBFE_OK;
         }))
@@ -1418,12 +1442,11 @@ extern "C" int orbfe_distinctive_descriptors_device(OrbfeMatcher *m, int ngroups
         return fail(ORBFE_ERR_ARG, "orbfe_distinctive_descriptors_device: NULL argument");
     if (((uintptr_t)d_desc | (uintptr_t)d_mp_desc) % 16)
         return fail(ORBFE_ERR_ARG, "orbfe_distinctive_descriptors_device: d_desc and d_mp_desc must be 16-byte aligned");
-    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
-    cudaStream_t s = stream ? (cudaStream_t)stream : m->stream;
+    cudaStream_t s = m->hs.pick(stream);
+    if (int rc = m->hs.enter(s)) return rc;
     launch_distinctive_obs(d_desc, d_counts, nframes, cap, d_group_ptr, d_obs, nobs, ngroups, d_best, d_mp_desc, m->d_err, s);
-    ORBFE_CUDA_TRY(cudaGetLastError());
     m->launches += 1;
-    return ORBFE_OK;
+    return m->hs.leave(s, false);
 }
 
 // MapPoint::UpdateNormalAndDepth for many map points in one launch, on the frame store (include/orbfe_bow.h).  Arguments
@@ -1440,13 +1463,12 @@ extern "C" int orbfe_normal_and_depth_device(OrbfeMatcher *m, int npoints, const
     if (!d_kps || !d_counts || !d_centers || !d_group_ptr || !d_obs || !d_world || !d_ref_obs || !scale_factors || !d_normal ||
         !d_min_dist || !d_max_dist)
         return fail(ORBFE_ERR_ARG, "orbfe_normal_and_depth_device: NULL argument");
-    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
-    cudaStream_t s = stream ? (cudaStream_t)stream : m->stream;
+    cudaStream_t s = m->hs.pick(stream);
+    if (int rc = m->hs.enter(s)) return rc;
     launch_normal_depth_obs(d_kps, d_counts, nframes, cap, d_centers, d_group_ptr, d_obs, nobs, d_world, d_ref_obs, scale_factor, nlevels,
                             scale_factors, npoints, d_normal, d_min_dist, d_max_dist, m->d_err, s);
-    ORBFE_CUDA_TRY(cudaGetLastError());
     m->launches += 1;
-    return ORBFE_OK;
+    return m->hs.leave(s, false);
 }
 
 // The same for callers without a frame store: every centre given on the host, staged through the matcher's block and run
@@ -1485,7 +1507,7 @@ extern "C" int orbfe_normal_and_depth(OrbfeMatcher *m, int npoints, const float 
     if (int rc = matcher_round_trip(m, false, nbytes, o_normal, nbytes, [&]() -> int {
             launch_normal_depth((const float *)(D + o_obs), (const int *)(D + o_ptr), (const float *)(D + o_world),
                                 (const float *)(D + o_ref), (const int *)(D + o_oct), scale_factor, nlevels, scale_factors, npoints,
-                                (float *)(D + o_normal), (float *)(D + o_min), (float *)(D + o_max), m->stream);
+                                (float *)(D + o_normal), (float *)(D + o_min), (float *)(D + o_max), m->hs.stream);
             ORBFE_CUDA_TRY(cudaGetLastError());
             return ORBFE_OK;
         }))
@@ -1521,7 +1543,7 @@ int orbfe::bow_db_score(OrbfeMatcher *m, int nq, const int32_t *q_ids, const dou
     if (int rc = matcher_round_trip(m, false, o_c, o_c, total, [&]() -> int {
             launch_bow_db_score(nq, (const int *)(D + o_qi), (const double *)(D + o_qv), nkf, (const int *)(D + o_kp),
                                 (const int *)(D + o_di), (const double *)(D + o_dv), (int *)(D + o_c), (int *)(D + o_f),
-                                (double *)(D + o_s), m->stream);
+                                (double *)(D + o_s), m->hs.stream);
             ORBFE_CUDA_TRY(cudaGetLastError());
             return ORBFE_OK;
         }))
@@ -1539,11 +1561,10 @@ extern "C" int orbfe_knn2_groups_device(OrbfeMatcher *m, const uint8_t *d_q, int
     if (!m || nq < 0 || ngroups < 0 || group_size < 0) return fail(ORBFE_ERR_ARG, "bad arguments");
     if (nq == 0 || ngroups == 0) return ORBFE_OK;
     if (!d_q || !d_db || !d_best || !d_best_idx || !d_second) return fail(ORBFE_ERR_ARG, "NULL argument");
-    ORBFE_CUDA_TRY(cudaSetDevice(m->device));
-    launch_knn2_groups(d_q, nq, d_db, ngroups, group_size, d_best, d_best_idx, d_second,
-                       stream ? (cudaStream_t)stream : m->stream);
-    ORBFE_CUDA_TRY(cudaGetLastError());
-    return ORBFE_OK;
+    cudaStream_t s = m->hs.pick(stream);
+    if (int rc = m->hs.enter(s)) return rc;
+    launch_knn2_groups(d_q, nq, d_db, ngroups, group_size, d_best, d_best_idx, d_second, s);
+    return m->hs.leave(s, false);
 }
 
 // The database is staged through the handle's pinned block, which keeps the size of the largest call; a bulk sweep belongs on
@@ -1566,7 +1587,7 @@ extern "C" int orbfe_knn2_groups(OrbfeMatcher *m, const uint8_t *q, int nq, cons
     memcpy(H + o_db, db, b_db);
     if (int rc = matcher_round_trip(m, false, o_best, o_best, total, [&] {
             return orbfe_knn2_groups_device(m, D + o_q, nq, D + o_db, ngroups, group_size, (uint16_t *)(D + o_best),
-                                            (int32_t *)(D + o_idx), (uint16_t *)(D + o_second), m->stream);
+                                            (int32_t *)(D + o_idx), (uint16_t *)(D + o_second), m->hs.stream);
         }))
         return rc;
     memcpy(best, H + o_best, sizeof(uint16_t) * no);
@@ -1718,7 +1739,7 @@ int orbfe::sbp_frames_host(OrbfeMatcher *m, int npairs, const OrbfeFrameView *cu
             const int rc = launch_sbp_device(P, smem, n, (const OrbfeKeyPoint *)(D + o_kps), D + o_desc, (const int *)(D + o_cnt),
                                              (const int *)(D + o_ci) + k0, (const int *)(D + o_li) + k0, (const float *)(D + o_world),
                                              D + o_flags, (const float *)(D + o_T) + (size_t)k0 * 12, m->scratch,
-                                             (int *)(D + o_mp) + (size_t)k0 * cap, (int *)(D + o_nm) + k0, m->d_err, m->stream);
+                                             (int *)(D + o_mp) + (size_t)k0 * cap, (int *)(D + o_nm) + k0, m->d_err, m->hs.stream);
             if (int e = sbp_launched(m, rc)) return e;
         }
         return ORBFE_OK;
@@ -1799,7 +1820,7 @@ int orbfe::guided_host(OrbfeMatcher *m, const OrbfeFrameView &f, int nq, const G
                                                 (const float *)(D + o_qr), (const int *)(D + o_lo), (const int *)(D + o_hi), D + o_qd,
                                                 (const float *)(D + o_qa), (const int *)(D + o_qb) + c, (const int *)(D + o_qc) + c,
                                                 m->scratch, (int *)(D + o_mp), best_out ? (int *)(D + o_best) : nullptr,
-                                                (int *)(D + o_nm) + c, m->d_err, m->stream);
+                                                (int *)(D + o_nm) + c, m->d_err, m->hs.stream);
             if (int e = sbp_launched(m, rc)) return e;
         }
         return ORBFE_OK;
@@ -1845,7 +1866,7 @@ int orbfe::init_host(OrbfeMatcher *m, const OrbfeFrameView &f1, const OrbfeFrame
         const int *d_idx = (const int *)(D + o_idx);
         return sbp_launched(m, launch_init_device(P, smem, 1, (const OrbfeKeyPoint *)(D + o_kps), D + o_desc, (const int *)(D + o_cnt),
                                                   d_idx, d_idx + 1, (float *)(D + o_prev), m->scratch, (int *)(D + o_m12),
-                                                  (int *)(D + o_nm), m->d_err, m->stream));
+                                                  (int *)(D + o_nm), m->d_err, m->hs.stream));
     };
     if (int rc = run_staged(m, o_prev, o_m12, total, init_scratch_per_pair(cap), pack_prev, launch)) return rc;
     if (f1.n) {

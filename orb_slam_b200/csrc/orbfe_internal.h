@@ -231,15 +231,16 @@ struct DeviceBuffers {
 
 // The own stream of a handle whose entries may also run on caller streams, and the rule that makes that safe: every call
 // enters (its stream waits for the handle's last work) and leaves (records its own), so the handle's calls run in call order
-// whichever streams they were enqueued on.
+// whichever streams they were enqueued on.  Whatever reads or frees the handle's device state from the host (a sync, a
+// buffer that grows) first waits for `last`.
 struct HandleStream {
     int device = 0;
     cudaStream_t stream = nullptr;   // non-blocking
     cudaEvent_t last = nullptr;      // the handle's most recent work
-    cudaError_t create(int dev) {
+    cudaError_t create(int dev, int priority = 0) {
         device = dev;
         cudaError_t e = cudaSetDevice(dev);
-        if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
+        if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&stream, cudaStreamNonBlocking, priority);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&last, cudaEventDisableTiming);
         return e;
     }
