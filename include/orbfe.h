@@ -88,10 +88,36 @@ int orbfe_extract_batch(OrbfeExtractor *ex, const uint8_t *imgs, int width, int 
 int orbfe_extract_batch_device(OrbfeExtractor *ex, const uint8_t *d_imgs, int width, int height, size_t stride,
                                size_t frame_stride, int batch, OrbfeKeyPoint *d_kps, uint8_t *d_desc,
                                int *d_counts, void *stream);
+/* Mixed geometries: frames of up to ORBFE_MULTI_MAX_GROUPS image geometries (a rig whose cameras differ in resolution) in
+ * one launch chain, as long as one group's (nlevels + 4 kernels, whatever ngroups is).  Frames are numbered group by group
+ * in the order of `groups`; frame f of the call is at f * cap (host form: kps, desc, n_out[total frames]) or
+ * f * nfeatures (device form: d_kps, d_desc, d_counts), as orbfe_extract_batch* lays out a batch.  Per frame, keypoints,
+ * descriptors, count and order are those of orbfe_extract_batch_device with that frame's geometry.  A group with a NULL
+ * image or W/H <= 0 yields zero keypoints for its `batch` frames.  Argument errors are ORBFE_ERR_ARG; a group whose
+ * geometry the single-geometry entries reject gives ORBFE_ERR_UNSUPPORTED naming the group; nothing is launched then.
+ * The handle keeps one plan for the single-geometry entries and one multi plan, keyed by the ordered (W, H) list of the
+ * non-empty groups, holding as many frames per group as the largest call has passed: alternating single and multi calls,
+ * or multi calls with the same geometry list, re-plans neither.  The limit on ngroups sizes the multi plan's level table
+ * (ORBFE_MULTI_MAX_GROUPS x ORBFE_MAX_LEVELS entries) and the group scan each kernel does to place a thread block. */
+#define ORBFE_MULTI_MAX_GROUPS 8
+typedef struct {
+    int width, height;      /* this group's geometry */
+    size_t stride;          /* row stride in bytes */
+    size_t frame_stride;    /* bytes between consecutive frames of the group */
+    int batch;              /* frames in this group (>= 1) */
+    const uint8_t *imgs;    /* host pointer (orbfe_extract_multi) or device pointer (_device) */
+} OrbfeImageGroup;
+int orbfe_extract_multi(OrbfeExtractor *ex, int ngroups, const OrbfeImageGroup *groups,
+                        OrbfeKeyPoint *kps, uint8_t *desc, int cap, int *n_out);
+int orbfe_extract_multi_device(OrbfeExtractor *ex, int ngroups, const OrbfeImageGroup *groups,
+                               OrbfeKeyPoint *d_kps, uint8_t *d_desc, int *d_counts, void *stream);
+
 /* block until the handle's calls are done, whichever streams they were enqueued on */
 int orbfe_extractor_sync(OrbfeExtractor *ex);
 /* number of kernels the last extract call launched (for bench.py's gpu_launches) */
 int orbfe_extractor_last_launches(const OrbfeExtractor *ex);
+/* number of plans (single-geometry and multi) the handle has built since it was created */
+int orbfe_extractor_plan_builds(const OrbfeExtractor *ex);
 
 /* How orbfe_extract_batch schedules a batch (default 0).
  *   0 "chunked": the upload of chunk k+1 overlaps ALL kernels of chunk k;

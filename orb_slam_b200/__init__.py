@@ -14,7 +14,8 @@ import os
 
 import numpy as np
 
-__all__ = ["ORBextractor", "ORBmatcher", "OrbfeError", "KP_DTYPE", "lib", "library_path", "HARRIS_SCORE", "FAST_SCORE"]
+__all__ = ["ORBextractor", "ORBmatcher", "OrbfeError", "KP_DTYPE", "OrbfeImageGroup", "lib", "library_path", "HARRIS_SCORE",
+           "FAST_SCORE"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SO = os.path.join(_HERE, "liborbfe.so")
@@ -22,6 +23,15 @@ _SO = os.path.join(_HERE, "liborbfe.so")
 HARRIS_SCORE, FAST_SCORE = 0, 1  # ORBextractor.h:37
 ORBFE_OK, ORBFE_ERR_ARG, ORBFE_ERR_UNSUPPORTED, ORBFE_ERR_CAPACITY = 0, -1, -2, -3
 ORBFE_ERR_CUDA, ORBFE_ERR_NO_DEVICE, ORBFE_ERR_INTERNAL = -4, -5, -6
+
+ORBFE_MULTI_MAX_GROUPS = 8   # include/orbfe.h
+
+
+class OrbfeImageGroup(C.Structure):
+    """One image geometry of an orbfe_extract_multi* call (include/orbfe.h)"""
+    _fields_ = [("width", C.c_int), ("height", C.c_int), ("stride", C.c_size_t), ("frame_stride", C.c_size_t),
+                ("batch", C.c_int), ("imgs", C.c_void_p)]
+
 
 # cv::KeyPoint layout (28 bytes)
 KP_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4"), ("response", "<f4"),
@@ -34,6 +44,7 @@ ABI_SYMBOLS = [
     "orbfe_extractor_tables", "orbfe_extract", "orbfe_extract_batch", "orbfe_extract_batch_device",
     "orbfe_extractor_sync", "orbfe_extractor_last_launches", "orbfe_extractor_set_profiling", "orbfe_extractor_set_batch_mode",
     "orbfe_extractor_stage_times", "orbfe_debug_level_size", "orbfe_debug_read_level",
+    "orbfe_extract_multi", "orbfe_extract_multi_device", "orbfe_extractor_plan_builds",
     "orbfe_matcher_create", "orbfe_matcher_destroy", "orbfe_hamming_csr", "orbfe_hamming_dense",
     "orbfe_knn2_groups", "orbfe_knn2_groups_device", "orbfe_hamming_csr_device", "orbfe_matcher_sync",
     "orbfe_matcher_counters",
@@ -98,6 +109,10 @@ def lib():
     L.orbfe_extract.argtypes = [vp, vp, C.c_int, C.c_int, C.c_size_t, vp, vp, C.c_int, ip]
     L.orbfe_extract_batch.argtypes = [vp, vp, C.c_int, C.c_int, C.c_size_t, C.c_size_t, C.c_int, vp, vp, C.c_int, vp]
     L.orbfe_extract_batch_device.argtypes = [vp, vp, C.c_int, C.c_int, C.c_size_t, C.c_size_t, C.c_int, vp, vp, vp, vp]
+    gp = C.POINTER(OrbfeImageGroup)
+    L.orbfe_extract_multi.argtypes = [vp, C.c_int, gp, vp, vp, C.c_int, vp]
+    L.orbfe_extract_multi_device.argtypes = [vp, C.c_int, gp, vp, vp, vp, vp]
+    L.orbfe_extractor_plan_builds.argtypes = [vp]
     L.orbfe_extractor_sync.argtypes = [vp]
     L.orbfe_extractor_last_launches.argtypes = [vp]
     L.orbfe_extractor_set_profiling.argtypes = [vp, C.c_int]
@@ -206,6 +221,44 @@ class ORBextractor:
         _check(lib().orbfe_extract_batch_device(self._h, C.c_void_p(d_imgs), W, H, stride, frame_stride, B,
                                                 C.c_void_p(d_kps), C.c_void_p(d_desc), C.c_void_p(d_counts),
                                                 C.c_void_p(stream)))
+
+    def extract_multi(self, images, cap=None):
+        """Frames of several geometries in one call (orbfe_extract_multi).  images: a list of groups, each a uint8 array
+        [H, W] (one frame) or [B, H, W] (rows with unit pixel stride), or None / an empty array (one frame without
+        keypoints).  Returns one (keypoints[KP_DTYPE], descriptors[N, 32]) per frame, group by group."""
+        arrays, groups = [], (OrbfeImageGroup * max(len(images), 1))()
+        for g, img in zip(groups, images):
+            if img is None or img.size == 0:
+                g.batch = img.shape[0] if img is not None and img.ndim == 3 and img.shape[0] else 1
+                continue
+            assert img.dtype == np.uint8 and img.ndim in (2, 3), "CV_8UC1 frames expected"
+            a = img if img.ndim == 3 else img[None]
+            if a.strides[2] != 1:
+                a = np.ascontiguousarray(a)
+            arrays.append(a)
+            g.batch, g.height, g.width = a.shape
+            g.stride, g.frame_stride, g.imgs = a.strides[1], a.strides[0], a.ctypes.data
+        F = sum(g.batch for g in groups[:len(images)])
+        cap = cap or max(self.nfeatures, 1)
+        kps = np.zeros((F, cap), KP_DTYPE)
+        desc = np.zeros((F, cap, 32), np.uint8)
+        counts = np.zeros(F, np.int32)
+        _check(lib().orbfe_extract_multi(self._h, len(images), groups, _p(kps), _p(desc), cap, _p(counts)))
+        return [(kps[f, :n], desc[f, :n]) for f, n in enumerate(counts)]
+
+    def extract_multi_device(self, groups, d_kps, d_desc, d_counts, stream=0):
+        """Device-pointer form of extract_multi: groups = [(d_imgs, W, H, stride, frame_stride, B), ...] (ints = raw device
+        addresses); frame f of the call goes to slot f * nfeatures of d_kps / d_desc.  Enqueues on `stream`, does not
+        synchronise."""
+        arr = (OrbfeImageGroup * max(len(groups), 1))()
+        for g, (p, W, H, stride, frame_stride, B) in zip(arr, groups):
+            g.imgs, g.width, g.height, g.stride, g.frame_stride, g.batch = p or None, W, H, stride, frame_stride, B
+        _check(lib().orbfe_extract_multi_device(self._h, len(groups), arr, C.c_void_p(d_kps), C.c_void_p(d_desc),
+                                                C.c_void_p(d_counts), C.c_void_p(stream)))
+
+    def plan_builds(self):
+        """plans (single-geometry and multi) this handle has built"""
+        return lib().orbfe_extractor_plan_builds(self._h)
 
     def set_batch_mode(self, mode):
         """0 = chunked (one handle), 1 = phased (two alternating handles); see include/orbfe.h."""

@@ -15,24 +15,38 @@
 // (no FMA contraction).  No tensor cores: there is no dense contraction on this path.
 #include <cuda_fp16.h>
 
+#include <atomic>
+
 #include "orbfe_internal.h"
 
 namespace orbfe {
 
-__global__ void cell_select_harris_kernel(const PlanDev *__restrict__ plan, WorkDev wk, int f0);
-__global__ void level_select_harris_kernel(const PlanDev *__restrict__ plan, WorkDev wk, int f0);
+template <bool kMulti> __global__ void cell_select_harris_kernel(const PlanOf<kMulti> *__restrict__ plan, WorkDev wk, int f0);
+template <bool kMulti> __global__ void level_select_harris_kernel(const PlanOf<kMulti> *__restrict__ plan, WorkDev wk, int f0);
 
-__device__ __forceinline__ int find_level_by(const PlanDev *plan, int idx, int which) {
+// v0: the first entry of the level table searched (a group's levels in a multi plan)
+template <class Plan>
+__device__ __forceinline__ int find_level_by(const Plan *plan, int idx, int which, int v0 = 0) {
     // which: 0 = ftile_base, 1 = btile_base, 2 = cell_base, 3 = kp_base
     int l = 0;
     const int n = plan->nlevels;
     for (int k = 1; k < n; k++) {
-        const LevelDev &L = plan->lv[k];
+        const LevelDev &L = plan->lv[v0 + k];
         const int base = which == 0 ? L.ftile_base : which == 1 ? L.btile_base : which == 2 ? L.cell_base : L.kp_base;
         // levels with zero extent share a base with their successor: the LAST level whose base <= idx wins
         if (idx >= base) l = k;
     }
     return l;
+}
+
+// Multi plan: the group that holds item i of a per-call numbering whose group starts are ascending (GroupDev::frame0,
+// fwork0 or cwork0); empty ranges share a start with their successor and lose to it
+template <int GroupDev::*Start>
+__device__ __forceinline__ int group_of(const MultiPlanDev *plan, int i) {
+    int g = 0;
+    for (int k = 1; k < plan->ngroups; k++)
+        if (i >= plan->grp[k].*Start) g = k;
+    return g;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -70,11 +84,17 @@ static inline void launch_k(void (*kern)(P...), dim3 grid, dim3 block, size_t sm
 // ------------------------------------------------------------------------------------------------
 #define RZ_ROWS 4  // destination rows per thread (the horizontal taps are loaded once and reused)
 
-__global__ void __launch_bounds__(256) resize_level_kernel(const PlanDev *__restrict__ plan, int level, int f0) {
+template <bool kMulti>
+__global__ void __launch_bounds__(256) resize_level_kernel(const PlanOf<kMulti> *__restrict__ plan, int level, int f0) {
     pdl_prologue();
-    const LevelDev &D = plan->lv[level];
-    const LevelDev &S = plan->lv[level - 1];
-    const int f = blockIdx.z + f0;
+    int lv = level, f = blockIdx.z + f0;
+    if constexpr (kMulti) {   // blockIdx.z = the call's work frame: level `level` of its group, frame f of that group's planes
+        const int g = group_of<&GroupDev::frame0>(plan, blockIdx.z);
+        lv = g * plan->nlevels + level;
+        f = blockIdx.z - plan->grp[g].frame0;
+    }
+    const LevelDev &D = plan->lv[lv];
+    const LevelDev &S = plan->lv[lv - 1];
     const int ybase = (blockIdx.y * blockDim.y + threadIdx.y) * RZ_ROWS;
     const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     const int dw = D.w, dh = D.h;
@@ -181,7 +201,19 @@ void launch_resize_level(const PlanDev *d_plan, const PlanDev &hp, int level, in
     const LevelDev &D = hp.lv[level];
     dim3 block(64, 4);
     dim3 grid((D.w + 255) / 256, (D.h + 4 * RZ_ROWS - 1) / (4 * RZ_ROWS), nf);
-    launch_k(resize_level_kernel, grid, block, 0, s, hp.pdl != 0, d_plan, level, f0);
+    launch_k(resize_level_kernel<false>, grid, block, 0, s, hp.pdl != 0, d_plan, level, f0);
+}
+
+// one launch for level `level` of every group: the grid covers the largest group's level; blocks outside a frame's own
+// level return at once
+void launch_resize_level_multi(const MultiPlanDev *d_plan, const MultiPlanDev &hp, int level, cudaStream_t s) {
+    int gx = 1, gy = 1;
+    for (int g = 0; g < hp.ngroups; g++) {
+        const LevelDev &D = hp.lv[g * hp.nlevels + level];
+        gx = std::max(gx, (D.w + 255) / 256);
+        gy = std::max(gy, (D.h + 4 * RZ_ROWS - 1) / (4 * RZ_ROWS));
+    }
+    launch_k(resize_level_kernel<true>, dim3(gx, gy, hp.nframes), dim3(64, 4), 0, s, hp.pdl != 0, d_plan, level, 0);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -358,8 +390,10 @@ __device__ __forceinline__ void cell_window(const LevelDev &L, int xmax, int yma
 // Everything after the pixel tile is staged: m map, NMS passes, candidate conversion and flush.
 // pix: staged pixel rows (stride F2_TW); mt: 16 KB m tile; s_cand: candidate list (F2_MAXC entries).
 // tile indexes wk.ftile_info; the tile's FTileInfo and level are re-read after the score loop, so that none of the geometry
-// the NMS and the flush need occupies registers while the 7-row window is live.
-__device__ __forceinline__ void fast_tile_compute(const PlanDev *__restrict__ plan, const WorkDev &wk, int tile, int level, int f, int x0, int y0, const uint8_t *pix, uint32_t *mt,
+// the NMS and the flush need occupies registers while the 7-row window is live.  f indexes the per-frame work arrays, pf the
+// frame in the level's planes (the same frame unless the plan is a multi plan).
+template <class Plan>
+__device__ __forceinline__ void fast_tile_compute(const Plan *__restrict__ plan, const WorkDev &wk, int tile, int level, int f, int pf, int x0, int y0, const uint8_t *pix, uint32_t *mt,
                                                   uint32_t *s_cand, int &s_n, int *s_cnt_lo, int *s_cnt_hi,
                                                   long long *s_kbase, int *s_klim) {
     const int tlo = plan->t_lo;
@@ -545,7 +579,7 @@ __device__ __forceinline__ void fast_tile_compute(const PlanDev *__restrict__ pl
             const size_t kidx = (size_t)(s_kbase[lc] + slot);
             if (wk.cand_keys64) {
                 // HARRIS_SCORE (:616-620): rank by the Harris response; the FAST score rides along for eligibility
-                const float resp = harris_response(L.pyr + (size_t)f * L.plane, L.pitch, x, y, plan->harris_scale4);
+                const float resp = harris_response(L.pyr + (size_t)pf * L.plane, L.pitch, x, y, plan->harris_scale4);
                 wk.cand_keys64[kidx] = ((unsigned long long)float_order_key(resp) << 32) |
                                        ((unsigned long long)(0xFFFFFFu - raster) << 8) | (unsigned long long)(m - 1);
             } else {
@@ -592,7 +626,17 @@ __device__ __forceinline__ void tma_load_3d(void *smem_dst, const void *tmap, ui
 #define F2_TMA_SMEM (2 * F2_PIXSLOT + F2_MH * 32 * 2 * 4 + 128)
 static_assert(F2_MAXC * 4 <= F2_PIXSLOT, "the candidate queue lives in the pixel slot that was just consumed");
 
-__global__ void __launch_bounds__(256, ORBFE_FAST_BLOCKS_PER_SM) fast_nms_tma_kernel(const PlanDev *__restrict__ plan, WorkDev wk, int f0, int nwork) {
+// Work item wi of a multi plan: its tile in the flat table, its work frame f and its frame pf in the group's level planes
+__device__ __forceinline__ void fast_item_multi(const MultiPlanDev *plan, int wi, int &tile, int &f, int &pf) {
+    const GroupDev &G = plan->grp[group_of<&GroupDev::fwork0>(plan, wi)];
+    const int r = wi - G.fwork0;
+    tile = G.ftile0 + r % G.nftiles;
+    pf = r / G.nftiles;
+    f = G.frame0 + pf;
+}
+
+template <bool kMulti>
+__global__ void __launch_bounds__(256, ORBFE_FAST_BLOCKS_PER_SM) fast_nms_tma_kernel(const PlanOf<kMulti> *__restrict__ plan, WorkDev wk, int f0, int nwork) {
     extern __shared__ __align__(128) uint8_t dsm[];
     uint8_t *pixbuf0 = dsm, *pixbuf1 = dsm + F2_PIXSLOT;
     uint32_t *mt = reinterpret_cast<uint32_t *>(dsm + 2 * F2_PIXSLOT);
@@ -610,15 +654,18 @@ __global__ void __launch_bounds__(256, ORBFE_FAST_BLOCKS_PER_SM) fast_nms_tma_ke
     pdl_prologue();   // the barriers above are private to the CTA; the first TMA load reads what the resize kernels wrote
     int wi = blockIdx.x;
     if (wi < nwork && threadIdx.x == 0) {
-        const FTileInfo t0 = wk.ftile_info[wi % ntiles];
+        int tile = wi % ntiles, pf = f0 + wi / ntiles;
+        if constexpr (kMulti) { int f; fast_item_multi(plan, wi, tile, f, pf); }
+        const FTileInfo t0 = wk.ftile_info[tile];
         mbar_expect_tx(&bar[0], F2_PIXBYTES);
-        tma_load_3d(pixbuf0, &wk.tmaps[t0.level], &bar[0], (ORBFE_EDGE + t0.tx * F2_W - 8) & ~15, ORBFE_EDGE + t0.ty * F2_H - 4, f0 + wi / ntiles);
+        tma_load_3d(pixbuf0, &wk.tmaps[t0.level], &bar[0], (ORBFE_EDGE + t0.tx * F2_W - 8) & ~15, ORBFE_EDGE + t0.ty * F2_H - 4, pf);
     }
     for (int it = 0; wi < nwork; it++, wi += gridDim.x) {
         const int cur = it & 1;
         const int nxt = wi + gridDim.x;
-        const FTileInfo ti = wk.ftile_info[wi % ntiles];
-        const int f = f0 + wi / ntiles;
+        int tile = wi % ntiles, f = f0 + wi / ntiles, pf = f;
+        if constexpr (kMulti) fast_item_multi(plan, wi, tile, f, pf);
+        const FTileInfo ti = wk.ftile_info[tile];
         const int x0 = ORBFE_EDGE + ti.tx * F2_W, y0 = ORBFE_EDGE + ti.ty * F2_H;
         // No barrier ends an item: a thread gets here once every thread has passed the previous item's flush barrier,
         // so the counters are no longer read; the previous item's key stores may still read its candidate queue (the
@@ -631,21 +678,25 @@ __global__ void __launch_bounds__(256, ORBFE_FAST_BLOCKS_PER_SM) fast_nms_tma_ke
         // prefetch the next tile into the other buffer: every thread has finished the previous item, whose candidate
         // queue lived there, and has waited on that buffer's mbarrier phase
         if (nxt < nwork && threadIdx.x == 0) {
-            const FTileInfo tn = wk.ftile_info[nxt % ntiles];
+            int ntile = nxt % ntiles, npf = f0 + nxt / ntiles;
+            if constexpr (kMulti) { int nf; fast_item_multi(plan, nxt, ntile, nf, npf); }
+            const FTileInfo tn = wk.ftile_info[ntile];
             mbar_expect_tx(&bar[cur ^ 1], F2_PIXBYTES);
             tma_load_3d(cur ? pixbuf0 : pixbuf1, &wk.tmaps[tn.level], &bar[cur ^ 1], (ORBFE_EDGE + tn.tx * F2_W - 8) & ~15,
-                        ORBFE_EDGE + tn.ty * F2_H - 4, f0 + nxt / ntiles);
+                        ORBFE_EDGE + tn.ty * F2_H - 4, npf);
         }
         // the candidate queue reuses the current pixel slot (dead once m is computed; the next TMA into it is
         // only issued after the first barrier of the next item)
         uint8_t *slot_cur = cur ? pixbuf1 : pixbuf0;
-        fast_tile_compute(plan, wk, wi % ntiles, ti.level, f, x0, y0, slot_cur + ((x0 - 8) & 15), mt, reinterpret_cast<uint32_t *>(slot_cur),
+        fast_tile_compute(plan, wk, tile, ti.level, f, pf, x0, y0, slot_cur + ((x0 - 8) & 15), mt, reinterpret_cast<uint32_t *>(slot_cur),
                           s_n, s_cnt_lo, s_cnt_hi, s_kbase, s_klim);
     }
 }
 
 int fast_tma_setup() {
-    return (int)cudaFuncSetAttribute(fast_nms_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, F2_TMA_SMEM);
+    cudaError_t e = cudaFuncSetAttribute(fast_nms_tma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, F2_TMA_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(fast_nms_tma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, F2_TMA_SMEM);
+    return (int)e;
 }
 
 void launch_fast_nms(const PlanDev *d_plan, const PlanDev &hp, WorkDev w, int f0, int nf, cudaStream_t s) {
@@ -654,7 +705,12 @@ void launch_fast_nms(const PlanDev *d_plan, const PlanDev &hp, WorkDev w, int f0
     // one CTA per (tile, frame): the block scheduler hands the next tile to whichever CTA slot frees first.  The cost of a
     // tile varies with its candidates, and a persistent grid of 3 CTAs per SM walking a fixed share of the tiles finished
     // later (H100, 64 x 1080p: 1.51 ms against 1.68 ms, DESIGN.md §4.2).
-    launch_k(fast_nms_tma_kernel, dim3(nwork), dim3(256), F2_TMA_SMEM, s, hp.pdl != 0, d_plan, w, f0, nwork);
+    launch_k(fast_nms_tma_kernel<false>, dim3(nwork), dim3(256), F2_TMA_SMEM, s, hp.pdl != 0, d_plan, w, f0, nwork);
+}
+
+void launch_fast_nms_multi(const MultiPlanDev *d_plan, const MultiPlanDev &hp, WorkDev w, cudaStream_t s) {
+    if (hp.nfwork == 0) return;
+    launch_k(fast_nms_tma_kernel<true>, dim3(hp.nfwork), dim3(256), F2_TMA_SMEM, s, hp.pdl != 0, d_plan, w, 0, hp.nfwork);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -666,11 +722,19 @@ __device__ __forceinline__ int warp_sum(int v) {
     return v;
 }
 
-__global__ void __launch_bounds__(32) cell_quota_kernel(const PlanDev *__restrict__ plan, WorkDev wk, int f0) {
+// Multi plan: the first level-table entry of the group that holds work frame f
+__device__ __forceinline__ int group_levels(const MultiPlanDev *plan, int f) {
+    return group_of<&GroupDev::frame0>(plan, f) * plan->nlevels;
+}
+
+template <bool kMulti>
+__global__ void __launch_bounds__(32) cell_quota_kernel(const PlanOf<kMulti> *__restrict__ plan, WorkDev wk, int f0) {
     pdl_prologue();
     __shared__ uint32_t no_more[128];  // bitmap, up to 4096 cells per level
     const int l = blockIdx.x, f = blockIdx.y + f0;
-    const LevelDev &L = plan->lv[l];
+    int v0 = 0;
+    if constexpr (kMulti) v0 = group_levels(plan, f);
+    const LevelDev &L = plan->lv[v0 + l];
     const int lane = threadIdx.x;
     const int nCells = L.ncells, nfc = L.nfc;
     const size_t fb = (size_t)f * plan->ncells_total + L.cell_base;
@@ -721,7 +785,11 @@ __global__ void __launch_bounds__(32) cell_quota_kernel(const PlanDev *__restric
 
 void launch_cell_quota(const PlanDev *d_plan, const PlanDev &hp, WorkDev w, int f0, int nf, cudaStream_t s) {
     dim3 grid(hp.nlevels, nf);
-    launch_k(cell_quota_kernel, grid, dim3(32), 0, s, hp.pdl != 0, d_plan, w, f0);
+    launch_k(cell_quota_kernel<false>, grid, dim3(32), 0, s, hp.pdl != 0, d_plan, w, f0);
+}
+
+void launch_cell_quota_multi(const MultiPlanDev *d_plan, const MultiPlanDev &hp, WorkDev w, cudaStream_t s) {
+    launch_k(cell_quota_kernel<true>, dim3(hp.nlevels, hp.nframes), dim3(32), 0, s, hp.pdl != 0, d_plan, w, 0);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -732,18 +800,27 @@ void launch_cell_quota(const PlanDev *d_plan, const PlanDev &hp, WorkDev w, int 
 //   score(8) << 36 | (4095 - cell)(12) << 24 | (0xFFFFFF - raster)(24).
 // ------------------------------------------------------------------------------------------------
 #define CS_LIST 256   // candidates sharing the score at the cut that are ranked directly
-__global__ void __launch_bounds__(128) cell_select_kernel(const PlanDev *__restrict__ plan, WorkDev wk, int f0) {
+template <bool kMulti>
+__global__ void __launch_bounds__(128) cell_select_kernel(const PlanOf<kMulti> *__restrict__ plan, WorkDev wk, int f0) {
     pdl_prologue();
     __shared__ int hist[256];
     __shared__ uint32_t s_prefix, s_mask, s_list[CS_LIST];
     __shared__ int s_k, s_base, s_fill, s_bin_cnt, s_ln;
 
-    const int gcell = blockIdx.x, f = blockIdx.y + f0;
+    int gcell = blockIdx.x, f = blockIdx.y + f0, v0 = 0;
+    if constexpr (kMulti) {   // one block per (work frame, cell of its group)
+        const int g = group_of<&GroupDev::cwork0>(plan, blockIdx.x);
+        const GroupDev &G = plan->grp[g];
+        const int r = blockIdx.x - G.cwork0;
+        gcell = G.cell0 + r % G.ncells;
+        f = G.frame0 + r / G.ncells;
+        v0 = g * plan->nlevels;
+    }
     const size_t fc = (size_t)f * plan->ncells_total + gcell;
     const int keep = wk.cell_keep[fc];
     if (keep <= 0) return;
-    const int l = find_level_by(plan, gcell, 2);
-    const LevelDev &L = plan->lv[l];
+    const int l = find_level_by(plan, gcell, 2, v0);
+    const LevelDev &L = plan->lv[v0 + l];
     const int n = min(wk.cell_cnt_lo[fc], wk.cell_cand_cap[gcell]);
     const uint32_t min_key = wk.cell_min_key[fc];
     const uint32_t *__restrict__ keys = wk.cand_keys + (size_t)f * plan->cand_total + wk.cell_cand_base[gcell];
@@ -841,8 +918,14 @@ __global__ void __launch_bounds__(128) cell_select_kernel(const PlanDev *__restr
 void launch_cell_select(const PlanDev *d_plan, const PlanDev &hp, WorkDev w, int f0, int nf, cudaStream_t s) {
     if (hp.ncells_total == 0) return;
     dim3 grid(hp.ncells_total, nf);
-    if (w.cand_keys64) { cell_select_harris_kernel<<<grid, 128, 0, s>>>(d_plan, w, f0); return; }
-    launch_k(cell_select_kernel, grid, dim3(128), 0, s, hp.pdl != 0, d_plan, w, f0);
+    if (w.cand_keys64) { cell_select_harris_kernel<false><<<grid, 128, 0, s>>>(d_plan, w, f0); return; }
+    launch_k(cell_select_kernel<false>, grid, dim3(128), 0, s, hp.pdl != 0, d_plan, w, f0);
+}
+
+void launch_cell_select_multi(const MultiPlanDev *d_plan, const MultiPlanDev &hp, WorkDev w, cudaStream_t s) {
+    if (hp.ncwork == 0) return;
+    if (w.cand_keys64) { cell_select_harris_kernel<true><<<hp.ncwork, 128, 0, s>>>(d_plan, w, 0); return; }
+    launch_k(cell_select_kernel<true>, dim3(hp.ncwork), dim3(128), 0, s, hp.pdl != 0, d_plan, w, 0);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -866,11 +949,14 @@ __device__ void bitonic_sort_desc(unsigned long long *a, int n2) {
     }
 }
 
-__global__ void __launch_bounds__(512) level_select_kernel(const PlanDev *__restrict__ plan, WorkDev wk, int f0) {
+template <bool kMulti>
+__global__ void __launch_bounds__(512) level_select_kernel(const PlanOf<kMulti> *__restrict__ plan, WorkDev wk, int f0) {
     pdl_prologue();
     extern __shared__ unsigned long long skeys[];
     const int l = blockIdx.x, f = blockIdx.y + f0;
-    const LevelDev &L = plan->lv[l];
+    int v0 = 0;
+    if constexpr (kMulti) v0 = group_levels(plan, f);
+    const LevelDev &L = plan->lv[v0 + l];
     int n = min(wk.kept_cnt[(size_t)f * plan->nlevels + l], L.kept_cap);
     int n2 = 1;
     while (n2 < n) n2 <<= 1;
@@ -913,17 +999,26 @@ __global__ void __launch_bounds__(512) level_select_kernel(const PlanDev *__rest
 // eligibility still comes from the FAST score (low byte >= the cell's threshold).  Kept entries carry
 // (order(resp), cell, raster, score); the level trim ranks by counting (n is at most a few thousand).
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) cell_select_harris_kernel(const PlanDev *__restrict__ plan, WorkDev wk, int f0) {
+template <bool kMulti>
+__global__ void __launch_bounds__(128) cell_select_harris_kernel(const PlanOf<kMulti> *__restrict__ plan, WorkDev wk, int f0) {
     __shared__ int hist[256];
     __shared__ unsigned long long s_prefix, s_mask;
     __shared__ int s_k, s_base, s_fill;
 
-    const int gcell = blockIdx.x, f = blockIdx.y + f0;
+    int gcell = blockIdx.x, f = blockIdx.y + f0, v0 = 0;
+    if constexpr (kMulti) {   // one block per (work frame, cell of its group)
+        const int g = group_of<&GroupDev::cwork0>(plan, blockIdx.x);
+        const GroupDev &G = plan->grp[g];
+        const int r = blockIdx.x - G.cwork0;
+        gcell = G.cell0 + r % G.ncells;
+        f = G.frame0 + r / G.ncells;
+        v0 = g * plan->nlevels;
+    }
     const size_t fc = (size_t)f * plan->ncells_total + gcell;
     const int keep = wk.cell_keep[fc];
     if (keep <= 0) return;
-    const int l = find_level_by(plan, gcell, 2);
-    const LevelDev &L = plan->lv[l];
+    const int l = find_level_by(plan, gcell, 2, v0);
+    const LevelDev &L = plan->lv[v0 + l];
     const int n = min(wk.cell_cnt_lo[fc], wk.cell_cand_cap[gcell]);
     const unsigned long long min_score = wk.cell_min_key[fc] >> 24;  // threshold t: eligible <=> score >= t
     const unsigned long long *__restrict__ keys = wk.cand_keys64 + (size_t)f * plan->cand_total + wk.cell_cand_base[gcell];
@@ -982,10 +1077,13 @@ __global__ void __launch_bounds__(128) cell_select_harris_kernel(const PlanDev *
     }
 }
 
-__global__ void __launch_bounds__(512) level_select_harris_kernel(const PlanDev *__restrict__ plan, WorkDev wk, int f0) {
+template <bool kMulti>
+__global__ void __launch_bounds__(512) level_select_harris_kernel(const PlanOf<kMulti> *__restrict__ plan, WorkDev wk, int f0) {
     extern __shared__ unsigned long long skeys[];  // [n] hi keys, then [n] u32 lo keys, then [n] u8 survivor flags
     const int l = blockIdx.x, f = blockIdx.y + f0;
-    const LevelDev &L = plan->lv[l];
+    int v0 = 0;
+    if constexpr (kMulti) v0 = group_levels(plan, f);
+    const LevelDev &L = plan->lv[v0 + l];
     const int n = min(wk.kept_cnt[(size_t)f * plan->nlevels + l], L.kept_cap);
     uint32_t *slo = reinterpret_cast<uint32_t *>(skeys + L.kept_cap);
     uint8_t *keepf = reinterpret_cast<uint8_t *>(slo + L.kept_cap);
@@ -1030,8 +1128,20 @@ __global__ void __launch_bounds__(512) level_select_harris_kernel(const PlanDev 
 }
 
 int level_select_harris_smem_bytes(int max_kept) { return max_kept * (8 + 4 + 1) + 16; }
+// The attribute belongs to the kernel, not to a plan: it only ever grows, so that a handle's multi plan and its
+// single-geometry plan (or another handle) never lower the limit the other launches with.
+static int grow_smem_limit(std::atomic<int> &limit, int bytes) {
+    int cur = limit.load();
+    while (cur < bytes && !limit.compare_exchange_weak(cur, bytes)) {}
+    return std::max(cur, bytes);
+}
+
 int set_level_select_harris_smem(int bytes) {
-    return (int)cudaFuncSetAttribute(level_select_harris_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    static std::atomic<int> limit{0};
+    bytes = grow_smem_limit(limit, bytes);
+    cudaError_t e = cudaFuncSetAttribute(level_select_harris_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(level_select_harris_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    return (int)e;
 }
 
 int level_select_smem_bytes(int max_kept) {
@@ -1041,13 +1151,23 @@ int level_select_smem_bytes(int max_kept) {
 }
 
 int set_level_select_smem(int bytes) {
-    return (int)cudaFuncSetAttribute(level_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    static std::atomic<int> limit{0};
+    bytes = grow_smem_limit(limit, bytes);
+    cudaError_t e = cudaFuncSetAttribute(level_select_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(level_select_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    return (int)e;
 }
 
 void launch_level_select(const PlanDev *d_plan, const PlanDev &hp, WorkDev w, size_t smem_bytes, int f0, int nf, cudaStream_t s) {
     dim3 grid(hp.nlevels, nf);
-    if (w.cand_keys64) { level_select_harris_kernel<<<grid, 512, smem_bytes, s>>>(d_plan, w, f0); return; }
-    launch_k(level_select_kernel, grid, dim3(512), smem_bytes, s, hp.pdl != 0, d_plan, w, f0);
+    if (w.cand_keys64) { level_select_harris_kernel<false><<<grid, 512, smem_bytes, s>>>(d_plan, w, f0); return; }
+    launch_k(level_select_kernel<false>, grid, dim3(512), smem_bytes, s, hp.pdl != 0, d_plan, w, f0);
+}
+
+void launch_level_select_multi(const MultiPlanDev *d_plan, const MultiPlanDev &hp, WorkDev w, size_t smem_bytes, cudaStream_t s) {
+    const dim3 grid(hp.nlevels, hp.nframes);
+    if (w.cand_keys64) { level_select_harris_kernel<true><<<grid, 512, smem_bytes, s>>>(d_plan, w, 0); return; }
+    launch_k(level_select_kernel<true>, grid, dim3(512), smem_bytes, s, hp.pdl != 0, d_plan, w, 0);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1232,8 +1352,10 @@ __device__ __forceinline__ int brief_byte_fused(const __half2 *pp, float a, floa
 // PEERS: the exchange of a camera rig fused into the kernel (include/orbfe_comm.h): every keypoint / descriptor / count is
 // stored into slot [rank] of EVERY rank's gather buffer (st.global on peer pointers over NVLink) instead of one local
 // output, and the last thread block to finish publishes the epoch to every rank's flag word (release at system scope).
-template <bool PEERS>
-__device__ __forceinline__ void describe_fused_body(const PlanDev *__restrict__ plan, const WorkDev &wk,
+// kMulti: f is the call's work frame; the keypoints come from its group's levels (frame pf of their planes) and go to
+// output frame of (GroupDev::out0)
+template <bool PEERS, bool kMulti>
+__device__ __forceinline__ void describe_fused_body(const PlanOf<kMulti> *__restrict__ plan, const WorkDev &wk,
                                                     const int8_t *__restrict__ g_pattern,
                                                     OrbfeKeyPoint *__restrict__ out_kps,
                                                     uint8_t *__restrict__ out_desc, int *__restrict__ out_counts, int f0,
@@ -1252,12 +1374,19 @@ __device__ __forceinline__ void describe_fused_body(const PlanDev *__restrict__ 
     const int lane = threadIdx.x & 31;
     const int slot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int nlev = plan->nlevels;
+    int v0 = 0, pf = f, of = f;
+    if constexpr (kMulti) {
+        const GroupDev &G = plan->grp[group_of<&GroupDev::frame0>(plan, f)];
+        v0 = (int)(&G - plan->grp) * nlev;
+        pf = f - G.frame0;
+        of = G.out0 + pf;
+    }
     const int *__restrict__ lcnt = wk.level_cnt + (size_t)f * nlev;
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         int tot = 0;
         for (int k = 0; k < nlev; k++) tot += lcnt[k];
         if (PEERS) { for (int p = 0; p < po.n; p++) po.counts[p][f] = tot; }
-        else out_counts[f] = tot;
+        else out_counts[of] = tot;
     }
     if (slot >= plan->nfeatures) return;
     // level of this slot and its position in the frame's output, warp-cooperatively: lane k holds level k's slot
@@ -1265,7 +1394,7 @@ __device__ __forceinline__ void describe_fused_body(const PlanDev *__restrict__ 
     const int base_k = lane < nlev ? plan->lv[lane].kp_base : 0x7FFFFFFF;
     const int cnt_k = lane < nlev ? lcnt[lane] : 0;
     const int l = 31 - __clz(__ballot_sync(0xffffffffu, slot >= base_k));
-    const LevelDev &L = plan->lv[l];
+    const LevelDev &L = plan->lv[v0 + l];
     const int idx = slot - __shfl_sync(0xffffffffu, base_k, l);
     if (idx >= __shfl_sync(0xffffffffu, cnt_k, l)) return;
     const int out_idx = idx + warp_sum(lane < l ? cnt_k : 0);
@@ -1273,7 +1402,7 @@ __device__ __forceinline__ void describe_fused_body(const PlanDev *__restrict__ 
     const int2 kp = wk.kp_xy_score[(size_t)f * plan->nfeatures + slot];
     const int x = kp.x & 0xFFFF, y = kp.x >> 16;
     const int w = L.w, h = L.h, pitch = L.pitch;
-    const uint8_t *__restrict__ img = L.pyr + (size_t)f * L.plane;
+    const uint8_t *__restrict__ img = L.pyr + (size_t)pf * L.plane;
 
     uint32_t *rawW = patch + (threadIdx.x >> 5) * DF_WARP_WORDS;   // [43][13] words
     uint32_t *vpW = rawW + DF_ROWS * DF_RW + 1;                    // [37][24] words = [37][48] u16 (8-byte aligned)
@@ -1390,7 +1519,7 @@ __device__ __forceinline__ void describe_fused_body(const PlanDev *__restrict__ 
     word |= __shfl_down_sync(0xffffffffu, (uint32_t)val, 1) << 8;
     word |= __shfl_down_sync(0xffffffffu, (uint32_t)val, 2) << 16;
     word |= __shfl_down_sync(0xffffffffu, (uint32_t)val, 3) << 24;
-    const size_t o = (size_t)f * plan->nfeatures + out_idx;
+    const size_t o = (size_t)of * plan->nfeatures + out_idx;
     if (PEERS) {
         // remote stores over NVLink: 16-byte descriptor halves from lanes 0 and 16, the seven keypoint fields from lanes 0..6
         // (one coalesced 28-byte segment per destination) -- every lane holds the same keypoint values
@@ -1420,14 +1549,15 @@ __device__ __forceinline__ void describe_fused_body(const PlanDev *__restrict__ 
     }
 }
 
-__global__ void __launch_bounds__(256) describe_fused_kernel(const PlanDev *__restrict__ plan, WorkDev wk,
+template <bool kMulti>
+__global__ void __launch_bounds__(256) describe_fused_kernel(const PlanOf<kMulti> *__restrict__ plan, WorkDev wk,
                                                              const int8_t *__restrict__ g_pattern,
                                                              OrbfeKeyPoint *__restrict__ out_kps,
                                                              uint8_t *__restrict__ out_desc, int *__restrict__ out_counts, int f0) {
     pdl_prologue();
     PeerOut none;
     none.n = 0;
-    describe_fused_body<false>(plan, wk, g_pattern, out_kps, out_desc, out_counts, f0, none);
+    describe_fused_body<false, kMulti>(plan, wk, g_pattern, out_kps, out_desc, out_counts, f0, none);
 }
 
 __global__ void __launch_bounds__(256) describe_fused_exchange_kernel(const PlanDev *__restrict__ plan, WorkDev wk,
@@ -1446,7 +1576,7 @@ __global__ void __launch_bounds__(256) describe_fused_exchange_kernel(const Plan
         } while (true);
     }
     __syncthreads();
-    describe_fused_body<true>(plan, wk, g_pattern, nullptr, nullptr, nullptr, f0, po);
+    describe_fused_body<true, false>(plan, wk, g_pattern, nullptr, nullptr, nullptr, f0, po);
     // ---- publish.  The block barrier orders every warp's remote stores before thread 0, whose RELEASE increment of the arrival
     //      counter (gpu scope: the counter is only read by this GPU's blocks) is cumulative over them.  The last block to
     //      arrive has read the counter after all the others' releases; its acq_rel fence at SYSTEM scope then orders all of that
@@ -1471,7 +1601,13 @@ void launch_describe_fused(const PlanDev *d_plan, const PlanDev &hp, WorkDev w, 
     dim3 grid((hp.nfeatures + 7) / 8, nf);
     if (grid.x == 0) grid.x = 1;
     if (peers && peers->n > 0) { describe_fused_exchange_kernel<<<grid, 256, 0, s>>>(d_plan, w, d_pattern, f0, *peers); return; }
-    launch_k(describe_fused_kernel, grid, dim3(256), 0, s, hp.pdl != 0, d_plan, w, d_pattern, d_kps, d_desc, d_counts, f0);
+    launch_k(describe_fused_kernel<false>, grid, dim3(256), 0, s, hp.pdl != 0, d_plan, w, d_pattern, d_kps, d_desc, d_counts, f0);
+}
+
+void launch_describe_multi(const MultiPlanDev *d_plan, const MultiPlanDev &hp, WorkDev w, const int8_t *d_pattern,
+                           OrbfeKeyPoint *d_kps, uint8_t *d_desc, int *d_counts, cudaStream_t s) {
+    const dim3 grid(std::max((hp.nfeatures + 7) / 8, 1), hp.nframes);
+    launch_k(describe_fused_kernel<true>, grid, dim3(256), 0, s, hp.pdl != 0, d_plan, w, d_pattern, d_kps, d_desc, d_counts, 0);
 }
 
 }  // namespace orbfe

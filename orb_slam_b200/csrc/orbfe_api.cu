@@ -19,6 +19,8 @@
 #include <utility>
 #include <vector>
 #include <atomic>
+#include <climits>
+#include <memory>
 #include <thread>
 #include <unordered_map>
 
@@ -98,10 +100,24 @@ struct OrbfeExtractor {
     int *h_err = nullptr;     // pinned
     size_t h_counts_cap = 0;
 
+    // multi plan (orbfe_extract_multi): keyed by the (W, H) list of its groups, holding mcap[g] frames of group g
+    std::vector<int> mgeom, mcap;
+    MultiPlanDev *mhp = nullptr;     // host copy (large: on the heap)
+    MultiPlanDev *mdp = nullptr;
+    WorkDev mwork;
+    DeviceBuffers mplan_mem;
+    void *mcounters = nullptr;
+    size_t mcounters_bytes = 0, mls_smem = 0;
+    LevelDev mown0[ORBFE_MULTI_MAX_GROUPS];   // each group's level 0 in the plan's own planes
+    OrbfeKeyPoint *md_kps = nullptr;          // own outputs (host-API path), [sum of mcap] frames
+    uint8_t *md_desc = nullptr;
+    int *md_counts = nullptr;
+
     HandleStream hs;             // every call enters and leaves it, whichever stream it is enqueued on
     cudaStream_t copy_stream = nullptr;
     std::vector<cudaEvent_t> chunk_ev;
     int last_launches = 0;
+    int plan_builds = 0;
     bool profiling = false;
     StageTimer timer;
     std::vector<float> stage_ms;
@@ -117,6 +133,29 @@ static void free_plan(OrbfeExtractor *ex) {
     ex->d_desc = nullptr;
     ex->d_counts = nullptr;
     ex->W = ex->H = ex->Bcap = 0;
+}
+
+static void free_multi_plan(OrbfeExtractor *ex) {
+    ex->mplan_mem.release();
+    ex->mdp = nullptr;
+    ex->mcounters = nullptr;
+    ex->md_kps = nullptr;
+    ex->md_desc = nullptr;
+    ex->md_counts = nullptr;
+    ex->mgeom.clear();
+    ex->mcap.clear();
+}
+
+// the pinned block the host-array entries read the counts back into
+static int grow_host_counts(OrbfeExtractor *ex, int n) {
+    if (ex->h_counts_cap < (size_t)n) {
+        if (ex->h_counts) cudaFreeHost(ex->h_counts);
+        ex->h_counts = nullptr;
+        ex->h_counts_cap = 0;
+        ORBFE_CUDA_TRY(cudaHostAlloc((void **)&ex->h_counts, sizeof(int) * n, cudaHostAllocDefault));
+        ex->h_counts_cap = n;
+    }
+    return ORBFE_OK;
 }
 
 // cv::resize INTER_LINEAR tap tables for one axis (OpenCV imgproc resize.cpp semantics, see SURVEY 8c)
@@ -152,41 +191,24 @@ static CUresult encode_level_map(void *encode, CUtensorMap *map, uint8_t *ptr, i
                               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
-static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
-    if (ex->W == W && ex->H == H && B <= ex->Bcap) return ORBFE_OK;
-    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
-    ORBFE_CUDA_TRY(cudaEventSynchronize(ex->hs.last));   // the handle's pending calls still use the plan
-    free_plan(ex);
-    PlanDev &P = ex->hplan;
-    memset(&P, 0, sizeof(P));
-    P.nlevels = ex->nlevels;
-    P.batch = B;
-    P.nfeatures = ex->nfeatures;
-    // cv::FAST keeps a pixel only if its score is strictly above all 8 neighbours', and a non-corner scores 0: a corner of
-    // score 0 (a pixel that is a corner at threshold 0 only) is never kept and suppresses nothing.  Threshold 0 therefore
-    // detects exactly what threshold 1 detects; the kernel, whose NMS input is m - t_lo, runs it as 1.
-    const int th = std::max(ex->fast_th, 1);
-    P.t_lo = std::min(th, 7);
-    P.t_hi = std::max(th, 7);
-    P.t1_is_lo = th <= 7;
-    P.score_type = ex->score_type;
-    {   // programmatic dependent launch of the pipeline's kernels (extract_kernels.cu, pdl_prologue); ORBFE_PDL=0 turns it off
-        const char *e = getenv("ORBFE_PDL");
-        P.pdl = !(e && *e == '0');
-    }
-    {   // HarrisResponses scale (ORBextractor.cc:90-92)
-        float scale = (float)(1 << 2) * (float)7 * 255.0f;
-        scale = 1.0f / scale;
-        P.harris_scale4 = scale * scale * scale * scale;
-    }
+// Running totals of a level table being laid out.  Cell ids and FAST / blur tiles run on across the geometries of a multi
+// plan; candidate slots, kept lists and keypoint slots restart at 0 in each geometry, so the per-frame strides are the
+// largest geometry's.
+struct PlanLayout {
+    int cell_base = 0, ft_base = 0, bt_base = 0, max_kept = 0, kept_total = 0, kp_total = 0;
+    long long cand_total = 0;
+    std::vector<long long> cand_base;   // [cells] first candidate slot of each cell inside its frame
+    std::vector<int> cand_cap;          // [cells]
+};
 
+// The levels of one W x H geometry in lv[0, nlevels): sizes, cell grid, bases, tile counts and candidate slots.  Host only:
+// nothing is allocated or launched.  ORBFE_ERR_UNSUPPORTED for a geometry outside the supported domain.
+static int layout_geometry(const OrbfeExtractor *ex, int W, int H, LevelDev *lv, PlanLayout &A) {
     const float ratio = (float)W / (float)H;  // :527 (level-0 dims)
-    int cell_base = 0, kp_base = 0, kept_base = 0, ft_base = 0, bt_base = 0, max_kept = 0;
-    std::vector<long long> cand_base;
-    std::vector<int> cand_cap;
+    int kp_base = 0, kept_base = 0;
     long long cand_total = 0;
     for (int l = 0; l < ex->nlevels; l++) {
-        LevelDev &L = P.lv[l];
+        LevelDev &L = lv[l];
         L.w = cv_round((double)((float)W * ex->inv_scale[l]));  // :785-786
         L.h = cv_round((double)((float)H * ex->inv_scale[l]));
         if (L.w < 1 || L.h < 1 || L.w > 65535 || L.h > 32767)
@@ -228,58 +250,69 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
             if (L.ncells > 4096 || (long long)L.cw * L.ch > (1 << 24))
                 return fail(ORBFE_ERR_UNSUPPORTED, "level %d: %d cells of %dx%d exceed the key layout", l, L.ncells, L.cw, L.ch);
         }
-        L.cell_base = cell_base;
-        cell_base += L.ncells;
+        L.cell_base = A.cell_base;
+        A.cell_base += L.ncells;
         L.kp_base = kp_base;
         kp_base += L.quota;
         L.kept_base = kept_base;
         L.kept_cap = L.quota + 2 * L.ncells + 64;
         kept_base += L.kept_cap;
-        max_kept = std::max(max_kept, L.kept_cap);
+        A.max_kept = std::max(A.max_kept, L.kept_cap);
         L.ftiles_x = empty_level ? 0 : (Wd + ORBFE_FT_W - 1) / ORBFE_FT_W;
         L.ftiles_y = empty_level ? 0 : (Hd + ORBFE_FT_H - 1) / ORBFE_FT_H;
-        L.ftile_base = ft_base;
-        ft_base += L.ftiles_x * L.ftiles_y;
+        L.ftile_base = A.ft_base;
+        A.ft_base += L.ftiles_x * L.ftiles_y;
         L.btiles_x = (L.w + ORBFE_BT_W - 1) / ORBFE_BT_W;
         L.btiles_y = (L.h + ORBFE_BT_H - 1) / ORBFE_BT_H;
-        L.btile_base = bt_base;
-        bt_base += L.btiles_x * L.btiles_y;
+        L.btile_base = A.bt_base;
+        A.bt_base += L.btiles_x * L.btiles_y;
         for (int i = 0; i < L.rows; i++)
             for (int j = 0; j < L.cols; j++) {
                 const int ww = (j == L.cols - 1) ? Wd - j * L.cw : L.cw;
                 const int hh = (i == L.rows - 1) ? Hd - i * L.ch : L.ch;
                 const int cap = std::max(1, ((ww + 1) / 2) * ((hh + 1) / 2));  // strict 8-neighbour maxima bound
-                cand_base.push_back(cand_total);
-                cand_cap.push_back(cap);
+                A.cand_base.push_back(cand_total);
+                A.cand_cap.push_back(cap);
                 cand_total += cap;
             }
     }
-    P.ncells_total = cell_base;
-    P.nftiles_total = ft_base;
-    P.nbtiles_total = bt_base;
-    P.kept_total = kept_base;
-    P.cand_total = cand_total;
+    A.cand_total = std::max(A.cand_total, cand_total);
+    A.kept_total = std::max(A.kept_total, kept_base);
     // keypoint slots = sum of the per-level quotas; equals nfeatures whenever the last-level remainder
     // max(nfeatures - sum, 0) is not clipped (:487)
-    P.nfeatures = kp_base;
+    A.kp_total = kp_base;
+    return ORBFE_OK;
+}
 
-    ex->ls_smem = ex->score_type == 0 ? (size_t)level_select_harris_smem_bytes(max_kept) : (size_t)level_select_smem_bytes(max_kept);
-    if (ex->ls_smem > 200 * 1024)
-        return fail(ORBFE_ERR_UNSUPPORTED, "nfeatures too large for the level-select kernel (%zu B smem)", ex->ls_smem);
+// Shared memory of the level-select kernels for a plan whose largest kept list is max_kept; the kernels' attribute only ever
+// grows (it is per process, and another plan may need more)
+static int level_select_smem(const OrbfeExtractor *ex, int max_kept, size_t *bytes) {
+    *bytes = ex->score_type == 0 ? (size_t)level_select_harris_smem_bytes(max_kept) : (size_t)level_select_smem_bytes(max_kept);
+    if (*bytes > 200 * 1024)
+        return fail(ORBFE_ERR_UNSUPPORTED, "nfeatures too large for the level-select kernel (%zu B smem)", *bytes);
+    return ORBFE_OK;
+}
 
-    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
-    if (ex->ls_smem > 48 * 1024) {
-        cudaError_t e = (cudaError_t)(ex->score_type == 0 ? set_level_select_harris_smem((int)ex->ls_smem) : set_level_select_smem((int)ex->ls_smem));
+static int set_level_select_attr(const OrbfeExtractor *ex, size_t bytes) {
+    if (bytes > 48 * 1024) {
+        cudaError_t e = (cudaError_t)(ex->score_type == 0 ? set_level_select_harris_smem((int)bytes) : set_level_select_smem((int)bytes));
         if (e != cudaSuccess) return fail(ORBFE_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     }
-    // ---- device memory ----
+    return ORBFE_OK;
+}
+
+// Device part of one geometry laid out in lv[0, nlevels) (entries v0 .. v0 + nlevels - 1 of the level table): the level
+// planes for B frames (level 0 too: it serves callers whose frames cannot be read in place), the resize tables, and the
+// geometry's FAST and blur tile entries and tensor maps, written into the plan's tables.
+static int alloc_geometry(OrbfeExtractor *ex, DeviceBuffers &mem, LevelDev *lv, int B, int v0, void *encode,
+                          std::vector<FTileInfo> &info, std::vector<BTileInfo> &binfo, std::vector<CUtensorMap> &maps) {
     for (int l = 0; l < ex->nlevels; l++) {
-        LevelDev &L = P.lv[l];
-        ORBFE_CUDA_TRY(ex->plan_mem.alloc(&L.pyr, L.plane * B + 256));
-        ORBFE_CUDA_TRY(ex->plan_mem.alloc(&L.blur, L.plane + 256));  // one plane, for orbfe_debug_read_level
+        LevelDev &L = lv[l];
+        ORBFE_CUDA_TRY(mem.alloc(&L.pyr, L.plane * B + 256));
+        ORBFE_CUDA_TRY(mem.alloc(&L.blur, L.plane + 256));  // one plane, for orbfe_debug_read_level
         ORBFE_CUDA_TRY(cudaMemsetAsync(L.pyr, 0, L.plane * B + 256, ex->hs.stream));
         if (l > 0) {
-            const LevelDev &S = P.lv[l - 1];
+            const LevelDev &S = lv[l - 1];
             std::vector<int> xo, yo;
             std::vector<short2> xab, yab;
             resize_axis(L.w, S.w, true, xo, xab);
@@ -300,10 +333,10 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
                     if (xo[x4 + 2] - (xo[x4] & ~3) > 6) L.rz_fast = 1;
             }
             int *dxo; short2 *dxab; int2 *dyr; short2 *dyab;
-            ORBFE_CUDA_TRY(ex->plan_mem.alloc(&dxo, xo.size()));
-            ORBFE_CUDA_TRY(ex->plan_mem.alloc(&dxab, xab.size()));
-            ORBFE_CUDA_TRY(ex->plan_mem.alloc(&dyr, (size_t)L.h));
-            ORBFE_CUDA_TRY(ex->plan_mem.alloc(&dyab, (size_t)L.h));
+            ORBFE_CUDA_TRY(mem.alloc(&dxo, xo.size()));
+            ORBFE_CUDA_TRY(mem.alloc(&dxab, xab.size()));
+            ORBFE_CUDA_TRY(mem.alloc(&dyr, (size_t)L.h));
+            ORBFE_CUDA_TRY(mem.alloc(&dyab, (size_t)L.h));
             ORBFE_CUDA_TRY(cudaMemcpy(dxo, xo.data(), sizeof(int) * xo.size(), cudaMemcpyHostToDevice));
             ORBFE_CUDA_TRY(cudaMemcpy(dxab, xab.data(), sizeof(short2) * xab.size(), cudaMemcpyHostToDevice));
             ORBFE_CUDA_TRY(cudaMemcpy(dyr, yr.data(), sizeof(int2) * L.h, cudaMemcpyHostToDevice));
@@ -311,117 +344,160 @@ static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
             L.xofs = dxo; L.xab = dxab; L.yrows = dyr; L.yab = dyab;
         }
     }
-    WorkDev &Wk = ex->work;
+    // per-tile cell geometry for the FAST kernel
+    for (int l = 0; l < ex->nlevels; l++) {
+        const LevelDev &L = lv[l];
+        const int xmax = L.w - ORBFE_EDGE, ymax = L.h - ORBFE_EDGE;
+        for (int ty = 0; ty < L.ftiles_y; ty++)
+            for (int tx = 0; tx < L.ftiles_x; tx++) {
+                FTileInfo &T = info[(size_t)L.ftile_base + ty * L.ftiles_x + tx];
+                const int x0 = ORBFE_EDGE + tx * ORBFE_FT_W, y0 = ORBFE_EDGE + ty * ORBFE_FT_H;
+                const int x1 = std::min(x0 + ORBFE_FT_W, xmax) - 1, y1 = std::min(y0 + ORBFE_FT_H, ymax) - 1;
+                const int cj0 = std::min((x0 - ORBFE_EDGE) / L.cw, L.cols - 1), cj1 = std::min((x1 - ORBFE_EDGE) / L.cw, L.cols - 1);
+                const int ci0 = std::min((y0 - ORBFE_EDGE) / L.ch, L.rows - 1), ci1 = std::min((y1 - ORBFE_EDGE) / L.ch, L.rows - 1);
+                T.cj0 = (short)cj0; T.ci0 = (short)ci0; T.ncj = (short)(cj1 - cj0 + 1); T.nci = (short)(ci1 - ci0 + 1);
+                T.level = (short)(v0 + l); T.tx = (short)tx; T.ty = (short)ty; T.pad = 0;
+                // interior cell boundaries: y = 16 + ci*ch (ci >= 1) and x = 16 + cj*cw (cj >= 1)
+                T.hmask = 0;
+                for (int r = 0; r < ORBFE_FT_H + 2; r++) {
+                    const int y = y0 - 1 + r;
+                    const int d = y - ORBFE_EDGE;
+                    if (d >= L.ch && d % L.ch == 0 && d / L.ch <= L.rows - 1) T.hmask |= 1ull << r;
+                }
+                for (int w = 0; w < 4; w++) T.vmask[w] = 0;
+                for (int c = 0; c < 128; c++) {
+                    const int d = x0 - 4 + c - ORBFE_EDGE;
+                    if (d >= L.cw && d % L.cw == 0 && d / L.cw <= L.cols - 1) T.vmask[c >> 5] |= 1u << (c & 31);
+                }
+                if (T.ncj * T.nci > 64) return fail(ORBFE_ERR_UNSUPPORTED, "level %d: a FAST tile overlaps %d cells", l, T.ncj * T.nci);
+            }
+        for (int ty = 0; ty < L.btiles_y; ty++)
+            for (int tx = 0; tx < L.btiles_x; tx++) {
+                BTileInfo &T = binfo[(size_t)L.btile_base + ty * L.btiles_x + tx];
+                T.level = (short)(v0 + l); T.tx = (short)tx; T.ty = (short)ty; T.pad = 0;
+            }
+        // the 3-D (x, y, frame) tensor map of the level for the FAST kernel's pixel tiles
+        const CUresult r = encode_level_map(encode, &maps[v0 + l], L.pyr, L.w, L.h, B, L.pitch, L.plane);
+        if (r != CUDA_SUCCESS) return fail(ORBFE_ERR_CUDA, "cuTensorMapEncodeTiled(level %d) failed: %d", l, (int)r);
+    }
+    return ORBFE_OK;
+}
+
+static int tensor_map_encoder(void **fn) {
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", fn, cudaEnableDefault, &qres) != cudaSuccess || !*fn ||
+        qres != cudaDriverEntryPointSuccess)
+        return fail(ORBFE_ERR_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
+    return ORBFE_OK;
+}
+
+// The tile and candidate tables, the tensor maps and the per-frame work buffers for B frames at P's strides.  The counters
+// (cell_cnt_lo | cell_cnt_hi | kept_cnt, zeroed per call) are one allocation: *counters, *counters_bytes.
+template <class T>
+static int upload(DeviceBuffers &mem, const std::vector<T> &v, const T **out) {
+    T *d;
+    ORBFE_CUDA_TRY(mem.alloc(&d, v.size()));
+    ORBFE_CUDA_TRY(cudaMemcpy(d, v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice));
+    *out = d;
+    return ORBFE_OK;
+}
+
+static int alloc_work(OrbfeExtractor *ex, DeviceBuffers &mem, const PlanHead &P, int B, const PlanLayout &A,
+                      const std::vector<FTileInfo> &info, const std::vector<BTileInfo> &binfo, const std::vector<CUtensorMap> &maps,
+                      WorkDev &Wk, void **counters, size_t *counters_bytes) {
     memset(&Wk, 0, sizeof(Wk));
-    {   // per-tile cell geometry for the FAST kernel
-        std::vector<FTileInfo> info((size_t)P.nftiles_total);
-        for (int l = 0; l < ex->nlevels; l++) {
-            const LevelDev &L = P.lv[l];
-            const int xmax = L.w - ORBFE_EDGE, ymax = L.h - ORBFE_EDGE;
-            for (int ty = 0; ty < L.ftiles_y; ty++)
-                for (int tx = 0; tx < L.ftiles_x; tx++) {
-                    FTileInfo &T = info[(size_t)L.ftile_base + ty * L.ftiles_x + tx];
-                    const int x0 = ORBFE_EDGE + tx * ORBFE_FT_W, y0 = ORBFE_EDGE + ty * ORBFE_FT_H;
-                    const int x1 = std::min(x0 + ORBFE_FT_W, xmax) - 1, y1 = std::min(y0 + ORBFE_FT_H, ymax) - 1;
-                    const int cj0 = std::min((x0 - ORBFE_EDGE) / L.cw, L.cols - 1), cj1 = std::min((x1 - ORBFE_EDGE) / L.cw, L.cols - 1);
-                    const int ci0 = std::min((y0 - ORBFE_EDGE) / L.ch, L.rows - 1), ci1 = std::min((y1 - ORBFE_EDGE) / L.ch, L.rows - 1);
-                    T.cj0 = (short)cj0; T.ci0 = (short)ci0; T.ncj = (short)(cj1 - cj0 + 1); T.nci = (short)(ci1 - ci0 + 1);
-                    T.level = (short)l; T.tx = (short)tx; T.ty = (short)ty; T.pad = 0;
-                    // interior cell boundaries: y = 16 + ci*ch (ci >= 1) and x = 16 + cj*cw (cj >= 1)
-                    T.hmask = 0;
-                    for (int r = 0; r < ORBFE_FT_H + 2; r++) {
-                        const int y = y0 - 1 + r;
-                        const int d = y - ORBFE_EDGE;
-                        if (d >= L.ch && d % L.ch == 0 && d / L.ch <= L.rows - 1) T.hmask |= 1ull << r;
-                    }
-                    for (int w = 0; w < 4; w++) T.vmask[w] = 0;
-                    for (int c = 0; c < 128; c++) {
-                        const int d = x0 - 4 + c - ORBFE_EDGE;
-                        if (d >= L.cw && d % L.cw == 0 && d / L.cw <= L.cols - 1) T.vmask[c >> 5] |= 1u << (c & 31);
-                    }
-                    if (T.ncj * T.nci > 64) return fail(ORBFE_ERR_UNSUPPORTED, "level %d: a FAST tile overlaps %d cells", l, T.ncj * T.nci);
-                }
-        }
-        FTileInfo *d_info;
-        ORBFE_CUDA_TRY(ex->plan_mem.alloc(&d_info, info.size()));
-        ORBFE_CUDA_TRY(cudaMemcpy(d_info, info.data(), sizeof(FTileInfo) * info.size(), cudaMemcpyHostToDevice));
-        Wk.ftile_info = d_info;
-        std::vector<BTileInfo> binfo((size_t)P.nbtiles_total);
-        for (int l = 0; l < ex->nlevels; l++) {
-            const LevelDev &L = P.lv[l];
-            for (int ty = 0; ty < L.btiles_y; ty++)
-                for (int tx = 0; tx < L.btiles_x; tx++) {
-                    BTileInfo &T = binfo[(size_t)L.btile_base + ty * L.btiles_x + tx];
-                    T.level = (short)l; T.tx = (short)tx; T.ty = (short)ty; T.pad = 0;
-                }
-        }
-        BTileInfo *d_binfo;
-        ORBFE_CUDA_TRY(ex->plan_mem.alloc(&d_binfo, binfo.size()));
-        ORBFE_CUDA_TRY(cudaMemcpy(d_binfo, binfo.data(), sizeof(BTileInfo) * binfo.size(), cudaMemcpyHostToDevice));
-        Wk.btile_info = d_binfo;
-    }
-    long long *d_cb; int *d_cc;
-    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&d_cb, cand_base.size()));
-    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&d_cc, cand_cap.size()));
-    ORBFE_CUDA_TRY(cudaMemcpy(d_cb, cand_base.data(), sizeof(long long) * cand_base.size(), cudaMemcpyHostToDevice));
-    ORBFE_CUDA_TRY(cudaMemcpy(d_cc, cand_cap.data(), sizeof(int) * cand_cap.size(), cudaMemcpyHostToDevice));
-    Wk.cell_cand_base = d_cb;
-    Wk.cell_cand_cap = d_cc;
-    // ---- TMA tensor maps (one per level: x, y, frame) for the FAST kernel's pixel tiles ----
-    {
-        void *fn = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn ||
-            qres != cudaDriverEntryPointSuccess)
-            return fail(ORBFE_ERR_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
-        std::vector<CUtensorMap> maps(ex->nlevels);
-        for (int l = 0; l < ex->nlevels; l++) {
-            const LevelDev &L = P.lv[l];
-            const CUresult r = encode_level_map(fn, &maps[l], L.pyr, L.w, L.h, B, L.pitch, L.plane);
-            if (r != CUDA_SUCCESS) return fail(ORBFE_ERR_CUDA, "cuTensorMapEncodeTiled(level %d) failed: %d", l, (int)r);
-        }
-        CUtensorMap *d_maps;
-        ORBFE_CUDA_TRY(ex->plan_mem.alloc(&d_maps, maps.size()));
-        ORBFE_CUDA_TRY(cudaMemcpy(d_maps, maps.data(), sizeof(CUtensorMap) * maps.size(), cudaMemcpyHostToDevice));
-        Wk.tmaps = d_maps;
-        ex->tma_encode = fn;
-        ex->d_maps = d_maps;
-        cudaError_t e = (cudaError_t)fast_tma_setup();
-        if (e != cudaSuccess) return fail(ORBFE_ERR_CUDA, "cudaFuncSetAttribute(fast_nms_tma_kernel): %s", cudaGetErrorString(e));
-    }
-    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.cand_keys, (size_t)cand_total * B));
+    if (int rc = upload(mem, info, &Wk.ftile_info)) return rc;
+    if (int rc = upload(mem, binfo, &Wk.btile_info)) return rc;
+    if (int rc = upload(mem, A.cand_base, &Wk.cell_cand_base)) return rc;
+    if (int rc = upload(mem, A.cand_cap, &Wk.cell_cand_cap)) return rc;
+    if (int rc = upload(mem, maps, &Wk.tmaps)) return rc;
+    cudaError_t e = (cudaError_t)fast_tma_setup();
+    if (e != cudaSuccess) return fail(ORBFE_ERR_CUDA, "cudaFuncSetAttribute(fast_nms_tma_kernel): %s", cudaGetErrorString(e));
+    ORBFE_CUDA_TRY(mem.alloc(&Wk.cand_keys, (size_t)P.cand_total * B));
     if (ex->score_type == 0) {
-        ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.cand_keys64, (size_t)cand_total * B));
-        ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.kept_aux, (size_t)P.kept_total * B));
+        ORBFE_CUDA_TRY(mem.alloc(&Wk.cand_keys64, (size_t)P.cand_total * B));
+        ORBFE_CUDA_TRY(mem.alloc(&Wk.kept_aux, (size_t)P.kept_total * B));
     }
     const size_t nc = (size_t)P.ncells_total * B, nl = (size_t)P.nlevels * B;
     int *cnt;
-    ex->counters_bytes = sizeof(int) * (2 * nc + nl);
-    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&cnt, 2 * nc + nl));
-    ex->counters = cnt;
+    *counters_bytes = sizeof(int) * (2 * nc + nl);
+    ORBFE_CUDA_TRY(mem.alloc(&cnt, 2 * nc + nl));
+    *counters = cnt;
     Wk.cell_cnt_lo = cnt;
     Wk.cell_cnt_hi = cnt + nc;
     Wk.kept_cnt = cnt + 2 * nc;
-    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.cell_keep, nc));
-    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.cell_min_key, nc));
-    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.kept_keys, (size_t)P.kept_total * B));
-    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.kp_xy_score, (size_t)std::max(P.nfeatures, 1) * B));
-    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.level_cnt, nl));
-    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&Wk.err_flag, 1));
+    ORBFE_CUDA_TRY(mem.alloc(&Wk.cell_keep, nc));
+    ORBFE_CUDA_TRY(mem.alloc(&Wk.cell_min_key, nc));
+    ORBFE_CUDA_TRY(mem.alloc(&Wk.kept_keys, (size_t)P.kept_total * B));
+    ORBFE_CUDA_TRY(mem.alloc(&Wk.kp_xy_score, (size_t)std::max(P.nfeatures, 1) * B));
+    ORBFE_CUDA_TRY(mem.alloc(&Wk.level_cnt, nl));
+    ORBFE_CUDA_TRY(mem.alloc(&Wk.err_flag, 1));
     ORBFE_CUDA_TRY(cudaMemsetAsync(Wk.err_flag, 0, sizeof(int), ex->hs.stream));
+    return ORBFE_OK;
+}
+
+// The head of a plan for this handle: thresholds, score type, PDL switch
+static void plan_head(const OrbfeExtractor *ex, PlanHead &P, int B) {
+    P.nlevels = ex->nlevels;
+    P.batch = B;
+    // cv::FAST keeps a pixel only if its score is strictly above all 8 neighbours', and a non-corner scores 0: a corner of
+    // score 0 (a pixel that is a corner at threshold 0 only) is never kept and suppresses nothing.  Threshold 0 therefore
+    // detects exactly what threshold 1 detects; the kernel, whose NMS input is m - t_lo, runs it as 1.
+    const int th = std::max(ex->fast_th, 1);
+    P.t_lo = std::min(th, 7);
+    P.t_hi = std::max(th, 7);
+    P.t1_is_lo = th <= 7;
+    P.score_type = ex->score_type;
+    {   // programmatic dependent launch of the pipeline's kernels (extract_kernels.cu, pdl_prologue); ORBFE_PDL=0 turns it off
+        const char *e = getenv("ORBFE_PDL");
+        P.pdl = !(e && *e == '0');
+    }
+    {   // HarrisResponses scale (ORBextractor.cc:90-92)
+        float scale = (float)(1 << 2) * (float)7 * 255.0f;
+        scale = 1.0f / scale;
+        P.harris_scale4 = scale * scale * scale * scale;
+    }
+}
+
+static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
+    if (ex->W == W && ex->H == H && B <= ex->Bcap) return ORBFE_OK;
+    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
+    ORBFE_CUDA_TRY(cudaEventSynchronize(ex->hs.last));   // the handle's pending calls still use the plan
+    free_plan(ex);
+    PlanDev &P = ex->hplan;
+    memset(&P, 0, sizeof(P));
+    plan_head(ex, P, B);
+    PlanLayout A;
+    if (int rc = layout_geometry(ex, W, H, P.lv, A)) return rc;
+    P.ncells_total = A.cell_base;
+    P.nftiles_total = A.ft_base;
+    P.nbtiles_total = A.bt_base;
+    P.kept_total = A.kept_total;
+    P.cand_total = A.cand_total;
+    P.nfeatures = A.kp_total;
+    if (int rc = level_select_smem(ex, A.max_kept, &ex->ls_smem)) return rc;
+    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
+    if (int rc = set_level_select_attr(ex, ex->ls_smem)) return rc;
+    // ---- device memory ----
+    void *fn = nullptr;
+    if (int rc = tensor_map_encoder(&fn)) return rc;
+    std::vector<FTileInfo> info((size_t)P.nftiles_total);
+    std::vector<BTileInfo> binfo((size_t)P.nbtiles_total);
+    std::vector<CUtensorMap> maps(ex->nlevels);
+    if (int rc = alloc_geometry(ex, ex->plan_mem, P.lv, B, 0, fn, info, binfo, maps)) return rc;
+    if (int rc = alloc_work(ex, ex->plan_mem, P, B, A, info, binfo, maps, ex->work, &ex->counters, &ex->counters_bytes)) return rc;
+    ex->tma_encode = fn;
+    ex->d_maps = const_cast<CUtensorMap *>(ex->work.tmaps);
     ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->d_kps, (size_t)std::max(P.nfeatures, 1) * B));
     ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->d_desc, (size_t)std::max(P.nfeatures, 1) * B * 32));
     ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->d_counts, (size_t)B));
     ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->dplan, 1));
     ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->dplan, &P, sizeof(P), cudaMemcpyHostToDevice, ex->hs.stream));
-    if (ex->h_counts_cap < (size_t)B) {
-        if (ex->h_counts) cudaFreeHost(ex->h_counts);
-        ORBFE_CUDA_TRY(cudaHostAlloc((void **)&ex->h_counts, sizeof(int) * B, cudaHostAllocDefault));
-        ex->h_counts_cap = B;
-    }
+    if (int rc = grow_host_counts(ex, B)) return rc;
     ORBFE_CUDA_TRY(cudaStreamSynchronize(ex->hs.stream));
     ex->W = W; ex->H = H; ex->Bcap = B;
     ex->own_pyr0 = P.lv[0].pyr; ex->own_pitch0 = P.lv[0].pitch; ex->own_plane0 = P.lv[0].plane;
+    ex->plan_builds++;
     return ORBFE_OK;
 }
 
@@ -518,6 +594,8 @@ extern "C" int orbfe_extractor_destroy(OrbfeExtractor *ex) {
     if (ex->hs.last) cudaEventSynchronize(ex->hs.last);
     if (ex->hs.stream) cudaStreamSynchronize(ex->hs.stream);
     free_plan(ex);
+    free_multi_plan(ex);
+    delete ex->mhp;
     if (ex->d_pattern) cudaFree(ex->d_pattern);
     if (ex->h_counts) cudaFreeHost(ex->h_counts);
     if (ex->h_err) cudaFreeHost(ex->h_err);
@@ -747,6 +825,262 @@ extern "C" int orbfe_extract(OrbfeExtractor *ex, const uint8_t *img, int width, 
     return orbfe_extract_batch(ex, img, width, height, stride, stride * (size_t)std::max(height, 0), 1, kps, desc, cap, n_out);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Mixed geometries (orbfe_extract_multi*): the groups of a call run as one chain on the multi plan
+// ------------------------------------------------------------------------------------------------
+static bool group_empty(const OrbfeImageGroup &G) { return !G.imgs || G.width <= 0 || G.height <= 0; }
+
+// The argument checks of both entries, made before the handle is used; *frames = the call's frames
+static int check_groups(const OrbfeExtractor *ex, int ngroups, const OrbfeImageGroup *groups, int *frames) {
+    if (!ex) return fail(ORBFE_ERR_ARG, "ex is NULL");
+    if (ngroups < 1 || ngroups > ORBFE_MULTI_MAX_GROUPS)
+        return fail(ORBFE_ERR_ARG, "ngroups %d outside 1..%d", ngroups, ORBFE_MULTI_MAX_GROUPS);
+    if (!groups) return fail(ORBFE_ERR_ARG, "groups is NULL");
+    long long n = 0;
+    for (int g = 0; g < ngroups; g++) {
+        const OrbfeImageGroup &G = groups[g];
+        if (G.batch < 1) return fail(ORBFE_ERR_ARG, "group %d: batch %d", g, G.batch);
+        if (!group_empty(G) && G.stride < (size_t)G.width) return fail(ORBFE_ERR_ARG, "group %d: stride %zu < width %d", g, G.stride, G.width);
+        n += G.batch;
+    }
+    if (n > 65535) return fail(ORBFE_ERR_ARG, "%lld frames in one call (at most 65535: one grid row per frame)", n);
+    *frames = (int)n;
+    return ORBFE_OK;
+}
+
+// The multi plan for the non-empty groups of a call.  It is rebuilt only when their (W, H) list changes or a group has more
+// frames than the plan holds (then every group keeps at least its old capacity).  All geometries are laid out, on the host,
+// before anything is freed: a rejected group leaves both plans of the handle as they were.
+static int build_multi_plan(OrbfeExtractor *ex, int ngroups, const OrbfeImageGroup *groups) {
+    std::vector<int> geom, want, gidx;
+    for (int g = 0; g < ngroups; g++) {
+        if (group_empty(groups[g])) continue;
+        geom.push_back(groups[g].width);
+        geom.push_back(groups[g].height);
+        want.push_back(groups[g].batch);
+        gidx.push_back(g);
+    }
+    const int n = (int)want.size(), nl = ex->nlevels;
+    if (n == 0) return ORBFE_OK;
+    if (geom == ex->mgeom) {
+        bool fits = true;
+        for (int i = 0; i < n; i++) fits = fits && want[i] <= ex->mcap[i];
+        if (fits) return ORBFE_OK;
+        for (int i = 0; i < n; i++) want[i] = std::max(want[i], ex->mcap[i]);
+    }
+    std::unique_ptr<MultiPlanDev> M(new MultiPlanDev());
+    memset(M.get(), 0, sizeof(MultiPlanDev));
+    plan_head(ex, *M, 0);
+    PlanLayout A;
+    for (int i = 0; i < n; i++) {
+        if (int rc = layout_geometry(ex, geom[2 * i], geom[2 * i + 1], &M->lv[i * nl], A)) {
+            const std::string why = g_err;
+            return fail(rc, "group %d (%dx%d): %s", gidx[i], geom[2 * i], geom[2 * i + 1], why.c_str());
+        }
+        GroupDev &G = M->grp[i];
+        G.ftile0 = M->lv[i * nl].ftile_base;
+        G.nftiles = A.ft_base - G.ftile0;
+        G.cell0 = M->lv[i * nl].cell_base;
+        G.ncells = A.cell_base - G.cell0;
+    }
+    size_t ls = 0;
+    if (int rc = level_select_smem(ex, A.max_kept, &ls)) return rc;
+    M->ngroups = n;
+    M->ncells_total = A.cell_base;
+    M->nftiles_total = A.ft_base;
+    M->nbtiles_total = A.bt_base;
+    M->kept_total = A.kept_total;
+    M->cand_total = A.cand_total;
+    M->nfeatures = A.kp_total;
+    int frames = 0;
+    for (int i = 0; i < n; i++) frames += want[i];
+    M->batch = frames;
+
+    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
+    ORBFE_CUDA_TRY(cudaEventSynchronize(ex->hs.last));   // the handle's pending calls still use the plan
+    free_multi_plan(ex);
+    delete ex->mhp;
+    ex->mhp = M.release();
+    MultiPlanDev &P = *ex->mhp;
+    if (int rc = set_level_select_attr(ex, ls)) return rc;
+    ex->mls_smem = ls;
+    void *fn = nullptr;
+    if (int rc = tensor_map_encoder(&fn)) return rc;
+    std::vector<FTileInfo> info((size_t)P.nftiles_total);
+    std::vector<BTileInfo> binfo((size_t)P.nbtiles_total);
+    std::vector<CUtensorMap> maps((size_t)n * nl);
+    for (int i = 0; i < n; i++) {
+        if (int rc = alloc_geometry(ex, ex->mplan_mem, &P.lv[i * nl], want[i], i * nl, fn, info, binfo, maps)) return rc;
+        ex->mown0[i] = P.lv[i * nl];
+    }
+    if (int rc = alloc_work(ex, ex->mplan_mem, P, frames, A, info, binfo, maps, ex->mwork, &ex->mcounters, &ex->mcounters_bytes))
+        return rc;
+    ex->tma_encode = fn;
+    ORBFE_CUDA_TRY(ex->mplan_mem.alloc(&ex->md_kps, (size_t)std::max(P.nfeatures, 1) * frames));
+    ORBFE_CUDA_TRY(ex->mplan_mem.alloc(&ex->md_desc, (size_t)std::max(P.nfeatures, 1) * frames * 32));
+    ORBFE_CUDA_TRY(ex->mplan_mem.alloc(&ex->md_counts, (size_t)frames));
+    ORBFE_CUDA_TRY(ex->mplan_mem.alloc(&ex->mdp, 1));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->mdp, &P, sizeof(P), cudaMemcpyHostToDevice, ex->hs.stream));
+    ORBFE_CUDA_TRY(cudaStreamSynchronize(ex->hs.stream));
+    ex->mgeom = geom;
+    ex->mcap = want;
+    ex->plan_builds++;
+    return ORBFE_OK;
+}
+
+// Point group i's level 0 at `ptr` (the caller's frames, or the plan's own planes); stream-ordered like set_level0
+static int set_group_level0(OrbfeExtractor *ex, int i, uint8_t *ptr, int pitch, size_t plane, cudaStream_t s) {
+    const int v = i * ex->nlevels;
+    LevelDev &L0 = ex->mhp->lv[v];
+    if (L0.pyr == ptr && L0.pitch == pitch && L0.plane == plane) return ORBFE_OK;
+    L0.pyr = ptr; L0.pitch = pitch; L0.plane = plane;
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(&ex->mdp->lv[v], &L0, sizeof(LevelDev), cudaMemcpyHostToDevice, s));
+    CUtensorMap m;
+    const CUresult r = encode_level_map(ex->tma_encode, &m, ptr, L0.w, L0.h, ex->mcap[i], pitch, plane);
+    if (r != CUDA_SUCCESS) return fail(ORBFE_ERR_CUDA, "cuTensorMapEncodeTiled(group %d level 0) failed: %d", i, (int)r);
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(const_cast<CUtensorMap *>(ex->mwork.tmaps) + v, &m, sizeof(m), cudaMemcpyHostToDevice, s));
+    return ORBFE_OK;
+}
+
+// On s, after the handle's earlier calls: this call's frame and work ranges of the planned groups, their level 0 (device
+// frames read in place when base and strides are 16-byte aligned, else copied, host frames uploaded into the plan's own
+// planes) and the zeroed counters.  Device outputs (d_counts != NULL): a group's frames are written at their place in the
+// call, and the counts of empty groups are zeroed here; host outputs: the planned frames are written packed, and out_frame[i]
+// receives the call's frame of planned group i's first frame.  Returns the number of planned frames in *planned.
+static int begin_multi(OrbfeExtractor *ex, int ngroups, const OrbfeImageGroup *groups, bool host, int *d_counts, cudaStream_t s,
+                       std::vector<int> &out_frame, int *planned) {
+    int i = 0, frame = 0, out = 0, fw = 0, cw = 0;
+    out_frame.clear();
+    for (int g = 0; g < ngroups; g++) {
+        const OrbfeImageGroup &Gi = groups[g];
+        if (group_empty(Gi)) {
+            if (d_counts) ORBFE_CUDA_TRY(cudaMemsetAsync(d_counts + out, 0, sizeof(int) * Gi.batch, s));
+            out += Gi.batch;
+            continue;
+        }
+        MultiPlanDev &M = *ex->mhp;
+        GroupDev &G = M.grp[i];
+        G.frame0 = frame;
+        G.nframes = Gi.batch;
+        G.out0 = host ? frame : out;
+        G.fwork0 = fw;
+        G.cwork0 = cw;
+        fw += G.nftiles * Gi.batch;
+        cw += G.ncells * Gi.batch;
+        out_frame.push_back(out);
+        const LevelDev &own = ex->mown0[i];
+        const bool in_place = !host && !getenv("ORBFE_INGEST_COPY") && ((uintptr_t)Gi.imgs % 16 == 0) && Gi.stride % 16 == 0 &&
+                              Gi.frame_stride % 16 == 0 && Gi.stride <= (size_t)INT_MAX && Gi.frame_stride >= Gi.stride * (size_t)Gi.height;
+        if (in_place) {
+            if (int rc = set_group_level0(ex, i, const_cast<uint8_t *>(Gi.imgs), (int)Gi.stride, Gi.frame_stride, s)) return rc;
+        } else {
+            if (int rc = set_group_level0(ex, i, own.pyr, own.pitch, own.plane, s)) return rc;
+            const cudaMemcpyKind kind = host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+            for (int f = 0; f < Gi.batch; f++)
+                ORBFE_CUDA_TRY(cudaMemcpy2DAsync(own.pyr + f * own.plane, own.pitch, Gi.imgs + f * Gi.frame_stride, Gi.stride, Gi.width,
+                                                 Gi.height, kind, s));
+        }
+        frame += Gi.batch;
+        out += Gi.batch;
+        i++;
+    }
+    *planned = frame;
+    if (frame == 0) return ORBFE_OK;
+    MultiPlanDev &M = *ex->mhp;
+    M.nframes = frame;
+    M.nfwork = fw;
+    M.ncwork = cw;
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->mdp->grp, M.grp, sizeof(M.grp), cudaMemcpyHostToDevice, s));
+    stage_mark(ex, s, "ingest");
+    ORBFE_CUDA_TRY(cudaMemsetAsync(ex->mcounters, 0, ex->mcounters_bytes, s));
+    return ORBFE_OK;
+}
+
+// One launch per stage for all groups: nlevels - 1 resizes, then FAST, quota, cell select, level select, describe
+static int enqueue_multi(OrbfeExtractor *ex, OrbfeKeyPoint *d_kps, uint8_t *d_desc, int *d_counts, cudaStream_t s) {
+    const MultiPlanDev &M = *ex->mhp;
+    for (int l = 1; l < M.nlevels; l++) launch_resize_level_multi(ex->mdp, M, l, s);
+    stage_mark(ex, s, "pyramid");
+    launch_fast_nms_multi(ex->mdp, M, ex->mwork, s);
+    stage_mark(ex, s, "fast_nms");
+    launch_cell_quota_multi(ex->mdp, M, ex->mwork, s);
+    stage_mark(ex, s, "cell_quota");
+    launch_cell_select_multi(ex->mdp, M, ex->mwork, s);
+    stage_mark(ex, s, "cell_select");
+    launch_level_select_multi(ex->mdp, M, ex->mwork, ex->mls_smem, s);
+    stage_mark(ex, s, "level_select");
+    launch_describe_multi(ex->mdp, M, ex->mwork, ex->d_pattern, d_kps, d_desc, d_counts, s);
+    stage_mark(ex, s, "describe");
+    ORBFE_CUDA_TRY(cudaGetLastError());
+    ex->last_launches += M.nlevels + 4;
+    return ORBFE_OK;
+}
+
+extern "C" int orbfe_extract_multi_device(OrbfeExtractor *ex, int ngroups, const OrbfeImageGroup *groups, OrbfeKeyPoint *d_kps,
+                                          uint8_t *d_desc, int *d_counts, void *stream) {
+    int frames = 0, planned = 0;
+    if (int rc = check_groups(ex, ngroups, groups, &frames)) return rc;
+    if (!d_kps || !d_desc || !d_counts) return fail(ORBFE_ERR_ARG, "NULL output");
+    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
+    if (int rc = build_multi_plan(ex, ngroups, groups)) return rc;
+    const cudaStream_t s = ex->hs.pick(stream);
+    if (int rc = ex->hs.enter(s)) return rc;
+    profiling_begin(ex, s);
+    ex->last_launches = 0;
+    std::vector<int> out_frame;
+    if (int rc = begin_multi(ex, ngroups, groups, false, d_counts, s, out_frame, &planned)) return rc;
+    if (planned)
+        if (int rc = enqueue_multi(ex, d_kps, d_desc, d_counts, s)) return rc;
+    return ex->hs.leave(s, false);
+}
+
+extern "C" int orbfe_extract_multi(OrbfeExtractor *ex, int ngroups, const OrbfeImageGroup *groups, OrbfeKeyPoint *kps,
+                                   uint8_t *desc, int cap, int *n_out) {
+    int frames = 0, planned = 0;
+    if (int rc = check_groups(ex, ngroups, groups, &frames)) return rc;
+    if (!n_out || cap < 0 || (cap > 0 && (!kps || !desc))) return fail(ORBFE_ERR_ARG, "bad output arguments");
+    for (int f = 0; f < frames; f++) n_out[f] = 0;
+    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
+    if (int rc = build_multi_plan(ex, ngroups, groups)) return rc;
+    if (int rc = grow_host_counts(ex, frames)) return rc;
+    const cudaStream_t s = ex->hs.stream;
+    if (int rc = ex->hs.enter(s)) return rc;
+    profiling_begin(ex, s);
+    ex->last_launches = 0;
+    std::vector<int> out_frame;
+    if (int rc = begin_multi(ex, ngroups, groups, true, nullptr, s, out_frame, &planned)) return rc;
+    if (!planned) return ex->hs.leave(s, false);
+    if (int rc = enqueue_multi(ex, ex->md_kps, ex->md_desc, ex->md_counts, s)) return rc;
+    const MultiPlanDev &M = *ex->mhp;
+    const int nf = M.nfeatures, ncopy = std::min(cap, nf);
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->h_counts, ex->md_counts, sizeof(int) * planned, cudaMemcpyDeviceToHost, s));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->h_err, ex->mwork.err_flag, sizeof(int), cudaMemcpyDeviceToHost, s));
+    for (int i = 0; ncopy > 0 && i < M.ngroups; i++) {
+        const GroupDev &G = M.grp[i];
+        ORBFE_CUDA_TRY(cudaMemcpy2DAsync(kps + (size_t)out_frame[i] * cap, sizeof(OrbfeKeyPoint) * cap, ex->md_kps + (size_t)G.frame0 * nf,
+                                         sizeof(OrbfeKeyPoint) * nf, sizeof(OrbfeKeyPoint) * ncopy, G.nframes, cudaMemcpyDeviceToHost, s));
+        ORBFE_CUDA_TRY(cudaMemcpy2DAsync(desc + (size_t)out_frame[i] * cap * 32, (size_t)32 * cap, ex->md_desc + (size_t)G.frame0 * nf * 32,
+                                         (size_t)32 * nf, (size_t)32 * ncopy, G.nframes, cudaMemcpyDeviceToHost, s));
+    }
+    stage_mark(ex, s, "d2h");
+    if (int rc = ex->hs.leave(s, true)) return rc;
+    if (*ex->h_err) {
+        const int code = *ex->h_err;
+        cudaMemsetAsync(ex->mwork.err_flag, 0, sizeof(int), s);
+        ex->hs.leave(s, false);
+        return fail(ORBFE_ERR_INTERNAL, "device overflow flag %d", code);
+    }
+    int status = ORBFE_OK;
+    for (int i = 0; i < M.ngroups; i++)
+        for (int f = 0; f < M.grp[i].nframes; f++) {
+            const int n = ex->h_counts[M.grp[i].frame0 + f];
+            n_out[out_frame[i] + f] = n;
+            if (n > cap) status = ORBFE_ERR_CAPACITY;
+        }
+    if (status) return fail(status, "caller capacity %d too small", cap);
+    return ORBFE_OK;
+}
+
 extern "C" int orbfe_extractor_sync(OrbfeExtractor *ex) {
     if (!ex) return fail(ORBFE_ERR_ARG, "ex is NULL");
     if (int rc = ex->hs.enter(ex->hs.stream)) return rc;   // the handle's last call may have run on a caller's stream
@@ -755,6 +1089,7 @@ extern "C" int orbfe_extractor_sync(OrbfeExtractor *ex) {
 }
 
 extern "C" int orbfe_extractor_last_launches(const OrbfeExtractor *ex) { return ex ? ex->last_launches : 0; }
+extern "C" int orbfe_extractor_plan_builds(const OrbfeExtractor *ex) { return ex ? ex->plan_builds : 0; }
 
 extern "C" int orbfe_extractor_set_batch_mode(OrbfeExtractor *ex, int mode) {
     if (!ex || mode < 0 || mode > 1) return fail(ORBFE_ERR_ARG, "bad arguments");

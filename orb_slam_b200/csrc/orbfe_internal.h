@@ -8,6 +8,7 @@
 
 #include <algorithm>
 #include <initializer_list>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -53,7 +54,9 @@ struct LevelDev {
     int rz_fast;          // >= 1: the 4 source columns of every aligned destination quad fit three aligned words; 2: see build_plan
 };
 
-struct PlanDev {
+// What the single-geometry plan and the multi plan share; the per-frame strides (ncells_total, kept_total, cand_total,
+// nlevels, nfeatures) index the work buffers.
+struct PlanHead {
     int nlevels, batch, nfeatures;
     int ncells_total, nftiles_total, nbtiles_total, kept_total;
     int t_lo, t_hi;      // min / max of (max(fastTh, 1), 7): threshold 0 detects what 1 does (build_plan)
@@ -62,8 +65,31 @@ struct PlanDev {
     int pdl;             // host side only: launch the pipeline's kernels with programmatic stream serialization (ORBFE_PDL, default 1)
     float harris_scale4;   // (1 / (4 * 7 * 255))^4 as the reference computes it (ORBextractor.cc:90-92)
     long long cand_total;  // candidate slots per frame
+};
+
+struct PlanDev : PlanHead {
     LevelDev lv[ORBFE_MAX_LEVELS];
 };
+
+// The multi plan (orbfe_extract_multi): one level table for all groups, group g's level l at lv[g * nlevels + l].  Cell ids,
+// FAST and blur tiles are numbered across the groups; candidate slots, kept lists and keypoint slots restart at 0 in every
+// group, so the per-frame strides cand_total and kept_total are the largest group's and ncells_total is the sum.  The
+// per-frame work arrays are indexed by the call's work frame (the frames of the planned groups, in call order); level planes
+// by the frame inside its group.  grp[] and the level-0 entries are rewritten by every call.
+struct GroupDev {
+    int frame0, nframes;   // the group's work frames [frame0, frame0 + nframes) in this call
+    int out0;              // output frame of its first frame
+    int ftile0, nftiles;   // its FAST tiles in the flat table
+    int cell0, ncells;     // its cells
+    int fwork0, cwork0;    // its first FAST work item and its first cell-select block in this call
+};
+struct MultiPlanDev : PlanHead {
+    LevelDev lv[ORBFE_MULTI_MAX_GROUPS * ORBFE_MAX_LEVELS];
+    int ngroups;
+    int nframes, nfwork, ncwork;   // host side only: this call's work frames, FAST work items and cell-select blocks
+    GroupDev grp[ORBFE_MULTI_MAX_GROUPS];
+};
+template <bool kMulti> using PlanOf = typename std::conditional<kMulti, MultiPlanDev, PlanDev>::type;
 
 // Cell geometry of one FAST tile (host-precomputed): cells overlapped and interior cell boundaries inside it
 struct FTileInfo {
@@ -121,6 +147,15 @@ void launch_level_select(const PlanDev *d_plan, const PlanDev &h_plan, WorkDev w
 void launch_blur(const PlanDev *d_plan, const PlanDev &h_plan, WorkDev w, int f0, int nf, cudaStream_t s);
 void launch_describe_fused(const PlanDev *d_plan, const PlanDev &h_plan, WorkDev w, const int8_t *d_pattern,
                      OrbfeKeyPoint *d_kps, uint8_t *d_desc, int *d_counts, int f0, int nf, cudaStream_t s, const PeerOut *peers = nullptr);
+// the same chain over every group of a multi plan: one launch per stage (the resize of level l covers level l of every
+// group), the frames of this call as h_plan's grp[] and totals describe them
+void launch_resize_level_multi(const MultiPlanDev *d_plan, const MultiPlanDev &h_plan, int level, cudaStream_t s);
+void launch_fast_nms_multi(const MultiPlanDev *d_plan, const MultiPlanDev &h_plan, WorkDev w, cudaStream_t s);
+void launch_cell_quota_multi(const MultiPlanDev *d_plan, const MultiPlanDev &h_plan, WorkDev w, cudaStream_t s);
+void launch_cell_select_multi(const MultiPlanDev *d_plan, const MultiPlanDev &h_plan, WorkDev w, cudaStream_t s);
+void launch_level_select_multi(const MultiPlanDev *d_plan, const MultiPlanDev &h_plan, WorkDev w, size_t smem_bytes, cudaStream_t s);
+void launch_describe_multi(const MultiPlanDev *d_plan, const MultiPlanDev &h_plan, WorkDev w, const int8_t *d_pattern,
+                           OrbfeKeyPoint *d_kps, uint8_t *d_desc, int *d_counts, cudaStream_t s);
 int fast_tma_setup();
 int level_select_smem_bytes(int max_kept);
 int level_select_harris_smem_bytes(int max_kept);

@@ -69,6 +69,10 @@
                    of tests/covis_scenes.py scene_large, for frames of about 300, 1000 and 2000 matched points
                    (tests/local_map_scenes.py large_frames): the median of CUDA-event windows of one call each, and the wall
                    time of the reference's own UpdateReference() on the same map with the same lists (results compared).
+  --what multigeom  a three-camera rig step (one 1920x1080 and two 1280x720 cameras, 2000 kp, 8 levels) at 1 and 4 frames per
+                   camera: CUDA-event ms and wall ms per step of one orbfe_extract_multi_device call, of three handles one after
+                   another on one stream and of three handles on three streams (forked from and joined to one stream by events).
+                   The three ways run alternately, five rounds of 200 steps each; the median round is reported.
 Prints one JSON object per --what; never a bench value when run under ncu."""
 import argparse
 import ctypes as C
@@ -924,6 +928,91 @@ def latency(args):
             acc[name] = acc.get(name, 0.0) + ms / n
         out[tag] = {"ms_per_call": ms_plain, "pdl": os.environ.get("ORBFE_PDL", "1"), "stages": {k: round(v, 4) for k, v in acc.items()}}
         ex.close()
+    return out
+
+
+def multigeom(args):
+    """See the module docstring (--what multigeom)."""
+    import torch
+    import orb_slam_b200 as fe
+    from orb_slam_b200.synth import textured_frame
+    dev = torch.device("cuda", 0)
+    cams = [(1920, 1080), (1280, 720), (1280, 720)]
+    NF, steps, rounds = 2000, 200, 5
+    main = torch.cuda.Stream(device=dev)
+    side = [torch.cuda.Stream(device=dev) for _ in cams]
+    out = {"what": "rig step of 1x1920x1080 + 2x1280x720 cameras, %d kp, 8 levels, device-resident: ms per step (median of %d rounds "
+                   "of %d steps)" % (NF, rounds, steps)}
+    for B in (1, 4):
+        frames = [torch.from_numpy(np.stack([textured_frame(W, H, seed=10 * c + i) for i in range(B)])).to(dev)
+                  for c, (W, H) in enumerate(cams)]
+        F = B * len(cams)
+        multi = fe.ORBextractor(NF, 1.2, 8, fe.FAST_SCORE, 20)
+        singles = [fe.ORBextractor(NF, 1.2, 8, fe.FAST_SCORE, 20) for _ in cams]
+        slots = int(multi.tables()[2].sum())
+        d_kps = torch.empty((F, slots, 28), dtype=torch.uint8, device=dev)
+        d_desc = torch.empty((F, slots, 32), dtype=torch.uint8, device=dev)
+        d_cnt = torch.empty((F,), dtype=torch.int32, device=dev)
+        groups = [(f.data_ptr(), W, H, W, W * H, B) for f, (W, H) in zip(frames, cams)]
+
+        def run_multi():
+            multi.extract_multi_device(groups, d_kps.data_ptr(), d_desc.data_ptr(), d_cnt.data_ptr(), main.cuda_stream)
+
+        def run_serial(streams=None):
+            for c, (ex, (p, W, H, st, fs, b)) in enumerate(zip(singles, groups)):
+                s = streams[c] if streams else main
+                ex.extract_batch_device(p, W, H, st, fs, b, d_kps[c * B].data_ptr(), d_desc[c * B].data_ptr(), d_cnt[c * B].data_ptr(),
+                                        s.cuda_stream)
+
+        def run_streams():
+            fork = torch.cuda.Event()
+            fork.record(main)
+            for s in side:
+                s.wait_event(fork)
+            run_serial(side)
+            for s in side:
+                ev = torch.cuda.Event()
+                ev.record(s)
+                main.wait_event(ev)
+
+        ways = {"multi_one_call": run_multi, "three_handles_one_stream": run_serial, "three_handles_three_streams": run_streams}
+        res = {k: {"event_ms": [], "wall_ms": []} for k in ways}
+        for fn in ways.values():
+            for _ in range(max(args.warmup, 10)):
+                fn()
+        torch.cuda.synchronize()
+        want = None
+        for r in range(rounds):
+            for name, fn in ways.items():
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                e0.record(main)
+                for _ in range(steps):
+                    fn()
+                e1.record(main)
+                e1.synchronize()
+                torch.cuda.synchronize()
+                res[name]["wall_ms"].append((time.perf_counter() - t0) * 1e3 / steps)
+                res[name]["event_ms"].append(e0.elapsed_time(e1) / steps)
+                got = (d_cnt.cpu().numpy().tolist(), int(d_desc.sum().item()))
+                want = want or got
+                res[name]["same_outputs"] = res[name].get("same_outputs", True) and got == want
+        out["%d_frame_per_camera" % B] = {k: {"event_ms": round(float(np.median(v["event_ms"])), 4),
+                                              "wall_ms": round(float(np.median(v["wall_ms"])), 4),
+                                              "event_ms_min_max": [round(min(v["event_ms"]), 4), round(max(v["event_ms"]), 4)],
+                                              "same_outputs": v["same_outputs"]} for k, v in res.items()}
+        out["%d_frame_per_camera" % B]["multi_launches"] = multi.last_launches()
+        multi.close()
+        for ex in singles:
+            ex.close()
+    _gpu_and_power_limit(out)
+    try:
+        import subprocess
+        out["sm_clock"] = subprocess.run(["nvidia-smi", "--query-gpu=clocks.sm,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                                         capture_output=True, text=True).stdout.strip()
+    except Exception as e:
+        out["sm_clock"] = "unknown: %r" % e
     return out
 
 
@@ -1906,4 +1995,4 @@ if __name__ == "__main__":
                           "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb, "kfdbbatch": kfdbbatch, "bowchain": bowchain,
                           "windowed": windowed, "guided": guided, "loopscore": loopscore, "vocload": vocload,
                           "normaldepth": normaldepth, "covis": covis, "observations": observations, "kfculling": kfculling,
-                          "localmap": localmap}[w](args)))
+                          "localmap": localmap, "multigeom": multigeom}[w](args)))
