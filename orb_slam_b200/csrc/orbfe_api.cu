@@ -873,7 +873,15 @@ static int build_multi_plan(OrbfeExtractor *ex, int ngroups, const OrbfeImageGro
     plan_head(ex, *M, 0);
     PlanLayout A;
     for (int i = 0; i < n; i++) {
-        if (int rc = layout_geometry(ex, geom[2 * i], geom[2 * i + 1], &M->lv[i * nl], A)) {
+        // a geometry's kept lists (quota + 2 * cells + 64) decide its level-select footprint, so that refusal names the group too
+        int rc = layout_geometry(ex, geom[2 * i], geom[2 * i + 1], &M->lv[i * nl], A);
+        if (!rc) {
+            int kept = 0;
+            size_t bytes = 0;
+            for (int l = 0; l < nl; l++) kept = std::max(kept, M->lv[i * nl + l].kept_cap);
+            rc = level_select_smem(ex, kept, &bytes);
+        }
+        if (rc) {
             const std::string why = g_err;
             return fail(rc, "group %d (%dx%d): %s", gidx[i], geom[2 * i], geom[2 * i + 1], why.c_str());
         }

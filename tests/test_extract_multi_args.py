@@ -58,6 +58,15 @@ def test_bad_group_is_rejected_wherever_it_stands():
             assert _calls(h, len(specs), _groups(*specs)) == (fe.ORBFE_ERR_ARG, fe.ORBFE_ERR_ARG), (bad, len(specs))
 
 
+def test_more_than_65535_frames_across_groups_are_rejected():
+    """one grid row per frame: 65536 frames split across groups are ORBFE_ERR_ARG before the handle is used"""
+    keep, h = _fake_handle()
+    for split in ((65535, 1), (32768, 32768), (1, 1, 65534)):
+        groups = _groups(*[(640, 480, 640, b, IMG) for b in split])
+        assert _calls(h, len(split), groups) == (fe.ORBFE_ERR_ARG, fe.ORBFE_ERR_ARG), split
+        assert b"65536 frames" in fe.lib().orbfe_last_error()
+
+
 def test_null_outputs_and_negative_cap_are_rejected():
     L = fe.lib()
     keep, h = _fake_handle()

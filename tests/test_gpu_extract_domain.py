@@ -308,12 +308,8 @@ def test_one_handle_across_ingest_paths_and_plans(gpu_required):
     ex.close()
 
 
-def test_mixed_content_batch_of_64(gpu_required):
-    """One call over 64 frames of mixed content at 640x480: flat, binary 0/255 noise, two-tone single-pixel corners,
-    textured, and one frame all zero; per frame equal to the oracle."""
-    import torch
-    D = _Dev(torch)
-    W, H, B = 640, 480, 64
+def mixed_frames(W=640, H=480, B=64):
+    """B frames of mixed content: flat, binary 0/255 noise, two-tone single-pixel corners, textured, and frame 17 all zero"""
     frames = []
     for i in range(B):
         kind = i % 4
@@ -327,7 +323,16 @@ def test_mixed_content_batch_of_64(gpu_required):
         else:
             frames.append(textured_frame(W, H, seed=200 + i))
     frames[17] = np.zeros((H, W), np.uint8)
-    frames = np.stack(frames)
+    return np.stack(frames)
+
+
+def test_mixed_content_batch_of_64(gpu_required):
+    """One call over 64 frames of mixed content at 640x480: flat, binary 0/255 noise, two-tone single-pixel corners,
+    textured, and one frame all zero; per frame equal to the oracle."""
+    import torch
+    D = _Dev(torch)
+    W, H, B = 640, 480, 64
+    frames = mixed_frames(W, H, B)
     want = _oracle(frames)
     assert sum(len(k) == 0 for k, _ in want) >= 16 and sum(len(k) == 1000 for k, _ in want) >= 16
     ex = fe.ORBextractor(1000, 1.2, 8)

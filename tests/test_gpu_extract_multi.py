@@ -14,6 +14,7 @@ import pytest
 import oracle as O
 import orb_slam_b200 as fe
 from orb_slam_b200.synth import textured_frame
+from multi_domain_scenes import empty_levels
 
 pytestmark = pytest.mark.gpu
 
@@ -144,19 +145,11 @@ def test_multi_equals_single_geometry_entry(gpu_required, geoms, setting):
     same(got, want, (geoms, setting))
 
 
-def _empty_levels(params, w, h):
-    """levels whose reference cell grid is empty (ORBextractor.cc:533-547: levelCols or levelRows is 0)"""
-    ratio = np.float32(w) / np.float32(h)
-    q = fe.ORBextractor(*params).tables()[2]
-    cols = [int(np.sqrt(np.float32(x) / (np.float32(5) * ratio))) for x in q]
-    return [l for l, c in enumerate(cols) if c < 1 or int(ratio * np.float32(c)) < 1]
-
-
 def test_multi_with_empty_cell_grid_levels(gpu_required):
     torch, _ = _torch()
     params = (200, 1.2, 8, fe.FAST_SCORE, 20)
     spec = [(640, 480, 1), (1001, 333, 2), (480, 640, 1)]
-    assert _empty_levels(params, 1001, 333) and _empty_levels(params, 480, 640) and not _empty_levels(params, 640, 480)
+    assert empty_levels(params, 1001, 333) and empty_levels(params, 480, 640) and not empty_levels(params, 640, 480)
     groups = _groups(spec, seed=5)
     ex = fe.ORBextractor(*params)
     try:

@@ -181,35 +181,47 @@ def test_chain_extract_backproject_sbp_rotating_camera(gpu_required):
     kd = d_kps.cpu().numpy().view(S.KP_DTYPE).reshape(B, cap)
     for i in range(B):
         assert cnt[i] == len(okps[i]) and np.array_equal(kd[i, :cnt[i]], okps[i])
-    world = np.zeros((B, cap, 3), np.float32)
-    flags = np.zeros((B, cap), np.uint8)
-    for i in range(B):
-        k = okps[i]
-        world[i, :len(k), 0] = (k["x"] - S.CX) / S.FX * np.float32(4)
-        world[i, :len(k), 1] = (k["y"] - S.CY) / S.FY * np.float32(4)
+    ex.close()
+    for n_o in sbp_chain(d_kps, d_desc, d_cnt, cap, okps, odesc, [(i + 1, i) for i in range(B - 1)], W, H):
+        assert n_o > 50
+
+
+def sbp_chain(d_kps, d_desc, d_cnt, cap, okps, odesc, pairs, W, H, cx=S.CX, cy=S.CY):
+    """orbfe_search_by_projection_device over `pairs` [(current, last)] of a device frame store whose frames hold the
+    oracle's keypoints okps / odesc: the last frame's keypoints back-projected at depth 4, a general rotation per pair
+    (0.3-0.5 degrees about a tilted axis, plus the translation of a 3 px, 2 px image shift), image bounds (0, 0, W, H); the
+    matches equal the oracle's SearchByProjection.  Returns the oracle's match count of each pair."""
+    import torch
+    F, P = len(okps), len(pairs)
+    world = np.zeros((F, cap, 3), np.float32)
+    flags = np.zeros((F, cap), np.uint8)
+    for i, k in enumerate(okps):
+        world[i, :len(k), 0] = (k["x"] - cx) / S.FX * np.float32(4)
+        world[i, :len(k), 1] = (k["y"] - cy) / S.FY * np.float32(4)
         world[i, :len(k), 2] = 4
         flags[i, :len(k)] = 1
     T = np.stack([S.pose((0.2, 0.3 * (-1) ** i, 0.93), 0.3 + 0.05 * i, (-3 * 4 / float(S.FX), -2 * 4 / float(S.FY), 0.01))
-                  for i in range(B - 1)]).astype(np.float32)
-    d_mp = torch.full((B - 1, cap), -1, dtype=torch.int32, device="cuda:0")
-    d_nm = torch.zeros(B - 1, dtype=torch.int32, device="cuda:0")
-    d_args = [dev(np.arange(1, B, dtype=np.int32)), dev(np.arange(0, B - 1, dtype=np.int32)), dev(world), dev(flags),
-              dev(T.reshape(B - 1, 12))]
+                  for i in range(P)]).astype(np.float32)
+    d_mp = torch.full((P, cap), -1, dtype=torch.int32, device="cuda:0")
+    d_nm = torch.zeros(P, dtype=torch.int32, device="cuda:0")
+    d_args = [dev(np.array([c for c, _ in pairs], np.int32)), dev(np.array([l for _, l in pairs], np.int32)), dev(world), dev(flags),
+              dev(T.reshape(P, 12))]
     m = fe.ORBmatcher(0.9, True)
     L = M._bind()
-    rc = L.orbfe_search_by_projection_device(m.handle, B - 1, C.c_void_p(d_kps.data_ptr()), C.c_void_p(d_desc.data_ptr()),
+    rc = L.orbfe_search_by_projection_device(m.handle, P, C.c_void_p(d_kps.data_ptr()), C.c_void_p(d_desc.data_ptr()),
                                              C.c_void_p(d_cnt.data_ptr()), cap, *[C.c_void_p(x.data_ptr()) for x in d_args],
-                                             0.0, 0.0, float(W), float(H), 1.2, 8, float(S.FX), float(S.FY), float(S.CX), float(S.CY),
+                                             0.0, 0.0, float(W), float(H), 1.2, 8, float(S.FX), float(S.FY), float(cx), float(cy),
                                              7.0, 1, C.c_void_p(d_mp.data_ptr()), C.c_void_p(d_nm.data_ptr()), None)
     assert rc == 0
     m.sync()
-    ex.close()
     m.close()
     mp, nm = d_mp.cpu().numpy(), d_nm.cpu().numpy()
-    for j in range(B - 1):
-        nl = len(okps[j])
-        n_o, mp_o = O.search_by_projection_ff(O.OracleFrame(okps[j + 1], odesc[j + 1], W, H), O.OracleFrame(okps[j], odesc[j], W, H),
-                                              np.ones(nl, np.uint8), np.zeros(nl, np.uint8), world[j, :nl], T[j], S.FX, S.FY, S.CX,
-                                              S.CY, 7.0, check_orientation=True)
-        assert nm[j] == n_o and np.array_equal(mp[j, :len(okps[j + 1])], mp_o), j
-        assert n_o > 50, j
+    out = []
+    for j, (c, l) in enumerate(pairs):
+        nl = len(okps[l])
+        n_o, mp_o = O.search_by_projection_ff(O.OracleFrame(okps[c], odesc[c], W, H), O.OracleFrame(okps[l], odesc[l], W, H),
+                                              np.ones(nl, np.uint8), np.zeros(nl, np.uint8), world[l, :nl], T[j], S.FX, S.FY, cx,
+                                              cy, 7.0, check_orientation=True)
+        assert nm[j] == n_o and np.array_equal(mp[j, :len(okps[c])], mp_o), (c, l)
+        out.append(n_o)
+    return out
