@@ -108,6 +108,43 @@ int orbfe_guided_search_device(OrbfeMatcher *m, int njobs, const OrbfeKeyPoint *
                                float min_y, float max_x, float max_y, int rule, float nnratio, int th_dist,
                                int check_orientation, int *d_slot_owner, int *d_nmatches, void *stream);
 
+/* ---- Camera rigs: the three device entries above over frames of several cameras in one launch ----
+ *
+ * A frame store filled by orbfe_extract_multi_device holds frames of up to ORBFE_MULTI_MAX_GROUPS image geometries.  The
+ * *_cams_device entries below are the device entries above with the per-call geometry replaced by a camera table: `cams`
+ * is a HOST array of 1 <= ncams <= ORBFE_MULTI_MAX_GROUPS cameras, d_frame_cam a DEVICE array with one camera index per
+ * frame of the store.  A pair or job takes the camera of the frame it searches: the Current frame d_cur_idx[j] (its
+ * bounds, grid and intrinsics), F2 = d_f2_idx[j] (its bounds; F1 may belong to another camera) or d_frame_idx[j].
+ * scale_factor, nlevels, cap, qcap, thresholds and rules stay per call: one extractor made the store.  Every output of a
+ * pair equals what the single-geometry entry writes when called with that pair's camera, bit for bit, in one launch.
+ * The table travels in the kernel's parameters: the calls stay enqueue-only, with the matcher's stream-order rule.
+ * ORBFE_ERR_ARG before anything is enqueued: ncams outside [1, ORBFE_MULTI_MAX_GROUPS], cams or d_frame_cam NULL, a
+ * camera without max_x > min_x and max_y > min_y, and every check of the single-geometry entry.  A pair whose searched
+ * frame has a camera index outside [0, ncams) gets d_nmatches[j] = -1 and its other outputs untouched;
+ * orbfe_matcher_sync then reports ORBFE_ERR_ARG, even when another pair of the launch overflowed the candidate scratch.
+ * The other pairs are unaffected.  Frame indices are not checked. */
+typedef struct {
+    float min_x, min_y, max_x, max_y; /* Frame::mnMinX.. of this camera (e.g. from orbfe_image_bounds) */
+    float fx, fy, cx, cy;             /* read only by the projection search */
+} OrbfeCamera;
+
+int orbfe_search_by_projection_cams_device(OrbfeMatcher *m, int npairs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
+                                           const int *d_counts, int cap, const int *d_cur_idx, const int *d_last_idx,
+                                           const float *d_world, const uint8_t *d_flags, const float *d_Tcw, int ncams,
+                                           const OrbfeCamera *cams, const int *d_frame_cam, float scale_factor, int nlevels,
+                                           float th, int check_orientation, int *d_cur_mp, int *d_nmatches, void *stream);
+int orbfe_search_for_initialization_cams_device(OrbfeMatcher *m, int npairs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
+                                                const int *d_counts, int cap, const int *d_f1_idx, const int *d_f2_idx,
+                                                float *d_prev_matched, int ncams, const OrbfeCamera *cams, const int *d_frame_cam,
+                                                int window, float nnratio, int check_orientation, int *d_match12, int *d_nmatches,
+                                                void *stream);
+int orbfe_guided_search_cams_device(OrbfeMatcher *m, int njobs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
+                                    const int *d_counts, int cap, const int *d_frame_idx, const float *d_qu, const float *d_qv,
+                                    const float *d_qr, const int *d_qlo, const int *d_qhi, const uint8_t *d_qdesc,
+                                    const float *d_qangle, const int *d_q_base, const int *d_q_cnt, int qcap, int ncams,
+                                    const OrbfeCamera *cams, const int *d_frame_cam, int rule, float nnratio, int th_dist,
+                                    int check_orientation, int *d_slot_owner, int *d_nmatches, void *stream);
+
 /* int ORBmatcher::SearchByProjection(Frame &F, const vector<MapPoint*>&, float th) (ORBmatcher.cc:49-125), local-map
  * tracking.  Per map point: in_view = mbTrackInView && !isBad(); proj_xy = (mTrackProjX, mTrackProjY); level =
  * mnTrackScaleLevel; view_cos = mTrackViewCos; desc = GetDescriptor().  f_mp_inout[i2] >= 0 <=> F.mvpMapPoints[i2] set

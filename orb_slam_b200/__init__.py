@@ -14,7 +14,7 @@ import os
 
 import numpy as np
 
-__all__ = ["ORBextractor", "ORBmatcher", "OrbfeError", "KP_DTYPE", "OrbfeImageGroup", "lib", "library_path", "HARRIS_SCORE",
+__all__ = ["ORBextractor", "ORBmatcher", "OrbfeError", "KP_DTYPE", "OrbfeImageGroup", "OrbfeCamera", "lib", "library_path", "HARRIS_SCORE",
            "FAST_SCORE"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -31,6 +31,11 @@ class OrbfeImageGroup(C.Structure):
     """One image geometry of an orbfe_extract_multi* call (include/orbfe.h)"""
     _fields_ = [("width", C.c_int), ("height", C.c_int), ("stride", C.c_size_t), ("frame_stride", C.c_size_t),
                 ("batch", C.c_int), ("imgs", C.c_void_p)]
+
+
+class OrbfeCamera(C.Structure):
+    """One camera of a *_cams_device matcher call (include/orbfe_match.h)"""
+    _fields_ = [(f, C.c_float) for f in ("min_x", "min_y", "max_x", "max_y", "fx", "fy", "cx", "cy")]
 
 
 # cv::KeyPoint layout (28 bytes)
@@ -55,6 +60,7 @@ ABI_SYMBOLS = [
     "orbfe_search_by_projection_f1f2", "orbfe_search_by_bow", "orbfe_guided_search", "orbfe_guided_best", "orbfe_search_for_triangulation",
     "orbfe_window_search",
     "orbfe_search_for_initialization",
+    "orbfe_search_by_projection_cams_device", "orbfe_search_for_initialization_cams_device", "orbfe_guided_search_cams_device",
     "orbfe_undistort_keypoints_device", "orbfe_undistort_keypoints", "orbfe_image_bounds",
     # include/orbfe_comm.h
     "orbfe_comm_unique_id", "orbfe_comm_create", "orbfe_comm_destroy", "orbfe_comm_world", "orbfe_comm_rank", "orbfe_comm_nccl_version",

@@ -191,25 +191,30 @@ __device__ __forceinline__ int cell_bound(float f) {
     return (f >= -2147483648.0f && f < 2147483648.0f) ? (int)f : (int)0x80000000u;
 }
 
+// The image geometry the fused kernel reads -- bounds, grid cell sizes and intrinsics -- comes from a type G with the fields
+// of that name: the call's SbpParams itself (single-geometry launches) or one camera's SbpCam of a camera-table launch.
+
 // cell range of Frame::GetFeaturesInArea (Frame.cc:205-223); false if the window misses the grid
-__device__ __forceinline__ bool sbp_cell_range(const SbpParams &P, SbpQuery &q) {
-    int x0 = cell_bound(floorf(__fmul_rn(__fsub_rn(__fsub_rn(q.u, P.min_x), q.r), P.gw)));
+template <class G>
+__device__ __forceinline__ bool sbp_cell_range(const G &g, SbpQuery &q) {
+    int x0 = cell_bound(floorf(__fmul_rn(__fsub_rn(__fsub_rn(q.u, g.min_x), q.r), g.gw)));
     x0 = max(0, x0);
     if (x0 >= SBP_GCOLS) return false;
-    int x1 = cell_bound(ceilf(__fmul_rn(__fadd_rn(__fsub_rn(q.u, P.min_x), q.r), P.gw)));
+    int x1 = cell_bound(ceilf(__fmul_rn(__fadd_rn(__fsub_rn(q.u, g.min_x), q.r), g.gw)));
     x1 = min(SBP_GCOLS - 1, x1);
     if (x1 < 0) return false;
-    int y0 = cell_bound(floorf(__fmul_rn(__fsub_rn(__fsub_rn(q.v, P.min_y), q.r), P.gh)));
+    int y0 = cell_bound(floorf(__fmul_rn(__fsub_rn(__fsub_rn(q.v, g.min_y), q.r), g.gh)));
     y0 = max(0, y0);
     if (y0 >= SBP_GROWS) return false;
-    int y1 = cell_bound(ceilf(__fmul_rn(__fadd_rn(__fsub_rn(q.v, P.min_y), q.r), P.gh)));
+    int y1 = cell_bound(ceilf(__fmul_rn(__fadd_rn(__fsub_rn(q.v, g.min_y), q.r), g.gh)));
     y1 = min(SBP_GROWS - 1, y1);
     if (y1 < 0) return false;
     q.x0 = x0; q.x1 = x1; q.y0 = y0; q.y1 = y1;
     return true;
 }
 
-__device__ __forceinline__ SbpQuery sbp_project(const SbpParams &P, const OrbfeKeyPoint &kl, const float *X, const float *T) {
+template <class G>
+__device__ __forceinline__ SbpQuery sbp_project(const SbpParams &P, const G &g, const OrbfeKeyPoint &kl, const float *X, const float *T) {
     SbpQuery q;
     q.ok = false;
     float xc3[3];
@@ -221,14 +226,14 @@ __device__ __forceinline__ SbpQuery sbp_project(const SbpParams &P, const OrbfeK
         xc3[k] = (float)__dadd_rn((double)s, (double)T[4 * k + 3]);
     }
     const float invzc = (float)(1.0 / (double)xc3[2]);
-    q.u = __fadd_rn(__fmul_rn(__fmul_rn(P.fx, xc3[0]), invzc), P.cx);
-    q.v = __fadd_rn(__fmul_rn(__fmul_rn(P.fy, xc3[1]), invzc), P.cy);
-    if (q.u < P.min_x || q.u > P.max_x) return q;
-    if (q.v < P.min_y || q.v > P.max_y) return q;
+    q.u = __fadd_rn(__fmul_rn(__fmul_rn(g.fx, xc3[0]), invzc), g.cx);
+    q.v = __fadd_rn(__fmul_rn(__fmul_rn(g.fy, xc3[1]), invzc), g.cy);
+    if (q.u < g.min_x || q.u > g.max_x) return q;
+    if (q.v < g.min_y || q.v > g.max_y) return q;
     q.lo = kl.octave - 1;
     q.hi = kl.octave + 1;
     q.r = __fmul_rn(P.th, P.scale[kl.octave]);
-    q.ok = sbp_cell_range(P, q);
+    q.ok = sbp_cell_range(g, q);
     return q;
 }
 
@@ -278,14 +283,15 @@ __device__ __forceinline__ int rot_hist_bin(float a1, float a2) {
 //         around their previously matched position (`world` holds vbPrevMatched, 2 floats per F1 feature, updated in place,
 //         :708-710); an F2 feature can be RE-assigned to a later, closer F1 feature (:637, :656-663); cur_mp receives
 //         vnMatches12 (per F1 feature).
-template <int MODE>
-__global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, const OrbfeKeyPoint *__restrict__ kps,
-                                                                 const uint8_t *__restrict__ desc, const int *__restrict__ counts,
-                                                                 const int *__restrict__ cur_idx, const int *__restrict__ last_idx,
-                                                                 const float *__restrict__ world, const uint8_t *__restrict__ flags,
-                                                                 const float *__restrict__ Tcw, GuidedQueries GQ,
-                                                                 uint32_t *__restrict__ scratch, int *__restrict__ cur_mp,
-                                                                 int *__restrict__ nmatches, int *__restrict__ err) {
+// The body of one thread block; `g` is the searched frame's geometry (see sbp_cell_range).
+template <int MODE, class G>
+__device__ __forceinline__ void sbp_block(const SbpParams &P, const G &g, const OrbfeKeyPoint *__restrict__ kps,
+                                          const uint8_t *__restrict__ desc, const int *__restrict__ counts,
+                                          const int *__restrict__ cur_idx, const int *__restrict__ last_idx,
+                                          const float *__restrict__ world, const uint8_t *__restrict__ flags,
+                                          const float *__restrict__ Tcw, GuidedQueries GQ,
+                                          uint32_t *__restrict__ scratch, int *__restrict__ cur_mp,
+                                          int *__restrict__ nmatches, int *__restrict__ err) {
     extern __shared__ __align__(16) unsigned char smem[];
     const int cap = P.cap;
     int *cell_start = reinterpret_cast<int *>(smem);                 // [NCELL + 1]
@@ -331,7 +337,7 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
             SbpQuery Q;
             Q.u = GQ.qu[qb + q]; Q.v = GQ.qv[qb + q]; Q.r = GQ.qr[qb + q];
             Q.lo = GQ.qlo[qb + q]; Q.hi = GQ.qhi[qb + q];
-            Q.ok = sbp_cell_range(P, Q);
+            Q.ok = sbp_cell_range(g, Q);
             return Q;
         }
         if (INIT) {   // :609-618: level-0 features only, window around the previously matched position, same level
@@ -340,10 +346,10 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
             if (kl[q].octave > 0) return Q;
             Q.u = wl[2 * q]; Q.v = wl[2 * q + 1]; Q.r = P.th;
             Q.lo = 0; Q.hi = 0;
-            Q.ok = sbp_cell_range(P, Q);
+            Q.ok = sbp_cell_range(g, Q);
             return Q;
         }
-        return sbp_project(P, kl[q], wl + 3 * q, T);
+        return sbp_project(P, g, kl[q], wl + 3 * q, T);
     };
     auto query_angle = [&](int q) -> float { return EXPLICIT ? GQ.qangle[qb + q] : kl[q].angle; };
 
@@ -386,8 +392,8 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
     for (int i = tid; i < nc; i += SBP_THREADS) {
         const OrbfeKeyPoint k = kc[i];
         kx[i] = k.x; ky[i] = k.y; koct[i] = (uint8_t)k.octave;
-        const float px = roundf(__fmul_rn(__fsub_rn(k.x, P.min_x), P.gw));
-        const float py = roundf(__fmul_rn(__fsub_rn(k.y, P.min_y), P.gh));
+        const float px = roundf(__fmul_rn(__fsub_rn(k.x, g.min_x), g.gw));
+        const float py = roundf(__fmul_rn(__fsub_rn(k.y, g.min_y), g.gh));
         int cell = -1;
         // MODE 2 asks for level-0 features only (:618): the other levels never enter the grid, so the window walks touch
         // one keypoint in five
@@ -414,8 +420,8 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
     }
     __syncthreads();
     for (int i = tid; i < nc; i += SBP_THREADS) {
-        const float px = roundf(__fmul_rn(__fsub_rn(kx[i], P.min_x), P.gw));
-        const float py = roundf(__fmul_rn(__fsub_rn(ky[i], P.min_y), P.gh));
+        const float px = roundf(__fmul_rn(__fsub_rn(kx[i], g.min_x), g.gw));
+        const float py = roundf(__fmul_rn(__fsub_rn(ky[i], g.min_y), g.gh));
         if (px >= 0.f && px < (float)SBP_GCOLS && py >= 0.f && py < (float)SBP_GROWS && !(INIT && koct[i] != 0)) {
             const int cell = (int)px * SBP_GROWS + (int)py;
             items[atomicAdd(&cell_cur[cell], 1)] = (uint16_t)i;
@@ -463,7 +469,13 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
     __syncthreads();
     const int T_total = run_total;
     if (T_total > P.scratch_per_pair) {   // err[1]: the most entries any overflowing job needed, for a relaunch that fits
-        if (tid == 0) { atomicExch(err, 1); atomicMax(err + 1, T_total); nmatches[pair] = -1; }
+        if (tid == 0) {
+            // a camera-table launch may also raise the bad-camera bit: keep it (an exchange would clear it)
+            if constexpr (std::is_same<G, SbpParams>::value) atomicExch(err, 1);
+            else atomicOr(err, 1);
+            atomicMax(err + 1, T_total);
+            nmatches[pair] = -1;
+        }
         publish_ack();
         return;
     }
@@ -560,7 +572,9 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
                     for (int p = b; p < e; p++) {
                         const uint32_t cur = ent[p];
                         const uint32_t key = ((cur & 0xFFFF0000u) | (uint32_t)(p - b)) + 1u;
-                        if (key > lower && key < next && (int)(cur >> 16) <= P.th_dist && holder[cur & 0xFFFF] > q) next = key;
+                        // key < next first: with sbp_block inlined, this order keeps sbp_device_kernel's instructions the
+                        // ones whose timings DESIGN.md reports (the tests commute)
+                        if (key < next && key > lower && (int)(cur >> 16) <= P.th_dist && holder[cur & 0xFFFF] > q) next = key;
                     }
                     changed = true;
                     pos = next == 0xFFFFFFFFu ? 0xFFFF : (int)((next - 1u) & 0xFFFF);
@@ -854,6 +868,37 @@ __global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, co
     if (tid == 0) nmatches[pair] = s_nm - s_removed;
 }
 
+template <int MODE>
+__global__ void __launch_bounds__(SBP_THREADS) sbp_device_kernel(SbpParams P, const OrbfeKeyPoint *__restrict__ kps,
+                                                                 const uint8_t *__restrict__ desc, const int *__restrict__ counts,
+                                                                 const int *__restrict__ cur_idx, const int *__restrict__ last_idx,
+                                                                 const float *__restrict__ world, const uint8_t *__restrict__ flags,
+                                                                 const float *__restrict__ Tcw, GuidedQueries GQ,
+                                                                 uint32_t *__restrict__ scratch, int *__restrict__ cur_mp,
+                                                                 int *__restrict__ nmatches, int *__restrict__ err) {
+    sbp_block<MODE>(P, P, kps, desc, counts, cur_idx, last_idx, world, flags, Tcw, GQ, scratch, cur_mp, nmatches, err);
+}
+
+// The same kernel over a camera table: a block takes the geometry of its searched frame's camera (frame_cam[cur_idx[j]]).
+// The table is a __grid_constant__ parameter, read in place with the camera index, so the launch needs no copy.  A camera
+// index outside [0, cams.n) sets bit 32 of *err and the block's nmatches to -1, and leaves its other outputs untouched.
+template <int MODE>
+__global__ void __launch_bounds__(SBP_THREADS) sbp_cams_kernel(SbpParams P, const OrbfeKeyPoint *__restrict__ kps,
+                                                               const uint8_t *__restrict__ desc, const int *__restrict__ counts,
+                                                               const int *__restrict__ cur_idx, const int *__restrict__ last_idx,
+                                                               const float *__restrict__ world, const uint8_t *__restrict__ flags,
+                                                               const float *__restrict__ Tcw, GuidedQueries GQ,
+                                                               uint32_t *__restrict__ scratch, int *__restrict__ cur_mp,
+                                                               int *__restrict__ nmatches, int *__restrict__ err,
+                                                               const __grid_constant__ SbpCams cams, const int *__restrict__ frame_cam) {
+    const int c = frame_cam[cur_idx[blockIdx.x]];
+    if (c < 0 || c >= cams.n) {
+        if (threadIdx.x == 0) { atomicOr(err, 32); nmatches[blockIdx.x] = -1; }
+        return;
+    }
+    sbp_block<MODE>(P, cams.cam[c], kps, desc, counts, cur_idx, last_idx, world, flags, Tcw, GQ, scratch, cur_mp, nmatches, err);
+}
+
 size_t sbp_smem_fixed_bytes(int cap, int qcap) {
     size_t b = sizeof(int) * (SBP_NCELL + 1) + sizeof(int) * SBP_NCELL + sizeof(int) * ((size_t)qcap + 1) +   // cell_start, cell_cur, q_off
                2 * sizeof(float) * (size_t)cap + sizeof(uint32_t) * (((size_t)cap + 31) / 32) +              // kx, ky, taken
@@ -864,50 +909,56 @@ size_t sbp_smem_fixed_bytes(int cap, int qcap) {
     return (b + 15) / 16 * 16;
 }
 
-int launch_sbp_device(const SbpParams &P, size_t smem_bytes, int npairs, const OrbfeKeyPoint *kps, const uint8_t *desc,
+// One launch of the fused kernel: single-geometry, or over the camera table `cams` (NULL = single-geometry)
+template <int MODE>
+static int sbp_launch(const SbpParams &P, size_t smem_bytes, int nblocks, const OrbfeKeyPoint *kps, const uint8_t *desc,
                       const int *counts, const int *cur_idx, const int *last_idx, const float *world, const uint8_t *flags,
-                      const float *Tcw, uint32_t *scratch, int *cur_mp, int *nmatches, int *err, cudaStream_t s) {
+                      const float *Tcw, const GuidedQueries &G, uint32_t *scratch, int *cur_mp, int *nmatches, int *err,
+                      const SbpCams *cams, const int *frame_cam, cudaStream_t s) {
     if (smem_bytes > 48 * 1024) {  // per device/context attribute: set on every call (cheap), never cached process-wide
-        cudaError_t e = cudaFuncSetAttribute(sbp_device_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+        cudaError_t e = cams ? cudaFuncSetAttribute(sbp_cams_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes)
+                             : cudaFuncSetAttribute(sbp_device_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
         if (e != cudaSuccess) return (int)e;
     }
+    if (cams)
+        sbp_cams_kernel<MODE><<<nblocks, SBP_THREADS, smem_bytes, s>>>(P, kps, desc, counts, cur_idx, last_idx, world, flags, Tcw, G,
+                                                                       scratch, cur_mp, nmatches, err, *cams, frame_cam);
+    else
+        sbp_device_kernel<MODE><<<nblocks, SBP_THREADS, smem_bytes, s>>>(P, kps, desc, counts, cur_idx, last_idx, world, flags, Tcw, G,
+                                                                         scratch, cur_mp, nmatches, err);
+    return 0;
+}
+
+int launch_sbp_device(const SbpParams &P, size_t smem_bytes, int npairs, const OrbfeKeyPoint *kps, const uint8_t *desc,
+                      const int *counts, const int *cur_idx, const int *last_idx, const float *world, const uint8_t *flags,
+                      const float *Tcw, uint32_t *scratch, int *cur_mp, int *nmatches, int *err, cudaStream_t s,
+                      const SbpCams *cams, const int *frame_cam) {
     GuidedQueries none;
     memset(&none, 0, sizeof(none));
-    sbp_device_kernel<0><<<npairs, SBP_THREADS, smem_bytes, s>>>(P, kps, desc, counts, cur_idx, last_idx, world, flags, Tcw, none,
-                                                             scratch, cur_mp, nmatches, err);
-    return 0;
+    return sbp_launch<0>(P, smem_bytes, npairs, kps, desc, counts, cur_idx, last_idx, world, flags, Tcw, none, scratch, cur_mp,
+                         nmatches, err, cams, frame_cam, s);
 }
 
 int launch_init_device(const SbpParams &P, size_t smem_bytes, int npairs, const OrbfeKeyPoint *kps, const uint8_t *desc,
                        const int *counts, const int *f1_idx, const int *f2_idx, float *prev_matched, uint32_t *scratch, int *match12,
-                       int *nmatches, int *err, cudaStream_t s) {
-    if (smem_bytes > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(sbp_device_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-        if (e != cudaSuccess) return (int)e;
-    }
+                       int *nmatches, int *err, cudaStream_t s, const SbpCams *cams, const int *frame_cam) {
     GuidedQueries none;
     memset(&none, 0, sizeof(none));
     // cur = F2 (the searched frame), last = F1 (the querying frame)
-    sbp_device_kernel<2><<<npairs, SBP_THREADS, smem_bytes, s>>>(P, kps, desc, counts, f2_idx, f1_idx, prev_matched, nullptr, nullptr, none,
-                                                            scratch, match12, nmatches, err);
-    return 0;
+    return sbp_launch<2>(P, smem_bytes, npairs, kps, desc, counts, f2_idx, f1_idx, prev_matched, nullptr, nullptr, none, scratch,
+                         match12, nmatches, err, cams, frame_cam, s);
 }
 
 int launch_guided_device(const SbpParams &P, size_t smem_bytes, int njobs, const OrbfeKeyPoint *kps, const uint8_t *desc,
                          const int *counts, const int *frame_idx, const float *qu, const float *qv, const float *qr,
                          const int *qlo, const int *qhi, const uint8_t *qdesc, const float *qangle, const int *q_base,
                          const int *q_cnt, uint32_t *scratch, int *slot_owner, int *best_out, int *nmatches, int *err,
-                         cudaStream_t s) {
-    if (smem_bytes > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(sbp_device_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-        if (e != cudaSuccess) return (int)e;
-    }
+                         cudaStream_t s, const SbpCams *cams, const int *frame_cam) {
     GuidedQueries G;
     G.qu = qu; G.qv = qv; G.qr = qr; G.qangle = qangle; G.qlo = qlo; G.qhi = qhi; G.qdesc = qdesc; G.q_base = q_base; G.q_cnt = q_cnt;
     G.best = best_out;
-    sbp_device_kernel<1><<<njobs, SBP_THREADS, smem_bytes, s>>>(P, kps, desc, counts, frame_idx, nullptr, nullptr, nullptr, nullptr, G,
-                                                            scratch, slot_owner, nmatches, err);
-    return 0;
+    return sbp_launch<1>(P, smem_bytes, njobs, kps, desc, counts, frame_idx, nullptr, nullptr, nullptr, nullptr, G, scratch,
+                         slot_owner, nmatches, err, cams, frame_cam, s);
 }
 
 // ------------------------------------------------------------------------------------------------

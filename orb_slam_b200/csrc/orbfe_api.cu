@@ -1248,6 +1248,9 @@ extern "C" int orbfe_matcher_sync(OrbfeMatcher *m) {
         if (flags & 16)
             return fail(ORBFE_ERR_ARG, "orbfe_normal_and_depth_device: a point's group pointers, an observation or reference slot, "
                                        "or its reference octave are out of range (its outputs are untouched)");
+        if (flags & 32)
+            return fail(ORBFE_ERR_ARG, "device matcher (*_cams_device): a pair's searched frame has a camera index outside "
+                                       "[0, ncams) (its nmatches is -1, its other outputs are untouched)");
         return fail(ORBFE_ERR_CAPACITY, "device matcher: a job's candidate entries exceeded its global scratch (its nmatches is -1; "
                                         "%d entries were needed)", m->h_err[1]);
     }
@@ -1256,14 +1259,17 @@ extern "C" int orbfe_matcher_sync(OrbfeMatcher *m) {
 
 static constexpr size_t kSbpSmemMax = 220 * 1024;   // shared memory per block sbp_prepare grants the fused kernel
 
+// mfGridElementWidthInv / HeightInv (Frame.cc:77-78): `cells` grid cells over [lo, hi]
+static float grid_inv(int cells, float lo, float hi) { return (float)cells / (float)(hi - lo); }
+
 // Prepares one launch of sbp_device_kernel over `njobs` jobs of at most `cap` features and `qcap` queries each: the image
 // bounds and their grid cell sizes (Frame.cc:77-78) in P, the split of the dynamic shared memory (returned in *smem) and
 // `per_job` global scratch entries per job.  The one place that decides whether a job fits the kernel.
 static int sbp_prepare(OrbfeMatcher *m, SbpParams &P, float min_x, float min_y, float max_x, float max_y, int cap, int qcap,
                        int njobs, size_t per_job, size_t *smem) {
     P.min_x = min_x; P.min_y = min_y; P.max_x = max_x; P.max_y = max_y;
-    P.gw = (float)64 / (float)(max_x - min_x);
-    P.gh = (float)48 / (float)(max_y - min_y);
+    P.gw = grid_inv(64, min_x, max_x);
+    P.gh = grid_inv(48, min_y, max_y);
     P.cap = cap; P.qcap = qcap;
     const size_t fixed = sbp_smem_fixed_bytes(cap, qcap);
     const size_t total = sbp_smem_total(m, fixed, njobs);
@@ -1296,13 +1302,32 @@ static int sbp_launched(OrbfeMatcher *m, int rc) {
     return ORBFE_OK;
 }
 
-// SearchByProjection(Frame &Current, const Frame &Last, th) for `npairs` pairs, everything device-resident.
-extern "C" int orbfe_search_by_projection_device(OrbfeMatcher *m, int npairs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
-                                                 const int *d_counts, int cap, const int *d_cur_idx, const int *d_last_idx,
-                                                 const float *d_world, const uint8_t *d_flags, const float *d_Tcw,
-                                                 float min_x, float min_y, float max_x, float max_y, float scale_factor,
-                                                 int nlevels, float fx, float fy, float cx, float cy, float th,
-                                                 int check_orientation, int *d_cur_mp, int *d_nmatches, void *stream) {
+// The camera table of a *_cams_device call: each camera's bounds checked and its grid cell sizes computed as sbp_prepare
+// computes them.  Host-side only.
+static int cams_table(int ncams, const OrbfeCamera *cams, const int *d_frame_cam, SbpCams &T) {
+    if (ncams < 1 || ncams > ORBFE_MULTI_MAX_GROUPS) return fail(ORBFE_ERR_ARG, "ncams %d outside 1..%d", ncams, ORBFE_MULTI_MAX_GROUPS);
+    if (!cams || !d_frame_cam) return fail(ORBFE_ERR_ARG, "NULL camera table or frame-camera array");
+    memset(&T, 0, sizeof(T));
+    T.n = ncams;
+    for (int c = 0; c < ncams; c++) {
+        const OrbfeCamera &k = cams[c];
+        if (!(k.max_x > k.min_x) || !(k.max_y > k.min_y)) return fail(ORBFE_ERR_ARG, "bad image bounds of camera %d", c);
+        SbpCam &t = T.cam[c];
+        t.min_x = k.min_x; t.min_y = k.min_y; t.max_x = k.max_x; t.max_y = k.max_y;
+        t.gw = grid_inv(64, k.min_x, k.max_x);
+        t.gh = grid_inv(48, k.min_y, k.max_y);
+        t.fx = k.fx; t.fy = k.fy; t.cx = k.cx; t.cy = k.cy;
+    }
+    return ORBFE_OK;
+}
+
+// SearchByProjection(Frame &Current, const Frame &Last, th) for `npairs` pairs, everything device-resident.  T: NULL, or the
+// camera table the kernel takes each pair's geometry from (the geometry arguments are then camera 0's, for the checks only).
+static int sbp_projection(OrbfeMatcher *m, int npairs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc, const int *d_counts,
+                          int cap, const int *d_cur_idx, const int *d_last_idx, const float *d_world, const uint8_t *d_flags,
+                          const float *d_Tcw, float min_x, float min_y, float max_x, float max_y, float scale_factor, int nlevels,
+                          float fx, float fy, float cx, float cy, float th, int check_orientation, int *d_cur_mp, int *d_nmatches,
+                          void *stream, const SbpCams *T, const int *d_frame_cam) {
     if (!m || npairs < 0 || cap < 1 || cap > 65535 || nlevels < 1 || nlevels > ORBFE_MAX_LEVELS) return fail(ORBFE_ERR_ARG, "bad arguments");
     if (npairs == 0) return ORBFE_OK;
     if (!d_kps || !d_desc || !d_counts || !d_cur_idx || !d_last_idx || !d_world || !d_flags || !d_Tcw || !d_cur_mp || !d_nmatches)
@@ -1320,9 +1345,34 @@ extern "C" int orbfe_search_by_projection_device(OrbfeMatcher *m, int npairs, co
     size_t smem;
     if (int rc = sbp_prepare(m, P, min_x, min_y, max_x, max_y, cap, cap, npairs, (size_t)64 * cap, &smem)) return rc;
     if (int rc = sbp_launched(m, launch_sbp_device(P, smem, npairs, d_kps, d_desc, d_counts, d_cur_idx, d_last_idx, d_world, d_flags, d_Tcw,
-                                                   m->scratch, d_cur_mp, d_nmatches, m->d_err, s)))
+                                                   m->scratch, d_cur_mp, d_nmatches, m->d_err, s, T, d_frame_cam)))
         return rc;
     return m->hs.leave(s, false);
+}
+
+extern "C" int orbfe_search_by_projection_device(OrbfeMatcher *m, int npairs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
+                                                 const int *d_counts, int cap, const int *d_cur_idx, const int *d_last_idx,
+                                                 const float *d_world, const uint8_t *d_flags, const float *d_Tcw,
+                                                 float min_x, float min_y, float max_x, float max_y, float scale_factor,
+                                                 int nlevels, float fx, float fy, float cx, float cy, float th,
+                                                 int check_orientation, int *d_cur_mp, int *d_nmatches, void *stream) {
+    return sbp_projection(m, npairs, d_kps, d_desc, d_counts, cap, d_cur_idx, d_last_idx, d_world, d_flags, d_Tcw, min_x, min_y, max_x,
+                          max_y, scale_factor, nlevels, fx, fy, cx, cy, th, check_orientation, d_cur_mp, d_nmatches, stream, nullptr,
+                          nullptr);
+}
+
+extern "C" int orbfe_search_by_projection_cams_device(OrbfeMatcher *m, int npairs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
+                                                      const int *d_counts, int cap, const int *d_cur_idx, const int *d_last_idx,
+                                                      const float *d_world, const uint8_t *d_flags, const float *d_Tcw, int ncams,
+                                                      const OrbfeCamera *cams, const int *d_frame_cam, float scale_factor,
+                                                      int nlevels, float th, int check_orientation, int *d_cur_mp, int *d_nmatches,
+                                                      void *stream) {
+    SbpCams T;
+    if (int rc = cams_table(ncams, cams, d_frame_cam, T)) return rc;
+    const SbpCam &c = T.cam[0];
+    return sbp_projection(m, npairs, d_kps, d_desc, d_counts, cap, d_cur_idx, d_last_idx, d_world, d_flags, d_Tcw, c.min_x, c.min_y,
+                          c.max_x, c.max_y, scale_factor, nlevels, c.fx, c.fy, c.cx, c.cy, th, check_orientation, d_cur_mp, d_nmatches,
+                          stream, &T, d_frame_cam);
 }
 
 // SearchForInitialization(F1, F2, vbPrevMatched, vnMatches12, windowSize) for `npairs` (F1, F2) pairs, device-resident
@@ -1355,12 +1405,12 @@ static SbpParams init_params(int window, float nnratio, int check_orientation) {
 // a 100-px window at 720p holds a few hundred level-0 candidates per query: entries live in the global scratch
 static size_t init_scratch_per_pair(int cap) { return (size_t)256 * cap; }
 
-// `hooks`: only the xw_* fields are read (rig exchange: wait for the epoch's data at kernel start, publish the release at its end)
-int orbfe_search_for_initialization_hooked(OrbfeMatcher *m, int npairs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
-                                           const int *d_counts, int cap, const int *d_f1_idx, const int *d_f2_idx,
-                                           float *d_prev_matched, float min_x, float min_y, float max_x, float max_y,
-                                           int window, float nnratio, int check_orientation, int *d_match12,
-                                           int *d_nmatches, void *stream, const SbpParams *hooks) {
+// `hooks`: only the xw_* fields are read (rig exchange: wait for the epoch's data at kernel start, publish the release at its end).
+// T: camera table (see sbp_projection), or NULL.
+static int init_device(OrbfeMatcher *m, int npairs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc, const int *d_counts, int cap,
+                       const int *d_f1_idx, const int *d_f2_idx, float *d_prev_matched, float min_x, float min_y, float max_x,
+                       float max_y, int window, float nnratio, int check_orientation, int *d_match12, int *d_nmatches, void *stream,
+                       const SbpParams *hooks, const SbpCams *T, const int *d_frame_cam) {
     if (!m || npairs < 0 || cap < 1 || cap > 65534 || window < 0) return fail(ORBFE_ERR_ARG, "bad arguments");
     if (npairs == 0) return ORBFE_OK;
     if (!d_kps || !d_desc || !d_counts || !d_f1_idx || !d_f2_idx || !d_prev_matched || !d_match12 || !d_nmatches)
@@ -1376,19 +1426,40 @@ int orbfe_search_for_initialization_hooked(OrbfeMatcher *m, int npairs, const Or
     size_t smem;
     if (int rc = sbp_prepare(m, P, min_x, min_y, max_x, max_y, cap, cap, npairs, init_scratch_per_pair(cap), &smem)) return rc;
     if (int rc = sbp_launched(m, launch_init_device(P, smem, npairs, d_kps, d_desc, d_counts, d_f1_idx, d_f2_idx, d_prev_matched, m->scratch,
-                                                    d_match12, d_nmatches, m->d_err, s)))
+                                                    d_match12, d_nmatches, m->d_err, s, T, d_frame_cam)))
         return rc;
     return m->hs.leave(s, false);
 }
 
-// Guided search with explicit query windows, device-resident (same kernel, EXPLICIT query source).
-extern "C" int orbfe_guided_search_device(OrbfeMatcher *m, int njobs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
-                                          const int *d_counts, int cap, const int *d_frame_idx, const float *d_qu,
-                                          const float *d_qv, const float *d_qr, const int *d_qlo, const int *d_qhi,
-                                          const uint8_t *d_qdesc, const float *d_qangle, const int *d_q_base,
-                                          const int *d_q_cnt, int qcap, float min_x, float min_y, float max_x, float max_y,
-                                          int rule, float nnratio, int th_dist, int check_orientation, int *d_slot_owner,
-                                          int *d_nmatches, void *stream) {
+int orbfe_search_for_initialization_hooked(OrbfeMatcher *m, int npairs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
+                                           const int *d_counts, int cap, const int *d_f1_idx, const int *d_f2_idx,
+                                           float *d_prev_matched, float min_x, float min_y, float max_x, float max_y,
+                                           int window, float nnratio, int check_orientation, int *d_match12,
+                                           int *d_nmatches, void *stream, const SbpParams *hooks) {
+    return init_device(m, npairs, d_kps, d_desc, d_counts, cap, d_f1_idx, d_f2_idx, d_prev_matched, min_x, min_y, max_x, max_y, window,
+                       nnratio, check_orientation, d_match12, d_nmatches, stream, hooks, nullptr, nullptr);
+}
+
+extern "C" int orbfe_search_for_initialization_cams_device(OrbfeMatcher *m, int npairs, const OrbfeKeyPoint *d_kps,
+                                                           const uint8_t *d_desc, const int *d_counts, int cap, const int *d_f1_idx,
+                                                           const int *d_f2_idx, float *d_prev_matched, int ncams,
+                                                           const OrbfeCamera *cams, const int *d_frame_cam, int window, float nnratio,
+                                                           int check_orientation, int *d_match12, int *d_nmatches, void *stream) {
+    SbpCams T;
+    if (int rc = cams_table(ncams, cams, d_frame_cam, T)) return rc;
+    const SbpCam &c = T.cam[0];
+    return init_device(m, npairs, d_kps, d_desc, d_counts, cap, d_f1_idx, d_f2_idx, d_prev_matched, c.min_x, c.min_y, c.max_x, c.max_y,
+                       window, nnratio, check_orientation, d_match12, d_nmatches, stream, nullptr, &T, d_frame_cam);
+}
+
+// Guided search with explicit query windows, device-resident (same kernel, EXPLICIT query source).  T: camera table (see
+// sbp_projection), or NULL.
+static int guided_device(OrbfeMatcher *m, int njobs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc, const int *d_counts, int cap,
+                         const int *d_frame_idx, const float *d_qu, const float *d_qv, const float *d_qr, const int *d_qlo,
+                         const int *d_qhi, const uint8_t *d_qdesc, const float *d_qangle, const int *d_q_base, const int *d_q_cnt,
+                         int qcap, float min_x, float min_y, float max_x, float max_y, int rule, float nnratio, int th_dist,
+                         int check_orientation, int *d_slot_owner, int *d_nmatches, void *stream, const SbpCams *T,
+                         const int *d_frame_cam) {
     if (!m || njobs < 0 || cap < 1 || cap > 65535 || qcap < 1 || qcap > 65535 || rule < 0 || rule > 2) return fail(ORBFE_ERR_ARG, "bad arguments");
     if (njobs == 0) return ORBFE_OK;
     if (!d_kps || !d_desc || !d_counts || !d_frame_idx || !d_qu || !d_qv || !d_qr || !d_qlo || !d_qhi || !d_qdesc || !d_q_base ||
@@ -1405,9 +1476,36 @@ extern "C" int orbfe_guided_search_device(OrbfeMatcher *m, int njobs, const Orbf
     if (int rc = sbp_prepare(m, P, min_x, min_y, max_x, max_y, cap, qcap, njobs, (size_t)64 * std::max(cap, qcap), &smem)) return rc;
     if (int rc = sbp_launched(m, launch_guided_device(P, smem, njobs, d_kps, d_desc, d_counts, d_frame_idx, d_qu, d_qv, d_qr, d_qlo, d_qhi,
                                                       d_qdesc, d_qangle, d_q_base, d_q_cnt, m->scratch, d_slot_owner, nullptr, d_nmatches,
-                                                      m->d_err, s)))
+                                                      m->d_err, s, T, d_frame_cam)))
         return rc;
     return m->hs.leave(s, false);
+}
+
+extern "C" int orbfe_guided_search_device(OrbfeMatcher *m, int njobs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
+                                          const int *d_counts, int cap, const int *d_frame_idx, const float *d_qu,
+                                          const float *d_qv, const float *d_qr, const int *d_qlo, const int *d_qhi,
+                                          const uint8_t *d_qdesc, const float *d_qangle, const int *d_q_base,
+                                          const int *d_q_cnt, int qcap, float min_x, float min_y, float max_x, float max_y,
+                                          int rule, float nnratio, int th_dist, int check_orientation, int *d_slot_owner,
+                                          int *d_nmatches, void *stream) {
+    return guided_device(m, njobs, d_kps, d_desc, d_counts, cap, d_frame_idx, d_qu, d_qv, d_qr, d_qlo, d_qhi, d_qdesc, d_qangle, d_q_base,
+                         d_q_cnt, qcap, min_x, min_y, max_x, max_y, rule, nnratio, th_dist, check_orientation, d_slot_owner, d_nmatches,
+                         stream, nullptr, nullptr);
+}
+
+extern "C" int orbfe_guided_search_cams_device(OrbfeMatcher *m, int njobs, const OrbfeKeyPoint *d_kps, const uint8_t *d_desc,
+                                               const int *d_counts, int cap, const int *d_frame_idx, const float *d_qu,
+                                               const float *d_qv, const float *d_qr, const int *d_qlo, const int *d_qhi,
+                                               const uint8_t *d_qdesc, const float *d_qangle, const int *d_q_base,
+                                               const int *d_q_cnt, int qcap, int ncams, const OrbfeCamera *cams,
+                                               const int *d_frame_cam, int rule, float nnratio, int th_dist, int check_orientation,
+                                               int *d_slot_owner, int *d_nmatches, void *stream) {
+    SbpCams T;
+    if (int rc = cams_table(ncams, cams, d_frame_cam, T)) return rc;
+    const SbpCam &c = T.cam[0];
+    return guided_device(m, njobs, d_kps, d_desc, d_counts, cap, d_frame_idx, d_qu, d_qv, d_qr, d_qlo, d_qhi, d_qdesc, d_qangle, d_q_base,
+                         d_q_cnt, qcap, c.min_x, c.min_y, c.max_x, c.max_y, rule, nnratio, th_dist, check_orientation, d_slot_owner,
+                         d_nmatches, stream, &T, d_frame_cam);
 }
 
 int orbfe::Stage::layout(std::initializer_list<std::pair<size_t *, size_t>> arrays, size_t *total) {

@@ -184,22 +184,34 @@ struct SbpParams {
     unsigned xw_epoch;
     int owner_base;                            // guided search: added to the job-local query index a matched slot receives
 };
+// One camera of a camera-table launch (the *_cams_device entries): the SbpParams fields that depend on the camera
+struct SbpCam {
+    float min_x, min_y, max_x, max_y, gw, gh;
+    float fx, fy, cx, cy;
+};
+struct SbpCams {
+    SbpCam cam[ORBFE_MULTI_MAX_GROUPS];
+    int n;
+};
 // Guided-search accept rule without slots (orbfe_guided_best): each query keeps the first minimum of its whole candidate
 // list iff best <= th_dist, written to best_out; slot_owner is read but never written.  Internal: the exported guided searches
 // take rules 0..2 (3 is SearchForInitialization's).
 #define SBP_RULE_BEST 4
 size_t sbp_smem_fixed_bytes(int cap, int qcap);
+// The fused kernel's launchers.  cams / frame_cam (device, one camera index per frame): launch over a camera table, each
+// block with its searched frame's camera; P's own geometry is then not read.
 int launch_guided_device(const SbpParams &P, size_t smem_bytes, int njobs, const OrbfeKeyPoint *kps, const uint8_t *desc,
                          const int *counts, const int *frame_idx, const float *qu, const float *qv, const float *qr,
                          const int *qlo, const int *qhi, const uint8_t *qdesc, const float *qangle, const int *q_base,
                          const int *q_cnt, uint32_t *scratch, int *slot_owner, int *best_out, int *nmatches, int *err,
-                         cudaStream_t s);
+                         cudaStream_t s, const SbpCams *cams = nullptr, const int *frame_cam = nullptr);
 int launch_init_device(const SbpParams &P, size_t smem_bytes, int npairs, const OrbfeKeyPoint *kps, const uint8_t *desc,
                        const int *counts, const int *f1_idx, const int *f2_idx, float *prev_matched, uint32_t *scratch, int *match12,
-                       int *nmatches, int *err, cudaStream_t s);
+                       int *nmatches, int *err, cudaStream_t s, const SbpCams *cams = nullptr, const int *frame_cam = nullptr);
 int launch_sbp_device(const SbpParams &P, size_t smem_bytes, int npairs, const OrbfeKeyPoint *kps, const uint8_t *desc,
                       const int *counts, const int *cur_idx, const int *last_idx, const float *world, const uint8_t *flags,
-                      const float *Tcw, uint32_t *scratch, int *cur_mp, int *nmatches, int *err, cudaStream_t s);
+                      const float *Tcw, uint32_t *scratch, int *cur_mp, int *nmatches, int *err, cudaStream_t s,
+                      const SbpCams *cams = nullptr, const int *frame_cam = nullptr);
 
 // One query window of the guided search: candidates = GetFeaturesInArea(u, v, r, lo, hi) of the searched frame; a match
 // writes `owner` into the frame's slot

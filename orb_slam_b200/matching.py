@@ -9,7 +9,7 @@ import ctypes as C
 
 import numpy as np
 
-from . import KP_DTYPE, ORBmatcher, OrbfeError, lib
+from . import KP_DTYPE, ORBmatcher, OrbfeCamera, OrbfeError, lib
 
 GRID_COLS, GRID_ROWS = 64, 48  # Frame.h:35-36
 
@@ -62,6 +62,13 @@ def _bind():
                                              vp, vp, vp]
     L.orbfe_search_for_triangulation_device.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int,
                                                         C.c_int, vp, vp, vp]
+    cp = C.POINTER(OrbfeCamera)
+    L.orbfe_search_by_projection_cams_device.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp, C.c_int, cp, vp,
+                                                         C.c_float, C.c_int, C.c_float, C.c_int, vp, vp, vp]
+    L.orbfe_search_for_initialization_cams_device.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, C.c_int, cp, vp, C.c_int,
+                                                              C.c_float, C.c_int, vp, vp, vp]
+    L.orbfe_guided_search_cams_device.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int,
+                                                  C.c_int, cp, vp, C.c_int, C.c_float, C.c_int, C.c_int, vp, vp, vp]
     _bound = True
     return L
 
@@ -216,6 +223,51 @@ def search_by_projection_device(matcher: ORBmatcher, npairs, d_kps, d_desc, d_co
                                                0.0, 0.0, float(width), float(height), scale_factor, nlevels,
                                                fx, fy, cx, cy, th, int(matcher.mbCheckOrientation), vp(d_cur_mp),
                                                vp(d_nmatches), vp(stream)))
+
+
+def cameras(cams):
+    """A host OrbfeCamera array from [(min_x, min_y, max_x, max_y, fx, fy, cx, cy)] (fx..cy are read by the projection
+    search only)"""
+    arr = (OrbfeCamera * max(len(cams), 1))()
+    for a, c in zip(arr, cams):
+        a.min_x, a.min_y, a.max_x, a.max_y, a.fx, a.fy, a.cx, a.cy = [float(v) for v in c]
+    return arr
+
+
+def search_by_projection_cams_device(matcher: ORBmatcher, npairs, d_kps, d_desc, d_counts, cap, d_cur_idx, d_last_idx, d_world,
+                                     d_flags, d_Tcw, cams, d_frame_cam, scale_factor, nlevels, th, d_cur_mp, d_nmatches, stream=0):
+    """search_by_projection_device over a camera rig in one launch: `cams` as in cameras(), d_frame_cam one camera index
+    per frame of the store; each pair takes its Current frame's camera.  See include/orbfe_match.h."""
+    L = _bind()
+    vp = C.c_void_p
+    _check(L.orbfe_search_by_projection_cams_device(matcher.handle, npairs, vp(d_kps), vp(d_desc), vp(d_counts), cap, vp(d_cur_idx),
+                                                    vp(d_last_idx), vp(d_world), vp(d_flags), vp(d_Tcw), len(cams), cameras(cams),
+                                                    vp(d_frame_cam), scale_factor, nlevels, th, int(matcher.mbCheckOrientation),
+                                                    vp(d_cur_mp), vp(d_nmatches), vp(stream)))
+
+
+def search_for_initialization_cams_device(matcher: ORBmatcher, npairs, d_kps, d_desc, d_counts, cap, d_f1_idx, d_f2_idx,
+                                          d_prev_matched, cams, d_frame_cam, window, d_match12, d_nmatches, stream=0):
+    """search_for_initialization_device over a camera rig in one launch; each pair takes F2's camera bounds."""
+    L = _bind()
+    vp = C.c_void_p
+    _check(L.orbfe_search_for_initialization_cams_device(matcher.handle, npairs, vp(d_kps), vp(d_desc), vp(d_counts), cap, vp(d_f1_idx),
+                                                         vp(d_f2_idx), vp(d_prev_matched), len(cams), cameras(cams), vp(d_frame_cam),
+                                                         int(window), float(matcher.mfNNratio), int(matcher.mbCheckOrientation),
+                                                         vp(d_match12), vp(d_nmatches), vp(stream)))
+
+
+def guided_search_cams_device(matcher: ORBmatcher, njobs, d_kps, d_desc, d_counts, cap, d_frame_idx, d_qu, d_qv, d_qr, d_qlo, d_qhi,
+                              d_qdesc, d_qangle, d_q_base, d_q_cnt, qcap, cams, d_frame_cam, rule, th_dist, d_slot_owner, d_nmatches,
+                              stream=0):
+    """guided_search_device over a camera rig in one launch; each job takes its searched frame's camera bounds."""
+    L = _bind()
+    vp = C.c_void_p
+    _check(L.orbfe_guided_search_cams_device(matcher.handle, njobs, vp(d_kps), vp(d_desc), vp(d_counts), cap, vp(d_frame_idx), vp(d_qu),
+                                             vp(d_qv), vp(d_qr), vp(d_qlo), vp(d_qhi), vp(d_qdesc), vp(d_qangle), vp(d_q_base),
+                                             vp(d_q_cnt), qcap, len(cams), cameras(cams), vp(d_frame_cam), rule,
+                                             float(matcher.mfNNratio), th_dist, int(matcher.mbCheckOrientation), vp(d_slot_owner),
+                                             vp(d_nmatches), vp(stream)))
 
 
 def guided_search_device(matcher: ORBmatcher, njobs, d_kps, d_desc, d_counts, cap, d_frame_idx, d_qu, d_qv, d_qr, d_qlo, d_qhi,

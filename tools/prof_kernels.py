@@ -73,6 +73,13 @@
                    camera: CUDA-event ms and wall ms per step of one orbfe_extract_multi_device call, of three handles one after
                    another on one stream and of three handles on three streams (forked from and joined to one stream by events).
                    The three ways run alternately, five rounds of 200 steps each; the median round is reported.
+  --what multitrack the matching half of that rig step: frame-to-frame SearchByProjection for every camera of the --what
+                   multigeom rig (frames extracted in one orbfe_extract_multi_device call) at 1 and 4 pairs per camera:
+                   CUDA-event ms and wall ms per step of one orbfe_search_by_projection_cams_device call, of three
+                   single-geometry calls one after another on one stream and of three calls on three streams (three matcher
+                   handles, forked from and joined to one stream by events).  Every step first resets the Current frames'
+                   slots (one fill on the main stream, in all three ways).  Alternating rounds as --what multigeom; the
+                   outputs of the three ways are compared.
 Prints one JSON object per --what; never a bench value when run under ncu."""
 import argparse
 import ctypes as C
@@ -1013,6 +1020,137 @@ def multigeom(args):
                                          capture_output=True, text=True).stdout.strip()
     except Exception as e:
         out["sm_clock"] = "unknown: %r" % e
+    return out
+
+
+def multitrack(args):
+    """See the module docstring (--what multitrack)."""
+    import torch
+    import orb_slam_b200 as fe
+    from orb_slam_b200 import matching as M
+    from orb_slam_b200.synth import textured_frame
+    dev = torch.device("cuda", 0)
+    cams = [(1920, 1080), (1280, 720), (1280, 720)]
+    NF, steps, rounds, TH = 2000, 200, 5, 7.0
+    main = torch.cuda.Stream(device=dev)
+    side = [torch.cuda.Stream(device=dev) for _ in cams]
+    table = [(0.0, 0.0, float(W), float(H), 0.7 * W, 0.7 * W, W / 2, H / 2) for W, H in cams]
+    out = {"what": "rig SearchByProjection(Frame, Frame) of 1x1920x1080 + 2x1280x720 cameras, %d kp, 8 levels, device-resident: ms "
+                   "per step (median of %d rounds of %d steps)" % (NF, rounds, steps)}
+    for B in (1, 4):
+        # B + 1 frames per camera, each shifted by (3, 2) px from the one before; pair i of a camera = (frame i + 1, frame i)
+        frames = []
+        for c, (W, H) in enumerate(cams):
+            base = textured_frame(W + 3 * B + 3, H + 2 * B + 2, seed=20 + c)
+            frames.append(torch.from_numpy(np.stack([np.ascontiguousarray(base[2 * i:2 * i + H, 3 * i:3 * i + W])
+                                                     for i in range(B + 1)])).to(dev))
+        F, P = (B + 1) * len(cams), B * len(cams)
+        ex = fe.ORBextractor(NF, 1.2, 8, fe.FAST_SCORE, 20)
+        cap = int(ex.tables()[2].sum())
+        d_kps = torch.empty((F, cap, 28), dtype=torch.uint8, device=dev)
+        d_desc = torch.empty((F, cap, 32), dtype=torch.uint8, device=dev)
+        d_cnt = torch.empty((F,), dtype=torch.int32, device=dev)
+        ex.extract_multi_device([(f.data_ptr(), W, H, W, W * H, B + 1) for f, (W, H) in zip(frames, cams)], d_kps.data_ptr(),
+                                d_desc.data_ptr(), d_cnt.data_ptr())
+        ex.sync()
+        torch.cuda.synchronize()
+        ex.close()
+        kps = d_kps.cpu().numpy().view(fe.KP_DTYPE).reshape(F, cap)
+        cnt = d_cnt.cpu().numpy()
+        world = np.zeros((F, cap, 3), np.float32)
+        flags = np.zeros((F, cap), np.uint8)
+        frame_cam = np.repeat(np.arange(len(cams), dtype=np.int32), B + 1)
+        for f in range(F):
+            _, _, _, _, fx, fy, cx, cy = table[frame_cam[f]]
+            k = kps[f, :cnt[f]]
+            world[f, :cnt[f], 0] = (k["x"] - np.float32(cx)) / np.float32(fx) * np.float32(4)
+            world[f, :cnt[f], 1] = (k["y"] - np.float32(cy)) / np.float32(fy) * np.float32(4)
+            world[f, :cnt[f], 2] = 4
+            flags[f, :cnt[f]] = 1
+        cur = np.array([c * (B + 1) + i + 1 for c in range(len(cams)) for i in range(B)], np.int32)
+        Tcw = np.zeros((P, 12), np.float32)
+        for j, f in enumerate(cur):
+            fx = np.float32(table[frame_cam[f]][4])
+            Tcw[j] = [1, 0, 0, -12 / fx, 0, 1, 0, -8 / fx, 0, 0, 1, 0.01]
+        t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+        d_cur, d_last, d_world, d_flags, d_T, d_fc = t(cur), t(cur - 1), t(world), t(flags), t(Tcw), t(frame_cam)
+        d_mp = torch.full((P, cap), -1, dtype=torch.int32, device=dev)
+        d_nm = torch.zeros((P,), dtype=torch.int32, device=dev)
+        store = [d_kps.data_ptr(), d_desc.data_ptr(), d_cnt.data_ptr()]
+        multi = fe.ORBmatcher(0.9, True)
+        singles = [fe.ORBmatcher(0.9, True) for _ in cams]
+        L = M._bind()
+        vp = C.c_void_p
+
+        def reset():
+            with torch.cuda.stream(main):
+                d_mp.fill_(-1)
+
+        def run_multi():
+            reset()
+            M.search_by_projection_cams_device(multi, P, *store, cap, d_cur.data_ptr(), d_last.data_ptr(), d_world.data_ptr(),
+                                               d_flags.data_ptr(), d_T.data_ptr(), table, d_fc.data_ptr(), 1.2, 8, TH,
+                                               d_mp.data_ptr(), d_nm.data_ptr(), main.cuda_stream)
+
+        def run_serial(streams=None):
+            if streams is None:
+                reset()
+            for c, cam in enumerate(table):
+                x0, y0, x1, y1, fx, fy, cx, cy = cam
+                s = streams[c] if streams else main
+                m = singles[c]
+                rc = L.orbfe_search_by_projection_device(m.handle, B, *[vp(p) for p in store], cap, vp(d_cur[c * B].data_ptr()),
+                                                         vp(d_last[c * B].data_ptr()), vp(d_world.data_ptr()), vp(d_flags.data_ptr()),
+                                                         vp(d_T[c * B].data_ptr()), x0, y0, x1, y1, 1.2, 8, fx, fy, cx, cy, TH, 1,
+                                                         vp(d_mp[c * B].data_ptr()), vp(d_nm[c * B:].data_ptr()), vp(s.cuda_stream))
+                assert rc == 0, L.orbfe_last_error()
+
+        def run_streams():
+            reset()
+            fork = torch.cuda.Event()
+            fork.record(main)
+            for s in side:
+                s.wait_event(fork)
+            run_serial(side)
+            for s in side:
+                ev = torch.cuda.Event()
+                ev.record(s)
+                main.wait_event(ev)
+
+        ways = {"cams_one_call": run_multi, "three_calls_one_stream": run_serial, "three_calls_three_streams": run_streams}
+        res = {k: {"event_ms": [], "wall_ms": []} for k in ways}
+        for fn in ways.values():
+            for _ in range(max(args.warmup, 10)):
+                fn()
+        torch.cuda.synchronize()
+        want = None
+        for r in range(rounds):
+            for name, fn in ways.items():
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                e0.record(main)
+                for _ in range(steps):
+                    fn()
+                e1.record(main)
+                e1.synchronize()
+                torch.cuda.synchronize()
+                res[name]["wall_ms"].append((time.perf_counter() - t0) * 1e3 / steps)
+                res[name]["event_ms"].append(e0.elapsed_time(e1) / steps)
+                got = (d_nm.cpu().numpy().tolist(), d_mp.cpu().numpy().tobytes())
+                want = want or got
+                res[name]["same_outputs"] = res[name].get("same_outputs", True) and got == want
+        for m in [multi] + singles:
+            m.sync()
+        out["%d_pair_per_camera" % B] = {k: {"event_ms": round(float(np.median(v["event_ms"])), 4),
+                                             "wall_ms": round(float(np.median(v["wall_ms"])), 4),
+                                             "event_ms_min_max": [round(min(v["event_ms"]), 4), round(max(v["event_ms"]), 4)],
+                                             "same_outputs": v["same_outputs"]} for k, v in res.items()}
+        out["%d_pair_per_camera" % B]["nmatches"] = want[0]
+        multi.close()
+        for m in singles:
+            m.close()
+    _gpu_and_power_limit(out)
     return out
 
 
@@ -1995,4 +2133,4 @@ if __name__ == "__main__":
                           "reloc": reloc, "mapping": mapping, "mapdesc": mapdesc, "kfdb": kfdb, "kfdbbatch": kfdbbatch, "bowchain": bowchain,
                           "windowed": windowed, "guided": guided, "loopscore": loopscore, "vocload": vocload,
                           "normaldepth": normaldepth, "covis": covis, "observations": observations, "kfculling": kfculling,
-                          "localmap": localmap, "multigeom": multigeom}[w](args)))
+                          "localmap": localmap, "multigeom": multigeom, "multitrack": multitrack}[w](args)))
