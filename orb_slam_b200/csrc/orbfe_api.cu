@@ -69,6 +69,31 @@ struct StageTimer {
     bool origin_pending = true;
 };
 
+// One plan of a handle: a level table (PlanDev: one geometry; MultiPlanDev: up to ORBFE_MULTI_MAX_GROUPS) with its level
+// planes, work buffers and the outputs of the host-array entries.  Keyed by the (W, H) list of its groups and the frames
+// each group holds; an empty key means no plan.
+template <class PD>
+struct Plan {
+    std::vector<int> geom, cap;   // key: (W, H) of group g at geom[2g], geom[2g + 1]; cap[g] frames of group g
+    std::unique_ptr<PD> hp;       // host copy (a MultiPlanDev is large: on the heap)
+    PD *dp = nullptr;             // device copy
+    WorkDev work;
+    DeviceBuffers mem;            // every device allocation of the plan
+    void *counters = nullptr;     // cell_cnt_lo | cell_cnt_hi | kept_cnt (zeroed per call)
+    size_t counters_bytes = 0, ls_smem = 0;
+    // level 0 of a group either lives in the plan's own pitched planes or IS the caller's device buffer (no ingest copy)
+    LevelDev own0[ORBFE_MULTI_MAX_GROUPS];
+    OrbfeKeyPoint *d_kps = nullptr;   // outputs of the host-array entries, [sum of cap] frames
+    uint8_t *d_desc = nullptr;
+    int *d_counts = nullptr;
+
+    void release() {
+        mem.release();
+        geom.clear();
+        cap.clear();
+    }
+};
+
 struct OrbfeExtractor {
     int nfeatures = 0, nlevels = 0, score_type = 1, fast_th = 20, device = 0;
     int batch_mode = 0;         // orbfe_extractor_set_batch_mode
@@ -76,44 +101,15 @@ struct OrbfeExtractor {
     float scale[ORBFE_MAX_LEVELS], inv_scale[ORBFE_MAX_LEVELS];
     int quota[ORBFE_MAX_LEVELS];
 
-    // plan
-    int W = 0, H = 0, Bcap = 0;
-    PlanDev hplan;
-    PlanDev *dplan = nullptr;
-    WorkDev work;
-    DeviceBuffers plan_mem;      // device allocations of the current plan
-    void *counters = nullptr;    // cell_cnt_lo | cell_cnt_hi | kept_cnt (zeroed per call)
-    size_t counters_bytes = 0;
-    size_t ls_smem = 0;
+    Plan<PlanDev> single;        // orbfe_extract, orbfe_extract_batch*
+    Plan<MultiPlanDev> multi;    // orbfe_extract_multi*
     int8_t *d_pattern = nullptr;
-    // level 0 either lives in the plan's own pitched planes or IS the caller's device buffer (no ingest copy)
-    uint8_t *own_pyr0 = nullptr;
-    int own_pitch0 = 0;
-    size_t own_plane0 = 0;
-    void *tma_encode = nullptr;      // cuTensorMapEncodeTiled
-    CUtensorMap *d_maps = nullptr;   // [nlevels] in device memory
-    // own outputs (host-API path)
-    OrbfeKeyPoint *d_kps = nullptr;
-    uint8_t *d_desc = nullptr;
-    int *d_counts = nullptr;
-    int *h_counts = nullptr;  // pinned
-    int *h_err = nullptr;     // pinned
+    void *tma_encode = nullptr;  // cuTensorMapEncodeTiled
+    int *h_counts = nullptr;     // pinned
+    int *h_err = nullptr;        // pinned
     size_t h_counts_cap = 0;
 
-    // multi plan (orbfe_extract_multi): keyed by the (W, H) list of its groups, holding mcap[g] frames of group g
-    std::vector<int> mgeom, mcap;
-    MultiPlanDev *mhp = nullptr;     // host copy (large: on the heap)
-    MultiPlanDev *mdp = nullptr;
-    WorkDev mwork;
-    DeviceBuffers mplan_mem;
-    void *mcounters = nullptr;
-    size_t mcounters_bytes = 0, mls_smem = 0;
-    LevelDev mown0[ORBFE_MULTI_MAX_GROUPS];   // each group's level 0 in the plan's own planes
-    OrbfeKeyPoint *md_kps = nullptr;          // own outputs (host-API path), [sum of mcap] frames
-    uint8_t *md_desc = nullptr;
-    int *md_counts = nullptr;
-
-    HandleStream hs;             // every call enters and leaves it, whichever stream it is enqueued on
+    HandleStream hs;            // every call enters and leaves it, whichever stream it is enqueued on
     cudaStream_t copy_stream = nullptr;
     std::vector<cudaEvent_t> chunk_ev;
     int last_launches = 0;
@@ -123,28 +119,6 @@ struct OrbfeExtractor {
     std::vector<float> stage_ms;
     std::vector<std::string> stage_names;
 };
-
-static void free_plan(OrbfeExtractor *ex) {
-    ex->plan_mem.release();
-    ex->dplan = nullptr;
-    ex->own_pyr0 = nullptr; ex->d_maps = nullptr;
-    ex->counters = nullptr;
-    ex->d_kps = nullptr;
-    ex->d_desc = nullptr;
-    ex->d_counts = nullptr;
-    ex->W = ex->H = ex->Bcap = 0;
-}
-
-static void free_multi_plan(OrbfeExtractor *ex) {
-    ex->mplan_mem.release();
-    ex->mdp = nullptr;
-    ex->mcounters = nullptr;
-    ex->md_kps = nullptr;
-    ex->md_desc = nullptr;
-    ex->md_counts = nullptr;
-    ex->mgeom.clear();
-    ex->mcap.clear();
-}
 
 // the pinned block the host-array entries read the counts back into
 static int grow_host_counts(OrbfeExtractor *ex, int n) {
@@ -459,82 +433,139 @@ static void plan_head(const OrbfeExtractor *ex, PlanHead &P, int B) {
     }
 }
 
-static int build_plan(OrbfeExtractor *ex, int W, int H, int B) {
-    if (ex->W == W && ex->H == H && B <= ex->Bcap) return ORBFE_OK;
-    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
-    ORBFE_CUDA_TRY(cudaEventSynchronize(ex->hs.last));   // the handle's pending calls still use the plan
-    free_plan(ex);
-    PlanDev &P = ex->hplan;
-    memset(&P, 0, sizeof(P));
-    plan_head(ex, P, B);
+// Builds `plan` for the groups of the (W, H) list `geom`, cap[g] frames of group g, unless it already holds them: it is
+// rebuilt only when the list changes or a group outgrows its capacity, and a rebuild for the same list keeps every group's
+// old capacity.  All geometries are laid out, on the host, before anything is freed: a refused call leaves the handle's
+// plans as they were.  gidx: the call's index of each group, named in a refusal (NULL: the message names no group).
+template <class PD>
+static int build(OrbfeExtractor *ex, Plan<PD> &plan, const std::vector<int> &geom, std::vector<int> cap, const int *gidx) {
+    const int n = (int)cap.size(), nl = ex->nlevels;
+    if (geom == plan.geom) {
+        bool fits = true;
+        for (int i = 0; i < n; i++) fits = fits && cap[i] <= plan.cap[i];
+        if (fits) return ORBFE_OK;
+        for (int i = 0; i < n; i++) cap[i] = std::max(cap[i], plan.cap[i]);
+    }
+    std::unique_ptr<PD> hp(new PD());
+    PD &P = *hp;
+    int frames = 0;
+    for (int c : cap) frames += c;
+    plan_head(ex, P, frames);
     PlanLayout A;
-    if (int rc = layout_geometry(ex, W, H, P.lv, A)) return rc;
+    for (int i = 0; i < n; i++) {
+        // a geometry's kept lists (quota + 2 * cells + 64) decide its level-select footprint, so that refusal names the group too
+        int rc = layout_geometry(ex, geom[2 * i], geom[2 * i + 1], &P.lv[i * nl], A);
+        if (!rc) {
+            int kept = 0;
+            size_t bytes = 0;
+            for (int l = 0; l < nl; l++) kept = std::max(kept, P.lv[i * nl + l].kept_cap);
+            rc = level_select_smem(ex, kept, &bytes);
+        }
+        if (rc && gidx) {
+            const std::string why = g_err;
+            return fail(rc, "group %d (%dx%d): %s", gidx[i], geom[2 * i], geom[2 * i + 1], why.c_str());
+        }
+        if (rc) return rc;
+        if constexpr (std::is_same<PD, MultiPlanDev>::value) {   // the group table (a PlanDev is one group and has none)
+            GroupDev &G = P.grp[P.ngroups++];
+            G.ftile0 = P.lv[i * nl].ftile_base;
+            G.nftiles = A.ft_base - G.ftile0;
+            G.cell0 = P.lv[i * nl].cell_base;
+            G.ncells = A.cell_base - G.cell0;
+        }
+    }
+    size_t ls = 0;
+    if (int rc = level_select_smem(ex, A.max_kept, &ls)) return rc;
     P.ncells_total = A.cell_base;
     P.nftiles_total = A.ft_base;
     P.nbtiles_total = A.bt_base;
     P.kept_total = A.kept_total;
     P.cand_total = A.cand_total;
     P.nfeatures = A.kp_total;
-    if (int rc = level_select_smem(ex, A.max_kept, &ex->ls_smem)) return rc;
+
     ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
-    if (int rc = set_level_select_attr(ex, ex->ls_smem)) return rc;
-    // ---- device memory ----
+    ORBFE_CUDA_TRY(cudaEventSynchronize(ex->hs.last));   // the handle's pending calls still use the plan
+    plan.release();
+    plan.hp = std::move(hp);
+    if (int rc = set_level_select_attr(ex, ls)) return rc;
+    plan.ls_smem = ls;
     void *fn = nullptr;
     if (int rc = tensor_map_encoder(&fn)) return rc;
     std::vector<FTileInfo> info((size_t)P.nftiles_total);
     std::vector<BTileInfo> binfo((size_t)P.nbtiles_total);
-    std::vector<CUtensorMap> maps(ex->nlevels);
-    if (int rc = alloc_geometry(ex, ex->plan_mem, P.lv, B, 0, fn, info, binfo, maps)) return rc;
-    if (int rc = alloc_work(ex, ex->plan_mem, P, B, A, info, binfo, maps, ex->work, &ex->counters, &ex->counters_bytes)) return rc;
+    std::vector<CUtensorMap> maps((size_t)n * nl);
+    for (int i = 0; i < n; i++) {
+        if (int rc = alloc_geometry(ex, plan.mem, &P.lv[i * nl], cap[i], i * nl, fn, info, binfo, maps)) return rc;
+        plan.own0[i] = P.lv[i * nl];
+    }
+    if (int rc = alloc_work(ex, plan.mem, P, frames, A, info, binfo, maps, plan.work, &plan.counters, &plan.counters_bytes))
+        return rc;
     ex->tma_encode = fn;
-    ex->d_maps = const_cast<CUtensorMap *>(ex->work.tmaps);
-    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->d_kps, (size_t)std::max(P.nfeatures, 1) * B));
-    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->d_desc, (size_t)std::max(P.nfeatures, 1) * B * 32));
-    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->d_counts, (size_t)B));
-    ORBFE_CUDA_TRY(ex->plan_mem.alloc(&ex->dplan, 1));
-    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->dplan, &P, sizeof(P), cudaMemcpyHostToDevice, ex->hs.stream));
-    if (int rc = grow_host_counts(ex, B)) return rc;
+    ORBFE_CUDA_TRY(plan.mem.alloc(&plan.d_kps, (size_t)std::max(P.nfeatures, 1) * frames));
+    ORBFE_CUDA_TRY(plan.mem.alloc(&plan.d_desc, (size_t)std::max(P.nfeatures, 1) * frames * 32));
+    ORBFE_CUDA_TRY(plan.mem.alloc(&plan.d_counts, (size_t)frames));
+    ORBFE_CUDA_TRY(plan.mem.alloc(&plan.dp, 1));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(plan.dp, &P, sizeof(P), cudaMemcpyHostToDevice, ex->hs.stream));
+    if (int rc = grow_host_counts(ex, frames)) return rc;
     ORBFE_CUDA_TRY(cudaStreamSynchronize(ex->hs.stream));
-    ex->W = W; ex->H = H; ex->Bcap = B;
-    ex->own_pyr0 = P.lv[0].pyr; ex->own_pitch0 = P.lv[0].pitch; ex->own_plane0 = P.lv[0].plane;
+    plan.geom = geom;
+    plan.cap = cap;
     ex->plan_builds++;
     return ORBFE_OK;
 }
 
-// Point level 0 of the plan at `ptr` (the plan's own planes, or the caller's device frames when they can be read in place:
-// 16-byte aligned base and strides, as the level-0 tensor map requires).  Stream-ordered: the device copy of the level
-// descriptor and the level-0 tensor map are rewritten on `s` before the kernels that read them.
-static int set_level0(OrbfeExtractor *ex, uint8_t *ptr, int pitch, size_t plane, int batch, cudaStream_t s) {
-    LevelDev &L0 = ex->hplan.lv[0];
+// Point level 0 of group g of `plan` at `ptr` (the plan's own planes, or the caller's device frames read in place).
+// Stream-ordered: the device copy of the level descriptor and the level-0 tensor map are rewritten on `s` before the
+// kernels that read them.
+template <class PD>
+static int bind_level0(OrbfeExtractor *ex, Plan<PD> &plan, int g, uint8_t *ptr, int pitch, size_t plane, cudaStream_t s) {
+    const int v = g * ex->nlevels;
+    LevelDev &L0 = plan.hp->lv[v];
     if (L0.pyr == ptr && L0.pitch == pitch && L0.plane == plane) return ORBFE_OK;
     L0.pyr = ptr; L0.pitch = pitch; L0.plane = plane;
-    ORBFE_CUDA_TRY(cudaMemcpyAsync(&ex->dplan->lv[0], &L0, sizeof(LevelDev), cudaMemcpyHostToDevice, s));
-    if (ex->d_maps && ex->tma_encode) {
-        CUtensorMap m;
-        const CUresult r = encode_level_map(ex->tma_encode, &m, ptr, L0.w, L0.h, std::max(batch, ex->Bcap), pitch, plane);
-        if (r != CUDA_SUCCESS) return fail(ORBFE_ERR_CUDA, "cuTensorMapEncodeTiled(level 0, in place) failed: %d", (int)r);
-        ORBFE_CUDA_TRY(cudaMemcpyAsync(&ex->d_maps[0], &m, sizeof(m), cudaMemcpyHostToDevice, s));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(&plan.dp->lv[v], &L0, sizeof(LevelDev), cudaMemcpyHostToDevice, s));
+    CUtensorMap m;
+    const CUresult r = encode_level_map(ex->tma_encode, &m, ptr, L0.w, L0.h, plan.cap[g], pitch, plane);
+    if (r != CUDA_SUCCESS) return fail(ORBFE_ERR_CUDA, "cuTensorMapEncodeTiled(group %d level 0) failed: %d", g, (int)r);
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(const_cast<CUtensorMap *>(plan.work.tmaps) + v, &m, sizeof(m), cudaMemcpyHostToDevice, s));
+    return ORBFE_OK;
+}
+
+// Device frames can be level 0 as they are (no copy) when the level-0 tensor map takes them: 16-byte aligned base and
+// strides, a row stride that fits an int, frames that do not overlap.  ORBFE_INGEST_COPY=1 copies them always.
+static bool readable_in_place(const uint8_t *imgs, int height, size_t stride, size_t frame_stride) {
+    return !getenv("ORBFE_INGEST_COPY") && (uintptr_t)imgs % 16 == 0 && stride % 16 == 0 && frame_stride % 16 == 0 &&
+           stride <= (size_t)INT_MAX && frame_stride >= stride * (size_t)height;
+}
+
+// Frames [f0, f1) of the caller's frames into the same frames of level 0 L0: one linear copy when both sides are fully
+// contiguous, one 2-D copy when the frames of each side follow each other row after row, else one 2-D copy per frame.
+static int copy_frames(const LevelDev &L0, const uint8_t *src, int width, int height, size_t stride, size_t frame_stride, int f0,
+                       int f1, cudaMemcpyKind kind, cudaStream_t s) {
+    uint8_t *dst = L0.pyr + (size_t)f0 * L0.plane;
+    src += (size_t)f0 * frame_stride;
+    const bool rows = frame_stride == stride * (size_t)height && L0.plane == (size_t)L0.pitch * height;
+    if (rows && stride == (size_t)width && L0.pitch == width) {
+        ORBFE_CUDA_TRY(cudaMemcpyAsync(dst, src, (size_t)width * height * (f1 - f0), kind, s));
+    } else if (rows) {
+        ORBFE_CUDA_TRY(cudaMemcpy2DAsync(dst, L0.pitch, src, stride, width, (size_t)height * (f1 - f0), kind, s));
+    } else {
+        for (int f = 0; f < f1 - f0; f++)
+            ORBFE_CUDA_TRY(cudaMemcpy2DAsync(dst + f * L0.plane, L0.pitch, src + f * frame_stride, stride, width, height, kind, s));
     }
     return ORBFE_OK;
 }
 
-// Level 0 = the caller's device frames (no copy) when base and strides are 16-byte aligned; else a 2-D copy into the plan's planes.
-static int ingest_device(OrbfeExtractor *ex, const uint8_t *d_imgs, int width, int height, size_t stride, size_t frame_stride, int batch,
-                         cudaStream_t s) {
-    const bool in_place = !getenv("ORBFE_INGEST_COPY") && ((uintptr_t)d_imgs % 16 == 0) && stride % 16 == 0 && frame_stride % 16 == 0 &&
-                          stride <= (size_t)INT_MAX && frame_stride >= stride * (size_t)height;
-    if (in_place) return set_level0(ex, const_cast<uint8_t *>(d_imgs), (int)stride, frame_stride, batch, s);
-    int rc = set_level0(ex, ex->own_pyr0, ex->own_pitch0, ex->own_plane0, batch, s);
-    if (rc) return rc;
-    const LevelDev &L0 = ex->hplan.lv[0];
-    if (frame_stride == stride * (size_t)height && L0.plane == (size_t)L0.pitch * height) {
-        ORBFE_CUDA_TRY(cudaMemcpy2DAsync(L0.pyr, L0.pitch, d_imgs, stride, width, (size_t)height * batch, cudaMemcpyDeviceToDevice, s));
-    } else {
-        for (int f = 0; f < batch; f++)
-            ORBFE_CUDA_TRY(cudaMemcpy2DAsync(L0.pyr + f * L0.plane, L0.pitch, d_imgs + f * frame_stride, stride, width, height,
-                                     cudaMemcpyDeviceToDevice, s));
-    }
-    return ORBFE_OK;
+// Level 0 of group g for `nframes` frames on s: the caller's device frames read in place when they can be, else copied
+// (host frames: uploaded) into the plan's own planes
+template <class PD>
+static int ingest(OrbfeExtractor *ex, Plan<PD> &plan, int g, const uint8_t *imgs, int width, int height, size_t stride,
+                  size_t frame_stride, int nframes, cudaMemcpyKind kind, cudaStream_t s) {
+    if (kind == cudaMemcpyDeviceToDevice && readable_in_place(imgs, height, stride, frame_stride))
+        return bind_level0(ex, plan, g, const_cast<uint8_t *>(imgs), (int)stride, frame_stride, s);
+    const LevelDev &own = plan.own0[g];
+    if (int rc = bind_level0(ex, plan, g, own.pyr, own.pitch, own.plane, s)) return rc;
+    return copy_frames(own, imgs, width, height, stride, frame_stride, 0, nframes, kind, s);
 }
 
 extern "C" int orbfe_extractor_create(int nfeatures, float scale_factor, int nlevels, int score_type, int fast_th,
@@ -593,9 +624,8 @@ extern "C" int orbfe_extractor_destroy(OrbfeExtractor *ex) {
     cudaSetDevice(ex->device);
     if (ex->hs.last) cudaEventSynchronize(ex->hs.last);
     if (ex->hs.stream) cudaStreamSynchronize(ex->hs.stream);
-    free_plan(ex);
-    free_multi_plan(ex);
-    delete ex->mhp;
+    ex->single.release();
+    ex->multi.release();
     if (ex->d_pattern) cudaFree(ex->d_pattern);
     if (ex->h_counts) cudaFreeHost(ex->h_counts);
     if (ex->h_err) cudaFreeHost(ex->h_err);
@@ -633,34 +663,37 @@ static void stage_mark(OrbfeExtractor *ex, cudaStream_t s, const char *name) {
     cudaEventRecord(T.ev[i + 1], s);
 }
 
-// Enqueue the device pipeline for frames [f0, f0+nf) whose level-0 images are already in lv[0].pyr.
-// The per-call counters must have been zeroed (zero_counters) before the first chunk.
-static int zero_counters(OrbfeExtractor *ex, cudaStream_t s) {
-    ORBFE_CUDA_TRY(cudaMemsetAsync(ex->counters, 0, ex->counters_bytes, s));
+// The per-call counters of a plan, zeroed on s before the call's first launch
+template <class PD>
+static int zero_counters(const Plan<PD> &plan, cudaStream_t s) {
+    ORBFE_CUDA_TRY(cudaMemsetAsync(plan.counters, 0, plan.counters_bytes, s));
     return ORBFE_OK;
 }
 
 static void enqueue_pyramid(OrbfeExtractor *ex, int f0, int nf, cudaStream_t s) {
-    const PlanDev &hp = ex->hplan;
-    for (int l = 1; l < hp.nlevels; l++) launch_resize_level(ex->dplan, hp, l, f0, nf, s);
+    const PlanDev &hp = *ex->single.hp;
+    for (int l = 1; l < hp.nlevels; l++) launch_resize_level(ex->single.dp, hp, l, f0, nf, s);
     ex->last_launches += hp.nlevels - 1;
     stage_mark(ex, s, "pyramid");
 }
 
+// Enqueue the device pipeline for frames [f0, f0+nf) whose level-0 images are already in lv[0].pyr.
+// The per-call counters must have been zeroed (zero_counters) before the first chunk.
 static int enqueue_pipeline(OrbfeExtractor *ex, int f0, int nf, OrbfeKeyPoint *d_kps, uint8_t *d_desc, int *d_counts,
                             cudaStream_t s, bool with_pyramid = true, const PeerOut *peers = nullptr) {
-    const PlanDev &hp = ex->hplan;
+    const Plan<PlanDev> &P = ex->single;
+    const PlanDev &hp = *P.hp;
     int launches = 0;
     if (with_pyramid) enqueue_pyramid(ex, f0, nf, s);
-    launch_fast_nms(ex->dplan, hp, ex->work, f0, nf, s); launches++;
+    launch_fast_nms(P.dp, hp, P.work, f0, nf, s); launches++;
     stage_mark(ex, s, "fast_nms");
-    launch_cell_quota(ex->dplan, hp, ex->work, f0, nf, s); launches++;
+    launch_cell_quota(P.dp, hp, P.work, f0, nf, s); launches++;
     stage_mark(ex, s, "cell_quota");
-    launch_cell_select(ex->dplan, hp, ex->work, f0, nf, s); launches++;
+    launch_cell_select(P.dp, hp, P.work, f0, nf, s); launches++;
     stage_mark(ex, s, "cell_select");
-    launch_level_select(ex->dplan, hp, ex->work, ex->ls_smem, f0, nf, s); launches++;
+    launch_level_select(P.dp, hp, P.work, P.ls_smem, f0, nf, s); launches++;
     stage_mark(ex, s, "level_select");
-    launch_describe_fused(ex->dplan, hp, ex->work, ex->d_pattern, d_kps, d_desc, d_counts, f0, nf, s, peers); launches++;
+    launch_describe_fused(P.dp, hp, P.work, ex->d_pattern, d_kps, d_desc, d_counts, f0, nf, s, peers); launches++;
     stage_mark(ex, s, "describe");
     ORBFE_CUDA_TRY(cudaGetLastError());
     ex->last_launches += launches;
@@ -689,6 +722,45 @@ static void profiling_collect(OrbfeExtractor *ex) {
     T.origin_pending = true;
 }
 
+// Frames [frame0, frame0 + n) of a plan's outputs: the caller's frames from `out` on
+struct FrameRun { int frame0, n, out; };
+
+// The end of both host-array entries, enqueued on s after their launches: the counts, the overflow flag and each run's
+// keypoints and descriptors (one 2-D copy each, `cap` slots per caller frame) back to the host; then the wait for them and
+// the caller's counts.
+template <class PD>
+static int read_back(OrbfeExtractor *ex, const Plan<PD> &plan, const std::vector<FrameRun> &runs, OrbfeKeyPoint *kps, uint8_t *desc,
+                     int cap, int *n_out, cudaStream_t s) {
+    const int nf = plan.hp->nfeatures, ncopy = std::min(cap, nf);
+    int frames = 0;
+    for (const FrameRun &r : runs) frames += r.n;
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->h_counts, plan.d_counts, sizeof(int) * frames, cudaMemcpyDeviceToHost, s));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->h_err, plan.work.err_flag, sizeof(int), cudaMemcpyDeviceToHost, s));
+    for (size_t i = 0; ncopy > 0 && i < runs.size(); i++) {
+        const FrameRun &r = runs[i];
+        ORBFE_CUDA_TRY(cudaMemcpy2DAsync(kps + (size_t)r.out * cap, sizeof(OrbfeKeyPoint) * cap, plan.d_kps + (size_t)r.frame0 * nf,
+                                         sizeof(OrbfeKeyPoint) * nf, sizeof(OrbfeKeyPoint) * ncopy, r.n, cudaMemcpyDeviceToHost, s));
+        ORBFE_CUDA_TRY(cudaMemcpy2DAsync(desc + (size_t)r.out * cap * 32, (size_t)32 * cap, plan.d_desc + (size_t)r.frame0 * nf * 32,
+                                         (size_t)32 * nf, (size_t)32 * ncopy, r.n, cudaMemcpyDeviceToHost, s));
+    }
+    stage_mark(ex, s, "d2h");
+    if (int rc = ex->hs.leave(s, true)) return rc;
+    if (*ex->h_err) {
+        const int code = *ex->h_err;
+        cudaMemsetAsync(plan.work.err_flag, 0, sizeof(int), s);
+        ex->hs.leave(s, false);
+        return fail(ORBFE_ERR_INTERNAL, "device overflow flag %d", code);
+    }
+    int status = ORBFE_OK;
+    for (const FrameRun &r : runs)
+        for (int f = 0; f < r.n; f++) {
+            n_out[r.out + f] = ex->h_counts[r.frame0 + f];
+            if (n_out[r.out + f] > cap) status = ORBFE_ERR_CAPACITY;
+        }
+    if (status) return fail(status, "caller capacity %d too small", cap);
+    return ORBFE_OK;
+}
+
 // Head of both device-resident extract entries: the plan for this geometry, then on *s (the caller's stream, or the handle's),
 // behind the handle's earlier calls, level 0 taken from the caller's device frames and the per-call counters zeroed.  The
 // entry leaves the handle's stream after its last launch.
@@ -696,16 +768,16 @@ static int begin_device_extract(OrbfeExtractor *ex, const uint8_t *d_imgs, int w
                                 int batch, void *stream, cudaStream_t *s) {
     if (width <= 0 || height <= 0 || batch <= 0 || stride < (size_t)width) return fail(ORBFE_ERR_ARG, "bad geometry");
     ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
-    int rc = build_plan(ex, width, height, batch);
+    int rc = build(ex, ex->single, {width, height}, {batch}, nullptr);
     if (rc) return rc;
     *s = ex->hs.pick(stream);
     if ((rc = ex->hs.enter(*s))) return rc;
     profiling_begin(ex, *s);
-    rc = ingest_device(ex, d_imgs, width, height, stride, frame_stride, batch, *s);
+    rc = ingest(ex, ex->single, 0, d_imgs, width, height, stride, frame_stride, batch, cudaMemcpyDeviceToDevice, *s);
     if (rc) return rc;
     stage_mark(ex, *s, "ingest");
     ex->last_launches = 0;
-    return zero_counters(ex, *s);
+    return zero_counters(ex->single, *s);
 }
 
 extern "C" int orbfe_extract_batch_device(OrbfeExtractor *ex, const uint8_t *d_imgs, int width, int height,
@@ -725,9 +797,9 @@ int orbfe_extract_batch_device_peers(OrbfeExtractor *ex, const uint8_t *d_imgs, 
     if (!ex || !d_imgs) return fail(ORBFE_ERR_ARG, "NULL argument");
     cudaStream_t s;
     if (int rc = begin_device_extract(ex, d_imgs, width, height, stride, frame_stride, batch, stream, &s)) return rc;
-    if (cap != ex->hplan.nfeatures) {
+    if (cap != ex->single.hp->nfeatures) {
         ex->hs.leave(s, false);   // the ingest is enqueued
-        return fail(ORBFE_ERR_ARG, "exchange capacity %d != keypoint slots per frame %d", cap, ex->hplan.nfeatures);
+        return fail(ORBFE_ERR_ARG, "exchange capacity %d != keypoint slots per frame %d", cap, ex->single.hp->nfeatures);
     }
     if (int rc = enqueue_pipeline(ex, 0, batch, nullptr, nullptr, nullptr, s, true, &po)) return rc;
     return ex->hs.leave(s, false);
@@ -741,17 +813,17 @@ extern "C" int orbfe_extract_batch(OrbfeExtractor *ex, const uint8_t *imgs, int 
     if (!imgs || width <= 0 || height <= 0) return ORBFE_OK;  // empty image: silent return (ORBextractor.cc:721-722)
     if (batch <= 0 || stride < (size_t)width || cap < 0 || (cap > 0 && (!kps || !desc))) return fail(ORBFE_ERR_ARG, "bad arguments");
     ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
-    int rc = build_plan(ex, width, height, batch);
+    Plan<PlanDev> &P = ex->single;
+    int rc = build(ex, P, {width, height}, {batch}, nullptr);
     if (rc) return rc;
     cudaStream_t s = ex->hs.stream;
     if ((rc = ex->hs.enter(s))) return rc;
-    rc = set_level0(ex, ex->own_pyr0, ex->own_pitch0, ex->own_plane0, batch, s);   // the uploads land in the plan's own planes
+    const LevelDev &own = P.own0[0];
+    rc = bind_level0(ex, P, 0, own.pyr, own.pitch, own.plane, s);   // the uploads land in the plan's own planes
     if (rc) return rc;
-    const PlanDev &P = ex->hplan;
-    const LevelDev &L0 = P.lv[0];
     profiling_begin(ex, s);
     ex->last_launches = 0;
-    rc = zero_counters(ex, s);
+    rc = zero_counters(P, s);
     if (rc) return rc;
     // H2D of chunk k+1 (copy stream) overlaps the kernels of chunk k (compute stream)
     int nchunks = batch >= 8 ? 4 : 1;   // H100, 400 W (64 x 1080p, bench.py's three handles): 1, 2 and 4 chunks within 2 % (37.4-38.1 Mkp/s end to end)
@@ -769,55 +841,21 @@ extern "C" int orbfe_extract_batch(OrbfeExtractor *ex, const uint8_t *imgs, int 
     for (int k = 0; k < nchunks; k++) {
         const int f0 = (int)((long long)batch * k / nchunks), f1 = (int)((long long)batch * (k + 1) / nchunks);
         if (f1 <= f0) continue;
-        if (frame_stride == stride * (size_t)height && stride == (size_t)width && L0.pitch == width) {
-            // fully contiguous on both sides: one linear DMA
-            ORBFE_CUDA_TRY(cudaMemcpyAsync(L0.pyr + (size_t)f0 * L0.plane, imgs + (size_t)f0 * frame_stride, (size_t)width * height * (f1 - f0),
-                                   cudaMemcpyHostToDevice, ex->copy_stream));
-        } else if (frame_stride == stride * (size_t)height) {
-            ORBFE_CUDA_TRY(cudaMemcpy2DAsync(L0.pyr + (size_t)f0 * L0.plane, L0.pitch, imgs + (size_t)f0 * frame_stride, stride, width,
-                                     (size_t)height * (f1 - f0), cudaMemcpyHostToDevice, ex->copy_stream));
-        } else {
-            for (int f = f0; f < f1; f++)
-                ORBFE_CUDA_TRY(cudaMemcpy2DAsync(L0.pyr + f * L0.plane, L0.pitch, imgs + f * frame_stride, stride, width, height,
-                                         cudaMemcpyHostToDevice, ex->copy_stream));
-        }
+        if ((rc = copy_frames(own, imgs, width, height, stride, frame_stride, f0, f1, cudaMemcpyHostToDevice, ex->copy_stream))) return rc;
         ORBFE_CUDA_TRY(cudaEventRecord(ex->chunk_ev[k], ex->copy_stream));
         ORBFE_CUDA_TRY(cudaStreamWaitEvent(s, ex->chunk_ev[k], 0));
         if (ex->batch_mode == 1) {
             enqueue_pyramid(ex, f0, f1 - f0, s);   // phased: only the pyramids follow the upload chunk by chunk
         } else {
-            rc = enqueue_pipeline(ex, f0, f1 - f0, ex->d_kps, ex->d_desc, ex->d_counts, s);
+            rc = enqueue_pipeline(ex, f0, f1 - f0, P.d_kps, P.d_desc, P.d_counts, s);
             if (rc) return rc;
         }
     }
     if (ex->batch_mode == 1) {   // ... detection and description run once over the whole batch (full-size launches)
-        rc = enqueue_pipeline(ex, 0, batch, ex->d_kps, ex->d_desc, ex->d_counts, s, false);
+        rc = enqueue_pipeline(ex, 0, batch, P.d_kps, P.d_desc, P.d_counts, s, false);
         if (rc) return rc;
     }
-    const int ncopy = std::min(cap, P.nfeatures);
-    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->h_counts, ex->d_counts, sizeof(int) * batch, cudaMemcpyDeviceToHost, s));
-    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->h_err, ex->work.err_flag, sizeof(int), cudaMemcpyDeviceToHost, s));
-    if (ncopy > 0) {
-        ORBFE_CUDA_TRY(cudaMemcpy2DAsync(kps, sizeof(OrbfeKeyPoint) * cap, ex->d_kps, sizeof(OrbfeKeyPoint) * P.nfeatures,
-                                 sizeof(OrbfeKeyPoint) * ncopy, batch, cudaMemcpyDeviceToHost, s));
-        ORBFE_CUDA_TRY(cudaMemcpy2DAsync(desc, (size_t)32 * cap, ex->d_desc, (size_t)32 * P.nfeatures, (size_t)32 * ncopy, batch,
-                                 cudaMemcpyDeviceToHost, s));
-    }
-    stage_mark(ex, s, "d2h");
-    if ((rc = ex->hs.leave(s, true))) return rc;
-    if (*ex->h_err) {
-        int code = *ex->h_err;
-        cudaMemsetAsync(ex->work.err_flag, 0, sizeof(int), s);
-        ex->hs.leave(s, false);
-        return fail(ORBFE_ERR_INTERNAL, "device overflow flag %d", code);
-    }
-    int status = ORBFE_OK;
-    for (int f = 0; f < batch; f++) {
-        n_out[f] = ex->h_counts[f];
-        if (n_out[f] > cap) status = ORBFE_ERR_CAPACITY;
-    }
-    if (status) return fail(status, "caller capacity %d too small", cap);
-    return ORBFE_OK;
+    return read_back(ex, P, {{0, batch, 0}}, kps, desc, cap, n_out, s);
 }
 
 extern "C" int orbfe_extract(OrbfeExtractor *ex, const uint8_t *img, int width, int height, size_t stride,
@@ -848,117 +886,28 @@ static int check_groups(const OrbfeExtractor *ex, int ngroups, const OrbfeImageG
     return ORBFE_OK;
 }
 
-// The multi plan for the non-empty groups of a call.  It is rebuilt only when their (W, H) list changes or a group has more
-// frames than the plan holds (then every group keeps at least its old capacity).  All geometries are laid out, on the host,
-// before anything is freed: a rejected group leaves both plans of the handle as they were.
-static int build_multi_plan(OrbfeExtractor *ex, int ngroups, const OrbfeImageGroup *groups) {
-    std::vector<int> geom, want, gidx;
+// The multi plan for the non-empty groups of a call, keyed by their (W, H) list (a call without one plans nothing)
+static int build_multi(OrbfeExtractor *ex, int ngroups, const OrbfeImageGroup *groups) {
+    std::vector<int> geom, cap, gidx;
     for (int g = 0; g < ngroups; g++) {
         if (group_empty(groups[g])) continue;
         geom.push_back(groups[g].width);
         geom.push_back(groups[g].height);
-        want.push_back(groups[g].batch);
+        cap.push_back(groups[g].batch);
         gidx.push_back(g);
     }
-    const int n = (int)want.size(), nl = ex->nlevels;
-    if (n == 0) return ORBFE_OK;
-    if (geom == ex->mgeom) {
-        bool fits = true;
-        for (int i = 0; i < n; i++) fits = fits && want[i] <= ex->mcap[i];
-        if (fits) return ORBFE_OK;
-        for (int i = 0; i < n; i++) want[i] = std::max(want[i], ex->mcap[i]);
-    }
-    std::unique_ptr<MultiPlanDev> M(new MultiPlanDev());
-    memset(M.get(), 0, sizeof(MultiPlanDev));
-    plan_head(ex, *M, 0);
-    PlanLayout A;
-    for (int i = 0; i < n; i++) {
-        // a geometry's kept lists (quota + 2 * cells + 64) decide its level-select footprint, so that refusal names the group too
-        int rc = layout_geometry(ex, geom[2 * i], geom[2 * i + 1], &M->lv[i * nl], A);
-        if (!rc) {
-            int kept = 0;
-            size_t bytes = 0;
-            for (int l = 0; l < nl; l++) kept = std::max(kept, M->lv[i * nl + l].kept_cap);
-            rc = level_select_smem(ex, kept, &bytes);
-        }
-        if (rc) {
-            const std::string why = g_err;
-            return fail(rc, "group %d (%dx%d): %s", gidx[i], geom[2 * i], geom[2 * i + 1], why.c_str());
-        }
-        GroupDev &G = M->grp[i];
-        G.ftile0 = M->lv[i * nl].ftile_base;
-        G.nftiles = A.ft_base - G.ftile0;
-        G.cell0 = M->lv[i * nl].cell_base;
-        G.ncells = A.cell_base - G.cell0;
-    }
-    size_t ls = 0;
-    if (int rc = level_select_smem(ex, A.max_kept, &ls)) return rc;
-    M->ngroups = n;
-    M->ncells_total = A.cell_base;
-    M->nftiles_total = A.ft_base;
-    M->nbtiles_total = A.bt_base;
-    M->kept_total = A.kept_total;
-    M->cand_total = A.cand_total;
-    M->nfeatures = A.kp_total;
-    int frames = 0;
-    for (int i = 0; i < n; i++) frames += want[i];
-    M->batch = frames;
-
-    ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
-    ORBFE_CUDA_TRY(cudaEventSynchronize(ex->hs.last));   // the handle's pending calls still use the plan
-    free_multi_plan(ex);
-    delete ex->mhp;
-    ex->mhp = M.release();
-    MultiPlanDev &P = *ex->mhp;
-    if (int rc = set_level_select_attr(ex, ls)) return rc;
-    ex->mls_smem = ls;
-    void *fn = nullptr;
-    if (int rc = tensor_map_encoder(&fn)) return rc;
-    std::vector<FTileInfo> info((size_t)P.nftiles_total);
-    std::vector<BTileInfo> binfo((size_t)P.nbtiles_total);
-    std::vector<CUtensorMap> maps((size_t)n * nl);
-    for (int i = 0; i < n; i++) {
-        if (int rc = alloc_geometry(ex, ex->mplan_mem, &P.lv[i * nl], want[i], i * nl, fn, info, binfo, maps)) return rc;
-        ex->mown0[i] = P.lv[i * nl];
-    }
-    if (int rc = alloc_work(ex, ex->mplan_mem, P, frames, A, info, binfo, maps, ex->mwork, &ex->mcounters, &ex->mcounters_bytes))
-        return rc;
-    ex->tma_encode = fn;
-    ORBFE_CUDA_TRY(ex->mplan_mem.alloc(&ex->md_kps, (size_t)std::max(P.nfeatures, 1) * frames));
-    ORBFE_CUDA_TRY(ex->mplan_mem.alloc(&ex->md_desc, (size_t)std::max(P.nfeatures, 1) * frames * 32));
-    ORBFE_CUDA_TRY(ex->mplan_mem.alloc(&ex->md_counts, (size_t)frames));
-    ORBFE_CUDA_TRY(ex->mplan_mem.alloc(&ex->mdp, 1));
-    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->mdp, &P, sizeof(P), cudaMemcpyHostToDevice, ex->hs.stream));
-    ORBFE_CUDA_TRY(cudaStreamSynchronize(ex->hs.stream));
-    ex->mgeom = geom;
-    ex->mcap = want;
-    ex->plan_builds++;
-    return ORBFE_OK;
+    return cap.empty() ? ORBFE_OK : build(ex, ex->multi, geom, cap, gidx.data());
 }
 
-// Point group i's level 0 at `ptr` (the caller's frames, or the plan's own planes); stream-ordered like set_level0
-static int set_group_level0(OrbfeExtractor *ex, int i, uint8_t *ptr, int pitch, size_t plane, cudaStream_t s) {
-    const int v = i * ex->nlevels;
-    LevelDev &L0 = ex->mhp->lv[v];
-    if (L0.pyr == ptr && L0.pitch == pitch && L0.plane == plane) return ORBFE_OK;
-    L0.pyr = ptr; L0.pitch = pitch; L0.plane = plane;
-    ORBFE_CUDA_TRY(cudaMemcpyAsync(&ex->mdp->lv[v], &L0, sizeof(LevelDev), cudaMemcpyHostToDevice, s));
-    CUtensorMap m;
-    const CUresult r = encode_level_map(ex->tma_encode, &m, ptr, L0.w, L0.h, ex->mcap[i], pitch, plane);
-    if (r != CUDA_SUCCESS) return fail(ORBFE_ERR_CUDA, "cuTensorMapEncodeTiled(group %d level 0) failed: %d", i, (int)r);
-    ORBFE_CUDA_TRY(cudaMemcpyAsync(const_cast<CUtensorMap *>(ex->mwork.tmaps) + v, &m, sizeof(m), cudaMemcpyHostToDevice, s));
-    return ORBFE_OK;
-}
-
-// On s, after the handle's earlier calls: this call's frame and work ranges of the planned groups, their level 0 (device
-// frames read in place when base and strides are 16-byte aligned, else copied, host frames uploaded into the plan's own
-// planes) and the zeroed counters.  Device outputs (d_counts != NULL): a group's frames are written at their place in the
-// call, and the counts of empty groups are zeroed here; host outputs: the planned frames are written packed, and out_frame[i]
-// receives the call's frame of planned group i's first frame.  Returns the number of planned frames in *planned.
+// On s, after the handle's earlier calls: this call's frame and work ranges of the planned groups, their level 0 (ingest)
+// and the zeroed counters.  Device outputs (d_counts != NULL): a group's frames are written at their place in the call, and
+// the counts of empty groups are zeroed here; host outputs: the planned frames are written packed.  runs[i]: planned group
+// i's frames in the plan's outputs and the call's frame of its first frame.
 static int begin_multi(OrbfeExtractor *ex, int ngroups, const OrbfeImageGroup *groups, bool host, int *d_counts, cudaStream_t s,
-                       std::vector<int> &out_frame, int *planned) {
+                       std::vector<FrameRun> &runs) {
+    Plan<MultiPlanDev> &P = ex->multi;
     int i = 0, frame = 0, out = 0, fw = 0, cw = 0;
-    out_frame.clear();
+    runs.clear();
     for (int g = 0; g < ngroups; g++) {
         const OrbfeImageGroup &Gi = groups[g];
         if (group_empty(Gi)) {
@@ -966,8 +915,7 @@ static int begin_multi(OrbfeExtractor *ex, int ngroups, const OrbfeImageGroup *g
             out += Gi.batch;
             continue;
         }
-        MultiPlanDev &M = *ex->mhp;
-        GroupDev &G = M.grp[i];
+        GroupDev &G = P.hp->grp[i];
         G.frame0 = frame;
         G.nframes = Gi.batch;
         G.out0 = host ? frame : out;
@@ -975,49 +923,39 @@ static int begin_multi(OrbfeExtractor *ex, int ngroups, const OrbfeImageGroup *g
         G.cwork0 = cw;
         fw += G.nftiles * Gi.batch;
         cw += G.ncells * Gi.batch;
-        out_frame.push_back(out);
-        const LevelDev &own = ex->mown0[i];
-        const bool in_place = !host && !getenv("ORBFE_INGEST_COPY") && ((uintptr_t)Gi.imgs % 16 == 0) && Gi.stride % 16 == 0 &&
-                              Gi.frame_stride % 16 == 0 && Gi.stride <= (size_t)INT_MAX && Gi.frame_stride >= Gi.stride * (size_t)Gi.height;
-        if (in_place) {
-            if (int rc = set_group_level0(ex, i, const_cast<uint8_t *>(Gi.imgs), (int)Gi.stride, Gi.frame_stride, s)) return rc;
-        } else {
-            if (int rc = set_group_level0(ex, i, own.pyr, own.pitch, own.plane, s)) return rc;
-            const cudaMemcpyKind kind = host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
-            for (int f = 0; f < Gi.batch; f++)
-                ORBFE_CUDA_TRY(cudaMemcpy2DAsync(own.pyr + f * own.plane, own.pitch, Gi.imgs + f * Gi.frame_stride, Gi.stride, Gi.width,
-                                                 Gi.height, kind, s));
-        }
+        runs.push_back({frame, Gi.batch, out});
+        if (int rc = ingest(ex, P, i, Gi.imgs, Gi.width, Gi.height, Gi.stride, Gi.frame_stride, Gi.batch,
+                            host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, s))
+            return rc;
         frame += Gi.batch;
         out += Gi.batch;
         i++;
     }
-    *planned = frame;
     if (frame == 0) return ORBFE_OK;
-    MultiPlanDev &M = *ex->mhp;
+    MultiPlanDev &M = *P.hp;
     M.nframes = frame;
     M.nfwork = fw;
     M.ncwork = cw;
-    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->mdp->grp, M.grp, sizeof(M.grp), cudaMemcpyHostToDevice, s));
+    ORBFE_CUDA_TRY(cudaMemcpyAsync(P.dp->grp, M.grp, sizeof(M.grp), cudaMemcpyHostToDevice, s));
     stage_mark(ex, s, "ingest");
-    ORBFE_CUDA_TRY(cudaMemsetAsync(ex->mcounters, 0, ex->mcounters_bytes, s));
-    return ORBFE_OK;
+    return zero_counters(P, s);
 }
 
 // One launch per stage for all groups: nlevels - 1 resizes, then FAST, quota, cell select, level select, describe
 static int enqueue_multi(OrbfeExtractor *ex, OrbfeKeyPoint *d_kps, uint8_t *d_desc, int *d_counts, cudaStream_t s) {
-    const MultiPlanDev &M = *ex->mhp;
-    for (int l = 1; l < M.nlevels; l++) launch_resize_level_multi(ex->mdp, M, l, s);
+    const Plan<MultiPlanDev> &P = ex->multi;
+    const MultiPlanDev &M = *P.hp;
+    for (int l = 1; l < M.nlevels; l++) launch_resize_level_multi(P.dp, M, l, s);
     stage_mark(ex, s, "pyramid");
-    launch_fast_nms_multi(ex->mdp, M, ex->mwork, s);
+    launch_fast_nms_multi(P.dp, M, P.work, s);
     stage_mark(ex, s, "fast_nms");
-    launch_cell_quota_multi(ex->mdp, M, ex->mwork, s);
+    launch_cell_quota_multi(P.dp, M, P.work, s);
     stage_mark(ex, s, "cell_quota");
-    launch_cell_select_multi(ex->mdp, M, ex->mwork, s);
+    launch_cell_select_multi(P.dp, M, P.work, s);
     stage_mark(ex, s, "cell_select");
-    launch_level_select_multi(ex->mdp, M, ex->mwork, ex->mls_smem, s);
+    launch_level_select_multi(P.dp, M, P.work, P.ls_smem, s);
     stage_mark(ex, s, "level_select");
-    launch_describe_multi(ex->mdp, M, ex->mwork, ex->d_pattern, d_kps, d_desc, d_counts, s);
+    launch_describe_multi(P.dp, M, P.work, ex->d_pattern, d_kps, d_desc, d_counts, s);
     stage_mark(ex, s, "describe");
     ORBFE_CUDA_TRY(cudaGetLastError());
     ex->last_launches += M.nlevels + 4;
@@ -1026,67 +964,40 @@ static int enqueue_multi(OrbfeExtractor *ex, OrbfeKeyPoint *d_kps, uint8_t *d_de
 
 extern "C" int orbfe_extract_multi_device(OrbfeExtractor *ex, int ngroups, const OrbfeImageGroup *groups, OrbfeKeyPoint *d_kps,
                                           uint8_t *d_desc, int *d_counts, void *stream) {
-    int frames = 0, planned = 0;
+    int frames = 0;
     if (int rc = check_groups(ex, ngroups, groups, &frames)) return rc;
     if (!d_kps || !d_desc || !d_counts) return fail(ORBFE_ERR_ARG, "NULL output");
     ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
-    if (int rc = build_multi_plan(ex, ngroups, groups)) return rc;
+    if (int rc = build_multi(ex, ngroups, groups)) return rc;
     const cudaStream_t s = ex->hs.pick(stream);
     if (int rc = ex->hs.enter(s)) return rc;
     profiling_begin(ex, s);
     ex->last_launches = 0;
-    std::vector<int> out_frame;
-    if (int rc = begin_multi(ex, ngroups, groups, false, d_counts, s, out_frame, &planned)) return rc;
-    if (planned)
+    std::vector<FrameRun> runs;
+    if (int rc = begin_multi(ex, ngroups, groups, false, d_counts, s, runs)) return rc;
+    if (!runs.empty())
         if (int rc = enqueue_multi(ex, d_kps, d_desc, d_counts, s)) return rc;
     return ex->hs.leave(s, false);
 }
 
 extern "C" int orbfe_extract_multi(OrbfeExtractor *ex, int ngroups, const OrbfeImageGroup *groups, OrbfeKeyPoint *kps,
                                    uint8_t *desc, int cap, int *n_out) {
-    int frames = 0, planned = 0;
+    int frames = 0;
     if (int rc = check_groups(ex, ngroups, groups, &frames)) return rc;
     if (!n_out || cap < 0 || (cap > 0 && (!kps || !desc))) return fail(ORBFE_ERR_ARG, "bad output arguments");
     for (int f = 0; f < frames; f++) n_out[f] = 0;
     ORBFE_CUDA_TRY(cudaSetDevice(ex->device));
-    if (int rc = build_multi_plan(ex, ngroups, groups)) return rc;
-    if (int rc = grow_host_counts(ex, frames)) return rc;
+    if (int rc = build_multi(ex, ngroups, groups)) return rc;
     const cudaStream_t s = ex->hs.stream;
     if (int rc = ex->hs.enter(s)) return rc;
     profiling_begin(ex, s);
     ex->last_launches = 0;
-    std::vector<int> out_frame;
-    if (int rc = begin_multi(ex, ngroups, groups, true, nullptr, s, out_frame, &planned)) return rc;
-    if (!planned) return ex->hs.leave(s, false);
-    if (int rc = enqueue_multi(ex, ex->md_kps, ex->md_desc, ex->md_counts, s)) return rc;
-    const MultiPlanDev &M = *ex->mhp;
-    const int nf = M.nfeatures, ncopy = std::min(cap, nf);
-    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->h_counts, ex->md_counts, sizeof(int) * planned, cudaMemcpyDeviceToHost, s));
-    ORBFE_CUDA_TRY(cudaMemcpyAsync(ex->h_err, ex->mwork.err_flag, sizeof(int), cudaMemcpyDeviceToHost, s));
-    for (int i = 0; ncopy > 0 && i < M.ngroups; i++) {
-        const GroupDev &G = M.grp[i];
-        ORBFE_CUDA_TRY(cudaMemcpy2DAsync(kps + (size_t)out_frame[i] * cap, sizeof(OrbfeKeyPoint) * cap, ex->md_kps + (size_t)G.frame0 * nf,
-                                         sizeof(OrbfeKeyPoint) * nf, sizeof(OrbfeKeyPoint) * ncopy, G.nframes, cudaMemcpyDeviceToHost, s));
-        ORBFE_CUDA_TRY(cudaMemcpy2DAsync(desc + (size_t)out_frame[i] * cap * 32, (size_t)32 * cap, ex->md_desc + (size_t)G.frame0 * nf * 32,
-                                         (size_t)32 * nf, (size_t)32 * ncopy, G.nframes, cudaMemcpyDeviceToHost, s));
-    }
-    stage_mark(ex, s, "d2h");
-    if (int rc = ex->hs.leave(s, true)) return rc;
-    if (*ex->h_err) {
-        const int code = *ex->h_err;
-        cudaMemsetAsync(ex->mwork.err_flag, 0, sizeof(int), s);
-        ex->hs.leave(s, false);
-        return fail(ORBFE_ERR_INTERNAL, "device overflow flag %d", code);
-    }
-    int status = ORBFE_OK;
-    for (int i = 0; i < M.ngroups; i++)
-        for (int f = 0; f < M.grp[i].nframes; f++) {
-            const int n = ex->h_counts[M.grp[i].frame0 + f];
-            n_out[out_frame[i] + f] = n;
-            if (n > cap) status = ORBFE_ERR_CAPACITY;
-        }
-    if (status) return fail(status, "caller capacity %d too small", cap);
-    return ORBFE_OK;
+    std::vector<FrameRun> runs;
+    if (int rc = begin_multi(ex, ngroups, groups, true, nullptr, s, runs)) return rc;
+    if (runs.empty()) return ex->hs.leave(s, false);
+    const Plan<MultiPlanDev> &P = ex->multi;
+    if (int rc = enqueue_multi(ex, P.d_kps, P.d_desc, P.d_counts, s)) return rc;
+    return read_back(ex, P, runs, kps, desc, cap, n_out, s);
 }
 
 extern "C" int orbfe_extractor_sync(OrbfeExtractor *ex) {
@@ -1126,22 +1037,23 @@ extern "C" int orbfe_extractor_stage_times(const OrbfeExtractor *ex_c, char (*na
 }
 
 extern "C" int orbfe_debug_level_size(const OrbfeExtractor *ex, int level, int *w, int *h) {
-    if (!ex || level < 0 || level >= ex->nlevels || !ex->Bcap) return fail(ORBFE_ERR_ARG, "no plan / bad level");
-    if (w) *w = ex->hplan.lv[level].w;
-    if (h) *h = ex->hplan.lv[level].h;
+    if (!ex || level < 0 || level >= ex->nlevels || ex->single.geom.empty()) return fail(ORBFE_ERR_ARG, "no plan / bad level");
+    if (w) *w = ex->single.hp->lv[level].w;
+    if (h) *h = ex->single.hp->lv[level].h;
     return ORBFE_OK;
 }
 
 extern "C" int orbfe_debug_read_level(OrbfeExtractor *ex, int frame, int level, int which, uint8_t *out, size_t out_stride) {
-    if (!ex || !out || level < 0 || level >= ex->nlevels || frame < 0 || frame >= ex->Bcap)
+    if (!ex || !out || level < 0 || level >= ex->nlevels || frame < 0 || ex->single.geom.empty() || frame >= ex->single.cap[0])
         return fail(ORBFE_ERR_ARG, "bad arguments");
+    const Plan<PlanDev> &P = ex->single;
     // the levels of the handle's last call, whichever stream it ran on
     cudaStream_t s = ex->hs.stream;
     if (int rc = ex->hs.enter(s)) return rc;
-    const LevelDev &L = ex->hplan.lv[level];
+    const LevelDev &L = P.hp->lv[level];
     const uint8_t *src = which ? L.blur : L.pyr + (size_t)frame * L.plane;
     // the pipeline smooths only descriptor patches; materialise the smoothed level of this frame on demand
-    if (which) launch_blur(ex->dplan, ex->hplan, ex->work, frame, 1, s);
+    if (which) launch_blur(P.dp, *P.hp, P.work, frame, 1, s);
     if (int rc = ex->hs.leave(s, true)) return rc;
     ORBFE_CUDA_TRY(cudaMemcpy2D(out, out_stride, src, L.pitch, L.w, L.h, cudaMemcpyDeviceToHost));
     return ORBFE_OK;

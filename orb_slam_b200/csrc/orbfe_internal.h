@@ -51,7 +51,7 @@ struct LevelDev {
     const short2 *xab;    // [w]  11-bit weights (a0, a1)
     const int2 *yrows;    // [h]  source rows (r0, r1), each clipped to [0, h_src-1]
     const short2 *yab;    // [h]  (b0, b1)
-    int rz_fast;          // >= 1: the 4 source columns of every aligned destination quad fit three aligned words; 2: see build_plan
+    int rz_fast;          // >= 1: the 4 source columns of every aligned destination quad fit three aligned words; 2: see alloc_geometry
 };
 
 // What the single-geometry plan and the multi plan share; the per-frame strides (ncells_total, kept_total, cand_total,
@@ -59,7 +59,7 @@ struct LevelDev {
 struct PlanHead {
     int nlevels, batch, nfeatures;
     int ncells_total, nftiles_total, nbtiles_total, kept_total;
-    int t_lo, t_hi;      // min / max of (max(fastTh, 1), 7): threshold 0 detects what 1 does (build_plan)
+    int t_lo, t_hi;      // min / max of (max(fastTh, 1), 7): threshold 0 detects what 1 does (plan_head)
     int t1_is_lo;        // fastTh <= 7
     int score_type;
     int pdl;             // host side only: launch the pipeline's kernels with programmatic stream serialization (ORBFE_PDL, default 1)
@@ -106,7 +106,7 @@ struct WorkDev {
     const int *cell_cand_cap;         // [ncells_total]
     const FTileInfo *ftile_info;      // [nftiles_total]
     const BTileInfo *btile_info;      // [nbtiles_total]
-    const CUtensorMap *tmaps;         // [nlevels] 3-D (x, y, frame) tensor maps of the unblurred levels; never NULL (build_plan fails without TMA)
+    const CUtensorMap *tmaps;         // [nlevels] 3-D (x, y, frame) tensor maps of the unblurred levels; never NULL (a plan is not built without TMA)
     uint32_t *cand_keys;              // [batch][cand_total]   (score<<24 | 0xFFFFFF - raster)
     unsigned long long *cand_keys64;  // HARRIS_SCORE only: order(resp)<<32 | (0xFFFFFF - raster)<<8 | score; NULL otherwise
     uint32_t *kept_aux;               // HARRIS_SCORE only: low raster bits + score of each kept entry

@@ -4,7 +4,7 @@ Shared by test_oracle_multi_domain.py (CPU: the restatement against the oracle's
 each scene's facts) and test_gpu_multi_domain.py (the CUDA entries against the oracle and the single-geometry entry).
 numpy only.
 
-The restatement follows orbfe_extractor_create (level scales and quotas) and layout_geometry / build_multi_plan /
+The restatement follows orbfe_extractor_create (level scales and quotas) and layout_geometry / build / build_multi /
 begin_multi (orbfe_api.cu) in float32 where they compute in float: per geometry its level sizes, cell grids, FAST tiles,
 candidate slots and kept lists, and whether the library accepts it; per call the groups' frame, FAST-work and cell-work
 ranges; per plan the totals, the level-select kernel's shared memory and the group that drives each; and the capacity rule
@@ -214,7 +214,7 @@ class Plan:
 
 
 def capacity(calls, grow=True):
-    """The capacity rule of build_multi_plan over a sequence of calls on one handle, each [(W, H, B)] (W or H 0: empty).
+    """The capacity rule of the multi plan's build over a sequence of calls on one handle, each [(W, H, B)] (W or H 0: empty).
     A call keeps the plan when its non-empty groups' (W, H) list equals the plan's and every group fits; when only the
     frames grow, every group keeps at least its old capacity (grow=False: the rule without that).  Returns [(rebuilt, capacities after the call)]."""
     geom, cap, out = None, None, []

@@ -4,7 +4,7 @@ Every FAST threshold class (0 .. 254) on content whose ring differences sit exac
 level kept, with corners placed across every cell seam, FAST-tile seam and the detect border; the level-select kernel past
 48 KB of shared memory and at the plan's refusal boundary; 16 and 32 levels, scale factors 1.01 .. 3.0; and every way a
 frame is ingested by orbfe_extract_batch_device (in place, pitched, the 2-D copy path), with one handle switching between
-them and the host entry.
+them and the host entry; a refused geometry keeps the handle's plan.
 
 Bar (as test_gpu_extract.py): x, y, size, response, octave, class_id equal; angle equal as float32 bits; descriptors equal.
 """
@@ -306,6 +306,25 @@ def test_one_handle_across_ingest_paths_and_plans(gpu_required):
     G3 = D.upload(_layout(g2, 1, W2 + 1, (W2 + 1) * H2))
     _same_all(D.run(ex, G3.data_ptr() + 1, W2, H2, W2 + 1, (W2 + 1) * H2, B2), want2)
     ex.close()
+
+
+def test_refused_geometry_keeps_the_plan(gpu_required):
+    """A call refused for its geometry leaves the handle's plan as it was, as a refused multi call does: 1280x960 at
+    4 levels of 2.0 is planned, 640x480 is refused (test_refused_level_geometries), and 1280x960 again is not re-planned
+    and gives the first call's keypoints and descriptors."""
+    img = textured_frame(1280, 960, seed=21)
+    ex = fe.ORBextractor(1000, 2.0, 4)
+    try:
+        k1, d1 = ex(img)
+        assert len(k1) > 0 and ex.plan_builds() == 1
+        with pytest.raises(fe.OrbfeError) as e:
+            ex(textured_frame(640, 480, seed=21))
+        assert e.value.code == fe.ORBFE_ERR_UNSUPPORTED and ex.plan_builds() == 1
+        k2, d2 = ex(img)
+        assert ex.plan_builds() == 1
+    finally:
+        ex.close()
+    _same(k2, d2, k1, d1)
 
 
 def mixed_frames(W=640, H=480, B=64):
